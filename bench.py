@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the DALL-E data-parallel training step (the north-star hot path) on N B200s.
+"""bench.py — throughput of the DALL-E data-parallel training step (the north-star hot path) on N H100s.
 
     python bench.py --gpus 1 --steps 10 --warmup 3              # N=1
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
            bench.py --gpus N --steps K --warmup W                # N>1, one rank per GPU over NCCL
     python bench.py --impl reference ...                         # the CPU restatement of the reference on host cores
+    python bench.py --gpus 1 --steps 10 --dump-outputs DIR       # also write the last timed step's results as .npy
 
 Workload (config.workload): configs/dalle_example_b200.json = BASELINE.json configs[1]: n_embd 512, 6 layers, 4 heads,
 sequence 256 text + 1024 image tokens (dataset.image_size 256 through the 3-stage vae_example tokenizer), bf16,
@@ -15,8 +16,15 @@ One JSON line on rank 0:
   value        whole-job tokens/s with the step's inputs (images, captions) already resident in HBM
   e2e          same through the public API (dalle_model_fn's train_op) with PINNED HOST inputs: the H2D copy of
                the images / captions and a D2H read of the loss are inside the timed region, every step
-  roofline     the dominant kernel (tcgen05 GEMM, all launches of a step): algorithmic 2*M*N*K FLOPs / CUDA-event
-               time of those launches, against MEASURED_PEAKS.json's sustained bf16 figure
+  roofline     the dominant kernel (wgmma GEMM, all launches of a step): algorithmic 2*M*N*K FLOPs / CUDA-event
+               time of those launches, against MEASURED_PEAKS.json's sustained bf16 figure (else the H100 SXM data
+               sheet's dense bf16 rate, which a power-limited card does not reach)
+
+--dump-outputs DIR writes, after the timed steps of the headline workload, what its last timed step returned to the
+caller: the loss, the token ids it trained on (VAE codes of the images after the caption) and a fixed, seeded sample of
+the updated fp32 parameters (with their flat indices).  Inputs and initial weights are seeded, so two builds run with
+the same arguments can be compared output for output.  Every sum over CTAs in the DALL-E step is added in a fixed order
+(no float atomics), so a build writes bit-identical outputs on every run.
   cpu_baseline the oracle (CPU port of the reference math, "reference-faithful" variant: one-hot embedding / CE,
                materialised attention) timed on the box's host cores on a bounded sample of the same workload
 """
@@ -42,9 +50,10 @@ WORKLOADS = {
     # name: (config file, sequences per GPU, d, layers, vocab)
     "dalle_example": ("dalle_example_b200.json", 32, 512, 6, 50771),
     "dalle_coco": ("dalle_coco_b200.json", 16, 1024, 24, 50258 + 8192 + 1),
-    # BASELINE.json configs[4]: 12 B parameters, optimiser state sharded over the data-parallel ranks (needs >= 2 GPUs,
-    # quoted at 8), per-block recompute, synthetic inputs, throughput only
-    "dalle_12b": ("dalle_12b_b200.json", 4, 4096, 64, 50258 + 8192 + 1),
+    # BASELINE.json configs[4] width (d = 4096, 32 heads) at 40 layers = 8.5 B parameters, so that bf16 weights + fp32
+    # gradients + 1/8 of the optimiser state + activations fit an 80 GB GPU; optimiser state sharded over the
+    # data-parallel ranks (needs >= 2 GPUs, sized for 8), per-block recompute, synthetic inputs, throughput only
+    "dalle_12b": ("dalle_12b_b200.json", 4, 4096, 40, 50258 + 8192 + 1),
 }
 
 
@@ -80,7 +89,7 @@ def load_params(n_gpus, workload="dalle_example", scaling="weak"):
 
 
 def csrc_hash():
-    """sha256 over the CUDA sources the .so is built from: ties a committed ncu capture to the build it was taken on."""
+    """sha256 over the CUDA sources the .so is built from: ties a bench line or an output dump to the build it came from."""
     import glob
     import hashlib
     h = hashlib.sha256()
@@ -88,22 +97,6 @@ def csrc_hash():
         h.update(os.path.basename(f).encode())
         h.update(open(f, "rb").read())
     return h.hexdigest()[:16]
-
-
-def ncu_gemm_traffic(workload, launches_per_step):
-    """`roofline.traffic`: DRAM bytes (read + write) per GEMM launch from an `ncu --set full` capture.  A profiler
-    number cannot be measured inside this run, so it is taken from profiles/ncu_gemm_step_r02.json ONLY IF that
-    capture was made on exactly these sources (csrc_hash) for this workload and launch count; otherwise null."""
-    path = os.path.join(ROOT, "profiles", "ncu_gemm_step_r02.json")
-    try:
-        with open(path) as f:
-            rec = json.load(f)
-    except (OSError, ValueError):
-        return None
-    if rec.get("csrc_hash") != csrc_hash() or rec.get("workload") != workload or \
-            rec.get("launches") != int(round(launches_per_step)):
-        return None
-    return rec["dram_bytes_per_launch"]
 
 
 def vae_train_flops_per_image(convblocks, size, K, C=3):
@@ -157,12 +150,12 @@ def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -356,6 +349,8 @@ def measure_dalle(args, dp, device, workload, steps, warmup, full):
     t_begin = sampler.mark()
     ms_total = timed(dev_batches, steps, False)
     t_end = sampler.mark()
+    if full and args.dump_outputs and dp.rank == 0:
+        dump_outputs(args.dump_outputs, spec)
     launches = L.launch_count() - n0
     prof, ops.GEMM_PROFILE = ops.GEMM_PROFILE, None
     aprof, ops.ATTN_PROFILE = ops.ATTN_PROFILE, None
@@ -406,21 +401,22 @@ def measure_dalle(args, dp, device, workload, steps, warmup, full):
                                     f"tokens), V={V}" + (", recompute_grad" if params.get("recompute_grad") else "")),
                        "global_batch": per_gpu_batch * args.gpus, "per_gpu_batch": per_gpu_batch, "seq_len": S,
                        "parallelism": f"dp{args.gpus}", "step": "vae-encode + fwd + bwd + allreduce + clip + adam",
-                       "l2": "inputs rotate over 4 batches; each step streams several GB of activations (>> 126 MB L2)"},
+                       "l2": "inputs rotate over 4 batches; each step streams several GB of activations (>> 50 MB L2)"},
             "tokens_per_sec_per_gpu": value / args.gpus,
             "model_flops_fraction": (value / args.gpus) * f_tok / (peak_tf * 1e12),
             "loss": loss_now,
             "e2e": {"value": tokens_per_step * 1000.0 / ms_e2e, "unit": UNIT, "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4},
             "gpu_launches": int(launches),
+            "csrc_hash": csrc_hash(),
             "clocks": clocks,
-            "roofline": {"kernel": "gemm_tc_kernel (tcgen05, all launches of the step)", "bound": "tensor",
+            "roofline": {"kernel": "gemm_tc_kernel (wgmma, all launches of the step)", "bound": "tensor",
                          "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
                          "peak_kind": f"bf16_tflops_sustained ({peak_kind})",
-                         "traffic": ncu_gemm_traffic(workload, len(prof) / steps),
+                         "traffic": None,
                          "launches_per_step": len(prof) / steps, "share_of_step": gemm_ms / ms_total,
                          "flops_per_launch": gemm_flops / max(len(prof), 1)},
-            # second roofline: the causal attention kernels (tcgen05, warp-specialised), causal-algorithmic FLOPs
+            # second roofline: the causal attention kernels (wgmma), causal-algorithmic FLOPs
             # (forward 4 S^2 dh B H / 2, backward 2.5 x) / CUDA-event time of their launches
             "roofline_attention": {k: dict(v, frac=v["tflops"] / peak_tf, peak=peak_tf, unit="TFLOP/s", bound="tensor")
                                    for k, v in attn.items()},
@@ -434,6 +430,29 @@ def measure_dalle(args, dp, device, workload, steps, warmup, full):
     del spec
     torch.cuda.empty_cache()
     return line
+
+
+DUMP_PARAM_SAMPLE = 1 << 21   # 8 MiB of fp32 values + 16 MiB of float64 indices
+
+
+def dump_outputs(out_dir, spec):
+    """What the timed train_op computed in its last step, as float32 / float64 .npy files (see the module doc)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    eng = spec.engine
+    torch.cuda.synchronize()
+    loss = float(spec.loss_sum.item()) * spec.loss_scale
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
+    tokens = getattr(eng, "_tokens", None)     # the (last micro-batch's) tokens of the step's forward
+    if tokens is not None:
+        np.save(os.path.join(out_dir, "tokens.npy"), tokens.detach().cpu().numpy().astype(np.float64))
+    master = eng.master[:eng.n_params_padded] if eng.zero is None else eng.master
+    n = master.numel()
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randint(0, n, (min(DUMP_PARAM_SAMPLE, n),), generator=g).sort().values
+    vals = master[idx.to(master.device)].float().cpu().numpy()
+    np.save(os.path.join(out_dir, "params_sample.npy"), vals.astype(np.float32))
+    np.save(os.path.join(out_dir, "params_sample_index.npy"), idx.numpy().astype(np.float64))
 
 
 def run_reference(args):
@@ -465,7 +484,7 @@ def main():
     ap.add_argument("--impl", type=str, default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--workload", type=str, default="dalle_example", choices=sorted(WORKLOADS),
-                    help="dalle_example = BASELINE.json configs[1] (the default, what the driver measures); "
+                    help="dalle_example = BASELINE.json configs[1] (the default, the headline workload); "
                          "dalle_coco = configs[3] shape (n_embd 1024, 24 layers, 16 heads, 16 sequences per GPU)")
     ap.add_argument("--scaling", type=str, default="weak", choices=["weak", "strong"],
                     help="weak: 32 sequences per GPU (global batch 32 N); strong: global batch fixed at 32 (32 / N per GPU)")
@@ -474,6 +493,9 @@ def main():
     ap.add_argument("--no-extra", action="store_true", help="skip the bounded dalle_coco / vae_coco side measurements")
     ap.add_argument("--vae-example", action="store_true",
                     help="measure only configs/vae_example.json (BASELINE configs[0]: 32x32, fp32, batch 32)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write the last timed step's loss, token ids and a seeded sample of "
+                         "the updated parameters to DIR/<name>.npy")
     ap.add_argument("--vae-coco", action="store_true",
                     help="measure configs/vae_coco_b200.json (256x256, K=8192, bf16, 16 images per GPU) instead")
     args = ap.parse_args()
@@ -508,8 +530,7 @@ def main():
         return 0
     line = measure_dalle(args, dp, device, args.workload, args.steps, args.warmup, full=True)
     if line is not None and args.gpus == 1 and args.workload == "dalle_example" and not args.no_extra:
-        # BASELINE.json's other single-GPU-measurable configurations, bounded, measured under the same driver run
-        # (README / BASELINE.md quote these lines instead of builder-run numbers)
+        # BASELINE.json's other single-GPU-measurable configurations, bounded, measured in the same run
         extra = {}
         try:
             extra["dalle_coco_b200"] = measure_dalle(args, dp, device, "dalle_coco", 5, 3, full=False)

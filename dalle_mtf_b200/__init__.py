@@ -1,4 +1,4 @@
-"""dalle_mtf_b200 — B200-native (sm_100a) engine behind the DALLE-mtf config / model_fn surface.
+"""dalle_mtf_b200 — H100-native (sm_90a) engine behind the DALLE-mtf config / model_fn surface.
 
 Only what the data-parallel training hot path needs lives here:
   csrc/            hand-written CUDA kernels + the C ABI (include/dalle_b200.h) -> libdalle_b200.so

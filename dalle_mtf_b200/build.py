@@ -1,4 +1,4 @@
-"""In-tree build of libdalle_b200.so with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""In-tree build of libdalle_b200.so with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 

@@ -1,23 +1,23 @@
 // K4 — causal flash attention, forward and backward: the C-ABI entry points and the row-wise delta pre-pass.
 //
 // Replaces mtf_transformer.attention.attention + the [S,S] additive -1e10 mask the reference materialises
-// (src/dalle_mtf/models.py:221-227, 287-299).  Logits are fp32 (TMEM accumulators), softmax is fp32, P is rounded to
+// (src/dalle_mtf/models.py:221-227, 287-299).  Logits are fp32 (wgmma accumulators), softmax is fp32, P is rounded to
 // bf16 for the PV product (what mtf does when it casts the weights to v's dtype), nothing of size S x S reaches HBM.
 // `scale` multiplies q.k (reference: 1.0 — mtf folds 1/sqrt(dh) into the q initialiser).
 //
 // Layout: qkv bf16 [B][S][3][H][dh] (the fused q|k|v projection output), out / dout bf16 [B][S][H][dh],
 //         lse f32 [B][H][S] (natural log of sum exp(scale*s)), dqkv like qkv.
 //
-// The kernels are the warp-specialised ones of attn_ws.cu (TMA warp, MMA-issuer warp, softmax warpgroups, P / dS handed
-// over through TMEM); this file validates the arguments, runs delta = rowsum(dO * O) and launches them.
+// The kernels are in attn_fa.cu (one warpgroup per 64 rows, P / dS handed to the next wgmma in registers); this file
+// validates the arguments, runs delta = rowsum(dO * O) and launches them.
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace db200 {
 
-int attn_fwd_ws_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
-                       float scale);
-int attn_bwd_ws_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
+int attn_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
+                    float scale);
+int attn_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
                        void* dqkv, int B, int S, int H, int dh, float scale);
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -68,7 +68,7 @@ extern "C" int db200_attn_causal_fwd(db200_stream_t stream_, const void* qkv, vo
                 "attn_fwd: NULL or unaligned pointer");
   DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_fwd: scale must be > 0");
   if (dh != 64 && dh != 128) return set_error(DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
-  return attn_fwd_ws_launch(stream, qkv, out, lse, B, S, H, dh, scale);
+  return attn_fwd_launch(stream, qkv, out, lse, B, S, H, dh, scale);
 }
 
 extern "C" int db200_attn_causal_bwd(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
@@ -93,5 +93,5 @@ extern "C" int db200_attn_causal_bwd(db200_stream_t stream_, const void* qkv, co
   }
   int rc = check_launch("attn_delta_kernel");
   if (rc != DB200_OK) return rc;
-  return attn_bwd_ws_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, scale);
+  return attn_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, scale);
 }

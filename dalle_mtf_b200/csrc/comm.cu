@@ -107,8 +107,8 @@ extern "C" int db200_comm_create(int device, int rank, int world, const void* un
   c->device = device; c->rank = rank; c->world = world;
   ncclConfig_t cfg = NCCL_CONFIG_INITIALIZER;
   cfg.blocking = 1;
-  // Cap the CTAs NCCL may occupy: the persistent tcgen05 GEMM grids of backward run concurrently with the bucket
-  // collectives, and every SM NCCL holds is one the 148-CTA grids wait for (NVLS needs few CTAs to saturate NVLink).
+  // Cap the CTAs NCCL may occupy: the persistent wgmma GEMM grids of backward run concurrently with the bucket
+  // collectives, and every SM NCCL holds is one the one-CTA-per-SM grids wait for.
   if (max_ctas > 0) cfg.maxCTAs = max_ctas;
   ncclUniqueId id;
   memcpy(&id, unique_id, sizeof(id));

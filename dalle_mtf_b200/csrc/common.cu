@@ -108,6 +108,47 @@ static int make_tmap_bf16_uncached(CUtensorMap* out, const void* base, int rank,
   return DB200_OK;
 }
 
+// block = 32 columns x 8 row lanes: lane k sums rows k, k + 8, ... in order, then the 8 lane sums are added in lane order
+__global__ void __launch_bounds__(256)
+reduce_rows_add_kernel(const float* __restrict__ ws, int rows, int cols, float* __restrict__ dst) {
+  __shared__ float part[8][32];
+  const int cx = threadIdx.x & 31, k = threadIdx.x >> 5;
+  const int c = blockIdx.x * 32 + cx;
+  float s = 0.f;
+  if (c < cols)
+    for (int r = k; r < rows; r += 8) s += ws[(long long)r * cols + c];
+  part[k][cx] = s;
+  __syncthreads();
+  if (k == 0 && c < cols) {
+    float t = part[0][cx];
+#pragma unroll
+    for (int j = 1; j < 8; ++j) t += part[j][cx];
+    dst[c] += t;
+  }
+}
+
+__global__ void reduce_splits_add_kernel(const float* __restrict__ ws, int splits, int M, int N, float* __restrict__ D,
+                                         long long ldd) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long mn = (long long)M * N;
+  if (i >= mn) return;
+  float s = 0.f;
+  for (int k = 0; k < splits; ++k) s += ws[k * mn + i];
+  const long long m = i / N, n = i - m * N;
+  D[m * ldd + n] += s;
+}
+
+int reduce_rows_add(cudaStream_t stream, const float* ws, int rows, int cols, float* dst) {
+  reduce_rows_add_kernel<<<(cols + 31) / 32, 256, 0, stream>>>(ws, rows, cols, dst);
+  return check_launch("reduce_rows_add_kernel");
+}
+
+int reduce_splits_add(cudaStream_t stream, const float* ws, int splits, int M, int N, float* D, long long ldd) {
+  const long long mn = (long long)M * N;
+  reduce_splits_add_kernel<<<(unsigned)((mn + 255) / 256), 256, 0, stream>>>(ws, splits, M, N, D, ldd);
+  return check_launch("reduce_splits_add_kernel");
+}
+
 int g_reserved_sms = 0;   // SMs left to a concurrently running collective (set once at start-up)
 
 int sm_count() {
@@ -118,7 +159,7 @@ int sm_count() {
   if (cached[dev] == 0) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = n > 0 ? n : 148;
+    cached[dev] = n > 0 ? n : 132;
   }
   const int n = cached[dev] - g_reserved_sms;
   return n > 16 ? n : 16;
@@ -139,17 +180,17 @@ int db200_device_check(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10)
-    return db200::set_error(DB200_E_UNSUPPORTED, "device %d is sm_%d%d; libdalle_b200 ships sm_100a code only", dev,
+  if (major != 9 || minor != 0)
+    return db200::set_error(DB200_E_UNSUPPORTED, "device %d is sm_%d%d; libdalle_b200 ships sm_90a code only", dev,
                             major, minor);
   return DB200_OK;
 }
 }
 
-// The persistent kernels (GEMM, convolutions, attention) launch one CTA per SM that needs the whole SM (shared memory,
+// The persistent kernels (GEMM, convolutions) launch one CTA per SM that needs the whole SM (shared memory,
 // registers): a collective whose CTAs occupy k SMs while they run would push k of those CTAs into a second wave.
 // With k SMs reserved the grids are sized to sm_count - k and both fit side by side (data-parallel runs reserve the
-// CTA cap of the overlapped communicator; measured at 8 GPUs without it: GEMMs -5.5 %, attention backward -10 %).
+// CTA cap of the overlapped communicator).
 extern "C" int db200_set_reserved_sms(int n) {
   if (n < 0 || n > 64) return db200::set_error(DB200_E_INVALID, "set_reserved_sms: %d not in [0, 64]", n);
   db200::g_reserved_sms = n;

@@ -50,4 +50,17 @@ static inline int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inne
 
 int sm_count();  // cached cudaDevAttrMultiProcessorCount of the current device
 
+// ---- order-fixed reductions ------------------------------------------------------------------------
+// Sums that many CTAs contribute to are not accumulated with float atomics (their order, and so the rounding, would
+// change from run to run): every CTA stores its partial into a workspace the caller passes in, and one reduction kernel
+// adds the partials in a fixed order on the same stream.
+// true if the caller's workspace holds `need` bytes and is 16-byte aligned
+static inline bool workspace_ok(const void* ws, int64_t bytes, int64_t need) {
+  return need <= 0 || (ws != nullptr && bytes >= need && aligned16(ws));
+}
+// dst[c] += sum over r = 0, 1, ... rows-1 of ws[r * cols + c]
+int reduce_rows_add(cudaStream_t stream, const float* ws, int rows, int cols, float* dst);
+// D[m * ldd + n] += sum over s = 0 .. splits-1 of ws[(s * M + m) * N + n]
+int reduce_splits_add(cudaStream_t stream, const float* ws, int splits, int M, int N, float* D, long long ldd);
+
 }  // namespace db200

@@ -664,7 +664,7 @@ extern "C" int db200_conv2d_first_fwd(db200_stream_t stream_, const float* x, co
   DB200_REQUIRE(H % 2 == 0 && W % 2 == 0 && Cout % 64 == 0 && Cout <= 256, DB200_E_UNSUPPORTED,
                 "conv2d_first_fwd: needs even H, W and Cout in {64,128,192,256}");
   DB200_REQUIRE(aligned16(w) && aligned16(y_bf16), DB200_E_ALIGN, "conv2d_first_fwd: unaligned pointer");
-  return conv_first_tc_launch(stream, x, w, bias, y_bf16, N, H, W, Cout);  // tcgen05 (conv_first_tc.cu)
+  return conv_first_tc_launch(stream, x, w, bias, y_bf16, N, H, W, Cout);  // wgmma (conv_first_tc.cu)
 }
 
 // CUDA-core version of the first layer (fp32 FMA; kept for A/B measurements: FMA-bound at ~5x the tensor-core kernel)

@@ -1,17 +1,17 @@
 // K11 (fp32 activations) — the discrete-VAE convolutions of an fp32 configuration (vae_example: `bf_16` absent,
-// src/vae_tf/models.py:95-109,139-155) on tcgen05 with fp32-accurate products.
+// src/vae_tf/models.py:95-109,139-155) on wgmma with fp32-accurate products.
 //
 // An fp32 value is split into three bf16 parts x = h + m + l (|m| <= 2^-9 |x|, |l| <= 2^-18 |x|, residual <= 2^-27 |x|);
 // a product of two split values keeps the six terms down to 2^-18 (hh, hm, mh, hl, lh, mm) — the dropped ones are below
-// fp32's own rounding — and all of them accumulate in fp32 in TMEM.  The split happens inside the kernel: the CTA's
+// fp32's own rounding — and all of them accumulate in fp32 registers.  The split happens inside the kernel: the CTA's
 // threads read the fp32 pixels / weights from global memory (coalesced, zero-filled outside the image), split them in
-// registers and store the three bf16 tiles straight into the 128-byte-swizzled shared-memory layout the UMMA
+// registers and store the three bf16 tiles straight into the 128-byte-swizzled shared-memory layout the wgmma
 // descriptors expect; there is no bf16 copy of anything in HBM and no TMA (the producer is the math threads).
-// Nine warps: eight producers (load -> split -> store into one of three smem stages, two chunks of look-ahead in
-// registers) and one MMA-issuer warp that waits on the stage's "full" mbarrier, issues the six-product group and commits
-// the stage's "empty" barrier.  (The issue of 24 tcgen05.mma blocks for most of their execution time — the queue is
-// shallow — so with the issuer also being a producer warp and __syncthreads per chunk, every chunk cost the SUM of the
-// split and the MMA time: 1.7 us per chunk in the launch list of the first version.)
+// Eight warps = two warpgroups, each of them producer and consumer in turn: store chunk c into one of three smem
+// stages, refill the registers with chunk c+2, arrive on the stage's "full" mbarrier, wait for both warpgroups'
+// stores, issue the six-product wgmma group for the warpgroup's 64 rows asynchronously, and hand the stage of chunk
+// c-1 back ("empty" mbarrier) once its MMAs have retired — the split of chunk c+1 overlaps the MMAs of chunk c.  (In
+// the wgrad kernel ptxas currently serialises the wgmma groups (C7518), so there the overlap does not happen.)
 //
 //   gather-GEMM (forward, conv-transpose forward, both dgrads; the ConvGemmParams of conv.cu):
 //       D[128 pixels][64 channels] += A[128 pixels][64 k] * B[64 k][64 channels]      per (tap, 64-channel k chunk)
@@ -23,6 +23,7 @@
 #include "common.cuh"
 #include "ptx.cuh"
 #include "conv_params.cuh"
+#include "wgmma.cuh"
 
 namespace db200 {
 namespace {
@@ -32,6 +33,7 @@ constexpr uint32_t FT_B_PART = 64 * 128;    // [64 rows][64 bf16]
 constexpr uint32_t FT_STAGE = 3 * FT_A_PART + 3 * FT_B_PART;   // 72 KiB
 constexpr int FT_NSTAGE = 3;
 constexpr size_t FT_SMEM = 1024 + FT_NSTAGE * FT_STAGE + 64;
+static_assert(FT_SMEM <= 227 * 1024, "shared memory exceeds the H100 per-block limit");
 
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
@@ -63,27 +65,27 @@ __device__ __forceinline__ void stage8(uint32_t base, uint32_t part, uint32_t ro
   st_shared_v4(base + 2 * part + off, l);
 }
 
-// the six products with weight >= 2^-18, smallest first
-__device__ __forceinline__ void mma6(uint32_t tmem, const uint64_t (&ad)[3], const uint64_t (&bd)[3], uint64_t astep,
-                                     uint64_t bstep, uint32_t idesc, bool first) {
+// the six products with weight >= 2^-18, smallest first (m64 x 64 x 16 each, this warpgroup's 64 rows)
+template <int TA, int TB>
+__device__ __forceinline__ void mma6(float* d, const uint64_t (&ad)[3], const uint64_t (&bd)[3], uint64_t astep,
+                                     uint64_t bstep, bool first) {
 #pragma unroll
   for (int kk = 0; kk < 4; ++kk) {
     const uint64_t a0 = ad[0] + kk * astep, a1 = ad[1] + kk * astep, a2 = ad[2] + kk * astep;
     const uint64_t b0 = bd[0] + kk * bstep, b1 = bd[1] + kk * bstep, b2 = bd[2] + kk * bstep;
-    umma_bf16_ss(tmem, a1, b1, idesc, (first && kk == 0) ? 0u : 1u);
-    umma_bf16_ss(tmem, a0, b2, idesc, 1u);
-    umma_bf16_ss(tmem, a2, b0, idesc, 1u);
-    umma_bf16_ss(tmem, a0, b1, idesc, 1u);
-    umma_bf16_ss(tmem, a1, b0, idesc, 1u);
-    umma_bf16_ss(tmem, a0, b0, idesc, 1u);
+    wgmma_m64n64<TA, TB>(d, a1, b1, (first && kk == 0) ? 0u : 1u);
+    wgmma_m64n64<TA, TB>(d, a0, b2, 1u);
+    wgmma_m64n64<TA, TB>(d, a2, b0, 1u);
+    wgmma_m64n64<TA, TB>(d, a0, b1, 1u);
+    wgmma_m64n64<TA, TB>(d, a1, b0, 1u);
+    wgmma_m64n64<TA, TB>(d, a0, b0, 1u);
   }
 }
 
-constexpr int FT_THREADS = 288;   // 8 producer warps + 1 MMA-issuer warp
+constexpr int FT_THREADS = 256;   // two warpgroups: producers and wgmma consumers in turn
 struct FtSmem {
   uint32_t stage0;     // stage s at stage0 + s * FT_STAGE: A parts first, B parts at + 3 * FT_A_PART
   uint32_t bar0;       // bar0 + 8 s: "the MMAs that read stage s have retired";  bar0 + 8 (3 + s): "stage s is written"
-  uint32_t tmem_slot;
   __device__ __forceinline__ uint32_t stage(int s) const { return stage0 + s * FT_STAGE; }
   __device__ __forceinline__ uint32_t bar(int s) const { return bar0 + 8 * s; }
   __device__ __forceinline__ uint32_t full(int s) const { return bar0 + 8 * (FT_NSTAGE + s); }
@@ -95,7 +97,6 @@ __device__ __forceinline__ FtSmem ft_carve(uint8_t* raw_ptr) {
   FtSmem s;
   s.stage0 = base;
   s.bar0 = base + FT_NSTAGE * FT_STAGE;
-  s.tmem_slot = s.bar0 + 16 * FT_NSTAGE;
   return s;
 }
 
@@ -108,23 +109,17 @@ __global__ void __launch_bounds__(FT_THREADS)
 conv_gemm_f32_tc_kernel(const ConvGemmParams p) {
   extern __shared__ uint8_t ft_smem_raw[];
   const FtSmem sm = ft_carve(ft_smem_raw);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(ft_smem_raw + (sm.tmem_slot - smem_u32(ft_smem_raw)));
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const long long M = (long long)p.NB * p.OH * p.OW;
   const long long m0 = (long long)blockIdx.x * 128;
   const int n0 = blockIdx.y * 64;
   const float* x = reinterpret_cast<const float*>(p.x);
 
   if (tid == 0) {
-    for (int i = 0; i < FT_NSTAGE; ++i) { mbar_init(sm.bar(i), 1); mbar_init(sm.full(i), 8); }
+    for (int i = 0; i < FT_NSTAGE; ++i) { mbar_init(sm.bar(i), 2); mbar_init(sm.full(i), 8); }
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc(sm.tmem_slot, 64);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
 
   // A loader: pixel row (tid >> 1), channels (tid & 1) * 32 .. + 31 of the chunk
   const uint32_t a_row = tid >> 1, a_seg0 = (tid & 1) * 4;
@@ -171,41 +166,33 @@ conv_gemm_f32_tc_kernel(const ConvGemmParams p) {
     for (int j = 0; j < 2; ++j) stage8(sB, FT_B_PART, b_row, b_seg0 + j, rb[2 * j], rb[2 * j + 1]);
   };
 
-  const uint32_t idesc = umma_idesc_bf16(128, 64, 0, b_mn ? 1 : 0);
   // chunk c: registers -> stage c % 3 (once the MMAs of chunk c-3 have read it), refill the register set with chunk
-  // c+2, publish, issue the six-product MMA group
-  if (warp == 8) {
-    // ---------------------------------------------------------------------------------------------- MMA issuer
-    for (int c = 0; c < nchunk; ++c) {
-      const int s = c % FT_NSTAGE;
-      mbar_wait(sm.full(s), (uint32_t)((c / FT_NSTAGE) & 1));
-      tc_fence_after();
-      const uint32_t sA = sm.stage(s), sB = sm.stage(s) + 3 * FT_A_PART;
-      uint64_t ad[3], bd[3];
+  // c+2, publish, wait for the other warpgroup's half, issue this warpgroup's six-product group (rows 64 wg ..)
+  float d[32];
+  auto do_chunk = [&](int c, float4 (&ra)[8], float4 (&rb)[4]) {
+    const int s = c % FT_NSTAGE;
+    if (c >= FT_NSTAGE) mbar_wait_mma(sm.bar(s), (uint32_t)((c / FT_NSTAGE - 1) & 1));
+    store_chunk(s, ra, rb);
+    if (c + 2 < nchunk) load_chunk(c + 2, ra, rb);
+    fence_proxy_async_smem();   // generic-proxy stores -> visible to wgmma (async proxy)
+    __syncwarp();
+    if (lane == 0) mbar_arrive(sm.full(s));
+    mbar_wait_mma(sm.full(s), (uint32_t)((c / FT_NSTAGE) & 1));
+    const uint32_t sA = sm.stage(s) + wg * (64u * 128u), sB = sm.stage(s) + 3 * FT_A_PART;
+    uint64_t ad[3], bd[3];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        ad[i] = umma_smem_desc_sw128(sA + i * FT_A_PART, 0, 1024);
-        bd[i] = b_mn ? umma_smem_desc_sw128(sB + i * FT_B_PART, FT_B_PART, 1024)
-                     : umma_smem_desc_sw128(sB + i * FT_B_PART, 0, 1024);
-      }
-      if (elect_one_sync()) {
-        mma6(tmem, ad, bd, 2u, b_mn ? 128u : 2u, idesc, c == 0);
-        umma_commit(sm.bar(s));
-      }
-      __syncwarp();
+    for (int i = 0; i < 3; ++i) {
+      ad[i] = smem_desc_sw128(sA + i * FT_A_PART, 0, 1024);
+      bd[i] = smem_desc_sw128(sB + i * FT_B_PART, b_mn ? FT_B_PART : 0u, 1024);
     }
-  } else {
-    // ---------------------------------------------------------------------------------------------- producers
-    // chunk c: registers -> stage c % 3 (once the MMAs of chunk c-3 have read it), refill the register set with chunk c+2
-    auto do_chunk = [&](int c, float4 (&ra)[8], float4 (&rb)[4]) {
-      const int s = c % FT_NSTAGE;
-      if (c >= FT_NSTAGE) mbar_wait(sm.bar(s), (uint32_t)((c / FT_NSTAGE - 1) & 1));
-      store_chunk(s, ra, rb);
-      if (c + 2 < nchunk) load_chunk(c + 2, ra, rb);
-      fence_proxy_async_smem();   // generic-proxy stores -> visible to tcgen05.mma (async proxy)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sm.full(s));
-    };
+    wgmma_fence();
+    if (b_mn) mma6<0, 1>(d, ad, bd, 2u, 128u, c == 0);
+    else      mma6<0, 0>(d, ad, bd, 2u, 2u, c == 0);
+    wgmma_commit();
+    wgmma_wait<1>();   // chunk c-1 has retired: its stage may be overwritten
+    if (c > 0 && (tid & 127) == 0) mbar_arrive(sm.bar((c - 1) % FT_NSTAGE));
+  };
+  {
     float4 ra0[8], rb0[4], ra1[8], rb1[4];
     load_chunk(0, ra0, rb0);
     if (nchunk > 1) load_chunk(1, ra1, rb1);
@@ -213,16 +200,18 @@ conv_gemm_f32_tc_kernel(const ConvGemmParams p) {
       do_chunk(c, ra0, rb0);
       if (c + 1 < nchunk) do_chunk(c + 1, ra1, rb1);
     }
-    mbar_wait(sm.bar((nchunk - 1) % FT_NSTAGE), (uint32_t)(((nchunk - 1) / FT_NSTAGE) & 1));   // in-order: all retired
-    tc_fence_after();
+    wgmma_wait<0>();
+    __syncthreads();   // every MMA has read its stage: stage 0 holds the accumulator tile from here on
+    acc_store_smem<64>(d, sm.stage(0) >> 2, 64 * wg);
+    __syncthreads();
+  }
 
-  // ---- epilogue: warp w reads TMEM lanes 32 (w & 3) .., columns 32 (w >> 2) ..; one pixel x 32 channels per thread
+  // ---- epilogue: warp w reads accumulator rows 32 (w & 3) .., columns 32 (w >> 2) ..; one pixel x 32 channels per thread
   {
     const int q = warp & 3, half = warp >> 2;
     const long long m = m0 + q * 32 + lane;
     uint32_t r[32];
-    tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + half * 32, r);
-    tmem_ld_wait();
+    acc_ld_x32((sm.stage(0) >> 2) + (q * 32 + lane) * 64 + half * 32, r);
     if (m < M) {
       const int ox = (int)(m % p.OW);
       const int oy = (int)((m / p.OW) % p.OH);
@@ -260,13 +249,6 @@ conv_gemm_f32_tc_kernel(const ConvGemmParams p) {
       }
     }
   }
-  }  // producers
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 64);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -276,9 +258,7 @@ __global__ void __launch_bounds__(FT_THREADS)
 conv_wgrad_f32_tc_kernel(const ConvWgradParams p) {
   extern __shared__ uint8_t ft_smem_raw[];
   const FtSmem sm = ft_carve(ft_smem_raw);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(ft_smem_raw + (sm.tmem_slot - smem_u32(ft_smem_raw)));
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int a0 = blockIdx.x * 128, b0 = blockIdx.y * 64;
   const int t = blockIdx.z % p.ntaps, split = blockIdx.z / p.ntaps;
   const long long M = (long long)p.NB * p.OH * p.OW;
@@ -289,14 +269,10 @@ conv_wgrad_f32_tc_kernel(const ConvWgradParams p) {
   const WgradTap tap = p.taps[t];
 
   if (tid == 0) {
-    for (int i = 0; i < FT_NSTAGE; ++i) { mbar_init(sm.bar(i), 1); mbar_init(sm.full(i), 8); }
+    for (int i = 0; i < FT_NSTAGE; ++i) { mbar_init(sm.bar(i), 2); mbar_init(sm.full(i), 8); }
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc(sm.tmem_slot, 64);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
   const int nchunk = mbeg < mend ? (int)((mend - mbeg + 63) / 64) : 0;
 
   // loader: pixel row (tid >> 2) of the 64-pixel chunk; P channels a0 + (tid & 3) * 32 .. + 31 (slab (tid & 3) >> 1),
@@ -333,64 +309,52 @@ conv_wgrad_f32_tc_kernel(const ConvWgradParams p) {
     for (int j = 0; j < 2; ++j) stage8(sB, FT_B_PART, row, q_seg0 + j, rq[2 * j], rq[2 * j + 1]);
   };
 
-  constexpr uint32_t idesc = umma_idesc_bf16(128, 64, 1, 1);   // both operands MN-major (K = pixels)
-  if (warp == 8) {
-    // ---------------------------------------------------------------------------------------------- MMA issuer
-    for (int c = 0; c < nchunk; ++c) {
-      const int s = c % FT_NSTAGE;
-      mbar_wait(sm.full(s), (uint32_t)((c / FT_NSTAGE) & 1));
-      tc_fence_after();
-      const uint32_t sA = sm.stage(s), sB = sm.stage(s) + 3 * FT_A_PART;
-      uint64_t ad[3], bd[3];
+  // both operands MN-major (K = pixels); warpgroup wg takes the 64-channel slab wg of P (accumulator rows 64 wg ..)
+  float d[32];
+  auto do_chunk = [&](int c, float4 (&rp)[8], float4 (&rq)[4]) {
+    const int s = c % FT_NSTAGE;
+    if (c >= FT_NSTAGE) mbar_wait_mma(sm.bar(s), (uint32_t)((c / FT_NSTAGE - 1) & 1));
+    store_chunk(s, rp, rq);
+    if (c + 2 < nchunk) load_chunk(c + 2, rp, rq);
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(sm.full(s));
+    mbar_wait_mma(sm.full(s), (uint32_t)((c / FT_NSTAGE) & 1));
+    const uint32_t sA = sm.stage(s) + wg * FT_B_PART, sB = sm.stage(s) + 3 * FT_A_PART;
+    uint64_t ad[3], bd[3];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        ad[i] = umma_smem_desc_sw128(sA + i * FT_A_PART, FT_B_PART, 1024);   // two 64-channel slabs 8 KiB apart
-        bd[i] = umma_smem_desc_sw128(sB + i * FT_B_PART, FT_B_PART, 1024);
-      }
-      if (elect_one_sync()) {
-        mma6(tmem, ad, bd, 128u, 128u, idesc, c == 0);    // 16 pixels = 16 rows x 128 B = 2 KiB per K-step
-        umma_commit(sm.bar(s));
-      }
-      __syncwarp();
+    for (int i = 0; i < 3; ++i) {
+      ad[i] = smem_desc_sw128(sA + i * FT_A_PART, FT_B_PART, 1024);
+      bd[i] = smem_desc_sw128(sB + i * FT_B_PART, FT_B_PART, 1024);
     }
-  } else {
-    // ---------------------------------------------------------------------------------------------- producers
-    auto do_chunk = [&](int c, float4 (&rp)[8], float4 (&rq)[4]) {
-      const int s = c % FT_NSTAGE;
-      if (c >= FT_NSTAGE) mbar_wait(sm.bar(s), (uint32_t)((c / FT_NSTAGE - 1) & 1));
-      store_chunk(s, rp, rq);
-      if (c + 2 < nchunk) load_chunk(c + 2, rp, rq);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sm.full(s));
-    };
+    wgmma_fence();
+    mma6<1, 1>(d, ad, bd, 128u, 128u, c == 0);    // 16 pixels = 16 rows x 128 B = 2 KiB per K-step
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (c > 0 && (tid & 127) == 0) mbar_arrive(sm.bar((c - 1) % FT_NSTAGE));
+  };
+  if (nchunk == 0) return;  // uniform across the CTA
+  {
     float4 rp0[8], rq0[4], rp1[8], rq1[4];
-    if (nchunk > 0) load_chunk(0, rp0, rq0);
+    load_chunk(0, rp0, rq0);
     if (nchunk > 1) load_chunk(1, rp1, rq1);
     for (int c = 0; c < nchunk; c += 2) {
       do_chunk(c, rp0, rq0);
       if (c + 1 < nchunk) do_chunk(c + 1, rp1, rq1);
     }
-    if (nchunk > 0) {
-      mbar_wait(sm.bar((nchunk - 1) % FT_NSTAGE), (uint32_t)(((nchunk - 1) / FT_NSTAGE) & 1));
-      tc_fence_after();
-      const int q = warp & 3, half = warp >> 2;
-      const int a = a0 + q * 32 + lane;
-      uint32_t r[32];
-      tmem_ld_x32(tmem + ((uint32_t)(q * 32) << 16) + half * 32, r);
-      tmem_ld_wait();
-      if (a < p.pC) {
-        float* dw = p.dw + tap.w_off + (long long)a * p.a_stride + (long long)(b0 + half * 32) * p.b_stride;
+    wgmma_wait<0>();
+    __syncthreads();   // every MMA has read its stage: stage 0 holds the accumulator tile from here on
+    acc_store_smem<64>(d, sm.stage(0) >> 2, 64 * wg);
+    __syncthreads();
+    const int q = warp & 3, half = warp >> 2;
+    const int a = a0 + q * 32 + lane;
+    uint32_t r[32];
+    acc_ld_x32((sm.stage(0) >> 2) + (q * 32 + lane) * 64 + half * 32, r);
+    if (a < p.pC) {
+      float* dw = p.dw + tap.w_off + (long long)a * p.a_stride + (long long)(b0 + half * 32) * p.b_stride;
 #pragma unroll
-        for (int e = 0; e < 32; ++e) atomicAdd(dw + (long long)e * p.b_stride, __uint_as_float(r[e]));
-      }
+      for (int e = 0; e < 32; ++e) atomicAdd(dw + (long long)e * p.b_stride, __uint_as_float(r[e]));
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 64);
   }
 }
 

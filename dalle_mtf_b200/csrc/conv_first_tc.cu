@@ -1,21 +1,22 @@
-// K11 (first layer) — the 4x4 / stride-2 / SAME convolution of the RGB image (Cin = 3) on tcgen05.
+// K11 (first layer) — the 4x4 / stride-2 / SAME convolution of the RGB image (Cin = 3) on wgmma.
 //
 // Reference: the first conv_downsample of DiscreteVAE.encoder, src/vae_tf/models.py:95 (tf.layers.conv2d, HWIO kernel).
 // K = 4*4*3 = 48 is too thin for a TMA-fed implicit GEMM (a 3-channel pixel is 12 bytes), so the CTA gathers the
 // patches itself: a 128-pixel output tile (8 x 16) is staged as an A operand [128 pixels][64] (48 taps + 16 zero columns)
-// in the 128-byte-swizzled K-major layout the UMMA descriptor expects, the weights as B [Cout][64] likewise, and ONE
-// group of tcgen05.mma (M = 128, N = Cout, K = 64) produces the tile in TMEM.  The fp32 pixels are split into bf16
-// hi + lo parts (two A tiles, two accumulating MMA groups), so the input keeps ~16 bits of mantissa; the weights are
-// rounded to bf16 like those of every other tensor-core layer.  Output: bias added in fp32, rounded to bf16, NHWC —
-// each thread writes its pixel's Cout channels as contiguous 16-byte stores.  Also absorbs the fp32 -> bf16 cast of
-// the image.  HBM-bound by design: 12 B read + 2*Cout B written per output pixel.
+// in the 128-byte-swizzled K-major layout the wgmma descriptor expects, the weights as B [Cout][64] likewise, and the
+// CTA's warpgroup produces the tile in 64 x 64 blocks (wgmma m64n64k16, K = 64) in registers.  The fp32 pixels are split
+// into bf16 hi + lo parts (two A tiles, two accumulating MMA groups), so the input keeps ~16 bits of mantissa; the
+// weights are rounded to bf16 like those of every other tensor-core layer.  Output: bias added in fp32, rounded to
+// bf16, NHWC, straight from the accumulator fragment.  Also absorbs the fp32 -> bf16 cast of the image.  HBM-bound by
+// design: 12 B read + 2*Cout B written per output pixel.
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace db200 {
 namespace {
 
-constexpr int CFT_TH = 8, CFT_TW = 16;                    // output tile (128 pixels = TMEM lanes)
+constexpr int CFT_TH = 8, CFT_TW = 16;                    // output tile (128 pixels = accumulator rows)
 constexpr int CFT_PH = 2 * CFT_TH + 2, CFT_PW = 2 * CFT_TW + 2;
 constexpr uint32_t CFT_A_BYTES = 128 * 128;               // [128][64] bf16
 constexpr uint32_t CFT_PATCH_FLOATS = CFT_PH * CFT_PW * 3;
@@ -26,28 +27,25 @@ __device__ __forceinline__ void st_shared_v4u(uint32_t addr, uint32_t a, uint32_
 
 }  // namespace
 
-// smem: [1024 align] A_hi | A_lo | B [Cout][64] bf16 | patch f32 [PH][PW][3] | bias f32 [Cout] | barrier + tmem slot
+// smem: [1024 align] A_hi | A_lo | B [Cout][64] bf16 | patch f32 [PH][PW][3] | bias f32 [Cout]
 __global__ void __launch_bounds__(128)
 conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,
-                     bf16* __restrict__ y, int NB, int H, int W, int Cout, int tmem_cols) {
+                     bf16* __restrict__ y, int NB, int H, int W, int Cout) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   const uint32_t sAh = base, sAl = sAh + CFT_A_BYTES, sB = sAl + CFT_A_BYTES;
   const uint32_t sPatch = sB + Cout * 128;
   const uint32_t sBias = sPatch + CFT_PATCH_FLOATS * 4;
-  const uint32_t bar = (sBias + Cout * 4 + 15u) & ~15u;
-  const uint32_t tmem_slot = bar + 8;
   float* patch = reinterpret_cast<float*>(smem_raw + (sPatch - raw));
   float* sbias = reinterpret_cast<float*>(smem_raw + (sBias - raw));
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int Ho = H / 2, Wo = W / 2;
   const int tiles_w = (Wo + CFT_TW - 1) / CFT_TW, tiles_h = (Ho + CFT_TH - 1) / CFT_TH;
   const int n_tiles = tiles_w * tiles_h * NB;
 
-  // ---- once per CTA: weights -> B[n][k] = bf16(w[k][n]) (k < 48; zero beyond), swizzled K-major; bias; barrier; TMEM
+  // ---- once per CTA: weights -> B[n][k] = bf16(w[k][n]) (k < 48; zero beyond), swizzled K-major; bias
   for (int i = tid; i < Cout * 8; i += 128) {  // (row n, 16-byte chunk j of 8 taps)
     const int n = i >> 3, j = i & 7;
     uint32_t pk[4];
@@ -61,20 +59,11 @@ conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, c
     st_shared_v4u(sB + n * 128 + (((j ^ (n & 7)) & 7) << 4), pk[0], pk[1], pk[2], pk[3]);
   }
   for (int i = tid; i < Cout; i += 128) sbias[i] = bias ? bias[i] : 0.f;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, (uint32_t)tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  const uint32_t lane_off = uint32_t(warp * 32) << 16;
-  const uint32_t idesc = umma_idesc_bf16(128, Cout, 0, 0);
   const int ly = tid / CFT_TW, lx = tid % CFT_TW;
+  // accumulator fragment of m64n64: rows 16 warp + lane/4 (+8), columns 8 i + 2 (lane % 4) (+1)
+  const int lane = tid & 31, fr = 16 * warp + (lane >> 2), fc = 2 * (lane & 3);
 
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     int t = tile;
     const int tw = t % tiles_w; t /= tiles_w;
@@ -115,54 +104,36 @@ conv_first_tc_kernel(const float* __restrict__ x, const float* __restrict__ w, c
       st_shared_v4u(sAh + off, hi[0], hi[1], hi[2], hi[3]);
       st_shared_v4u(sAl + off, lo[0], lo[1], lo[2], lo[3]);
     }
-    fence_proxy_async_smem();  // generic-proxy stores -> visible to tcgen05.mma (async proxy)
-    tc_fence_before();
+    fence_proxy_async_smem();  // generic-proxy stores -> visible to wgmma (async proxy)
     __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      const uint64_t dh = umma_smem_desc_sw128(sAh, 0, 1024), dl = umma_smem_desc_sw128(sAl, 0, 1024);
-      const uint64_t db = umma_smem_desc_sw128(sB, 0, 1024);
-      if (elect_one_sync()) {
+    // ---- 64 x 64 output blocks: hi and lo products, then + bias, bf16, NHWC
+    for (int mh = 0; mh < 2; ++mh) {
+      const uint64_t dh = smem_desc_sw128(sAh + mh * 64 * 128, 0, 1024), dl = smem_desc_sw128(sAl + mh * 64 * 128, 0, 1024);
+      for (int nb = 0; nb < Cout / 64; ++nb) {
+        const uint64_t db = smem_desc_sw128(sB + nb * 64 * 128, 0, 1024);
+        float d[32];
+        wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma_bf16_ss(tmem, dh + 2u * kk, db + 2u * kk, idesc, kk > 0);
+        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64<0, 0>(d, dh + 2u * kk, db + 2u * kk, kk > 0);
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma_bf16_ss(tmem, dl + 2u * kk, db + 2u * kk, idesc, 1u);
-        umma_commit(bar);
-      }
-      __syncwarp();
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    tc_fence_after();
-    // ---- epilogue: + bias, bf16, one pixel's channels per thread
-    const int oy = oy0 + ly, ox = ox0 + lx;
-    const bool ok = oy < Ho && ox < Wo;
-    bf16* dst = y + (((long long)n * Ho + oy) * Wo + ox) * Cout;
-    for (int c0 = 0; c0 < Cout; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld_x32(tmem + lane_off + c0, r);
-      tmem_ld_wait();
-      if (ok) {
+        for (int kk = 0; kk < 4; ++kk) wgmma_m64n64<0, 0>(d, dl + 2u * kk, db + 2u * kk, 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
 #pragma unroll
-        for (int e = 0; e < 32; e += 8) {
-          uint4 q;
-          q.x = pack_bf16x2(__uint_as_float(r[e]) + sbias[c0 + e], __uint_as_float(r[e + 1]) + sbias[c0 + e + 1]);
-          q.y = pack_bf16x2(__uint_as_float(r[e + 2]) + sbias[c0 + e + 2], __uint_as_float(r[e + 3]) + sbias[c0 + e + 3]);
-          q.z = pack_bf16x2(__uint_as_float(r[e + 4]) + sbias[c0 + e + 4], __uint_as_float(r[e + 5]) + sbias[c0 + e + 5]);
-          q.w = pack_bf16x2(__uint_as_float(r[e + 6]) + sbias[c0 + e + 6], __uint_as_float(r[e + 7]) + sbias[c0 + e + 7]);
-          *reinterpret_cast<uint4*>(dst + c0 + e) = q;
+        for (int h = 0; h < 2; ++h) {
+          const int r = mh * 64 + fr + 8 * h;
+          const int oy = oy0 + r / CFT_TW, ox = ox0 + r % CFT_TW;
+          if (oy >= Ho || ox >= Wo) continue;
+          bf16* dst = y + (((long long)n * Ho + oy) * Wo + ox) * Cout + nb * 64 + fc;
+          const float* bb = sbias + nb * 64 + fc;
+#pragma unroll
+          for (int i = 0; i < 8; ++i)
+            *reinterpret_cast<uint32_t*>(dst + 8 * i) =
+                pack_bf16x2(d[4 * i + 2 * h] + bb[8 * i], d[4 * i + 2 * h + 1] + bb[8 * i + 1]);
         }
       }
     }
-    tc_fence_before();
-    __syncthreads();  // TMEM tile, A tiles and the patch are free for the next tile
-    tc_fence_after();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, (uint32_t)tmem_cols);
+    __syncthreads();  // A tiles and the patch are free for the next tile
   }
 }
 
@@ -174,13 +145,10 @@ int conv_first_tc_launch(cudaStream_t stream, const float* x, const float* w, co
   static const cudaError_t attr_rc = cudaFuncSetAttribute(conv_first_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                           96 * 1024);  // once, thread-safe
   DB200_CUDA(attr_rc);
-  const int tmem_cols = Cout <= 64 ? 64 : (Cout <= 128 ? 128 : 256);
-  // several CTAs per SM hide each other's gather / MMA / store phases (smem ~50 KB and 64..256 TMEM columns each)
-  const int per_sm = tmem_cols <= 128 ? 4 : 2;
-  int grid = sm_count() * per_sm;
+  // several CTAs per SM hide each other's gather / MMA / store phases (smem ~50 KB each)
+  int grid = sm_count() * 4;
   if (grid > tiles) grid = tiles;
-  conv_first_tc_kernel<<<grid, 128, smem, stream>>>(x, w, bias, reinterpret_cast<bf16*>(y_bf16), N, H, W, Cout,
-                                                    tmem_cols);
+  conv_first_tc_kernel<<<grid, 128, smem, stream>>>(x, w, bias, reinterpret_cast<bf16*>(y_bf16), N, H, W, Cout);
   return check_launch("conv_first_tc_kernel");
 }
 

@@ -46,7 +46,7 @@ struct ConvWgradParams {
 };
 
 
-// conv_f32_tc.cu: fp32 activations on tcgen05 through a three-way bf16 split (fp32-accurate products)
+// conv_f32_tc.cu: fp32 activations on wgmma through a three-way bf16 split (fp32-accurate products)
 bool conv_gemm_f32_tc_ok(const ConvGemmParams& p);
 int conv_gemm_f32_tc_launch(cudaStream_t stream, const ConvGemmParams& p);
 bool conv_wgrad_f32_tc_ok(const ConvWgradParams& p);

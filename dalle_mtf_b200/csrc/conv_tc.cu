@@ -1,4 +1,4 @@
-// K11 (tensor-core path) — NHWC bf16 convolutions as im2col-free implicit GEMMs on tcgen05.
+// K11 (tensor-core path) — NHWC bf16 convolutions as im2col-free implicit GEMMs on wgmma.
 //
 // (1) gather-GEMM  (forward conv, forward conv-transpose, every dgrad):
 //        y[pix, n] = epi( sum_{tap} sum_k  x[src(pix, tap), k] * W_tap[k][n] )
@@ -11,11 +11,13 @@
 //     forward, stride-2 dgrad) run one launch per output parity.  No im2col buffer exists in HBM or smem.
 // (2) wgrad:  dW_tap[a][b] += sum_pix P[src(pix,tap), a] * Q[src'(pix,tap), b]
 //     M = a (channels of P), N = b (channels of Q), K = pixels: both operands are the same 4-D TMA boxes used as
-//     MN-major UMMA operands (k rows = pixels); split over pixels, fp32 accumulation in TMEM, red.add into dW.
+//     MN-major wgmma operands (k rows = pixels); split over pixels, fp32 accumulation in registers, red.add into dW.
 //
-// Same warp-specialised pipeline as gemm.cu (TMA producer / MMA issuer / TMEM accumulators / 8 epilogue warps).
+// Same warp-specialised pipeline as gemm.cu (TMA producer warp / two wgmma consumer warpgroups whose accumulators go
+// through a shared-memory tile to the 8-warp epilogue).
 // Reference: tf.layers.conv2d / conv2d_transpose call sites src/vae_tf/models.py:95-109, 139-155 and their gradients.
 #include "gemm_common.cuh"  // staging helpers for coalesced epilogue I/O
+#include "wgmma.cuh"
 
 namespace db200 {
 
@@ -25,11 +27,14 @@ constexpr uint32_t CT_SLAB = 64 * 128;
 
 template <int BN>
 struct ConvTcCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
+  static_assert(BN == 64 || BN == 128, "wgmma tile width");
+  static constexpr int STAGES = 4;
   static constexpr uint32_t B_BYTES = BN * 64 * 2;
   static constexpr uint32_t STAGE_BYTES = CT_A_BYTES + B_BYTES;
-  static constexpr uint32_t TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
-  static constexpr size_t SMEM_BYTES = 1024 + size_t(STAGES) * STAGE_BYTES + 256 + 8 * 4096 /*epilogue staging*/;
+  static constexpr uint32_t ACC_BYTES = 128 * BN * 4;  // fp32 accumulator tile
+  static constexpr size_t SMEM_BYTES =
+      1024 + ACC_BYTES + size_t(STAGES) * STAGE_BYTES + 256 + 8 * 4096 /*epilogue staging*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "conv shared memory exceeds the H100 per-block limit");
 };
 
 struct ConvTcTap {
@@ -77,12 +82,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t sA = base;
-  const uint32_t sB = base + STAGES * CT_A_BYTES;
-  const uint32_t bars = base + STAGES * Cfg::STAGE_BYTES;
-  const uint32_t full_bar = bars, empty_bar = bars + 8 * STAGES, tfull_bar = bars + 16 * STAGES,
-                 tempty_bar = tfull_bar + 16, tmem_slot = tempty_bar + 16;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
+  const uint32_t sAcc = base;
+  const uint32_t sA = base + Cfg::ACC_BYTES;
+  const uint32_t sB = sA + STAGES * CT_A_BYTES;
+  const uint32_t bars = sA + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t full_bar = bars, empty_bar = bars + 8 * STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (warp == 0 && lane == 0) {
@@ -92,19 +96,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(full_bar + 8 * i, 1);
-      mbar_init(empty_bar + 8 * i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(tfull_bar + 8 * i, 1);
-      mbar_init(tempty_bar + 8 * i, 8);
+      mbar_init(empty_bar + 8 * i, 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   const int total_tiles = p.tiles_n * p.tiles_h * p.tiles_w * p.tiles_c;
   const int nkb = p.ntaps * p.kchunks;
@@ -120,7 +116,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const ConvTcTap tp = p.taps[tap];
           for (int kc = 0; kc < p.kchunks; ++kc) {
-            mbar_wait(empty_bar + 8 * stage, phase ^ 1);
+            mbar_wait_mma(empty_bar + 8 * stage, phase ^ 1);
             const uint32_t fb = full_bar + 8 * stage;
             if (elect_one_sync()) {
             mbar_expect_tx(fb, Cfg::STAGE_BYTES);
@@ -142,43 +138,43 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = umma_idesc_bf16(128, BN, 0, p.b_kmajor ? 0 : 1);
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(full_bar + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t a_base = sA + stage * CT_A_BYTES, b_base = sB + stage * Cfg::B_BYTES;
-        const uint64_t ad0 = umma_smem_desc_sw128(a_base, 0, 1024);
-        const uint64_t bd0 = p.b_kmajor ? umma_smem_desc_sw128(b_base, 0, 1024) : umma_smem_desc_sw128(b_base, CT_SLAB, 1024);
-        const uint64_t bstep = p.b_kmajor ? 2u : 128u;      // (32 B | 2 KiB) >> 4 per 16-deep K-step
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16_ss(d_tmem, ad0 + 2u * k, bd0 + bstep * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar + 8 * stage);
-          if (kb == nkb - 1) umma_commit(tfull_bar + 8 * acc);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
   } else if (warp >= 4) {
-    // Epilogue.  A thread owns one output PIXEL (accumulator row) and its channels are contiguous in NHWC, so the
-    // same coalescing scheme as the GEMM applies: 32 pixels x 64 channels are transposed through a swizzled 4 KiB smem
-    // block and every global access covers 4 pixels x 128 contiguous bytes (outputs, residual and ReLU-mask operands).
-    const int ew = warp - 4, wq = ew & 3, half = ew >> 2;
+    // Consumers: warpgroup g computes accumulator rows (pixels) [64 g, 64 g + 64) with wgmma, then all 8 warps run the
+    // epilogue from the shared-memory accumulator tile.  A thread owns one output PIXEL (accumulator row) and its
+    // channels are contiguous in NHWC, so the same coalescing scheme as the GEMM applies: 32 pixels x 64 channels are
+    // transposed through a swizzled 4 KiB smem block and every global access covers 4 pixels x 128 contiguous bytes
+    // (outputs, residual and ReLU-mask operands).
+    const int ew = warp - 4, wq = ew & 3, half = ew >> 2, wg = ew >> 2;
     constexpr int HALF = BN / 2;
     const uint32_t stg = bars + 256 + ew * STG_BYTES;
     const int slot = lane & 7, rsub = lane >> 3;
-    uint32_t acc = 0, acc_phase = 0;
+    const uint64_t bstep = p.b_kmajor ? 2u : 128u;      // (32 B | 2 KiB) >> 4 per 16-deep K-step
+    float d[BN / 2];
+    uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const ConvTile t = conv_decode(p, tile);
+      uint32_t prev_stage = 0;
+      for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait_mma(full_bar + 8 * stage, phase);
+        const uint32_t a_base = sA + stage * CT_A_BYTES + wg * (64u * 128u), b_base = sB + stage * Cfg::B_BYTES;
+        const uint64_t ad0 = smem_desc_sw128(a_base, 0, 1024);
+        const uint64_t bd0 = smem_desc_sw128(b_base, p.b_kmajor ? 0u : CT_SLAB, 1024);
+        wgmma_fence();
+        if (p.b_kmajor) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_m64<BN, 0, 0>(d, ad0 + 2u * k, bd0 + bstep * k, (kb > 0 || k > 0) ? 1u : 0u);
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_m64<BN, 0, 1>(d, ad0 + 2u * k, bd0 + bstep * k, (kb > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
       // element offsets (or -1) of the 8 pixels this lane moves during block loads / stores
       long long poff[8];
 #pragma unroll
@@ -190,9 +186,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
                       ? (((long long)n * p.out_H + (oy * p.out_stride + p.oa)) * p.out_W + (ox * p.out_stride + p.ob)) * p.Nn
                       : -1;
       }
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + acc * BN + half * HALF + (uint32_t(wq * 32) << 16);
+      named_bar_sync(1, 256);  // the previous tile's epilogue is done with the accumulator tile
+      acc_store_smem<BN>(d, sAcc >> 2, 64 * wg);
+      named_bar_sync(1, 256);
+      const uint32_t t_addr = (sAcc >> 2) + (wq * 32 + lane) * BN + half * HALF;
       const int cbase = t.c_blk * BN + half * HALF;
       constexpr int CW = (HALF >= 64) ? 64 : 32;  // channels per staged block
 #pragma unroll 1
@@ -203,8 +200,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
 #pragma unroll
         for (int h = 0; h < CW / 32; ++h) {
           uint32_t rr[32];
-          tmem_ld_x32(t_addr + cb * CW + h * 32, rr);
-          tmem_ld_wait();
+          acc_ld_x32(t_addr + cb * CW + h * 32, rr);
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[h * 32 + j] = __uint_as_float(rr[j]);
         }
@@ -257,17 +253,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         }
         __syncwarp();
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar + 8 * acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
@@ -344,7 +330,7 @@ static int run_gather(cudaStream_t stream, ConvTcParams& p, const CUtensorMap* t
   p.tiles_h = (p.OH + p.TH - 1) / p.TH;
   p.tiles_n = (p.NB + p.TN - 1) / p.TN;
   p.kchunks = p.K / 64;
-  const int bn = p.Nn >= 256 ? 256 : (p.Nn >= 128 ? 128 : 64);
+  const int bn = p.Nn >= 128 ? 128 : 64;
   p.tiles_c = (p.Nn + bn - 1) / bn;
   CUtensorMap tmB;
   int rc;
@@ -357,13 +343,12 @@ static int run_gather(cudaStream_t stream, ConvTcParams& p, const CUtensorMap* t
     rc = make_tmap_bf16(&tmB, w_bf16, 3, dims, str, box);
   } else rc = make_tmap_2d(&tmB, w_bf16, (uint64_t)p.Nn, (uint64_t)wrows, (uint64_t)p.Nn, 64, 64);
   if (rc != DB200_OK) return rc;
-  if (bn == 256) return conv_tc_launch<256>(stream, tmA, tmB, p);
   if (bn == 128) return conv_tc_launch<128>(stream, tmA, tmB, p);
   return conv_tc_launch<64>(stream, tmA, tmB, p);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// wgrad on tcgen05
+// wgrad on wgmma
 // ------------------------------------------------------------------------------------------------------------------
 struct WgradTcTap {
   int pmap, pdy, pdx, qmap, qdy, qdx;
@@ -381,11 +366,14 @@ struct WgradTcParams {
 
 template <int BN>
 struct WgradCfg {
-  static constexpr int STAGES = (BN == 256) ? 2 : 3;
+  static_assert(BN == 64 || BN == 128, "wgmma tile width");
+  static constexpr int STAGES = (BN == 128) ? 2 : 3;
   static constexpr uint32_t A_BYTES = 2 * 128 * 128;         // two 64-channel slabs of [128 pixels][64 ch]
   static constexpr uint32_t B_BYTES = (BN / 64) * 128 * 128;
   static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr size_t SMEM_BYTES = 1024 + size_t(STAGES) * STAGE_BYTES + 256;
+  static constexpr uint32_t ACC_BYTES = 128 * BN * 4;        // fp32 accumulator tile
+  static constexpr size_t SMEM_BYTES = 1024 + ACC_BYTES + size_t(STAGES) * STAGE_BYTES + 256;
+  static_assert(SMEM_BYTES <= 227 * 1024, "wgrad shared memory exceeds the H100 per-block limit");
 };
 
 template <int BN>
@@ -400,12 +388,11 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmP0, const __grid_cons
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  const uint32_t sA = base;
-  const uint32_t sB = base + STAGES * Cfg::A_BYTES;
-  const uint32_t bars = base + STAGES * Cfg::STAGE_BYTES;
-  const uint32_t full_bar = bars, empty_bar = bars + 8 * STAGES, done_bar = bars + 16 * STAGES,
-                 tmem_slot = done_bar + 8;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
+  const uint32_t sAcc = base;
+  const uint32_t sA = base + Cfg::ACC_BYTES;
+  const uint32_t sB = sA + STAGES * Cfg::A_BYTES;
+  const uint32_t bars = sA + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t full_bar = bars, empty_bar = bars + 8 * STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // work item: (tap, a tile, b tile, pixel split)
@@ -422,16 +409,11 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmP0, const __grid_cons
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(full_bar + 8 * i, 1);
-      mbar_init(empty_bar + 8 * i, 1);
+      mbar_init(empty_bar + 8 * i, 2);  // one arrive per consumer warpgroup
     }
-    mbar_init(done_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, BN < 32 ? 32 : BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   if (pt1 > pt0) {
     if (warp == 0) {
@@ -444,7 +426,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmP0, const __grid_cons
           const int ox0 = (t % p.tiles_w) * p.TW; t /= p.tiles_w;
           const int oy0 = (t % p.tiles_h) * p.TH; t /= p.tiles_h;
           const int n0 = t * p.TN;
-          mbar_wait(empty_bar + 8 * stage, phase ^ 1);
+          mbar_wait_mma(empty_bar + 8 * stage, phase ^ 1);
           const uint32_t fb = full_bar + 8 * stage;
           const uint32_t a_dst = sA + stage * Cfg::A_BYTES, b_dst = sB + stage * Cfg::B_BYTES;
           if (elect_one_sync()) {
@@ -457,39 +439,38 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmP0, const __grid_cons
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
-    } else if (warp == 1) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BN, 1, 1);  // both operands MN-major (K = pixels)
-      uint32_t stage = 0, phase = 0;
+    } else if (warp >= 4) {
+      // consumers: warpgroup g owns accumulator rows [64 g, 64 g + 64) = the g-th 64-channel slab of P
+      const int ew = warp - 4, wq = ew & 3, half = ew >> 2, wg = ew >> 2;
+      constexpr int HALF = BN / 2;
+      float d[BN / 2];
+      uint32_t stage = 0, phase = 0, prev_stage = 0;
       for (int pt = pt0; pt < pt1; ++pt) {
-        mbar_wait(full_bar + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t a_base = sA + stage * Cfg::A_BYTES, b_base = sB + stage * Cfg::B_BYTES;
-        const uint64_t ad0 = umma_smem_desc_sw128(a_base, 128 * 128, 1024), bd0 = umma_smem_desc_sw128(b_base, 128 * 128, 1024);
-        if (elect_one_sync()) {
+        mbar_wait_mma(full_bar + 8 * stage, phase);
+        const uint32_t a_base = sA + stage * Cfg::A_BYTES + wg * (128u * 128u), b_base = sB + stage * Cfg::B_BYTES;
+        const uint64_t ad0 = smem_desc_sw128(a_base, 128 * 128, 1024), bd0 = smem_desc_sw128(b_base, 128 * 128, 1024);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 8; ++k)  // 16 pixels (2 KiB) per MMA; 64-channel atoms are 16 KiB apart
-            umma_bf16_ss(tmem_base, ad0 + 128u * k, bd0 + 128u * k, idesc, (pt > pt0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar + 8 * stage);
-          if (pt == pt1 - 1) umma_commit(done_bar);
-        }
-        __syncwarp();
+        for (int k = 0; k < 8; ++k)  // 16 pixels (2 KiB) per MMA; 64-channel atoms are 16 KiB apart
+          wgmma_m64<BN, 1, 1>(d, ad0 + 128u * k, bd0 + 128u * k, (pt > pt0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (pt > pt0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+        prev_stage = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-    } else if (warp >= 4) {
-      const int ew = warp - 4, wq = ew & 3, half = ew >> 2;
-      constexpr int HALF = BN / 2;
-      mbar_wait(done_bar, 0);
-      tc_fence_after();
+      wgmma_wait<0>();
+      acc_store_smem<BN>(d, sAcc >> 2, 64 * wg);
+      named_bar_sync(1, 256);
       const int a = a_blk * 128 + wq * 32 + lane;  // row of the accumulator = channel of P
       float* dst = p.dw + tp.w_off + (long long)a * p.a_stride;
-      const uint32_t t_addr = tmem_base + half * HALF + (uint32_t(wq * 32) << 16);
+      const uint32_t t_addr = (sAcc >> 2) + (wq * 32 + lane) * BN + half * HALF;
 #pragma unroll 1
       for (int c = 0; c < HALF / 32; ++c) {
         const int b0 = b_blk * BN + half * HALF + c * 32;
         if (b0 >= p.qC) break;
         uint32_t r[32];
-        tmem_ld_x32(t_addr + c * 32, r);
-        tmem_ld_wait();
+        acc_ld_x32(t_addr + c * 32, r);
         if (a >= p.pC) continue;
         if (p.b_stride == 1 && b0 + 32 <= p.qC && (((tp.w_off + (long long)a * p.a_stride + b0) & 3) == 0)) {
 #pragma unroll
@@ -505,12 +486,6 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmP0, const __grid_cons
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN < 32 ? 32 : BN);
   }
 }
 
@@ -708,7 +683,7 @@ extern "C" int db200_conv2d_wgrad_tc(db200_stream_t stream_, const db200_conv_de
   WgradTcParams p{};
   p.dw = dw;
   p.pC = c->Cin; p.qC = c->Cout;
-  const int wg_bn = p.qC >= 256 ? 256 : (p.qC >= 128 ? 128 : 64);
+  const int wg_bn = p.qC >= 128 ? 128 : 64;
   p.ntaps = c->KH * c->KW;
   const bf16* xb = reinterpret_cast<const bf16*>(x_bf16);
   const bf16* dyb = reinterpret_cast<const bf16*>(dy_bf16);
@@ -766,7 +741,6 @@ extern "C" int db200_conv2d_wgrad_tc(db200_stream_t stream_, const db200_conv_de
   if (splits < 1) splits = 1;
   const int per = (total_ptiles + splits - 1) / splits;
   p.splits = (total_ptiles + per - 1) / per;  // every split owns at least one pixel tile
-  if (bn == 256) return wgrad_tc_launch<256>(stream, tmP, tmQ, p);
   if (bn == 128) return wgrad_tc_launch<128>(stream, tmP, tmQ, p);
   return wgrad_tc_launch<64>(stream, tmP, tmQ, p);
 }

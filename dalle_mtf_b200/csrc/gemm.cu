@@ -1,54 +1,49 @@
-// K3/K5/K6/K7/K8 — persistent, warp-specialised bf16 GEMM on tcgen05 for sm_100a.
+// K3/K5/K6/K7/K8 — persistent, warp-specialised bf16 GEMM on wgmma for sm_90a.
 //
-//   D[M,N] = A[M,K] * B[K,N],  fp32 accumulation in TMEM, operands staged in shared memory by TMA (128B swizzle).
+//   D[M,N] = A[M,K] * B[K,N],  fp32 accumulation in registers, operands staged in shared memory by TMA (128B swizzle).
 //
-//   warp 0   : TMA producer (one elected lane)            smem ring: STAGES x {A 128x64, B BNx64} bf16
-//   warp 1   : MMA issuer  (one elected lane, tcgen05.mma cta_group::1, UMMA 128 x BN x 16)
-//   warp 2   : TMEM allocator / deallocator (2 accumulator stages of BN columns -> epilogue overlaps next tile)
-//   warp 3   : idle
-//   warps 4-11: epilogue (tcgen05.ld; each accumulator row is split between two threads) -> bias / ReLU /
-//               residual / split-K reduction / cross-entropy statistics and gradient
+//   warp 0    : TMA producer (one elected lane)            smem ring: STAGES x {A 128x64, B BNx64} bf16
+//   warps 1-3 : idle
+//   warps 4-11: two consumer warpgroups.  Warpgroup g issues wgmma m64 x BN x 16 for rows [64g, 64g+64) of the tile;
+//               at the end of a tile both write their accumulators to a shared-memory tile, and the 8 warps run the
+//               epilogue on it (each accumulator row split between two threads) -> bias / ReLU / residual / split-K
+//               reduction / cross-entropy statistics and gradient.  The producer keeps loading the next tile meanwhile.
 //
-// Either operand may be K-major or MN-major in global memory; the tensor maps and the UMMA descriptors absorb the
+// Either operand may be K-major or MN-major in global memory; the tensor maps and the wgmma descriptors absorb the
 // difference, so forward (x*W), dgrad (dy*W^T) and wgrad (x^T*dy) are the same kernel.
 //
 // Reference call sites replaced: every mtf einsum / mtf.layers.dense of src/dalle_mtf/models.py (235-244, 303-311,
 // 317-324, 361-371, 391-395) and their gradients produced by mtf.gradients (src/optimizers.py:34).
-#include <cstdlib>
-
 #include "gemm_common.cuh"
+#include "wgmma.cuh"
 
 namespace db200 {
 
-template <int BN>
-struct GemmCfg {
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
-  static constexpr uint32_t B_BYTES = BN * BK * 2;
-  static constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr uint32_t TMEM_COLS = 2 * BN;  // 512 or 256: power of two >= 32
-  static constexpr size_t SMEM_BYTES =
-      1024 /*align slack*/ + size_t(STAGES) * STAGE_BYTES + 256 /*barriers*/ + 8 * 4096 /*epilogue staging*/;
-};
+// BN = 128: the 128 x 128 fp32 accumulator tile (64 KiB) and four 32 KiB stages fit the 227 KiB of an H100 SM.
+constexpr int GBN = 128;
+constexpr int G_STAGES = 4;
+constexpr uint32_t G_B_BYTES = GBN * BK * 2;
+constexpr uint32_t G_STAGE_BYTES = A_BYTES + G_B_BYTES;
+constexpr uint32_t G_ACC_BYTES = BM * GBN * 4;
+constexpr size_t G_SMEM_BYTES =
+    1024 /*align slack*/ + G_ACC_BYTES + size_t(G_STAGES) * G_STAGE_BYTES + 256 /*barriers*/ + 8 * 4096 /*staging*/;
+static_assert(G_SMEM_BYTES <= 227 * 1024, "GEMM shared memory exceeds the H100 per-block limit");
 
-template <int BN>
+template <int TA, int TB>  // operand majors (1 = MN-major), compile-time for wgmma
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using Cfg = GemmCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
+  constexpr int BN = GBN;
+  constexpr int STAGES = G_STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024-byte alignment
-  const uint32_t sA = base;
-  const uint32_t sB = base + STAGES * A_BYTES;
-  const uint32_t bars = base + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t sAcc = base;
+  const uint32_t sA = base + G_ACC_BYTES;
+  const uint32_t sB = sA + STAGES * A_BYTES;
+  const uint32_t bars = sA + STAGES * G_STAGE_BYTES;
   const uint32_t full_bar = bars;                   // STAGES x 8 B
   const uint32_t empty_bar = bars + 8 * STAGES;     // STAGES x 8 B
-  const uint32_t tfull_bar = bars + 16 * STAGES;    // 2 x 8 B
-  const uint32_t tempty_bar = tfull_bar + 16;       // 2 x 8 B
-  const uint32_t tmem_slot = tempty_bar + 16;       // 4 B
   const uint32_t stg_base = bars + 256;             // 8 x STG_BYTES, 16-byte aligned
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -60,38 +55,29 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(full_bar + 8 * i, 1);
-      mbar_init(empty_bar + 8 * i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(tfull_bar + 8 * i, 1);
-      mbar_init(tempty_bar + 8 * i, 8);  // one arrive per epilogue warp
+      mbar_init(empty_bar + 8 * i, 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   const int total_tiles = p.m_tiles * p.n_tiles * p.splits;
 
   if (warp == 0) {
     // ------------------------------------------------------------------ TMA producer
-    // converged warp, issuer picked by elect.sync (see gemm2.cu): TMA instructions compile to plain uniform-datapath code
-    {
-      uint32_t stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const TileCoord t = decode_tile(p, tile);
-        const int m0 = t.m_blk * BM, n0 = t.n_blk * BN;
-        for (int kb = t.kb0; kb < t.kb1; ++kb) {
-          mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-          const uint32_t fb = full_bar + 8 * stage;
-          if (elect_one_sync()) {
-          mbar_expect_tx(fb, Cfg::STAGE_BYTES);
+    // converged warp, issuer picked by elect.sync: TMA instructions compile to plain uniform-datapath code
+    uint32_t stage = 0, phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
+      const int m0 = t.m_blk * BM, n0 = t.n_blk * BN;
+      for (int kb = t.kb0; kb < t.kb1; ++kb) {
+        mbar_wait_mma(empty_bar + 8 * stage, phase ^ 1);
+        const uint32_t fb = full_bar + 8 * stage;
+        if (elect_one_sync()) {
+          mbar_expect_tx(fb, G_STAGE_BYTES);
           const int k0 = kb * BK;
           const uint32_t a_dst = sA + stage * A_BYTES;
-          const uint32_t b_dst = sB + stage * Cfg::B_BYTES;
+          const uint32_t b_dst = sB + stage * G_B_BYTES;
           if (p.a_3d) {
             tma_load_3d(a_dst, &tmA, fb, 0, k0, m0 >> 6);
           } else if (p.a_mn) {
@@ -108,134 +94,125 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           } else {
             tma_load_2d(b_dst, &tmB, fb, k0, n0);
           }
-          }  // elect
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    const uint32_t idesc = umma_idesc_bf16(BM, BN, p.a_mn, p.b_mn);
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const TileCoord t = decode_tile(p, tile);
-      mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = t.kb0; kb < t.kb1; ++kb) {
-        mbar_wait(full_bar + 8 * stage, phase);
-        tc_fence_after();
-        // K-major: a K-step advances 16 elements (32 B) inside the 128 B swizzle row; MN-major: 16 k-rows (2 KiB), 64-wide
-        // MN atoms are SLAB_BYTES apart (LBO).  One descriptor base per operand tile + a constant per K-step, all in
-        // uniform registers; the issuing lane is picked by elect.sync.
-        const uint32_t a_base = sA + stage * A_BYTES;
-        const uint32_t b_base = sB + stage * Cfg::B_BYTES;
-        const uint64_t ad0 = p.a_mn ? umma_smem_desc_sw128(a_base, SLAB_BYTES, 1024) : umma_smem_desc_sw128(a_base, 0, 1024);
-        const uint64_t bd0 = p.b_mn ? umma_smem_desc_sw128(b_base, SLAB_BYTES, 1024) : umma_smem_desc_sw128(b_base, 0, 1024);
-        const uint64_t astep = p.a_mn ? 128u : 2u, bstep = p.b_mn ? 128u : 2u;
-        if (elect_one_sync()) {
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_bf16_ss(d_tmem, ad0 + k * astep, bd0 + k * bstep, idesc, (kb > t.kb0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar + 8 * stage);                  // frees the smem slot when these MMAs retire
-          if (kb == t.kb1 - 1) umma_commit(tfull_bar + 8 * acc);  // accumulator complete -> epilogue
         }
         __syncwarp();
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
   } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue: 8 warps
-    // warp w may only touch TMEM lanes 32*(w%4)..+31, so warps 4-7 take the left half of the tile's columns and
-    // warps 8-11 the right half: every accumulator row is finished by two threads.
+    // ------------------------------------------------------------------ consumers: MMA, then epilogue
     const int ew = warp - 4;
-    const int wq = ew & 3;
-    const int half = ew >> 2;
-    constexpr int CH = BN / 64;  // 32-column chunks per half
+    const int wg = ew >> 2;        // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
+    const int wq = ew & 3;         // epilogue: rows [32 wq, 32 wq + 32) ...
+    const int half = ew >> 2;      // ... and columns [half * BN/2, (half + 1) * BN/2)
+    constexpr int CH = BN / 64;    // 32-column chunks per half
     const uint32_t stg = stg_base + ew * STG_BYTES;
-    uint32_t acc = 0, acc_phase = 0;
+    // K-major: a K-step advances 16 elements (32 B) inside the 128 B swizzle row and warpgroup g starts 64 rows (8 KiB)
+    // in; MN-major: a K-step is 16 k-rows (2 KiB) and warpgroup g takes the g-th 64-wide slab (SLAB_BYTES apart).
+    constexpr uint64_t astep = TA ? 128u : 2u, bstep = TB ? 128u : 2u;
+    const uint32_t a_wg = wg * (TA ? SLAB_BYTES : 64u * 128u);
+    float d[BN / 2];
+    uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
       const int row0 = t.m_blk * BM + wq * 32;
       const int row = row0 + lane;
       const bool row_ok = row < p.M;
       const int cbase = t.n_blk * BN + half * (BN / 2);
-      // pull this half-tile's bias into L1 while the accumulator is still being produced: the epilogue's first use of
-      // it sat on an L2 round trip per 32-column chunk (ncu source page: top stall of the CE epilogues)
+      // pull this half-tile's bias into L1 and the per-element operands (ReLU mask / residual rows) into L2 while
+      // the accumulator is being produced
       if (p.bias && lane < BN / 64 && cbase + lane * 32 < p.N)
         asm volatile("prefetch.global.L1 [%0];" ::"l"(p.bias + cbase + lane * 32));
-      // same for the per-element operands the epilogue will read (ReLU mask / residual rows): DRAM -> L2 now
       if (row_ok && cbase < p.N) {
-        if (p.aux) {
-          const bf16* a = p.aux + (long long)row * p.ldaux + cbase;
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(a));
-          if (BN == 256 && cbase + 64 < p.N) asm volatile("prefetch.global.L2 [%0];" ::"l"(a + 64));
-        }
-        if (p.residual) {
-          const bf16* a = p.residual + (long long)row * p.ldr + cbase;
-          asm volatile("prefetch.global.L2 [%0];" ::"l"(a));
-          if (BN == 256 && cbase + 64 < p.N) asm volatile("prefetch.global.L2 [%0];" ::"l"(a + 64));
-        }
+        if (p.aux) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.aux + (long long)row * p.ldaux + cbase));
+        if (p.residual) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + (long long)row * p.ldr + cbase));
       }
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + acc * BN + half * (BN / 2) + (uint32_t(wq * 32) << 16);
+      uint32_t prev_stage = 0;
+      // zero the accumulator here rather than through wgmma's scale-d: its registers are then dead between the
+      // shared-memory store of one tile and the start of the next (no spill around the epilogue)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      for (int kb = t.kb0; kb < t.kb1; ++kb) {
+        mbar_wait_mma(full_bar + 8 * stage, phase);
+        const uint32_t a_base = sA + stage * A_BYTES + a_wg;
+        const uint32_t b_base = sB + stage * G_B_BYTES;
+        const uint64_t ad0 = smem_desc_sw128(a_base, TA ? SLAB_BYTES : 0u, 1024);
+        const uint64_t bd0 = smem_desc_sw128(b_base, TB ? SLAB_BYTES : 0u, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_m64n128<TA, TB>(d, ad0 + k * astep, bd0 + k * bstep, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (kb > t.kb0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+      named_bar_sync(1, 256);  // the previous tile's epilogue has finished reading the accumulator tile
+      acc_store_smem<BN>(d, sAcc >> 2, 64 * wg);
+      named_bar_sync(1, 256);
+      const uint32_t t_addr = (sAcc >> 2) + (wq * 32 + lane) * BN + half * (BN / 2);
       switch (p.mode) {
         case DB200_EPI_STORE:    epi_store<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
-        case DB200_EPI_ATOMIC:   epi_atomic<CH>(p, t_addr, row, row_ok, cbase); break;
+        case DB200_EPI_ATOMIC:
+          epi_atomic<CH>(p, reinterpret_cast<float*>(p.D) + (long long)t.split * p.M * p.ldd, row, row_ok, cbase,
+                         t_addr);
+          break;
         case DB200_EPI_RELU_BWD: epi_relu_bwd<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
         case DB200_EPI_CE_STATS: epi_ce_stats<CH>(p, t_addr, row, row_ok, cbase, t.n_blk * 2 + half); break;
         case DB200_EPI_CE_GRAD:  epi_ce_grad<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
-        default: break;  // mode -1 (DB200_GEMM_NOEPI=1, timing experiments only): drain nothing
+        default: break;
       }
-      // release the accumulator stage back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar + 8 * acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
-template <int BN>
+template <int TA, int TB>
 static int launch_gemm(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
-  using Cfg = GemmCfg<BN>;
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)Cfg::SMEM_BYTES);  // once, thread-safe (magic static)
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB>,
+                                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                          (int)G_SMEM_BYTES);  // once, thread-safe (magic static)
   DB200_CUDA(attr_rc);
   const int total = p.m_tiles * p.n_tiles * p.splits;
   const int grid = total < sm_count() ? total : sm_count();
-  gemm_tc_kernel<BN><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_tc_kernel<TA, TB><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
   return check_launch("gemm_tc_kernel");
-}
-
-int launch_gemm_2cta(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p);
-
-// 2-CTA pairs (gemm2.cu) when there are enough 256x256 tiles to fill the 74 SM pairs.
-static bool use_2cta(const GemmParams& p, int bn) {
-#ifdef DB200_DEV_KNOBS  // development builds only: DB200_GEMM_2CTA=0 disables the pair kernel for A/B timing
-  static const int enabled = [] { const char* e = getenv("DB200_GEMM_2CTA"); return (e == nullptr) ? 1 : (atoi(e) != 0); }();
-  if (!enabled) return false;
-#endif
-  if (bn != 256) return false;
-  const int pair_tiles = ((p.M + 255) / 256) * p.n_tiles * p.splits;
-  return pair_tiles >= sm_count() / 2;
 }
 
 }  // namespace db200
 
 using namespace db200;
 
-extern "C" int db200_gemm_ce_tiles(int N) { return 2 * ((N + 255) / 256); }
+extern "C" int db200_gemm_ce_tiles(int N) { return 2 * ((N + GBN - 1) / GBN); }
+
+// K splits of an ATOMIC product (1 for every other mode)
+static int gemm_splits(int M, int N, int K, const db200_gemm_epilogue* epi) {
+  if (epi->mode != DB200_EPI_ATOMIC) return 1;
+  const int kb_total = (K + BK - 1) / BK;
+  int splits = epi->split_k;
+  if (splits <= 0) {  // auto: fill the machine, keep >= 4 k-blocks per split
+    const int tiles = ((M + BM - 1) / BM) * ((N + GBN - 1) / GBN);
+    splits = sm_count() / (tiles > 0 ? tiles : 1);
+    if (splits > kb_total / 4) splits = kb_total / 4;
+    if (splits < 1) splits = 1;
+  }
+  if (splits > kb_total) splits = kb_total;
+  if (splits < 1) splits = 1;
+  // every split must own at least one k-block
+  const int per = (kb_total + splits - 1) / splits;
+  return (kb_total + per - 1) / per;
+}
+
+extern "C" int64_t db200_gemm_workspace_bytes(int M, int N, int K, const db200_gemm_epilogue* epi) {
+  if (!epi || M <= 0 || N <= 0 || K <= 0) return 0;
+  const int splits = gemm_splits(M, N, K, epi);
+  if (splits > 1) return (int64_t)splits * M * N * (int64_t)sizeof(float);
+  const bool colsum = (epi->mode == DB200_EPI_CE_GRAD || epi->mode == DB200_EPI_RELU_BWD) && epi->colsum;
+  if (colsum) return (int64_t)((M + BM - 1) / BM) * (BM / 32) * N * (int64_t)sizeof(float);
+  return 0;
+}
 
 extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B,
                                int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
@@ -275,23 +252,12 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   if (mode == DB200_EPI_CE_GRAD)
     DB200_REQUIRE(epi->labels && epi->lse && epi->n_valid > 0 && epi->n_valid <= N && epi->alpha > 0.f,
                   DB200_E_INVALID, "gemm: CE_GRAD needs labels/lse, 0 < n_valid <= N and alpha > 0");
-  int splits = 1;
+  DB200_REQUIRE(mode == DB200_EPI_ATOMIC || epi->split_k <= 1, DB200_E_INVALID,
+                "gemm: split_k > 1 is only valid with DB200_EPI_ATOMIC");
+  const int splits = gemm_splits(M, N, K, epi);
   const int kb_total = (K + BK - 1) / BK;
-  if (mode == DB200_EPI_ATOMIC) {
-    splits = epi->split_k;
-    if (splits <= 0) {  // auto: fill the machine, keep >= 4 k-blocks per split
-      const int tiles = ((M + BM - 1) / BM) * ((N + 255) / 256);
-      splits = sm_count() / (tiles > 0 ? tiles : 1);
-      if (splits > kb_total / 4) splits = kb_total / 4;
-      if (splits < 1) splits = 1;
-    }
-    if (splits > kb_total) splits = kb_total;
-    // every split must own at least one k-block
-    const int per = (kb_total + splits - 1) / splits;
-    splits = (kb_total + per - 1) / per;
-  } else {
-    DB200_REQUIRE(epi->split_k <= 1, DB200_E_INVALID, "gemm: split_k > 1 is only valid with DB200_EPI_ATOMIC");
-  }
+  DB200_REQUIRE(workspace_ok(epi->workspace, epi->workspace_bytes, db200_gemm_workspace_bytes(M, N, K, epi)),
+                DB200_E_INVALID, "gemm: needs an aligned epi->workspace of db200_gemm_workspace_bytes() bytes");
 
   GemmParams p;
   p.M = M; p.N = N; p.K = K;
@@ -301,12 +267,6 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   p.splits = splits;
   p.kb_total = kb_total;
   p.mode = mode;
-#ifdef DB200_DEV_KNOBS  // development builds only (make DEV=1): never compiled into the shipped library
-  {  // timing experiments: skip the epilogue work (results are garbage) to expose the TMA + MMA ceiling
-    static const bool noepi = [] { const char* e = getenv("DB200_GEMM_NOEPI"); return e && e[0] == '1'; }();
-    if (noepi) p.mode = -1;
-  }
-#endif
   p.out_f32 = epi->out_f32;
   p.relu = epi->relu;
   p.alpha = epi->alpha;
@@ -325,22 +285,9 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   p.n_valid = epi->n_valid;
   p.colsum = (mode == DB200_EPI_CE_GRAD || mode == DB200_EPI_RELU_BWD) ? epi->colsum : nullptr;
 
-  // tile width: 256 unless that leaves most SMs idle (CE epilogues are defined on 256-wide tiles)
-  int bn = 256;
-  if (mode != DB200_EPI_CE_STATS && mode != DB200_EPI_CE_GRAD) {
-    const int tiles256 = p.m_tiles * ((N + 255) / 256) * splits;
-    if (N <= 128 || tiles256 * 2 <= sm_count()) bn = 128;
-#ifdef DB200_DEV_KNOBS
-    if (const char* e = getenv("DB200_GEMM_BN")) {  // tuning knob (experiments only)
-      const int v = atoi(e);
-      if (v == 128 || v == 256) bn = v;
-    }
-#endif
-  }
-  p.n_tiles = (N + bn - 1) / bn;
+  p.n_tiles = (N + GBN - 1) / GBN;
   p.n_parts = 2 * p.n_tiles;
 
-  const bool two_cta = use_2cta(p, bn);
   // MN-major operands whose MN extent is a multiple of 64: one rank-3 map {64, K, MN/64} (stride of the slab index =
   // 128 bytes) fetches every 64-wide slab of a stage with a single TMA instruction instead of one per slab.
   p.a_3d = (p.a_mn && M % 64 == 0) ? 1 : 0;
@@ -355,17 +302,30 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   } else if (p.a_mn) rc = make_tmap_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 64, BK);
   else               rc = make_tmap_2d(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM);
   if (rc != DB200_OK) return rc;
-  const uint32_t b_cols = two_cta ? 128u : (uint32_t)bn;  // columns of B staged per CTA
   if (p.b_3d) {
     uint64_t dims[3] = {64, (uint64_t)K, (uint64_t)N / 64};
     uint64_t str[2] = {(uint64_t)ldb * 2, 128};
-    uint32_t box[3] = {64, BK, b_cols / 64};
+    uint32_t box[3] = {64, BK, GBN / 64};
     rc = make_tmap_bf16(&tmB, B, 3, dims, str, box);
   } else if (p.b_mn) rc = make_tmap_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, 64, BK);
-  else               rc = make_tmap_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BK, b_cols);
+  else               rc = make_tmap_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BK, GBN);
   if (rc != DB200_OK) return rc;
 
-  if (two_cta) return launch_gemm_2cta(stream, tmA, tmB, p);
-  if (bn == 256) return launch_gemm<256>(stream, tmA, tmB, p);
-  return launch_gemm<128>(stream, tmA, tmB, p);
+  // Sums over tiles go through a workspace and are added in a fixed order after the GEMM (run-to-run identical results):
+  // the per-split slices of a split-K product, and the per-32-row-block column sums of the fused bias gradient.
+  float* const colsum_out = p.colsum;
+  float* const d_out = reinterpret_cast<float*>(D);
+  const int row_blocks = p.m_tiles * (BM / 32);
+  if (p.splits > 1) {
+    p.D = epi->workspace;
+    p.ldd = N;
+  } else if (colsum_out) {
+    p.colsum = static_cast<float*>(epi->workspace);
+  }
+  if (p.a_mn) rc = p.b_mn ? launch_gemm<1, 1>(stream, tmA, tmB, p) : launch_gemm<1, 0>(stream, tmA, tmB, p);
+  else        rc = p.b_mn ? launch_gemm<0, 1>(stream, tmA, tmB, p) : launch_gemm<0, 0>(stream, tmA, tmB, p);
+  if (rc != DB200_OK) return rc;
+  if (p.splits > 1) return reduce_splits_add(stream, static_cast<const float*>(p.D), p.splits, M, N, d_out, ldd);
+  if (colsum_out) return reduce_rows_add(stream, p.colsum, row_blocks, N, colsum_out);
+  return DB200_OK;
 }

@@ -1,14 +1,15 @@
-// Shared between gemm.cu (1-CTA tiles) and gemm2.cu (2-CTA pairs): kernel parameters, tile decoding and the epilogue
-// routines that turn a TMEM accumulator row block into global-memory results.
+// GEMM kernel parameters, tile decoding and the epilogue routines that turn the shared-memory accumulator tile
+// (wgmma.cuh: acc_store_smem / acc_ld_x32) into global-memory results; the convolutions reuse the staging helpers.
 #pragma once
 #include "common.cuh"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace db200 {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int GEMM_THREADS = 384;  // 4 control warps + 8 epilogue warps
+constexpr int GEMM_THREADS = 384;  // 4 control warps + 2 consumer warpgroups
 constexpr int GROUP_M = 8;
 constexpr uint32_t SLAB_BYTES = BK * 128;  // one MN-major slab: [BK k-rows][64 bf16] = 8 KiB
 constexpr uint32_t A_BYTES = BM * BK * 2;  // 16 KiB
@@ -34,11 +35,11 @@ struct GemmParams {
   const float* lse;
   int n_valid;
   int n_parts;  // CE_STATS: partials per row = 2 * n_tiles (one per half tile)
-  float* colsum;  // CE_GRAD / RELU_BWD: colsum[n] += sum_m D[m,n] (bias gradient), or NULL
+  float* colsum;  // CE_GRAD / RELU_BWD: workspace [M/32 row blocks][N] of column sums (bias gradient), or NULL
 };
 
 struct TileCoord {
-  int m_blk, n_blk, kb0, kb1;
+  int m_blk, n_blk, kb0, kb1, split;
 };
 
 __device__ __forceinline__ TileCoord decode_tile(const GemmParams& p, int tile) {
@@ -54,6 +55,7 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmParams& p, int tile) 
   t.m_blk = first_m + in_group % gm;
   t.n_blk = in_group / gm;
   const int per = (p.kb_total + p.splits - 1) / p.splits;
+  t.split = split;
   t.kb0 = split * per;
   t.kb1 = min(p.kb_total, t.kb0 + per);
   return t;
@@ -61,8 +63,8 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmParams& p, int tile) 
 
 
 // ------------------------------------------------------------------------------------------------------------------
-// epilogues.  One thread = one accumulator row x (BN/2) columns, processed in 32-column chunks straight out of TMEM.
-// All tcgen05.ld are executed by the whole warp (they are .sync.aligned); predicates only guard the global accesses.
+// epilogues.  One thread = one accumulator row x (BN/2) columns, processed in 32-column chunks of the shared-memory
+// accumulator tile (`t_addr`: word address of this thread's row at the half tile's first column).
 // ------------------------------------------------------------------------------------------------------------------
 constexpr float kLog2e = 1.4426950408889634f;
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -87,8 +89,8 @@ __device__ __forceinline__ void load8_bf16(const bf16* sp, float* o) {
 }
 
 // Coalesced epilogue I/O.  A thread owns one accumulator ROW, so touching global memory directly would make every
-// warp-level access hit 32 different rows with 16 bytes each (partial sectors -> L2 read-modify-write: ncu showed
-// 1.5-2 GB of DRAM reads for a 4.1 GB write, even with 64-byte segments).  Each epilogue warp therefore owns a 4 KiB
+// warp-level access hit 32 different rows with 16 bytes each (partial sectors -> L2 read-modify-write and DRAM reads
+// on a pure write).  Each epilogue warp therefore owns a 4 KiB
 // smem buffer holding a [32 rows][128 B] block (16-byte slots XOR-swizzled by row: conflict-free both ways); global
 // traffic is 8 instructions of 4 rows x 128 contiguous bytes = whole cache lines, for outputs AND for the
 // residual / ReLU-mask operands.
@@ -184,10 +186,7 @@ __device__ __forceinline__ void stage_fetch_bf16(uint32_t stg, const bf16* src, 
   __syncwarp();
 }
 
-// Asynchronous variant (cp.async, L2 -> smem without registers): the epilogue operand of the NEXT block is brought in
-// while the current one is processed, and the first block of a tile while the warp still waits for the accumulator —
-// the ncu source page showed the epilogues with a residual / ReLU-mask operand spending half of their time on the
-// long scoreboard of exactly these loads (one DRAM / L2 round trip per 32 x 64 block on the critical path).
+// cp.async (L2 -> smem without registers), 16 bytes, zero-filled when `ok` is false
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool ok) {
   const uint32_t sz = ok ? 16u : 0u;  // src-size 0: nothing is read, the 16 bytes are zero-filled
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
@@ -196,32 +195,9 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-__device__ __forceinline__ void stage_prefetch_bf16(uint32_t stg, const bf16* src, long long ld, int row0, int col0, int M,
-                                                    int N, int lane) {
-  const int slot = lane & 7, rsub = lane >> 3;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int r = i * 4 + rsub;
-    const int row = row0 + r, col = col0 + slot * 8;
-    const bool ok = row < M && col + 8 <= N;
-    cp_async16_zfill(stg_addr(stg, r, slot), ok ? src + (long long)row * ld + col : src, ok);
-  }
-}
-// block `pc` of a half tile lives in buffer (pc & 1); called with the operand of block pc already requested:
-// requests block pc + 1 (if any), then waits for block pc
-template <int NBLK>
-__device__ __forceinline__ uint32_t stage_pipeline_step(uint32_t stg0, uint32_t stg1, const bf16* src, long long ld, int row0,
-                                                        int cbase, int pc, int M, int N, int lane) {
-  const bool more = pc + 1 < NBLK && cbase + (pc + 1) * 64 < N;   // warp-uniform
-  if (more) stage_prefetch_bf16((pc & 1) ? stg0 : stg1, src, ld, row0, cbase + (pc + 1) * 64, M, N, lane);
-  cp_async_commit();
-  cp_async_wait<1>();   // everything but the group just committed (empty when there is no next block)
-  __syncwarp();
-  return (pc & 1) ? stg1 : stg0;
-}
-
-// column sums of the staged [32 rows][64 bf16] block (the values exactly as they are written to D), accumulated into
-// colsum[col0 .. col0+64): lane l owns columns 2l, 2l+1.  Rows >= M hold zeros (their `o` was zeroed).
+// column sums of the staged [32 rows][64 bf16] block (the values exactly as they are written to D), stored into
+// colsum[col0 .. col0+64) of this row block's workspace row: lane l owns columns 2l, 2l+1.  Rows >= M hold zeros (their
+// `o` was zeroed).  The host adds the row blocks in order afterwards.
 __device__ __forceinline__ void stage_colsum_bf16(uint32_t stg, float* colsum, int col0, int N, int lane) {
   __syncwarp();
   // word `lane` of row r sits at r*128 + (((lane>>2) ^ r) & 7)*16 + (lane&3)*4: the swizzle depends on r & 7 only, so 8
@@ -243,27 +219,22 @@ __device__ __forceinline__ void stage_colsum_bf16(uint32_t stg, float* colsum, i
     }
   }
   const int col = col0 + 2 * lane;
-  if (col < N) atomicAdd(colsum + col, s0 + s2);
-  if (col + 1 < N) atomicAdd(colsum + col + 1, s1 + s3);
+  if (col < N) colsum[col] = s0 + s2;
+  if (col + 1 < N) colsum[col + 1] = s1 + s3;
 }
 
-// PF: the residual of block 0 was requested with stage_prefetch_bf16 into `stg_` before the accumulator wait (caller),
-// blocks alternate between `stg_` and `stg2`.
-template <int CH, bool PF = false>
+template <int CH>
 __device__ __forceinline__ void epi_store(const GemmParams& p, uint32_t t_addr, int row, bool row_ok, int cbase,
-                                          uint32_t stg_, int row0, int lane, uint32_t stg2 = 0) {
+                                          uint32_t stg, int row0, int lane) {
   static_assert(CH % 2 == 0, "epilogue works on pairs of 32-column chunks");
 #pragma unroll 1
   for (int pc = 0; pc < CH / 2; ++pc) {
     const int colp = cbase + pc * 64;
     if (colp >= p.N) break;  // warp-uniform
-    uint32_t rr2[2][32];  // both chunks of the pair in flight, one wait: halves the exposed TMEM-load latency
-    tmem_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
-    tmem_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
-    uint32_t stg = stg_;
-    if (PF && p.residual) stg = stage_pipeline_step<CH / 2>(stg_, stg2, p.residual, p.ldr, row0, cbase, pc, p.M, p.N, lane);
-    else if (p.residual) stage_fetch_bf16(stg, p.residual, p.ldr, row0, colp, p.M, p.N, lane);
-    tmem_ld_wait();
+    uint32_t rr2[2][32];
+    acc_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
+    acc_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
+    if (p.residual) stage_fetch_bf16(stg, p.residual, p.ldr, row0, colp, p.M, p.N, lane);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int col0 = colp + h * 32;
@@ -316,18 +287,25 @@ __device__ __forceinline__ void epi_store(const GemmParams& p, uint32_t t_addr, 
   (void)row; (void)row_ok;
 }
 
+// split_k == 1: D += alpha * acc with red.add (one contribution per element and call).  split_k > 1: D is this split's
+// slice of a workspace and is overwritten; the host then adds the slices in split order (same result every run).
 template <int CH>
-__device__ __forceinline__ void epi_atomic(const GemmParams& p, uint32_t t_addr, int row, bool row_ok, int cbase) {
+__device__ __forceinline__ void epi_atomic(const GemmParams& p, float* D, int row, bool row_ok, int cbase,
+                                           uint32_t t_addr) {
+  const bool store = p.splits > 1;
 #pragma unroll 1
   for (int c = 0; c < CH; ++c) {
     const int col0 = cbase + c * 32;
     if (col0 >= p.N) break;
     uint32_t r[32];
-    tmem_ld_x32(t_addr + c * 32, r);
-    tmem_ld_wait();
+    acc_ld_x32(t_addr + c * 32, r);
     if (!row_ok) continue;
-    float* dp = reinterpret_cast<float*>(p.D) + (long long)row * p.ldd + col0;
-    if (col0 + 32 <= p.N && (p.ldd & 3) == 0) {
+    float* dp = D + (long long)row * p.ldd + col0;
+    if (store) {
+#pragma unroll
+      for (int j = 0; j < 32; ++j)
+        if (col0 + j < p.N) dp[j] = __uint_as_float(r[j]) * p.alpha;
+    } else if (col0 + 32 <= p.N && (p.ldd & 3) == 0) {
 #pragma unroll
       for (int j = 0; j < 32; j += 4)  // REDG.E.ADD.F32x4: one vector reduction per 16 bytes
         asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dp + j),
@@ -342,20 +320,17 @@ __device__ __forceinline__ void epi_atomic(const GemmParams& p, uint32_t t_addr,
   }
 }
 
-template <int CH, bool PF = false>
+template <int CH>
 __device__ __forceinline__ void epi_relu_bwd(const GemmParams& p, uint32_t t_addr, int row, bool row_ok, int cbase,
-                                             uint32_t stg_, int row0, int lane, uint32_t stg2 = 0) {
+                                             uint32_t stg, int row0, int lane) {
 #pragma unroll 1
   for (int pc = 0; pc < CH / 2; ++pc) {
     const int colp = cbase + pc * 64;
     if (colp >= p.N) break;
     uint32_t rr2[2][32];
-    tmem_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
-    tmem_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
-    uint32_t stg = stg_;
-    if (PF) stg = stage_pipeline_step<CH / 2>(stg_, stg2, p.aux, p.ldaux, row0, cbase, pc, p.M, p.N, lane);
-    else    stage_fetch_bf16(stg, p.aux, p.ldaux, row0, colp, p.M, p.N, lane);
-    tmem_ld_wait();
+    acc_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
+    acc_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
+    stage_fetch_bf16(stg, p.aux, p.ldaux, row0, colp, p.M, p.N, lane);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float am[32], o[32];
@@ -364,7 +339,7 @@ __device__ __forceinline__ void epi_relu_bwd(const GemmParams& p, uint32_t t_add
       for (int j = 0; j < 32; ++j) o[j] = am[j] > 0.f ? __uint_as_float(rr2[h][j]) * p.alpha : 0.f;
       stage_put_bf16(stg, lane, h, o);  // in place: this lane overwrites the slots it just read
     }
-    if (p.colsum) stage_colsum_bf16(stg, p.colsum, colp, p.N, lane);
+    if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, lane);
     stage_flush<2>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
   }
   (void)row; (void)row_ok;
@@ -381,8 +356,7 @@ __device__ __forceinline__ void epi_ce_stats(const GemmParams& p, uint32_t t_add
     const int col0 = cbase + c * 32;
     if (col0 >= p.N) break;
     uint32_t r[32];
-    tmem_ld_x32(t_addr + c * 32, r);
-    tmem_ld_wait();
+    acc_ld_x32(t_addr + c * 32, r);
     if (!row_ok || col0 >= p.n_valid) continue;
     float v[32];
     if (col0 + 32 <= p.n_valid) {  // interior chunk (warp-uniform): no per-element masking
@@ -437,9 +411,8 @@ __device__ __forceinline__ void epi_ce_grad(const GemmParams& p, uint32_t t_addr
     const int colp = cbase + pc * 64;
     if (colp >= p.N) break;
     uint32_t rr2[2][32];
-    tmem_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
-    tmem_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
-    tmem_ld_wait();
+    acc_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
+    acc_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int col0 = colp + h * 32;
@@ -474,7 +447,7 @@ __device__ __forceinline__ void epi_ce_grad(const GemmParams& p, uint32_t t_addr
       }
       stage_put_bf16(stg, lane, h, o);
     }
-    if (p.colsum) stage_colsum_bf16(stg, p.colsum, colp, p.N, lane);
+    if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, lane);
     stage_flush<2, true>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);  // 4 GB of dlogits: stream past L2
   }
 }

@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ g
     float s = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) s += red[w];
-    atomicAdd(out, s);
+    out[blockIdx.x] = s;  // one partial per block, summed in block order by reduce_rows_add
   }
 }
 
@@ -97,16 +97,28 @@ adam_kernel(float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
 
 using namespace db200;
 
-extern "C" int db200_sqnorm_f32(db200_stream_t stream_, const float* g, size_t n, float* out_accum) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (n == 0) return DB200_OK;
-  DB200_REQUIRE(g && out_accum && aligned16(g), DB200_E_ALIGN, "sqnorm: NULL or unaligned pointer");
+static size_t sqnorm_blocks(size_t n) {
   size_t blocks = (n / 4 + 255) / 256;
   const size_t cap = (size_t)sm_count() * 8;
   if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  sqnorm_kernel<<<(int)blocks, 256, 0, stream>>>(g, n, out_accum);
-  return check_launch("sqnorm_kernel");
+  return blocks < 1 ? 1 : blocks;
+}
+
+extern "C" int64_t db200_sqnorm_workspace_bytes(size_t n) { return (int64_t)(sqnorm_blocks(n) * sizeof(float)); }
+
+extern "C" int db200_sqnorm_f32(db200_stream_t stream_, const float* g, size_t n, float* out_accum, void* workspace,
+                                int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (n == 0) return DB200_OK;
+  DB200_REQUIRE(g && out_accum && aligned16(g), DB200_E_ALIGN, "sqnorm: NULL or unaligned pointer");
+  const size_t blocks = sqnorm_blocks(n);
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, (int64_t)(blocks * sizeof(float))), DB200_E_INVALID,
+                "sqnorm: needs an aligned workspace of db200_sqnorm_workspace_bytes() bytes");
+  float* ws = static_cast<float*>(workspace);
+  sqnorm_kernel<<<(int)blocks, 256, 0, stream>>>(g, n, ws);
+  const int rc = check_launch("sqnorm_kernel");
+  if (rc != DB200_OK) return rc;
+  return reduce_rows_add(stream, ws, (int)blocks, 1, out_accum);
 }
 
 extern "C" int db200_adam_step(db200_stream_t stream_, float* p, float* m, float* v, float* g, void* p_bf16,

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma operand descriptors.
 // Everything here is device-side and header-only.  No CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdint>
@@ -54,7 +54,17 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA store / tcgen05.mma operand reads)
+// Same bound without the report, for waits inside a wgmma pipeline: a printf call there makes ptxas serialise the
+// warpgroup MMAs of the whole kernel.
+__device__ __forceinline__ void mbar_wait_mma(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity))
+    if ((++spins & 0x3ff) == 0 && clock64() - t0 > 4000000000ll) __trap();
+}
+
+// generic-proxy writes (st.shared) -> visible to the async proxy (TMA store / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -113,43 +123,6 @@ __device__ __forceinline__ void tma_store_wait_read0() {
 }
 __device__ __forceinline__ void tma_store_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, loads
-// ----------------------------------------------------------------------------------------------
-// Whole warp executes.  Writes the TMEM base address (lane 0, column c) to *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc];  single thread issues.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M = 128 lanes, K bf16 elements packed two per 32-bit column,
-// element k of row i in lane i, column k/2, low half = even k) is read from tensor memory — this is how a softmax /
-// gradient warpgroup hands P or dS to the next product without a shared-memory round trip.  Single thread issues.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 // elect.sync: true in exactly one (the lowest active) lane of a converged warp.  ptxas recognises the pattern and emits a
 // single ELECT + predicated / uniformly-branched code for the guarded block — unlike `lane == 0`, which it must treat as
 // an arbitrary per-thread predicate (a lane-by-lane "waterfall" loop around every uniform-datapath instruction).
@@ -165,88 +138,23 @@ __device__ __forceinline__ bool elect_one_sync() {
   return pred != 0;
 }
 
-// Arrive (once) on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// TMEM -> registers: each thread of the warp reads its own lane (row), N consecutive 32-bit columns.
-// taddr must carry the warp's lane quarter: ((warp_id % 4) * 32) << 16.
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM (same addressing as tmem_ld_x32)
-__device__ __forceinline__ void tmem_st_x32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (layout per PTX ISA "tcgen05 matrix/instruction descriptor"; field positions cross-checked
-// against cute/arch/mma_sm100_desc.hpp shipped in this image).
-// ----------------------------------------------------------------------------------------------
-// Shared-memory operand descriptor, 128-byte swizzle.
+// wgmma shared-memory operand descriptor (PTX ISA "Matrix Descriptor Format" for wgmma), 128-byte swizzle.
 //   K-major tile  [rows][64 bf16]        : rows are 128 B apart, 8-row groups SBO=1024 B apart, LBO unused.
 //   MN-major slab [k rows][64 bf16 of MN]: k rows 128 B apart, 8-k groups SBO=1024 B apart,
 //                                          64-wide MN atoms LBO bytes apart.
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);             // [0,14)  start address >> 4
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;     // [16,30) leading byte offset >> 4
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;     // [32,46) stride byte offset >> 4
-  d |= 1ull << 46;                                                   // [46,48) descriptor version (Blackwell)
-  d |= 2ull << 61;                                                   // [61,64) SWIZZLE_128B
+  d |= 1ull << 62;                                                   // [62,64) layout type 1 = SWIZZLE_128B
   return d;
-}
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                                   // D format  = F32
-         | (1u << 7)                                 // A format  = BF16
-         | (1u << 10)                                // B format  = BF16
-         | (static_cast<uint32_t>(a_mn_major) << 15)  // A major: 0 = K, 1 = MN
-         | (static_cast<uint32_t>(b_mn_major) << 16)  // B major
-         | (static_cast<uint32_t>(N >> 3) << 17)      // N / 8
-         | (static_cast<uint32_t>(M >> 4) << 24);     // M / 16
 }
 
 // Byte offset of element (row, col) inside a [rows][64 bf16] tile stored with the 128-byte swizzle that TMA
-// (CU_TENSOR_MAP_SWIZZLE_128B) and the UMMA SW128 descriptor agree on: 16-byte chunk index XOR (row % 8).
+// (CU_TENSOR_MAP_SWIZZLE_128B) and the wgmma SW128 descriptor agree on: 16-byte chunk index XOR (row % 8).
 __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t col) {
   return row * 128u + ((((col >> 3) ^ (row & 7u)) & 7u) << 4) + ((col & 7u) << 1);
 }

@@ -43,13 +43,19 @@ __global__ void embed_fwd_kernel(const int* __restrict__ ids, const bf16* __rest
 
 // dwte[ids[t]] += dx[t].  A thread owns 8 columns of a strip of EMB_STRIP consecutive tokens and merges RUNS of equal
 // ids in registers before touching memory: captions are right-padded with one id (src/input_fns.py:32-38), so the
-// ~220 consecutive padding positions of every sequence collapse into one red.add per strip instead of 220 serialised
-// reductions on the same 2 KiB row of dwte (same-address reductions serialise in L2; that run was most of this
-// kernel's time).  Different ids still go through red.global.add.v4.f32.
+// ~220 consecutive padding positions of every sequence collapse into one reduction per strip instead of 220 serialised
+// reductions on the same row (same-address reductions serialise in L2).  Strips of different tokens meet on the same
+// row in no fixed order, so the run sums go into a 64-bit fixed-point accumulator in the caller's workspace (cleared
+// on the stream first; integer addition is associative: the result does not depend on that order) that
+// embed_fixed_flush_kernel then adds to dwte.
+constexpr double EMB_FIX_SCALE = 1099511627776.0;  // 2^40: resolution 9.1e-13, magnitude up to 8.4e6
+__device__ __forceinline__ void fixed_add(unsigned long long* dst, float v) {
+  atomicAdd(dst, static_cast<unsigned long long>(__double2ll_rn(static_cast<double>(v) * EMB_FIX_SCALE)));
+}
 constexpr int EMB_STRIP = 32;
 __global__ void __launch_bounds__(256)
-embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, float* __restrict__ dwte, int T, int d,
-                     int V) {
+embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, unsigned long long* __restrict__ acc64,
+                     int T, int d, int V) {
   const int vec_per_row = d >> 3;
   const long long total = (long long)((T + EMB_STRIP - 1) / EMB_STRIP) * vec_per_row;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
@@ -61,13 +67,9 @@ embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, f
     int cur = -1;
     auto flush = [&]() {
       if (cur >= 0 && cur < V) {
-        float* dst = dwte + (long long)cur * d + c;  // 32-byte aligned: two REDG.E.ADD.F32x4
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(acc[0]), "f"(acc[1]), "f"(acc[2]),
-                     "f"(acc[3])
-                     : "memory");
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4), "f"(acc[4]), "f"(acc[5]),
-                     "f"(acc[6]), "f"(acc[7])
-                     : "memory");
+        unsigned long long* dst = acc64 + (long long)cur * d + c;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) fixed_add(dst + j, acc[j]);
       }
     };
     for (int t = t0; t < t1; ++t) {
@@ -84,6 +86,17 @@ embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, f
       for (int j = 0; j < 8; ++j) acc[j] += g[j];
     }
     flush();
+  }
+}
+
+// dwte += acc64 / 2^40 where acc64 is non-zero
+__global__ void __launch_bounds__(256)
+embed_fixed_flush_kernel(const unsigned long long* __restrict__ acc64, float* __restrict__ dwte, long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long v = static_cast<long long>(acc64[i]);
+    if (v != 0) {
+      dwte[i] += static_cast<float>(static_cast<double>(v) * (1.0 / EMB_FIX_SCALE));
+    }
   }
 }
 
@@ -175,7 +188,7 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, co
 }
 
 // Each warp walks rows with a grid stride, keeps per-lane partial dg/db in registers, then one block-level
-// reduction through shared memory and one atomicAdd per column per block.
+// reduction through shared memory and one partial row of dg / db (/ dxsum) per block, summed in block order afterwards.
 template <int NCH>
 __global__ void __launch_bounds__(128)
 layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ g,
@@ -255,9 +268,9 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
       for (int j = 0; j < 8; ++j)
         red[warp][(c * 32 + lane) * 8 + j] = pass == 0 ? adg[c][j] : (pass == 1 ? adb[c][j] : adx[c][j]);
     __syncthreads();
-    float* dst = pass == 0 ? dg : (pass == 1 ? db : dxsum);
+    float* dst = (pass == 0 ? dg : (pass == 1 ? db : dxsum)) + (long long)blockIdx.x * d;  // this block's partial row
     for (int col = threadIdx.x; col < d; col += 128)
-      atomicAdd(dst + col, red[0][col] + red[1][col] + red[2][col] + red[3][col]);
+      dst[col] = red[0][col] + red[1][col] + red[2][col] + red[3][col];
     __syncthreads();
   }
 }
@@ -265,7 +278,7 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
 // Wide rows (d = 4096, the 12 B configuration): ONE CTA of 128 threads per row, thread t owns columns
 // {(c*128 + t)*8 .. +7 : c < NCW} (16-byte accesses, 2 KiB contiguous per c across the CTA).  Row statistics go through
 // a two-level (warp shuffle + 4-float shared) reduction; in backward every thread owns its columns for the whole row
-// walk, so dgamma / dbeta / dxsum need no cross-thread reduction at all: one atomicAdd per column per CTA at the end.
+// walk, so dgamma / dbeta / dxsum need no cross-thread reduction at all: one partial row per CTA at the end.
 __device__ __forceinline__ float2 block128_sum2(float a, float b, float* red /*[8]*/) {
   a = warp_sum(a);
   b = warp_sum(b);
@@ -395,9 +408,10 @@ layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ 
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int col = (c * 128 + threadIdx.x) * 8 + j;
-      atomicAdd(dg + col, adg[c][j]);
-      atomicAdd(db + col, adb[c][j]);
-      if (dxsum) atomicAdd(dxsum + col, adx[c][j]);
+      const long long o = (long long)blockIdx.x * d + col;  // this block's partial row
+      dg[o] = adg[c][j];
+      db[o] = adb[c][j];
+      if (dxsum) dxsum[o] = adx[c][j];
     }
 }
 
@@ -425,7 +439,7 @@ colsum_kernel(const bf16* __restrict__ x, long long ld, int rows, int cols, floa
     float s = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) s += red[w][c];
-    atomicAdd(out + blockIdx.x * 256 + c, s);
+    out[(long long)blockIdx.y * cols + blockIdx.x * 256 + c] = s;  // partial of row split blockIdx.y
   }
 }
 
@@ -529,7 +543,7 @@ ce_finish_kernel(const float* __restrict__ part_max, const float* __restrict__ p
       loss_rows[row] = loss;
     }
     loss = warp_sum(loss);
-    if (r == 0) atomicAdd(loss_sum, loss);
+    if (r == 0) loss_sum[blockIdx.x] = loss;  // per-block partial, summed in block order by the launcher
   }
 }
 
@@ -545,21 +559,34 @@ extern "C" int db200_embed_fwd(db200_stream_t stream_, const int32_t* ids, const
   DB200_REQUIRE(ids && aligned16(wte) && aligned16(wpe) && aligned16(out), DB200_E_ALIGN,
                 "embed_fwd: NULL or unaligned pointer");
   const long long total = (long long)B * S * (d / 8);
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const int blocks = (int)((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
   embed_fwd_kernel<<<blocks, 256, 0, stream>>>(ids, (const bf16*)wte, (const bf16*)wpe, (bf16*)out, B * S, S, d, V);
   return check_launch("embed_fwd_kernel");
 }
 
+extern "C" int64_t db200_embed_bwd_workspace_bytes(int d, int V) {
+  return (int64_t)V * d * (int64_t)sizeof(unsigned long long);
+}
+
 extern "C" int db200_embed_bwd(db200_stream_t stream_, const int32_t* ids, const void* dx, float* dwte, float* dwpe,
-                               int B, int S, int d, int V) {
+                               int B, int S, int d, int V, void* workspace, int64_t workspace_bytes) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(B > 0 && S > 0 && d > 0 && V > 0 && d % 8 == 0, DB200_E_INVALID,
                 "embed_bwd: need B,S,V > 0 and d %% 8 == 0");
   DB200_REQUIRE(ids && aligned16(dx) && dwte && dwpe, DB200_E_ALIGN, "embed_bwd: NULL or unaligned pointer");
   const long long total = (long long)(((long long)B * S + EMB_STRIP - 1) / EMB_STRIP) * (d / 8);
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
-  embed_bwd_wte_kernel<<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, dwte, B * S, d, V);
+  const int blocks = (int)((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
+  const long long n_wte = (long long)V * d;
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_embed_bwd_workspace_bytes(d, V)), DB200_E_INVALID,
+                "embed_bwd: needs an aligned workspace of db200_embed_bwd_workspace_bytes() bytes");
+  auto* acc64 = static_cast<unsigned long long*>(workspace);
+  DB200_CUDA(cudaMemsetAsync(acc64, 0, (size_t)n_wte * sizeof(unsigned long long), stream));
+  embed_bwd_wte_kernel<<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V);
   int rc = check_launch("embed_bwd_wte_kernel");
+  if (rc != DB200_OK) return rc;
+  const long long fblocks = (n_wte + 255) / 256 < sm_count() * 16 ? (n_wte + 255) / 256 : sm_count() * 16;
+  embed_fixed_flush_kernel<<<(int)fblocks, 256, 0, stream>>>(acc64, dwte, n_wte);
+  rc = check_launch("embed_fixed_flush_kernel");
   if (rc != DB200_OK) return rc;
   const int total_pe = S * (d / 8);
   embed_bwd_wpe_kernel<<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d);
@@ -608,50 +635,89 @@ extern "C" int db200_layernorm_fwd(db200_stream_t stream_, const void* x, const 
   return check_launch("layernorm_fwd_kernel");
 }
 
+static int layernorm_bwd_grid(int rows, int d) {
+  int grid = d == 4096 ? rows : (rows + 3) / 4;
+  if (grid > sm_count() * 4) grid = sm_count() * 4;
+  return grid < 1 ? 1 : grid;
+}
+
+extern "C" int64_t db200_layernorm_bwd_workspace_bytes(int rows, int d) {
+  return (int64_t)3 * layernorm_bwd_grid(rows, d) * d * (int64_t)sizeof(float);
+}
+
 extern "C" int db200_layernorm_bwd_ex(db200_stream_t stream_, const void* dy, const void* x, const float* g,
                                       const float* mean, const float* rstd, const void* dres, void* dx, float* dg,
-                                      float* db, float* dxsum, int rows, int d) {
+                                      float* db, float* dxsum, int rows, int d, void* workspace,
+                                      int64_t workspace_bytes) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(rows > 0, DB200_E_INVALID, "layernorm_bwd: rows must be positive");
   DB200_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx) && aligned16(g) && mean && rstd && dg && db &&
                     aligned16(dres),
                 DB200_E_ALIGN, "layernorm_bwd: NULL or unaligned pointer");
-  int grid = (rows + 3) / 4;
-  if (grid > sm_count() * 4) grid = sm_count() * 4;
+  const int grid = layernorm_bwd_grid(rows, d);
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_layernorm_bwd_workspace_bytes(rows, d)),
+                DB200_E_INVALID, "layernorm_bwd: needs an aligned workspace of db200_layernorm_bwd_workspace_bytes() bytes");
   const bf16 *dyp = (const bf16*)dy, *xp = (const bf16*)x, *drp = (const bf16*)dres;
   bf16* dxp = (bf16*)dx;
+  // per-block partial rows of dg | db | dxsum, reduced in block order below
+  float* ws = static_cast<float*>(workspace);
+  float* const dg_out = dg;
+  float* const db_out = db;
+  float* const dxsum_out = dxsum;
+  dg = ws;
+  db = ws + (size_t)grid * d;
+  dxsum = dxsum_out ? ws + (size_t)2 * grid * d : nullptr;
   switch (d) {
     case 256:  layernorm_bwd_kernel<1><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
     case 512:  layernorm_bwd_kernel<2><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
     case 768:  layernorm_bwd_kernel<3><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
     case 1024: layernorm_bwd_kernel<4><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
     case 2048: layernorm_bwd_kernel<8><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
-    case 4096: layernorm_bwd_wide_kernel<4><<<min(rows, sm_count() * 4), 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
+    case 4096: layernorm_bwd_wide_kernel<4><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
     default:
       return set_error(DB200_E_UNSUPPORTED, "layernorm: d=%d not in {256,512,768,1024,2048,4096}", d);
   }
-  return check_launch("layernorm_bwd_kernel");
+  int rc = check_launch("layernorm_bwd_kernel");
+  if (rc == DB200_OK) rc = reduce_rows_add(stream, dg, grid, d, dg_out);
+  if (rc == DB200_OK) rc = reduce_rows_add(stream, db, grid, d, db_out);
+  if (rc == DB200_OK && dxsum_out) rc = reduce_rows_add(stream, dxsum, grid, d, dxsum_out);
+  return rc;
 }
 
 extern "C" int db200_layernorm_bwd(db200_stream_t stream_, const void* dy, const void* x, const float* g,
                                    const float* mean, const float* rstd, const void* dres, void* dx, float* dg,
-                                   float* db, int rows, int d) {
-  return db200_layernorm_bwd_ex(stream_, dy, x, g, mean, rstd, dres, dx, dg, db, nullptr, rows, d);
+                                   float* db, int rows, int d, void* workspace, int64_t workspace_bytes) {
+  return db200_layernorm_bwd_ex(stream_, dy, x, g, mean, rstd, dres, dx, dg, db, nullptr, rows, d, workspace,
+                                workspace_bytes);
+}
+
+static int colsum_row_splits(int rows, int cols) {
+  const int gx = (cols + 255) / 256;
+  int gy = (sm_count() * 4 + gx - 1) / gx;
+  if (gy > (rows + 7) / 8) gy = (rows + 7) / 8;
+  return gy < 1 ? 1 : gy;
+}
+
+extern "C" int64_t db200_colsum_workspace_bytes(int rows, int cols) {
+  return (int64_t)colsum_row_splits(rows, cols) * cols * (int64_t)sizeof(float);
 }
 
 extern "C" int db200_colsum_bf16(db200_stream_t stream_, const void* x, int64_t ld, int rows, int cols,
-                                 float* out_accum) {
+                                 float* out_accum, void* workspace, int64_t workspace_bytes) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(rows > 0 && cols > 0 && cols % 8 == 0 && ld % 8 == 0 && ld >= cols, DB200_E_INVALID,
                 "colsum: need rows,cols > 0 and cols, ld multiples of 8 (got rows=%d cols=%d ld=%lld)", rows, cols,
                 (long long)ld);
   DB200_REQUIRE(aligned16(x) && out_accum, DB200_E_ALIGN, "colsum: NULL or unaligned pointer");
   const int gx = (cols + 255) / 256;
-  int gy = (sm_count() * 4 + gx - 1) / gx;
-  if (gy > (rows + 7) / 8) gy = (rows + 7) / 8;
-  if (gy < 1) gy = 1;
-  colsum_kernel<<<dim3(gx, gy), 256, 0, stream>>>((const bf16*)x, ld, rows, cols, out_accum);
-  return check_launch("colsum_kernel");
+  const int gy = colsum_row_splits(rows, cols);
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_colsum_workspace_bytes(rows, cols)), DB200_E_INVALID,
+                "colsum: needs an aligned workspace of db200_colsum_workspace_bytes() bytes");
+  float* ws = static_cast<float*>(workspace);
+  colsum_kernel<<<dim3(gx, gy), 256, 0, stream>>>((const bf16*)x, ld, rows, cols, ws);
+  const int rc = check_launch("colsum_kernel");
+  if (rc != DB200_OK) return rc;
+  return reduce_rows_add(stream, ws, gy, cols, out_accum);
 }
 
 extern "C" int db200_cast_f32_to_bf16(db200_stream_t stream_, const float* src, void* dst, size_t n) {
@@ -659,7 +725,7 @@ extern "C" int db200_cast_f32_to_bf16(db200_stream_t stream_, const float* src, 
   if (n == 0) return DB200_OK;
   DB200_REQUIRE(aligned16(src) && aligned16(dst) && src && dst, DB200_E_ALIGN, "cast: NULL or unaligned pointer");
   size_t blocks = (n / 8 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
   if (blocks < 1) blocks = 1;
   cast_f32_bf16_kernel<<<(int)blocks, 256, 0, stream>>>(src, (bf16*)dst, n);
   return check_launch("cast_f32_bf16_kernel");
@@ -669,7 +735,7 @@ extern "C" int db200_cast_bf16_to_f32(db200_stream_t stream_, const void* src, f
   if (n == 0) return DB200_OK;
   DB200_REQUIRE(aligned16(src) && aligned16(dst) && src && dst, DB200_E_ALIGN, "cast: NULL or unaligned pointer");
   size_t blocks = (n / 8 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
   if (blocks < 1) blocks = 1;
   cast_bf16_f32_kernel<<<(int)blocks, 256, 0, stream>>>((const bf16*)src, dst, n);
   return check_launch("cast_bf16_f32_kernel");
@@ -701,20 +767,30 @@ extern "C" int db200_split_f32_to_bf16x2(db200_stream_t stream_, const float* sr
   DB200_REQUIRE(src && hi && aligned16(src) && aligned16(hi) && aligned16(lo_or_null), DB200_E_ALIGN,
                 "split_f32: NULL or unaligned pointer");
   size_t blocks = (n / 8 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
   if (blocks < 1) blocks = 1;
   split_f32_kernel<<<(int)blocks, 256, 0, stream>>>(src, (bf16*)hi, (bf16*)lo_or_null, n);
   return check_launch("split_f32_kernel");
 }
 
+extern "C" int64_t db200_ce_finish_workspace_bytes(int M) {
+  return (int64_t)((M + CEF_ROWS - 1) / CEF_ROWS) * (int64_t)sizeof(float);
+}
+
 extern "C" int db200_ce_finish(db200_stream_t stream_, const float* part_max, const float* part_sum,
                                const float* label_logit, float* lse, float* loss_rows, float* loss_sum, int M,
-                               int n_tiles) {
+                               int n_tiles, void* workspace, int64_t workspace_bytes) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(M > 0 && n_tiles > 0, DB200_E_INVALID, "ce_finish: M and n_tiles must be positive");
   DB200_REQUIRE(part_max && part_sum && label_logit && lse && loss_rows && loss_sum, DB200_E_INVALID,
                 "ce_finish: NULL pointer");
-  ce_finish_kernel<<<(M + CEF_ROWS - 1) / CEF_ROWS, CEF_ROWS * CEF_GROUPS, 0, stream>>>(part_max, part_sum, label_logit, lse, loss_rows, loss_sum, M,
-                                                    n_tiles);
-  return check_launch("ce_finish_kernel");
+  const int blocks = (M + CEF_ROWS - 1) / CEF_ROWS;
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_ce_finish_workspace_bytes(M)), DB200_E_INVALID,
+                "ce_finish: needs an aligned workspace of db200_ce_finish_workspace_bytes() bytes");
+  float* ws = static_cast<float*>(workspace);
+  ce_finish_kernel<<<blocks, CEF_ROWS * CEF_GROUPS, 0, stream>>>(part_max, part_sum, label_logit, lse, loss_rows, ws, M,
+                                                                 n_tiles);
+  const int rc = check_launch("ce_finish_kernel");
+  if (rc != DB200_OK) return rc;
+  return reduce_rows_add(stream, ws, blocks, 1, loss_sum);
 }

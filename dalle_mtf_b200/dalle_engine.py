@@ -1,4 +1,4 @@
-"""DALL-E transformer training engine on the sm_100a kernels (host side: buffer plan + kernel sequencing).
+"""DALL-E transformer training engine on the sm_90a kernels (host side: buffer plan + kernel sequencing).
 
 Mirrors what the reference builds as an mtf graph in src/dalle_mtf/models.py:141-416 and differentiates with
 mtf.gradients (src/optimizers.py:34): here forward and backward are explicit kernel sequences over pre-allocated
@@ -479,7 +479,7 @@ class DalleEngine:
 
     # ------------------------------------------------------------------------------------------ optimiser
     def zero_grads(self):
-        """Gradients accumulate (red.add), so every step starts from zeros.  The Adam kernel writes those zeros while it
+        """Gradients accumulate (+=), so every step starts from zeros.  The Adam kernel writes those zeros while it
         streams the gradient it consumes, so after an optimiser step only the 64 aux scalars (loss) need clearing; the
         full 4 B/param memset runs only when backward ran without an optimiser step in between (tests, first step)."""
         if self._grads_clean:

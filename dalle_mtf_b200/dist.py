@@ -1,4 +1,4 @@
-"""Data parallelism: one process per GPU, NCCL over NVLink 5 / NVSwitch, bucketed gradient all-reduce that overlaps
+"""Data parallelism: one process per GPU, NCCL over NVLink / NVSwitch, bucketed gradient all-reduce that overlaps
 with the rest of backward.
 
 The reference's only parallelism is the layout rule "batch_dim:data" (configs/dalle_example.json:20-21): mtf lowers
@@ -36,7 +36,7 @@ class DataParallel:
     Without a GPU (the world-size-2 CPU tests of the bucket logic) the collectives go through torch.distributed/gloo.
     """
 
-    # CTAs NCCL may occupy while the persistent 148-CTA tcgen05 grids of backward are running (0 = NCCL's default).
+    # CTAs NCCL may occupy while the persistent one-CTA-per-SM wgmma grids of backward are running (0 = NCCL's default).
     # The same number of SMs is taken out of the persistent kernels' grids (db200_set_reserved_sms), so that the two fit
     # side by side; the overlapped all-reduce only has to move 287 MB during ~10 ms of backward: four CTAs are plenty.
     MAX_CTAS = int(os.environ.get("DB200_NCCL_MAX_CTAS", "4"))

@@ -1,7 +1,7 @@
 """ctypes binding of libdalle_b200.so (the C ABI declared in include/dalle_b200.h).
 
-The library is built in-tree by ``dalle_mtf_b200.build.build()`` (nvcc, sm_100a only).  There is no CPU fallback
-and no PyTorch-eager fallback: if the shared object is missing, or the device is not a B200-class GPU, every op
+The library is built in-tree by ``dalle_mtf_b200.build.build()`` (nvcc, sm_90a only).  There is no CPU fallback
+and no PyTorch-eager fallback: if the shared object is missing, or the device is not an H100 (sm_90), every op
 raises.  PyTorch is used only for device memory, streams and torch.distributed.
 """
 import ctypes
@@ -31,6 +31,7 @@ class GemmEpilogue(ctypes.Structure):
         ("bias", c_vp), ("residual", c_vp), ("ldr", c_i64), ("aux", c_vp), ("ldaux", c_i64),
         ("labels", c_vp), ("part_max", c_vp), ("part_sum", c_vp), ("label_logit", c_vp), ("lse", c_vp),
         ("n_valid", ctypes.c_int32), ("reserved", ctypes.c_int32), ("colsum", c_vp),
+        ("workspace", c_vp), ("workspace_bytes", c_i64),
     ]
 
 
@@ -46,12 +47,13 @@ _SIGNATURES = {
     "db200_version": [],
     "db200_device_check": [],
     "db200_embed_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
-    "db200_embed_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
+    "db200_embed_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64],
     "db200_assemble_tokens": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_shift_labels": [c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_layernorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
-    "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int],
-    "db200_layernorm_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int],
+    "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
+    "db200_layernorm_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp,
+                               c_i64],
     "db200_gemm_bf16": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
                         ctypes.POINTER(GemmEpilogue)],
     "db200_gemm_ce_tiles": [c_int],
@@ -68,14 +70,14 @@ _SIGNATURES = {
     "db200_tfrecord_frame": [c_vp, c_u64, c_vp],
     "db200_tfrecord_index": [c_vp, c_u64, c_int, c_vp, c_vp, c_u64, c_vp],
     "db200_image_crop_resize_normalize": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int],
-    "db200_ce_finish": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int],
+    "db200_ce_finish": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
     "db200_attn_causal_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_causal_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
-    "db200_colsum_bf16": [c_vp, c_vp, c_i64, c_int, c_int, c_vp],
+    "db200_colsum_bf16": [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_i64],
     "db200_cast_f32_to_bf16": [c_vp, c_vp, c_vp, c_sz],
     "db200_cast_bf16_to_f32": [c_vp, c_vp, c_vp, c_sz],
     "db200_split_f32_to_bf16x2": [c_vp, c_vp, c_vp, c_vp, c_sz],
-    "db200_sqnorm_f32": [c_vp, c_vp, c_sz, c_vp],
+    "db200_sqnorm_f32": [c_vp, c_vp, c_sz, c_vp, c_vp, c_i64],
     "db200_adam_step": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_f32, c_f32, c_f32, c_f32, c_f32, c_vp, c_f32,
                         c_f32, c_int, c_int, c_int],
     "db200_conv2d_fwd": [c_vp, ctypes.POINTER(ConvDesc), c_vp, c_vp, c_vp, c_vp, c_vp],
@@ -106,7 +108,16 @@ _SIGNATURES = {
     "db200_bucket_all_gather_launch": [c_vp, c_vp, c_vp, c_vp, c_sz, c_int],
     "db200_bucket_allreduce_wait": [c_vp, c_vp],
 }
-EXPORTED_SYMBOLS = ["db200_last_error", "db200_launch_count"] + sorted(_SIGNATURES)
+# scratch sizes of the ops whose reductions go through a caller-provided workspace (restype int64)
+_WORKSPACE_QUERIES = {
+    "db200_gemm_workspace_bytes": [c_int, c_int, c_int, ctypes.POINTER(GemmEpilogue)],
+    "db200_layernorm_bwd_workspace_bytes": [c_int, c_int],
+    "db200_colsum_workspace_bytes": [c_int, c_int],
+    "db200_sqnorm_workspace_bytes": [c_sz],
+    "db200_ce_finish_workspace_bytes": [c_int],
+    "db200_embed_bwd_workspace_bytes": [c_int, c_int],
+}
+EXPORTED_SYMBOLS = ["db200_last_error", "db200_launch_count"] + sorted(_SIGNATURES) + sorted(_WORKSPACE_QUERIES)
 
 _lib = None
 MISSING_SYMBOLS = []
@@ -138,6 +149,14 @@ def load():
             continue
         fn.argtypes = argtypes
         fn.restype = c_int
+    for name, argtypes in _WORKSPACE_QUERIES.items():
+        try:
+            fn = getattr(lib, name)
+        except AttributeError:
+            MISSING_SYMBOLS.append(name)
+            continue
+        fn.argtypes = argtypes
+        fn.restype = c_i64
     _lib = lib
     return lib
 
@@ -152,7 +171,7 @@ _device_ok = False
 
 
 def require_device():
-    """Fail loudly unless the current CUDA device can run the sm_100a cubins."""
+    """Fail loudly unless the current CUDA device can run the sm_90a cubins."""
     global _device_ok
     if _device_ok:
         return
@@ -168,6 +187,13 @@ def launch_count():
 
 def stream_ptr():
     return torch.cuda.current_stream().cuda_stream
+
+
+def workspace(nbytes):
+    """Scratch for one call's ordered reductions, from PyTorch's caching allocator on the current stream (None if 0)."""
+    if nbytes <= 0:
+        return None
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=torch.cuda.current_device())
 
 
 def ptr(t):

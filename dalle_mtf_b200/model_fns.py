@@ -65,7 +65,7 @@ def load_vae_model(params, device):
     convblocks = vae_params.get("convblocks") or [(3, 64), (3, 128), (3, 256)]
     vae = VaeEngine(num_tokens=vae_params["num_tokens"], image_size=D, convblocks=convblocks,
                     input_channels=vae_params.get("input_channels") or 3,
-                    use_bf16=bool(vae_params.get("use_bf16")),   # bf16 -> tcgen05 implicit-GEMM convolutions
+                    use_bf16=bool(vae_params.get("use_bf16")),   # bf16 -> wgmma implicit-GEMM convolutions
                     stack_factor=vae_params.get("stack_factor") or 1, device=device)
     ckpt = params.get("vae_checkpoint_path")
     if ckpt is None:
@@ -93,7 +93,7 @@ def dalle_model_fn(features, labels, mode, params):
         state = load_checkpoint(local_path(vae_ckpt))
         vae.load_params({k[len("vae/"):]: v for k, v in state.items() if k.startswith("vae/")})
     elif params.get("vae_random_init"):
-        vae.init_params(seed=params.get("vae_seed") or 0)   # B200 extension key: throughput runs without a checkpoint
+        vae.init_params(seed=params.get("vae_seed") or 0)   # extension key: throughput runs without a checkpoint
     else:
         raise AssertionError("pretrained vae needed for training")              # model_fns.py:41
     image_seq_len = vae.image_seq_len                                           # model_fns.py:68
@@ -104,11 +104,11 @@ def dalle_model_fn(features, labels, mode, params):
                         text_vocab_size=params["text_vocab_size"], image_vocab_size=params["image_vocab_size"],
                         text_seq_len=params["text_seq_len"], image_seq_len=image_seq_len, device=device,
                         recompute_grad=bool(params.get("recompute_grad")) and mode == TRAIN,   # models.py:342
-                        # B200 extension key: shard fp32 master + Adam slots across the data-parallel ranks (ZeRO-1) —
-                        # what lets the 12 B configuration (README.md:5) fit 180 GB GPUs in pure data parallelism
+                        # extension key: shard fp32 master + Adam slots across the data-parallel ranks (ZeRO-1) —
+                        # what lets the d = 4096 configuration fit 80 GB GPUs in pure data parallelism
                         zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None)
     if params["bf_16"] is False and dp.rank == 0:
-        print("note: bf_16=false — the B200 engine still runs activations and matmul operands in bf16 with fp32 "
+        print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")
     if vae.K > params["image_vocab_size"]:
         raise ValueError(f"vae num_tokens {vae.K} exceeds image_vocab_size {params['image_vocab_size']}: image ids "
@@ -233,7 +233,7 @@ def vae_model_fn(features, labels, mode, params):
     if dp.rank == 0:
         print_n_params(model.n_params())
         if params.get("recompute_grad"):
-            print("note: recompute_grad=true (src/vae_tf/models.py:8-43) — the B200 engine keeps the residual-pair "
+            print("note: recompute_grad=true (src/vae_tf/models.py:8-43) — the engine keeps the residual-pair "
                   "activations instead of recomputing them (they fit in HBM many times over); gradients are identical")
     tg = params.get("train_gumbel_hard")
     eg = params.get("eval_gumbel_hard")

@@ -1,5 +1,5 @@
 """Model classes with the reference's constructor / forward signatures (src/dalle_mtf/models.py:141-416 DALLE,
-src/vae_tf/models.py:46-184 DiscreteVAE), backed by the B200 engines.  These are the objects a user of the reference
+src/vae_tf/models.py:46-184 DiscreteVAE), backed by the engines.  These are the objects a user of the reference
 instantiates directly; training goes through model_fns.* which drive the same engines.
 """
 import torch

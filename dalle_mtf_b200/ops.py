@@ -27,15 +27,19 @@ def _chk(t, dtype, name):
 
 
 # ----------------------------------------------------------------------------------------------- GEMM
-# bench.py sets GEMM_PROFILE to a list to time every tcgen05 GEMM launch with CUDA events on the launching stream:
+# bench.py sets GEMM_PROFILE to a list to time every wgmma GEMM launch with CUDA events on the launching stream:
 # entries are (start_event, end_event, algorithmic_flops).
 GEMM_PROFILE = None
+
+
+def _nbytes(ws):
+    return ws.numel() if ws is not None else 0
 
 
 def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=None, mode=L.EPI_STORE,
          alpha=1.0, bias=None, relu=False, residual=None, aux=None, split_k=1, labels=None, part_max=None,
          part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None):
-    """D[M,N] = A[M,K] @ B[K,N] on tcgen05.  a_mn / b_mn: operand is stored with M (resp. N) contiguous.
+    """D[M,N] = A[M,K] @ B[K,N] on wgmma.  a_mn / b_mn: operand is stored with M (resp. N) contiguous.
 
     a: [M,K] (k-major) or [K,M] (mn-major);  b: [N,K] (k-major) or [K,N] (mn-major).
     """
@@ -70,6 +74,8 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
         ldd = ldd if ldd is not None else out.stride(0)
     else:
         ldd = 0
+    ws = L.workspace(L.load().db200_gemm_workspace_bytes(M, N, K, ctypes.byref(e)))
+    e.workspace, e.workspace_bytes = ptr(ws), (ws.numel() if ws is not None else 0)
     prof = GEMM_PROFILE
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -99,7 +105,7 @@ def linear_dgrad(dy, w, out, relu_mask_of=None, colsum=None):
 
 
 def linear_wgrad(x, dy, dw, N=None):
-    """dw[K,N] (f32) += x[T,K]^T @ dy[T,N]      (both operands mn-major, split-K + red.add)."""
+    """dw[K,N] (f32) += x[T,K]^T @ dy[T,N]      (both operands mn-major, split-K summed in split order)."""
     T, K = x.shape
     N = N if N is not None else dy.shape[1]
     return gemm(x, dy, dw, K, N, T, a_mn=True, b_mn=True, mode=L.EPI_ATOMIC, split_k=0)
@@ -112,8 +118,10 @@ def ce_tiles(N):
 def ce_finish(part_max, part_sum, label_logit, lse, loss_rows, loss_sum):
     L.require_device()
     n_tiles, M = part_max.shape          # tile-major partials [n_tiles][M]
+    ws = L.workspace(L.load().db200_ce_finish_workspace_bytes(M))
     check(L.load().db200_ce_finish(stream_ptr(), ptr(part_max), ptr(part_sum), ptr(label_logit), ptr(lse),
-                                   ptr(loss_rows), ptr(loss_sum), M, n_tiles), "db200_ce_finish")
+                                   ptr(loss_rows), ptr(loss_sum), M, n_tiles, ptr(ws), _nbytes(ws)),
+          "db200_ce_finish")
 
 
 # ----------------------------------------------------------------------------------------------- row ops
@@ -131,7 +139,9 @@ def embed_bwd(ids, dx, dwte, dwpe):
     _chk(ids, I32, "ids"); _chk(dx, BF16, "dx"); _chk(dwte, F32, "dwte"); _chk(dwpe, F32, "dwpe")
     B, S = ids.shape
     V, d = dwte.shape
-    check(L.load().db200_embed_bwd(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V), "embed_bwd")
+    ws = L.workspace(L.load().db200_embed_bwd_workspace_bytes(d, V))
+    check(L.load().db200_embed_bwd(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V, ptr(ws),
+                                   _nbytes(ws)), "embed_bwd")
 
 
 def assemble_tokens(text_ids, image_idx, tokens, image_offset):
@@ -168,8 +178,10 @@ def layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=None):
     _chk(dy, BF16, "dy"); _chk(x, BF16, "x"); _chk(dres, BF16, "dres"); _chk(dx, BF16, "dx")
     _chk(g, F32, "g"); _chk(dg, F32, "dg"); _chk(db, F32, "db"); _chk(dxsum, F32, "dxsum")
     rows, d = x.shape
+    ws = L.workspace(L.load().db200_layernorm_bwd_workspace_bytes(rows, d))
     check(L.load().db200_layernorm_bwd_ex(stream_ptr(), ptr(dy), ptr(x), ptr(g), ptr(mean), ptr(rstd), ptr(dres),
-                                          ptr(dx), ptr(dg), ptr(db), ptr(dxsum), rows, d), "layernorm_bwd")
+                                          ptr(dx), ptr(dg), ptr(db), ptr(dxsum), rows, d, ptr(ws), _nbytes(ws)),
+          "layernorm_bwd")
     return dx
 
 
@@ -178,7 +190,9 @@ def colsum(x, out_accum, rows=None, cols=None):
     _chk(x, BF16, "x"); _chk(out_accum, F32, "out_accum")
     rows = rows if rows is not None else x.shape[0]
     cols = cols if cols is not None else x.shape[1]
-    check(L.load().db200_colsum_bf16(stream_ptr(), ptr(x), x.stride(0), rows, cols, ptr(out_accum)), "colsum")
+    ws = L.workspace(L.load().db200_colsum_workspace_bytes(rows, cols))
+    check(L.load().db200_colsum_bf16(stream_ptr(), ptr(x), x.stride(0), rows, cols, ptr(out_accum), ptr(ws),
+                                     _nbytes(ws)), "colsum")
 
 
 def cast_f32_to_bf16(src, dst):
@@ -243,7 +257,8 @@ def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0)
 def sqnorm(g, out_accum):
     L.require_device()
     _chk(g, F32, "g"); _chk(out_accum, F32, "out_accum")
-    check(L.load().db200_sqnorm_f32(stream_ptr(), ptr(g), g.numel(), ptr(out_accum)), "sqnorm")
+    ws = L.workspace(L.load().db200_sqnorm_workspace_bytes(g.numel()))
+    check(L.load().db200_sqnorm_f32(stream_ptr(), ptr(g), g.numel(), ptr(out_accum), ptr(ws), _nbytes(ws)), "sqnorm")
 
 
 def adam_step(p, m, v, g, p_bf16, lr, beta1=0.9, beta2=0.999, eps=1e-6, weight_decay=0.0, gnorm_sq=None,
@@ -296,7 +311,7 @@ def conv2d_fwd(c, x, w, bias, residual, y):
 
 
 def conv2d_fwd_tc(c, x, w_bf16, bias, residual, y):
-    """tcgen05 implicit-GEMM forward (bf16 activations / kernel).  Raises if the shape is not supported."""
+    """wgmma implicit-GEMM forward (bf16 activations / kernel).  Raises if the shape is not supported."""
     L.require_device()
     _chk(x, BF16, "x"); _chk(w_bf16, BF16, "w"); _chk(y, BF16, "y"); _chk(residual, BF16, "residual")
     check(L.load().db200_conv2d_fwd_tc(stream_ptr(), ctypes.byref(c), ptr(x), ptr(w_bf16), ptr(bias), ptr(residual),
@@ -323,7 +338,7 @@ def _tc_geometry_ok(c):
 
 
 def conv_tc_supported(c):
-    """forward (conv or conv-transpose) on tcgen05"""
+    """forward (conv or conv-transpose) on wgmma"""
     return _tc_geometry_ok(c) and c.Cin % 64 == 0 and c.Cout % 8 == 0
 
 

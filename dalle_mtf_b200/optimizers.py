@@ -27,7 +27,7 @@ class OptimizerConfig:
             raise ValueError(f"weight_decay must be a non-negative number, got {self.weight_decay!r}")
         if self.optimizer != "adam":
             # the Adafactor branch (optimizers.py:90-97) is selected by no reference config (SURVEY.md §2 row 7)
-            raise ValueError(f"{self.optimizer} not recognized (only 'adam' is implemented on B200)")
+            raise ValueError(f"{self.optimizer} not recognized (only 'adam' is implemented)")
 
     def learning_rate(self, step):
         """Value used for the update taken at global step `step` (the step counter before the increment,

@@ -1,4 +1,4 @@
-"""Discrete-VAE engine (host side) on the sm_100a kernels: encoder / Gumbel-softmax quantiser / decoder, forward and
+"""Discrete-VAE engine (host side) on the sm_90a kernels: encoder / Gumbel-softmax quantiser / decoder, forward and
 backward as explicit kernel sequences, flat fp32 parameter / gradient / Adam buffers.
 
 Mirrors src/vae_tf/models.py:46-184 (DiscreteVAE), src/vae_tf/layers.py:4-25 and the optimiser wiring of
@@ -37,7 +37,7 @@ class VaeEngine:
         self.C = self.img_C * self.stack_factor ** 2
         self.use_bf16 = bool(use_bf16)
         # src/vae_tf/models.py:8-43 re-runs every residual pair inside backward to save activation memory.  Here the
-        # activations are simply kept: at vae_coco (256 px, 16 images per GPU, bf16) they take ~6 GB of the 180 GB, and
+        # activations are simply kept: at vae_coco (256 px, 16 images per GPU, bf16) they take ~6 GB of the 80 GB, and
         # recomputing would add a forward pass of FLOPs for nothing.  Gradients are identical either way (the
         # recomputation is deterministic), so the flag only changes memory, never numbers; model_fns says so at start-up.
         self.recompute_grad = bool(recompute_grad)
@@ -93,7 +93,7 @@ class VaeEngine:
         # bf16 copy of the kernels for the tensor-core convolutions (use_bf16 only)
         self.shadow = torch.zeros(n, dtype=BF16, device=dev) if self.use_bf16 else None
         # codebook matmuls: the reference keeps them in fp32 (models.py:115-118).  In bf16 mode they run on the
-        # tcgen05 GEMM with every fp32 operand split into bf16 hi + lo parts (fp32 accumulation): ~2^-16 relative.
+        # wgmma GEMM with every fp32 operand split into bf16 hi + lo parts (fp32 accumulation): ~2^-16 relative.
         self._cb_tc = self.use_bf16 and self.n_hid % 8 == 0 and self.K % 8 == 0
         if self._cb_tc:
             self.cb_hi = torch.zeros(self.n_hid, self.K, dtype=BF16, device=dev)
@@ -131,7 +131,7 @@ class VaeEngine:
             ops.split_f32(self.P("codebook/codebook"), self.cb_hi, self.cb_lo)
 
     def _mm_split(self, a_parts, b_parts, out_f32, M, N, K, b_mn):
-        """out = sum over the listed (a, b) pairs of a @ b on tcgen05 (first product stores, the rest red.add)."""
+        """out = sum over the listed (a, b) pairs of a @ b on wgmma (first product stores, the rest red.add)."""
         first = True
         for a, bb in zip(a_parts, b_parts):
             if first:
@@ -142,7 +142,7 @@ class VaeEngine:
         return out_f32
 
     def _conv_fwd(self, dsc, x, name, residual, y):
-        """One forward convolution: tcgen05 implicit GEMM when the layer qualifies (bf16, Cin % 64 == 0), else the
+        """One forward convolution: wgmma implicit GEMM when the layer qualifies (bf16, Cin % 64 == 0), else the
         shared-memory-staged direct kernel (first layer with 3 input channels, transposed convs, fp32 mode)."""
         if self.use_bf16 and ops.conv_tc_supported(dsc):
             return ops.conv2d_fwd_tc(dsc, x, self.W16(name + "/kernel"), self.P(name + "/bias"), residual, y)

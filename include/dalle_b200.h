@@ -1,4 +1,4 @@
-/* dalle_b200.h — C ABI of libdalle_b200.so (hand-written sm_100a kernels for the DALL-E / dVAE training hot path).
+/* dalle_b200.h — C ABI of libdalle_b200.so (hand-written sm_90a kernels for the DALL-E / dVAE training hot path).
  *
  * The reference (EleutherAI/DALLE-mtf) has no FFI: its arithmetic is executed by mesh-tensorflow / TensorFlow ops
  * called from Python graph-building code.  Each entry point below replaces the library call(s) the reference makes
@@ -10,6 +10,10 @@
  *     Nothing throws, nothing calls exit().  Shape / alignment violations are checked and reported.
  *   - all tensor pointers are raw DEVICE pointers owned by the caller (PyTorch); row-major, innermost dim contiguous,
  *     16-byte aligned.  The library never allocates or frees device memory and keeps no pointers across calls.
+ *   - reductions over many CTAs are never float atomics: each CTA stores a partial into a scratch WORKSPACE the caller
+ *     passes in (its size comes from the matching db200_*_workspace_bytes query, which depends on the shape and the
+ *     device's SM count), and the partials are added in a fixed order on the same stream, so results are identical
+ *     from run to run.  A workspace may be reused as soon as the call's work on that stream has finished.
  *   - `stream` is a cudaStream_t (CUstream) passed as void*; kernels are enqueued on it and the call returns
  *     without synchronising.
  *   - bf16 = __nv_bfloat16 (2 bytes).  "f32" = IEEE float.
@@ -36,18 +40,21 @@ const char* db200_last_error(void);
 int db200_version(void);
 /* number of kernels this library has launched in this process (monotonic; used for bench.py's gpu_launches) */
 unsigned long long db200_launch_count(void);
-/* 0 if the current CUDA device is compute capability 10.x (sm_100a cubins can run), else DB200_E_UNSUPPORTED. */
+/* 0 if the current CUDA device is compute capability 9.0 (sm_90a cubins can run), else DB200_E_UNSUPPORTED. */
 int db200_device_check(void);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * K1  token + position embedding.   Replaces mtf.gather(wte, ids) + mtf.gather(wpe, range) + add
  *     src/dalle_mtf/models.py:186-219.   out[b,s,:] = wte[ids[b,s],:] + wpe[s,:]
- *     bwd: dwte[ids[b,s],:] += dx[b,s,:]   (fp32 atomics),  dwpe[s,:] += sum_b dx[b,s,:]
+ *     bwd: dwte[ids[b,s],:] += dx[b,s,:]   (order-independent: 64-bit fixed point),  dwpe[s,:] += sum_b dx[b,s,:]
  * ------------------------------------------------------------------------------------------------------------------ */
 int db200_embed_fwd(db200_stream_t stream, const int32_t* ids, const void* wte_bf16, const void* wpe_bf16,
                     void* out_bf16, int B, int S, int d, int V);
+/* embed_bwd sums dwte rows in 64-bit fixed point (2^-40 resolution, |sum| < 8.4e6) in the workspace: integer addition
+ * does not depend on the order in which tokens with the same id arrive. */
 int db200_embed_bwd(db200_stream_t stream, const int32_t* ids, const void* dx_bf16, float* dwte, float* dwpe, int B,
-                    int S, int d, int V);
+                    int S, int d, int V, void* workspace, int64_t workspace_bytes);
+int64_t db200_embed_bwd_workspace_bytes(int d, int V);
 
 /* T0 token assembly: tokens[b] = concat(text_ids[b], image_idx[b] + image_offset).  Replaces tf.concat at
  * src/model_fns.py:117-122 (image_offset = text_vocab_size). */
@@ -67,15 +74,17 @@ int db200_layernorm_fwd(db200_stream_t stream, const void* x_bf16, const float* 
                         float* mean, float* rstd, int rows, int d, float eps);
 int db200_layernorm_bwd(db200_stream_t stream, const void* dy_bf16, const void* x_bf16, const float* g,
                         const float* mean, const float* rstd, const void* dres_bf16_or_null, void* dx_bf16, float* dg,
-                        float* db, int rows, int d);
+                        float* db, int rows, int d, void* workspace, int64_t workspace_bytes);
 /* same, and additionally dxsum[c] += sum_rows dx[row][c]: the bias gradient of the linear layer whose output
  * gradient dx is (fuses the column-sum pass; dxsum may be NULL) */
 int db200_layernorm_bwd_ex(db200_stream_t stream, const void* dy_bf16, const void* x_bf16, const float* g,
                            const float* mean, const float* rstd, const void* dres_bf16_or_null, void* dx_bf16,
-                           float* dg, float* db, float* dxsum_or_null, int rows, int d);
+                           float* dg, float* db, float* dxsum_or_null, int rows, int d, void* workspace,
+                           int64_t workspace_bytes);
+int64_t db200_layernorm_bwd_workspace_bytes(int rows, int d);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * K3/K5/K6/K8  bf16 GEMM on tcgen05 (TMA-fed, TMEM accumulators, fp32 accumulate):   D[M,N] = A[M,K] * B[K,N]
+ * K3/K5/K6/K8  bf16 GEMM on wgmma (TMA-fed, register accumulators, fp32 accumulate):   D[M,N] = A[M,K] * B[K,N]
  *     Replaces every mtf einsum / mtf.layers.dense on the path: q/k/v/o projections src/dalle_mtf/models.py:235-244,
  *     303-311; MLP :317-324, 361-371; to_logits :391-395; and their mtf.gradients (src/optimizers.py:34).
  *   Operand storage:  a_mn_major = 0: A stored [M][K] (lda = row pitch in elements);  1: A stored [K][M].
@@ -84,7 +93,7 @@ int db200_layernorm_bwd_ex(db200_stream_t stream, const void* dy_bf16, const voi
  * ------------------------------------------------------------------------------------------------------------------ */
 enum {
   DB200_EPI_STORE = 0,    /* D = act(alpha*acc + bias[n]) + residual[m,n]  -> bf16 or f32                          */
-  DB200_EPI_ATOMIC = 1,   /* D(f32) += alpha*acc  (red.global.add; used for split-K / gradient accumulation)       */
+  DB200_EPI_ATOMIC = 1,   /* D(f32) += alpha*acc  (gradient accumulation; split-K slices summed in split order)   */
   DB200_EPI_RELU_BWD = 2, /* D(bf16) = alpha*acc * (aux[m,n] > 0)          (backward of the MLP's ReLU)            */
   DB200_EPI_CE_STATS = 3, /* no D: per (row, n-tile) max & sum-exp of acc+bias over valid columns + label logit    */
   DB200_EPI_CE_GRAD = 4   /* D(bf16) = alpha * (exp(acc+bias - lse[m]) - [n == label[m]]), 0 for n >= n_valid; alpha > 0 */
@@ -109,12 +118,16 @@ typedef struct db200_gemm_epilogue {
   int32_t n_valid;       /* CE_*: number of real vocabulary columns (<= N)                        */
   int32_t reserved;
   float* colsum;         /* CE_GRAD / RELU_BWD: colsum[n] += sum_m D[m][n] (fused bias gradient) or NULL */
+  void* workspace;       /* device scratch of db200_gemm_workspace_bytes() bytes (16-byte aligned), or NULL when 0 */
+  int64_t workspace_bytes;
 } db200_gemm_epilogue;
 
 int db200_gemm_bf16(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
                     int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi);
 /* number of N tiles the CE_STATS epilogue writes per row for a given N (host helper for sizing part_max/part_sum) */
 int db200_gemm_ce_tiles(int N);
+/* epi->workspace size for this product: split-K slices (ATOMIC) or fused column sums (CE_GRAD / RELU_BWD with colsum) */
+int64_t db200_gemm_workspace_bytes(int M, int N, int K, const db200_gemm_epilogue* epi);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * K7  cross-entropy pieces around the vocabulary GEMM (logits never reach HBM in fp32).
@@ -122,10 +135,12 @@ int db200_gemm_ce_tiles(int N);
  *     ce_finish:  lse[m] = logsumexp over tiles;  loss_rows[m] = lse[m] - label_logit[m];  *loss_sum += sum_m loss_rows
  * ------------------------------------------------------------------------------------------------------------------ */
 int db200_ce_finish(db200_stream_t stream, const float* part_max, const float* part_sum, const float* label_logit,
-                    float* lse, float* loss_rows, float* loss_sum, int M, int n_tiles);
+                    float* lse, float* loss_rows, float* loss_sum, int M, int n_tiles, void* workspace,
+                    int64_t workspace_bytes);
+int64_t db200_ce_finish_workspace_bytes(int M);
 
 /* ------------------------------------------------------------------------------------------------------------------
- * K4  causal flash attention on tcgen05.  Replaces mtf_transformer.attention.attention with the [S,S] -1e10 mask:
+ * K4  causal flash attention on wgmma.  Replaces mtf_transformer.attention.attention with the [S,S] -1e10 mask:
  *     src/dalle_mtf/models.py:221-227, 287-299.   qkv: bf16 [B][S][3][H][dh] (output of the fused q|k|v GEMM),
  *     out: bf16 [B][S][H][dh],  lse: f32 [B][H][S] (natural-log sum-exp of scale*q.k).  Reference scale = 1.0.
  *     bwd: dqkv same layout as qkv; dq_accum f32 [B][S][H][dh] and delta f32 [B][H][S] are caller workspaces.
@@ -140,7 +155,9 @@ int db200_attn_causal_bwd(db200_stream_t stream, const void* qkv_bf16, const voi
  * small HBM-bound helpers
  * ------------------------------------------------------------------------------------------------------------------ */
 /* out[c] += sum_r x[r][c]   (bias gradients) */
-int db200_colsum_bf16(db200_stream_t stream, const void* x_bf16, int64_t ld, int rows, int cols, float* out_accum);
+int db200_colsum_bf16(db200_stream_t stream, const void* x_bf16, int64_t ld, int rows, int cols, float* out_accum,
+                      void* workspace, int64_t workspace_bytes);
+int64_t db200_colsum_workspace_bytes(int rows, int cols);
 int db200_cast_f32_to_bf16(db200_stream_t stream, const float* src, void* dst_bf16, size_t n);
 int db200_cast_bf16_to_f32(db200_stream_t stream, const void* src_bf16, float* dst, size_t n);
 /* hi = bf16(x), lo = bf16(x - hi) (lo may be NULL): an fp32 operand as two bf16 tensor-core operands */
@@ -156,10 +173,12 @@ int db200_split_f32_to_bf16x2(db200_stream_t stream, const float* src, void* hi_
  *            bias_correction == 0:  p -= lr * (m / (sqrt(v) + eps) + wd*p)
  *            bias_correction == 1:  p -= lr*sqrt(1-b2^t)/(1-b1^t) * m / (sqrt(v) + eps)      (t = step, >= 1)
  *            p_bf16 (optional) receives the rounded updated parameter (compute copy).
- *            zero_grad != 0: g is overwritten with 0 once consumed (the gradient buffer accumulates with red.add, so it
+ *            zero_grad != 0: g is overwritten with 0 once consumed (the gradient buffer accumulates (+=), so it
  *            must start every step at zero: this folds that memset into the pass that already streams g).
  * ------------------------------------------------------------------------------------------------------------------ */
-int db200_sqnorm_f32(db200_stream_t stream, const float* g, size_t n, float* out_accum);
+int db200_sqnorm_f32(db200_stream_t stream, const float* g, size_t n, float* out_accum, void* workspace,
+                     int64_t workspace_bytes);
+int64_t db200_sqnorm_workspace_bytes(size_t n);
 int db200_adam_step(db200_stream_t stream, float* p, float* m, float* v, float* g, void* p_bf16_or_null,
                     size_t n, float lr, float beta1, float beta2, float eps, float weight_decay,
                     const float* gnorm_sq_or_null, float clip, float grad_scale, int bias_correction, int step,
@@ -186,7 +205,7 @@ typedef struct db200_conv_desc {
 
 int db200_conv2d_fwd(db200_stream_t stream, const db200_conv_desc* c, const void* x, const float* w,
                      const float* bias_or_null, const void* residual_or_null, void* y);
-/* Tensor-core paths (tcgen05 implicit GEMM; 4-D TMA boxes per filter tap, no im2col), bf16 NHWC activations, bf16
+/* Tensor-core paths (wgmma implicit GEMM; 4-D TMA boxes per filter tap, no im2col), bf16 NHWC activations, bf16
  * kernels (same memory layout as the f32 kernels: HWIO, or [kh][kw][out][in] for conv2d_transpose), f32 bias / dw.
  *   fwd_tc   : conv or conv2d_transpose forward; needs Cin % 64 == 0, Cout % 8 == 0
  *   dgrad_tc : needs Cout % 64 == 0, Cin % 8 == 0; optional ReLU mask (dx *= x_mask > 0) and residual-gradient add
@@ -309,7 +328,7 @@ int db200_space_to_depth_f32(db200_stream_t stream, const float* in, float* out,
  *   comm_unique_id    : ncclGetUniqueId into a caller buffer (>= 128 bytes); rank 0 creates it, the host code ships it
  *                       to the other ranks (any side channel), every rank then calls comm_create.
  *   comm_create       : ncclCommInitRankConfig on `device`; max_ctas > 0 caps the CTAs NCCL may occupy so that the
- *                       persistent tcgen05 GEMM grids running concurrently keep their SMs (0 = NCCL's default).
+ *                       persistent wgmma GEMM grids running concurrently keep their SMs (0 = NCCL's default).
  *   comm_register     : ncclCommRegister of a long-lived buffer (the flat gradient buffer); best effort.
  *   bucket_allreduce_launch : in-place SUM all-reduce of buf[0..count) (dtype DB200_F32 / DB200_BF16) on the comm
  *                       stream, ordered after everything already enqueued on compute_stream; does not block it.

@@ -62,7 +62,7 @@ def _worker(rank, world, port, out):
 
 def test_two_rank_step_equals_single_rank_step_on_concatenated_batch():
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     ctx = mp.get_context("spawn")
     out = ctx.Queue()
     port = _free_port()
@@ -121,7 +121,7 @@ def test_zero1_sharded_optimizer_matches_replicated_optimizer():
     """ZeRO-1 (optimiser-state sharding for the 12 B configuration, SURVEY.md §7): three steps with sharded
     master / Adam slots + in-place all-gather of the bf16 parameters == three steps with replicated state."""
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     ctx = mp.get_context("spawn")
     out = ctx.Queue()
     port = _free_port()

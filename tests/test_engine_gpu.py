@@ -82,7 +82,7 @@ def test_dalle_training_curve_tracks_oracle_for_several_steps():
     (Bias-correction-free Adam takes sign-like steps of size lr while v is tiny, so bf16 gradient noise is amplified
     step after step; with lr = 2e-3 the two trajectories drift apart by 9 % after six steps although every single-step
     quantity matches — hence a moderate lr here and a per-step bound that grows from 2e-3 to 2e-2;
-    measured drift on B200: 3e-7, 2e-5, 3e-4, 2e-3, 3e-3, 1e-2.)"""
+    measured drift: 3e-7, 2e-5, 3e-4, 2e-3, 3e-3, 1e-2.)"""
     from oracle import dalle as O
     from oracle import optim as OO
     cfg, params, tokens, eng = _dalle_case(256, 2, 2, 300, 60, 20, 12, 4, False, seed=3)
@@ -124,7 +124,7 @@ def test_dalle_class_mirrors_reference_forward_signature():
 @pytest.mark.parametrize("N,H,Cin,Cout,k,stride,transposed", [
     (2, 8, 16, 24, 3, 1, False), (2, 9, 5, 70, 3, 1, False), (2, 8, 3, 32, 4, 2, False), (3, 12, 20, 36, 4, 2, False),
     (2, 6, 24, 16, 4, 2, True), (1, 5, 70, 9, 4, 2, True), (2, 8, 16, 3, 1, 1, False),
-    # channel counts that are multiples of 64 run on tcgen05 through the three-way bf16 split (conv_f32_tc.cu)
+    # channel counts that are multiples of 64 run on wgmma through the three-way bf16 split (conv_f32_tc.cu)
     (2, 8, 64, 64, 3, 1, False), (3, 9, 128, 64, 3, 1, False), (2, 8, 64, 128, 4, 2, False),
     (2, 6, 128, 64, 4, 2, True), (1, 4, 256, 256, 3, 1, False), (2, 8, 64, 512, 1, 1, False),
     (5, 16, 64, 64, 3, 1, False)])
@@ -146,7 +146,7 @@ def test_direct_conv_fwd_dgrad_wgrad_fp32(N, H, Cin, Cout, k, stride, transposed
     ops.conv2d_fwd(c, xd, wd, bd, None, yd)
     ops.conv2d_dgrad(c, dyd, wd, None, None, dxd)
     ops.conv2d_wgrad(c, xd, dyd, dwd, dbd)
-    # CUDA-core path: fp32 FMA chains (1e-5).  tcgen05 path (channels % 64 == 0): products are exact to ~2^-24 through the
+    # CUDA-core path: fp32 FMA chains (1e-5).  wgmma path (channels % 64 == 0): products are exact to ~2^-24 through the
     # three-way split, but the tensor core adds partial sums with truncation, so long contractions (K = 9 x 256) sit at
     # ~1e-5 relative — still two orders below one bf16 rounding (4e-3)
     tol = 3e-5 if (Cin % 64 == 0 and Cout % 64 == 0) else 1e-5
@@ -180,7 +180,7 @@ def test_tensor_core_conv_forward_bf16(N, H, Cin, Cout, k, stride, relu, res):
     (2, 16, 64, 128, 4, 2, False), (2, 8, 128, 64, 4, 2, True), (5, 4, 256, 128, 4, 2, True),
     (1, 32, 256, 256, 3, 1, False)])
 def test_tensor_core_conv_training_kernels_bf16(N, H, Cin, Cout, k, stride, transposed):
-    """conv-transpose forward, dgrad (with ReLU mask + residual-gradient add) and wgrad on tcgen05 vs autograd."""
+    """conv-transpose forward, dgrad (with ReLU mask + residual-gradient add) and wgrad on wgmma vs autograd."""
     from dalle_mtf_b200 import ops
     from oracle import vae as OV
     g = torch.Generator().manual_seed(Cin * 7 + Cout + H)
@@ -209,7 +209,7 @@ def test_tensor_core_conv_training_kernels_bf16(N, H, Cin, Cout, k, stride, tran
 
 
 def test_vae_engine_bf16_training_step_on_tensor_cores():
-    """Whole VAE step with bf16 activations (tcgen05 conv fwd/dgrad/wgrad): loss and gradients vs the fp32 oracle."""
+    """Whole VAE step with bf16 activations (wgmma conv fwd/dgrad/wgrad): loss and gradients vs the fp32 oracle."""
     from dalle_mtf_b200.vae_engine import VaeEngine
     from oracle import vae as OV
     cb, K, size, B = [[2, 64], [2, 128]], 128, 32, 4
@@ -415,3 +415,32 @@ def test_vae_stack_factor_2_matches_oracle():
     eg = eng.export_params(eng.grads)
     for k in p:
         assert relfro(eg[k], leaves[k].grad) < 2e-2, k
+
+
+def test_training_step_is_bitwise_reproducible():
+    """Two engines from the same weights, fed the same tokens, agree bit for bit after three steps.  The shape takes the
+    split-K wgrad path (T = 512 tokens: two K splits), repeats token ids (embedding scatter onto shared rows) and runs
+    every ordered reduction of the step (LayerNorm dg / db, bias column sums, gradient norm, loss)."""
+    from dalle_mtf_b200.dalle_engine import DalleEngine
+    runs = []
+    for _ in range(2):
+        eng = DalleEngine(256, 2, 2, 500, 64, 64, 64)
+        eng.init_params(3)
+        tok = torch.randint(0, 40, (4, eng.S), generator=torch.Generator(device=DEV).manual_seed(7), device=DEV,
+                            dtype=torch.int32)
+        losses, grads = [], []
+        for _ in range(3):
+            eng.zero_grads()
+            acc = eng.forward(tok)
+            eng.backward(1.0 / tok.numel())
+            grads.append(eng.grads.clone())
+            losses.append(acc.clone())
+            eng.optimizer_step(1e-3)
+        torch.cuda.synchronize()
+        runs.append((losses, grads, eng.master.clone()))
+    (l0, g0, p0), (l1, g1, p1) = runs
+    for a, b in zip(l0, l1):
+        assert torch.equal(a, b)
+    for a, b in zip(g0, g1):
+        assert torch.isfinite(a).all() and torch.equal(a, b)
+    assert torch.equal(p0, p1)

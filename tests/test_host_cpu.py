@@ -216,8 +216,9 @@ def _free_port():
 
 
 def _dp_worker(rank, world, port, out):
+    # the host-only path under test: hide any GPU (a machine with fewer GPUs than ranks must still run this test)
     os.environ.update({"RANK": str(rank), "WORLD_SIZE": str(world), "LOCAL_RANK": str(rank),
-                       "MASTER_ADDR": "127.0.0.1", "MASTER_PORT": str(port)})
+                       "MASTER_ADDR": "127.0.0.1", "MASTER_PORT": str(port), "CUDA_VISIBLE_DEVICES": ""})
     from dalle_mtf_b200.dist import DataParallel
     dp = DataParallel().init(backend="gloo")
     assert dp.shard(8) == (rank * 4, 4)

@@ -34,17 +34,22 @@ def bf(x):
 # ------------------------------------------------------------------------------------------------------- GEMM
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (256, 512, 512), (200, 264, 200), (1000, 128, 328), (2048, 1536, 512),
                                    (1, 8, 8), (129, 8, 72),
-                                   (2504, 2056, 200)])  # 10 x 9 ragged 256x256 pair tiles >= 74: the 2-CTA kernel
+                                   (2504, 2056, 200)])  # ragged in M and N, more tiles than SMs
 @pytest.mark.parametrize("a_mn", [False, True])
 @pytest.mark.parametrize("b_mn", [False, True])
 def test_gemm_all_operand_layouts(ops, M, N, K, a_mn, b_mn):
-    if (a_mn and M % 8) or (b_mn and N % 8):
-        pytest.skip("mn-major operands need a 16-byte row pitch")
     g = torch.Generator().manual_seed(M + N + K)
     A, B = bf(torch.randn(M, K, generator=g)), bf(torch.randn(K, N, generator=g))
     ref = A.float() @ B.float()
-    a = (A.t().contiguous() if a_mn else A).to(DEV)
-    b = (B if b_mn else B.t().contiguous()).to(DEV)
+
+    def pitched(x):  # rows padded to a 16-byte pitch (what TMA needs): the GEMM reads the view through its row stride
+        rows, cols = x.shape
+        buf = torch.zeros(rows, (cols + 7) // 8 * 8, dtype=x.dtype)
+        buf[:, :cols] = x
+        return buf.to(DEV)[:, :cols]
+
+    a = pitched(A.t()) if a_mn else A.to(DEV)
+    b = pitched(B) if b_mn else B.t().contiguous().to(DEV)
     out = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
     ops.gemm(a, b, out, M, N, K, a_mn=a_mn, b_mn=b_mn)
     assert relmax(out, ref) < 1e-2
@@ -79,12 +84,12 @@ def test_gemm_epilogues(ops):
     assert L.EPI_ATOMIC == 1
 
 
-def test_gemm_epilogues_on_the_2cta_kernel(ops):
-    """Same epilogues on a ragged shape big enough (>= 74 pair tiles) to take the cta_group::2 path, including rows /
-    columns that end inside a 256x256 tile and the half of a pair that is entirely out of range."""
+def test_gemm_epilogues_on_a_large_ragged_shape(ops):
+    """Same epilogues on a ragged shape with more tiles than SMs (persistent CTAs take several tiles), including rows /
+    columns that end inside a tile."""
     from dalle_mtf_b200 import lib as L
     g = torch.Generator().manual_seed(11)
-    M, N, K = 2600, 2056, 136                      # 11 x 9 pair tiles; last pair: rows 2560..2599 only in CTA 0
+    M, N, K = 2600, 2056, 136                      # 21 x 17 tiles of 128 x 128; the last rows end mid-tile
     A, W = bf(torch.randn(M, K, generator=g)), bf(torch.randn(K, N, generator=g) * 0.1)
     bias, res = torch.randn(N, generator=g), bf(torch.randn(M, N, generator=g))
     a, w = A.to(DEV), W.to(DEV)
@@ -102,7 +107,7 @@ def test_gemm_epilogues_on_the_2cta_kernel(ops):
     ops.linear_dgrad(DY.to(DEV), W2.to(DEV), dx, relu_mask_of=H.to(DEV), colsum=cs)
     assert relmax(dx, (DY.float() @ W2.float().t()) * (H.float() > 0)) < 1e-2
     assert relmax(cs, dx.float().sum(0)) < 1e-5
-    # cross-entropy statistics and gradient over 11 x 8 pair tiles
+    # cross-entropy statistics and gradient over 21 x 16 tiles
     T, d, V, Vpad = 2600, 128, 2000, 2048
     X = bf(torch.randn(T, d, generator=g))
     Wv = torch.zeros(d, Vpad); Wv[:, :V] = torch.randn(d, V, generator=g) * 0.2; Wv = bf(Wv)

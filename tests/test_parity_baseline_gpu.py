@@ -4,7 +4,7 @@ The small-shape engine tests (tests/test_engine_gpu.py) stop at d <= 512, L = 2,
 shapes the bench is quoted on, with the batch cut to what the CPU oracle finishes in seconds:
 
   * EX   = configs[1] dalle_example @ BASELINE: d512 / L6 / H4 (dh128) / S = 256 + 1024 / V = 50 771 (odd: the padded
-           vocabulary tail Vpad = 50 816 and the 2-CTA cross-entropy epilogues are only exercised at this size), B = 2;
+           vocabulary tail Vpad = 50 816 and the cross-entropy epilogues over 397 column tiles are only exercised here), B = 2;
   * CO   = configs[3] dalle_coco  @ BASELINE geometry: d1024 / H16 (dh64) / S = 1280 / recompute_grad, L cut to 2, B = 1;
   * VC   = configs[2] vae_coco    @ BASELINE geometry: 256 px, convblocks [[2,128],[3,256],[5,512]], K = 8192 (bf16
            activations, fp32-split codebook GEMMs), B = 1;
@@ -24,9 +24,8 @@ Tolerances (north_star: "logits/loss within 1e-3 rel bf16, token indices bit-exa
   * token ids: bit-exact in fp32 mode (tests/test_engine_gpu.py); for the bf16 tensor-core tokenizer: exact-match
     rate >= 0.99 and every mismatch is a near-tie (margin < 0.1 * median margin).
 
-Measured values are appended to gpurun_out/parity_r02.jsonl (copied to profiles/ when committed).
+Measured values are printed as one `[parity]` line per case (pytest -s shows them).
 """
-import json
 import os
 
 import pytest
@@ -34,7 +33,6 @@ import torch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def relfro(a, b):
@@ -43,13 +41,6 @@ def relfro(a, b):
 
 
 def record(name, **kv):
-    out = os.path.join(ROOT, "gpurun_out")
-    try:
-        os.makedirs(out, exist_ok=True)
-        with open(os.path.join(out, "parity_r02.jsonl"), "a") as f:
-            f.write(json.dumps(dict(case=name, **kv)) + "\n")
-    except OSError:
-        pass
     print(f"[parity] {name}: " + ", ".join(f"{k}={v}" for k, v in kv.items()), flush=True)
 
 
@@ -142,7 +133,7 @@ def test_dalle_coco_geometry_recompute_matches_oracle():
 
 def test_vae_coco_geometry_k8192_bf16_matches_oracle():
     """VC geometry (configs/vae_coco_b200.json): 256 px, [[2,128],[3,256],[5,512]], K = 8192, bf16 activations with the
-    fp32 codebook matmuls on tcgen05 through the bf16 hi/lo split (src/vae_tf/models.py:81-184), soft Gumbel, B = 1."""
+    fp32 codebook matmuls on wgmma through the bf16 hi/lo split (src/vae_tf/models.py:81-184), soft Gumbel, B = 1."""
     from dalle_mtf_b200.vae_engine import VaeEngine
     from oracle import vae as OV
     torch.set_num_threads(max(1, os.cpu_count() or 1))
@@ -189,7 +180,7 @@ def test_vae_coco_geometry_k8192_bf16_matches_oracle():
 
 def test_bench_tokenizer_config_token_match_rate_and_near_tie_margins():
     """TOK: the tokenizer the bench runs in front of the transformer (configs/vae_example_b200.json: 256 px, K = 512,
-    use_bf16 -> tcgen05 convolutions; src/model_fns.py:72-77).  Token ids vs the fp32 oracle: exact-match rate and the
+    use_bf16 -> wgmma convolutions; src/model_fns.py:72-77).  Token ids vs the fp32 oracle: exact-match rate and the
     fp32 top-1 / top-2 margin of every mismatch (a flip is only acceptable where the fp32 logits are a near-tie)."""
     from dalle_mtf_b200.vae_engine import VaeEngine
     from oracle import vae as OV
@@ -213,7 +204,7 @@ def test_bench_tokenizer_config_token_match_rate_and_near_tie_margins():
                          median_margin=margin.median().item())
         record(f"TOK 256px K512 {mode}", **out[mode])
     assert out["fp32"]["n_mismatch"] == 0                                     # token indices: bit-exact
-    # 2 027 / 2 048 with every convolution (the first layer included, bf16-rounded weights) on tcgen05; what matters is
+    # 2 027 / 2 048 with every convolution (the first layer included, bf16-rounded weights) on wgmma; what matters is
     # that every flip is a near-tie of the fp32 logits (margin test below)
     assert out["bf16_tc"]["match"] >= 0.985
     assert out["bf16_tc"]["worst_mismatch_margin"] <= 0.1 * out["bf16_tc"]["median_margin"] + 1e-3

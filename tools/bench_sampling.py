@@ -1,4 +1,4 @@
-"""Generation throughput of the K/V-cache decoder (N4) on one B200: dalle_example_b200 shape (d=512, L=6, H=4,
+"""Generation throughput of the K/V-cache decoder (N4) on one GPU: dalle_example_b200 shape (d=512, L=6, H=4,
 256 text + 1024 image positions), random-init weights, batch 32.  Prints one JSON line."""
 import json
 import os

@@ -1,5 +1,5 @@
 """GPU diagnostics: runs every kernel family against CPU fp32 torch math and prints error statistics WITHOUT
-stopping at the first failure (one gpurun call should tell us as much as possible).  Not part of the test-suite;
+stopping at the first failure (one GPU session should tell as much as possible).  Not part of the test-suite;
 tests/ hold the real parity tests.  Usage: python tools/gpu_diag.py [gemm|rowops|optim|attn|all] ...
 """
 import os
@@ -249,7 +249,7 @@ def main():
         gemm_case(200, 264, 200, False, False, seed=6)
         gemm_case(1000, 128, 328, False, True, seed=7)     # BN=128 path
         gemm_case(2048, 1536, 512, False, True, seed=8)    # multi-wave persistent
-        for a_mn in (False, True):           # large M: takes the 2-CTA (cta_group::2) path
+        for a_mn in (False, True):           # large M: more tiles than SMs
             for b_mn in (False, True):
                 gemm_case(19976, 520, 264, a_mn, b_mn, seed=9)
         gemm_case(40960, 512, 512, False, True, seed=10)

@@ -56,7 +56,7 @@ def run(report, guarded):
     case(1, 520, 3, 64, 1.0, 1.5, 7)
     case(1, 129, 1, 128, 1.0, 0.5, 8)      # second tile has a single valid row
     case(2, 1280, 3, 64, 0.125, 1.0, 9)
-    # more (tile, head, batch) items than SMs: the persistent forward walks several items per CTA
+    # more (tile, head, batch) blocks than SMs
     case(8, 1280, 5, 128, 1.0, 0.25, 10)
     case(6, 1280, 8, 64, 0.125, 1.0, 11)
     case(5, 640, 8, 128, 1.0, 1.2, 12)

@@ -1,5 +1,5 @@
 """DALL-E training entry point — same flags and config surface as the reference's train_dalle.py
-(--tpu --gpu_ids --model --new; configs/*.json with the same keys), B200 engine underneath.
+(--tpu --gpu_ids --model --new; configs/*.json with the same keys), CUDA engine underneath.
 
 Launch one process per GPU:   python train_dalle.py --model dalle_example_b200
                               torchrun --nproc-per-node 8 --master-addr 127.0.0.1 train_dalle.py --model ...

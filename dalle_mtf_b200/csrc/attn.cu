@@ -16,9 +16,9 @@
 namespace db200 {
 
 int attn_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
-                    float scale);
+                    float scale, const db200_dropout* drop);
 int attn_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
-                       void* dqkv, int B, int S, int H, int dh, float scale);
+                       void* dqkv, int B, int S, int H, int dh, float scale, const db200_dropout* drop);
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward: delta = rowsum(dO * O)
@@ -60,20 +60,25 @@ attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ dout, flo
 
 using namespace db200;
 
-extern "C" int db200_attn_causal_fwd(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B, int S,
-                                     int H, int dh, float scale) {
+extern "C" int db200_attn_causal_fwd_ex(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B,
+                                        int S, int H, int dh, float scale, const db200_dropout* drop) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_fwd: B,S,H must be positive");
   DB200_REQUIRE(qkv && out && lse && aligned16(qkv) && aligned16(out), DB200_E_ALIGN,
                 "attn_fwd: NULL or unaligned pointer");
   DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_fwd: scale must be > 0");
   if (dh != 64 && dh != 128) return set_error(DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
-  return attn_fwd_launch(stream, qkv, out, lse, B, S, H, dh, scale);
+  return attn_fwd_launch(stream, qkv, out, lse, B, S, H, dh, scale, drop);
 }
 
-extern "C" int db200_attn_causal_bwd(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
-                                     const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S, int H,
-                                     int dh, float scale) {
+extern "C" int db200_attn_causal_fwd(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B, int S,
+                                     int H, int dh, float scale) {
+  return db200_attn_causal_fwd_ex(stream_, qkv, out, lse, B, S, H, dh, scale, nullptr);
+}
+
+extern "C" int db200_attn_causal_bwd_ex(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
+                                        const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S,
+                                        int H, int dh, float scale, const db200_dropout* drop) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   (void)dq_accum;  // kept in the ABI for an atomics-based variant; the two-kernel scheme does not need it
   DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_bwd: B,S,H must be positive");
@@ -93,5 +98,12 @@ extern "C" int db200_attn_causal_bwd(db200_stream_t stream_, const void* qkv, co
   }
   int rc = check_launch("attn_delta_kernel");
   if (rc != DB200_OK) return rc;
-  return attn_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, scale);
+  // delta = rowsum(dO * O) needs no dropout term: O already is the dropped output
+  return attn_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, scale, drop);
+}
+
+extern "C" int db200_attn_causal_bwd(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
+                                     const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S, int H,
+                                     int dh, float scale) {
+  return db200_attn_causal_bwd_ex(stream_, qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale, nullptr);
 }

@@ -9,6 +9,7 @@
 //
 // Layout: qkv bf16 [B][S][3][H][dh], out / dout bf16 [B][S][H][dh], lse / delta f32 [B][H][S], dqkv like qkv.
 #include "gemm_common.cuh"  // cp.async helpers
+#include "philox.cuh"
 #include "wgmma.cuh"
 
 namespace db200 {
@@ -57,15 +58,17 @@ __device__ __forceinline__ void fa_qk(float* s, uint32_t a_tile, uint32_t b_tile
   wgmma_wait<0>();
 }
 // acc[64 x DH] += P[64 x 64] (registers, fp32 fragment packed to bf16 here) * tile[64 x DH]
-template <int DH>
-__device__ __forceinline__ void fa_pv(float* acc, const float* p, uint32_t tile) {
+// DROP: fragment element x is multiplied by (bit x of kb) ? sc : 0 on the way (dropout of P)
+template <int DH, bool DROP = false>
+__device__ __forceinline__ void fa_pv(float* acc, const float* p, uint32_t tile, uint32_t kb = 0u, float sc = 1.f) {
   uint32_t a[4][4];
+  auto pk = [&](int x) { return DROP ? (((kb >> x) & 1u) ? p[x] * sc : 0.f) : p[x]; };
 #pragma unroll
   for (int ks = 0; ks < 4; ++ks) {
-    a[ks][0] = pack_bf16x2(p[8 * ks + 0], p[8 * ks + 1]);
-    a[ks][1] = pack_bf16x2(p[8 * ks + 2], p[8 * ks + 3]);
-    a[ks][2] = pack_bf16x2(p[8 * ks + 4], p[8 * ks + 5]);
-    a[ks][3] = pack_bf16x2(p[8 * ks + 6], p[8 * ks + 7]);
+    a[ks][0] = pack_bf16x2(pk(8 * ks + 0), pk(8 * ks + 1));
+    a[ks][1] = pack_bf16x2(pk(8 * ks + 2), pk(8 * ks + 3));
+    a[ks][2] = pack_bf16x2(pk(8 * ks + 4), pk(8 * ks + 5));
+    a[ks][3] = pack_bf16x2(pk(8 * ks + 6), pk(8 * ks + 7));
   }
   wgmma_fence();
 #pragma unroll
@@ -86,6 +89,31 @@ struct Frag {
     fc = 2 * (lane & 3);
   }
 };
+// Keep bits of this thread's 32 fragment elements of a 64 x 64 attention-weight tile (bit x = element x) whose first
+// row / column are r0 / c0.  QROWS: rows are queries and columns keys (forward, dQ); else rows are keys and columns
+// queries (dK / dV).  The two columns fc, fc + 1 of a row share one 2 x 2 block, so each Philox call serves two elements.
+template <bool QROWS>
+__device__ __forceinline__ uint32_t fa_keep_bits(const db200_dropout& dr, int b, int h, int H, int S2, int r0, int c0,
+                                                 const Frag& f) {
+  uint32_t kb = 0u;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = r0 + f.fr + 8 * hh, col = c0 + 8 * i + f.fc;  // col is even
+      const uint4 r = dropout_block(dr, QROWS ? dropout_attn_block(dr, b, h, H, S2, row, col)
+                                              : dropout_attn_block(dr, b, h, H, S2, col, row));
+      // word of (query i, key j) = 2 (i & 1) + (j & 1)
+      const uint32_t w0 = QROWS ? ((row & 1) ? r.z : r.x) : ((row & 1) ? r.y : r.x);
+      const uint32_t w1 = QROWS ? ((row & 1) ? r.w : r.y) : ((row & 1) ? r.w : r.z);
+      const int x = 4 * i + 2 * hh;
+      kb |= (uint32_t)(w0 >= dr.threshold) << x;
+      kb |= (uint32_t)(w1 >= dr.threshold) << (x + 1);
+    }
+  return kb;
+}
+__device__ __forceinline__ float fa_keep_mul(uint32_t kb, int x, float sc) { return ((kb >> x) & 1u) ? sc : 0.f; }
+
 __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -118,10 +146,10 @@ constexpr size_t fa_smem(int tiles) { return 1024 + size_t(tiles) * FA_ROWS * DH
 // ------------------------------------------------------------------------------------------------------------------
 // forward: grid (query blocks, B * H); online softmax in the exp2 domain
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(128, 1)
 attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale) {
+                float scale, const db200_dropout dr) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -181,7 +209,11 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
           v = exp2f(v - mb[hh]);
           l[hh] += v;
         }
-    fa_pv<DH>(o, s, sV);
+    // l (hence lse) sums the undropped weights; dropout acts on the normalised weights, i.e. on P before PV
+    if constexpr (DROP)
+      fa_pv<DH, true>(o, s, sV, fa_keep_bits<true>(dr, b, h, H, (S + 1) >> 1, q0, k0, f), dr.scale);
+    else
+      fa_pv<DH>(o, s, sV);
   }
   float inv[2];
 #pragma unroll
@@ -197,10 +229,11 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ: grid (query blocks, B * H).  P = exp(scale S - lse), dS = P (dO V^T - delta), dQ = scale dS K
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
-                   const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale) {
+                   const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
+                   const db200_dropout dr) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -234,6 +267,8 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
     float s[32], dp[32];
     fa_qk<DH>(s, sQ, sK);
     fa_qk<DH>(dp, sdO, sV);
+    // dropout: dS = P (dP keep scale - delta)
+    const uint32_t kb = DROP ? fa_keep_bits<true>(dr, b, h, H, (S + 1) >> 1, q0, k0, f) : 0u;
 #pragma unroll
     for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -243,7 +278,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           const int x = 4 * i + 2 * hh + e;
           const float p = (col <= row && col < S && row < S) ? exp2f(s[x] * sl2 - lse2[hh]) : 0.f;
-          s[x] = p * (dp[x] - dl[hh]);
+          s[x] = p * ((DROP ? dp[x] * fa_keep_mul(kb, x, dr.scale) : dp[x]) - dl[hh]);
         }
     fa_pv<DH>(dq, s, sK);
   }
@@ -255,10 +290,11 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
 // backward, dK / dV: grid (key blocks, B * H), transposed products so that the key index is the accumulator row.
 //   P^T = exp(scale K Q^T - lse), dV = P^T dO, dS^T = P^T (V dO^T - delta), dK = scale dS^T Q
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH>
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
-                    const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale) {
+                    const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
+                    const db200_dropout dr) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -302,7 +338,10 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
           const int x = 4 * ii + 2 * hh + e;
           st[x] = (key <= q && q < S && key < S) ? exp2f(st[x] * sl2 - s_lse[cq]) : 0.f;
         }
-    fa_pv<DH>(dv, st, sdO);
+    // dropout: dV += (P keep scale)^T dO,  dS = P (dP keep scale - delta)
+    const uint32_t kb = DROP ? fa_keep_bits<false>(dr, b, h, H, (S + 1) >> 1, k0, q0, f) : 0u;
+    if constexpr (DROP) fa_pv<DH, true>(dv, st, sdO, kb, dr.scale);
+    else fa_pv<DH>(dv, st, sdO);
     fa_qk<DH>(dpt, sV, sdO);
 #pragma unroll
     for (int ii = 0; ii < 8; ++ii)
@@ -311,7 +350,7 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int x = 4 * ii + 2 * hh + e;
-          st[x] = st[x] * (dpt[x] - s_dl[8 * ii + f.fc + e]);
+          st[x] = st[x] * ((DROP ? dpt[x] * fa_keep_mul(kb, x, dr.scale) : dpt[x]) - s_dl[8 * ii + f.fc + e]);
         }
     fa_pv<DH>(dk, st, sQ);
   }
@@ -321,47 +360,57 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
   fa_store_rows<DH>(dst + 2LL * H * DH, ldq, dv, one, S - k0, f);
 }
 
-template <int DH>
-static int fa_fwd(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, float scale) {
+template <int DH, bool DROP>
+static int fa_fwd(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, float scale,
+                  const db200_dropout& dr) {
   constexpr size_t smem = fa_smem<DH>(3);
   static const cudaError_t attr_rc =
-      cudaFuncSetAttribute(attn_fwd_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(attr_rc);
   const dim3 grid((S + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_fwd_kernel<DH><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale);
+  attn_fwd_kernel<DH, DROP><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale, dr);
   return check_launch("attn_fwd_kernel");
 }
 
-template <int DH>
+template <int DH, bool DROP>
 static int fa_bwd(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
-                  void* dqkv, int B, int S, int H, float scale) {
+                  void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr) {
   constexpr size_t smem = fa_smem<DH>(4);
   static const cudaError_t rc1 =
-      cudaFuncSetAttribute(attn_bwd_dq_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   static const cudaError_t rc2 =
-      cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(rc1);
   DB200_CUDA(rc2);
   const dim3 grid((S + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_bwd_dq_kernel<DH><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta, (bf16*)dqkv,
-                                                      S, H, scale);
+  attn_bwd_dq_kernel<DH, DROP><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
+                                                            (bf16*)dqkv, S, H, scale, dr);
   int rc = check_launch("attn_bwd_dq_kernel");
   if (rc != DB200_OK) return rc;
-  attn_bwd_dkv_kernel<DH><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta, (bf16*)dqkv,
-                                                       S, H, scale);
+  attn_bwd_dkv_kernel<DH, DROP><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
+                                                             (bf16*)dqkv, S, H, scale, dr);
   return check_launch("attn_bwd_dkv_kernel");
 }
 
+// drop == NULL (or threshold 0): the kernels without dropout
 int attn_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
-                    float scale) {
-  return dh == 128 ? fa_fwd<128>(stream, qkv, out, lse, B, S, H, scale)
-                   : fa_fwd<64>(stream, qkv, out, lse, B, S, H, scale);
+                    float scale, const db200_dropout* drop) {
+  const db200_dropout none{};
+  if (dropout_active(drop))
+    return dh == 128 ? fa_fwd<128, true>(stream, qkv, out, lse, B, S, H, scale, *drop)
+                     : fa_fwd<64, true>(stream, qkv, out, lse, B, S, H, scale, *drop);
+  return dh == 128 ? fa_fwd<128, false>(stream, qkv, out, lse, B, S, H, scale, none)
+                   : fa_fwd<64, false>(stream, qkv, out, lse, B, S, H, scale, none);
 }
 
 int attn_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
-                    void* dqkv, int B, int S, int H, int dh, float scale) {
-  return dh == 128 ? fa_bwd<128>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale)
-                   : fa_bwd<64>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale);
+                    void* dqkv, int B, int S, int H, int dh, float scale, const db200_dropout* drop) {
+  const db200_dropout none{};
+  if (dropout_active(drop))
+    return dh == 128 ? fa_bwd<128, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, *drop)
+                     : fa_bwd<64, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, *drop);
+  return dh == 128 ? fa_bwd<128, false>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none)
+                   : fa_bwd<64, false>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none);
 }
 
 }  // namespace db200

@@ -29,7 +29,8 @@ constexpr size_t G_SMEM_BYTES =
     1024 /*align slack*/ + G_ACC_BYTES + size_t(G_STAGES) * G_STAGE_BYTES + 256 /*barriers*/ + 8 * 4096 /*staging*/;
 static_assert(G_SMEM_BYTES <= 227 * 1024, "GEMM shared memory exceeds the H100 per-block limit");
 
-template <int TA, int TB>  // operand majors (1 = MN-major), compile-time for wgmma
+// operand majors (1 = MN-major), compile-time for wgmma; DROP: dropout in the STORE epilogue
+template <int TA, int TB, bool DROP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr int BN = GBN;
@@ -155,7 +156,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       named_bar_sync(1, 256);
       const uint32_t t_addr = (sAcc >> 2) + (wq * 32 + lane) * BN + half * (BN / 2);
       switch (p.mode) {
-        case DB200_EPI_STORE:    epi_store<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
+        case DB200_EPI_STORE:    epi_store<CH, DROP>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
         case DB200_EPI_ATOMIC:
           epi_atomic<CH>(p, reinterpret_cast<float*>(p.D) + (long long)t.split * p.M * p.ldd, row, row_ok, cbase,
                          t_addr);
@@ -169,15 +170,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
-template <int TA, int TB>
+template <int TA, int TB, bool DROP>
 static int launch_gemm(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                           (int)G_SMEM_BYTES);  // once, thread-safe (magic static)
   DB200_CUDA(attr_rc);
   const int total = p.m_tiles * p.n_tiles * p.splits;
   const int grid = total < sm_count() ? total : sm_count();
-  gemm_tc_kernel<TA, TB><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_tc_kernel<TA, TB, DROP><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
   return check_launch("gemm_tc_kernel");
 }
 
@@ -217,8 +218,16 @@ extern "C" int64_t db200_gemm_workspace_bytes(int M, int N, int K, const db200_g
 extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B,
                                int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
                                const db200_gemm_epilogue* epi) {
+  return db200_gemm_bf16_ex(stream_, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr);
+}
+
+extern "C" int db200_gemm_bf16_ex(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B,
+                                  int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                                  const db200_gemm_epilogue* epi, const db200_dropout* dropout) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(epi != nullptr, DB200_E_INVALID, "gemm: epilogue descriptor is NULL");
+  const bool drop = dropout_active(dropout);
+  DB200_REQUIRE(!drop || epi->mode == DB200_EPI_STORE, DB200_E_INVALID, "gemm: dropout needs the STORE epilogue");
   DB200_REQUIRE(M > 0 && N > 0 && K > 0, DB200_E_INVALID, "gemm: M,N,K must be positive (got %d,%d,%d)", M, N, K);
   DB200_REQUIRE(A && B, DB200_E_INVALID, "gemm: NULL operand");
   DB200_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, DB200_E_ALIGN,
@@ -284,6 +293,7 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   p.lse = epi->lse;
   p.n_valid = epi->n_valid;
   p.colsum = (mode == DB200_EPI_CE_GRAD || mode == DB200_EPI_RELU_BWD) ? epi->colsum : nullptr;
+  p.drop = drop ? *dropout : db200_dropout{};
 
   p.n_tiles = (N + GBN - 1) / GBN;
   p.n_parts = 2 * p.n_tiles;
@@ -322,8 +332,11 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   } else if (colsum_out) {
     p.colsum = static_cast<float*>(epi->workspace);
   }
-  if (p.a_mn) rc = p.b_mn ? launch_gemm<1, 1>(stream, tmA, tmB, p) : launch_gemm<1, 0>(stream, tmA, tmB, p);
-  else        rc = p.b_mn ? launch_gemm<0, 1>(stream, tmA, tmB, p) : launch_gemm<0, 0>(stream, tmA, tmB, p);
+  if (drop)    // residual dropout runs in forward products only: A k-major, B mn-major
+    rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, true>(stream, tmA, tmB, p)
+                             : set_error(DB200_E_UNSUPPORTED, "gemm: dropout needs a k-major A and an mn-major B");
+  else if (p.a_mn) rc = p.b_mn ? launch_gemm<1, 1, false>(stream, tmA, tmB, p) : launch_gemm<1, 0, false>(stream, tmA, tmB, p);
+  else             rc = p.b_mn ? launch_gemm<0, 1, false>(stream, tmA, tmB, p) : launch_gemm<0, 0, false>(stream, tmA, tmB, p);
   if (rc != DB200_OK) return rc;
   if (p.splits > 1) return reduce_splits_add(stream, static_cast<const float*>(p.D), p.splits, M, N, d_out, ldd);
   if (colsum_out) return reduce_rows_add(stream, p.colsum, row_blocks, N, colsum_out);

@@ -2,6 +2,7 @@
 // (wgmma.cuh: acc_store_smem / acc_ld_x32) into global-memory results; the convolutions reuse the staging helpers.
 #pragma once
 #include "common.cuh"
+#include "philox.cuh"
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -36,6 +37,7 @@ struct GemmParams {
   int n_valid;
   int n_parts;  // CE_STATS: partials per row = 2 * n_tiles (one per half tile)
   float* colsum;  // CE_GRAD / RELU_BWD: workspace [M/32 row blocks][N] of column sums (bias gradient), or NULL
+  db200_dropout drop;  // STORE with dropout (kernel instantiated with DROP = true): elementwise mask over [M][N]
 };
 
 struct TileCoord {
@@ -223,7 +225,21 @@ __device__ __forceinline__ void stage_colsum_bf16(uint32_t stg, float* colsum, i
   if (col + 1 < N) colsum[col + 1] = s1 + s3;
 }
 
-template <int CH>
+// o[j] *= keep ? scale : 0 for columns col0 .. col0 + 31 of row `row` (elementwise mask over [M][N]; col0 and N are
+// multiples of 4, so the 32 columns are 8 whole Philox blocks)
+__device__ __forceinline__ void dropout_row32(const db200_dropout& dr, int row, int N, int col0, float* o) {
+  const uint64_t n0 = dropout_elem_block(dr, row, N, col0);
+#pragma unroll
+  for (int g = 0; g < 8; ++g) {
+    const uint4 r = dropout_block(dr, n0 + g);
+    o[4 * g + 0] *= dropout_mul(dr, r.x);
+    o[4 * g + 1] *= dropout_mul(dr, r.y);
+    o[4 * g + 2] *= dropout_mul(dr, r.z);
+    o[4 * g + 3] *= dropout_mul(dr, r.w);
+  }
+}
+
+template <int CH, bool DROP = false>
 __device__ __forceinline__ void epi_store(const GemmParams& p, uint32_t t_addr, int row, bool row_ok, int cbase,
                                           uint32_t stg, int row0, int lane) {
   static_assert(CH % 2 == 0, "epilogue works on pairs of 32-column chunks");
@@ -258,6 +274,7 @@ __device__ __forceinline__ void epi_store(const GemmParams& p, uint32_t t_addr, 
 #pragma unroll
         for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], 0.f);
       }
+      if constexpr (DROP) dropout_row32(p.drop, row, p.N, col0, o);
       if (p.residual) {
         float rr[32];
         stage_get_bf16(stg, lane, h, rr);

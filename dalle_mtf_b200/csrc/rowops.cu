@@ -5,6 +5,7 @@
 // Reference: src/dalle_mtf/models.py:186-219 (embedding), :373-389 + src/dalle_mtf/layers.py:30-33 (LayerNorm),
 //            :348-359 (loss reduction).
 #include "common.cuh"
+#include "philox.cuh"
 #include "ptx.cuh"
 
 namespace db200 {
@@ -41,6 +42,39 @@ __global__ void embed_fwd_kernel(const int* __restrict__ ids, const bf16* __rest
   }
 }
 
+// 8 keep multipliers (keep ? scale : 0) of columns c .. c + 7 of row r of an elementwise mask over [rows][cols]
+__device__ __forceinline__ void dropout_mul8(const db200_dropout& dr, long long r, int cols, int c, float* m) {
+  const uint64_t n0 = dropout_elem_block(dr, r, cols, c);
+  const uint4 a = dropout_block(dr, n0), b = dropout_block(dr, n0 + 1);
+  m[0] = dropout_mul(dr, a.x); m[1] = dropout_mul(dr, a.y); m[2] = dropout_mul(dr, a.z); m[3] = dropout_mul(dr, a.w);
+  m[4] = dropout_mul(dr, b.x); m[5] = dropout_mul(dr, b.y); m[6] = dropout_mul(dr, b.z); m[7] = dropout_mul(dr, b.w);
+}
+
+// embedding dropout (src/dalle_mtf/models.py:198-200, 215-217): out = wte[id] * keep_wte * scale + wpe[s] * keep_wpe *
+// scale; the wte mask is over the [T][d] gathered rows, the wpe mask over [S][d] (shared by the batch)
+__global__ void embed_fwd_drop_kernel(const int* __restrict__ ids, const bf16* __restrict__ wte,
+                                      const bf16* __restrict__ wpe, bf16* __restrict__ out, int T, int S, int d, int V,
+                                      const db200_dropout dw, const db200_dropout dp) {
+  const int vec_per_row = d >> 3;
+  const long long total = (long long)T * vec_per_row;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int t = (int)(i / vec_per_row);
+    const int c = (int)(i - (long long)t * vec_per_row) << 3;
+    int id = ids[t];
+    id = id < 0 ? 0 : (id >= V ? V - 1 : id);
+    const int s = t % S;
+    float a[8], b[8], ma[8], mb[8];
+    unpack8(*reinterpret_cast<const uint4*>(wte + (long long)id * d + c), a);
+    unpack8(*reinterpret_cast<const uint4*>(wpe + (long long)s * d + c), b);
+    dropout_mul8(dw, t, d, c, ma);
+    dropout_mul8(dp, s, d, c, mb);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) a[j] = a[j] * ma[j] + b[j] * mb[j];
+    *reinterpret_cast<uint4*>(out + (long long)t * d + c) = pack8(a);
+  }
+}
+
 // dwte[ids[t]] += dx[t].  A thread owns 8 columns of a strip of EMB_STRIP consecutive tokens and merges RUNS of equal
 // ids in registers before touching memory: captions are right-padded with one id (src/input_fns.py:32-38), so the
 // ~220 consecutive padding positions of every sequence collapse into one reduction per strip instead of 220 serialised
@@ -52,10 +86,12 @@ constexpr double EMB_FIX_SCALE = 1099511627776.0;  // 2^40: resolution 9.1e-13, 
 __device__ __forceinline__ void fixed_add(unsigned long long* dst, float v) {
   atomicAdd(dst, static_cast<unsigned long long>(__double2ll_rn(static_cast<double>(v) * EMB_FIX_SCALE)));
 }
+// DROP: dx[t] is multiplied by the wte keep mask first.
 constexpr int EMB_STRIP = 32;
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, unsigned long long* __restrict__ acc64,
-                     int T, int d, int V) {
+                     int T, int d, int V, const db200_dropout dw) {
   const int vec_per_row = d >> 3;
   const long long total = (long long)((T + EMB_STRIP - 1) / EMB_STRIP) * vec_per_row;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
@@ -82,6 +118,12 @@ embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, u
       }
       float g[8];
       unpack8(*reinterpret_cast<const uint4*>(dx + (long long)t * d + c), g);
+      if constexpr (DROP) {
+        float m[8];
+        dropout_mul8(dw, t, d, c, m);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) g[j] *= m[j];
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] += g[j];
     }
@@ -100,8 +142,11 @@ embed_fixed_flush_kernel(const unsigned long long* __restrict__ acc64, float* __
   }
 }
 
-// one thread owns (s, 8 columns): dwpe[s][c..c+8) += sum_b dx[b][s][c..c+8)
-__global__ void embed_bwd_wpe_kernel(const bf16* __restrict__ dx, float* __restrict__ dwpe, int B, int S, int d) {
+// one thread owns (s, 8 columns): dwpe[s][c..c+8) += sum_b dx[b][s][c..c+8)   (DROP: times the wpe keep mask of s,
+// which every sequence shares)
+template <bool DROP>
+__global__ void embed_bwd_wpe_kernel(const bf16* __restrict__ dx, float* __restrict__ dwpe, int B, int S, int d,
+                                     const db200_dropout dp) {
   const int vec_per_row = d >> 3;
   const int total = S * vec_per_row;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -114,6 +159,12 @@ __global__ void embed_bwd_wpe_kernel(const bf16* __restrict__ dx, float* __restr
     unpack8(*reinterpret_cast<const uint4*>(dx + ((long long)b * S + s) * d + c), g);
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] += g[j];
+  }
+  if constexpr (DROP) {
+    float m[8];
+    dropout_mul8(dp, s, d, c, m);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] *= m[j];
   }
   float* dst = dwpe + (long long)s * d + c;
 #pragma unroll
@@ -187,14 +238,40 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, co
   }
 }
 
+// store 8 columns of dx; DROP: also dxm = dx * keep * scale (mask of row `row` over [rows][d]).  The column sum adx
+// takes the values exactly as stored (bf16-rounded), of dxm when DROP and of dx otherwise, like a separate column-sum
+// pass would.
+template <bool DROP>
+__device__ __forceinline__ void ln_bwd_store8(const float* o, bf16* dx, bf16* dxm, long long row, int d, int col,
+                                              bool dxsum, const db200_dropout& dr, float* adx) {
+  const uint4 packed = pack8(o);
+  *reinterpret_cast<uint4*>(dx + row * d + col) = packed;
+  float ro[8];
+  unpack8(packed, ro);
+  if constexpr (DROP) {
+    float m[8];
+    dropout_mul8(dr, row, d, col, m);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) ro[j] *= m[j];
+    const uint4 pm = pack8(ro);
+    *reinterpret_cast<uint4*>(dxm + row * d + col) = pm;
+    unpack8(pm, ro);
+  }
+  if (dxsum) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) adx[j] += ro[j];
+  }
+}
+
 // Each warp walks rows with a grid stride, keeps per-lane partial dg/db in registers, then one block-level
 // reduction through shared memory and one partial row of dg / db (/ dxsum) per block, summed in block order afterwards.
-template <int NCH>
+template <int NCH, bool DROP>
 __global__ void __launch_bounds__(128)
 layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ g,
                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                      const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ dg,
-                     float* __restrict__ db, float* __restrict__ dxsum, int rows) {
+                     float* __restrict__ db, float* __restrict__ dxsum, int rows, bf16* __restrict__ dxm,
+                     const db200_dropout dr) {
   constexpr int d = NCH * 256;
   __shared__ float red[4][d];  // NCH <= 8 -> <= 32 KiB
   const int lane = threadIdx.x & 31;
@@ -235,7 +312,6 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
       }
     }
     const float c1 = warp_sum(s1) * (1.f / d), c2 = warp_sum(s2) * (1.f / d);
-    bf16* dxr = dx + (long long)row * d;
 #pragma unroll
     for (int c = 0; c < NCH; ++c) {
       const int col = (c * 32 + lane) * 8;
@@ -248,14 +324,7 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] += r[j];
       }
-      const uint4 packed = pack8(o);
-      *reinterpret_cast<uint4*>(dxr + col) = packed;
-      if (dxsum) {  // sum the values exactly as stored (bf16-rounded), like a separate column-sum pass would
-        float ro[8];
-        unpack8(packed, ro);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) adx[c][j] += ro[j];
-      }
+      ln_bwd_store8<DROP>(o, dx, dxm, row, d, col, dxsum != nullptr, dr, adx[c]);
     }
   }
   // block reduction of dg, then db (then dxsum)
@@ -336,12 +405,13 @@ layernorm_fwd_wide_kernel(const bf16* __restrict__ x, const float* __restrict__ 
   }
 }
 
-template <int NCW>
+template <int NCW, bool DROP>
 __global__ void __launch_bounds__(128)
 layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ g,
                           const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                           const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ dg,
-                          float* __restrict__ db, float* __restrict__ dxsum, int rows) {
+                          float* __restrict__ db, float* __restrict__ dxsum, int rows, bf16* __restrict__ dxm,
+                          const db200_dropout dr) {
   constexpr int d = NCW * 1024;
   __shared__ float red[8];
   float gg[NCW][8], adg[NCW][8], adb[NCW][8], adx[NCW][8];
@@ -380,7 +450,6 @@ layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ 
     }
     const float2 ss = block128_sum2(s1, s2, red);
     const float c1 = ss.x * (1.f / d), c2 = ss.y * (1.f / d);
-    bf16* dxr = dx + (long long)row * d;
 #pragma unroll
     for (int c = 0; c < NCW; ++c) {
       const int col = (c * 128 + threadIdx.x) * 8;
@@ -393,14 +462,7 @@ layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ 
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] += r[j];
       }
-      const uint4 packed = pack8(o);
-      *reinterpret_cast<uint4*>(dxr + col) = packed;
-      if (dxsum) {
-        float ro[8];
-        unpack8(packed, ro);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) adx[c][j] += ro[j];
-      }
+      ln_bwd_store8<DROP>(o, dx, dxm, row, d, col, dxsum != nullptr, dr, adx[c]);
     }
   }
 #pragma unroll
@@ -564,13 +626,41 @@ extern "C" int db200_embed_fwd(db200_stream_t stream_, const int32_t* ids, const
   return check_launch("embed_fwd_kernel");
 }
 
+extern "C" int db200_embed_fwd_ex(db200_stream_t stream_, const int32_t* ids, const void* wte, const void* wpe,
+                                  void* out, int B, int S, int d, int V, const db200_dropout* wte_drop,
+                                  const db200_dropout* wpe_drop) {
+  if (!dropout_active(wte_drop) && !dropout_active(wpe_drop))
+    return db200_embed_fwd(stream_, ids, wte, wpe, out, B, S, d, V);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(B > 0 && S > 0 && d > 0 && V > 0 && d % 8 == 0, DB200_E_INVALID,
+                "embed_fwd: need B,S,V > 0 and d %% 8 == 0 (got B=%d S=%d d=%d V=%d)", B, S, d, V);
+  DB200_REQUIRE(ids && aligned16(wte) && aligned16(wpe) && aligned16(out), DB200_E_ALIGN,
+                "embed_fwd: NULL or unaligned pointer");
+  db200_dropout keep_all{};  // threshold 0: every element kept, scale 1
+  keep_all.scale = 1.f;
+  const long long total = (long long)B * S * (d / 8);
+  const int blocks = (int)((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
+  embed_fwd_drop_kernel<<<blocks, 256, 0, stream>>>(ids, (const bf16*)wte, (const bf16*)wpe, (bf16*)out, B * S, S, d,
+                                                    V, dropout_active(wte_drop) ? *wte_drop : keep_all,
+                                                    dropout_active(wpe_drop) ? *wpe_drop : keep_all);
+  return check_launch("embed_fwd_drop_kernel");
+}
+
 extern "C" int64_t db200_embed_bwd_workspace_bytes(int d, int V) {
   return (int64_t)V * d * (int64_t)sizeof(unsigned long long);
 }
 
 extern "C" int db200_embed_bwd(db200_stream_t stream_, const int32_t* ids, const void* dx, float* dwte, float* dwpe,
                                int B, int S, int d, int V, void* workspace, int64_t workspace_bytes) {
+  return db200_embed_bwd_ex(stream_, ids, dx, dwte, dwpe, B, S, d, V, workspace, workspace_bytes, nullptr, nullptr);
+}
+
+extern "C" int db200_embed_bwd_ex(db200_stream_t stream_, const int32_t* ids, const void* dx, float* dwte,
+                                  float* dwpe, int B, int S, int d, int V, void* workspace, int64_t workspace_bytes,
+                                  const db200_dropout* wte_drop, const db200_dropout* wpe_drop) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const db200_dropout* dw = dropout_active(wte_drop) ? wte_drop : nullptr;
+  const db200_dropout* dp = dropout_active(wpe_drop) ? wpe_drop : nullptr;
   DB200_REQUIRE(B > 0 && S > 0 && d > 0 && V > 0 && d % 8 == 0, DB200_E_INVALID,
                 "embed_bwd: need B,S,V > 0 and d %% 8 == 0");
   DB200_REQUIRE(ids && aligned16(dx) && dwte && dwpe, DB200_E_ALIGN, "embed_bwd: NULL or unaligned pointer");
@@ -581,7 +671,8 @@ extern "C" int db200_embed_bwd(db200_stream_t stream_, const int32_t* ids, const
                 "embed_bwd: needs an aligned workspace of db200_embed_bwd_workspace_bytes() bytes");
   auto* acc64 = static_cast<unsigned long long*>(workspace);
   DB200_CUDA(cudaMemsetAsync(acc64, 0, (size_t)n_wte * sizeof(unsigned long long), stream));
-  embed_bwd_wte_kernel<<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V);
+  if (dw) embed_bwd_wte_kernel<true><<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V, *dw);
+  else    embed_bwd_wte_kernel<false><<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V, db200_dropout{});
   int rc = check_launch("embed_bwd_wte_kernel");
   if (rc != DB200_OK) return rc;
   const long long fblocks = (n_wte + 255) / 256 < sm_count() * 16 ? (n_wte + 255) / 256 : sm_count() * 16;
@@ -589,7 +680,8 @@ extern "C" int db200_embed_bwd(db200_stream_t stream_, const int32_t* ids, const
   rc = check_launch("embed_fixed_flush_kernel");
   if (rc != DB200_OK) return rc;
   const int total_pe = S * (d / 8);
-  embed_bwd_wpe_kernel<<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d);
+  if (dp) embed_bwd_wpe_kernel<true><<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d, *dp);
+  else    embed_bwd_wpe_kernel<false><<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d, db200_dropout{});
   return check_launch("embed_bwd_wpe_kernel");
 }
 
@@ -645,11 +737,11 @@ extern "C" int64_t db200_layernorm_bwd_workspace_bytes(int rows, int d) {
   return (int64_t)3 * layernorm_bwd_grid(rows, d) * d * (int64_t)sizeof(float);
 }
 
-extern "C" int db200_layernorm_bwd_ex(db200_stream_t stream_, const void* dy, const void* x, const float* g,
-                                      const float* mean, const float* rstd, const void* dres, void* dx, float* dg,
-                                      float* db, float* dxsum, int rows, int d, void* workspace,
-                                      int64_t workspace_bytes) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+template <bool DROP>
+static int layernorm_bwd_impl(cudaStream_t stream, const void* dy, const void* x, const float* g, const float* mean,
+                              const float* rstd, const void* dres, void* dx, float* dg, float* db, float* dxsum,
+                              int rows, int d, void* workspace, int64_t workspace_bytes, void* dxm,
+                              const db200_dropout& dr) {
   DB200_REQUIRE(rows > 0, DB200_E_INVALID, "layernorm_bwd: rows must be positive");
   DB200_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx) && aligned16(g) && mean && rstd && dg && db &&
                     aligned16(dres),
@@ -658,7 +750,7 @@ extern "C" int db200_layernorm_bwd_ex(db200_stream_t stream_, const void* dy, co
   DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_layernorm_bwd_workspace_bytes(rows, d)),
                 DB200_E_INVALID, "layernorm_bwd: needs an aligned workspace of db200_layernorm_bwd_workspace_bytes() bytes");
   const bf16 *dyp = (const bf16*)dy, *xp = (const bf16*)x, *drp = (const bf16*)dres;
-  bf16* dxp = (bf16*)dx;
+  bf16 *dxp = (bf16*)dx, *dxmp = (bf16*)dxm;
   // per-block partial rows of dg | db | dxsum, reduced in block order below
   float* ws = static_cast<float*>(workspace);
   float* const dg_out = dg;
@@ -668,12 +760,12 @@ extern "C" int db200_layernorm_bwd_ex(db200_stream_t stream_, const void* dy, co
   db = ws + (size_t)grid * d;
   dxsum = dxsum_out ? ws + (size_t)2 * grid * d : nullptr;
   switch (d) {
-    case 256:  layernorm_bwd_kernel<1><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
-    case 512:  layernorm_bwd_kernel<2><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
-    case 768:  layernorm_bwd_kernel<3><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
-    case 1024: layernorm_bwd_kernel<4><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
-    case 2048: layernorm_bwd_kernel<8><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
-    case 4096: layernorm_bwd_wide_kernel<4><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows); break;
+    case 256:  layernorm_bwd_kernel<1, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+    case 512:  layernorm_bwd_kernel<2, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+    case 768:  layernorm_bwd_kernel<3, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+    case 1024: layernorm_bwd_kernel<4, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+    case 2048: layernorm_bwd_kernel<8, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+    case 4096: layernorm_bwd_wide_kernel<4, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
     default:
       return set_error(DB200_E_UNSUPPORTED, "layernorm: d=%d not in {256,512,768,1024,2048,4096}", d);
   }
@@ -682,6 +774,31 @@ extern "C" int db200_layernorm_bwd_ex(db200_stream_t stream_, const void* dy, co
   if (rc == DB200_OK) rc = reduce_rows_add(stream, db, grid, d, db_out);
   if (rc == DB200_OK && dxsum_out) rc = reduce_rows_add(stream, dxsum, grid, d, dxsum_out);
   return rc;
+}
+
+extern "C" int db200_layernorm_bwd_ex(db200_stream_t stream_, const void* dy, const void* x, const float* g,
+                                      const float* mean, const float* rstd, const void* dres, void* dx, float* dg,
+                                      float* db, float* dxsum, int rows, int d, void* workspace,
+                                      int64_t workspace_bytes) {
+  return layernorm_bwd_impl<false>(reinterpret_cast<cudaStream_t>(stream_), dy, x, g, mean, rstd, dres, dx, dg, db,
+                                   dxsum, rows, d, workspace, workspace_bytes, nullptr, db200_dropout{});
+}
+
+extern "C" int db200_layernorm_bwd_dropout(db200_stream_t stream_, const void* dy, const void* x, const float* g,
+                                           const float* mean, const float* rstd, const void* dres, void* dx,
+                                           void* dxm, float* dg, float* db, float* dxsum, int rows, int d,
+                                           const db200_dropout* drop, void* workspace, int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(aligned16(dxm) && dxm, DB200_E_ALIGN, "layernorm_bwd_dropout: NULL or unaligned dxm");
+  if (!dropout_active(drop)) {  // keep everything: dxm = dx
+    const int rc = layernorm_bwd_impl<false>(stream, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, rows, d, workspace,
+                                             workspace_bytes, nullptr, db200_dropout{});
+    if (rc != DB200_OK) return rc;
+    DB200_CUDA(cudaMemcpyAsync(dxm, dx, (size_t)rows * d * sizeof(bf16), cudaMemcpyDeviceToDevice, stream));
+    return DB200_OK;
+  }
+  return layernorm_bwd_impl<true>(stream, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, rows, d, workspace,
+                                  workspace_bytes, dxm, *drop);
 }
 
 extern "C" int db200_layernorm_bwd(db200_stream_t stream_, const void* dy, const void* x, const float* g,

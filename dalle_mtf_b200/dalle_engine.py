@@ -66,8 +66,13 @@ class DalleEngine:
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lnf_g", "lnf_b", "bout")
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
-                 device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None):
-        """zero: a DataParallel with world > 1 turns on optimiser-state sharding (ZeRO-1, SURVEY.md §7 "12 B in pure
+                 device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
+                 dropout_seed=0):
+        """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
+        198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
+        pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
+
+        zero: a DataParallel with world > 1 turns on optimiser-state sharding (ZeRO-1, SURVEY.md §7 "12 B in pure
         DP"): fp32 master / Adam m / Adam v exist only for this rank's 1/N slice of the flat buffer, the bf16 compute
         copy and the fp32 gradients stay full; after the (all-reduced) gradients are final every rank updates its
         slice and the bf16 parameters are all-gathered in place.  Still data parallel: same batch split, same maths."""
@@ -89,6 +94,13 @@ class DalleEngine:
         self.recompute_grad = bool(recompute_grad)
         self.attn_scale = float(attn_scale)
         self.ln_eps = float(ln_eps)
+        self.dropout = tuple(float(r) for r in dropout)
+        if len(self.dropout) != 3:
+            raise ValueError("dropout = (embed, attention, residual) rates")
+        for r in self.dropout:
+            L.dropout_threshold(r)   # rejects a rate outside [0, 1)
+        self.dropout_seed = int(dropout_seed)
+        self._drop = None            # descriptors of the current forward (None: no dropout)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         lay = ParamLayout()
@@ -362,33 +374,67 @@ class DalleEngine:
             "dx_a": e(T, d), "dx_b": e(T, d), "dtmp": e(T, d), "dh1": e(T, 4 * d), "dqkv": e(T, 3 * d),
             "delta": e(B, self.H, S, dtype=F32), "dq_acc": e(1, dtype=F32),
         }
+        if self.dropout[2] > 0:   # gradient of a branch output before its residual dropout
+            b["dxm"] = e(T, d)
         self._bufs, self._buf_key = b, key
         return b
 
+    # ------------------------------------------------------------------------------------------ dropout
+    def _dropout_descs(self, step, row0):
+        """Descriptors of every dropout site for one forward of sequences [row0, row0 + B) of the global batch at
+        optimiser step `step` (None where the rate is 0).  Elementwise sites index global token rows row0 * S + t; the
+        wpe mask is indexed by position only, so every sequence shares it."""
+        emb, att, res = self.dropout
+        if step is None or not (emb or att or res):
+            return None
+        mk = lambda rate, site, r0: L.make_dropout(rate, self.dropout_seed, step, site, r0)
+        rows0 = row0 * self.S
+        return {
+            "wte": mk(emb, L.SITE_WTE, rows0), "wpe": mk(emb, L.SITE_WPE, 0),
+            "attn": [mk(att, L.dropout_site_attn(i), row0) for i in range(self.L)],
+            "attn_out": [mk(res, L.dropout_site_attn_out(i), rows0) for i in range(self.L)],
+            "mlp_out": [mk(res, L.dropout_site_mlp_out(i), rows0) for i in range(self.L)],
+        }
+
+    def _site(self, kind, i):
+        return self._drop[kind][i] if self._drop is not None else None
+
     # ------------------------------------------------------------------------------------------ forward
     def _block_fwd(self, i, x_in, x_out, sv, B):
-        """DALLE.block (src/dalle_mtf/models.py:326-335): x += attn(LN1 x); x += mlp(LN2 x)."""
+        """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x))."""
         p = f"l{i}."
         ops.layernorm_fwd(x_in, self.P(p + "ln1_g"), self.P(p + "ln1_b"), sv["ln1"], sv["mean1"], sv["rstd1"],
                           self.ln_eps)
         ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
-        ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, self.S, self.H, self.dh, self.attn_scale)
-        ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in)  # :303-311,330
+        ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, self.S, self.H, self.dh, self.attn_scale,
+                     dropout=self._site("attn", i))                                     # :290-299
+        ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in,
+                       dropout=self._site("attn_out", i))                               # :303-314,330
         ops.layernorm_fwd(sv["xmid"], self.P(p + "ln2_g"), self.P(p + "ln2_b"), sv["ln2"], sv["mean2"], sv["rstd2"],
                           self.ln_eps)
         ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), relu=True)     # :320
-        ops.linear_fwd(sv["h1"], self.W(p + "w2"), x_out, bias=self.P(p + "b2"), residual=sv["xmid"])  # :321,333
+        ops.linear_fwd(sv["h1"], self.W(p + "w2"), x_out, bias=self.P(p + "b2"), residual=sv["xmid"],
+                       dropout=self._site("mlp_out", i))                                # :321-323,333
 
-    def forward(self, tokens, loss_accum=None):
+    def forward(self, tokens, loss_accum=None, step=None, row0=0):
         """tokens int32 [B,S] on the device.  Adds sum_t loss_rows[t] of this batch into the 1-element fp32 tensor
         `loss_accum` (default: the aux slot behind the gradients, which rides along with the gradient all-reduce)
-        and returns it.  The mean over all positions (src/dalle_mtf/models.py:353-354) is that sum / (global B*S)."""
+        and returns it.  The mean over all positions (src/dalle_mtf/models.py:353-354) is that sum / (global B*S).
+
+        step: the global optimiser step of a training forward; with a step the dropout rates apply (mode "train"),
+        without one they do not.  row0: global index of tokens[0] in the step's batch (rank and micro-batch offset),
+        so that the masks do not depend on how the batch is split."""
         B, S = tokens.shape
         assert S == self.S, f"expected sequence length {self.S}, got {S}"
         bufs = self._alloc(B)
         T = B * S
         self._tokens = tokens
-        ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), bufs["xs"][0].view(B, S, self.d))    # models.py:399
+        self._drop = self._dropout_descs(step, row0)
+        if self._drop is not None:
+            ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), bufs["xs"][0].view(B, S, self.d),
+                          wte_drop=self._drop["wte"], wpe_drop=self._drop["wpe"])            # models.py:198-217
+        else:
+            ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), bufs["xs"][0].view(B, S, self.d))  # models.py:399
         for i in range(self.L):
             sv = bufs["layers"][0 if self.recompute_grad else i]
             self._block_fwd(i, bufs["xs"][i], bufs["xs"][i + 1], sv, B)
@@ -417,29 +463,44 @@ class DalleEngine:
         return out.view(B, S, self.Vpad)[:, :, :self.V]
 
     # ------------------------------------------------------------------------------------------ backward
-    def _block_bwd(self, i, x_in, sv, dx_out, dx_in, bufs, B, dxsum_below):
+    def _ln_bwd(self, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, site):
+        """LayerNorm backward; when `site` (the residual-dropout site of the branch whose output x sums) is active it
+        also writes bufs["dxm"] = dx * keep * scale, and dxsum is colsum(dxm).  Returns the gradient of that branch
+        output (dxm, or dx without dropout)."""
+        if site is None:
+            ops.layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=dxsum)
+            return dx
+        dxm = self._bufs["dxm"]
+        ops.layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=dxsum, dxm=dxm, dropout=site)
+        return dxm
+
+    def _block_bwd(self, i, x_in, sv, dx_out, dx_in, bufs, B, dxsum_below, dbranch):
         """Backward of one block.  Bias gradients are column sums of activation gradients; they are produced by the
         kernel that WRITES that gradient (LayerNorm-backward / ReLU-mask epilogue) instead of separate passes:
-        db2 (= colsum of this block's output gradient) was already accumulated by whoever produced dx_out."""
+        db2 (= colsum of this block's output gradient) was already accumulated by whoever produced dx_out.
+        dbranch: gradient of the MLP output before its residual dropout (dx_out itself without dropout).  Returns the
+        same for the layer below."""
         p = f"l{i}."
         # ---- MLP
-        ops.linear_dgrad(dx_out, self.W(p + "w2"), bufs["dh1"], relu_mask_of=sv["h1"],
+        ops.linear_dgrad(dbranch, self.W(p + "w2"), bufs["dh1"], relu_mask_of=sv["h1"],
                          colsum=self.G(p + "b1"))                                       # dH = (dx W2^T)*[h1>0]; db1
-        ops.linear_wgrad(sv["h1"], dx_out, self.G(p + "w2"))
+        ops.linear_wgrad(sv["h1"], dbranch, self.G(p + "w2"))
         ops.linear_dgrad(bufs["dh1"], self.W(p + "w1"), bufs["dtmp"])                         # dLN2 out
         ops.linear_wgrad(sv["ln2"], bufs["dh1"], self.G(p + "w1"))
         dx_mid = bufs["dx_b"] if dx_out is bufs["dx_a"] else bufs["dx_a"]
-        ops.layernorm_bwd(bufs["dtmp"], sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
-                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), dxsum=self.G(p + "o_b"))  # do_b = colsum(dx_mid)
+        da = self._ln_bwd(bufs["dtmp"], sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
+                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), self.G(p + "o_b"),
+                          self._site("attn_out", i))                                    # do_b = colsum(da)
         # ---- attention
-        ops.linear_dgrad(dx_mid, self.W(p + "wo"), bufs["dtmp"])                              # d(attn out)
-        ops.linear_wgrad(sv["attn"], dx_mid, self.G(p + "wo"))
+        ops.linear_dgrad(da, self.W(p + "wo"), bufs["dtmp"])                                  # d(attn out)
+        ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
         ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"], B,
-                     self.S, self.H, self.dh, self.attn_scale)
+                     self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i))
         ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                      # dLN1 out
         ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
-        ops.layernorm_bwd(bufs["dtmp"], x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
-                          self.G(p + "ln1_g"), self.G(p + "ln1_b"), dxsum=dxsum_below)        # db2 of the layer below
+        return self._ln_bwd(bufs["dtmp"], x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
+                            self.G(p + "ln1_g"), self.G(p + "ln1_b"), dxsum_below,
+                            self._site("mlp_out", i - 1) if i > 0 else None)          # db2 of the layer below
 
     def backward(self, grad_scale, on_bucket_ready=None):
         """Back-propagates d(sum(loss_rows) * grad_scale).  Gradients ACCUMULATE into self.grads.
@@ -455,8 +516,9 @@ class DalleEngine:
         ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
         ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
         dx = bufs["dx_a"]
-        ops.layernorm_bwd(bufs["dtmp"], bufs["xs"][self.L], self.P("lnf_g"), bufs["meanf"], bufs["rstdf"], None, dx,
-                          self.G("lnf_g"), self.G("lnf_b"), dxsum=self.G(f"l{self.L - 1}.b2"))   # db2 of the last block
+        dbranch = self._ln_bwd(bufs["dtmp"], bufs["xs"][self.L], self.P("lnf_g"), bufs["meanf"], bufs["rstdf"], None,
+                               dx, self.G("lnf_g"), self.G("lnf_b"), self.G(f"l{self.L - 1}.b2"),
+                               self._site("mlp_out", self.L - 1))                          # db2 of the last block
         if on_bucket_ready:
             s, e = self.layout.span("lnf_g", "bout")
             on_bucket_ready(s, e + 64)  # + the aux scalars (loss) that sit behind the last parameter
@@ -468,11 +530,16 @@ class DalleEngine:
                 sv = bufs["layers"][i]
             # dx (grad w.r.t. the block output) is dead once dx_mid has been formed in the other buffer, so the
             # block's input gradient is written back into the same storage.
-            self._block_bwd(i, bufs["xs"][i], sv, dx, dx, bufs, B, self.G(f"l{i - 1}.b2") if i > 0 else None)
+            dbranch = self._block_bwd(i, bufs["xs"][i], sv, dx, dx, bufs, B,
+                                      self.G(f"l{i - 1}.b2") if i > 0 else None, dbranch)
             if on_bucket_ready:
                 s, e = self.layout.span(f"l{i}.ln1_g", f"l{i}.b2")
                 on_bucket_ready(s, e)
-        ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), self.G("wpe"))
+        if self._drop is not None:
+            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), self.G("wpe"), wte_drop=self._drop["wte"],
+                          wpe_drop=self._drop["wpe"])
+        else:
+            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), self.G("wpe"))
         if on_bucket_ready:
             s, e = self.layout.span("wte", "wpe")
             on_bucket_ready(s, e)

@@ -35,6 +35,47 @@ class GemmEpilogue(ctypes.Structure):
     ]
 
 
+class Dropout(ctypes.Structure):
+    """Mirror of ``struct db200_dropout`` (one dropout site of one step; see include/dalle_b200.h, D0)."""
+    _fields_ = [("seed", c_u64), ("step", ctypes.c_uint32), ("site", ctypes.c_uint32), ("threshold", ctypes.c_uint32),
+                ("scale", c_f32), ("row0", c_i64)]
+
+
+DROPOUT_ELEMENTWISE, DROPOUT_ATTENTION = 0, 1
+SITE_WTE, SITE_WPE = 0, 1
+
+
+def dropout_site_attn(layer):
+    return 2 + 3 * layer
+
+
+def dropout_site_attn_out(layer):
+    return 3 + 3 * layer
+
+
+def dropout_site_mlp_out(layer):
+    return 4 + 3 * layer
+
+
+def dropout_threshold(rate):
+    """Keep iff word >= floor(rate * 2^32) (computed in double); kept values are scaled by float(1 / (1 - rate))."""
+    rate = float(rate)
+    if not 0.0 <= rate < 1.0:
+        raise ValueError(f"dropout rate {rate} outside [0, 1)")
+    return int(rate * 4294967296.0), float(1.0 / (1.0 - rate))
+
+
+def make_dropout(rate, seed, step, site, row0):
+    """db200_dropout for one site, or None when rate == 0 (the kernels without dropout run)."""
+    thr, scale = dropout_threshold(rate)
+    if thr == 0:
+        return None
+    d = Dropout()
+    d.seed, d.step, d.site, d.threshold, d.scale, d.row0 = int(seed) & (2 ** 64 - 1), int(step), int(site), thr, \
+        scale, int(row0)
+    return d
+
+
 class ConvDesc(ctypes.Structure):
     """Mirror of ``struct db200_conv_desc``."""
     _fields_ = [(n, ctypes.c_int32) for n in
@@ -48,14 +89,23 @@ _SIGNATURES = {
     "db200_device_check": [],
     "db200_embed_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_embed_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64],
+    "db200_embed_fwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, ctypes.POINTER(Dropout),
+                           ctypes.POINTER(Dropout)],
+    "db200_embed_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64,
+                           ctypes.POINTER(Dropout), ctypes.POINTER(Dropout)],
+    "db200_dropout_mask": [c_vp, ctypes.POINTER(Dropout), c_int, c_i64, c_i64, c_i64, c_vp],
     "db200_assemble_tokens": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_shift_labels": [c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_layernorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
     "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
     "db200_layernorm_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp,
                                c_i64],
+    "db200_layernorm_bwd_dropout": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
+                                    c_int, ctypes.POINTER(Dropout), c_vp, c_i64],
     "db200_gemm_bf16": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
                         ctypes.POINTER(GemmEpilogue)],
+    "db200_gemm_bf16_ex": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
+                           ctypes.POINTER(GemmEpilogue), ctypes.POINTER(Dropout)],
     "db200_gemm_ce_tiles": [c_int],
     "db200_embed_fwd_at": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_attn_decode": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_f32],
@@ -73,6 +123,9 @@ _SIGNATURES = {
     "db200_ce_finish": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
     "db200_attn_causal_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_causal_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
+    "db200_attn_causal_fwd_ex": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32, ctypes.POINTER(Dropout)],
+    "db200_attn_causal_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32,
+                                 ctypes.POINTER(Dropout)],
     "db200_colsum_bf16": [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_i64],
     "db200_cast_f32_to_bf16": [c_vp, c_vp, c_vp, c_sz],
     "db200_cast_bf16_to_f32": [c_vp, c_vp, c_vp, c_sz],

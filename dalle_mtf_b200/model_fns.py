@@ -73,6 +73,22 @@ def load_vae_model(params, device):
     return vae, ckpt
 
 
+DROPOUT_KEYS = ("embed_dropout", "attention_dropout", "residual_dropout")
+
+
+def dropout_rates(params):
+    """(embed, attention, residual) dropout rates of a DALL-E config (src/dalle_mtf/models.py:198, 215, 290, 312, 318);
+    a missing or null key is 0.  A rate outside [0, 1) is rejected."""
+    rates = []
+    for k in DROPOUT_KEYS:
+        v = params.get(k)
+        r = 0.0 if v is None else float(v)
+        if not 0.0 <= r < 1.0:
+            raise ValueError(f"{k} = {v!r}: a dropout rate must lie in [0, 1)")
+        rates.append(r)
+    return tuple(rates)
+
+
 def dalle_model_fn(features, labels, mode, params):
     """src/model_fns.py:55-236.  features: images f32 [B,H,W,C] in [-1,1] (NHWC); labels: caption ids i32
     [B, text_seq_len].  (The reference's own comment has them swapped; the code uses them this way.)"""
@@ -98,7 +114,8 @@ def dalle_model_fn(features, labels, mode, params):
         raise AssertionError("pretrained vae needed for training")              # model_fns.py:41
     image_seq_len = vae.image_seq_len                                           # model_fns.py:68
     global_batch = params[f"{mode_str}_batch_size"]                             # model_fns.py:69
-    _, local_batch = dp.shard(global_batch)
+    first_row, local_batch = dp.shard(global_batch)
+    rates = dropout_rates(params)
 
     model = DalleEngine(n_embd=params["n_embd"], n_layers=params["n_layers"], n_heads=params["n_heads"],
                         text_vocab_size=params["text_vocab_size"], image_vocab_size=params["image_vocab_size"],
@@ -106,7 +123,8 @@ def dalle_model_fn(features, labels, mode, params):
                         recompute_grad=bool(params.get("recompute_grad")) and mode == TRAIN,   # models.py:342
                         # extension key: shard fp32 master + Adam slots across the data-parallel ranks (ZeRO-1) —
                         # what lets the d = 4096 configuration fit 80 GB GPUs in pure data parallelism
-                        zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None)
+                        zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None,
+                        dropout=rates, dropout_seed=params.get("seed") or 0)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")
@@ -151,7 +169,9 @@ def dalle_model_fn(features, labels, mode, params):
         mb = local_batch // num_microbatches
         hook = dp.make_bucket_hook(model.grads)
         for i in range(num_microbatches):
-            model.forward(toks[i * mb:(i + 1) * mb])
+            # dropout masks of the global step, indexed by the global sequence index of each row: the same masks
+            # whatever the rank count or micro-batch size (models.py:198-323 apply them in mode "train" only)
+            model.forward(toks[i * mb:(i + 1) * mb], step=spec.global_step, row0=first_row + i * mb)
             last = i == num_microbatches - 1
             if last:
                 dp.begin_overlap()

@@ -6,6 +6,7 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
+from .model_fns import dropout_rates
 from .vae_engine import VaeEngine
 
 
@@ -27,11 +28,10 @@ class DALLE:
         self.total_tokens = text_vocab_size + image_vocab_size + 1
         self.eos_token_id = self.total_tokens - 1 if eos_token_id is None else eos_token_id
         self.batch_size, self.bf_16, self.mode = batch_size, bf_16, mode
-        for k in ("embed_dropout", "attention_dropout", "residual_dropout"):
-            if params.get(k):
-                raise L.DB200Error(f"{k} > 0 is not implemented (every reference config leaves it at 0)")
         self.engine = DalleEngine(n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len,
-                                  image_seq_len, recompute_grad=bool(params.get("recompute_grad")) and mode == "train")
+                                  image_seq_len, recompute_grad=bool(params.get("recompute_grad")) and mode == "train",
+                                  dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0)
+        self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id
         self.engine.init_params(seed=params.get("seed") or 0)
 
@@ -44,7 +44,10 @@ class DALLE:
         if not return_loss:
             return self.engine.logits(tokens)
         acc = torch.zeros(1, dtype=torch.float32, device=self.engine.device)
-        self.engine.forward(tokens, loss_accum=acc)
+        step = None
+        if self.mode == "train":   # dropout only in train mode (models.py:198, 215, 290, 312, 318)
+            step, self._step = self._step, self._step + 1
+        self.engine.forward(tokens, loss_accum=acc, step=step)
         loss = acc / float(B * S)   # reduce_mean over every position (models.py:353-354); scalar glue only
         loss_batch = self.engine._bufs["loss_rows"].view(B, S)
         if return_logits:

@@ -10,6 +10,11 @@ import torch
 from . import lib as L
 from .lib import GemmEpilogue, ConvDesc, check, ptr, stream_ptr
 
+
+def _ref(d):
+    """ctypes argument of an optional db200_dropout (None -> NULL)."""
+    return ctypes.byref(d) if d is not None else None
+
 BF16 = torch.bfloat16
 F32 = torch.float32
 I32 = torch.int32
@@ -38,10 +43,11 @@ def _nbytes(ws):
 
 def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=None, mode=L.EPI_STORE,
          alpha=1.0, bias=None, relu=False, residual=None, aux=None, split_k=1, labels=None, part_max=None,
-         part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None):
+         part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None, dropout=None):
     """D[M,N] = A[M,K] @ B[K,N] on wgmma.  a_mn / b_mn: operand is stored with M (resp. N) contiguous.
 
     a: [M,K] (k-major) or [K,M] (mn-major);  b: [N,K] (k-major) or [K,N] (mn-major).
+    dropout (lib.Dropout, STORE only): D = residual + keep * scale * act(alpha * acc + bias).
     """
     L.require_device()
     _chk(a, BF16, "gemm A")
@@ -80,19 +86,23 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-    check(L.load().db200_gemm_bf16(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out), ldd,
-                                   M, N, K, ctypes.byref(e)), "db200_gemm_bf16")
+    if dropout is None:
+        check(L.load().db200_gemm_bf16(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out), ldd,
+                                       M, N, K, ctypes.byref(e)), "db200_gemm_bf16")
+    else:
+        check(L.load().db200_gemm_bf16_ex(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out),
+                                          ldd, M, N, K, ctypes.byref(e), ctypes.byref(dropout)), "db200_gemm_bf16_ex")
     if prof is not None:
         ev1.record()
         prof.append((ev0, ev1, 2.0 * M * N * K, (M, N, K, mode, int(a_mn), int(b_mn))))
     return out
 
 
-def linear_fwd(x, w, out, bias=None, relu=False, residual=None):
-    """out[T,N] = act(x[T,K] @ w[K,N] + bias) + residual      (forward: A k-major, B mn-major)."""
+def linear_fwd(x, w, out, bias=None, relu=False, residual=None, dropout=None):
+    """out[T,N] = dropout(act(x[T,K] @ w[K,N] + bias)) + residual      (forward: A k-major, B mn-major)."""
     T, K = x.shape
     N = w.shape[1]
-    return gemm(x, w, out, T, N, K, a_mn=False, b_mn=True, bias=bias, relu=relu, residual=residual)
+    return gemm(x, w, out, T, N, K, a_mn=False, b_mn=True, bias=bias, relu=relu, residual=residual, dropout=dropout)
 
 
 def linear_dgrad(dy, w, out, relu_mask_of=None, colsum=None):
@@ -125,23 +135,33 @@ def ce_finish(part_max, part_sum, label_logit, lse, loss_rows, loss_sum):
 
 
 # ----------------------------------------------------------------------------------------------- row ops
-def embed_fwd(ids, wte, wpe, out):
+def embed_fwd(ids, wte, wpe, out, wte_drop=None, wpe_drop=None):
+    """out = wte[ids] + wpe[s]; with embedding dropout (lib.Dropout descriptors of the wte / wpe sites) each term is
+    multiplied by its keep mask * scale."""
     L.require_device()
     _chk(ids, I32, "ids"); _chk(wte, BF16, "wte"); _chk(wpe, BF16, "wpe"); _chk(out, BF16, "out")
     B, S = ids.shape
     V, d = wte.shape
-    check(L.load().db200_embed_fwd(stream_ptr(), ptr(ids), ptr(wte), ptr(wpe), ptr(out), B, S, d, V), "embed_fwd")
+    if wte_drop is None and wpe_drop is None:
+        check(L.load().db200_embed_fwd(stream_ptr(), ptr(ids), ptr(wte), ptr(wpe), ptr(out), B, S, d, V), "embed_fwd")
+    else:
+        check(L.load().db200_embed_fwd_ex(stream_ptr(), ptr(ids), ptr(wte), ptr(wpe), ptr(out), B, S, d, V,
+                                          _ref(wte_drop), _ref(wpe_drop)), "embed_fwd_ex")
     return out
 
 
-def embed_bwd(ids, dx, dwte, dwpe):
+def embed_bwd(ids, dx, dwte, dwpe, wte_drop=None, wpe_drop=None):
     L.require_device()
     _chk(ids, I32, "ids"); _chk(dx, BF16, "dx"); _chk(dwte, F32, "dwte"); _chk(dwpe, F32, "dwpe")
     B, S = ids.shape
     V, d = dwte.shape
     ws = L.workspace(L.load().db200_embed_bwd_workspace_bytes(d, V))
-    check(L.load().db200_embed_bwd(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V, ptr(ws),
-                                   _nbytes(ws)), "embed_bwd")
+    if wte_drop is None and wpe_drop is None:
+        check(L.load().db200_embed_bwd(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V, ptr(ws),
+                                       _nbytes(ws)), "embed_bwd")
+    else:
+        check(L.load().db200_embed_bwd_ex(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V, ptr(ws),
+                                          _nbytes(ws), _ref(wte_drop), _ref(wpe_drop)), "embed_bwd_ex")
 
 
 def assemble_tokens(text_ids, image_idx, tokens, image_offset):
@@ -172,17 +192,35 @@ def layernorm_fwd(x, g, b, y, mean, rstd, eps=1e-5):
     return y
 
 
-def layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=None):
-    """dxsum (optional, f32 [d]): += column sums of the produced dx (fused bias gradient of the layer below)."""
+def layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=None, dxm=None, dropout=None):
+    """dxsum (optional, f32 [d]): += column sums of the produced dx (fused bias gradient of the layer below).
+    dxm (with `dropout`, the residual-dropout site of the branch below): also writes dxm = dx * keep * scale, and dxsum
+    then sums dxm."""
     L.require_device()
     _chk(dy, BF16, "dy"); _chk(x, BF16, "x"); _chk(dres, BF16, "dres"); _chk(dx, BF16, "dx")
-    _chk(g, F32, "g"); _chk(dg, F32, "dg"); _chk(db, F32, "db"); _chk(dxsum, F32, "dxsum")
+    _chk(g, F32, "g"); _chk(dg, F32, "dg"); _chk(db, F32, "db"); _chk(dxsum, F32, "dxsum"); _chk(dxm, BF16, "dxm")
     rows, d = x.shape
     ws = L.workspace(L.load().db200_layernorm_bwd_workspace_bytes(rows, d))
-    check(L.load().db200_layernorm_bwd_ex(stream_ptr(), ptr(dy), ptr(x), ptr(g), ptr(mean), ptr(rstd), ptr(dres),
-                                          ptr(dx), ptr(dg), ptr(db), ptr(dxsum), rows, d, ptr(ws), _nbytes(ws)),
-          "layernorm_bwd")
+    if dxm is None:
+        check(L.load().db200_layernorm_bwd_ex(stream_ptr(), ptr(dy), ptr(x), ptr(g), ptr(mean), ptr(rstd), ptr(dres),
+                                              ptr(dx), ptr(dg), ptr(db), ptr(dxsum), rows, d, ptr(ws), _nbytes(ws)),
+              "layernorm_bwd")
+    else:
+        check(L.load().db200_layernorm_bwd_dropout(stream_ptr(), ptr(dy), ptr(x), ptr(g), ptr(mean), ptr(rstd),
+                                                   ptr(dres), ptr(dx), ptr(dxm), ptr(dg), ptr(db), ptr(dxsum), rows, d,
+                                                   _ref(dropout), ptr(ws), _nbytes(ws)), "layernorm_bwd_dropout")
     return dx
+
+
+def dropout_mask(desc, layout, dims, keep):
+    """keep (uint8, contiguous): 1 where the site `desc` keeps the element.  layout lib.DROPOUT_ELEMENTWISE with
+    dims (rows, cols) -> [rows, cols]; lib.DROPOUT_ATTENTION with dims (B, H, S) -> [B, H, S, S]."""
+    L.require_device()
+    _chk(keep, torch.uint8, "keep")
+    dims = tuple(int(x) for x in dims) + (0,) * (3 - len(dims))
+    check(L.load().db200_dropout_mask(stream_ptr(), ctypes.byref(desc), int(layout), dims[0], dims[1], dims[2],
+                                      ptr(keep)), "dropout_mask")
+    return keep
 
 
 def colsum(x, out_accum, rows=None, cols=None):
@@ -234,22 +272,33 @@ def _attn_timed(kind, B, S, H, dh, call):
     prof.append((ev0, ev1, 2.0 * S * S * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
 
 
-def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0):
+def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None):
+    """dropout: lib.Dropout of the attention-weights site (row0 = global index of sequence 0), or None."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(lse, F32, "lse")
-    _attn_timed("fwd", B, S, H, dh, lambda: check(
-        L.load().db200_attn_causal_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh, scale),
-        "attn_causal_fwd"))
+    if dropout is None:
+        call = lambda: check(L.load().db200_attn_causal_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
+                                                            scale), "attn_causal_fwd")
+    else:
+        call = lambda: check(L.load().db200_attn_causal_fwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
+                                                               scale, ctypes.byref(dropout)), "attn_causal_fwd_ex")
+    _attn_timed("fwd", B, S, H, dh, call)
     return out
 
 
-def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0):
+def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None):
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(dout, BF16, "dout"); _chk(dqkv, BF16, "dqkv")
     _chk(lse, F32, "lse"); _chk(dq_accum, F32, "dq_accum"); _chk(delta, F32, "delta")
-    _attn_timed("bwd", B, S, H, dh, lambda: check(
-        L.load().db200_attn_causal_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dq_accum),
-                                       ptr(delta), ptr(dqkv), B, S, H, dh, scale), "attn_causal_bwd"))
+    if dropout is None:
+        call = lambda: check(L.load().db200_attn_causal_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
+                                                            ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, scale),
+                             "attn_causal_bwd")
+    else:
+        call = lambda: check(L.load().db200_attn_causal_bwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
+                                                               ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh,
+                                                               scale, ctypes.byref(dropout)), "attn_causal_bwd_ex")
+    _attn_timed("bwd", B, S, H, dh, call)
     return dqkv
 
 

@@ -44,6 +44,34 @@ unsigned long long db200_launch_count(void);
 int db200_device_check(void);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * D0  dropout masks.  Replaces mtf.dropout at src/dalle_mtf/models.py:198-200, 215-217, 312-314, 321-323 and the
+ *     dropout_rate of mtf_transformer.attention.attention at :290-299.  No mask is ever stored: the kernels that
+ *     apply a mask regenerate it from a counter-based generator (Philox4x32-10), so a keep decision is a pure function
+ *     of (seed, step, site, global element index):
+ *       key = (lo32(seed), hi32(seed)),  counter = (lo32(n), hi32(n), site, step),  the element reads word w
+ *       elementwise [rows][cols], row 0 = global row row0:  e = (row0 + r) * cols + c,  n = e >> 2,  w = e & 3
+ *       attention weights (b, h, i, j), b = row0 + local sequence index, S2 = ceil(S / 2):
+ *                                 n = ((b * H + h) * S2 + i / 2) * S2 + j / 2,  w = 2 * (i & 1) + (j & 1)
+ *       keep iff word >= threshold (= floor(rate * 2^32)); kept values are multiplied by scale (= 1 / (1 - rate)).
+ *     Every entry point that takes a `const db200_dropout*` treats NULL, or threshold 0, as "no dropout" and then runs
+ *     exactly the kernels of the entry point without dropout.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct db200_dropout {
+  uint64_t seed;
+  uint32_t step;      /* global optimiser step */
+  uint32_t site;      /* wte 0, wpe 1; layer l: attention weights 2+3l, attention output 3+3l, MLP output 4+3l */
+  uint32_t threshold; /* floor(rate * 2^32) */
+  float scale;        /* 1 / (1 - rate) */
+  int64_t row0;       /* elementwise: global row of row 0; attention: global sequence index of sequence 0 */
+} db200_dropout;
+
+#define DB200_DROPOUT_ELEMENTWISE 0 /* dims: rows, cols (cols % 4 == 0)     keep: uint8 [rows][cols]   */
+#define DB200_DROPOUT_ATTENTION 1   /* dims: B, H, S                         keep: uint8 [B][H][S][S]   */
+/* keep[...] = 1 where the element is kept, 0 where it is dropped (tests and oracle comparisons). */
+int db200_dropout_mask(db200_stream_t stream, const db200_dropout* d, int layout, int64_t dim0, int64_t dim1,
+                       int64_t dim2, uint8_t* keep);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * K1  token + position embedding.   Replaces mtf.gather(wte, ids) + mtf.gather(wpe, range) + add
  *     src/dalle_mtf/models.py:186-219.   out[b,s,:] = wte[ids[b,s],:] + wpe[s,:]
  *     bwd: dwte[ids[b,s],:] += dx[b,s,:]   (order-independent: 64-bit fixed point),  dwpe[s,:] += sum_b dx[b,s,:]
@@ -55,6 +83,15 @@ int db200_embed_fwd(db200_stream_t stream, const int32_t* ids, const void* wte_b
 int db200_embed_bwd(db200_stream_t stream, const int32_t* ids, const void* dx_bf16, float* dwte, float* dwpe, int B,
                     int S, int d, int V, void* workspace, int64_t workspace_bytes);
 int64_t db200_embed_bwd_workspace_bytes(int d, int V);
+/* with embedding dropout: out = drop_wte(wte[ids]) + drop_wpe(wpe[s]).  The wte mask is elementwise over the [B*S][d]
+ * rows (wte->row0 = global row of ids[0][0]); the wpe mask is elementwise over [S][d] (wpe->row0 = 0), one mask shared
+ * by every sequence.  bwd: dwte[ids] += dx * keep_wte * scale,  dwpe[s] += keep_wpe[s] * scale * sum_b dx[b,s]. */
+int db200_embed_fwd_ex(db200_stream_t stream, const int32_t* ids, const void* wte_bf16, const void* wpe_bf16,
+                       void* out_bf16, int B, int S, int d, int V, const db200_dropout* wte_drop,
+                       const db200_dropout* wpe_drop);
+int db200_embed_bwd_ex(db200_stream_t stream, const int32_t* ids, const void* dx_bf16, float* dwte, float* dwpe, int B,
+                       int S, int d, int V, void* workspace, int64_t workspace_bytes, const db200_dropout* wte_drop,
+                       const db200_dropout* wpe_drop);
 
 /* T0 token assembly: tokens[b] = concat(text_ids[b], image_idx[b] + image_offset).  Replaces tf.concat at
  * src/model_fns.py:117-122 (image_offset = text_vocab_size). */
@@ -82,6 +119,12 @@ int db200_layernorm_bwd_ex(db200_stream_t stream, const void* dy_bf16, const voi
                            float* dg, float* db, float* dxsum_or_null, int rows, int d, void* workspace,
                            int64_t workspace_bytes);
 int64_t db200_layernorm_bwd_workspace_bytes(int rows, int d);
+/* backward of LayerNorm whose input x = r + dropout(branch): also writes dxm = dx * keep * scale (the gradient of the
+ * branch output before its residual dropout, elementwise mask of `drop` over [rows][d]) and dxsum[c] += sum_rows dxm */
+int db200_layernorm_bwd_dropout(db200_stream_t stream, const void* dy_bf16, const void* x_bf16, const float* g,
+                                const float* mean, const float* rstd, const void* dres_bf16_or_null, void* dx_bf16,
+                                void* dxm_bf16, float* dg, float* db, float* dxsum_or_null, int rows, int d,
+                                const db200_dropout* drop, void* workspace, int64_t workspace_bytes);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * K3/K5/K6/K8  bf16 GEMM on wgmma (TMA-fed, register accumulators, fp32 accumulate):   D[M,N] = A[M,K] * B[K,N]
@@ -124,6 +167,11 @@ typedef struct db200_gemm_epilogue {
 
 int db200_gemm_bf16(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
                     int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi);
+/* residual dropout in the STORE epilogue: D = residual + keep * scale * act(alpha*acc + bias), mask elementwise over
+ * [M][N] (needs N % 8 == 0).  Other epilogues take no dropout. */
+int db200_gemm_bf16_ex(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
+                       int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi,
+                       const db200_dropout* dropout);
 /* number of N tiles the CE_STATS epilogue writes per row for a given N (host helper for sizing part_max/part_sum) */
 int db200_gemm_ce_tiles(int N);
 /* epi->workspace size for this product: split-K slices (ATOMIC) or fused column sums (CE_GRAD / RELU_BWD with colsum) */
@@ -150,6 +198,13 @@ int db200_attn_causal_fwd(db200_stream_t stream, const void* qkv_bf16, void* out
 int db200_attn_causal_bwd(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
                           const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H,
                           int dh, float scale);
+/* attention dropout on the normalised weights before the PV product (attention layout of `drop`; drop->row0 = global
+ * index of sequence 0).  lse is that of the undropped weights; out is the dropped output, which backward reads. */
+int db200_attn_causal_fwd_ex(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, float* lse, int B, int S,
+                             int H, int dh, float scale, const db200_dropout* drop);
+int db200_attn_causal_bwd_ex(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
+                             const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H,
+                             int dh, float scale, const db200_dropout* drop);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * small HBM-bound helpers

@@ -31,17 +31,16 @@ gumbel_softmax_fwd_kernel(const float* __restrict__ logits, const float* __restr
   const float* lr = logits + (long long)row * K;
   const float* ur = u ? u + (long long)row * K : nullptr;
   float* ys = y_soft + (long long)row * K;
-  // pass 1: z = (logit + g) / tau into y_soft, track max / argmax
+  // pass 1: z = (logit + g) / tau into y_soft, track max
   float mv = -INFINITY;
-  int mi = 0x7fffffff;
   for (int k = lane; k < K; k += 32) {
     float z = lr[k];
     if (ur) z += -logf(-logf(ur[k]));  // g = -log(-log(u)), src/vae_tf/layers.py:8-14
     z *= inv_tau;
     ys[k] = z;
-    argmax_combine(mv, mi, z, k);
+    mv = fmaxf(mv, z);
   }
-  warp_argmax(mv, mi);
+  mv = warp_max(mv);
   float s = 0.f;
   for (int k = lane; k < K; k += 32) {
     const float e = expf(ys[k] - mv);
@@ -51,10 +50,22 @@ gumbel_softmax_fwd_kernel(const float* __restrict__ logits, const float* __restr
   s = warp_sum(s);
   const float inv = 1.f / s;
   float* yo = y_out ? y_out + (long long)row * K : nullptr;
+  // pass 3: y = e / s, and the first maximum of y itself (tf.argmax(y), layers.py:17): z's that differ by an ulp can
+  // round to the same y, and then the lower index wins, so idx is not the argmax of z.  The search starts at index 0:
+  // a row with a NaN or +inf logit has y = NaN everywhere, which no comparison accepts, and it then gets idx 0 (and
+  // the hard one-hot stores stay inside the row) instead of an index past the end.
+  float my = -INFINITY;
+  int mi = 0;
   for (int k = lane; k < K; k += 32) {
     const float yk = ys[k] * inv;
     ys[k] = yk;
-    if (yo) yo[k] = hard ? (k == mi ? 1.f : 0.f) : yk;  // hard: one_hot(argmax y) forward value (layers.py:17-19)
+    if (yo) yo[k] = hard ? 0.f : yk;
+    argmax_combine(my, mi, yk, k);
+  }
+  warp_argmax(my, mi);
+  if (hard && yo) {
+    __syncwarp();  // orders this lane's 1 after the zero another lane of the warp stored there
+    if (lane == 0) yo[mi] = 1.f;  // hard: one_hot(argmax y) forward value (layers.py:17-19)
   }
   if (idx_out && lane == 0) idx_out[row] = mi;
 }
@@ -81,7 +92,7 @@ argmax_rows_kernel(const float* __restrict__ x, int* __restrict__ idx, int rows,
   if (row >= rows) return;
   const float* xr = x + (long long)row * K;
   float mv = -INFINITY;
-  int mi = 0x7fffffff;
+  int mi = 0;  // an all-NaN row yields 0, never an out-of-range token id
   for (int k = lane; k < K; k += 32) argmax_combine(mv, mi, xr[k], k);
   warp_argmax(mv, mi);
   if (lane == 0) idx[row] = mi;

@@ -93,7 +93,7 @@ class VaeEngine:
         # bf16 copy of the kernels for the tensor-core convolutions (use_bf16 only)
         self.shadow = torch.zeros(n, dtype=BF16, device=dev) if self.use_bf16 else None
         # codebook matmuls: the reference keeps them in fp32 (models.py:115-118).  In bf16 mode they run on the
-        # wgmma GEMM with every fp32 operand split into bf16 hi + lo parts (fp32 accumulation): ~2^-16 relative.
+        # wgmma GEMM with every fp32 operand split into bf16 hi + lo parts (fp32 accumulation): ~2^-16 of sum|a||b|.
         self._cb_tc = self.use_bf16 and self.n_hid % 8 == 0 and self.K % 8 == 0
         if self._cb_tc:
             self.cb_hi = torch.zeros(self.n_hid, self.K, dtype=BF16, device=dev)
@@ -287,7 +287,11 @@ class VaeEngine:
                 x = sv["out"]
             else:
                 x = self._res_fwd(B, name, ch, res, x, sv)
-        rows = B * self.hw * self.hw
+        return self._codebook_logits(x, B * self.hw * self.hw)
+
+    def _codebook_logits(self, x, rows):
+        """logits = enc @ codebook (src/vae_tf/models.py:115-118) for the encoder output x (activation dtype)."""
+        b = self._b
         if self._cb_tc:   # x is exactly bf16: logits = x @ (C_hi + C_lo)
             xb = x.view(rows, self.n_hid)
             self._enc_bf16 = xb
@@ -339,7 +343,10 @@ class VaeEngine:
         """z = y @ codebook^T for b["y_out"] (src/vae_tf/models.py:127, tied weight)."""
         b = self._b
         rows = B * self.hw * self.hw
-        if self._cb_tc:   # z = y @ C^T with y, C split into bf16 hi + lo (the lo*lo term is below fp32 resolution)
+        if self._cb_tc:
+            # z = y @ C^T with y, C split into bf16 hi + lo.  |lo| <= 2^-8 |x| and x - hi - lo <= 2^-16 |x|, so the
+            # dropped lo*lo term and the two split residuals cost <= 3.1 * 2^-16 * sum|y||C| per element: ~2^-16
+            # relative, not fp32's 2^-24 (tests/test_vae_kernels_gpu.py holds the products to that bound)
             ops.split_f32(b["y_out"], b["y_hi"], b["y_lo"])
             self._mm_split([b["y_hi"], b["y_hi"], b["y_lo"]], [self.cb_hi, self.cb_lo, self.cb_hi], b["z_f32"], rows,
                            self.n_hid, self.K, b_mn=False)
@@ -422,28 +429,10 @@ class VaeEngine:
             s0, _ = self.layout.span(self._first_dec, self._first_dec)
             _, e0 = self.layout.span("decoder/conv2d/bias", "decoder/conv2d/bias")
             on_bucket_ready(s0, e0 + 64)      # + the aux scalars (loss) behind the last parameter
-        # quantiser
-        cb = self.P("codebook/codebook")
-        gcb = self.G("codebook/codebook")
-        pair = b["gscratch"][(B, self.hw, self.hw, self.n_hid)]
-        if self._cb_tc:
-            dzb = dx.view(rows, self.n_hid)                                                       # exactly bf16
-            ops.linear_wgrad(dzb, b["y_hi"], gcb); ops.linear_wgrad(dzb, b["y_lo"], gcb)          # d codebook (decode)
-            self._mm_split([dzb, dzb], [self.cb_hi, self.cb_lo], b["dy"], rows, self.K, self.n_hid, b_mn=True)
-            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
-            ops.split_f32(b["dlogits"], b["dl_hi"], b["dl_lo"])
-            ops.linear_wgrad(self._enc_bf16, b["dl_hi"], gcb); ops.linear_wgrad(self._enc_bf16, b["dl_lo"], gcb)
-            self._mm_split([b["dl_hi"], b["dl_hi"], b["dl_lo"]], [self.cb_hi, self.cb_lo, self.cb_hi],
-                           b["denc_f32"], rows, self.n_hid, self.K, b_mn=False)
-        else:
-            dz = self._to_f32(dx.view(rows, self.n_hid), b["dz_f32"])
-            ops.rowmatmul_tn(dz, b["y_out"], gcb, rows, self.n_hid, self.K)                       # d codebook (decode)
-            ops.rowmatmul(dz, cb, b["dy"], rows, self.n_hid, self.K)                              # dy = dz @ C
-            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
-            ops.rowmatmul_tn(self._enc_f32, b["dlogits"], gcb, rows, self.n_hid, self.K)
-            ops.rowmatmul(b["dlogits"], cb, b["denc_f32"], rows, self.K, self.n_hid, b_transposed=True)
+        self._quantiser_backward(dx, rows)
         if on_bucket_ready:
             on_bucket_ready(*self.layout.span("codebook/codebook", "codebook/codebook"))
+        pair = b["gscratch"][(B, self.hw, self.hw, self.n_hid)]
         dx = self._to_act(b["denc_f32"], pair[0].view(rows, self.n_hid)).view(B, self.hw, self.hw, self.n_hid)
         if not self.use_bf16:
             dx = b["denc_f32"].view(B, self.hw, self.hw, self.n_hid)
@@ -468,6 +457,29 @@ class VaeEngine:
             s0, _ = self.layout.span(self.layout.order[0], self.layout.order[0])
             e0, _ = self.layout.span("codebook/codebook", "codebook/codebook")
             on_bucket_ready(s0, e0)
+
+    def _quantiser_backward(self, dx, rows):
+        """Backward of z = y_out @ codebook^T and of the straight-through Gumbel softmax, for dx = d(loss)/dz: adds the
+        codebook gradient (decode and encode side) into self.grads and leaves d(encoder output) in b["denc_f32"]."""
+        b = self._b
+        cb = self.P("codebook/codebook")
+        gcb = self.G("codebook/codebook")
+        if self._cb_tc:
+            dzb = dx.view(rows, self.n_hid)                                                       # exactly bf16
+            ops.linear_wgrad(dzb, b["y_hi"], gcb); ops.linear_wgrad(dzb, b["y_lo"], gcb)          # d codebook (decode)
+            self._mm_split([dzb, dzb], [self.cb_hi, self.cb_lo], b["dy"], rows, self.K, self.n_hid, b_mn=True)
+            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
+            ops.split_f32(b["dlogits"], b["dl_hi"], b["dl_lo"])
+            ops.linear_wgrad(self._enc_bf16, b["dl_hi"], gcb); ops.linear_wgrad(self._enc_bf16, b["dl_lo"], gcb)
+            self._mm_split([b["dl_hi"], b["dl_hi"], b["dl_lo"]], [self.cb_hi, self.cb_lo, self.cb_hi],
+                           b["denc_f32"], rows, self.n_hid, self.K, b_mn=False)
+        else:
+            dz = self._to_f32(dx.view(rows, self.n_hid), b["dz_f32"])
+            ops.rowmatmul_tn(dz, b["y_out"], gcb, rows, self.n_hid, self.K)                       # d codebook (decode)
+            ops.rowmatmul(dz, cb, b["dy"], rows, self.n_hid, self.K)                              # dy = dz @ C
+            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
+            ops.rowmatmul_tn(self._enc_f32, b["dlogits"], gcb, rows, self.n_hid, self.K)
+            ops.rowmatmul(b["dlogits"], cb, b["denc_f32"], rows, self.K, self.n_hid, b_transposed=True)
 
     # ------------------------------------------------------------------------------------------ optimiser
     def zero_grads(self):

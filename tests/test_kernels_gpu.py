@@ -228,7 +228,7 @@ def test_embedding_fwd_bwd_and_label_shift(ops):
     assert torch.equal(toks.cpu(), torch.cat([text, img + 50], 1))
 
 
-@pytest.mark.parametrize("d", [256, 512, 1024])
+@pytest.mark.parametrize("d", [256, 512, 768, 1024, 2048, 4096])   # 4096: the wide kernel (12 B width)
 def test_layernorm_fwd_bwd(ops, d):
     g = torch.Generator().manual_seed(d)
     rows = 203
@@ -251,6 +251,16 @@ def test_layernorm_fwd_bwd(ops, d):
     ops.layernorm_bwd(dy.to(DEV), x.to(DEV), gg.to(DEV), mean, rstd, dres.to(DEV), dx2, torch.zeros(d, device=DEV),
                       torch.zeros(d, device=DEV), dxsum=dxs)                    # fused column sums of dx
     assert torch.equal(dx2, dx) and relmax(dxs, dx.float().sum(0)) < 1e-5
+    # the entry point without dxsum: the same kernels, so the same bits
+    from dalle_mtf_b200 import lib as L
+    dyd, xd, gd, dresd = dy.to(DEV), x.to(DEV), gg.to(DEV), dres.to(DEV)
+    dx3, dg3, db3 = torch.empty_like(dx), torch.zeros(d, device=DEV), torch.zeros(d, device=DEV)
+    ws = L.workspace(L.load().db200_layernorm_bwd_workspace_bytes(rows, d))
+    L.check(L.load().db200_layernorm_bwd(L.stream_ptr(), dyd.data_ptr(), xd.data_ptr(), gd.data_ptr(), mean.data_ptr(),
+                                         rstd.data_ptr(), dresd.data_ptr(), dx3.data_ptr(), dg3.data_ptr(),
+                                         db3.data_ptr(), rows, d, L.ptr(ws), ws.numel() if ws is not None else 0),
+            "db200_layernorm_bwd")
+    assert torch.equal(dx3, dx) and torch.equal(dg3, dg) and torch.equal(db3, db)
 
 
 def test_colsum_and_casts(ops):

@@ -2,12 +2,17 @@
 //
 //   D[M,N] = A[M,K] * B[K,N],  fp32 accumulation in registers, operands staged in shared memory by TMA (128B swizzle).
 //
-//   warp 0    : TMA producer (one elected lane)            smem ring: STAGES x {A 128x64, B BNx64} bf16
-//   warps 1-3 : idle
-//   warps 4-11: two consumer warpgroups.  Warpgroup g issues wgmma m64 x BN x 16 for rows [64g, 64g+64) of the tile;
-//               at the end of a tile both write their accumulators to a shared-memory tile, and the 8 warps run the
-//               epilogue on it (each accumulator row split between two threads) -> bias / ReLU / residual / split-K
-//               reduction / cross-entropy statistics and gradient.  The producer keeps loading the next tile meanwhile.
+//   warp 0     : TMA producer (one elected lane)            smem ring: STAGES x {A 128x64, B BNx64} bf16
+//   warps 1-3  : idle (they hand their registers to the other warpgroups and exit)
+//   warps 4-11 : two MMA warpgroups.  Warpgroup g issues wgmma m64 x BN x 16 for rows [64g, 64g+64) of the tile and at
+//                the end of the tile writes its accumulators to a shared-memory accumulator tile.
+//   warps 12-15: the epilogue warpgroup.  Warp e owns rows [32e, 32e+32) of the accumulator tile, one row per thread,
+//                and runs the epilogue on it half tile by half tile -> bias / ReLU / residual / split-K reduction /
+//                cross-entropy statistics and gradient.
+//
+// The accumulator tile is single-buffered and handed over through two named barriers (FULL: written by the MMA
+// warpgroups; EMPTY: read by the epilogue).  The MMA warpgroups run the next tile's mainloop while the epilogue works
+// on the previous one, and wait for EMPTY only before their next store; the producer keeps loading throughout.
 //
 // Either operand may be K-major or MN-major in global memory; the tensor maps and the wgmma descriptors absorb the
 // difference, so forward (x*W), dgrad (dy*W^T) and wgrad (x^T*dy) are the same kernel.
@@ -19,15 +24,23 @@
 
 namespace db200 {
 
-// BN = 128: the 128 x 128 fp32 accumulator tile (64 KiB) and four 32 KiB stages fit the 227 KiB of an H100 SM.
+// BN = 128: the 128 x 128 fp32 accumulator tile (64 KiB), four 32 KiB stages and the epilogue warps' staging blocks fit
+// the 227 KiB of an H100 SM; a second accumulator tile or a fifth stage does not.
 constexpr int GBN = 128;
 constexpr int G_STAGES = 4;
 constexpr uint32_t G_B_BYTES = GBN * BK * 2;
 constexpr uint32_t G_STAGE_BYTES = A_BYTES + G_B_BYTES;
 constexpr uint32_t G_ACC_BYTES = BM * GBN * 4;
 constexpr size_t G_SMEM_BYTES =
-    1024 /*align slack*/ + G_ACC_BYTES + size_t(G_STAGES) * G_STAGE_BYTES + 256 /*barriers*/ + 8 * 4096 /*staging*/;
+    1024 /*align slack*/ + G_ACC_BYTES + size_t(G_STAGES) * G_STAGE_BYTES + 256 /*barriers*/ + 4 * STG_BYTES;
 static_assert(G_SMEM_BYTES <= 227 * 1024, "GEMM shared memory exceeds the H100 per-block limit");
+
+// 512 threads compile to 128 registers each; setmaxnreg moves the producer warpgroup's share to the MMA warpgroups
+// (64 accumulators + the mainloop) and the epilogue (two 32-column accumulator chunks + the output chunk in flight).
+constexpr int G_REGS_PRODUCER = 40, G_REGS_MMA = 152, G_REGS_EPI = 168;
+static_assert(128 * G_REGS_PRODUCER + 256 * G_REGS_MMA + 128 * G_REGS_EPI <= 65536, "GEMM register budget");
+// named barriers of the accumulator-tile hand-off: 256 MMA threads + 128 epilogue threads
+constexpr int G_BAR_FULL = 1, G_BAR_EMPTY = 2, G_BAR_HANDOFF_THREADS = 384;
 
 // operand majors (1 = MN-major), compile-time for wgmma; DROP: dropout in the STORE epilogue
 template <int TA, int TB, bool DROP>
@@ -44,7 +57,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t bars = sA + STAGES * G_STAGE_BYTES;
   const uint32_t full_bar = bars;                   // STAGES x 8 B
   const uint32_t empty_bar = bars + 8 * STAGES;     // STAGES x 8 B
-  const uint32_t stg_base = bars + 256;             // 8 x STG_BYTES, 16-byte aligned
+  const uint32_t stg_base = bars + 256;             // 4 x STG_BYTES, 16-byte aligned
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -56,7 +69,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(full_bar + 8 * i, 1);
-      mbar_init(empty_bar + 8 * i, 2);  // one arrive per consumer warpgroup
+      mbar_init(empty_bar + 8 * i, 2);  // one arrive per MMA warpgroup
     }
     fence_mbar_init();
   }
@@ -64,7 +77,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   const int total_tiles = p.m_tiles * p.n_tiles * p.splits;
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<G_REGS_PRODUCER>();
+    if (warp != 0) return;
     // ------------------------------------------------------------------ TMA producer
     // converged warp, issuer picked by elect.sync: TMA instructions compile to plain uniform-datapath code
     uint32_t stage = 0, phase = 0;
@@ -100,14 +115,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ consumers: MMA, then epilogue
-    const int ew = warp - 4;
-    const int wg = ew >> 2;        // consumer warpgroup: accumulator rows [64 wg, 64 wg + 64)
-    const int wq = ew & 3;         // epilogue: rows [32 wq, 32 wq + 32) ...
-    const int half = ew >> 2;      // ... and columns [half * BN/2, (half + 1) * BN/2)
-    constexpr int CH = BN / 64;    // 32-column chunks per half
-    const uint32_t stg = stg_base + ew * STG_BYTES;
+  } else if (warp < 12) {
+    // ------------------------------------------------------------------ MMA warpgroups
+    setmaxnreg_inc<G_REGS_MMA>();
+    const int wg = (warp - 4) >> 2;  // accumulator rows [64 wg, 64 wg + 64)
     // K-major: a K-step advances 16 elements (32 B) inside the 128 B swizzle row and warpgroup g starts 64 rows (8 KiB)
     // in; MN-major: a K-step is 16 k-rows (2 KiB) and warpgroup g takes the g-th 64-wide slab (SLAB_BYTES apart).
     constexpr uint64_t astep = TA ? 128u : 2u, bstep = TB ? 128u : 2u;
@@ -116,21 +127,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
-      const int row0 = t.m_blk * BM + wq * 32;
-      const int row = row0 + lane;
-      const bool row_ok = row < p.M;
-      const int cbase = t.n_blk * BN + half * (BN / 2);
-      // pull this half-tile's bias into L1 and the per-element operands (ReLU mask / residual rows) into L2 while
-      // the accumulator is being produced
-      if (p.bias && lane < BN / 64 && cbase + lane * 32 < p.N)
-        asm volatile("prefetch.global.L1 [%0];" ::"l"(p.bias + cbase + lane * 32));
-      if (row_ok && cbase < p.N) {
-        if (p.aux) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.aux + (long long)row * p.ldaux + cbase));
-        if (p.residual) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + (long long)row * p.ldr + cbase));
-      }
       uint32_t prev_stage = 0;
       // zero the accumulator here rather than through wgmma's scale-d: its registers are then dead between the
-      // shared-memory store of one tile and the start of the next (no spill around the epilogue)
+      // shared-memory store of one tile and the start of the next
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       for (int kb = t.kb0; kb < t.kb1; ++kb) {
@@ -151,21 +150,53 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       wgmma_wait<0>();
       if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
-      named_bar_sync(1, 256);  // the previous tile's epilogue has finished reading the accumulator tile
+      // the epilogue has finished reading the previous tile (it signals EMPTY after every tile but the last)
+      if (tile != blockIdx.x) named_bar_sync(G_BAR_EMPTY, G_BAR_HANDOFF_THREADS);
       acc_store_smem<BN>(d, sAcc >> 2, 64 * wg);
-      named_bar_sync(1, 256);
-      const uint32_t t_addr = (sAcc >> 2) + (wq * 32 + lane) * BN + half * (BN / 2);
-      switch (p.mode) {
-        case DB200_EPI_STORE:    epi_store<CH, DROP>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
-        case DB200_EPI_ATOMIC:
-          epi_atomic<CH>(p, reinterpret_cast<float*>(p.D) + (long long)t.split * p.M * p.ldd, row, row_ok, cbase,
-                         t_addr);
-          break;
-        case DB200_EPI_RELU_BWD: epi_relu_bwd<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
-        case DB200_EPI_CE_STATS: epi_ce_stats<CH>(p, t_addr, row, row_ok, cbase, t.n_blk * 2 + half); break;
-        case DB200_EPI_CE_GRAD:  epi_ce_grad<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
-        default: break;
+      named_bar_arrive(G_BAR_FULL, G_BAR_HANDOFF_THREADS);
+    }
+  } else {
+    // ------------------------------------------------------------------ epilogue warpgroup
+    setmaxnreg_inc<G_REGS_EPI>();
+    const int ew = warp - 12;      // rows [32 ew, 32 ew + 32) of the tile, one per lane
+    constexpr int CH = BN / 64;    // 32-column chunks per half tile
+    const uint32_t stg = stg_base + ew * STG_BYTES;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
+      const int row0 = t.m_blk * BM + ew * 32;
+      const int row = row0 + lane;
+      const bool row_ok = row < p.M;
+      const int n0 = t.n_blk * BN;
+      // pull this tile's bias into L1 and the per-element operands (ReLU mask / residual rows) into L2 while the
+      // accumulator is being produced
+      if (p.bias && lane < BN / 32 && n0 + lane * 32 < p.N)
+        asm volatile("prefetch.global.L1 [%0];" ::"l"(p.bias + n0 + lane * 32));
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int cbase = n0 + half * (BN / 2);
+        if (row_ok && cbase < p.N) {
+          if (p.aux) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.aux + (long long)row * p.ldaux + cbase));
+          if (p.residual) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + (long long)row * p.ldr + cbase));
+        }
       }
+      named_bar_sync(G_BAR_FULL, G_BAR_HANDOFF_THREADS);
+#pragma unroll 1
+      for (int half = 0; half < 2; ++half) {  // columns [half * BN/2, (half + 1) * BN/2) of the tile
+        const int cbase = n0 + half * (BN / 2);
+        const uint32_t t_addr = (sAcc >> 2) + (ew * 32 + lane) * BN + half * (BN / 2);
+        switch (p.mode) {
+          case DB200_EPI_STORE:    epi_store<CH, DROP>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
+          case DB200_EPI_ATOMIC:
+            epi_atomic<CH>(p, reinterpret_cast<float*>(p.D) + (long long)t.split * p.M * p.ldd, row, row_ok, cbase,
+                           t_addr);
+            break;
+          case DB200_EPI_RELU_BWD: epi_relu_bwd<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
+          case DB200_EPI_CE_STATS: epi_ce_stats<CH>(p, t_addr, row, row_ok, cbase, t.n_blk * 2 + half); break;
+          case DB200_EPI_CE_GRAD:  epi_ce_grad<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
+          default: break;
+        }
+      }
+      if (tile + (int)gridDim.x < total_tiles) named_bar_arrive(G_BAR_EMPTY, G_BAR_HANDOFF_THREADS);
     }
   }
 }

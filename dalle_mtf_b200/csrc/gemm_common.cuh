@@ -10,7 +10,7 @@ namespace db200 {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int GEMM_THREADS = 384;  // 4 control warps + 2 consumer warpgroups
+constexpr int GEMM_THREADS = 512;  // 4 control warps + 2 MMA warpgroups + 1 epilogue warpgroup
 constexpr int GROUP_M = 8;
 constexpr uint32_t SLAB_BYTES = BK * 128;  // one MN-major slab: [BK k-rows][64 bf16] = 8 KiB
 constexpr uint32_t A_BYTES = BM * BK * 2;  // 16 KiB

@@ -138,6 +138,17 @@ __device__ __forceinline__ bool elect_one_sync() {
   return pred != 0;
 }
 
+// setmaxnreg: change the calling warpgroup's per-thread register count (every warp of the warpgroup executes it;
+// R is a multiple of 8 in [24, 256]).  dec returns registers to the CTA's pool, inc waits until the pool can supply them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+
 // ----------------------------------------------------------------------------------------------
 // wgmma shared-memory operand descriptor (PTX ISA "Matrix Descriptor Format" for wgmma), 128-byte swizzle.
 //   K-major tile  [rows][64 bf16]        : rows are 128 B apart, 8-row groups SBO=1024 B apart, LBO unused.

@@ -111,5 +111,9 @@ __device__ __forceinline__ void acc_ld_x32(uint32_t addr_w, uint32_t* r) {
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// signal the same barrier without waiting: the producing side of a hand-off whose consumers bar.sync on it
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 }  // namespace db200

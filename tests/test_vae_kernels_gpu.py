@@ -36,6 +36,7 @@ least twice as many work tiles as the device has SMs (the persistent CTAs then w
 geometries: ragged spatial sizes, several images packed into one tile, 64-wide and ragged channel tiles, and a wgrad
 with fewer pixel tiles than the split count the host rule asks for.
 """
+import functools
 import json
 import math
 import os
@@ -43,15 +44,15 @@ import os
 import pytest
 import torch
 
+import float64_bounds
+from float64_bounds import DEV, NAN, U, UTC, nan_like
+
 pytestmark = pytest.mark.gpu
 
-DEV = "cuda"
 F32, F64, BF16, I32 = torch.float32, torch.float64, torch.bfloat16, torch.int32
-NAN = float("nan")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+check = functools.partial(float64_bounds.check, tag="vae-kernels")
 
-U = 2.0 ** -24          # fp32 unit roundoff
-UTC = 2.0 ** -23        # one wgmma accumulation step
 SPLIT1 = 1.01 * 2.0 ** -16
 SPLIT2 = 3.1 * 2.0 ** -16
 
@@ -73,28 +74,6 @@ def _gen(seed):
 
 def _randn(*shape, g, scale=1.0, dtype=F32):
     return (torch.randn(*shape, generator=g, device=DEV) * scale).to(dtype)
-
-
-def half_ulp_bf16(x):
-    """Half an ulp of bf16 at |x| (float64, x >= 0): the largest error of rounding a value of that size to bf16."""
-    return torch.exp2(torch.floor(torch.log2(x.clamp_min(2.0 ** -133))) - 8)
-
-
-def check(name, got, ref, absref, *, a=2 * U, b=0.0, bf16_out=False, floor=0.0):
-    """Per element |got - ref| <= a |ref| + b absref + floor (bf16 outputs: half a bf16 ulp instead of a |ref|)."""
-    got = got.to(F64)
-    bad = (~torch.isfinite(got)).sum().item()
-    assert bad == 0, f"{name}: {bad} outputs are not finite (never written over the NaN sentinel?)"
-    acc = b * absref + floor
-    rnd = half_ulp_bf16(ref.abs() + acc) if bf16_out else a * ref.abs()
-    ratio = ((got - ref).abs() / (rnd + acc).clamp_min(1e-300)).max().item()
-    print(f"[vae-kernels] {name}: worst err/bound {ratio:.4f}")
-    assert ratio < 1.0, f"{name}: worst err/bound {ratio:.4f}"
-    return ratio
-
-
-def nan_like(shape, dtype):
-    return torch.full(shape, NAN, dtype=dtype, device=DEV)
 
 
 def first_argmax(x):

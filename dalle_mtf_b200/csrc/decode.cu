@@ -7,6 +7,7 @@
 //   attn_decode    append this step's k,v to the cache at `pos`, then out[b,h,:] = softmax_j<=pos(scale q.k_j) v_j
 //                  fp32 scores / softmax, P rounded to bf16 for the PV product (same policy as attn.cu)
 //   sample_rows    idx = lo + argmax_{lo<=c<hi}(logits[c] * inv_temp + gumbel(u[c-lo]))   (first maximum; u NULL = greedy)
+//   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
 //   onehot_rows    y[r, idx[r]-offset] = 1, 0 elsewhere (codebook lookup input for the VAE decoder, vae_tf/models.py:127)
 #include "common.cuh"
 #include "ptx.cuh"
@@ -139,6 +140,10 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
   }
 }
 
+// The Gumbel-max perturbation x + g(u), g(u) = -log(-log u); the filtered sampler uses the same expression, so with its
+// filter off it selects exactly what sample_rows_kernel selects.
+__device__ __forceinline__ float gumbel_perturb(float x, float u) { return x + -logf(-logf(u)); }
+
 __global__ void __launch_bounds__(256)
 sample_rows_kernel(const float* __restrict__ logits, const float* __restrict__ u, int* __restrict__ idx, long long ld,
                    int lo, int hi, float inv_temp, const int* __restrict__ pos_dev, long long ld_idx) {
@@ -151,7 +156,7 @@ sample_rows_kernel(const float* __restrict__ logits, const float* __restrict__ u
   int arg = 0x7fffffff;
   for (int c = tid; c < n; c += 256) {
     float x = row[lo + c] * inv_temp;
-    if (u) x += -logf(-logf(u[(long long)r * n + c]));
+    if (u) x = gumbel_perturb(x, u[(long long)r * n + c]);
     if (x > best || (x == best && c < arg)) { best = x; arg = c; }
   }
 #pragma unroll
@@ -168,6 +173,229 @@ sample_rows_kernel(const float* __restrict__ logits, const float* __restrict__ u
     // pos_dev != NULL (graph replay): the sample is the token of position *pos_dev + 1 of the [rows][ld_idx] matrix
     int* dst = pos_dev ? idx + r * ld_idx + (*pos_dev + 1) : idx + r;
     *dst = lo + (arg == 0x7fffffff ? 0 : arg);  // all -inf / NaN row: first allowed id
+  }
+}
+
+// ---- top-k / nucleus (top-p) filtered sampling.  One CTA per row; the row's x = logits * inv_temp is staged in dynamic
+// shared memory as order-preserving uint32 keys, so "x_a > x_b" is "key_a > key_b" and every kept set is an upper set
+// of keys {key >= T}: the kernel finds T and then runs the Gumbel-max over the keys >= T.
+//   top-k: T_k = the k-th largest key (ties at T_k all kept), by MSB-first radix select (8-bit digits, 4 passes of a
+//          256-bin count histogram);
+//   top-p: over the keys >= T_k, w = exp(x - max), Z = sum w; x is kept iff the mass strictly above it is < p * Z.
+//          The same 4-pass descent over per-bin mass finds the smallest such key.  Masses are 64-bit fixed point
+//          (2^-46 units) summed with integer atomics, so the kept set is the same on every run.
+// NaN and -inf map to key 0 and are never kept; -0 is stored as +0 (the two compare equal, so must share a key);
+// +inf entries, if any, are the only ones kept (the softmax mass is undefined there).
+constexpr int SF_THREADS = 1024, SF_WARPS = SF_THREADS / 32;
+constexpr int SF_SMEM_BYTES = 200 * 1024;                       // dynamic shared memory: one uint32 key per id
+constexpr int SF_MAX_N = SF_SMEM_BYTES / 4;                      // 51 200 ids per row
+constexpr uint32_t SF_KEY_PINF = 0xff800000u;                   // key of +inf
+constexpr int SF_NONE = 256;                                    // histogram bin of ids a pass ignores
+
+__device__ __forceinline__ uint32_t sf_key(float x) {
+  if (!(x > -INFINITY)) return 0u;                              // NaN, -inf
+  const uint32_t b = __float_as_uint(x == 0.f ? 0.f : x);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+__device__ __forceinline__ float sf_value(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// Thread t < 256 passes v = the value of bin 255 - t and gets the total of the bins above that digit.  Called by every
+// thread of the CTA (it synchronises); wtot holds 8 partials.
+__device__ __forceinline__ unsigned long long sf_sum_above(unsigned long long v, unsigned long long* wtot) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  unsigned long long incl = 0;
+  if (tid < 256) {
+    incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    if (lane == 31) wtot[warp] = incl;
+  }
+  __syncthreads();
+  if (tid < 256)
+    for (int w = 0; w < warp; ++w) incl += wtot[w];
+  return incl - v;
+}
+
+__device__ __forceinline__ uint32_t sf_block_sum(uint32_t v, uint32_t* red) {
+  v = __reduce_add_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t s = 0;
+#pragma unroll 8
+  for (int w = 0; w < SF_WARPS; ++w) s += red[w];
+  __syncthreads();
+  return s;
+}
+
+__device__ __forceinline__ uint32_t sf_block_max(uint32_t v, uint32_t* red) {
+  v = __reduce_max_sync(0xffffffffu, v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  uint32_t s = 0;
+#pragma unroll 8
+  for (int w = 0; w < SF_WARPS; ++w) s = max(s, red[w]);
+  __syncthreads();
+  return s;
+}
+
+__device__ __forceinline__ unsigned long long sf_mass(uint32_t k, float xmax) {
+  return __float2ull_rn(expf(sf_value(k) - xmax) * 0x1p46f);  // w in (0, 1] -> [0, 2^46]
+}
+
+__global__ void __launch_bounds__(SF_THREADS)
+sample_rows_filtered_kernel(const float* __restrict__ logits, const float* __restrict__ u, int* __restrict__ idx,
+                            int* __restrict__ kept, long long ld, int lo, int hi, float inv_temp, int top_k, float top_p,
+                            const int* __restrict__ pos_dev, long long ld_idx) {
+  extern __shared__ uint32_t keys[];
+  __shared__ uint32_t mlo[SF_NONE + 1], mhi[SF_NONE + 1];  // per-bin mass = mhi * 2^32 + mlo (no 64-bit smem atomics)
+  __shared__ uint32_t cnt[SF_NONE + 1];
+  __shared__ unsigned long long wtot[SF_WARPS];
+  __shared__ uint32_t red[SF_WARPS];
+  __shared__ int sel;
+  __shared__ unsigned long long sel_above;
+  __shared__ float bv[SF_WARPS];
+  __shared__ int bi[SF_WARPS];
+  const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* row = logits + (long long)r * ld;
+  const int n = hi - lo;
+
+  uint32_t nv = 0, ninf = 0, kmax = 0;
+  for (int c = tid; c < n; c += SF_THREADS) {
+    const uint32_t k = sf_key(row[lo + c] * inv_temp);
+    keys[c] = k;
+    nv += k != 0;
+    ninf += k == SF_KEY_PINF;
+    kmax = max(kmax, k);
+  }
+  nv = sf_block_sum(nv, red);      // (the barriers inside also publish keys[])
+  ninf = sf_block_sum(ninf, red);
+  kmax = sf_block_max(kmax, red);
+
+  uint32_t T = 1;                  // smallest kept key; 0 (NaN, -inf) is never kept
+  if (nv == 0) {
+    T = 0xffffffffu;               // nothing is kept: the largest key in use is SF_KEY_PINF
+  } else if (ninf > 0) {
+    T = SF_KEY_PINF;
+  } else {
+    if (top_k > 0 && (uint32_t)top_k < nv) {
+      // radix select of the k-th largest key: `rem` ids are still to be counted from the top inside `prefix`
+      uint32_t prefix = 0, rem = (uint32_t)top_k;
+      for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        const uint32_t himask = pass == 0 ? 0u : ~0u << (shift + 8);
+        for (int b = tid; b <= SF_NONE; b += SF_THREADS) cnt[b] = 0;
+        __syncthreads();
+        for (int c0 = 0; c0 < n; c0 += SF_THREADS) {   // uniform trip count: whole warps take part in the match
+          const int c = c0 + tid;
+          const uint32_t k = c < n ? keys[c] : 0u;
+          const int d = (k != 0 && (k & himask) == prefix) ? (int)((k >> shift) & 255u) : SF_NONE;
+          if (!__any_sync(0xffffffffu, d != SF_NONE)) continue;
+          const unsigned peers = __match_any_sync(0xffffffffu, d);
+          if (d != SF_NONE && lane == __ffs(peers) - 1) atomicAdd(&cnt[d], (uint32_t)__popc(peers));
+        }
+        __syncthreads();
+        const unsigned long long above = sf_sum_above(tid < 256 ? cnt[255 - tid] : 0u, wtot);
+        if (tid < 256 && above < rem && above + cnt[255 - tid] >= rem) {
+          sel = 255 - tid;
+          sel_above = above;
+        }
+        __syncthreads();
+        prefix |= (uint32_t)sel << shift;
+        rem -= (uint32_t)sel_above;
+        __syncthreads();
+      }
+      T = prefix;
+    }
+    if (top_p < 1.f) {
+      const float xmax = sf_value(kmax);
+      unsigned long long z = 0;
+      for (int c = tid; c < n; c += SF_THREADS) {
+        const uint32_t k = keys[c];
+        if (k >= T) z += sf_mass(k, xmax);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+      if (lane == 0) wtot[warp] = z;
+      __syncthreads();
+      z = 0;
+      for (int w = 0; w < SF_WARPS; ++w) z += wtot[w];
+      __syncthreads();
+      const double pz = (double)top_p * (double)z;
+      // descent: `above` = mass of the kept-candidate ids (keys >= T) whose key lies above `prefix`
+      uint32_t prefix = 0;
+      unsigned long long above = 0;
+      for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        const uint32_t himask = pass == 0 ? 0u : ~0u << (shift + 8);
+        for (int b = tid; b <= SF_NONE; b += SF_THREADS) { cnt[b] = 0; mlo[b] = 0; mhi[b] = 0; }
+        if (tid == 0) sel = -1;
+        __syncthreads();
+        for (int c0 = 0; c0 < n; c0 += SF_THREADS) {
+          const int c = c0 + tid;
+          const uint32_t k = c < n ? keys[c] : 0u;
+          const int d = (k >= T && (k & himask) == prefix) ? (int)((k >> shift) & 255u) : SF_NONE;
+          if (!__any_sync(0xffffffffu, d != SF_NONE)) continue;
+          const unsigned long long w = d != SF_NONE ? sf_mass(k, xmax) : 0ull;
+          const unsigned peers = __match_any_sync(0xffffffffu, d);
+          // per-digit warp sums of the two 23-bit halves of w (at most 32 * 2^23 each: no overflow in 32 bits)
+          const uint32_t wlo = __reduce_add_sync(peers, (uint32_t)(w & 0x7fffffu));
+          const uint32_t whi = __reduce_add_sync(peers, (uint32_t)(w >> 23));
+          if (d != SF_NONE && lane == __ffs(peers) - 1) {
+            const unsigned long long add = ((unsigned long long)whi << 23) + wlo;
+            const uint32_t alo = (uint32_t)add, old = atomicAdd(&mlo[d], alo);
+            atomicAdd(&mhi[d], (uint32_t)(add >> 32) + (old + alo < old ? 1u : 0u));   // carry out of the low word
+            atomicAdd(&cnt[d], (uint32_t)__popc(peers));
+          }
+        }
+        __syncthreads();
+        // the largest key of bin 255 - tid has mass above + (bins above it) strictly above it: the lowest non-empty
+        // bin where that is < p * Z holds T_p
+        const unsigned long long in =
+            sf_sum_above(tid < 256 ? ((unsigned long long)mhi[255 - tid] << 32) + mlo[255 - tid] : 0ull, wtot);
+        if (tid < 256 && cnt[255 - tid] > 0 && (double)(above + in) < pz) atomicMax(&sel, tid);
+        __syncthreads();
+        if (tid == sel) sel_above = in;
+        __syncthreads();
+        prefix |= (uint32_t)(255 - sel) << shift;
+        above += sel_above;
+        __syncthreads();
+      }
+      T = prefix;
+    }
+  }
+
+  // Gumbel-max over the kept ids; first index on ties
+  float best = -INFINITY;
+  int arg = 0x7fffffff;
+  uint32_t nk = 0;
+  for (int c = tid; c < n; c += SF_THREADS) {
+    const uint32_t k = keys[c];
+    if (k < T) continue;
+    ++nk;
+    float x = sf_value(k);
+    if (u) x = gumbel_perturb(x, u[(long long)r * n + c]);
+    if (x > best || (x == best && c < arg)) { best = x; arg = c; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, arg, o);
+    if (ov > best || (ov == best && oi < arg)) { best = ov; arg = oi; }
+  }
+  if (lane == 0) { bv[warp] = best; bi[warp] = arg; }
+  nk = sf_block_sum(nk, red);
+  if (tid == 0) {
+    for (int w = 1; w < SF_WARPS; ++w)
+      if (bv[w] > best || (bv[w] == best && bi[w] < arg)) { best = bv[w]; arg = bi[w]; }
+    int* dst = pos_dev ? idx + r * ld_idx + (*pos_dev + 1) : idx + r;
+    *dst = lo + (arg == 0x7fffffff ? 0 : arg);  // no finite id: first allowed id
+    if (kept) kept[r] = (int)nk;
   }
 }
 
@@ -276,6 +504,43 @@ extern "C" int db200_sample_rows_at(db200_stream_t stream_, const float* logits,
                 "sample_rows_at: rows %d range [%d,%d) ld %lld", rows, lo, hi, ld);
   sample_rows_kernel<<<rows, 256, 0, stream>>>(logits, u_or_null, tokens, ld, lo, hi, inv_temp, pos_dev, ld_tokens);
   return check_launch("sample_rows_kernel");
+}
+
+static int sample_rows_filtered_launch(cudaStream_t stream, const float* logits, const float* u, int32_t* idx,
+                                       int32_t* kept, int rows, long long ld, int lo, int hi, float inv_temp, int top_k,
+                                       float top_p, const int32_t* pos_dev, long long ld_idx) {
+  DB200_REQUIRE(rows > 0 && lo >= 0 && hi > lo && hi <= ld, DB200_E_INVALID,
+                "sample_rows_filtered: rows %d range [%d,%d) ld %lld", rows, lo, hi, ld);
+  DB200_REQUIRE(inv_temp > 0.f, DB200_E_INVALID, "sample_rows_filtered: inv_temp must be positive");
+  DB200_REQUIRE(top_k >= 0, DB200_E_INVALID, "sample_rows_filtered: top_k %d < 0", top_k);
+  DB200_REQUIRE(top_p > 0.f && top_p <= 1.f, DB200_E_INVALID, "sample_rows_filtered: top_p %g outside (0, 1]",
+                (double)top_p);
+  DB200_REQUIRE(hi - lo <= SF_MAX_N, DB200_E_UNSUPPORTED, "sample_rows_filtered: %d ids exceed the %d one CTA holds",
+                hi - lo, SF_MAX_N);
+  static const cudaError_t attr = cudaFuncSetAttribute(sample_rows_filtered_kernel,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, SF_SMEM_BYTES);
+  DB200_CUDA(attr);
+  sample_rows_filtered_kernel<<<rows, SF_THREADS, (size_t)(hi - lo) * sizeof(uint32_t), stream>>>(
+      logits, u, idx, kept, ld, lo, hi, inv_temp, top_k, top_p, pos_dev, ld_idx);
+  return check_launch("sample_rows_filtered_kernel");
+}
+
+extern "C" int db200_sample_rows_filtered(db200_stream_t stream_, const float* logits, const float* u_or_null,
+                                          int32_t* idx, int32_t* kept_or_null, int rows, long long ld, int lo, int hi,
+                                          float inv_temp, int top_k, float top_p) {
+  DB200_REQUIRE(logits && idx, DB200_E_INVALID, "sample_rows_filtered: null pointer");
+  return sample_rows_filtered_launch(static_cast<cudaStream_t>(stream_), logits, u_or_null, idx, kept_or_null, rows, ld,
+                                     lo, hi, inv_temp, top_k, top_p, nullptr, 1);
+}
+
+// graph-replay variant: the sample of row r becomes tokens[r * ld_tokens + *pos_dev + 1]
+extern "C" int db200_sample_rows_filtered_at(db200_stream_t stream_, const float* logits, const float* u_or_null,
+                                             int32_t* tokens, long long ld_tokens, int32_t* kept_or_null, int rows,
+                                             long long ld, int lo, int hi, float inv_temp, int top_k, float top_p,
+                                             const int32_t* pos_dev) {
+  DB200_REQUIRE(logits && tokens && pos_dev, DB200_E_INVALID, "sample_rows_filtered_at: null pointer");
+  return sample_rows_filtered_launch(static_cast<cudaStream_t>(stream_), logits, u_or_null, tokens, kept_or_null, rows,
+                                     ld, lo, hi, inv_temp, top_k, top_p, pos_dev, ld_tokens);
 }
 
 extern "C" int db200_onehot_rows_f32(db200_stream_t stream_, const int32_t* idx, float* y, int rows, int K,

@@ -55,15 +55,16 @@ class DALLE:
         return loss, loss_batch
 
 
-    def sample(self, text_ids, temperature=1.0, generator=None):
+    def sample(self, text_ids, temperature=1.0, generator=None, top_k=None, top_p=None):
         """Autoregressive generation with a K/V cache ("next" row N4; the reference stubs inference):
         text_ids int [B, text_seq_len] -> int32 [B, text_seq_len + image_seq_len], image positions sampled from
-        softmax(logits / temperature) restricted to the image-token ids (temperature 0 = greedy)."""
+        softmax(logits / temperature) restricted to the image-token ids (temperature 0 = greedy), optionally truncated
+        to its top_k ids and / or its top_p nucleus (DalleSampler.generate)."""
         from .sampling import DalleSampler
         if getattr(self, "_sampler", None) is None:
             self._sampler = DalleSampler(self.engine)
         text_ids = text_ids.to(device=self.engine.device, dtype=torch.int32).contiguous()
-        return self._sampler.generate(text_ids, temperature, generator)
+        return self._sampler.generate(text_ids, temperature, generator, top_k=top_k, top_p=top_p)
 
 
 class DiscreteVAE:

@@ -538,6 +538,31 @@ def sample_rows_at(logits, u, tokens, lo, hi, inv_temp, pos_dev):
     return tokens
 
 
+def sample_rows_filtered(logits, u, idx, lo, hi, inv_temp, top_k, top_p, kept=None):
+    """sample_rows restricted to the top-k / nucleus set of logits * inv_temp over [lo, hi) (top_k 0 and top_p 1 are
+    off; ties at either threshold are kept).  kept (int32 [rows], optional) receives the size of each row's kept set."""
+    L.require_device()
+    _chk(logits, F32, "logits"); _chk(u, F32, "u"); _chk(idx, I32, "idx"); _chk(kept, I32, "kept")
+    rows = logits.shape[0]
+    if u is not None:
+        assert u.shape == (rows, hi - lo)
+    check(L.load().db200_sample_rows_filtered(stream_ptr(), ptr(logits), ptr(u), ptr(idx), ptr(kept), rows,
+                                              logits.stride(0), int(lo), int(hi), float(inv_temp), int(top_k),
+                                              float(top_p)), "db200_sample_rows_filtered")
+    return idx
+
+
+def sample_rows_filtered_at(logits, u, tokens, lo, hi, inv_temp, top_k, top_p, pos_dev, kept=None):
+    """tokens[r, pos + 1] = sample_rows_filtered's id for row r   (pos read on the device)."""
+    L.require_device()
+    _chk(logits, F32, "logits"); _chk(u, F32, "u"); _chk(tokens, I32, "tokens"); _chk(kept, I32, "kept")
+    check(L.load().db200_sample_rows_filtered_at(stream_ptr(), ptr(logits), ptr(u), ptr(tokens), tokens.stride(0),
+                                                 ptr(kept), logits.shape[0], logits.stride(0), int(lo), int(hi),
+                                                 float(inv_temp), int(top_k), float(top_p), ptr(pos_dev)),
+          "db200_sample_rows_filtered_at")
+    return tokens
+
+
 def incr_i32(p, delta=1):
     L.require_device()
     check(L.load().db200_incr_i32(stream_ptr(), ptr(p), int(delta)), "db200_incr_i32")

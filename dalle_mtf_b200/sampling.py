@@ -13,7 +13,8 @@ parameters and the same kernels' numerics as training:
 
 Prompt (text) positions are teacher-forced through the same step function, so there is a single code path; image
 positions are restricted to the image-token id range [text_vocab_size, text_vocab_size + image_vocab_size), matching
-the ids training builds (src/model_fns.py:117-122).  `temperature == 0` (or None) is greedy decoding.
+the ids training builds (src/model_fns.py:117-122).  `temperature == 0` (or None) is greedy decoding; `top_k` /
+`top_p` truncate the image-token distribution (after temperature) before the Gumbel-max draw.
 """
 import torch
 
@@ -86,24 +87,43 @@ class DalleSampler:
         ops.gemm(self.ln, e.W("wout"), self.logit, tokens.shape[0], e.Vpad, e.d, a_mn=False, b_mn=True, bias=e.P("bout"))
         return self.logit
 
-    def _capture(self, B, greedy, inv_t):
+    def _filter(self, top_k, top_p):
+        """(top_k, top_p) as the filtered kernel takes them, or None when neither truncates anything (the unfiltered
+        kernels then run, exactly as without the arguments)."""
+        if top_k is not None and (isinstance(top_k, bool) or int(top_k) != top_k or top_k < 1):
+            raise ValueError(f"top_k must be an integer >= 1 (or None), got {top_k!r}")
+        if top_p is not None and not 0.0 < top_p <= 1.0:
+            raise ValueError(f"top_p must lie in (0, 1] (or be None), got {top_p!r}")
+        k = 0 if top_k is None or top_k >= self.e.image_vocab_size else int(top_k)
+        p = 1.0 if top_p is None else float(top_p)
+        return None if (k == 0 and p == 1.0) else (k, p)
+
+    def _capture(self, B, greedy, inv_t, flt):
         """Two graphs over static buffers: the prompt step (teacher forcing: the next token is already in the token
         matrix) and the sampling step (step -> noise -> Gumbel-max into column pos + 1); both end by advancing pos_dev."""
         e = self.e
-        key = (B, greedy, inv_t)
+        key = (B, greedy, inv_t, flt)
         if getattr(self, "_graph_key", None) == key:
             return
         dev = e.device
         self.tokens = torch.zeros(B, e.S, dtype=I32, device=dev)
         self.pos_dev = torch.zeros(1, dtype=I32, device=dev)
         lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+
+        def sample(logits):
+            if flt is None:
+                ops.sample_rows_at(logits, self.u, self.tokens, lo, hi, inv_t, self.pos_dev)
+            else:
+                ops.sample_rows_filtered_at(logits, self.u, self.tokens, lo, hi, inv_t, *flt, self.pos_dev)
+
         self.u = None if greedy else torch.empty(B, hi - lo, dtype=F32, device=dev)
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):     # eager warm-up: function attributes, tensor maps, lazy allocations
-            self._step_dev(self.tokens)
+            logits = self._step_dev(self.tokens)
             if self.u is not None:
                 self.u.uniform_(1e-9, 1.0)
+            sample(logits)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.g_prompt, self.g_sample = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
@@ -114,22 +134,23 @@ class DalleSampler:
             logits = self._step_dev(self.tokens)
             if self.u is not None:
                 self.u.uniform_(1e-9, 1.0)          # default CUDA generator: graph-safe Philox offsets
-            ops.sample_rows_at(logits, self.u, self.tokens, lo, hi, inv_t, self.pos_dev)
+            sample(logits)
             ops.incr_i32(self.pos_dev, 1)
         self._graph_key = key
 
     @torch.no_grad()
-    def generate_graphed(self, text_ids, temperature=1.0):
+    def generate_graphed(self, text_ids, temperature=1.0, top_k=None, top_p=None):
         """generate() with the per-position step replayed from CUDA graphs (position kept on the device): removes the
         ~45 us of Python / ctypes / launch overhead per kernel that bounds eager generation.  Noise comes from torch's
-        default CUDA generator (seed it with torch.manual_seed)."""
+        default CUDA generator (seed it with torch.manual_seed).  Changing temperature, top_k or top_p re-captures."""
         e = self.e
         B, TL = text_ids.shape
         assert TL == e.text_seq_len, f"expected {e.text_seq_len} text positions, got {TL}"
+        flt = self._filter(top_k, top_p)
         self._alloc(B)
         greedy = temperature is None or temperature <= 0
         inv_t = 1.0 if greedy else 1.0 / float(temperature)
-        self._capture(B, greedy, inv_t)
+        self._capture(B, greedy, inv_t, flt)
         self.tokens.zero_()
         self.tokens[:, :TL] = text_ids
         self.pos_dev.zero_()
@@ -138,12 +159,17 @@ class DalleSampler:
         return self.tokens.clone()
 
     @torch.no_grad()
-    def generate(self, text_ids, temperature=1.0, generator=None, return_logits=False):
+    def generate(self, text_ids, temperature=1.0, generator=None, return_logits=False, top_k=None, top_p=None):
         """text_ids int32 [B, text_seq_len] (device) -> int32 [B, text_seq_len + image_seq_len]: the prompt followed by
-        image_seq_len sampled image-token ids (already offset by text_vocab_size, as in training)."""
+        image_seq_len sampled image-token ids (already offset by text_vocab_size, as in training).
+
+        top_k (>= 1) keeps the k most likely image tokens (all of a tie at the k-th), top_p (in (0, 1]) the smallest
+        set of them whose probability mass after temperature reaches p (nucleus sampling); with both, top-k applies
+        first.  None disables either; no filter at all runs the unfiltered sampler."""
         e = self.e
         B, TL = text_ids.shape
         assert TL == e.text_seq_len, f"expected {e.text_seq_len} text positions, got {TL}"
+        flt = self._filter(top_k, top_p)
         self._alloc(B)
         out = torch.empty(B, e.S, dtype=I32, device=e.device)
         out[:, :TL] = text_ids
@@ -161,6 +187,9 @@ class DalleSampler:
             u = None
             if not greedy:
                 u = torch.empty(B, hi - lo, dtype=F32, device=e.device).uniform_(1e-9, 1.0, generator=generator)
-            ops.sample_rows(logits, u, self.tok, lo, hi, inv_t)
+            if flt is None:
+                ops.sample_rows(logits, u, self.tok, lo, hi, inv_t)
+            else:
+                ops.sample_rows_filtered(logits, u, self.tok, lo, hi, inv_t, *flt)
             out[:, pos + 1] = self.tok
         return (out, kept) if return_logits else out

@@ -359,6 +359,26 @@ int db200_sample_rows_at(db200_stream_t stream, const float* logits, const float
                          long long ld_tokens, int rows, long long ld, int lo, int hi, float inv_temp,
                          const int32_t* pos_dev);
 int db200_incr_i32(db200_stream_t stream, int32_t* p, int delta);
+/* Top-k / nucleus (top-p) filtered sample_rows.  Per row, over x_c = logits[r][lo + c] * inv_temp (c < n = hi - lo):
+ *   top-k (top_k >= 1; 0 = off): keep x_c >= the k-th largest x (counting multiplicity; ties at it are all kept, so
+ *          more than k ids may survive; k >= n keeps everything);
+ *   top-p (0 < top_p <= 1; 1 = off): over the top-k survivors, with w = exp(x - max) and Z = sum w, keep x_c iff the
+ *          mass of the survivors strictly greater than x_c is < top_p * Z (independent of how ties are ordered; the
+ *          maximum is always kept);
+ *   idx[r] = lo + argmax over the kept c of (x_c - log(-log u[r][c])), first index on ties; u NULL = greedy, which
+ *          the filter cannot change.  With the filter off the selection is exactly sample_rows'.
+ * NaN and -inf are never kept; a row with no finite entry gives lo and a kept count of 0; +inf entries, if any, are
+ * the only ones kept.  kept_or_null (int32 [rows]) receives the number of kept ids; the kept set is the top that many
+ * x, so the count identifies it.  Results are bit-reproducible (masses are summed in 64-bit fixed point).
+ * One CTA holds a row: n <= 51 200, larger n returns DB200_E_UNSUPPORTED.  top_k < 0, top_p NaN / <= 0 / > 1,
+ * inv_temp <= 0 and an empty range return DB200_E_INVALID.  The _at variant writes tokens[r * ld_tokens + *pos_dev + 1]
+ * like db200_sample_rows_at. */
+int db200_sample_rows_filtered(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* idx,
+                               int32_t* kept_or_null, int rows, long long ld, int lo, int hi, float inv_temp,
+                               int top_k, float top_p);
+int db200_sample_rows_filtered_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
+                                  long long ld_tokens, int32_t* kept_or_null, int rows, long long ld, int lo, int hi,
+                                  float inv_temp, int top_k, float top_p, const int32_t* pos_dev);
 
 /* Segmented bf16 -> f32 gather (one launch): segment i copies table[3i+2] elements from src + table[3i] to
  * dst + table[3i+1]; `table_dev` is an int64 array in device memory.  ZeRO-1 mode: rebuilds the compact fp32 copy of the

@@ -407,6 +407,39 @@ __global__ void onehot_rows_kernel(const int* __restrict__ idx, float* __restric
   for (int c = threadIdx.x; c < K; c += blockDim.x) y[(long long)r * K + c] = (c == hot) ? 1.f : 0.f;
 }
 
+// ---- prompt prefill hand-off.  Pure copies in 16-byte vectors (8 bf16): one source vector is read once and stored
+// into every replica, so the source traffic does not grow with `rep`.
+// kv_cache_fill: vector c of (b, p, k|v) of qkv [B][P][3][H*dh/8] -> caches [B*rep][S_cache][H*dh/8] at position p.
+__global__ void __launch_bounds__(256)
+kv_cache_fill_kernel(const uint4* __restrict__ qkv, uint4* __restrict__ kc, uint4* __restrict__ vc, int P, int S_cache,
+                     int rep, int n16, long long total) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % n16);
+    long long t = i / n16;
+    const int kv = (int)(t & 1);
+    t >>= 1;
+    const int p = (int)(t % P);
+    const long long b = t / P;
+    const uint4 v = qkv[((b * P + p) * 3 + 1 + kv) * n16 + c];
+    uint4* dst = kv ? vc : kc;
+    for (int r = 0; r < rep; ++r) dst[((b * rep + r) * S_cache + p) * n16 + c] = v;
+  }
+}
+
+// rows_repeat: dst row b * rep + r = src row b (row stride ld16 vectors), d16 vectors per row.
+__global__ void __launch_bounds__(256)
+rows_repeat_kernel(const uint4* __restrict__ src, long long ld16, uint4* __restrict__ dst, int d16, int rep,
+                   long long total) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % d16);
+    const long long b = i / d16;
+    const uint4 v = src[b * ld16 + c];
+    for (int r = 0; r < rep; ++r) dst[(b * rep + r) * d16 + c] = v;
+  }
+}
+
 }  // namespace db200
 
 using namespace db200;
@@ -549,4 +582,40 @@ extern "C" int db200_onehot_rows_f32(db200_stream_t stream_, const int32_t* idx,
   DB200_REQUIRE(idx && y && rows > 0 && K > 0, DB200_E_INVALID, "onehot_rows: bad argument");
   onehot_rows_kernel<<<rows, 256, 0, stream>>>(idx, y, K, offset);
   return check_launch("onehot_rows_kernel");
+}
+
+static unsigned copy_blocks(long long total) {
+  const long long want = (total + 255) / 256, cap = (long long)sm_count() * 16;
+  return (unsigned)(want < cap ? want : cap);
+}
+
+extern "C" int db200_kv_cache_fill(db200_stream_t stream_, const void* qkv, void* k_cache, void* v_cache, int B, int P,
+                                   int H, int dh, int S_cache, int rep) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(qkv && k_cache && v_cache, DB200_E_INVALID, "kv_cache_fill: null pointer");
+  DB200_REQUIRE(B > 0 && P > 0 && H > 0 && dh > 0 && S_cache > 0 && rep >= 1, DB200_E_INVALID,
+                "kv_cache_fill: B %d P %d H %d dh %d S_cache %d rep %d", B, P, H, dh, S_cache, rep);
+  DB200_REQUIRE(P <= S_cache, DB200_E_INVALID, "kv_cache_fill: %d prompt positions exceed the cache's %d", P, S_cache);
+  DB200_REQUIRE((H * dh) % 8 == 0 && aligned16(qkv) && aligned16(k_cache) && aligned16(v_cache), DB200_E_ALIGN,
+                "kv_cache_fill: H*dh %d not a multiple of 8 or unaligned pointer", H * dh);
+  const int n16 = H * dh / 8;
+  const long long total = (long long)B * P * 2 * n16;
+  kv_cache_fill_kernel<<<copy_blocks(total), 256, 0, stream>>>(static_cast<const uint4*>(qkv),
+                                                              static_cast<uint4*>(k_cache),
+                                                              static_cast<uint4*>(v_cache), P, S_cache, rep, n16, total);
+  return check_launch("kv_cache_fill_kernel");
+}
+
+extern "C" int db200_rows_repeat(db200_stream_t stream_, const void* src, long long ld_src, void* dst, int B, int d,
+                                 int rep) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(src && dst, DB200_E_INVALID, "rows_repeat: null pointer");
+  DB200_REQUIRE(B > 0 && d > 0 && rep >= 1 && ld_src >= d, DB200_E_INVALID, "rows_repeat: B %d d %d rep %d ld %lld", B,
+                d, rep, ld_src);
+  DB200_REQUIRE(d % 8 == 0 && ld_src % 8 == 0 && aligned16(src) && aligned16(dst), DB200_E_ALIGN,
+                "rows_repeat: d %d / ld %lld not multiples of 8 or unaligned pointer", d, ld_src);
+  const long long total = (long long)B * (d / 8);
+  rows_repeat_kernel<<<copy_blocks(total), 256, 0, stream>>>(static_cast<const uint4*>(src), ld_src / 8,
+                                                            static_cast<uint4*>(dst), d / 8, rep, total);
+  return check_launch("rows_repeat_kernel");
 }

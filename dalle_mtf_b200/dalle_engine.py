@@ -400,13 +400,14 @@ class DalleEngine:
         return self._drop[kind][i] if self._drop is not None else None
 
     # ------------------------------------------------------------------------------------------ forward
-    def _block_fwd(self, i, x_in, x_out, sv, B):
-        """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x))."""
+    def _block_fwd(self, i, x_in, x_out, sv, B, S=None):
+        """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x)).
+        S: sequence length of the rows (default the model's; prefill runs a shorter prompt)."""
         p = f"l{i}."
         ops.layernorm_fwd(x_in, self.P(p + "ln1_g"), self.P(p + "ln1_b"), sv["ln1"], sv["mean1"], sv["rstd1"],
                           self.ln_eps)
         ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
-        ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, self.S, self.H, self.dh, self.attn_scale,
+        ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
                      dropout=self._site("attn", i))                                     # :290-299
         ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in,
                        dropout=self._site("attn_out", i))                               # :303-314,330
@@ -461,6 +462,59 @@ class DalleEngine:
         ops.gemm(self._bufs["hf"], self.W("wout"), out, T, self.Vpad, self.d, a_mn=False, b_mn=True,
                  bias=self.P("bout"))
         return out.view(B, S, self.Vpad)[:, :, :self.V]
+
+    # ------------------------------------------------------------------------------------------ prompt prefill
+    def _prefill_alloc(self, B, P, rep):
+        """Compact buffers of one prefill: B*P rows, shared by every layer (nothing is kept for a backward pass)."""
+        key = (B, P, rep)
+        if getattr(self, "_pf_key", None) == key:
+            return self._pf
+        dev, d, T = self.device, self.d, B * P
+        e = lambda *shape, dtype=BF16: torch.empty(*shape, dtype=dtype, device=dev)
+        self._pf = {
+            "xs": [e(T, d), e(T, d)],
+            "sv": {"ln1": e(T, d), "mean1": e(T, dtype=F32), "rstd1": e(T, dtype=F32), "qkv": e(T, 3 * d),
+                   "attn": e(T, d), "lse": e(B, self.H, P, dtype=F32), "xmid": e(T, d), "ln2": e(T, d),
+                   "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32), "h1": e(T, 4 * d)},
+            "x_last": e(B * rep, d), "hf": e(B * rep, d), "meanf": e(B * rep, dtype=F32),
+            "rstdf": e(B * rep, dtype=F32), "logits": e(B * rep, self.Vpad, dtype=F32),
+        }
+        self._pf_key = key
+        return self._pf
+
+    def prefill(self, tokens, k_caches, v_caches, rep=1):
+        """Runs a whole prompt, tokens int32 [B, P] (1 <= P < S), through the training forward kernels in one pass
+        and hands it to the decoder: every layer's k / v of positions < P go into k_caches[i] / v_caches[i] (bf16
+        [B*rep, S, H, dh], rows b*rep .. b*rep + rep - 1 all receive prompt b), and the result is the fp32 logits
+        [B*rep, Vpad] of position P for each replica.  No dropout (inference); the training buffers and the state a
+        pending backward() reads are left untouched."""
+        B, P = tokens.shape
+        if not 1 <= P < self.S:
+            raise ValueError(f"prefill: prompt length {P} outside [1, {self.S})")
+        if int(rep) != rep or rep < 1:
+            raise ValueError(f"prefill: rep must be an integer >= 1, got {rep!r}")
+        rep = int(rep)
+        shape = (B * rep, self.S, self.H, self.dh)
+        if len(k_caches) != self.L or len(v_caches) != self.L or \
+                any(tuple(c.shape) != shape for c in list(k_caches) + list(v_caches)):
+            raise ValueError(f"prefill: expected {self.L} k and v caches of shape {shape}")
+        b = self._prefill_alloc(B, P, rep)
+        d = self.d
+        ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), b["xs"][0].view(B, P, d))
+        drop, self._drop = self._drop, None        # restored below: backward() of a preceding forward() reads it
+        try:
+            x_in, x_out = b["xs"]
+            for i in range(self.L):
+                self._block_fwd(i, x_in, x_out, b["sv"], B, S=P)
+                ops.kv_cache_fill(b["sv"]["qkv"], k_caches[i], v_caches[i], P, rep)
+                x_in, x_out = x_out, x_in
+        finally:
+            self._drop = drop
+        ops.rows_repeat(x_in.view(B, P, d)[:, P - 1], b["x_last"], rep)
+        ops.layernorm_fwd(b["x_last"], self.P("lnf_g"), self.P("lnf_b"), b["hf"], b["meanf"], b["rstdf"], self.ln_eps)
+        ops.gemm(b["hf"], self.W("wout"), b["logits"], B * rep, self.Vpad, d, a_mn=False, b_mn=True,
+                 bias=self.P("bout"))
+        return b["logits"]
 
     # ------------------------------------------------------------------------------------------ backward
     def _ln_bwd(self, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, site):

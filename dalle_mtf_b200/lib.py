@@ -118,6 +118,8 @@ _SIGNATURES = {
     "db200_sample_rows_filtered": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_int, c_int, c_f32, c_int, c_f32],
     "db200_sample_rows_filtered_at": [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_i64, c_int, c_int, c_f32, c_int,
                                       c_f32, c_vp],
+    "db200_kv_cache_fill": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
+    "db200_rows_repeat": [c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int],
     "db200_crc32c": [c_vp, c_u64, c_vp],
     "db200_tfrecord_masked_crc": [c_vp, c_u64, c_vp],
     "db200_tfrecord_frame": [c_vp, c_u64, c_vp],

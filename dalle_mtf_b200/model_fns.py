@@ -67,10 +67,17 @@ def load_vae_model(params, device):
                     input_channels=vae_params.get("input_channels") or 3,
                     use_bf16=bool(vae_params.get("use_bf16")),   # bf16 -> wgmma implicit-GEMM convolutions
                     stack_factor=vae_params.get("stack_factor") or 1, device=device)
+    return vae, vae_checkpoint(params)
+
+
+def vae_checkpoint(params):
+    """The VAE checkpoint a DALL-E config names: vae_checkpoint_path, else the latest one under vae_params.model_path
+    (None when there is neither)."""
     ckpt = params.get("vae_checkpoint_path")
     if ckpt is None:
+        vae_params = params["vae_params"]
         ckpt = latest_checkpoint(vae_params["model_path"]) if vae_params.get("model_path") else None
-    return vae, ckpt
+    return ckpt
 
 
 DROPOUT_KEYS = ("embed_dropout", "attention_dropout", "residual_dropout")

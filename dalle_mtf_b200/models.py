@@ -66,6 +66,18 @@ class DALLE:
         text_ids = text_ids.to(device=self.engine.device, dtype=torch.int32).contiguous()
         return self._sampler.generate(text_ids, temperature, generator, top_k=top_k, top_p=top_p)
 
+    def complete(self, text_ids, image_prefix=None, samples_per_prompt=1, temperature=1.0, top_k=None, top_p=None):
+        """Image completion (DalleSampler.complete): text_ids int [B, text_seq_len] plus optionally the first n VAE codes
+        of each image, image_prefix int [B, n] -> int32 [B * samples_per_prompt, text_seq_len + image_seq_len].  The
+        prompt is prefilled in one forward pass; noise comes from torch's default CUDA generator."""
+        from .sampling import DalleSampler
+        if getattr(self, "_sampler", None) is None:
+            self._sampler = DalleSampler(self.engine)
+        text_ids = text_ids.to(device=self.engine.device, dtype=torch.int32).contiguous()
+        if image_prefix is not None:
+            image_prefix = image_prefix.to(device=self.engine.device, dtype=torch.int32).contiguous()
+        return self._sampler.complete(text_ids, image_prefix, samples_per_prompt, temperature, top_k, top_p)
+
 
 class DiscreteVAE:
     def __init__(self, num_tokens, dimensions, convblocks, dim=512, hidden_dim=64, input_channels=3,

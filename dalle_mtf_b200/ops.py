@@ -563,6 +563,30 @@ def sample_rows_filtered_at(logits, u, tokens, lo, hi, inv_temp, top_k, top_p, p
     return tokens
 
 
+def kv_cache_fill(qkv, k_cache, v_cache, P, rep=1):
+    """k_cache[b*rep + r, p] = qkv[b, p, 1], v_cache[b*rep + r, p] = qkv[b, p, 2] for p < P (qkv [B*P, 3*H*dh], caches
+    [B*rep, S_cache, H, dh]); later positions are left as they are."""
+    L.require_device()
+    _chk(qkv, BF16, "qkv"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache")
+    Brep, S_cache, H, dh = k_cache.shape
+    assert v_cache.shape == k_cache.shape and k_cache.is_contiguous() and v_cache.is_contiguous()
+    B = Brep // max(int(rep), 1)
+    assert qkv.is_contiguous() and qkv.numel() == B * P * 3 * H * dh, "qkv must be [B*P, 3*H*dh]"
+    check(L.load().db200_kv_cache_fill(stream_ptr(), ptr(qkv), ptr(k_cache), ptr(v_cache), B, int(P), H, dh, S_cache,
+                                       int(rep)), "db200_kv_cache_fill")
+
+
+def rows_repeat(src, dst, rep=1):
+    """dst[b*rep + r] = src[b] for a [B, d] view src (rows may be strided, e.g. x.view(B, P, d)[:, P - 1])."""
+    L.require_device()
+    _chk(src, BF16, "src"); _chk(dst, BF16, "dst")
+    B, d = src.shape
+    assert dst.is_contiguous() and dst.shape[-1] == d and dst.numel() == B * int(rep) * d
+    check(L.load().db200_rows_repeat(stream_ptr(), ptr(src), src.stride(0), ptr(dst), B, d, int(rep)),
+          "db200_rows_repeat")
+    return dst
+
+
 def incr_i32(p, delta=1):
     L.require_device()
     check(L.load().db200_incr_i32(stream_ptr(), ptr(p), int(delta)), "db200_incr_i32")

@@ -11,7 +11,9 @@ parameters and the same kernels' numerics as training:
                     x = x + a Wo + o_b;  x = x + relu(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows)
   logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
 
-Prompt (text) positions are teacher-forced through the same step function, so there is a single code path; image
+In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
+instead runs the whole prompt (text, optionally followed by the first rows of an image's codes) through the training
+forward kernels in one pass (DalleEngine.prefill) and continues from there with the same sampling step.  Image
 positions are restricted to the image-token id range [text_vocab_size, text_vocab_size + image_vocab_size), matching
 the ids training builds (src/model_fns.py:117-122).  `temperature == 0` (or None) is greedy decoding; `top_k` /
 `top_p` truncate the image-token distribution (after temperature) before the Gumbel-max draw.
@@ -156,6 +158,66 @@ class DalleSampler:
         self.pos_dev.zero_()
         for pos in range(e.S - 1):
             (self.g_prompt if pos + 1 < TL else self.g_sample).replay()
+        return self.tokens.clone()
+
+    @torch.no_grad()
+    def complete(self, text_ids, image_prefix=None, samples_per_prompt=1, temperature=1.0, top_k=None, top_p=None):
+        """Image completion: text_ids int32 [B, text_seq_len] (device) and optionally image_prefix int32 [B, n], the
+        first n (0 < n < image_seq_len) VAE codes in [0, image_vocab_size) in the VAE's row-major token order (e.g.
+        vae.encode_tokens(img)[:, :n]).  Returns int32 [B * samples_per_prompt, text_seq_len + image_seq_len]: row
+        b * samples_per_prompt + r is sample r of prompt b, the prompt (prefix offset by text_vocab_size) followed by
+        sampled image-token ids.
+
+        The whole prompt (P = text_seq_len + n positions) runs once per distinct prompt as one batched forward pass
+        (DalleEngine.prefill) that fills every replica's K/V cache; token P is drawn from its logits and the remaining
+        positions replay the captured sampling step of generate_graphed.  temperature, top_k and top_p mean what they
+        mean for generate(); noise comes from torch's default CUDA generator (seed it with torch.manual_seed)."""
+        e = self.e
+        if not torch.is_tensor(text_ids) or text_ids.dim() != 2 or text_ids.shape[1] != e.text_seq_len:
+            raise ValueError(f"text_ids must be [B, {e.text_seq_len}], got "
+                             f"{tuple(text_ids.shape) if torch.is_tensor(text_ids) else type(text_ids).__name__}")
+        B, TL = text_ids.shape
+        rep = samples_per_prompt
+        if isinstance(rep, bool) or int(rep) != rep or rep < 1:
+            raise ValueError(f"samples_per_prompt must be an integer >= 1, got {rep!r}")
+        rep = int(rep)
+        n = 0
+        if image_prefix is not None:
+            if not torch.is_tensor(image_prefix) or image_prefix.dim() != 2 or image_prefix.shape[0] != B:
+                raise ValueError(f"image_prefix must be [{B}, n]")
+            n = image_prefix.shape[1]
+            if not 0 < n < e.image_seq_len:
+                raise ValueError(f"image_prefix length {n} outside (0, {e.image_seq_len})")
+            if int(image_prefix.min()) < 0 or int(image_prefix.max()) >= e.image_vocab_size:
+                raise ValueError(f"image_prefix codes must lie in [0, {e.image_vocab_size})")
+        flt = self._filter(top_k, top_p)
+        P, R = TL + n, B * rep
+        self._alloc(R)
+        greedy = temperature is None or temperature <= 0
+        inv_t = 1.0 if greedy else 1.0 / float(temperature)
+        # capture before the prefill (the capture's warm-up step writes the caches), and without moving the default
+        # generator (its warm-up draws noise): a seeded call then samples the same whether or not it had to capture
+        rng = torch.cuda.get_rng_state(e.device)
+        self._capture(R, greedy, inv_t, flt)
+        torch.cuda.set_rng_state(rng, e.device)
+        prompt = torch.empty(B, P, dtype=I32, device=e.device)
+        prompt[:, :TL] = text_ids
+        if n:
+            prompt[:, TL:] = image_prefix.to(device=e.device, dtype=I32) + e.text_vocab_size
+        logits = e.prefill(prompt, self.kc, self.vc, rep)
+        lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+        if self.u is not None:
+            self.u.uniform_(1e-9, 1.0)
+        if flt is None:
+            ops.sample_rows(logits, self.u, self.tok, lo, hi, inv_t)
+        else:
+            ops.sample_rows_filtered(logits, self.u, self.tok, lo, hi, inv_t, *flt)
+        self.tokens.zero_()
+        self.tokens[:, :P] = prompt.repeat_interleave(rep, 0)
+        self.tokens[:, P] = self.tok
+        self.pos_dev.fill_(P)
+        for _ in range(P, e.S - 1):
+            self.g_sample.replay()
         return self.tokens.clone()
 
     @torch.no_grad()

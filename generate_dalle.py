@@ -1,0 +1,201 @@
+"""Image generation from a trained DALL-E run: loads the config and checkpoints the way train_dalle.py does, samples
+image tokens for each caption (optionally completing the top rows of a prompt image) and decodes them with the VAE.
+
+    python generate_dalle.py --model dalle_example_b200 --out DIR (--captions FILE | --caption_ids FILE.npy)
+        [--checkpoint PATH] [--image_prompt IMG ...] [--prompt_rows R] [--samples_per_prompt N]
+        [--temperature T] [--top_k K] [--top_p P] [--batch_size B] [--seed S]
+
+Writes DIR/{caption:05d}_{sample:02d}.png and DIR/tokens.npy (int32 [captions * samples_per_prompt, S]: caption ids,
+then image-token ids offset by text_vocab_size, as in training).  One process, one GPU.
+"""
+import argparse
+import os
+import sys
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+
+from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
+from dalle_mtf_b200.model_fns import vae_checkpoint
+from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
+
+PADDING_ID = 50257   # GPT-2 vocabulary + <|padding|> (src/data/tokenizer_utils.py), what training pads captions with
+
+
+def parse_args(argv=None):
+    p = argparse.ArgumentParser(description="Sample images from a trained DALL-E checkpoint.")
+    p.add_argument("--model", required=True, help="DALL-E config name (configs/NAME.json) or path to a .json file.")
+    p.add_argument("--out", required=True, help="Output directory for the PNGs and tokens.npy.")
+    src = p.add_mutually_exclusive_group(required=True)
+    src.add_argument("--captions", help="Text file, one caption per line (needs local GPT-2 BPE files).")
+    src.add_argument("--caption_ids", help=".npy file of token ids, [N, <= text_seq_len] (or [L] for one caption).")
+    p.add_argument("--checkpoint", help="DALL-E checkpoint (default: the latest model.ckpt-N.pt under model_path).")
+    p.add_argument("--image_prompt", nargs="+", help="Prompt image(s): one per caption, or one for all captions.")
+    p.add_argument("--prompt_rows", type=int, help="Rows of the prompt image's token grid to keep (0 < R < grid side).")
+    p.add_argument("--samples_per_prompt", type=int, default=1)
+    p.add_argument("--temperature", type=float, default=1.0, help="0 = greedy.")
+    p.add_argument("--top_k", type=int)
+    p.add_argument("--top_p", type=float)
+    p.add_argument("--batch_size", type=int, help="Captions per sampling call (default: predict_batch_size).")
+    p.add_argument("--seed", type=int, default=0)
+    args = p.parse_args(argv)
+    if (args.image_prompt is None) != (args.prompt_rows is None):
+        p.error("--image_prompt and --prompt_rows go together")
+    if args.samples_per_prompt < 1:
+        p.error("--samples_per_prompt must be >= 1")
+    if args.batch_size is not None and args.batch_size < 1:
+        p.error("--batch_size must be >= 1")
+    if args.top_k is not None and args.top_k < 1:
+        p.error("--top_k must be >= 1")
+    if args.top_p is not None and not 0.0 < args.top_p <= 1.0:
+        p.error("--top_p must lie in (0, 1]")
+    return args
+
+
+def load_params(model):
+    """The config as train_dalle.py loads it, with the VAE's config under vae_params."""
+    params = fetch_model_params(model)
+    if (params["model_type"] or "").lower() != "dalle":
+        raise SystemExit(f"{model}: model_type {params['model_type']!r} is not a DALL-E config")
+    params["vae_params"] = fetch_model_params(params["vae_model"])
+    return params
+
+
+def find_checkpoints(params, checkpoint=None):
+    """(DALL-E checkpoint, VAE checkpoint) paths; a clear error when either is missing."""
+    ckpt = checkpoint or latest_checkpoint(params["model_path"])
+    if ckpt is None or not os.path.exists(local_path(ckpt)):
+        raise SystemExit(f"no DALL-E checkpoint: {checkpoint or 'no model.ckpt-N.pt under ' + str(params['model_path'])}"
+                         " (train with train_dalle.py or pass --checkpoint)")
+    vae_ckpt = vae_checkpoint(params)
+    if vae_ckpt is None or not os.path.exists(local_path(vae_ckpt)):
+        where = vae_ckpt or f"no model.ckpt-N.pt under {params['vae_params']['model_path']}"
+        raise SystemExit(f"no VAE checkpoint: {where} (set vae_checkpoint_path or train the VAE with train_vae_tf.py)")
+    return local_path(ckpt), local_path(vae_ckpt)
+
+
+def pad_captions(rows, text_seq_len, text_vocab_size):
+    """Captions (lists of ids) -> int32 [N, text_seq_len], padded / truncated as in training."""
+    if len(rows) == 0:
+        raise SystemExit("no captions given")
+    out = np.stack([truncate_or_pad_label(r, text_seq_len, PADDING_ID) for r in rows])
+    if out.min() < 0 or out.max() >= text_vocab_size:
+        raise SystemExit(f"caption ids must lie in [0, {text_vocab_size})")
+    return out
+
+
+def load_caption_ids(path, text_seq_len, text_vocab_size):
+    ids = np.load(path)
+    if ids.ndim == 1:
+        ids = ids[None]
+    if ids.ndim != 2 or not np.issubdtype(ids.dtype, np.integer):
+        raise SystemExit(f"{path}: expected an integer array [N, <= {text_seq_len}], got {ids.dtype} {ids.shape}")
+    return pad_captions(list(ids), text_seq_len, text_vocab_size)
+
+
+def encode_captions(lines, tokenizer, text_seq_len, text_vocab_size):
+    try:
+        rows = [tokenizer.encode(line) for line in lines]
+    except NotImplementedError as err:
+        raise SystemExit(f"cannot tokenise captions ({err}); pass pre-tokenised ids with --caption_ids") from None
+    return pad_captions(rows, text_seq_len, text_vocab_size)
+
+
+def token_grid_side(params):
+    """Side of the VAE's token grid: image_size / stack_factor / 2^len(convblocks)."""
+    vp = params["vae_params"]
+    convblocks = vp.get("convblocks") or [(3, 64), (3, 128), (3, 256)]
+    return params["dataset"]["image_size"] // (vp.get("stack_factor") or 1) // (2 ** len(convblocks))
+
+
+def prefix_length(params, prompt_rows):
+    """Number of prompt-image tokens kept by --prompt_rows R: R whole rows of the hw x hw grid, 0 < R < hw."""
+    hw = token_grid_side(params)
+    if not 0 < prompt_rows < hw:
+        raise SystemExit(f"--prompt_rows must lie in (0, {hw}) for a {hw}x{hw} token grid, got {prompt_rows}")
+    return prompt_rows * hw
+
+
+def to_uint8(img):
+    """fp32 decoder output in [-1, 1] -> uint8 (values outside are clipped)."""
+    return np.round(np.clip(img, -1.0, 1.0) * 127.5 + 127.5).astype(np.uint8)
+
+
+def encode_image_prompts(paths, params, vae, device):
+    """Image files -> VAE codes int32 [len(paths), image_seq_len] through the training input transform."""
+    from dalle_mtf_b200.data_pipeline import device_stage, host_stage
+    with ThreadPoolExecutor(4) as pool:
+        hb = host_stage(paths, params, labeled=False, tfrecords=False, pool=pool)
+    return vae.encode_tokens(device_stage(hb, params, device)).clone()
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        raise SystemExit("generate_dalle.py is a single process on one GPU; do not launch it with torchrun")
+    params = load_params(args.model)
+    ckpt, vae_ckpt = find_checkpoints(params, args.checkpoint)
+    tl, tv, iv = params["text_seq_len"], params["text_vocab_size"], params["image_vocab_size"]
+    if args.caption_ids:
+        captions = load_caption_ids(args.caption_ids, tl, tv)
+    else:
+        from dalle_mtf_b200.tokenizer import get_tokenizer
+        with open(args.captions) as f:
+            lines = [ln.rstrip("\n") for ln in f if ln.strip()]
+        captions = encode_captions(lines, get_tokenizer(params["tokenizer"]), tl, tv)
+    N = len(captions)
+    n = 0
+    if args.image_prompt:
+        if len(args.image_prompt) not in (1, N):
+            raise SystemExit(f"{len(args.image_prompt)} prompt images for {N} captions: give one per caption or one")
+        n = prefix_length(params, args.prompt_rows)
+
+    import torch
+    from PIL import Image
+    from dalle_mtf_b200 import lib as L
+    from dalle_mtf_b200.dalle_engine import DalleEngine
+    from dalle_mtf_b200.model_fns import load_vae_model
+    from dalle_mtf_b200.sampling import DalleSampler
+
+    L.require_device()
+    device = torch.device("cuda", torch.cuda.current_device())
+    vae, _ = load_vae_model(params, device)
+    state = load_checkpoint(vae_ckpt)
+    vae.load_params({k[len("vae/"):]: v for k, v in state.items() if k.startswith("vae/")})
+    if vae.K < iv:
+        raise SystemExit(f"VAE has {vae.K} codes but image_vocab_size is {iv}: a sampled id would index past the "
+                         "codebook")
+    eng = DalleEngine(params["n_embd"], params["n_layers"], params["n_heads"], tv, iv, tl, vae.image_seq_len,
+                      device=device)
+    state = load_checkpoint(ckpt)
+    eng.load_params({k: v for k, v in state.items()
+                     if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})
+    del state
+    prefix = None
+    if n:
+        prefix = encode_image_prompts(args.image_prompt, params, vae, device)[:, :n]
+        if len(prefix) == 1:
+            prefix = prefix.expand(N, n)
+    sampler = DalleSampler(eng)
+    torch.manual_seed(args.seed)
+    rep = args.samples_per_prompt
+    bs = args.batch_size or params["predict_batch_size"] or 1
+    os.makedirs(args.out, exist_ok=True)
+    all_tokens = []
+    for c0 in range(0, N, bs):
+        text = torch.from_numpy(captions[c0:c0 + bs]).to(device)
+        pre = prefix[c0:c0 + bs].contiguous() if prefix is not None else None
+        toks = sampler.complete(text, pre, samples_per_prompt=rep, temperature=args.temperature, top_k=args.top_k,
+                                top_p=args.top_p)
+        imgs = to_uint8(vae.decode_tokens(toks[:, tl:].contiguous(), offset=tv).cpu().numpy())
+        for j, im in enumerate(imgs):
+            c, s = c0 + j // rep, j % rep
+            Image.fromarray(im if im.shape[-1] == 3 else im[..., 0]).save(
+                os.path.join(args.out, f"{c:05d}_{s:02d}.png"))
+        all_tokens.append(toks.cpu().numpy())
+    np.save(os.path.join(args.out, "tokens.npy"), np.concatenate(all_tokens).astype(np.int32))
+    print(f"wrote {N * rep} images to {args.out}")
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])

@@ -379,6 +379,20 @@ int db200_sample_rows_filtered(db200_stream_t stream, const float* logits, const
 int db200_sample_rows_filtered_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
                                   long long ld_tokens, int32_t* kept_or_null, int rows, long long ld, int lo, int hi,
                                   float inv_temp, int top_k, float top_p, const int32_t* pos_dev);
+/* Prompt prefill hand-off: a whole prompt runs through the training forward kernels at sequence length P, and these
+ * copies turn its results into the decoder's state (bandwidth-bound, 16-byte vector accesses).
+ *   kv_cache_fill : qkv bf16 [B][P][3][H][dh] (the fused q|k|v GEMM output attn_causal_fwd reads) -> caches bf16
+ *                   [B*rep][S_cache][H][dh] (the attn_decode layout): for b < B, p < P, r < rep
+ *                   k_cache[b*rep + r][p] = qkv[b][p][1], v_cache[b*rep + r][p] = qkv[b][p][2]; positions >= P are
+ *                   not written.  P > S_cache, rep < 1 or a non-positive size -> DB200_E_INVALID; H*dh not a multiple
+ *                   of 8 or an unaligned pointer -> DB200_E_ALIGN.
+ *   rows_repeat   : dst bf16 [B*rep][d] row b*rep + r = src row b, src rows ld_src elements apart (e.g. the last prompt
+ *                   position of a [B][P][d] residual stream: src = x + (P-1)*d, ld_src = P*d).  d and ld_src must be
+ *                   multiples of 8 and the pointers 16-byte aligned (DB200_E_ALIGN). */
+int db200_kv_cache_fill(db200_stream_t stream, const void* qkv_bf16, void* k_cache_bf16, void* v_cache_bf16, int B,
+                        int P, int H, int dh, int S_cache, int rep);
+int db200_rows_repeat(db200_stream_t stream, const void* src_bf16, long long ld_src, void* dst_bf16, int B, int d,
+                      int rep);
 
 /* Segmented bf16 -> f32 gather (one launch): segment i copies table[3i+2] elements from src + table[3i] to
  * dst + table[3i+1]; `table_dev` is an int64 array in device memory.  ZeRO-1 mode: rebuilds the compact fp32 copy of the

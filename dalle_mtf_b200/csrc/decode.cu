@@ -8,6 +8,8 @@
 //                  fp32 scores / softmax, P rounded to bf16 for the PV product (same policy as attn.cu)
 //   sample_rows    idx = lo + argmax_{lo<=c<hi}(logits[c] * inv_temp + gumbel(u[c-lo]))   (first maximum; u NULL = greedy)
 //   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
+//   sample_rows_guided     either of the two over the classifier-free-guidance mix u + s (c - u) of a conditional
+//                          and an unconditional row (the <true> instantiations); the draw goes to both rows' tokens
 //   onehot_rows    y[r, idx[r]-offset] = 1, 0 elsewhere (codebook lookup input for the VAE decoder, vae_tf/models.py:127)
 #include "common.cuh"
 #include "ptx.cuh"
@@ -144,18 +146,30 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
 // filter off it selects exactly what sample_rows_kernel selects.
 __device__ __forceinline__ float gumbel_perturb(float x, float u) { return x + -logf(-logf(u)); }
 
+// Classifier-free guidance: the combined logit u + s (c - u) of a conditional value c and an unconditional value u,
+// rounded op by op (no FMA contraction), so a float32 host computation reproduces it bit for bit.
+__device__ __forceinline__ float guided_logit(float c, float u, float s) {
+  return __fadd_rn(u, __fmul_rn(s, __fsub_rn(c, u)));
+}
+
+// GUIDED: logits holds 2 * rows rows, the conditional ones first; row r's value of id c is guided_logit(row r,
+// row rows + r, gscale), the noise has one row per pair, and the draw goes to column col of token rows r and rows + r.
+// GUIDED = false is the plain sampler (rows and gscale unused).
+template <bool GUIDED>
 __global__ void __launch_bounds__(256)
 sample_rows_kernel(const float* __restrict__ logits, const float* __restrict__ u, int* __restrict__ idx, long long ld,
-                   int lo, int hi, float inv_temp, const int* __restrict__ pos_dev, long long ld_idx) {
+                   int lo, int hi, float inv_temp, const int* __restrict__ pos_dev, long long ld_idx, int rows,
+                   float gscale) {
   __shared__ float bv[8];
   __shared__ int bi[8];
   const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* row = logits + (long long)r * ld;
+  const float* urow = GUIDED ? row + (long long)rows * ld : nullptr;
   const int n = hi - lo;
   float best = -INFINITY;
   int arg = 0x7fffffff;
   for (int c = tid; c < n; c += 256) {
-    float x = row[lo + c] * inv_temp;
+    float x = (GUIDED ? guided_logit(row[lo + c], urow[lo + c], gscale) : row[lo + c]) * inv_temp;
     if (u) x = gumbel_perturb(x, u[(long long)r * n + c]);
     if (x > best || (x == best && c < arg)) { best = x; arg = c; }
   }
@@ -170,9 +184,16 @@ sample_rows_kernel(const float* __restrict__ logits, const float* __restrict__ u
   if (tid == 0) {
     for (int w = 1; w < 8; ++w)
       if (bv[w] > best || (bv[w] == best && bi[w] < arg)) { best = bv[w]; arg = bi[w]; }
-    // pos_dev != NULL (graph replay): the sample is the token of position *pos_dev + 1 of the [rows][ld_idx] matrix
-    int* dst = pos_dev ? idx + r * ld_idx + (*pos_dev + 1) : idx + r;
-    *dst = lo + (arg == 0x7fffffff ? 0 : arg);  // all -inf / NaN row: first allowed id
+    const int id = lo + (arg == 0x7fffffff ? 0 : arg);  // all -inf / NaN row: first allowed id
+    if (GUIDED) {
+      const long long col = pos_dev ? *pos_dev + 1 : 0;
+      idx[r * ld_idx + col] = id;
+      idx[(rows + r) * ld_idx + col] = id;
+    } else {
+      // pos_dev != NULL (graph replay): the sample is the token of position *pos_dev + 1 of the [rows][ld_idx] matrix
+      int* dst = pos_dev ? idx + r * ld_idx + (*pos_dev + 1) : idx + r;
+      *dst = id;
+    }
   }
 }
 
@@ -248,10 +269,12 @@ __device__ __forceinline__ unsigned long long sf_mass(uint32_t k, float xmax) {
   return __float2ull_rn(expf(sf_value(k) - xmax) * 0x1p46f);  // w in (0, 1] -> [0, 2^46]
 }
 
+// GUIDED: the pair layout of sample_rows_kernel<true>; kept[r] counts the kept ids of pair r.
+template <bool GUIDED>
 __global__ void __launch_bounds__(SF_THREADS)
 sample_rows_filtered_kernel(const float* __restrict__ logits, const float* __restrict__ u, int* __restrict__ idx,
                             int* __restrict__ kept, long long ld, int lo, int hi, float inv_temp, int top_k, float top_p,
-                            const int* __restrict__ pos_dev, long long ld_idx) {
+                            const int* __restrict__ pos_dev, long long ld_idx, int rows, float gscale) {
   extern __shared__ uint32_t keys[];
   __shared__ uint32_t mlo[SF_NONE + 1], mhi[SF_NONE + 1];  // per-bin mass = mhi * 2^32 + mlo (no 64-bit smem atomics)
   __shared__ uint32_t cnt[SF_NONE + 1];
@@ -263,11 +286,12 @@ sample_rows_filtered_kernel(const float* __restrict__ logits, const float* __res
   __shared__ int bi[SF_WARPS];
   const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* row = logits + (long long)r * ld;
+  const float* urow = GUIDED ? row + (long long)rows * ld : nullptr;
   const int n = hi - lo;
 
   uint32_t nv = 0, ninf = 0, kmax = 0;
   for (int c = tid; c < n; c += SF_THREADS) {
-    const uint32_t k = sf_key(row[lo + c] * inv_temp);
+    const uint32_t k = sf_key((GUIDED ? guided_logit(row[lo + c], urow[lo + c], gscale) : row[lo + c]) * inv_temp);
     keys[c] = k;
     nv += k != 0;
     ninf += k == SF_KEY_PINF;
@@ -393,8 +417,15 @@ sample_rows_filtered_kernel(const float* __restrict__ logits, const float* __res
   if (tid == 0) {
     for (int w = 1; w < SF_WARPS; ++w)
       if (bv[w] > best || (bv[w] == best && bi[w] < arg)) { best = bv[w]; arg = bi[w]; }
-    int* dst = pos_dev ? idx + r * ld_idx + (*pos_dev + 1) : idx + r;
-    *dst = lo + (arg == 0x7fffffff ? 0 : arg);  // no finite id: first allowed id
+    const int id = lo + (arg == 0x7fffffff ? 0 : arg);  // no finite id: first allowed id
+    if (GUIDED) {
+      const long long col = pos_dev ? *pos_dev + 1 : 0;
+      idx[r * ld_idx + col] = id;
+      idx[(rows + r) * ld_idx + col] = id;
+    } else {
+      int* dst = pos_dev ? idx + r * ld_idx + (*pos_dev + 1) : idx + r;
+      *dst = id;
+    }
     if (kept) kept[r] = (int)nk;
   }
 }
@@ -523,7 +554,7 @@ extern "C" int db200_sample_rows(db200_stream_t stream_, const float* logits, co
   DB200_REQUIRE(rows > 0 && lo >= 0 && hi > lo && hi <= ld, DB200_E_INVALID, "sample_rows: rows %d range [%d,%d) ld %lld",
                 rows, lo, hi, ld);
   DB200_REQUIRE(inv_temp > 0.f, DB200_E_INVALID, "sample_rows: inv_temp must be positive");
-  sample_rows_kernel<<<rows, 256, 0, stream>>>(logits, u_or_null, idx, ld, lo, hi, inv_temp, nullptr, 1);
+  sample_rows_kernel<false><<<rows, 256, 0, stream>>>(logits, u_or_null, idx, ld, lo, hi, inv_temp, nullptr, 1, 0, 0.f);
   return check_launch("sample_rows_kernel");
 }
 
@@ -535,13 +566,16 @@ extern "C" int db200_sample_rows_at(db200_stream_t stream_, const float* logits,
   DB200_REQUIRE(logits && tokens && pos_dev, DB200_E_INVALID, "sample_rows_at: null pointer");
   DB200_REQUIRE(rows > 0 && lo >= 0 && hi > lo && hi <= ld && inv_temp > 0.f, DB200_E_INVALID,
                 "sample_rows_at: rows %d range [%d,%d) ld %lld", rows, lo, hi, ld);
-  sample_rows_kernel<<<rows, 256, 0, stream>>>(logits, u_or_null, tokens, ld, lo, hi, inv_temp, pos_dev, ld_tokens);
+  sample_rows_kernel<false><<<rows, 256, 0, stream>>>(logits, u_or_null, tokens, ld, lo, hi, inv_temp, pos_dev,
+                                                      ld_tokens, 0, 0.f);
   return check_launch("sample_rows_kernel");
 }
 
+// guided: rows pairs, logits [2 * rows][ld] (sample_rows_kernel<true>)
 static int sample_rows_filtered_launch(cudaStream_t stream, const float* logits, const float* u, int32_t* idx,
                                        int32_t* kept, int rows, long long ld, int lo, int hi, float inv_temp, int top_k,
-                                       float top_p, const int32_t* pos_dev, long long ld_idx) {
+                                       float top_p, const int32_t* pos_dev, long long ld_idx, bool guided = false,
+                                       float gscale = 0.f) {
   DB200_REQUIRE(rows > 0 && lo >= 0 && hi > lo && hi <= ld, DB200_E_INVALID,
                 "sample_rows_filtered: rows %d range [%d,%d) ld %lld", rows, lo, hi, ld);
   DB200_REQUIRE(inv_temp > 0.f, DB200_E_INVALID, "sample_rows_filtered: inv_temp must be positive");
@@ -550,11 +584,19 @@ static int sample_rows_filtered_launch(cudaStream_t stream, const float* logits,
                 (double)top_p);
   DB200_REQUIRE(hi - lo <= SF_MAX_N, DB200_E_UNSUPPORTED, "sample_rows_filtered: %d ids exceed the %d one CTA holds",
                 hi - lo, SF_MAX_N);
-  static const cudaError_t attr = cudaFuncSetAttribute(sample_rows_filtered_kernel,
+  static const cudaError_t attr = cudaFuncSetAttribute(sample_rows_filtered_kernel<false>,
                                                        cudaFuncAttributeMaxDynamicSharedMemorySize, SF_SMEM_BYTES);
+  static const cudaError_t attr_g = cudaFuncSetAttribute(sample_rows_filtered_kernel<true>,
+                                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SF_SMEM_BYTES);
   DB200_CUDA(attr);
-  sample_rows_filtered_kernel<<<rows, SF_THREADS, (size_t)(hi - lo) * sizeof(uint32_t), stream>>>(
-      logits, u, idx, kept, ld, lo, hi, inv_temp, top_k, top_p, pos_dev, ld_idx);
+  DB200_CUDA(attr_g);
+  const size_t smem = (size_t)(hi - lo) * sizeof(uint32_t);
+  if (guided)
+    sample_rows_filtered_kernel<true><<<rows, SF_THREADS, smem, stream>>>(logits, u, idx, kept, ld, lo, hi, inv_temp,
+                                                                          top_k, top_p, pos_dev, ld_idx, rows, gscale);
+  else
+    sample_rows_filtered_kernel<false><<<rows, SF_THREADS, smem, stream>>>(logits, u, idx, kept, ld, lo, hi, inv_temp,
+                                                                           top_k, top_p, pos_dev, ld_idx, 0, 0.f);
   return check_launch("sample_rows_filtered_kernel");
 }
 
@@ -574,6 +616,28 @@ extern "C" int db200_sample_rows_filtered_at(db200_stream_t stream_, const float
   DB200_REQUIRE(logits && tokens && pos_dev, DB200_E_INVALID, "sample_rows_filtered_at: null pointer");
   return sample_rows_filtered_launch(static_cast<cudaStream_t>(stream_), logits, u_or_null, tokens, kept_or_null, rows,
                                      ld, lo, hi, inv_temp, top_k, top_p, pos_dev, ld_tokens);
+}
+
+// classifier-free guidance over `rows` (conditional, unconditional) pairs; the unfiltered kernel when no filter applies
+extern "C" int db200_sample_rows_guided(db200_stream_t stream_, const float* logits, long long ld,
+                                        const float* u_or_null, int32_t* tokens, long long ld_tokens,
+                                        int32_t* kept_or_null, int rows, int lo, int hi, float inv_temp,
+                                        float guidance_scale, int top_k, float top_p, const int32_t* pos_dev_or_null) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(logits && tokens, DB200_E_INVALID, "sample_rows_guided: null pointer");
+  DB200_REQUIRE(ld_tokens > 0, DB200_E_INVALID, "sample_rows_guided: ld_tokens %lld", ld_tokens);
+  DB200_REQUIRE(isfinite(guidance_scale) && guidance_scale >= 0.f, DB200_E_INVALID,
+                "sample_rows_guided: guidance_scale %g must be finite and >= 0", (double)guidance_scale);
+  if (top_k != 0 || top_p != 1.f)
+    return sample_rows_filtered_launch(stream, logits, u_or_null, tokens, kept_or_null, rows, ld, lo, hi, inv_temp,
+                                       top_k, top_p, pos_dev_or_null, ld_tokens, true, guidance_scale);
+  DB200_REQUIRE(rows > 0 && lo >= 0 && hi > lo && hi <= ld, DB200_E_INVALID,
+                "sample_rows_guided: rows %d range [%d,%d) ld %lld", rows, lo, hi, ld);
+  DB200_REQUIRE(inv_temp > 0.f, DB200_E_INVALID, "sample_rows_guided: inv_temp must be positive");
+  DB200_REQUIRE(!kept_or_null, DB200_E_INVALID, "sample_rows_guided: kept counts need an active top_k / top_p filter");
+  sample_rows_kernel<true><<<rows, 256, 0, stream>>>(logits, u_or_null, tokens, ld, lo, hi, inv_temp, pos_dev_or_null,
+                                                     ld_tokens, rows, guidance_scale);
+  return check_launch("sample_rows_kernel");
 }
 
 extern "C" int db200_onehot_rows_f32(db200_stream_t stream_, const int32_t* idx, float* y, int rows, int K,

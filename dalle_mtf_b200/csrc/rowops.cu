@@ -189,6 +189,24 @@ __global__ void assemble_tokens_kernel(const int* __restrict__ text, const int* 
   out[i] = t < Tt ? text[b * Tt + t] : img[b * Ti + (t - Tt)] + offset;
 }
 
+// the same with caption dropout: row b's text positions all become `pad` when the Philox word of global sequence index
+// e = dr.row0 + b (elementwise layout with cols = 1: block e >> 2, word e & 3) is below dr.threshold
+__global__ void assemble_tokens_drop_kernel(const int* __restrict__ text, const int* __restrict__ img,
+                                            int* __restrict__ out, int B, int Tt, int Ti, int offset, int pad,
+                                            const db200_dropout dr) {
+  const int S = Tt + Ti;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * S) return;
+  const int b = i / S, t = i - b * S;
+  if (t < Tt) {
+    const uint4 words = dropout_block(dr, dropout_elem_block(dr, b, 1, 0));
+    const bool dropped = uint4_word(words, (int)((dr.row0 + b) & 3)) < dr.threshold;
+    out[i] = dropped ? pad : text[b * Tt + t];
+  } else {
+    out[i] = img[b * Ti + (t - Tt)] + offset;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ LayerNorm
 // One warp per row; the row lives in registers (NCH 16-byte chunks per lane, d = NCH * 256).
 template <int NCH>
@@ -703,6 +721,23 @@ extern "C" int db200_assemble_tokens(db200_stream_t stream_, const int32_t* text
   assemble_tokens_kernel<<<(n + 255) / 256, 256, 0, stream>>>(text_ids, image_idx, tokens, B, text_len, image_len,
                                                             image_offset);
   return check_launch("assemble_tokens_kernel");
+}
+
+extern "C" int db200_assemble_tokens_ex(db200_stream_t stream_, const int32_t* text_ids, const int32_t* image_idx,
+                                        int32_t* tokens, int B, int text_len, int image_len, int image_offset,
+                                        int32_t pad_id, const db200_dropout* caption_drop) {
+  if (!dropout_active(caption_drop))
+    return db200_assemble_tokens(stream_, text_ids, image_idx, tokens, B, text_len, image_len, image_offset);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(B > 0 && text_len >= 0 && image_len >= 0 && text_len + image_len > 0 && tokens &&
+                    (text_len == 0 || text_ids) && (image_len == 0 || image_idx),
+                DB200_E_INVALID, "assemble_tokens_ex: bad arguments");
+  DB200_REQUIRE(pad_id >= 0 && caption_drop->row0 >= 0, DB200_E_INVALID, "assemble_tokens_ex: pad_id %d row0 %lld",
+                pad_id, (long long)caption_drop->row0);
+  const int n = B * (text_len + image_len);
+  assemble_tokens_drop_kernel<<<(n + 255) / 256, 256, 0, stream>>>(text_ids, image_idx, tokens, B, text_len, image_len,
+                                                                  image_offset, pad_id, *caption_drop);
+  return check_launch("assemble_tokens_drop_kernel");
 }
 
 extern "C" int db200_layernorm_fwd(db200_stream_t stream_, const void* x, const float* g, const float* b, void* y,

@@ -43,6 +43,7 @@ class Dropout(ctypes.Structure):
 
 DROPOUT_ELEMENTWISE, DROPOUT_ATTENTION = 0, 1
 SITE_WTE, SITE_WPE = 0, 1
+SITE_CAPTION = 0xFFFFFFFF   # caption dropout (db200_assemble_tokens_ex): one decision per sequence
 
 
 def dropout_site_attn(layer):
@@ -95,6 +96,8 @@ _SIGNATURES = {
                            ctypes.POINTER(Dropout), ctypes.POINTER(Dropout)],
     "db200_dropout_mask": [c_vp, ctypes.POINTER(Dropout), c_int, c_i64, c_i64, c_i64, c_vp],
     "db200_assemble_tokens": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
+    "db200_assemble_tokens_ex": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, ctypes.c_int32,
+                                 ctypes.POINTER(Dropout)],
     "db200_shift_labels": [c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_layernorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
     "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
@@ -118,6 +121,8 @@ _SIGNATURES = {
     "db200_sample_rows_filtered": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_int, c_int, c_f32, c_int, c_f32],
     "db200_sample_rows_filtered_at": [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_int, c_i64, c_int, c_int, c_f32, c_int,
                                       c_f32, c_vp],
+    "db200_sample_rows_guided": [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_f32, c_f32, c_int,
+                                 c_f32, c_vp],
     "db200_kv_cache_fill": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_rows_repeat": [c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int],
     "db200_crc32c": [c_vp, c_u64, c_vp],

@@ -96,12 +96,30 @@ def dropout_rates(params):
     return tuple(rates)
 
 
+def caption_dropout(params):
+    """(rate, padding_id) of the config's caption dropout: in mode "train", each sequence's caption is replaced by
+    padding_id at every text position with probability `caption_dropout` (a missing or null key is 0), so the model
+    also learns p(image | empty caption), the unconditional half of classifier-free guidance.  The rate must lie in
+    [0, 1); when it is > 0, padding_id must be an integer in [0, text_vocab_size).  padding_id is None at rate 0."""
+    v = params.get("caption_dropout")
+    rate = 0.0 if v is None else float(v)
+    if not 0.0 <= rate < 1.0:
+        raise ValueError(f"caption_dropout = {v!r}: a dropout rate must lie in [0, 1)")
+    if rate == 0.0:
+        return 0.0, None
+    pad, tv = params.get("padding_id"), params.get("text_vocab_size")
+    if pad is None or isinstance(pad, bool) or int(pad) != pad or tv is None or not 0 <= pad < tv:
+        raise ValueError(f"caption_dropout = {rate} needs padding_id in [0, text_vocab_size = {tv}), got {pad!r}")
+    return rate, int(pad)
+
+
 def dalle_model_fn(features, labels, mode, params):
     """src/model_fns.py:55-236.  features: images f32 [B,H,W,C] in [-1,1] (NHWC); labels: caption ids i32
     [B, text_seq_len].  (The reference's own comment has them swapped; the code uses them this way.)"""
     mode_str = mode_to_str(mode)
     if mode == PREDICT:
         raise NotImplementedError                                             # model_fns.py:135-136
+    cap_rate, pad_id = caption_dropout(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -157,11 +175,12 @@ def dalle_model_fn(features, labels, mode, params):
     opt = OptimizerConfig(params) if mode == TRAIN else None
     spec = StepSpec(mode, model, dp=dp, extra={"vae": vae})
 
-    def assemble(features, labels):
+    def assemble(features, labels, caption_drop=None):
         img = _to_device(features, torch.float32, device).view(local_batch, vae.img_H, vae.img_W, vae.img_C)
         text = _to_device(labels, torch.int32, device).view(local_batch, params["text_seq_len"])
         img_ids = vae.encode_tokens(img)                                        # model_fns.py:72-77
-        ops.assemble_tokens(text, img_ids, tokens, model.text_vocab_size)       # model_fns.py:117-122
+        ops.assemble_tokens(text, img_ids, tokens, model.text_vocab_size,       # model_fns.py:117-122
+                            caption_drop=caption_drop, pad_id=pad_id)
         return tokens
 
     def loss_value():
@@ -171,7 +190,12 @@ def dalle_model_fn(features, labels, mode, params):
     dp.hint_tokens_per_gpu(local_batch * S)
 
     def train_op(features, labels):
-        toks = assemble(features, labels)
+        # caption dropout of the global step, one decision per global sequence index, drawn for the whole local batch
+        # before micro-batching: the same captions drop whatever the rank count, micro-batch size or resume point
+        # (labels are shifted from these tokens, so a dropped caption is dropped from the targets too)
+        cap = L.make_dropout(cap_rate, params.get("seed") or 0, spec.global_step, L.SITE_CAPTION, first_row) \
+            if cap_rate else None
+        toks = assemble(features, labels, cap)
         model.zero_grads()
         mb = local_batch // num_microbatches
         hook = dp.make_bucket_hook(model.grads)

@@ -34,6 +34,7 @@ class DALLE:
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id
         self.engine.init_params(seed=params.get("seed") or 0)
+        self.padding_id = params.get("padding_id")   # caption of guided sampling's unconditional rows (None: tv - 1)
 
     def forward(self, features, return_loss=True, return_logits=False):
         """features = {"tokens": int [B, S]}.  Returns what the reference returns (models.py:397-416):
@@ -55,28 +56,32 @@ class DALLE:
         return loss, loss_batch
 
 
-    def sample(self, text_ids, temperature=1.0, generator=None, top_k=None, top_p=None):
+    def _get_sampler(self):
+        from .sampling import DalleSampler
+        if getattr(self, "_sampler", None) is None:
+            self._sampler = DalleSampler(self.engine, padding_id=self.padding_id)
+        return self._sampler
+
+    def sample(self, text_ids, temperature=1.0, generator=None, top_k=None, top_p=None, guidance_scale=None):
         """Autoregressive generation with a K/V cache ("next" row N4; the reference stubs inference):
         text_ids int [B, text_seq_len] -> int32 [B, text_seq_len + image_seq_len], image positions sampled from
         softmax(logits / temperature) restricted to the image-token ids (temperature 0 = greedy), optionally truncated
-        to its top_k ids and / or its top_p nucleus (DalleSampler.generate)."""
-        from .sampling import DalleSampler
-        if getattr(self, "_sampler", None) is None:
-            self._sampler = DalleSampler(self.engine)
+        to its top_k ids and / or its top_p nucleus, optionally with classifier-free guidance of scale guidance_scale
+        against a padding-only caption (params["padding_id"], default text_vocab_size - 1) (DalleSampler.generate)."""
         text_ids = text_ids.to(device=self.engine.device, dtype=torch.int32).contiguous()
-        return self._sampler.generate(text_ids, temperature, generator, top_k=top_k, top_p=top_p)
+        return self._get_sampler().generate(text_ids, temperature, generator, top_k=top_k, top_p=top_p,
+                                            guidance_scale=guidance_scale)
 
-    def complete(self, text_ids, image_prefix=None, samples_per_prompt=1, temperature=1.0, top_k=None, top_p=None):
+    def complete(self, text_ids, image_prefix=None, samples_per_prompt=1, temperature=1.0, top_k=None, top_p=None,
+                 guidance_scale=None):
         """Image completion (DalleSampler.complete): text_ids int [B, text_seq_len] plus optionally the first n VAE codes
         of each image, image_prefix int [B, n] -> int32 [B * samples_per_prompt, text_seq_len + image_seq_len].  The
         prompt is prefilled in one forward pass; noise comes from torch's default CUDA generator."""
-        from .sampling import DalleSampler
-        if getattr(self, "_sampler", None) is None:
-            self._sampler = DalleSampler(self.engine)
         text_ids = text_ids.to(device=self.engine.device, dtype=torch.int32).contiguous()
         if image_prefix is not None:
             image_prefix = image_prefix.to(device=self.engine.device, dtype=torch.int32).contiguous()
-        return self._sampler.complete(text_ids, image_prefix, samples_per_prompt, temperature, top_k, top_p)
+        return self._get_sampler().complete(text_ids, image_prefix, samples_per_prompt, temperature, top_k, top_p,
+                                            guidance_scale)
 
 
 class DiscreteVAE:

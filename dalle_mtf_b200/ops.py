@@ -164,13 +164,20 @@ def embed_bwd(ids, dx, dwte, dwpe, wte_drop=None, wpe_drop=None):
                                           _nbytes(ws), _ref(wte_drop), _ref(wpe_drop)), "embed_bwd_ex")
 
 
-def assemble_tokens(text_ids, image_idx, tokens, image_offset):
+def assemble_tokens(text_ids, image_idx, tokens, image_offset, caption_drop=None, pad_id=None):
+    """tokens = concat(text_ids, image_idx + image_offset) per row.  caption_drop (lib.Dropout of site
+    lib.SITE_CAPTION, row0 = global index of row 0): a dropped row's caption is pad_id at every text position."""
     L.require_device()
     _chk(text_ids, I32, "text_ids"); _chk(image_idx, I32, "image_idx"); _chk(tokens, I32, "tokens")
     B, Tt = text_ids.shape
     Ti = image_idx.shape[1]
-    check(L.load().db200_assemble_tokens(stream_ptr(), ptr(text_ids), ptr(image_idx), ptr(tokens), B, Tt, Ti,
-                                         image_offset), "assemble_tokens")
+    if caption_drop is None:
+        check(L.load().db200_assemble_tokens(stream_ptr(), ptr(text_ids), ptr(image_idx), ptr(tokens), B, Tt, Ti,
+                                             image_offset), "assemble_tokens")
+    else:
+        check(L.load().db200_assemble_tokens_ex(stream_ptr(), ptr(text_ids), ptr(image_idx), ptr(tokens), B, Tt, Ti,
+                                                image_offset, int(pad_id), ctypes.byref(caption_drop)),
+              "assemble_tokens_ex")
     return tokens
 
 
@@ -560,6 +567,29 @@ def sample_rows_filtered_at(logits, u, tokens, lo, hi, inv_temp, top_k, top_p, p
                                                  ptr(kept), logits.shape[0], logits.stride(0), int(lo), int(hi),
                                                  float(inv_temp), int(top_k), float(top_p), ptr(pos_dev)),
           "db200_sample_rows_filtered_at")
+    return tokens
+
+
+def sample_rows_guided(logits, u, tokens, lo, hi, inv_temp, guidance_scale, top_k=0, top_p=1.0, pos_dev=None,
+                       kept=None):
+    """Classifier-free guidance over R = logits.shape[0] // 2 pairs: logits rows [0, R) conditional, [R, 2R)
+    unconditional; pair r draws from u + s (c - u) (rounded op by op) * inv_temp, filtered like sample_rows_filtered
+    (top_k 0 and top_p 1 are off: the unfiltered kernel runs).  The id goes to tokens[r, col] and tokens[R + r, col],
+    col = pos + 1 with pos read from pos_dev, else 0 (pass e.g. out[:, j:j + 1] to write column j).  u: [R, hi - lo]."""
+    L.require_device()
+    _chk(logits, F32, "logits"); _chk(u, F32, "u"); _chk(tokens, I32, "tokens"); _chk(kept, I32, "kept")
+    _chk(pos_dev, I32, "pos_dev")
+    rows2 = logits.shape[0]
+    if rows2 % 2 or tokens.shape[0] != rows2:
+        raise L.DB200Error(f"sample_rows_guided: logits rows {rows2} must be even and match tokens rows "
+                           f"{tokens.shape[0]}")
+    rows = rows2 // 2
+    if u is not None:
+        assert u.shape == (rows, hi - lo)
+    check(L.load().db200_sample_rows_guided(stream_ptr(), ptr(logits), logits.stride(0), ptr(u), ptr(tokens),
+                                            tokens.stride(0), ptr(kept), rows, int(lo), int(hi), float(inv_temp),
+                                            float(guidance_scale), int(top_k), float(top_p), ptr(pos_dev)),
+          "db200_sample_rows_guided")
     return tokens
 
 

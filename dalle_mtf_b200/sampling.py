@@ -17,7 +17,16 @@ forward kernels in one pass (DalleEngine.prefill) and continues from there with 
 positions are restricted to the image-token id range [text_vocab_size, text_vocab_size + image_vocab_size), matching
 the ids training builds (src/model_fns.py:117-122).  `temperature == 0` (or None) is greedy decoding; `top_k` /
 `top_p` truncate the image-token distribution (after temperature) before the Gumbel-max draw.
+
+Classifier-free guidance (`guidance_scale` s, "condition scale"): every sampled row gets a twin whose caption is
+text_seq_len padding ids (the unconditional prompt a model trained with caption dropout has learned).  The 2R rows run
+through the same step kernels (R conditional rows, then R unconditional ones) and each image token is drawn once per
+pair from u + s (c - u) of the two logit rows (db200_sample_rows_guided), then fed to both.  s = 1 (or None) is the
+plain sampler: no twin rows, the same kernels, the same tokens.
 """
+import math
+import numbers
+
 import torch
 
 from . import ops
@@ -26,13 +35,20 @@ BF16, F32, I32 = torch.bfloat16, torch.float32, torch.int32
 
 
 class DalleSampler:
-    def __init__(self, engine):
+    def __init__(self, engine, padding_id=None):
+        """padding_id: the caption id of the unconditional rows of guided sampling (default text_vocab_size - 1, the
+        id GPT-2 + <|padding|> captions are padded with)."""
         self.e = engine
+        pad = engine.text_vocab_size - 1 if padding_id is None else padding_id
+        if isinstance(pad, bool) or int(pad) != pad or not 0 <= pad < engine.text_vocab_size:
+            raise ValueError(f"padding_id must be an integer in [0, {engine.text_vocab_size}), got {padding_id!r}")
+        self.padding_id = int(pad)
         self._B = None
 
     def _alloc(self, B):
         if self._B == B:
             return
+        self._graph_key = None      # captured graphs point at the buffers replaced here
         e = self.e
         dev, d = e.device, e.d
         mk = lambda *shape, dtype=BF16: torch.empty(*shape, dtype=dtype, device=dev)
@@ -100,20 +116,38 @@ class DalleSampler:
         p = 1.0 if top_p is None else float(top_p)
         return None if (k == 0 and p == 1.0) else (k, p)
 
-    def _capture(self, B, greedy, inv_t, flt):
-        """Two graphs over static buffers: the prompt step (teacher forcing: the next token is already in the token
-        matrix) and the sampling step (step -> noise -> Gumbel-max into column pos + 1); both end by advancing pos_dev."""
+    @staticmethod
+    def _guidance(scale):
+        """The guidance scale as the guided kernel takes it, or None when guidance is off (None or 1.0: the plain
+        sampler runs, exactly as without the argument)."""
+        if scale is None:
+            return None
+        if isinstance(scale, bool) or not isinstance(scale, numbers.Real) or not math.isfinite(scale) or scale < 0:
+            raise ValueError(f"guidance_scale must be a finite number >= 0 (or None), got {scale!r}")
+        return None if float(scale) == 1.0 else float(scale)
+
+    def _sample_guided(self, logits, u, tokens, inv_t, flt, gs, pos_dev=None):
         e = self.e
-        key = (B, greedy, inv_t, flt)
+        lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+        ops.sample_rows_guided(logits, u, tokens, lo, hi, inv_t, gs, *(flt or (0, 1.0)), pos_dev=pos_dev)
+
+    def _capture(self, B, greedy, inv_t, flt, gs=None):
+        """Two graphs over static buffers: the prompt step (teacher forcing: the next token is already in the token
+        matrix) and the sampling step (step -> noise -> Gumbel-max into column pos + 1); both end by advancing pos_dev.
+        B sampled rows; with guidance (gs) the steps run 2B rows (self._alloc(2 * B) first) and the noise has B."""
+        e = self.e
+        key = (B, greedy, inv_t, flt, gs)
         if getattr(self, "_graph_key", None) == key:
             return
         dev = e.device
-        self.tokens = torch.zeros(B, e.S, dtype=I32, device=dev)
+        self.tokens = torch.zeros(2 * B if gs is not None else B, e.S, dtype=I32, device=dev)
         self.pos_dev = torch.zeros(1, dtype=I32, device=dev)
         lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
 
         def sample(logits):
-            if flt is None:
+            if gs is not None:
+                self._sample_guided(logits, self.u, self.tokens, inv_t, flt, gs, self.pos_dev)
+            elif flt is None:
                 ops.sample_rows_at(logits, self.u, self.tokens, lo, hi, inv_t, self.pos_dev)
             else:
                 ops.sample_rows_filtered_at(logits, self.u, self.tokens, lo, hi, inv_t, *flt, self.pos_dev)
@@ -141,27 +175,32 @@ class DalleSampler:
         self._graph_key = key
 
     @torch.no_grad()
-    def generate_graphed(self, text_ids, temperature=1.0, top_k=None, top_p=None):
+    def generate_graphed(self, text_ids, temperature=1.0, top_k=None, top_p=None, guidance_scale=None):
         """generate() with the per-position step replayed from CUDA graphs (position kept on the device): removes the
         ~45 us of Python / ctypes / launch overhead per kernel that bounds eager generation.  Noise comes from torch's
-        default CUDA generator (seed it with torch.manual_seed).  Changing temperature, top_k or top_p re-captures."""
+        default CUDA generator (seed it with torch.manual_seed).  Changing temperature, top_k, top_p or guidance_scale
+        re-captures."""
         e = self.e
         B, TL = text_ids.shape
         assert TL == e.text_seq_len, f"expected {e.text_seq_len} text positions, got {TL}"
         flt = self._filter(top_k, top_p)
-        self._alloc(B)
+        gs = self._guidance(guidance_scale)
+        self._alloc(2 * B if gs is not None else B)
         greedy = temperature is None or temperature <= 0
         inv_t = 1.0 if greedy else 1.0 / float(temperature)
-        self._capture(B, greedy, inv_t, flt)
+        self._capture(B, greedy, inv_t, flt, gs)
         self.tokens.zero_()
-        self.tokens[:, :TL] = text_ids
+        self.tokens[:B, :TL] = text_ids
+        if gs is not None:
+            self.tokens[B:, :TL] = self.padding_id
         self.pos_dev.zero_()
         for pos in range(e.S - 1):
             (self.g_prompt if pos + 1 < TL else self.g_sample).replay()
-        return self.tokens.clone()
+        return self.tokens[:B].clone()
 
     @torch.no_grad()
-    def complete(self, text_ids, image_prefix=None, samples_per_prompt=1, temperature=1.0, top_k=None, top_p=None):
+    def complete(self, text_ids, image_prefix=None, samples_per_prompt=1, temperature=1.0, top_k=None, top_p=None,
+                 guidance_scale=None):
         """Image completion: text_ids int32 [B, text_seq_len] (device) and optionally image_prefix int32 [B, n], the
         first n (0 < n < image_seq_len) VAE codes in [0, image_vocab_size) in the VAE's row-major token order (e.g.
         vae.encode_tokens(img)[:, :n]).  Returns int32 [B * samples_per_prompt, text_seq_len + image_seq_len]: row
@@ -170,8 +209,11 @@ class DalleSampler:
 
         The whole prompt (P = text_seq_len + n positions) runs once per distinct prompt as one batched forward pass
         (DalleEngine.prefill) that fills every replica's K/V cache; token P is drawn from its logits and the remaining
-        positions replay the captured sampling step of generate_graphed.  temperature, top_k and top_p mean what they
-        mean for generate(); noise comes from torch's default CUDA generator (seed it with torch.manual_seed)."""
+        positions replay the captured sampling step of generate_graphed.  temperature, top_k, top_p and guidance_scale
+        mean what they mean for generate(); noise comes from torch's default CUDA generator (seed it with
+        torch.manual_seed).  With guidance the one prefill runs 2B prompts, the captions and then as many padding
+        captions, each followed by the same image prefix: its b * samples_per_prompt + r row order puts the conditional
+        rows first and their unconditional twins second, the layout the guided sampler reads."""
         e = self.e
         if not torch.is_tensor(text_ids) or text_ids.dim() != 2 or text_ids.shape[1] != e.text_seq_len:
             raise ValueError(f"text_ids must be [B, {e.text_seq_len}], got "
@@ -191,24 +233,29 @@ class DalleSampler:
             if int(image_prefix.min()) < 0 or int(image_prefix.max()) >= e.image_vocab_size:
                 raise ValueError(f"image_prefix codes must lie in [0, {e.image_vocab_size})")
         flt = self._filter(top_k, top_p)
+        gs = self._guidance(guidance_scale)
         P, R = TL + n, B * rep
-        self._alloc(R)
+        self._alloc(2 * R if gs is not None else R)
         greedy = temperature is None or temperature <= 0
         inv_t = 1.0 if greedy else 1.0 / float(temperature)
         # capture before the prefill (the capture's warm-up step writes the caches), and without moving the default
         # generator (its warm-up draws noise): a seeded call then samples the same whether or not it had to capture
         rng = torch.cuda.get_rng_state(e.device)
-        self._capture(R, greedy, inv_t, flt)
+        self._capture(R, greedy, inv_t, flt, gs)
         torch.cuda.set_rng_state(rng, e.device)
-        prompt = torch.empty(B, P, dtype=I32, device=e.device)
-        prompt[:, :TL] = text_ids
-        if n:
-            prompt[:, TL:] = image_prefix.to(device=e.device, dtype=I32) + e.text_vocab_size
+        prompt = torch.empty(2 * B if gs is not None else B, P, dtype=I32, device=e.device)
+        prompt[:B, :TL] = text_ids
+        if gs is not None:
+            prompt[B:, :TL] = self.padding_id
+        if n:   # (with guidance the padding-caption prompts continue with the same image prefix)
+            prompt[:, TL:] = (image_prefix.to(device=e.device, dtype=I32) + e.text_vocab_size).repeat(len(prompt) // B, 1)
         logits = e.prefill(prompt, self.kc, self.vc, rep)
         lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
         if self.u is not None:
             self.u.uniform_(1e-9, 1.0)
-        if flt is None:
+        if gs is not None:
+            self._sample_guided(logits, self.u, self.tok.view(-1, 1), inv_t, flt, gs)
+        elif flt is None:
             ops.sample_rows(logits, self.u, self.tok, lo, hi, inv_t)
         else:
             ops.sample_rows_filtered(logits, self.u, self.tok, lo, hi, inv_t, *flt)
@@ -218,23 +265,32 @@ class DalleSampler:
         self.pos_dev.fill_(P)
         for _ in range(P, e.S - 1):
             self.g_sample.replay()
-        return self.tokens.clone()
+        return self.tokens[:R].clone()
 
     @torch.no_grad()
-    def generate(self, text_ids, temperature=1.0, generator=None, return_logits=False, top_k=None, top_p=None):
+    def generate(self, text_ids, temperature=1.0, generator=None, return_logits=False, top_k=None, top_p=None,
+                 guidance_scale=None):
         """text_ids int32 [B, text_seq_len] (device) -> int32 [B, text_seq_len + image_seq_len]: the prompt followed by
         image_seq_len sampled image-token ids (already offset by text_vocab_size, as in training).
 
         top_k (>= 1) keeps the k most likely image tokens (all of a tie at the k-th), top_p (in (0, 1]) the smallest
         set of them whose probability mass after temperature reaches p (nucleus sampling); with both, top-k applies
-        first.  None disables either; no filter at all runs the unfiltered sampler."""
+        first.  None disables either; no filter at all runs the unfiltered sampler.
+
+        guidance_scale s (finite, >= 0; None or 1 = off): classifier-free guidance, each image token drawn from
+        u + s (c - u) of the logits given the caption (c) and given a padding-only caption (u).  With guidance,
+        return_logits returns all 2B rows of each step, the conditional rows first."""
         e = self.e
         B, TL = text_ids.shape
         assert TL == e.text_seq_len, f"expected {e.text_seq_len} text positions, got {TL}"
         flt = self._filter(top_k, top_p)
-        self._alloc(B)
-        out = torch.empty(B, e.S, dtype=I32, device=e.device)
-        out[:, :TL] = text_ids
+        gs = self._guidance(guidance_scale)
+        rows = 2 * B if gs is not None else B
+        self._alloc(rows)
+        out = torch.empty(rows, e.S, dtype=I32, device=e.device)
+        out[:B, :TL] = text_ids
+        if gs is not None:
+            out[B:, :TL] = self.padding_id
         lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
         greedy = temperature is None or temperature <= 0
         inv_t = 1.0 if greedy else 1.0 / float(temperature)
@@ -249,9 +305,12 @@ class DalleSampler:
             u = None
             if not greedy:
                 u = torch.empty(B, hi - lo, dtype=F32, device=e.device).uniform_(1e-9, 1.0, generator=generator)
-            if flt is None:
+            if gs is not None:
+                self._sample_guided(logits, u, self.tok.view(-1, 1), inv_t, flt, gs)
+            elif flt is None:
                 ops.sample_rows(logits, u, self.tok, lo, hi, inv_t)
             else:
                 ops.sample_rows_filtered(logits, u, self.tok, lo, hi, inv_t, *flt)
             out[:, pos + 1] = self.tok
+        out = out[:B] if gs is not None else out
         return (out, kept) if return_logits else out

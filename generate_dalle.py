@@ -3,12 +3,13 @@ image tokens for each caption (optionally completing the top rows of a prompt im
 
     python generate_dalle.py --model dalle_example_b200 --out DIR (--captions FILE | --caption_ids FILE.npy)
         [--checkpoint PATH] [--image_prompt IMG ...] [--prompt_rows R] [--samples_per_prompt N]
-        [--temperature T] [--top_k K] [--top_p P] [--batch_size B] [--seed S]
+        [--temperature T] [--top_k K] [--top_p P] [--guidance_scale G] [--batch_size B] [--seed S]
 
 Writes DIR/{caption:05d}_{sample:02d}.png and DIR/tokens.npy (int32 [captions * samples_per_prompt, S]: caption ids,
 then image-token ids offset by text_vocab_size, as in training).  One process, one GPU.
 """
 import argparse
+import math
 import os
 import sys
 from concurrent.futures import ThreadPoolExecutor
@@ -36,6 +37,9 @@ def parse_args(argv=None):
     p.add_argument("--temperature", type=float, default=1.0, help="0 = greedy.")
     p.add_argument("--top_k", type=int)
     p.add_argument("--top_p", type=float)
+    p.add_argument("--guidance_scale", type=float,
+                   help="Classifier-free guidance scale (>= 0; 1 or unset = unguided).  Needs a model trained with "
+                        "caption_dropout > 0.")
     p.add_argument("--batch_size", type=int, help="Captions per sampling call (default: predict_batch_size).")
     p.add_argument("--seed", type=int, default=0)
     args = p.parse_args(argv)
@@ -49,7 +53,16 @@ def parse_args(argv=None):
         p.error("--top_k must be >= 1")
     if args.top_p is not None and not 0.0 < args.top_p <= 1.0:
         p.error("--top_p must lie in (0, 1]")
+    if args.guidance_scale is not None and not (math.isfinite(args.guidance_scale) and args.guidance_scale >= 0):
+        p.error("--guidance_scale must be a finite number >= 0")
     return args
+
+
+def padding_id(params):
+    """Caption id of the unconditional rows of guided sampling: the config's padding_id, else what captions are padded
+    with here."""
+    pad = params.get("padding_id")
+    return PADDING_ID if pad is None else pad
 
 
 def load_params(model):
@@ -136,6 +149,9 @@ def main(argv=None):
     params = load_params(args.model)
     ckpt, vae_ckpt = find_checkpoints(params, args.checkpoint)
     tl, tv, iv = params["text_seq_len"], params["text_vocab_size"], params["image_vocab_size"]
+    if args.guidance_scale is not None and not 0 <= padding_id(params) < tv:
+        raise SystemExit(f"--guidance_scale: padding id {padding_id(params)} outside [0, {tv}); set padding_id in the "
+                         "config")
     if args.caption_ids:
         captions = load_caption_ids(args.caption_ids, tl, tv)
     else:
@@ -176,7 +192,7 @@ def main(argv=None):
         prefix = encode_image_prompts(args.image_prompt, params, vae, device)[:, :n]
         if len(prefix) == 1:
             prefix = prefix.expand(N, n)
-    sampler = DalleSampler(eng)
+    sampler = DalleSampler(eng, padding_id=padding_id(params) if args.guidance_scale is not None else None)
     torch.manual_seed(args.seed)
     rep = args.samples_per_prompt
     bs = args.batch_size or params["predict_batch_size"] or 1
@@ -186,7 +202,7 @@ def main(argv=None):
         text = torch.from_numpy(captions[c0:c0 + bs]).to(device)
         pre = prefix[c0:c0 + bs].contiguous() if prefix is not None else None
         toks = sampler.complete(text, pre, samples_per_prompt=rep, temperature=args.temperature, top_k=args.top_k,
-                                top_p=args.top_p)
+                                top_p=args.top_p, guidance_scale=args.guidance_scale)
         imgs = to_uint8(vae.decode_tokens(toks[:, tl:].contiguous(), offset=tv).cpu().numpy())
         for j, im in enumerate(imgs):
             c, s = c0 + j // rep, j % rep

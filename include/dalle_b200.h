@@ -53,13 +53,18 @@ int db200_device_check(void);
  *       attention weights (b, h, i, j), b = row0 + local sequence index, S2 = ceil(S / 2):
  *                                 n = ((b * H + h) * S2 + i / 2) * S2 + j / 2,  w = 2 * (i & 1) + (j & 1)
  *       keep iff word >= threshold (= floor(rate * 2^32)); kept values are multiplied by scale (= 1 / (1 - rate)).
+ *       caption dropout (site DB200_SITE_CAPTION, db200_assemble_tokens_ex): one decision per sequence, the
+ *                                 elementwise layout with cols = 1, e = row0 + b; the caption is dropped iff
+ *                                 word < threshold.
  *     Every entry point that takes a `const db200_dropout*` treats NULL, or threshold 0, as "no dropout" and then runs
  *     exactly the kernels of the entry point without dropout.
  * ------------------------------------------------------------------------------------------------------------------ */
+#define DB200_SITE_CAPTION 0xFFFFFFFFu /* above every layer site 2+3l .. 4+3l of a model with fewer than 2^30 layers */
 typedef struct db200_dropout {
   uint64_t seed;
   uint32_t step;      /* global optimiser step */
-  uint32_t site;      /* wte 0, wpe 1; layer l: attention weights 2+3l, attention output 3+3l, MLP output 4+3l */
+  uint32_t site;      /* wte 0, wpe 1; layer l: attention weights 2+3l, attention output 3+3l, MLP output 4+3l;
+                         caption DB200_SITE_CAPTION */
   uint32_t threshold; /* floor(rate * 2^32) */
   float scale;        /* 1 / (1 - rate) */
   int64_t row0;       /* elementwise: global row of row 0; attention: global sequence index of sequence 0 */
@@ -97,6 +102,12 @@ int db200_embed_bwd_ex(db200_stream_t stream, const int32_t* ids, const void* dx
  * src/model_fns.py:117-122 (image_offset = text_vocab_size). */
 int db200_assemble_tokens(db200_stream_t stream, const int32_t* text_ids, const int32_t* image_idx, int32_t* tokens,
                           int B, int text_len, int image_len, int image_offset);
+/* with caption dropout (the training half of classifier-free guidance): every text position of row b becomes pad_id
+ * when sequence caption_drop->row0 + b is dropped (D0, site DB200_SITE_CAPTION); image positions are untouched.  NULL
+ * or threshold 0 runs db200_assemble_tokens.  pad_id < 0 or row0 < 0 -> DB200_E_INVALID. */
+int db200_assemble_tokens_ex(db200_stream_t stream, const int32_t* text_ids, const int32_t* image_idx, int32_t* tokens,
+                             int B, int text_len, int image_len, int image_offset, int32_t pad_id,
+                             const db200_dropout* caption_drop);
 
 /* label shift: labels[b][t] = ids[b][t+1], labels[b][S-1] = eos_id.  Replaces the pad + gather at
  * src/dalle_mtf/models.py:407-410 (pad op: src/dalle_mtf/ops.py:6-68). */
@@ -379,6 +390,20 @@ int db200_sample_rows_filtered(db200_stream_t stream, const float* logits, const
 int db200_sample_rows_filtered_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
                                   long long ld_tokens, int32_t* kept_or_null, int rows, long long ld, int lo, int hi,
                                   float inv_temp, int top_k, float top_p, const int32_t* pos_dev);
+/* Classifier-free guidance over `rows` pairs.  logits f32 [2*rows][ld]: rows [0, rows) are conditional (c), rows
+ * [rows, 2*rows) unconditional (u).  Pair r samples, with the rules above, from
+ *   x_c = g * inv_temp,  g = __fadd_rn(u, __fmul_rn(s, __fsub_rn(c, u)))   (s = guidance_scale; no FMA contraction,
+ *                                                                           so a float32 host computation matches)
+ * through top-k, then top-p, then the Gumbel-max with noise row r of u_or_null (f32 [rows][hi-lo]; NULL = greedy).
+ * A NaN g is never kept or selected.  The draw is written to tokens[r * ld_tokens + col] and
+ * tokens[(rows + r) * ld_tokens + col], col = pos_dev ? *pos_dev + 1 : 0, so both rows continue with the same token.
+ * top_k == 0 && top_p == 1 runs the unfiltered kernel (kept_or_null must then be NULL), anything else the filtered one
+ * (kept_or_null: int32 [rows]).  guidance_scale NaN / inf / < 0, ld_tokens < 1 and the argument errors of
+ * db200_sample_rows_filtered return DB200_E_INVALID. */
+int db200_sample_rows_guided(db200_stream_t stream, const float* logits, long long ld, const float* u_or_null,
+                             int32_t* tokens, long long ld_tokens, int32_t* kept_or_null, int rows, int lo, int hi,
+                             float inv_temp, float guidance_scale, int top_k, float top_p,
+                             const int32_t* pos_dev_or_null);
 /* Prompt prefill hand-off: a whole prompt runs through the training forward kernels at sequence length P, and these
  * copies turn its results into the decoder's state (bandwidth-bound, 16-byte vector accesses).
  *   kv_cache_fill : qkv bf16 [B][P][3][H][dh] (the fused q|k|v GEMM output attn_causal_fwd reads) -> caches bf16

@@ -143,7 +143,8 @@ class DataParallel:
     def begin_overlap(self):
         """Call right before the backward pass whose buckets are all-reduced on the fly: from here until wait() the
         persistent kernels size their grids to (SM count - CTA cap), so the collective's CTAs and theirs fit side by
-        side (grids are sized on the host at launch time; forward / optimizer kernels keep all SMs)."""
+        side (grids are sized on the host at launch time).  The forward and optimizer kernels keep all SMs,
+        except a block forward that recompute_grad recomputes inside backward: it runs with the reservation."""
         self._ensure_comm()
         if self.comm is not None and self._reserve:
             from . import lib as L

@@ -16,7 +16,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXEMPT = {
     "db200_launch_count": "launch counter read by bench.py, no computation",
     "db200_device_check": "called by lib.require_device() before every GPU test",
-    "db200_set_reserved_sms": "grid-size knob of the multi-GPU path; needs concurrent collectives to mean anything",
 }
 EXEMPT.update({s: "collective of the data-parallel path (tests/test_dp_gpu.py runs it where 2 GPUs exist)" for s in (
     "db200_comm_load_nccl", "db200_comm_unique_id", "db200_comm_create", "db200_comm_destroy", "db200_comm_register",

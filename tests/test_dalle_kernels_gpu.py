@@ -111,7 +111,7 @@ def _peak_memory(request):
 
 
 def _sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
+    return float64_bounds.sm_count()
 
 
 def _gen(seed):
@@ -448,13 +448,18 @@ def test_cross_entropy_at_the_real_vocabulary(ops, config):
     closes every sequence, in the last, ragged vocabulary tile), labels 0 and at tile boundaries, rows that one logit
     dominates (also at EOS and in the last half tile), a non-zero bias.  dalle_coco runs T = 40 960 rows, so dlogits
     has more than 2^31 elements."""
+    T = 40960 if config == "dalle_coco_b200" else CONFIGS[config]
+    if config == "dalle_coco_b200":
+        assert T * engine_calls(ops, config)[3] > 2 ** 31
+    real_vocabulary_cross_entropy(ops, config, T)
+
+
+def real_vocabulary_cross_entropy(ops, config, T):
+    """run_cross_entropy at the configuration's V / Vpad / width with T rows (see the test above)."""
     cfg = _config(config)
     calls, _, V, Vpad, S = engine_calls(ops, config)
     assert any(c[0] == "gemm" and c[13] == V for c in calls)          # the engine's n_valid is V
     K = cfg["n_embd"]
-    T = 40960 if config == "dalle_coco_b200" else CONFIGS[config]
-    if config == "dalle_coco_b200":
-        assert T * Vpad > 2 ** 31
     g = _gen(Vpad + T)
     last = (V - 1) // 128 * 128
     edge = sorted({0, 1, 63, 64, 127, 128, V // 2, last - 1, last, last + 63, last + 64, V - 20, V - 19, V - 2, V - 1,
@@ -469,7 +474,8 @@ def test_cross_entropy_at_the_real_vocabulary(ops, config):
     rows = torch.arange(7, T, 101, device=DEV)
     labels[rows] = torch.tensor(edge, dtype=I32, device=DEV)[torch.arange(rows.numel(), device=DEV) % len(edge)]
     labels[sel_rows] = torch.tensor(cols, dtype=I32, device=DEV)[torch.arange(sel_rows.numel(), device=DEV) % len(cols)]
-    run_cross_entropy(ops, f"{config} CE T={T} V={V}", T, K, V, Vpad, labels=labels.contiguous(), h=h, W=W, bias=bias)
+    return run_cross_entropy(ops, f"{config} CE T={T} V={V}", T, K, V, Vpad, labels=labels.contiguous(), h=h, W=W,
+                             bias=bias)
 
 
 @pytest.mark.parametrize("n_valid", [130, 1, 200])
@@ -799,7 +805,8 @@ def run_embedding(ops, tag, ids, V, d, dx_scale, g):
     for b0 in range(0, B, 8):
         ref = wte.to(F64)[ids[b0:b0 + 8].long()] + wpe.to(F64)[None]
         assert torch.equal(out[b0:b0 + 8].view(torch.int16), bf16_rne(ref).view(torch.int16)), f"{tag} forward"
-    print(f"[{TAG}] {tag} embed_fwd: bf16 RNE of the exact sum, bit for bit (worst err/bound 0)")
+    print(f"{float64_bounds.prefix()}[{TAG}] {tag} embed_fwd: bf16 RNE of the exact sum, bit for bit "
+          "(worst err/bound 0)")
     dx = _randn(B, S, d, g=g, scale=dx_scale, dtype=BF16)
     base_t = _randn(V, d, g=g, scale=dx_scale)
     base_p = _randn(S, d, g=g, scale=dx_scale)
@@ -823,9 +830,10 @@ def run_embedding(ops, tag, ids, V, d, dx_scale, g):
     r = w.report()
     pad = int(torch.bincount(flat, minlength=V).argmax())
     touched = runs > 0
-    print(f"[{TAG}] {tag} dwte: fixed-point term {share[pad].item():.4f} of the bound at the padding row "
-          f"({int(runs[pad])} runs, {int((flat == pad).sum())} tokens), median {share[touched].median().item():.4f}, "
-          f"max {share.max().item():.4f} over the {int(touched.sum())} rows hit")
+    print(f"{float64_bounds.prefix()}[{TAG}] {tag} dwte: fixed-point term {share[pad].item():.4f} of the bound at "
+          f"the padding row ({int(runs[pad])} runs, {int((flat == pad).sum())} tokens), "
+          f"median {share[touched].median().item():.4f}, max {share.max().item():.4f} over the {int(touched.sum())} "
+          "rows hit")
     dref = base_p.to(F64) + dx.to(F64).sum(0)
     dabs = base_p.abs().to(F64) + dx.to(F64).abs().sum(0)
     r = max(r, check(f"{tag} dwpe", dwpe, dref, dabs, a=2 * U, b=(B + 2) * U))

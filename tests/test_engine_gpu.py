@@ -8,6 +8,7 @@ Tolerances:
     tensor; the engine must be no worse than 1.25 * e_ref(k) + 1e-2 — i.e. within the reference's bf16 rounding noise.
   * VAE in fp32 mode: 1e-4 (fp32 kernels), token / code indices bit-exact.
 """
+import contextlib
 import os
 
 import pytest
@@ -22,7 +23,7 @@ def relfro(a, b):
     return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
-def _dalle_case(d, L, H, tv, iv, ts, isl, B, recompute, seed=0):
+def _dalle_case(d, L, H, tv, iv, ts, isl, B, recompute, seed=0, **engine_kw):
     from dalle_mtf_b200.dalle_engine import DalleEngine
     from oracle import dalle as O
     cfg = O.DalleConfig(d, L, H, tv, iv, ts, isl)
@@ -34,30 +35,47 @@ def _dalle_case(d, L, H, tv, iv, ts, isl, B, recompute, seed=0):
         if k.endswith("/g"):
             params[k] = 1 + torch.randn(params[k].shape, generator=g) * 0.05
     tokens = torch.randint(0, cfg.total_tokens - 1, (B, cfg.seq_len), generator=g)
-    eng = DalleEngine(d, L, H, tv, iv, ts, isl, recompute_grad=recompute)
+    eng = DalleEngine(d, L, H, tv, iv, ts, isl, recompute_grad=recompute, **engine_kw)
     eng.load_params(params)
     return cfg, params, tokens, eng
 
 
-@pytest.mark.parametrize("d,L,H,tv,iv,ts,isl,B,recompute", [
+DALLE_CASES = [
     (256, 2, 2, 1000, 100, 40, 24, 3, False),     # dh=128, S=64
     (256, 2, 4, 1000, 100, 100, 60, 2, False),    # dh=64,  S=160 (ragged 128-row tiles)
     (512, 2, 4, 3000, 512, 200, 100, 2, True),    # recompute_grad path, S=300
-])
+]
+
+
+@pytest.mark.parametrize("d,L,H,tv,iv,ts,isl,B,recompute", DALLE_CASES)
 def test_dalle_forward_backward_optimizer_match_oracle(d, L, H, tv, iv, ts, isl, B, recompute):
+    dalle_step_matches_oracle((d, L, H, tv, iv, ts, isl, B), recompute)
+
+
+def dalle_step_matches_oracle(case, recompute, during_backward=contextlib.nullcontext, dropout=None):
+    """Forward, backward (inside during_backward()) and one optimiser step of the engine against the fp32 oracle.
+    dropout: (rates, seed, step, row0) of the step, checked against oracle/dalle_dropout.py."""
     from oracle import dalle as O
+    from oracle import dalle_dropout as D
     from oracle import optim as OO
-    cfg, params, tokens, eng = _dalle_case(d, L, H, tv, iv, ts, isl, B, recompute)
-    loss32, _, logits32, g32 = O.loss_and_grads(params, tokens, cfg, bf16=False)
-    _, _, _, g16 = O.loss_and_grads(params, tokens, cfg, bf16=True)
+    kw = {} if dropout is None else {"dropout": dropout[0], "dropout_seed": dropout[1]}
+    cfg, params, tokens, eng = _dalle_case(*case, recompute, **kw)
+    if dropout is None:
+        loss32, _, logits32, g32 = O.loss_and_grads(params, tokens, cfg, bf16=False)
+        _, _, _, g16 = O.loss_and_grads(params, tokens, cfg, bf16=True)
+    else:
+        loss32, _, _, g32 = D.loss_and_grads(params, tokens, cfg, dropout, bf16=False)
+        _, _, _, g16 = D.loss_and_grads(params, tokens, cfg, dropout, bf16=True)
     tok = tokens.to(torch.int32).cuda()
     T = tokens.numel()
     eng.zero_grads()
-    acc = eng.forward(tok)
-    eng.backward(1.0 / T)
-    torch.cuda.synchronize()
+    acc = eng.forward(tok) if dropout is None else eng.forward(tok, step=dropout[2], row0=dropout[3])
+    with during_backward():
+        eng.backward(1.0 / T)
+        torch.cuda.synchronize()
     assert abs(acc.item() / T - loss32.item()) / loss32.item() < 2e-3
-    assert relfro(eng.logits(tok), logits32) < 2e-2
+    if dropout is None:
+        assert relfro(eng.logits(tok), logits32) < 2e-2
     grads = eng.export_params(eng.grads)
     for k in g32:
         e_engine, e_ref = relfro(grads[k], g32[k]), relfro(g16[k], g32[k])
@@ -210,6 +228,10 @@ def test_tensor_core_conv_training_kernels_bf16(N, H, Cin, Cout, k, stride, tran
 
 def test_vae_engine_bf16_training_step_on_tensor_cores():
     """Whole VAE step with bf16 activations (wgmma conv fwd/dgrad/wgrad): loss and gradients vs the fp32 oracle."""
+    vae_bf16_step_matches_oracle()
+
+
+def vae_bf16_step_matches_oracle(during_backward=contextlib.nullcontext):
     from dalle_mtf_b200.vae_engine import VaeEngine
     from oracle import vae as OV
     cb, K, size, B = [[2, 64], [2, 128]], 128, 32, 4
@@ -225,8 +247,9 @@ def test_vae_engine_bf16_training_step_on_tensor_cores():
     eng.zero_grads()
     acc = torch.zeros(1, device=DEV)
     eng.forward(img.to(DEV), u.to(DEV), 1.0, False, loss_accum=acc)
-    eng.backward()
-    torch.cuda.synchronize()
+    with during_backward():
+        eng.backward()
+        torch.cuda.synchronize()
     assert relfro(acc, loss.reshape(1)) < 2e-2
     eg = eng.export_params(eng.grads)
     for k in grads:   # no worse than the reference's own bf16 policy (+ slack)
@@ -421,6 +444,10 @@ def test_training_step_is_bitwise_reproducible():
     """Two engines from the same weights, fed the same tokens, agree bit for bit after three steps.  The shape takes the
     split-K wgrad path (T = 512 tokens: two K splits), repeats token ids (embedding scatter onto shared rows) and runs
     every ordered reduction of the step (LayerNorm dg / db, bias column sums, gradient norm, loss)."""
+    training_steps_are_bitwise_reproducible()
+
+
+def training_steps_are_bitwise_reproducible(during_backward=contextlib.nullcontext):
     from dalle_mtf_b200.dalle_engine import DalleEngine
     runs = []
     for _ in range(2):
@@ -432,7 +459,8 @@ def test_training_step_is_bitwise_reproducible():
         for _ in range(3):
             eng.zero_grads()
             acc = eng.forward(tok)
-            eng.backward(1.0 / tok.numel())
+            with during_backward():
+                eng.backward(1.0 / tok.numel())
             grads.append(eng.grads.clone())
             losses.append(acc.clone())
             eng.optimizer_step(1e-3)

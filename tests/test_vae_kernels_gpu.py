@@ -65,7 +65,7 @@ def ops():
 
 
 def _sm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
+    return float64_bounds.sm_count()
 
 
 def _gen(seed):
@@ -281,20 +281,30 @@ def production_batch(ops, kind, cin, cout, res, k, stride, transposed, dgrad, sm
 
 @pytest.mark.parametrize("config", ["vae_example_b200", "vae_coco_b200"])
 def test_convolutions_at_the_production_geometry(ops, config):
+    production_convolutions(ops, config)
+
+
+def production_convolutions(ops, config, several_splits=True):
+    """run_conv (bf16, and fp32 at a quarter of the batch) on every convolution of the configuration's training step,
+    at the batch production_batch() picks for the current SM count.  several_splits: every pixel-split wgrad must run
+    several splits of several pixel tiles (true of these geometries on a 132-SM H100; with fewer SMs, vae_coco's
+    512-channel layers ask for a single split).  Returns (layer, batch) per layer."""
     eng = _engine(config)
     sm = _sm()
     layers = engine_convs(eng)
     assert any(kind == "up" for kind, *_ in layers) and any(kind == "res" for kind, *_ in layers)
     worst = 0.0
+    batches = []
     for i, (kind, cin, cout, res, k, stride, transposed, dgrad) in enumerate(layers):
         n = production_batch(ops, kind, cin, cout, res, k, stride, transposed, dgrad, sm)
+        batches.append((layers[i], n))
         c = ops.conv_desc(n, res, res, cin, cout, k, k, stride, transposed=transposed, act_f32=False)
         fwd_t, dg_t = tc_tiles(n, res, cin, cout, stride, transposed)
         if ops.conv_tc_supported(c):
             assert fwd_t >= 2 * sm, (kind, cin, cout, res, n, fwd_t)
         if dgrad and ops.conv_dgrad_tc_supported(c):
             assert dg_t >= 2 * sm, (kind, cin, cout, res, n, dg_t)
-        if ops.conv_wgrad_tc_supported(c):   # the pixel-split wgrad: several splits, each over several pixel tiles
+        if several_splits and ops.conv_wgrad_tc_supported(c):   # several splits, each over several pixel tiles
             _, _, splits, per = wgrad_split(n, res, cin, cout, k, stride, transposed, sm)
             assert splits >= 2 and per >= 2, (kind, cin, cout, res, n, splits, per)
         tag = f"{config} {kind} {cin}->{cout} @{res} N={n}"
@@ -305,10 +315,11 @@ def test_convolutions_at_the_production_geometry(ops, config):
         worst = max([worst] + run_conv(ops, f"{config} {kind} {cin}->{cout} @{res} N={nf}", nf, res, cin, cout, k,
                                        stride, transposed, dgrad=dgrad, res_block=kind == "res", act_f32=True,
                                        seed=100 + i))
-    print(f"[vae-kernels] {config} convolutions: worst err/bound {worst:.4f}")
+    print(f"{float64_bounds.prefix()}[vae-kernels] {config} convolutions: worst err/bound {worst:.4f}")
+    return batches
 
 
-@pytest.mark.parametrize("N,H,Cin,Cout,k,stride,transposed", [
+EDGE_GEOMETRIES = [
     (3, 12, 64, 64, 3, 1, False),      # 12 px: tiles run past the image edge
     (2, 20, 64, 192, 3, 1, False),     # 20 px; Cout 192: the second 128-wide channel tile is half empty
     (2, 24, 128, 64, 4, 2, False),     # stride 2, 24 -> 12; 64-wide channel tile
@@ -319,7 +330,10 @@ def test_convolutions_at_the_production_geometry(ops, config):
     (7, 4, 64, 64, 4, 2, True),        # conv-transpose from 4 px: eight images per tile, N = 7
     (1, 8, 64, 64, 3, 1, False),       # wgrad: one pixel tile, fewer than the splits the SM count asks for
     (3, 8, 128, 128, 4, 2, False),     # wgrad over 4 px outputs, 3 images per 8-image tile
-])
+]
+
+
+@pytest.mark.parametrize("N,H,Cin,Cout,k,stride,transposed", EDGE_GEOMETRIES)
 def test_tensor_core_convolutions_at_edge_geometries(ops, N, H, Cin, Cout, k, stride, transposed):
     c = ops.conv_desc(N, H, H, Cin, Cout, k, k, stride, transposed=transposed, act_f32=False)
     assert ops.conv_tc_supported(c) and ops.conv_dgrad_tc_supported(c) and ops.conv_wgrad_tc_supported(c)

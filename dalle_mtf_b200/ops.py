@@ -27,7 +27,9 @@ def _chk(t, dtype, name):
         raise L.DB200Error(f"{name}: tensor must live on a CUDA device (no CPU fallback)")
     if t.dtype != dtype:
         raise L.DB200Error(f"{name}: expected dtype {dtype}, got {t.dtype}")
-    if t.dim() > 0 and t.stride(-1) != 1:
+    # a length-1 innermost dimension has no step to take: torch keeps any stride there (out[:, j].contiguous() of a
+    # one-row [1, S] matrix is a view with stride S), and the kernels never apply it
+    if t.dim() > 0 and t.stride(-1) != 1 and t.shape[-1] > 1:
         raise L.DB200Error(f"{name}: innermost dimension must be contiguous")
 
 

@@ -63,6 +63,7 @@ import functools
 import json
 import math
 import os
+import types
 
 import pytest
 import torch
@@ -253,43 +254,61 @@ def _mode_name(mode):
             L.EPI_CE_GRAD: "CE_GRAD"}[mode]
 
 
-def run_gemm_case(ops, desc, T_rec, T, seed, dropout=None, tag=""):
-    """Replay one recorded product with T tokens: fresh operands, NaN-filled or based outputs, float64 reference."""
+def gemm_case_name(desc, M, N, K, splits, tiles, dropout=None, tag=""):
     from dalle_mtf_b200 import lib as L
-    (_, M, N, K, a_mn, b_mn, mode, out_dt, has_bias, relu, has_res, has_aux, split_k, _, has_colsum, _) = desc
-    M, K = (T if M == T_rec else M), (T if K == T_rec else K)
-    g = _gen(seed)
-    sm = _sm()
-    splits = gemm_splits(M, N, K, mode, split_k, sm)
-    tiles = -(-M // 128) * -(-N // 128) * splits
-    name = f"{tag}{_mode_name(mode)} {M}x{N}x{K} aT={int(a_mn)} bT={int(b_mn)}" + \
+    (_, _, _, _, a_mn, b_mn, mode, out_dt, has_bias, relu, has_res, _, _, _, has_colsum, _) = desc
+    return f"{tag}{_mode_name(mode)} {M}x{N}x{K} aT={int(a_mn)} bT={int(b_mn)}" + \
         "".join(f" {f}" for f, on in (("bias", has_bias), ("relu", relu), ("res", has_res), ("colsum", has_colsum),
                                       ("f32", out_dt == "torch.float32" and mode == L.EPI_STORE),
                                       ("dropout", dropout is not None)) if on) + f" splits={splits} tiles={tiles}"
-    a = _randn(*((K, M) if a_mn else (M, K)), g=g, dtype=BF16)
-    b = _randn(*((K, N) if b_mn else (N, K)), g=g, scale=K ** -0.5, dtype=BF16)
-    bias = _randn(N, g=g, scale=0.1) if has_bias else None
-    res = _randn(M, N, g=g, dtype=BF16) if has_res else None
-    aux = _randn(M, N, g=g, dtype=BF16) if has_aux else None
-    cs_base = _randn(N, g=g, scale=math.sqrt(M)) if has_colsum else None
-    colsum = cs_base.clone() if has_colsum else None
+
+
+def gemm_operands(ops, desc, M, K, seed, dropout=None):
+    """Fresh operands of the recorded product `desc` at M rows and depth K: bf16 A and B (B at K^-1/2, so products
+    are O(1)), the epilogue inputs the recorded call had, the output NaN-filled (ATOMIC: a random base, also kept in
+    `base`), and the dropout keep mask.  Fields as check_gemm reads them."""
+    from dalle_mtf_b200 import lib as L
+    (_, _, N, _, a_mn, b_mn, mode, out_dt, has_bias, relu, has_res, has_aux, split_k, _, has_colsum, _) = desc
+    g = _gen(seed)
+    o = types.SimpleNamespace(M=M, N=N, K=K, a_mn=a_mn, b_mn=b_mn, mode=mode, relu=relu, split_k=split_k,
+                              dropout=dropout)
+    o.a = _randn(*((K, M) if a_mn else (M, K)), g=g, dtype=BF16)
+    o.b = _randn(*((K, N) if b_mn else (N, K)), g=g, scale=K ** -0.5, dtype=BF16)
+    o.bias = _randn(N, g=g, scale=0.1) if has_bias else None
+    o.res = _randn(M, N, g=g, dtype=BF16) if has_res else None
+    o.aux = _randn(M, N, g=g, dtype=BF16) if has_aux else None
+    o.cs_base = _randn(N, g=g, scale=math.sqrt(M)) if has_colsum else None
+    o.colsum = o.cs_base.clone() if has_colsum else None
     if mode == L.EPI_ATOMIC:
-        base = _randn(M, N, g=g)
-        out = base.clone()
+        o.base = _randn(M, N, g=g)
+        o.out = o.base.clone()
     else:
-        base = None
-        out = nan_like((M, N), F32 if out_dt == "torch.float32" else BF16)
-    keep = None
+        o.base = None
+        o.out = nan_like((M, N), F32 if out_dt == "torch.float32" else BF16)
+    o.keep = None
     if dropout is not None:
-        keep = torch.empty(M, N, dtype=torch.uint8, device=DEV)
-        ops.dropout_mask(dropout, L.DROPOUT_ELEMENTWISE, (M, N), keep)
-    ops.gemm(a, b, out, M, N, K, a_mn=a_mn, b_mn=b_mn, mode=mode, bias=bias, relu=relu, residual=res, aux=aux,
-             split_k=split_k, colsum=colsum, dropout=dropout)
-    A = a.t() if a_mn else a                         # [M, K]
-    Bm = b if b_mn else b.t()                        # [K, N]
+        o.keep = torch.empty(M, N, dtype=torch.uint8, device=DEV)
+        ops.dropout_mask(dropout, L.DROPOUT_ELEMENTWISE, (M, N), o.keep)
+    return o
+
+
+def run_gemm(ops, o):
+    ops.gemm(o.a, o.b, o.out, o.M, o.N, o.K, a_mn=o.a_mn, b_mn=o.b_mn, mode=o.mode, bias=o.bias, relu=o.relu,
+             residual=o.res, aux=o.aux, split_k=o.split_k, colsum=o.colsum, dropout=o.dropout)
+
+
+def check_gemm(name, o, splits, report=True):
+    """o.out (and o.colsum) against float64 on the operands in o (fields of gemm_operands; keep / base / cs_base None
+    where the call had none), in slabs.  report=False returns the worst err/bound of o.out without printing or
+    asserting, for callers that gather many calls into one case line."""
+    M, N, K = o.M, o.N, o.K
+    A = o.a.t() if o.a_mn else o.a                   # [M, K]
+    Bm = o.b if o.b_mn else o.b.t()                  # [K, N]
+    bias, res, aux, base, keep, out = o.bias, o.res, o.aux, o.base, o.keep, o.out
+    has_colsum = o.cs_base is not None
     w = Worst(name)
     bnd = (K + 8 + splits) * UTC
-    cs_ref, cs_abs = (cs_base.to(F64), cs_base.to(F64).abs()) if has_colsum else (None, None)
+    cs_ref, cs_abs = (o.cs_base.to(F64), o.cs_base.to(F64).abs()) if has_colsum else (None, None)
     bf = out.dtype == BF16
     for c0, c1 in _slabs(N, K):                      # column slabs of B, row slabs of A: float64 tiles <= SLAB
         B64 = Bm[:, c0:c1].to(F64)
@@ -299,10 +318,10 @@ def run_gemm_case(ops, desc, T_rec, T, seed, dropout=None, tag=""):
             ref, absref = A64 @ B64, A64.abs() @ Ba
             if bias is not None:
                 ref, absref = ref + bias[c0:c1].to(F64), absref + bias[c0:c1].abs().to(F64)
-            if relu:
+            if o.relu:
                 ref = ref.clamp_min(0)
             if keep is not None:
-                kk = keep[r0:r1, c0:c1].to(F64) * dropout.scale
+                kk = keep[r0:r1, c0:c1].to(F64) * o.dropout.scale
                 ref, absref = ref * kk, absref * kk
             if res is not None:
                 ref, absref = ref + res[r0:r1, c0:c1].to(F64), absref + res[r0:r1, c0:c1].abs().to(F64)
@@ -318,10 +337,23 @@ def run_gemm_case(ops, desc, T_rec, T, seed, dropout=None, tag=""):
                 cs_abs[c0:c1] += o64.abs().sum(0)
             del ref, absref, A64
         del B64, Ba
+    if not report:
+        return w.r
     r = w.report()
     if has_colsum:
-        r = max(r, check(name + " colsum", colsum, cs_ref, cs_abs, a=0.0, b=(32 + M / 32 + 8) * U))
-    return r, tiles, (M, N)
+        r = max(r, check(name + " colsum", o.colsum, cs_ref, cs_abs, a=0.0, b=(32 + M / 32 + 8) * U))
+    return r
+
+
+def run_gemm_case(ops, desc, T_rec, T, seed, dropout=None, tag=""):
+    """Replay one recorded product with T tokens: fresh operands, NaN-filled or based outputs, float64 reference."""
+    (_, M, N, K, _, _, mode, _, _, _, _, _, split_k, _, _, _) = desc
+    M, K = (T if M == T_rec else M), (T if K == T_rec else K)
+    splits = gemm_splits(M, N, K, mode, split_k, _sm())
+    tiles = -(-M // 128) * -(-N // 128) * splits
+    o = gemm_operands(ops, desc, M, K, seed, dropout)
+    run_gemm(ops, o)
+    return check_gemm(gemm_case_name(desc, M, N, K, splits, tiles, dropout, tag), o, splits), tiles, (M, N)
 
 
 @pytest.mark.parametrize("config", list(CONFIGS))
@@ -496,8 +528,9 @@ def test_cross_entropy_abi_edges(ops, n_valid):
 # ------------------------------------------------------------------------------------------------------- attention
 def attn_reference(q, k, v, do, o, scale, keep=None, kscale=1.0):
     """float64 causal attention forward / backward and the |.| graphs on [B, S, H, dh] operands (o: the kernel's
-    output, used in delta as the kernel uses it).  Returns dicts of ref, abs and the per-row exponent errors."""
-    q, k, v, do, o = (t.to(F64).permute(0, 2, 1, 3) for t in (q, k, v, do, o))     # [B, H, S, dh]
+    output, used in delta as the kernel uses it).  Returns dicts of ref, abs and the per-row exponent errors.
+    do = None: the forward only (O and lse; b_bwd is None)."""
+    q, k, v = (t.to(F64).permute(0, 2, 1, 3) for t in (q, k, v))                    # [B, H, S, dh]
     S, dh = q.shape[2], q.shape[3]
     mask = torch.ones(S, S, dtype=torch.bool, device=DEV).tril()
     s = scale * q @ k.transpose(-1, -2)
@@ -512,22 +545,55 @@ def attn_reference(q, k, v, do, o, scale, keep=None, kscale=1.0):
     eps_lse = eps_row + (S + 32) * U + (nblk + 4) * 2.0 ** -21 + 2 * U * lse.abs()
     Pk = P if keep is None else P * keep.to(F64) * kscale
     out = {"O": (Pk @ v, Pk @ v.abs()), "lse": (lse, eps_lse)}
-    dP = do @ v.transpose(-1, -2)
-    dPa = do.abs() @ v.abs().transpose(-1, -2)
-    if keep is not None:
-        dP, dPa = dP * keep.to(F64) * kscale, dPa * keep.to(F64) * kscale
-    delta = (do * o).sum(-1, keepdim=True)
-    deltaa = (do * o).abs().sum(-1, keepdim=True)
-    dS = P * (dP - delta)
-    dSa = P * (dPa + deltaa)
-    out["dQ"] = (scale * dS @ k, scale * dSa @ k.abs())
-    out["dK"] = (scale * dS.transpose(-1, -2) @ q, scale * dSa.transpose(-1, -2) @ q.abs())
-    out["dV"] = (Pk.transpose(-1, -2) @ do, Pk.transpose(-1, -2) @ do.abs())
     b_fwd = UBF + 2 * eps_row + (2 * nblk + 2) * 2.0 ** -21 + (2 * S + 2 * nblk + 32) * UTC
-    b_bwd = (eps_s + eps_lse[..., None]).masked_fill(~mask, 0).max().item() + 2.0 ** -20 + UBF + (S + dh + 24) * UTC
+    b_bwd = None
+    if do is not None:
+        do, o = do.to(F64).permute(0, 2, 1, 3), o.to(F64).permute(0, 2, 1, 3)
+        dP = do @ v.transpose(-1, -2)
+        dPa = do.abs() @ v.abs().transpose(-1, -2)
+        if keep is not None:
+            dP, dPa = dP * keep.to(F64) * kscale, dPa * keep.to(F64) * kscale
+        delta = (do * o).sum(-1, keepdim=True)
+        deltaa = (do * o).abs().sum(-1, keepdim=True)
+        dS = P * (dP - delta)
+        dSa = P * (dPa + deltaa)
+        out["dQ"] = (scale * dS @ k, scale * dSa @ k.abs())
+        out["dK"] = (scale * dS.transpose(-1, -2) @ q, scale * dSa.transpose(-1, -2) @ q.abs())
+        out["dV"] = (Pk.transpose(-1, -2) @ do, Pk.transpose(-1, -2) @ do.abs())
+        b_bwd = (eps_s + eps_lse[..., None]).masked_fill(~mask, 0).max().item() + 2.0 ** -20 + UBF + \
+            (S + dh + 24) * UTC
     out = {n: (r.permute(0, 2, 1, 3) if r.dim() == 4 else r, a.permute(0, 2, 1, 3) if a.dim() == 4 else a)
            for n, (r, a) in out.items()}
     return out, b_fwd.permute(0, 2, 1)[..., None], b_bwd
+
+
+def check_attention(tag, B, S, H, dh, scale, qkv, out, lse, dout=None, dqkv=None, *, keep_all=None, kscale=1.0,
+                    chunk=None, report=True):
+    """out / lse (and dqkv when dout is given) of attn_fwd / attn_bwd on the [B, S, 3, H, dh] operands qkv against
+    float64, in chunks of sequences; keep_all: the [B, H, S, S] dropout keep mask (kscale its fp32 scale).
+    report=False returns {name: worst err/bound} without printing or asserting."""
+    extra = 2 * U if keep_all is not None else 0.0
+    chunk = chunk or max(1, 16 // H)
+    names = ("O", "lse") + (("dQ", "dK", "dV") if dout is not None else ())
+    ws = {n: Worst(f"{tag} {n}") for n in names}
+    for b0 in range(0, B, chunk):
+        b1 = min(B, b0 + chunk)
+        q, k, v = qkv[b0:b1, :, 0], qkv[b0:b1, :, 1], qkv[b0:b1, :, 2]
+        keep = keep_all[b0:b1] if keep_all is not None else None
+        do = dout[b0:b1] if dout is not None else None
+        refs, b_fwd, b_bwd = attn_reference(q, k, v, do, out[b0:b1], scale, keep, kscale)
+        ref, absref = refs["O"]
+        ws["O"].add(out[b0:b1], ref, absref, b=b_fwd + extra, bf16_out=True, floor=2.0 ** -120)
+        ref, bnd = refs["lse"]
+        ws["lse"].add(lse[b0:b1], ref, bnd, a=0.0, b=1.0)
+        if dout is not None:
+            for i, n in enumerate(("dQ", "dK", "dV")):
+                ref, absref = refs[n]
+                ws[n].add(dqkv[b0:b1, :, i], ref, absref, b=b_bwd + extra, bf16_out=True, floor=2.0 ** -120)
+        del refs
+    if not report:
+        return {n: w.r for n, w in ws.items()}
+    return max(w.report() for w in ws.values())
 
 
 def run_attention(ops, tag, B, S, H, dh, scale, qkv, dout, *, dropout=None, chunk=None):
@@ -544,23 +610,8 @@ def run_attention(ops, tag, B, S, H, dh, scale, qkv, dout, *, dropout=None, chun
         keep_all = torch.empty(B, H, S, S, dtype=torch.uint8, device=DEV)
         ops.dropout_mask(dropout, L.DROPOUT_ATTENTION, (B, H, S), keep_all)
     kscale = float(torch.tensor(dropout.scale, dtype=F32)) if dropout is not None else 1.0
-    extra = 2 * U if dropout is not None else 0.0
-    chunk = chunk or max(1, 16 // H)
-    ws = {n: Worst(f"{tag} {n}") for n in ("O", "lse", "dQ", "dK", "dV")}
-    for b0 in range(0, B, chunk):
-        b1 = min(B, b0 + chunk)
-        q, k, v = qkv[b0:b1, :, 0], qkv[b0:b1, :, 1], qkv[b0:b1, :, 2]
-        keep = keep_all[b0:b1] if keep_all is not None else None
-        refs, b_fwd, b_bwd = attn_reference(q, k, v, dout[b0:b1], out[b0:b1], scale, keep, kscale)
-        ref, absref = refs["O"]
-        ws["O"].add(out[b0:b1], ref, absref, b=b_fwd + extra, bf16_out=True, floor=2.0 ** -120)
-        ref, bnd = refs["lse"]
-        ws["lse"].add(lse[b0:b1], ref, bnd, a=0.0, b=1.0)
-        for i, n in enumerate(("dQ", "dK", "dV")):
-            ref, absref = refs[n]
-            ws[n].add(dqkv[b0:b1, :, i], ref, absref, b=b_bwd + extra, bf16_out=True, floor=2.0 ** -120)
-        del refs
-    return max(w.report() for w in ws.values())
+    return check_attention(tag, B, S, H, dh, scale, qkv, out, lse, dout, dqkv, keep_all=keep_all, kscale=kscale,
+                           chunk=chunk)
 
 
 def _qkv(B, S, H, dh, g, mag=1.0):
@@ -675,17 +726,24 @@ def test_attn_decode(ops, dh):
         out = nan_like((B, H, dh), BF16)
         ops.attn_decode(step, kc, vc, out, pos, 1.0)
         assert torch.equal(kc[:, pos], step[:, 1]) and torch.equal(vc[:, pos], step[:, 2])
-        q = step[:, 0].to(F64)                                    # [B, H, dh]
-        k = kc[:, :pos + 1].to(F64).permute(0, 2, 1, 3)           # [B, H, n, dh]
-        v = vc[:, :pos + 1].to(F64).permute(0, 2, 1, 3)
-        s = (k @ q[..., None])[..., 0]
-        sa = (k.abs() @ q.abs()[..., None])[..., 0]
-        P = torch.softmax(s, -1)
-        eps = ((dh + 8) * U * sa + 3 * U * (s.abs() + s.max(-1, keepdim=True).values.abs())).max(-1).values
-        n = pos + 1
-        b = UBF + 2 * eps + 2.0 ** -20 + (n / 8 + 40) * U
-        check(f"attn_decode dh={dh} pos={pos}", out, (P[..., None, :] @ v)[..., 0, :],
-              (P[..., None, :] @ v.abs())[..., 0, :], b=b[..., None], bf16_out=True)
+        ref, absref, b = attn_decode_reference(step[:, 0], kc[:, :pos + 1], vc[:, :pos + 1], 1.0)
+        check(f"attn_decode dh={dh} pos={pos}", out, ref, absref, b=b, bf16_out=True)
+
+
+def attn_decode_reference(q, k, v, scale):
+    """float64 softmax_j(scale q.k_j) v_j of q [B, H, dh] over the keys k, v [B, n, H, dh], its |.| graph and the b of
+    the attn_decode bound (module docstring) per (b, h): ref, absref [B, H, dh] and b [B, H, 1]."""
+    dh = q.shape[-1]
+    q = q.to(F64)
+    k = k.to(F64).permute(0, 2, 1, 3)                         # [B, H, n, dh]
+    v = v.to(F64).permute(0, 2, 1, 3)
+    s = scale * (k @ q[..., None])[..., 0]
+    sa = abs(scale) * (k.abs() @ q.abs()[..., None])[..., 0]
+    P = torch.softmax(s, -1)
+    eps = ((dh + 8) * U * sa + 3 * U * (s.abs() + s.max(-1, keepdim=True).values.abs())).max(-1).values
+    n = k.shape[2]
+    b = UBF + 2 * eps + 2.0 ** -20 + (n / 8 + 40) * U
+    return (P[..., None, :] @ v)[..., 0, :], (P[..., None, :] @ v.abs())[..., 0, :], b[..., None]
 
 
 # ------------------------------------------------------------------------------------------------------- LayerNorm
@@ -697,15 +755,46 @@ def ln_inputs(rows, d, g):
     return x.to(BF16)
 
 
+def ln_operands(rows, d, g):
+    """ln_inputs rows, gamma 1 + N(0, 0.1), beta N(0, 0.1)."""
+    x = ln_inputs(rows, d, g)
+    gam = 1 + torch.randn(d, generator=g, device=DEV) * 0.1
+    bet = torch.randn(d, generator=g, device=DEV) * 0.1
+    return x, gam, bet
+
+
+def check_layernorm_fwd(tag, x, gam, bet, y, mean, rstd, eps, report=True):
+    """y / mean / rstd of layernorm_fwd on x [rows, d] against float64 (the LayerNorm bound), in row slabs.
+    report=False returns {name: worst err/bound} without printing or asserting."""
+    rows, d = x.shape
+    g64, b64 = gam.to(F64), bet.to(F64)
+    ws = {n: Worst(f"{tag} {n}") for n in ("y", "mean", "rstd")}
+    for r0, r1 in _slabs(rows, d):
+        x64 = x[r0:r1].to(F64)
+        mu = x64.mean(1, keepdim=True)
+        var = ((x64 - mu) ** 2).mean(1, keepdim=True)
+        r = 1 / torch.sqrt(var + eps)
+        dm = (d / 32 + 16) * U * x64.abs().mean(1, keepdim=True) + U * mu.abs()
+        eps_r = ((d / 32 + 24) * U * var + dm ** 2) / (var + eps) / 2 + 2.0 ** -22 + 2 * U
+        xh = (x64 - mu) * r
+        ws["mean"].add(mean[r0:r1], mu[:, 0], dm[:, 0], a=0.0, b=1.0)
+        ws["rstd"].add(rstd[r0:r1], r[:, 0], (eps_r * r)[:, 0], a=0.0, b=1.0)
+        ws["y"].add(y[r0:r1], xh * g64 + b64, g64.abs() * r * dm + g64.abs() * xh.abs() * (eps_r + 4 * U)
+                    + 2 * U * b64.abs(), b=1.0, bf16_out=True)
+        del x64, mu, var, r, dm, eps_r, xh
+    if not report:
+        return {n: w.r for n, w in ws.items()}
+    return max(w.report() for w in ws.values())
+
+
 def run_layernorm(ops, tag, rows, d, *, dres=True, dxsum=True, dropout=None, seed=0):
     from dalle_mtf_b200 import lib as L
     g = _gen(seed)
     eps = 1e-5
-    x = ln_inputs(rows, d, g)
-    gam = 1 + torch.randn(d, generator=g, device=DEV) * 0.1
-    bet = torch.randn(d, generator=g, device=DEV) * 0.1
+    x, gam, bet = ln_operands(rows, d, g)
     y, mean, rstd = nan_like((rows, d), BF16), nan_like((rows,), F32), nan_like((rows,), F32)
     ops.layernorm_fwd(x, gam, bet, y, mean, rstd, eps)
+    worst = check_layernorm_fwd(tag, x, gam, bet, y, mean, rstd, eps)
     dy = _randn(rows, d, g=g, dtype=BF16)
     dr = _randn(rows, d, g=g, dtype=BF16) if dres else None
     dx = nan_like((rows, d), BF16)
@@ -722,22 +811,12 @@ def run_layernorm(ops, tag, rows, d, *, dres=True, dxsum=True, dropout=None, see
     chain = -(-rows // grid) if d == 4096 else -(-rows // (4 * grid))
     n_acc = chain + grid + 16
     gam_n = n_acc * U / (1 - n_acc * U)
-    g64, b64 = gam.to(F64), bet.to(F64)
-    names = ["y", "mean", "rstd", "dx"] + (["dxm"] if dropout is not None else [])
+    g64 = gam.to(F64)
+    names = ["dx"] + (["dxm"] if dropout is not None else [])
     ws = {n: Worst(f"{tag} {n}") for n in names}
     sums = {n: [bb.to(F64), bb.abs().to(F64)] for n, bb in zip(("dg", "db", "dxsum"), base)}
     for r0, r1 in _slabs(rows, d):
         x64 = x[r0:r1].to(F64)
-        mu = x64.mean(1, keepdim=True)
-        var = ((x64 - mu) ** 2).mean(1, keepdim=True)
-        r = 1 / torch.sqrt(var + eps)
-        dm = (d / 32 + 16) * U * x64.abs().mean(1, keepdim=True) + U * mu.abs()
-        eps_r = ((d / 32 + 24) * U * var + dm ** 2) / (var + eps) / 2 + 2.0 ** -22 + 2 * U
-        xh = (x64 - mu) * r
-        ws["mean"].add(mean[r0:r1], mu[:, 0], dm[:, 0], a=0.0, b=1.0)
-        ws["rstd"].add(rstd[r0:r1], r[:, 0], (eps_r * r)[:, 0], a=0.0, b=1.0)
-        ws["y"].add(y[r0:r1], xh * g64 + b64, g64.abs() * r * dm + g64.abs() * xh.abs() * (eps_r + 4 * U)
-                    + 2 * U * b64.abs(), b=1.0, bf16_out=True)
         # backward on the kernel's own statistics
         m32, r32 = mean[r0:r1, None].to(F64), rstd[r0:r1, None].to(F64)
         h = (x64 - m32) * r32
@@ -758,7 +837,7 @@ def run_layernorm(ops, tag, rows, d, *, dres=True, dxsum=True, dropout=None, see
                          ("dxsum", got.sum(0), got.abs().sum(0))):
             sums[n][0] += v
             sums[n][1] += va
-    worst = max(w.report() for w in ws.values())
+    worst = max([worst] + [w.report() for w in ws.values()])
     for n, t in (("dg", dg), ("db", db), ("dxsum", dxs)):
         if t is not None:
             worst = max(worst, check(f"{tag} {n}", t, sums[n][0], sums[n][1], a=0.0, b=gam_n + 4 * U))

@@ -19,6 +19,10 @@ int attn_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse,
                     float scale, const db200_dropout* drop);
 int attn_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
                        void* dqkv, int B, int S, int H, int dh, float scale, const db200_dropout* drop);
+int attn_local_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
+                          int radius, float scale);
+int attn_local_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
+                          void* dqkv, int B, int S, int H, int dh, int radius, float scale);
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward: delta = rowsum(dO * O)
@@ -60,6 +64,17 @@ attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ dout, flo
 
 using namespace db200;
 
+static int attn_delta(cudaStream_t stream, const void* out, const void* dout, float* delta, int B, int S, int H,
+                      int dh) {
+  const long long threads = (long long)B * S * H * (dh / 8);
+  const unsigned blocks = (unsigned)((threads + 255) / 256);
+  if (dh == 128)
+    attn_delta_kernel<128><<<blocks, 256, 0, stream>>>((const bf16*)out, (const bf16*)dout, delta, B, S, H);
+  else
+    attn_delta_kernel<64><<<blocks, 256, 0, stream>>>((const bf16*)out, (const bf16*)dout, delta, B, S, H);
+  return check_launch("attn_delta_kernel");
+}
+
 extern "C" int db200_attn_causal_fwd_ex(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B,
                                         int S, int H, int dh, float scale, const db200_dropout* drop) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
@@ -87,16 +102,7 @@ extern "C" int db200_attn_causal_bwd_ex(db200_stream_t stream_, const void* qkv,
                 DB200_E_ALIGN, "attn_bwd: NULL or unaligned pointer");
   DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_bwd: scale must be > 0");
   DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
-  const long long rows = (long long)B * S * H;
-  {
-    const long long threads = rows * (dh / 8);
-    const unsigned blocks = (unsigned)((threads + 255) / 256);
-    if (dh == 128)
-      attn_delta_kernel<128><<<blocks, 256, 0, stream>>>((const bf16*)out, (const bf16*)dout, delta, B, S, H);
-    else
-      attn_delta_kernel<64><<<blocks, 256, 0, stream>>>((const bf16*)out, (const bf16*)dout, delta, B, S, H);
-  }
-  int rc = check_launch("attn_delta_kernel");
+  const int rc = attn_delta(stream, out, dout, delta, B, S, H, dh);
   if (rc != DB200_OK) return rc;
   // delta = rowsum(dO * O) needs no dropout term: O already is the dropped output
   return attn_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, scale, drop);
@@ -106,4 +112,35 @@ extern "C" int db200_attn_causal_bwd(db200_stream_t stream_, const void* qkv, co
                                      const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S, int H,
                                      int dh, float scale) {
   return db200_attn_causal_bwd_ex(stream_, qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale, nullptr);
+}
+
+// ---- local (sliding-window) attention, src/dalle_mtf/models.py:257-273: query i attends to keys (i - radius, i].
+// radius >= S is causal attention (same result as db200_attn_causal_*, bit for bit).  No dropout.
+extern "C" int db200_attn_local_fwd(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B, int S, int H,
+                                    int dh, int radius, float scale) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_local_fwd: B,S,H must be positive");
+  DB200_REQUIRE(radius >= 1, DB200_E_INVALID, "attn_local_fwd: radius %d < 1", radius);
+  DB200_REQUIRE(qkv && out && lse && aligned16(qkv) && aligned16(out), DB200_E_ALIGN,
+                "attn_local_fwd: NULL or unaligned pointer");
+  DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_local_fwd: scale must be > 0");
+  DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
+  return attn_local_fwd_launch(stream, qkv, out, lse, B, S, H, dh, radius, scale);
+}
+
+extern "C" int db200_attn_local_bwd(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
+                                    const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S, int H,
+                                    int dh, int radius, float scale) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  (void)dq_accum;
+  DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_local_bwd: B,S,H must be positive");
+  DB200_REQUIRE(radius >= 1, DB200_E_INVALID, "attn_local_bwd: radius %d < 1", radius);
+  DB200_REQUIRE(qkv && out && dout && lse && delta && dqkv && aligned16(qkv) && aligned16(out) && aligned16(dout) &&
+                    aligned16(dqkv),
+                DB200_E_ALIGN, "attn_local_bwd: NULL or unaligned pointer");
+  DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_local_bwd: scale must be > 0");
+  DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
+  const int rc = attn_delta(stream, out, dout, delta, B, S, H, dh);
+  if (rc != DB200_OK) return rc;
+  return attn_local_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, radius, scale);
 }

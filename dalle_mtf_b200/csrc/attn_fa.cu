@@ -8,6 +8,10 @@
 // fp32 accumulator fragments; P and dS are packed to bf16 in registers and fed to the next wgmma as its A operand.
 //
 // Layout: qkv bf16 [B][S][3][H][dh], out / dout bf16 [B][S][H][dh], lse / delta f32 [B][H][S], dqkv like qkv.
+//
+// LOCAL (sliding-window attention, mtf local_attention_1d with fully_autoregressive=True, src/dalle_mtf/models.py:
+// 257-273): query i sees key j iff i - radius < j <= i.  The loops visit only the key (query) blocks that intersect that
+// band and the masks add the lower edge; the global (causal) instantiations compile without either.
 #include "gemm_common.cuh"  // cp.async helpers
 #include "philox.cuh"
 #include "wgmma.cuh"
@@ -146,10 +150,10 @@ constexpr size_t fa_smem(int tiles) { return 1024 + size_t(tiles) * FA_ROWS * DH
 // ------------------------------------------------------------------------------------------------------------------
 // forward: grid (query blocks, B * H); online softmax in the exp2 domain
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP>
+template <int DH, bool DROP, bool LOCAL>
 __global__ void __launch_bounds__(128, 1)
 attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, const db200_dropout dr) {
+                float scale, const db200_dropout dr, int radius) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -165,7 +169,8 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
   float o[DH / 2], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
-  for (int j = 0; j <= qb; ++j) {
+  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : 0;
+  for (int j = j0; j <= qb; ++j) {
     const int k0 = j * FA_ROWS;
     __syncthreads();  // the previous block's K / V tiles are no longer read
     fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
@@ -182,7 +187,7 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
         for (int e = 0; e < 2; ++e) {
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           float& v = s[4 * i + 2 * hh + e];
-          v = (col <= row && col < S) ? v * sl2 : -INFINITY;
+          v = (col <= row && col < S && (!LOCAL || col > row - radius)) ? v * sl2 : -INFINITY;
           mx[hh] = fmaxf(mx[hh], v);
         }
     float alpha[2], mb[2];
@@ -229,11 +234,11 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ: grid (query blocks, B * H).  P = exp(scale S - lse), dS = P (dO V^T - delta), dQ = scale dS K
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP>
+template <int DH, bool DROP, bool LOCAL>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                    const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                   const db200_dropout dr) {
+                   const db200_dropout dr, int radius) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -258,7 +263,8 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
   float dq[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) dq[i] = 0.f;
-  for (int j = 0; j <= qb; ++j) {
+  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : 0;
+  for (int j = j0; j <= qb; ++j) {
     const int k0 = j * FA_ROWS;
     __syncthreads();
     fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
@@ -277,7 +283,8 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
         for (int e = 0; e < 2; ++e) {
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           const int x = 4 * i + 2 * hh + e;
-          const float p = (col <= row && col < S && row < S) ? exp2f(s[x] * sl2 - lse2[hh]) : 0.f;
+          const bool vis = col <= row && col < S && row < S && (!LOCAL || col > row - radius);
+          const float p = vis ? exp2f(s[x] * sl2 - lse2[hh]) : 0.f;
           s[x] = p * ((DROP ? dp[x] * fa_keep_mul(kb, x, dr.scale) : dp[x]) - dl[hh]);
         }
     fa_pv<DH>(dq, s, sK);
@@ -290,11 +297,11 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
 // backward, dK / dV: grid (key blocks, B * H), transposed products so that the key index is the accumulator row.
 //   P^T = exp(scale K Q^T - lse), dV = P^T dO, dS^T = P^T (V dO^T - delta), dK = scale dS^T Q
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP>
+template <int DH, bool DROP, bool LOCAL>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                     const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                    const db200_dropout dr) {
+                    const db200_dropout dr, int radius) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -307,7 +314,9 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
   const bf16* Q = qkv + (long long)b * S * ldq + (long long)h * DH;
   const Frag f;
   const float sl2 = scale * kLog2e;
-  const int nqb = (S + FA_ROWS - 1) / FA_ROWS;
+  // LOCAL: the last query that sees key k0 + 63 is k0 + 62 + radius
+  const int nqb = LOCAL ? min((S + FA_ROWS - 1) / FA_ROWS, (int)(((long long)k0 + 62 + radius) / FA_ROWS) + 1)
+                        : (S + FA_ROWS - 1) / FA_ROWS;
 
   fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
   fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
@@ -336,7 +345,8 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
         for (int e = 0; e < 2; ++e) {
           const int key = k0 + f.fr + 8 * hh, cq = 8 * ii + f.fc + e, q = q0 + cq;
           const int x = 4 * ii + 2 * hh + e;
-          st[x] = (key <= q && q < S && key < S) ? exp2f(st[x] * sl2 - s_lse[cq]) : 0.f;
+          const bool vis = key <= q && q < S && key < S && (!LOCAL || key > q - radius);
+          st[x] = vis ? exp2f(st[x] * sl2 - s_lse[cq]) : 0.f;
         }
     // dropout: dV += (P keep scale)^T dO,  dS = P (dP keep scale - delta)
     const uint32_t kb = DROP ? fa_keep_bits<false>(dr, b, h, H, (S + 1) >> 1, k0, q0, f) : 0u;
@@ -360,35 +370,36 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
   fa_store_rows<DH>(dst + 2LL * H * DH, ldq, dv, one, S - k0, f);
 }
 
-template <int DH, bool DROP>
+template <int DH, bool DROP, bool LOCAL = false>
 static int fa_fwd(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, float scale,
-                  const db200_dropout& dr) {
+                  const db200_dropout& dr, int radius = 0) {
   constexpr size_t smem = fa_smem<DH>(3);
-  static const cudaError_t attr_rc =
-      cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL>,
+                                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(attr_rc);
   const dim3 grid((S + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_fwd_kernel<DH, DROP><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale, dr);
+  attn_fwd_kernel<DH, DROP, LOCAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale, dr,
+                                                                radius);
   return check_launch("attn_fwd_kernel");
 }
 
-template <int DH, bool DROP>
+template <int DH, bool DROP, bool LOCAL = false>
 static int fa_bwd(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
-                  void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr) {
+                  void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr, int radius = 0) {
   constexpr size_t smem = fa_smem<DH>(4);
-  static const cudaError_t rc1 =
-      cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  static const cudaError_t rc2 =
-      cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(rc1);
   DB200_CUDA(rc2);
   const dim3 grid((S + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_bwd_dq_kernel<DH, DROP><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
-                                                            (bf16*)dqkv, S, H, scale, dr);
+  attn_bwd_dq_kernel<DH, DROP, LOCAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
+                                                                   (bf16*)dqkv, S, H, scale, dr, radius);
   int rc = check_launch("attn_bwd_dq_kernel");
   if (rc != DB200_OK) return rc;
-  attn_bwd_dkv_kernel<DH, DROP><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
-                                                             (bf16*)dqkv, S, H, scale, dr);
+  attn_bwd_dkv_kernel<DH, DROP, LOCAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
+                                                                    (bf16*)dqkv, S, H, scale, dr, radius);
   return check_launch("attn_bwd_dkv_kernel");
 }
 
@@ -411,6 +422,21 @@ int attn_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, cons
                      : fa_bwd<64, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, *drop);
   return dh == 128 ? fa_bwd<128, false>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none)
                    : fa_bwd<64, false>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none);
+}
+
+// sliding window of `radius` keys (radius >= 1); no attention dropout (local layers have none)
+int attn_local_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
+                          int radius, float scale) {
+  const db200_dropout none{};
+  return dh == 128 ? fa_fwd<128, false, true>(stream, qkv, out, lse, B, S, H, scale, none, radius)
+                   : fa_fwd<64, false, true>(stream, qkv, out, lse, B, S, H, scale, none, radius);
+}
+
+int attn_local_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
+                          void* dqkv, int B, int S, int H, int dh, int radius, float scale) {
+  const db200_dropout none{};
+  return dh == 128 ? fa_bwd<128, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, radius)
+                   : fa_bwd<64, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, radius);
 }
 
 }  // namespace db200

@@ -4,7 +4,8 @@
 // src/model_fns.py:135-136).  All of it is HBM / latency bound work on B rows per step.
 //
 //   embed_fwd_at   x[b,:] = wte[ids[b],:] + wpe[pos,:]                     (models.py:186-219 at one position)
-//   attn_decode    append this step's k,v to the cache at `pos`, then out[b,h,:] = softmax_j<=pos(scale q.k_j) v_j
+//   attn_decode    append this step's k,v to the cache at `pos`, then out[b,h,:] = softmax_{lo<=j<=pos}(scale q.k_j) v_j,
+//                  lo = max(0, pos - radius + 1) (radius >= S: every key <= pos; a local layer, models.py:257-273: its window)
 //                  fp32 scores / softmax, P rounded to bf16 for the PV product (same policy as attn.cu)
 //   sample_rows    idx = lo + argmax_{lo<=c<hi}(logits[c] * inv_temp + gumbel(u[c-lo]))   (first maximum; u NULL = greedy)
 //   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
@@ -34,11 +35,12 @@ __global__ void embed_at_kernel(const int* __restrict__ ids, const bf16* __restr
 // one CTA per (head, batch); 8 warps.  Keys are split over the warps in BOTH passes (scores, then P.V), a warp reads a
 // whole cached row per instruction (dh * 2 contiguous bytes) and keeps four rows in flight: the per-thread serial walk
 // over `pos` keys of the first version made generation latency-bound (~100 us per call at pos ~ 1000).
-// Scores live in dynamic shared memory (pos + 1 floats, or S when the position is read on the device).
+// Scores live in dynamic shared memory, indexed by j - lo (pos + 1 - lo floats, or min(S, radius) when the position is
+// read on the device).
 template <int DH>
 __global__ void __launch_bounds__(256)
 attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __restrict__ vc, bf16* __restrict__ out,
-                   int S, int H, int pos, float scale, const int* __restrict__ pos_dev) {
+                   int S, int H, int pos, float scale, const int* __restrict__ pos_dev, int radius) {
   extern __shared__ float sc[];
   __shared__ float red[8];
   __shared__ float part[8][DH];
@@ -60,7 +62,9 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
 #pragma unroll
   for (int e = 0; e < EPL; ++e) qr[e] = __bfloat162float(q[lane * EPL + e]);
   __syncthreads();  // this block's own global writes are visible to it after the barrier
-  const int n = pos + 1;
+  const int lo = max(0, pos - radius + 1), n = pos + 1 - lo;
+  const bf16* kw = kcb + (long long)lo * rs;         // key / value rows of the window: j - lo = 0 .. n - 1
+  const bf16* vw = vcb + (long long)lo * rs;
   auto load_row = [&](const bf16* base, int j, float* o) {
     if (EPL == 4) {
       const uint2 u = *reinterpret_cast<const uint2*>(base + (long long)j * rs + lane * 4);
@@ -77,7 +81,7 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
     float kr[4][EPL], s[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u)
-      if (j0 + 8 * u < n) load_row(kcb, j0 + 8 * u, kr[u]);
+      if (j0 + 8 * u < n) load_row(kw, j0 + 8 * u, kr[u]);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       s[u] = 0.f;
@@ -121,7 +125,7 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
     float vr[4][EPL];
 #pragma unroll
     for (int u = 0; u < 4; ++u)
-      if (j0 + 8 * u < n) load_row(vcb, j0 + 8 * u, vr[u]);
+      if (j0 + 8 * u < n) load_row(vw, j0 + 8 * u, vr[u]);
 #pragma unroll
     for (int u = 0; u < 4; ++u)
       if (j0 + 8 * u < n) {
@@ -505,15 +509,16 @@ extern "C" int db200_incr_i32(db200_stream_t stream_, int32_t* p, int delta) {
   return check_launch("incr_i32_kernel");
 }
 
-// pos_dev == NULL: position `pos` (scores need pos + 1 floats of shared memory); else the position is read on the
-// device and shared memory is sized for all S keys.
+// pos_dev == NULL: position `pos` (scores need min(pos + 1, radius) floats of shared memory); else the position is read
+// on the device and shared memory is sized for min(S, radius) keys.  radius >= S: every key <= pos.
 static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k_cache, void* v_cache, void* out, int B,
-                              int S, int H, int dh, int pos, float scale, const int32_t* pos_dev) {
+                              int S, int H, int dh, int pos, float scale, const int32_t* pos_dev, int radius) {
   DB200_REQUIRE(qkv_step && k_cache && v_cache && out, DB200_E_INVALID, "attn_decode: null pointer");
   DB200_REQUIRE(B > 0 && H > 0 && S > 0 && pos >= 0 && pos < S, DB200_E_INVALID, "attn_decode: B %d H %d pos %d of %d",
                 B, H, pos, S);
+  DB200_REQUIRE(radius >= 1, DB200_E_INVALID, "attn_decode: radius %d < 1", radius);
   DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn_decode: head_dim %d not in {64,128}", dh);
-  const size_t keys = pos_dev ? (size_t)S : (size_t)(pos + 1);
+  const size_t keys = (size_t)min(pos_dev ? S : pos + 1, radius);
   DB200_REQUIRE(keys * 4 <= 200 * 1024, DB200_E_UNSUPPORTED, "attn_decode: %zu keys exceed shared memory", keys);
   const size_t smem = keys * sizeof(float);
   dim3 grid(H, B);
@@ -526,25 +531,40 @@ static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k
   if (dh == 128)
     attn_decode_kernel<128><<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step),
                                                          static_cast<bf16*>(k_cache), static_cast<bf16*>(v_cache),
-                                                         static_cast<bf16*>(out), S, H, pos, scale, pos_dev);
+                                                         static_cast<bf16*>(out), S, H, pos, scale, pos_dev, radius);
   else
     attn_decode_kernel<64><<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step), static_cast<bf16*>(k_cache),
                                                         static_cast<bf16*>(v_cache), static_cast<bf16*>(out), S, H, pos,
-                                                        scale, pos_dev);
+                                                        scale, pos_dev, radius);
   return check_launch("attn_decode_kernel");
 }
 
 extern "C" int db200_attn_decode(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache, void* out,
                                  int B, int S, int H, int dh, int pos, float scale) {
   return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, pos, scale,
-                            nullptr);
+                            nullptr, S);
 }
 
 extern "C" int db200_attn_decode_dev(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
                                      void* out, int B, int S, int H, int dh, const int32_t* pos_dev, float scale) {
   DB200_REQUIRE(pos_dev, DB200_E_INVALID, "attn_decode_dev: null position pointer");
   return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
-                            pos_dev);
+                            pos_dev, S);
+}
+
+// local layers (src/dalle_mtf/models.py:257-273): the query of `pos` attends to keys [max(0, pos - radius + 1), pos]
+extern "C" int db200_attn_decode_local(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
+                                       void* out, int B, int S, int H, int dh, int pos, int radius, float scale) {
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, pos, scale,
+                            nullptr, radius);
+}
+
+extern "C" int db200_attn_decode_local_dev(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
+                                           void* out, int B, int S, int H, int dh, const int32_t* pos_dev, int radius,
+                                           float scale) {
+  DB200_REQUIRE(pos_dev, DB200_E_INVALID, "attn_decode_local_dev: null position pointer");
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
+                            pos_dev, radius);
 }
 
 extern "C" int db200_sample_rows(db200_stream_t stream_, const float* logits, const float* u_or_null, int32_t* idx,

@@ -14,6 +14,7 @@ HBM layout
   * activations bf16 [T = B*S, features]; per-layer intermediates are kept for backward unless recompute_grad.
 """
 import math
+import numbers
 
 import torch
 
@@ -60,6 +61,20 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
+def layer_radii(attention_types, radius, n_layers):
+    """Per-layer attention radius: None for a "global" layer, `radius` for a "local" one (attention_types None: every
+    layer global)."""
+    if isinstance(radius, bool) or not isinstance(radius, numbers.Integral) or radius < 1:
+        raise ValueError(f"local_attention_radius must be an integer >= 1, got {radius!r}")
+    if attention_types is None:
+        return [None] * n_layers
+    types = list(attention_types)
+    if len(types) != n_layers or any(t not in ("global", "local") for t in types):
+        raise ValueError(f"attention_types must list 'global' or 'local' for each of the {n_layers} layers, got "
+                         f"{attention_types!r}")
+    return [int(radius) if t == "local" else None for t in types]
+
+
 class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
@@ -67,10 +82,14 @@ class DalleEngine:
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
-                 dropout_seed=0):
+                 dropout_seed=0, attention_types=None, local_attention_radius=256):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
+
+        attention_types: one "global" or "local" per layer (None: every layer global).  A local layer attends from
+        position i to positions (i - local_attention_radius, i] (src/dalle_mtf/models.py:257-273) and applies no
+        attention dropout (the reference passes it none, :270); its residual dropout is unchanged.
 
         zero: a DataParallel with world > 1 turns on optimiser-state sharding (ZeRO-1, SURVEY.md §7 "12 B in pure
         DP"): fp32 master / Adam m / Adam v exist only for this rank's 1/N slice of the flat buffer, the bf16 compute
@@ -101,6 +120,8 @@ class DalleEngine:
             L.dropout_threshold(r)   # rejects a rate outside [0, 1)
         self.dropout_seed = int(dropout_seed)
         self._drop = None            # descriptors of the current forward (None: no dropout)
+        # per layer: None (global, causal attention) or the window radius of a local layer
+        self.radii = layer_radii(attention_types, local_attention_radius, n_layers)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         lay = ParamLayout()
@@ -391,7 +412,7 @@ class DalleEngine:
         rows0 = row0 * self.S
         return {
             "wte": mk(emb, L.SITE_WTE, rows0), "wpe": mk(emb, L.SITE_WPE, 0),
-            "attn": [mk(att, L.dropout_site_attn(i), row0) for i in range(self.L)],
+            "attn": [mk(att, L.dropout_site_attn(i), row0) if self.radii[i] is None else None for i in range(self.L)],
             "attn_out": [mk(res, L.dropout_site_attn_out(i), rows0) for i in range(self.L)],
             "mlp_out": [mk(res, L.dropout_site_mlp_out(i), rows0) for i in range(self.L)],
         }
@@ -408,7 +429,7 @@ class DalleEngine:
                           self.ln_eps)
         ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
         ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
-                     dropout=self._site("attn", i))                                     # :290-299
+                     dropout=self._site("attn", i), radius=self.radii[i])               # :257-299
         ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in,
                        dropout=self._site("attn_out", i))                               # :303-314,330
         ops.layernorm_fwd(sv["xmid"], self.P(p + "ln2_g"), self.P(p + "ln2_b"), sv["ln2"], sv["mean2"], sv["rstd2"],
@@ -549,7 +570,7 @@ class DalleEngine:
         ops.linear_dgrad(da, self.W(p + "wo"), bufs["dtmp"])                                  # d(attn out)
         ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
         ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"], B,
-                     self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i))
+                     self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i), radius=self.radii[i])
         ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                      # dLN1 out
         ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
         return self._ln_bwd(bufs["dtmp"], x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,

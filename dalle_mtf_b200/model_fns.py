@@ -96,6 +96,37 @@ def dropout_rates(params):
     return tuple(rates)
 
 
+def attention_layers(params):
+    """(attention_types, local_attention_radius) of a DALL-E config.
+
+    local_attention_radius: the reference's key (src/dalle_mtf/models.py:259, default 256), an integer >= 1.
+    attention_types: per-layer attention types in GPT-Neo's form, e.g. [[["global", "local"], 3]]: each inner list is
+    repeated `count` times and the expansion must give "global" or "local" for exactly n_layers layers.  A missing or
+    null key is None: every layer global.  Returns the expanded list (or None) and the radius."""
+    v = params.get("local_attention_radius")
+    radius = 256 if v is None else v
+    if isinstance(radius, bool) or not isinstance(radius, int) or radius < 1:
+        raise ValueError(f"local_attention_radius = {v!r}: must be an integer >= 1")
+    spec = params.get("attention_types")
+    if spec is None:
+        return None, radius
+    n_layers = params.get("n_layers")
+    types = []
+    if not isinstance(spec, (list, tuple)):
+        raise ValueError(f"attention_types = {spec!r}: expected a list of [[types...], count] items")
+    for item in spec:
+        if not (isinstance(item, (list, tuple)) and len(item) == 2 and isinstance(item[0], (list, tuple))
+                and isinstance(item[1], int) and not isinstance(item[1], bool) and item[1] >= 1):
+            raise ValueError(f"attention_types item {item!r}: expected [[types...], count] with an integer count >= 1")
+        for t in item[0]:
+            if t not in ("global", "local"):
+                raise ValueError(f"attention_types: unknown attention type {t!r} (expected 'global' or 'local')")
+        types += list(item[0]) * item[1]
+    if len(types) != n_layers:
+        raise ValueError(f"attention_types expands to {len(types)} layers, but n_layers = {n_layers}")
+    return types, radius
+
+
 def caption_dropout(params):
     """(rate, padding_id) of the config's caption dropout: in mode "train", each sequence's caption is replaced by
     padding_id at every text position with probability `caption_dropout` (a missing or null key is 0), so the model
@@ -120,6 +151,7 @@ def dalle_model_fn(features, labels, mode, params):
     if mode == PREDICT:
         raise NotImplementedError                                             # model_fns.py:135-136
     cap_rate, pad_id = caption_dropout(params)
+    attention_types, local_radius = attention_layers(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -149,7 +181,8 @@ def dalle_model_fn(features, labels, mode, params):
                         # extension key: shard fp32 master + Adam slots across the data-parallel ranks (ZeRO-1) —
                         # what lets the d = 4096 configuration fit 80 GB GPUs in pure data parallelism
                         zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None,
-                        dropout=rates, dropout_seed=params.get("seed") or 0)
+                        dropout=rates, dropout_seed=params.get("seed") or 0,
+                        attention_types=attention_types, local_attention_radius=local_radius)   # models.py:229-301
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

@@ -6,7 +6,7 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
-from .model_fns import dropout_rates
+from .model_fns import attention_layers, dropout_rates
 from .vae_engine import VaeEngine
 
 
@@ -21,6 +21,7 @@ class DALLE:
         if is_incremental_inference or context is not None:
             raise NotImplementedError("incremental inference is stubbed in the reference too (src/model_fns.py:135)")
         params = params or {}
+        attention_types, local_radius = attention_layers({**params, "n_layers": n_layers})
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
@@ -30,7 +31,8 @@ class DALLE:
         self.batch_size, self.bf_16, self.mode = batch_size, bf_16, mode
         self.engine = DalleEngine(n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len,
                                   image_seq_len, recompute_grad=bool(params.get("recompute_grad")) and mode == "train",
-                                  dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0)
+                                  dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0,
+                                  attention_types=attention_types, local_attention_radius=local_radius)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id
         self.engine.init_params(seed=params.get("seed") or 0)

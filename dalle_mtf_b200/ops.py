@@ -266,11 +266,20 @@ def split_f32(src, hi, lo=None):
 # ----------------------------------------------------------------------------------------------- attention
 # bench.py sets ATTN_PROFILE to a list to time every attention launch like GEMM_PROFILE: entries are
 # (start_event, end_event, causal-algorithmic flops, "fwd" | "bwd").  Forward = 2 products over the visible half of the
-# S x S logits: 4 S^2 dh B H / 2; backward = 2.5 x that (5 products).
+# S x S logits: 4 S^2 dh B H / 2; backward = 2.5 x that (5 products).  A local launch counts the (query, key) pairs of
+# its band instead: sum_i min(i + 1, radius).
 ATTN_PROFILE = None
 
 
-def _attn_timed(kind, B, S, H, dh, call):
+def attn_pairs(S, radius=None):
+    """(query, key) pairs a causal (radius None) or local attention of length S computes: sum_i min(i + 1, radius)."""
+    if radius is None or radius >= S:
+        return S * S / 2.0      # the causal count bench.py has always used (the diagonal counted half)
+    r = int(radius)
+    return r * (r + 1) / 2.0 + (S - r) * r
+
+
+def _attn_timed(kind, B, S, H, dh, call, radius=None):
     prof = ATTN_PROFILE
     if prof is None:
         return call()
@@ -278,28 +287,51 @@ def _attn_timed(kind, B, S, H, dh, call):
     ev0.record()
     call()
     ev1.record()
-    prof.append((ev0, ev1, 2.0 * S * S * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
+    prof.append((ev0, ev1, 4.0 * attn_pairs(S, radius) * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
 
 
-def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None):
-    """dropout: lib.Dropout of the attention-weights site (row0 = global index of sequence 0), or None."""
+def _radius(radius):
+    if radius is None:
+        return None
+    if isinstance(radius, bool) or int(radius) != radius or radius < 1:
+        raise L.DB200Error(f"attention radius must be an integer >= 1 (or None), got {radius!r}")
+    return int(radius)
+
+
+def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None):
+    """dropout: lib.Dropout of the attention-weights site (row0 = global index of sequence 0), or None.
+    radius: None = causal attention; else local attention, query i over keys (i - radius, i] (no dropout)."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(lse, F32, "lse")
-    if dropout is None:
+    radius = _radius(radius)
+    if radius is not None:
+        if dropout is not None:
+            raise L.DB200Error("attn_fwd: local attention has no dropout (src/dalle_mtf/models.py:270)")
+        call = lambda: check(L.load().db200_attn_local_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
+                                                           radius, scale), "attn_local_fwd")
+    elif dropout is None:
         call = lambda: check(L.load().db200_attn_causal_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                             scale), "attn_causal_fwd")
     else:
         call = lambda: check(L.load().db200_attn_causal_fwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_fwd_ex")
-    _attn_timed("fwd", B, S, H, dh, call)
+    _attn_timed("fwd", B, S, H, dh, call, radius)
     return out
 
 
-def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None):
+def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None, radius=None):
+    """radius: as attn_fwd's (None = causal)."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(dout, BF16, "dout"); _chk(dqkv, BF16, "dqkv")
     _chk(lse, F32, "lse"); _chk(dq_accum, F32, "dq_accum"); _chk(delta, F32, "delta")
-    if dropout is None:
+    radius = _radius(radius)
+    if radius is not None:
+        if dropout is not None:
+            raise L.DB200Error("attn_bwd: local attention has no dropout (src/dalle_mtf/models.py:270)")
+        call = lambda: check(L.load().db200_attn_local_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
+                                                           ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, radius,
+                                                           scale), "attn_local_bwd")
+    elif dropout is None:
         call = lambda: check(L.load().db200_attn_causal_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                             ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, scale),
                              "attn_causal_bwd")
@@ -307,7 +339,7 @@ def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0,
         call = lambda: check(L.load().db200_attn_causal_bwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                                ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_bwd_ex")
-    _attn_timed("bwd", B, S, H, dh, call)
+    _attn_timed("bwd", B, S, H, dh, call, radius)
     return dqkv
 
 
@@ -496,12 +528,18 @@ def embed_fwd_at(ids, wte, wpe, out, pos):
     return out
 
 
-def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale):
-    """Append this position's k, v to the caches and attend with its q over keys <= pos (models.py:246-254, 281-299)."""
+def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None):
+    """Append this position's k, v to the caches and attend with its q over keys <= pos (models.py:246-254, 281-299);
+    radius (local layer, models.py:257-273): over keys [max(0, pos - radius + 1), pos] only."""
     L.require_device()
     _chk(qkv_step, BF16, "qkv_step"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache"); _chk(out, BF16, "out")
     B, S, H, dh = k_cache.shape
     assert v_cache.shape == k_cache.shape and qkv_step.numel() == B * 3 * H * dh and out.numel() == B * H * dh
+    radius = _radius(radius)
+    if radius is not None:
+        check(L.load().db200_attn_decode_local(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S,
+                                               H, dh, int(pos), radius, float(scale)), "db200_attn_decode_local")
+        return out
     check(L.load().db200_attn_decode(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S, H, dh,
                                      int(pos), float(scale)), "db200_attn_decode")
     return out
@@ -529,9 +567,16 @@ def embed_fwd_at_dev(tokens, wte, wpe, out, pos_dev):
     return out
 
 
-def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale):
+def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None):
+    """attn_decode with the position read on the device from pos_dev (graph replay)."""
     L.require_device()
     B, S, H, dh = k_cache.shape
+    radius = _radius(radius)
+    if radius is not None:
+        check(L.load().db200_attn_decode_local_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B,
+                                                   S, H, dh, ptr(pos_dev), radius, float(scale)),
+              "db200_attn_decode_local_dev")
+        return out
     check(L.load().db200_attn_decode_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S, H, dh,
                                          ptr(pos_dev), float(scale)), "db200_attn_decode_dev")
     return out

@@ -216,6 +216,15 @@ int db200_attn_causal_fwd_ex(db200_stream_t stream, const void* qkv_bf16, void* 
 int db200_attn_causal_bwd_ex(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
                              const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H,
                              int dh, float scale, const db200_dropout* drop);
+/* Local (sliding-window) attention of the reference's "local" attention type (mtf local_attention_1d with
+ * fully_autoregressive=True, src/dalle_mtf/models.py:257-273): query i attends to keys j with i - radius < j <= i.
+ * Layouts, workspaces and numerics as db200_attn_causal_fwd / _bwd; radius >= S is causal attention (bit for bit).
+ * No dropout: the reference passes no dropout rate to local attention (models.py:270).  radius < 1: DB200_E_INVALID. */
+int db200_attn_local_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, float* lse, int B, int S, int H,
+                         int dh, int radius, float scale);
+int db200_attn_local_bwd(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
+                         const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H, int dh,
+                         int radius, float scale);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * small HBM-bound helpers
@@ -366,6 +375,14 @@ int db200_embed_fwd_at_dev(db200_stream_t stream, const int32_t* tokens, long lo
                            const void* wpe_bf16, void* out_bf16, int B, int d, int V, const int32_t* pos_dev);
 int db200_attn_decode_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16, void* v_cache_bf16,
                           void* out_bf16, int B, int S, int H, int dh, const int32_t* pos_dev, float scale);
+/* attn_decode / attn_decode_dev of a local layer (src/dalle_mtf/models.py:257-273): the query of position p attends to
+ * keys [max(0, p - radius + 1), p] of the same full-length cache.  radius >= S is attn_decode; radius < 1 is
+ * DB200_E_INVALID. */
+int db200_attn_decode_local(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16, void* v_cache_bf16,
+                            void* out_bf16, int B, int S, int H, int dh, int pos, int radius, float scale);
+int db200_attn_decode_local_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
+                                void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
+                                const int32_t* pos_dev, int radius, float scale);
 int db200_sample_rows_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
                          long long ld_tokens, int rows, long long ld, int lo, int hi, float inv_temp,
                          const int32_t* pos_dev);

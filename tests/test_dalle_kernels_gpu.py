@@ -182,7 +182,7 @@ def _describe(name, args, kw):
     if name in ("attn_fwd", "attn_bwd"):
         B, S, H, dh = args[3:7] if name == "attn_fwd" else args[7:11]
         scale = args[7] if name == "attn_fwd" and len(args) > 7 else (args[11] if len(args) > 11 else kw["scale"])
-        return (name, B, S, H, dh, float(scale), kw.get("dropout") is not None)
+        return (name, B, S, H, dh, float(scale), kw.get("dropout") is not None, kw.get("radius"))
     if name == "layernorm_fwd":
         return (name,) + tuple(args[0].shape)
     if name == "layernorm_bwd":
@@ -192,14 +192,17 @@ def _describe(name, args, kw):
     return (name,) + tuple(ids.shape) + (kw.get("wte_drop") is not None,)
 
 
-def engine_calls(ops, config):
+def engine_calls(ops, config, step=None, **engine_kw):
     """Distinct kernel calls of one forward + backward + logits() of a one-layer DalleEngine of `config` at B = 1,
-    S = 1280, and the standard deviation of the gradient that reaches the embedding."""
-    if config in _RECORDS:
-        return _RECORDS[config]
+    S = 1280, and the standard deviation of the gradient that reaches the embedding.  engine_kw go to the engine
+    (attention_types, local_attention_radius, dropout rates); step goes to forward() (dropout runs with a step)."""
+    key = (config, step, repr(sorted(engine_kw.items())))
+    if key in _RECORDS:
+        return _RECORDS[key]
     from dalle_mtf_b200.dalle_engine import DalleEngine
     cfg = _config(config)
-    eng = DalleEngine(cfg["n_embd"], 1, cfg["n_heads"], cfg["text_vocab_size"], cfg["image_vocab_size"], 256, 1024)
+    eng = DalleEngine(cfg["n_embd"], 1, cfg["n_heads"], cfg["text_vocab_size"], cfg["image_vocab_size"], 256, 1024,
+                      **engine_kw)
     eng.init_params(seed=1)
     seen, extra = {}, {}
     orig = {n: getattr(ops, n) for n in RECORDED}
@@ -217,7 +220,7 @@ def engine_calls(ops, config):
             setattr(ops, n, wrap(n))
         tokens = synthetic_tokens(cfg, 1, _gen(1))
         eng.zero_grads()
-        eng.forward(tokens)
+        eng.forward(tokens, step=step)
         eng.backward(1.0 / tokens.numel())
         eng.logits(tokens)
         torch.cuda.synchronize()
@@ -227,7 +230,7 @@ def engine_calls(ops, config):
     res = (list(seen), extra, eng.V, eng.Vpad, eng.S)
     del eng
     torch.cuda.empty_cache()
-    _RECORDS[config] = res
+    _RECORDS[key] = res
     return res
 
 
@@ -626,7 +629,8 @@ def test_attention_at_the_engine_shapes(ops, config):
     calls, _, _, _, S = engine_calls(ops, config)
     att = [c for c in calls if c[0] in ("attn_fwd", "attn_bwd")]
     assert {c[0] for c in att} == {"attn_fwd", "attn_bwd"} and len({c[1:] for c in att}) == 1
-    _, _, S_, H, dh, scale, _ = att[0]
+    _, _, S_, H, dh, scale, dropout, radius = att[0]
+    assert not dropout and radius is None                 # the configurations' engines run causal attention
     B = CONFIGS[config] // S
     qkv, dout = _qkv(B, S, H, dh, _gen(B * H))
     run_attention(ops, f"{config} attention B={B} S={S} H={H} dh={dh}", B, S, H, dh, scale, qkv, dout)

@@ -89,27 +89,32 @@ def _peak_memory(request):
 _ENGINE = {}
 
 
-def sharp_engine(config):
-    """One-layer DalleEngine at the configuration's width, heads and vocabulary, with init_params weights sharpened as
+def sharp_engine(config, attention_types=None):
+    """DalleEngine at the configuration's width, heads and vocabulary, with init_params weights sharpened as
     test_prefill_gpu.sharp_engine does: x4 on wte, wout and the layer kernels, biases and LayerNorm betas N(0, 0.02)
-    (bout zero past V).  Attention is then peaked rather than uniform.  One engine lives at a time."""
-    if config in _ENGINE:
-        return _ENGINE[config]
+    (bout zero past V).  Attention is then peaked rather than uniform.  One layer, or one per entry of
+    attention_types (local layers at the configuration's local_attention_radius, default 256).  One engine lives at
+    a time."""
+    key = (config, None if attention_types is None else tuple(attention_types))
+    if key in _ENGINE:
+        return _ENGINE[key]
     from dalle_mtf_b200.dalle_engine import DalleEngine
     _ENGINE.clear()
     torch.cuda.empty_cache()
     cfg = DK._config(config)
-    eng = DalleEngine(cfg["n_embd"], 1, cfg["n_heads"], cfg["text_vocab_size"], cfg["image_vocab_size"], TEXT_LEN,
-                      IMAGE_LEN)
+    n_layers = 1 if attention_types is None else len(attention_types)
+    eng = DalleEngine(cfg["n_embd"], n_layers, cfg["n_heads"], cfg["text_vocab_size"], cfg["image_vocab_size"],
+                      TEXT_LEN, IMAGE_LEN, attention_types=attention_types,
+                      local_attention_radius=cfg.get("local_attention_radius", 256))
     eng.init_params(seed=3)
     g = DK._gen(9)
-    for n in ("wte", "wout", "l0.wqkv", "l0.wo", "l0.w1", "l0.w2"):
+    for n in ("wte", "wout") + tuple(f"l{i}.{w}" for i in range(n_layers) for w in ("wqkv", "wo", "w1", "w2")):
         eng.P(n).mul_(4)
-    for n in ("l0.ln1_b", "l0.o_b", "l0.ln2_b", "l0.b1", "l0.b2", "lnf_b"):
+    for n in tuple(f"l{i}.{b}" for i in range(n_layers) for b in ("ln1_b", "o_b", "ln2_b", "b1", "b2")) + ("lnf_b",):
         eng.P(n).copy_(torch.randn(eng.P(n).shape, generator=g, device=DEV) * 0.02)
     eng.P("bout")[:eng.V].copy_(torch.randn(eng.V, generator=g, device=DEV) * 0.02)
     eng.refresh_shadow()
-    _ENGINE[config] = eng
+    _ENGINE[key] = eng
     return eng
 
 
@@ -123,7 +128,7 @@ def describe(name, args, kw):
     if name in ("gemm", "layernorm_fwd", "attn_fwd", "embed_fwd"):
         return DK._describe(name, args, kw)
     if name in ("attn_decode", "attn_decode_dev"):
-        return (name,) + tuple(args[1].shape) + (float(args[5]),)
+        return (name,) + tuple(args[1].shape) + (float(args[5]), kw.get("radius"))
     if name == "embed_fwd_at":
         return (name, args[3].shape[0], args[1].shape[0], args[3].shape[1])
     if name == "embed_fwd_at_dev":
@@ -154,14 +159,16 @@ def wrapped(ops, hook):
 _CALLS = {}
 
 
-def generation_calls(ops, config):
+def generation_calls(ops, config, attention_types=None):
     """Distinct calls of (a) eager DalleSampler.step at STEP_ROWS rows and positions 0, 1, 256, and (b) complete() of
     REC_B prompts with a REC_N-code image prefix, REC_REP samples per prompt and guidance (the captured step at
-    2 REC_B REC_REP rows and the prefill of 2 REC_B prompts).  Also returns the engine's dimensions."""
-    if config in _CALLS:
-        return _CALLS[config]
+    2 REC_B REC_REP rows and the prefill of 2 REC_B prompts), on sharp_engine(config, attention_types).  Also returns
+    the engine's dimensions and its per-layer radii (None: global)."""
+    key = (config, None if attention_types is None else tuple(attention_types))
+    if key in _CALLS:
+        return _CALLS[key]
     from dalle_mtf_b200.sampling import DalleSampler
-    eng = sharp_engine(config)
+    eng = sharp_engine(config, attention_types)
     smp = DalleSampler(eng)
     seen = {"step": {}, "complete": {}}
     phase = ["step"]
@@ -182,11 +189,12 @@ def generation_calls(ops, config):
         out = smp.complete(text, prefix, samples_per_prompt=REC_REP, temperature=0, guidance_scale=REC_GS)
         torch.cuda.synchronize()
     assert out.shape == (REC_B * REC_REP, eng.S)
-    dims = types.SimpleNamespace(d=eng.d, H=eng.H, dh=eng.dh, V=eng.V, Vpad=eng.Vpad, S=eng.S, scale=eng.attn_scale)
+    dims = types.SimpleNamespace(d=eng.d, H=eng.H, dh=eng.dh, V=eng.V, Vpad=eng.Vpad, S=eng.S, scale=eng.attn_scale,
+                                 radii=tuple(eng.radii))
     res = ({k: list(v) for k, v in seen.items()}, dims)
     del smp
     torch.cuda.empty_cache()
-    _CALLS[config] = res
+    _CALLS[key] = res
     return res
 
 
@@ -204,12 +212,25 @@ def step_products(M, dm):
 
 
 def expected_step_calls(rows, dm, graphed):
+    """The distinct calls of one step at `rows` rows: one attn_decode(_dev) shape per distinct layer radius."""
     s = set(step_products(rows, dm)) | {("layernorm_fwd", rows, dm.d)}
     if graphed:
-        s |= {("attn_decode_dev", rows, dm.S, dm.H, dm.dh, dm.scale), ("embed_fwd_at_dev", rows, dm.V, dm.d, dm.S)}
+        s |= {("attn_decode_dev", rows, dm.S, dm.H, dm.dh, dm.scale, r) for r in dm.radii}
+        s |= {("embed_fwd_at_dev", rows, dm.V, dm.d, dm.S)}
     else:
-        s |= {("attn_decode", rows, dm.S, dm.H, dm.dh, dm.scale), ("embed_fwd_at", rows, dm.V, dm.d)}
+        s |= {("attn_decode", rows, dm.S, dm.H, dm.dh, dm.scale, r) for r in dm.radii}
+        s |= {("embed_fwd_at", rows, dm.V, dm.d)}
     return s
+
+
+def expected_prefill_calls(dm):
+    """The distinct calls complete() adds to its step's for the prefill of generation_calls: one attn_fwd shape per
+    distinct layer radius, at S = P."""
+    B2, P, R2 = 2 * REC_B, TEXT_LEN + REC_N, 2 * REC_B * REC_REP
+    T = B2 * P
+    return set(step_products(T, dm)[:4]) | {("attn_fwd", B2, P, dm.H, dm.dh, dm.scale, False, r) for r in dm.radii} | {
+        ("layernorm_fwd", T, dm.d), ("embed_fwd", B2, P, False),
+        ("kv_cache_fill", T, (R2, dm.S, dm.H, dm.dh), P, REC_REP), ("rows_repeat", (B2, dm.d), P * dm.d, REC_REP)}
 
 
 @pytest.mark.parametrize("config", CONFIGS)
@@ -218,13 +239,11 @@ def test_generation_call_set(ops, config):
     embed_fwd_at.  complete() adds the prefill: its embedding, LayerNorm, 4 GEMMs and attention at 2 REC_B prompts of
     P = 256 + REC_N, then kv_cache_fill, rows_repeat, the final LayerNorm and the logits GEMM at the step's rows."""
     calls, dm = generation_calls(ops, config)
+    assert dm.radii == (None,)                            # the configurations' samplers run causal attention
     assert set(calls["step"]) == expected_step_calls(STEP_ROWS, dm, graphed=False), calls["step"]
-    B2, P, R2 = 2 * REC_B, TEXT_LEN + REC_N, 2 * REC_B * REC_REP
-    T = B2 * P
-    prefill = set(step_products(T, dm)[:4]) | {
-        ("layernorm_fwd", T, dm.d), ("attn_fwd", B2, P, dm.H, dm.dh, dm.scale, False), ("embed_fwd", B2, P, False),
-        ("kv_cache_fill", T, (R2, dm.S, dm.H, dm.dh), P, REC_REP), ("rows_repeat", (B2, dm.d), P * dm.d, REC_REP)}
-    assert set(calls["complete"]) == expected_step_calls(R2, dm, graphed=True) | prefill, calls["complete"]
+    R2 = 2 * REC_B * REC_REP
+    assert set(calls["complete"]) == expected_step_calls(R2, dm, graphed=True) | expected_prefill_calls(dm), \
+        calls["complete"]
     print(f"[{TAG}] {config}: eager step {len(calls['step'])} distinct calls, complete() {len(calls['complete'])} "
           f"(d={dm.d} H={dm.H} dh={dm.dh} V={dm.V} Vpad={dm.Vpad})")
 

@@ -52,15 +52,23 @@ def test_dalle_forward_backward_optimizer_match_oracle(d, L, H, tv, iv, ts, isl,
     dalle_step_matches_oracle((d, L, H, tv, iv, ts, isl, B), recompute)
 
 
-def dalle_step_matches_oracle(case, recompute, during_backward=contextlib.nullcontext, dropout=None):
+def dalle_step_matches_oracle(case, recompute, during_backward=contextlib.nullcontext, dropout=None, local=None):
     """Forward, backward (inside during_backward()) and one optimiser step of the engine against the fp32 oracle.
-    dropout: (rates, seed, step, row0) of the step, checked against oracle/dalle_dropout.py."""
+    dropout: (rates, seed, step, row0) of the step, checked against oracle/dalle_dropout.py.  local: (attention_types,
+    radius) of a model with local layers, checked against oracle/dalle_local.py."""
     from oracle import dalle as O
     from oracle import dalle_dropout as D
+    from oracle import dalle_local as OL
     from oracle import optim as OO
     kw = {} if dropout is None else {"dropout": dropout[0], "dropout_seed": dropout[1]}
+    if local is not None:
+        kw.update(attention_types=list(local[0]), local_attention_radius=local[1])
     cfg, params, tokens, eng = _dalle_case(*case, recompute, **kw)
-    if dropout is None:
+    if local is not None:
+        cfg = OL.LocalConfig(*case[:7], attention_types=tuple(local[0]), local_attention_radius=local[1])
+        loss32, _, logits32, g32 = OL.loss_and_grads(params, tokens, cfg, dropout, bf16=False)
+        _, _, _, g16 = OL.loss_and_grads(params, tokens, cfg, dropout, bf16=True)
+    elif dropout is None:
         loss32, _, logits32, g32 = O.loss_and_grads(params, tokens, cfg, bf16=False)
         _, _, _, g16 = O.loss_and_grads(params, tokens, cfg, bf16=True)
     else:

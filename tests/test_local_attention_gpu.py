@@ -55,8 +55,9 @@ def band(S, r):
 
 def local_reference(q, k, v, do, o, scale, r):
     """float64 local attention forward / backward, the |.| graphs and the bounds of the causal kernels' test on
-    [B, S, H, dh] operands (o: the kernel's own output, which delta uses as the kernel does)."""
-    q, k, v, do, o = (t.to(F64).permute(0, 2, 1, 3) for t in (q, k, v, do, o))
+    [B, S, H, dh] operands (o: the kernel's own output, which delta uses as the kernel does).  do = None: the forward
+    only (O and lse; b_bwd is None)."""
+    q, k, v = (t.to(F64).permute(0, 2, 1, 3) for t in (q, k, v))
     S, dh = q.shape[2], q.shape[3]
     mask = band(S, r)
     s = (scale * q @ k.transpose(-1, -2)).masked_fill(~mask, -math.inf)
@@ -70,14 +71,18 @@ def local_reference(q, k, v, do, o, scale, r):
     eps_lse = eps_row + (S + 32) * U + (nblk + 4) * 2.0 ** -21 + 2 * U * lse.abs()
     out = {"O": (P @ v, P @ v.abs()), "lse": (lse, eps_lse)}
     b_fwd = UBF + 2 * eps_row + (2 * nblk + 2) * 2.0 ** -21 + (2 * S + 2 * nblk + 32) * UTC
-    dP, dPa = do @ v.transpose(-1, -2), do.abs() @ v.abs().transpose(-1, -2)
-    delta, deltaa = (do * o).sum(-1, keepdim=True), (do * o).abs().sum(-1, keepdim=True)
-    dS, dSa = P * (dP - delta), P * (dPa + deltaa)
-    out["dQ"] = (scale * dS @ k, scale * dSa @ k.abs())
-    out["dK"] = (scale * dS.transpose(-1, -2) @ q, scale * dSa.transpose(-1, -2) @ q.abs())
-    out["dV"] = (P.transpose(-1, -2) @ do, P.transpose(-1, -2) @ do.abs())
-    b_bwd = (eps_s + eps_lse[..., None]).masked_fill(~mask, 0).max().item() + 2.0 ** -20 + UBF + (S + dh + 24) * UTC
-    out = {n: (x.permute(0, 2, 1, 3) if x.dim() == 4 else x, a.permute(0, 2, 1, 3) if a.dim() == 4 else a)
+    b_bwd = None
+    if do is not None:
+        do, o = do.to(F64).permute(0, 2, 1, 3), o.to(F64).permute(0, 2, 1, 3)
+        dP, dPa = do @ v.transpose(-1, -2), do.abs() @ v.abs().transpose(-1, -2)
+        delta, deltaa = (do * o).sum(-1, keepdim=True), (do * o).abs().sum(-1, keepdim=True)
+        dS, dSa = P * (dP - delta), P * (dPa + deltaa)
+        out["dQ"] = (scale * dS @ k, scale * dSa @ k.abs())
+        out["dK"] = (scale * dS.transpose(-1, -2) @ q, scale * dSa.transpose(-1, -2) @ q.abs())
+        out["dV"] = (P.transpose(-1, -2) @ do, P.transpose(-1, -2) @ do.abs())
+        b_bwd = (eps_s + eps_lse[..., None]).masked_fill(~mask, 0).max().item() + 2.0 ** -20 + UBF + \
+            (S + dh + 24) * UTC
+    out = {n:(x.permute(0, 2, 1, 3) if x.dim() == 4 else x, a.permute(0, 2, 1, 3) if a.dim() == 4 else a)
            for n, (x, a) in out.items()}
     return out, b_fwd.permute(0, 2, 1)[..., None], b_bwd
 

@@ -6,6 +6,8 @@ shapes the bench is quoted on, with the batch cut to what the CPU oracle finishe
   * EX   = configs[1] dalle_example @ BASELINE: d512 / L6 / H4 (dh128) / S = 256 + 1024 / V = 50 771 (odd: the padded
            vocabulary tail Vpad = 50 816 and the cross-entropy epilogues over 397 column tiles are only exercised here), B = 2;
   * CO   = configs[3] dalle_coco  @ BASELINE geometry: d1024 / H16 (dh64) / S = 1280 / recompute_grad, L cut to 2, B = 1;
+  * EXL / COL = EX / CO with local (sliding-window) layers of radius 256: [global, local] x 3 / [global, local],
+           against oracle/dalle_local.py under the same criteria;
   * VC   = configs[2] vae_coco    @ BASELINE geometry: 256 px, convblocks [[2,128],[3,256],[5,512]], K = 8192 (bf16
            activations, fp32-split codebook GEMMs), B = 1;
   * TOK  = the bench's tokenizer config (vae_example_b200: 256 px, K = 512, bf16 tensor-core convolutions): token
@@ -52,12 +54,19 @@ def _randomise_small_params(params, g):
             params[k] = 1 + torch.randn(params[k].shape, generator=g) * 0.05
 
 
-def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed):
+def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed, attention_types=None, radius=256):
+    """attention_types: one "global" / "local" per layer (local layers of `radius`), against oracle/dalle_local.py."""
     from dalle_mtf_b200.dalle_engine import DalleEngine
     from oracle import dalle as O
+    from oracle import dalle_local as OL
     from oracle import optim as OO
     torch.set_num_threads(max(1, os.cpu_count() or 1))
-    cfg = O.DalleConfig(d, L, H, tv, iv, ts, isl)
+    if attention_types is None:
+        cfg, oracle = O.DalleConfig(d, L, H, tv, iv, ts, isl), O
+    else:
+        cfg = OL.LocalConfig(d, L, H, tv, iv, ts, isl, attention_types=tuple(attention_types),
+                             local_attention_radius=radius)
+        oracle = OL
     params = O.init_params(cfg, seed)
     g = torch.Generator().manual_seed(seed + 1)
     _randomise_small_params(params, g)
@@ -67,10 +76,11 @@ def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed):
         text[b, 5 + 20 * b:] = tv - 1
     img = torch.randint(0, iv, (B, isl), generator=g)
     tokens = O.assemble_tokens(text, img, tv)
-    loss32, rows32, logits32, g32 = O.loss_and_grads(params, tokens, cfg, bf16=False)
-    _, rows16, logits16, g16 = O.loss_and_grads(params, tokens, cfg, bf16=True)
+    loss32, rows32, logits32, g32 = oracle.loss_and_grads(params, tokens, cfg, bf16=False)
+    _, rows16, logits16, g16 = oracle.loss_and_grads(params, tokens, cfg, bf16=True)
 
-    eng = DalleEngine(d, L, H, tv, iv, ts, isl, recompute_grad=recompute)
+    eng = DalleEngine(d, L, H, tv, iv, ts, isl, recompute_grad=recompute, attention_types=attention_types,
+                      local_attention_radius=radius)
     eng.load_params(params)
     tok = tokens.to(torch.int32).to(DEV)
     T = tokens.numel()
@@ -129,6 +139,19 @@ def test_dalle_example_full_baseline_shape_matches_oracle():
 def test_dalle_coco_geometry_recompute_matches_oracle():
     """CO geometry: d1024 / H16 (dh = 64) / S1280 / recompute_grad (src/dalle_mtf/models.py:342-343), L cut to 2."""
     _dalle_parity("CO d1024 L2 H16 S1280 V50771 B1 recompute", 1024, 2, 16, 50258, 512, 256, 1024, 1, True, seed=12)
+
+
+def test_dalle_example_with_local_layers_matches_oracle():
+    """EXL: the EX shape with layers [global, local] x 3 of radius 256 (configs/dalle_example_local_b200.json),
+    against oracle/dalle_local.py."""
+    _dalle_parity("EXL d512 L6 H4 S1280 V50771 B2 global/local r256", 512, 6, 4, 50258, 512, 256, 1024, 2, False,
+                  seed=14, attention_types=["global", "local"] * 3, radius=256)
+
+
+def test_dalle_coco_geometry_with_a_local_layer_matches_oracle():
+    """COL: the CO geometry (d1024 / H16 / S1280 / recompute_grad, L = 2) with layers [global, local] of radius 256."""
+    _dalle_parity("COL d1024 L2 H16 S1280 V50771 B1 recompute global/local r256", 1024, 2, 16, 50258, 512, 256, 1024,
+                  1, True, seed=15, attention_types=["global", "local"], radius=256)
 
 
 def test_vae_coco_geometry_k8192_bf16_matches_oracle():

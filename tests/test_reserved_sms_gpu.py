@@ -268,7 +268,10 @@ def test_edge_convolutions_with_64_sms_reserved(ops, N, H, Cin, Cout, k, stride,
 
 # ------------------------------------------------------------------------------------------------------- engines
 DROPOUT = ((0.1, 0.2, 0.15), 11, 6, 1)          # (embed, attention, residual) rates, seed, step, row0
-ENGINE_CASES = [(c[:8], c[8], None) for c in EG.DALLE_CASES] + [(EG.DALLE_CASES[2][:8], True, DROPOUT)]
+# a case may end in (attention_types, radius): the last one has a local layer (no attention dropout there)
+ENGINE_CASES = [(c[:8], c[8], None) for c in EG.DALLE_CASES] + [(EG.DALLE_CASES[2][:8], True, DROPOUT),
+                                                                 (EG.DALLE_CASES[2][:8] + (("global", "local"), 100),
+                                                                  True, DROPOUT)]
 
 
 @pytest.mark.parametrize("k", [4, 16])
@@ -277,7 +280,8 @@ def test_dalle_step_with_the_backward_under_reservation(ops, case, recompute, dr
     """As train_op runs it: forward with every SM, backward (and with recompute_grad the recomputed block forward)
     with k reserved, the optimiser step after the reservation ends; the criteria of
     test_dalle_forward_backward_optimizer_match_oracle."""
-    EG.dalle_step_matches_oracle(case, recompute, lambda: reserved_sms(k), dropout=dropout)
+    EG.dalle_step_matches_oracle(case[:8], recompute, lambda: reserved_sms(k), dropout=dropout,
+                                 local=case[8:] or None)
     line(k, max(device_sms() - k, 16), f"DalleEngine {case} recompute={recompute} dropout={dropout is not None}: "
          "forward / backward / optimizer step match the oracle")
 

@@ -2,6 +2,7 @@
 // error codes + thread-local message (the C ABI never throws, never exits), TMA tensor-map encoding via the
 // driver entry point (no link-time dependency on libcuda), launch checks.
 #pragma once
+#include <cmath>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -33,6 +34,17 @@ int check_launch(const char* what);             // cudaGetLastError() -> DB200_E
   } while (0)
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// the weighted cross-entropy descriptor (db200_gemm_bf16_ce_weighted, db200_ce_finish_weighted)
+static inline int ce_weights_check(const db200_ce_weights* w, const char* what) {
+  DB200_REQUIRE(w != nullptr, DB200_E_INVALID, "%s: NULL weights descriptor", what);
+  DB200_REQUIRE(w->period > 0 && w->text_rows >= 0 && w->text_rows <= w->period, DB200_E_INVALID,
+                "%s: need period > 0 and 0 <= text_rows <= period (got %d, %d)", what, w->period, w->text_rows);
+  DB200_REQUIRE(std::isfinite(w->a_text) && std::isfinite(w->a_image) && std::isfinite(w->z_loss) && w->a_text >= 0.f &&
+                    w->a_image >= 0.f && w->z_loss >= 0.f,
+                DB200_E_INVALID, "%s: a_text, a_image and z_loss must be finite and >= 0", what);
+  return DB200_OK;
+}
 
 // ---- TMA tensor maps ------------------------------------------------------------------------------
 // rank <= 5; dims[0] is the innermost (contiguous) dimension; strides_bytes[i] is the byte stride of dims[i+1].

@@ -42,8 +42,9 @@ static_assert(128 * G_REGS_PRODUCER + 256 * G_REGS_MMA + 128 * G_REGS_EPI <= 655
 // named barriers of the accumulator-tile hand-off: 256 MMA threads + 128 epilogue threads
 constexpr int G_BAR_FULL = 1, G_BAR_EMPTY = 2, G_BAR_HANDOFF_THREADS = 384;
 
-// operand majors (1 = MN-major), compile-time for wgmma; DROP: dropout in the STORE epilogue
-template <int TA, int TB, bool DROP>
+// operand majors (1 = MN-major), compile-time for wgmma; DROP: dropout in the STORE epilogue; WCE: the weighted CE_GRAD
+// epilogue (instantiated for the vocabulary product only: A K-major, B MN-major)
+template <int TA, int TB, bool DROP, bool WCE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr int BN = GBN;
@@ -184,6 +185,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int half = 0; half < 2; ++half) {  // columns [half * BN/2, (half + 1) * BN/2) of the tile
         const int cbase = n0 + half * (BN / 2);
         const uint32_t t_addr = (sAcc >> 2) + (ew * 32 + lane) * BN + half * (BN / 2);
+        if constexpr (WCE) {
+          epi_ce_grad_weighted<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane);
+          continue;
+        }
         switch (p.mode) {
           case DB200_EPI_STORE:    epi_store<CH, DROP>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
           case DB200_EPI_ATOMIC:
@@ -201,15 +206,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
-template <int TA, int TB, bool DROP>
+template <int TA, int TB, bool DROP, bool WCE = false>
 static int launch_gemm(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP, WCE>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                           (int)G_SMEM_BYTES);  // once, thread-safe (magic static)
   DB200_CUDA(attr_rc);
   const int total = p.m_tiles * p.n_tiles * p.splits;
   const int grid = total < sm_count() ? total : sm_count();
-  gemm_tc_kernel<TA, TB, DROP><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_tc_kernel<TA, TB, DROP, WCE><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
   return check_launch("gemm_tc_kernel");
 }
 
@@ -252,9 +257,10 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   return db200_gemm_bf16_ex(stream_, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr);
 }
 
-extern "C" int db200_gemm_bf16_ex(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B,
-                                  int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
-                                  const db200_gemm_epilogue* epi, const db200_dropout* dropout) {
+// every product: cew != NULL selects the weighted CE_GRAD epilogue (validated by db200_gemm_bf16_ce_weighted)
+static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
+                    int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi,
+                    const db200_dropout* dropout, const db200_ce_weights* cew) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(epi != nullptr, DB200_E_INVALID, "gemm: epilogue descriptor is NULL");
   const bool drop = dropout_active(dropout);
@@ -290,7 +296,7 @@ extern "C" int db200_gemm_bf16_ex(db200_stream_t stream_, const void* A, int a_m
                       epi->n_valid <= N,
                   DB200_E_INVALID, "gemm: CE_STATS needs labels/part_max/part_sum/label_logit and 0 < n_valid <= N");
   if (mode == DB200_EPI_CE_GRAD)
-    DB200_REQUIRE(epi->labels && epi->lse && epi->n_valid > 0 && epi->n_valid <= N && epi->alpha > 0.f,
+    DB200_REQUIRE(epi->labels && epi->lse && epi->n_valid > 0 && epi->n_valid <= N && (cew || epi->alpha > 0.f),
                   DB200_E_INVALID, "gemm: CE_GRAD needs labels/lse, 0 < n_valid <= N and alpha > 0");
   DB200_REQUIRE(mode == DB200_EPI_ATOMIC || epi->split_k <= 1, DB200_E_INVALID,
                 "gemm: split_k > 1 is only valid with DB200_EPI_ATOMIC");
@@ -325,6 +331,7 @@ extern "C" int db200_gemm_bf16_ex(db200_stream_t stream_, const void* A, int a_m
   p.n_valid = epi->n_valid;
   p.colsum = (mode == DB200_EPI_CE_GRAD || mode == DB200_EPI_RELU_BWD) ? epi->colsum : nullptr;
   p.drop = drop ? *dropout : db200_dropout{};
+  p.cew = cew ? *cew : db200_ce_weights{};
 
   p.n_tiles = (N + GBN - 1) / GBN;
   p.n_parts = 2 * p.n_tiles;
@@ -363,7 +370,10 @@ extern "C" int db200_gemm_bf16_ex(db200_stream_t stream_, const void* A, int a_m
   } else if (colsum_out) {
     p.colsum = static_cast<float*>(epi->workspace);
   }
-  if (drop)    // residual dropout runs in forward products only: A k-major, B mn-major
+  if (cew)     // the vocabulary product: A k-major, B mn-major
+    rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, true>(stream, tmA, tmB, p)
+                             : set_error(DB200_E_UNSUPPORTED, "gemm: weighted CE_GRAD needs a k-major A and an mn-major B");
+  else if (drop)    // residual dropout runs in forward products only: A k-major, B mn-major
     rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, true>(stream, tmA, tmB, p)
                              : set_error(DB200_E_UNSUPPORTED, "gemm: dropout needs a k-major A and an mn-major B");
   else if (p.a_mn) rc = p.b_mn ? launch_gemm<1, 1, false>(stream, tmA, tmB, p) : launch_gemm<1, 0, false>(stream, tmA, tmB, p);
@@ -372,4 +382,20 @@ extern "C" int db200_gemm_bf16_ex(db200_stream_t stream_, const void* A, int a_m
   if (p.splits > 1) return reduce_splits_add(stream, static_cast<const float*>(p.D), p.splits, M, N, d_out, ldd);
   if (colsum_out) return reduce_rows_add(stream, p.colsum, row_blocks, N, colsum_out);
   return DB200_OK;
+}
+
+extern "C" int db200_gemm_bf16_ex(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                                  int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                                  const db200_gemm_epilogue* epi, const db200_dropout* dropout) {
+  return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, dropout, nullptr);
+}
+
+extern "C" int db200_gemm_bf16_ce_weighted(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda,
+                                           const void* B, int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M,
+                                           int N, int K, const db200_gemm_epilogue* epi, const db200_ce_weights* w) {
+  DB200_REQUIRE(epi != nullptr && epi->mode == DB200_EPI_CE_GRAD, DB200_E_INVALID,
+                "gemm_ce_weighted: needs an epilogue descriptor with mode DB200_EPI_CE_GRAD");
+  const int rc = ce_weights_check(w, "gemm_ce_weighted");
+  if (rc != DB200_OK) return rc;
+  return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, w);
 }

@@ -38,6 +38,7 @@ struct GemmParams {
   int n_parts;  // CE_STATS: partials per row = 2 * n_tiles (one per half tile)
   float* colsum;  // CE_GRAD / RELU_BWD: workspace [M/32 row blocks][N] of column sums (bias gradient), or NULL
   db200_dropout drop;  // STORE with dropout (kernel instantiated with DROP = true): elementwise mask over [M][N]
+  db200_ce_weights cew;  // weighted CE_GRAD (kernel instantiated with WCE = true): per-row class coefficients and z
 };
 
 struct TileCoord {
@@ -466,6 +467,73 @@ __device__ __forceinline__ void epi_ce_grad(const GemmParams& p, uint32_t t_addr
     }
     if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, lane);
     stage_flush<2, true>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);  // 4 GB of dlogits: stream past L2
+  }
+}
+
+// Weighted CE_GRAD: dlogits = a (c' softmax - onehot) with a = a_text for rows t with t mod period < text_rows, else
+// a_image, and c' = 1 + 2 z lse (the z-loss z lse^2 adds 2 z lse softmax to the gradient).  c = a c' is formed once per
+// row; |c| is folded into the exponent as in epi_ce_grad and its sign applied afterwards.  c = 0 (a zero-weight class,
+// or c' = 0) gives log2 |c| = -inf, hence exp2(-inf) = 0: the row's softmax term is exactly 0, as is its label term.
+template <int CH>
+__device__ __forceinline__ void epi_ce_grad_weighted(const GemmParams& p, uint32_t t_addr, int row, bool row_ok,
+                                                     int cbase, uint32_t stg, int row0, int lane) {
+  const int label = row_ok ? p.labels[row] : -1;
+  float a = 0.f, l2 = 0.f;
+  bool neg = false;
+  if (row_ok) {
+    a = (row % p.cew.period) < p.cew.text_rows ? p.cew.a_text : p.cew.a_image;
+    const float lse = p.lse[row];
+    const float c = a * fmaf(2.f * p.cew.z_loss, lse, 1.f);
+    neg = c < 0.f;
+    l2 = fmaf(lse, kLog2e, -log2f(fabsf(c)));
+  }
+#pragma unroll 1
+  for (int pc = 0; pc < CH / 2; ++pc) {
+    const int colp = cbase + pc * 64;
+    if (colp >= p.N) break;
+    uint32_t rr2[2][32];
+    acc_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
+    acc_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int col0 = colp + h * 32;
+      const uint32_t* r = rr2[h];
+      float o[32];
+      if (col0 + 32 <= p.n_valid) {  // interior chunk (warp-uniform)
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          float b[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+          if (p.bias) load8(p.bias + col0 + g * 8, b);
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            o[g * 8 + j] = fast_exp2(fmaf(__uint_as_float(r[g * 8 + j]) + b[j], kLog2e, -l2));
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int cc = col0 + j;
+          o[j] = cc < p.n_valid
+                     ? fast_exp2(fmaf(__uint_as_float(r[j]) + (p.bias ? __ldg(p.bias + cc) : 0.f), kLog2e, -l2))
+                     : 0.f;
+        }
+      }
+      if (neg) {  // only rows with lse < -1 / (2 z)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) o[j] = -o[j];
+      }
+      if (label >= col0 && label < col0 + 32) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+          if (col0 + j == label) o[j] -= a;
+      }
+      if (!row_ok) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) o[j] = 0.f;
+      }
+      stage_put_bf16(stg, lane, h, o);
+    }
+    if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, lane);
+    stage_flush<2, true>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
   }
 }
 

@@ -575,13 +575,10 @@ __global__ void split_f32_kernel(const float* __restrict__ src, bf16* __restrict
 // line per store.  Here a block owns 32 consecutive rows; warp g of 8 folds tiles g, g+8, ... (every load is one
 // 128-byte line), then the 8 partial (max, sum) pairs of a row are merged through shared memory.
 constexpr int CEF_ROWS = 32, CEF_GROUPS = 8;
-__global__ void __launch_bounds__(CEF_ROWS * CEF_GROUPS)
-ce_finish_kernel(const float* __restrict__ part_max, const float* __restrict__ part_sum,
-                 const float* __restrict__ label_logit, float* __restrict__ lse, float* __restrict__ loss_rows,
-                 float* __restrict__ loss_sum, int M, int n_tiles) {
-  __shared__ float sm_m[CEF_GROUPS][CEF_ROWS], sm_s[CEF_GROUPS][CEF_ROWS];
-  const int r = threadIdx.x & 31, g = threadIdx.x >> 5;
-  const int row = blockIdx.x * CEF_ROWS + r;
+// warp g folds tiles g, g + 8, ... of row `row` into one (max, sum) pair, stored at sm_m / sm_s[g][r]; block barrier
+__device__ __forceinline__ void ce_fold_tiles(const float* __restrict__ part_max, const float* __restrict__ part_sum,
+                                              int M, int n_tiles, int row, int r, int g,
+                                              float (*sm_m)[CEF_ROWS], float (*sm_s)[CEF_ROWS]) {
   float m = -INFINITY, s = 0.f;
   if (row < M) {
     constexpr int U = 4;  // tiles in flight per thread: the loop is load-latency bound otherwise
@@ -607,23 +604,71 @@ ce_finish_kernel(const float* __restrict__ part_max, const float* __restrict__ p
   sm_m[g][r] = m;
   sm_s[g][r] = s;
   __syncthreads();
+}
+// lse of row r of the block from the CEF_GROUPS folded pairs
+__device__ __forceinline__ float ce_merge_lse(float (*sm_m)[CEF_ROWS], float (*sm_s)[CEF_ROWS], int r) {
+  float mm = -INFINITY;
+#pragma unroll
+  for (int i = 0; i < CEF_GROUPS; ++i) mm = fmaxf(mm, sm_m[i][r]);
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < CEF_GROUPS; ++i)
+    if (sm_m[i][r] > -INFINITY) ss += sm_s[i][r] * expf(sm_m[i][r] - mm);
+  return mm + logf(ss);
+}
+
+__global__ void __launch_bounds__(CEF_ROWS * CEF_GROUPS)
+ce_finish_kernel(const float* __restrict__ part_max, const float* __restrict__ part_sum,
+                 const float* __restrict__ label_logit, float* __restrict__ lse, float* __restrict__ loss_rows,
+                 float* __restrict__ loss_sum, int M, int n_tiles) {
+  __shared__ float sm_m[CEF_GROUPS][CEF_ROWS], sm_s[CEF_GROUPS][CEF_ROWS];
+  const int r = threadIdx.x & 31, g = threadIdx.x >> 5;
+  const int row = blockIdx.x * CEF_ROWS + r;
+  ce_fold_tiles(part_max, part_sum, M, n_tiles, row, r, g, sm_m, sm_s);
   if (g == 0) {
     float loss = 0.f;
     if (row < M) {
-      float mm = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < CEF_GROUPS; ++i) mm = fmaxf(mm, sm_m[i][r]);
-      float ss = 0.f;
-#pragma unroll
-      for (int i = 0; i < CEF_GROUPS; ++i)
-        if (sm_m[i][r] > -INFINITY) ss += sm_s[i][r] * expf(sm_m[i][r] - mm);
-      const float l = mm + logf(ss);
+      const float l = ce_merge_lse(sm_m, sm_s, r);
       loss = l - label_logit[row];
       lse[row] = l;
       loss_rows[row] = loss;
     }
     loss = warp_sum(loss);
     if (r == 0) loss_sum[blockIdx.x] = loss;  // per-block partial, summed in block order by the launcher
+  }
+}
+
+// Weighted finish: loss_rows = CE + z lse^2; per-block partials [blocks][4] of (sum a loss_rows, text CE, image CE,
+// z lse^2), added in block order by the launcher.
+__global__ void __launch_bounds__(CEF_ROWS * CEF_GROUPS)
+ce_finish_weighted_kernel(const float* __restrict__ part_max, const float* __restrict__ part_sum,
+                          const float* __restrict__ label_logit, float* __restrict__ lse, float* __restrict__ loss_rows,
+                          float* __restrict__ partials, int M, int n_tiles, const db200_ce_weights w) {
+  __shared__ float sm_m[CEF_GROUPS][CEF_ROWS], sm_s[CEF_GROUPS][CEF_ROWS];
+  const int r = threadIdx.x & 31, g = threadIdx.x >> 5;
+  const int row = blockIdx.x * CEF_ROWS + r;
+  ce_fold_tiles(part_max, part_sum, M, n_tiles, row, r, g, sm_m, sm_s);
+  if (g == 0) {
+    float weighted = 0.f, ce_text = 0.f, ce_image = 0.f, zterm = 0.f;
+    if (row < M) {
+      const float l = ce_merge_lse(sm_m, sm_s, r);
+      const float ce = l - label_logit[row];
+      zterm = w.z_loss * l * l;
+      const float loss = ce + zterm;
+      const bool text = (row % w.period) < w.text_rows;
+      weighted = (text ? w.a_text : w.a_image) * loss;
+      (text ? ce_text : ce_image) = ce;
+      lse[row] = l;
+      loss_rows[row] = loss;
+    }
+    weighted = warp_sum(weighted);
+    ce_text = warp_sum(ce_text);
+    ce_image = warp_sum(ce_image);
+    zterm = warp_sum(zterm);
+    if (r == 0) {
+      float* o = partials + 4 * (long long)blockIdx.x;
+      o[0] = weighted; o[1] = ce_text; o[2] = ce_image; o[3] = zterm;
+    }
   }
 }
 
@@ -945,4 +990,29 @@ extern "C" int db200_ce_finish(db200_stream_t stream_, const float* part_max, co
   const int rc = check_launch("ce_finish_kernel");
   if (rc != DB200_OK) return rc;
   return reduce_rows_add(stream, ws, blocks, 1, loss_sum);
+}
+
+extern "C" int64_t db200_ce_finish_weighted_workspace_bytes(int M) {
+  return (int64_t)((M + CEF_ROWS - 1) / CEF_ROWS) * 4 * (int64_t)sizeof(float);
+}
+
+extern "C" int db200_ce_finish_weighted(db200_stream_t stream_, const float* part_max, const float* part_sum,
+                                        const float* label_logit, float* lse, float* loss_rows, float* sums, int M,
+                                        int n_tiles, const db200_ce_weights* w, void* workspace,
+                                        int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(M > 0 && n_tiles > 0, DB200_E_INVALID, "ce_finish_weighted: M and n_tiles must be positive");
+  DB200_REQUIRE(part_max && part_sum && label_logit && lse && loss_rows && sums, DB200_E_INVALID,
+                "ce_finish_weighted: NULL pointer");
+  const int rc0 = ce_weights_check(w, "ce_finish_weighted");
+  if (rc0 != DB200_OK) return rc0;
+  const int blocks = (M + CEF_ROWS - 1) / CEF_ROWS;
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_ce_finish_weighted_workspace_bytes(M)), DB200_E_INVALID,
+                "ce_finish_weighted: needs an aligned workspace of db200_ce_finish_weighted_workspace_bytes() bytes");
+  float* ws = static_cast<float*>(workspace);
+  ce_finish_weighted_kernel<<<blocks, CEF_ROWS * CEF_GROUPS, 0, stream>>>(part_max, part_sum, label_logit, lse,
+                                                                          loss_rows, ws, M, n_tiles, *w);
+  const int rc = check_launch("ce_finish_weighted_kernel");
+  if (rc != DB200_OK) return rc;
+  return reduce_rows_add(stream, ws, blocks, 4, sums);
 }

@@ -75,6 +75,42 @@ def layer_radii(attention_types, radius, n_layers):
     return [int(radius) if t == "local" else None for t in types]
 
 
+def _real(v):
+    return isinstance(v, numbers.Real) and not isinstance(v, bool)
+
+
+def validate_loss_weights(text_loss_weight=None, image_loss_weight=None, z_loss=None):
+    """((w_text, w_image) or None, z) of the weighted loss.  Both weights or neither, each a finite real >= 0 with a
+    sum > 0; z a finite real >= 0 (None: 0)."""
+    if (text_loss_weight is None) != (image_loss_weight is None):
+        raise ValueError("text_loss_weight and image_loss_weight must be given together "
+                         f"(got {text_loss_weight!r}, {image_loss_weight!r})")
+    for name, v in (("text_loss_weight", text_loss_weight), ("image_loss_weight", image_loss_weight),
+                    ("z_loss", z_loss)):
+        if v is not None and not (_real(v) and math.isfinite(v) and v >= 0):
+            raise ValueError(f"{name} = {v!r}: must be a finite real number >= 0")
+    weights = None
+    if text_loss_weight is not None:
+        weights = (float(text_loss_weight), float(image_loss_weight))
+        if weights[0] + weights[1] <= 0:
+            raise ValueError("text_loss_weight + image_loss_weight must be > 0")
+    return weights, 0.0 if z_loss is None else float(z_loss)
+
+
+def loss_coefficients(loss_weights, text_seq_len, image_seq_len, global_batch):
+    """(a_text, a_image): the coefficient of one text / image row's loss in the weighted loss
+        (w_t sum_text l / (B (TL - 1)) + w_i sum_image l / (B (IL + 1))) / (w_t + w_i),  B = global_batch.
+    A text row predicts a text token (positions p < TL - 1), an image row an image token or EOS.  Without weights
+    (loss_weights None) every row carries 1 / (B S), the reference's mean over all positions."""
+    n_text, n_image = text_seq_len - 1, image_seq_len + 1
+    if loss_weights is None:
+        a = 1.0 / (global_batch * (n_text + n_image))
+        return a, a
+    wt, wi = loss_weights
+    a_text = wt / ((wt + wi) * global_batch * n_text) if n_text > 0 else 0.0
+    return a_text, wi / ((wt + wi) * global_batch * n_image)
+
+
 class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
@@ -82,7 +118,7 @@ class DalleEngine:
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
-                 dropout_seed=0, attention_types=None, local_attention_radius=256):
+                 dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -94,7 +130,12 @@ class DalleEngine:
         zero: a DataParallel with world > 1 turns on optimiser-state sharding (ZeRO-1, SURVEY.md §7 "12 B in pure
         DP"): fp32 master / Adam m / Adam v exist only for this rank's 1/N slice of the flat buffer, the bf16 compute
         copy and the fp32 gradients stay full; after the (all-reduced) gradients are final every rank updates its
-        slice and the bf16 parameters are all-gathered in place.  Still data parallel: same batch split, same maths."""
+        slice and the bf16 parameters are all-gathered in place.  Still data parallel: same batch split, same maths.
+
+        loss_weights = (w_text, w_image) and z_loss: the weighted loss of loss_coefficients() with z_loss * lse^2 added
+        to every row (validate_loss_weights).  With either active, forward() accumulates four sums (weighted loss,
+        text-row CE, image-row CE, z-term) and backward() runs the weighted CE_GRAD epilogue; otherwise the step is
+        the reference's."""
         L.require_device()
         self.d, self.L, self.H = n_embd, n_layers, n_heads
         assert n_embd % n_heads == 0, "n_state must be divisible by n_heads"  # src/dalle_mtf/models.py:232
@@ -122,6 +163,10 @@ class DalleEngine:
         self._drop = None            # descriptors of the current forward (None: no dropout)
         # per layer: None (global, causal attention) or the window radius of a local layer
         self.radii = layer_radii(attention_types, local_attention_radius, n_layers)
+        lw = (None, None) if loss_weights is None else tuple(loss_weights)
+        self.loss_weights, self.z_loss = validate_loss_weights(*lw, z_loss)
+        self.weighted_loss = self.loss_weights is not None or self.z_loss > 0
+        self._cew = None             # lib.CeWeights of the current forward (weighted loss only)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         lay = ParamLayout()
@@ -140,7 +185,8 @@ class DalleEngine:
         self.layout = lay
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
-        #   [0] = sum of per-token losses of this rank / (global tokens)
+        #   [0] = sum of per-token losses of this rank (weighted loss: sum of a_t * loss_t)
+        #   [1..3] = weighted loss only: text-row CE sum, image-row CE sum, z-term sum
         self.aux_off = lay.size
         n = lay.size + 64
         dev = self.device
@@ -438,10 +484,27 @@ class DalleEngine:
         ops.linear_fwd(sv["h1"], self.W(p + "w2"), x_out, bias=self.P(p + "b2"), residual=sv["xmid"],
                        dropout=self._site("mlp_out", i))                                # :321-323,333
 
-    def forward(self, tokens, loss_accum=None, step=None, row0=0):
+    def ce_weights(self, global_batch):
+        """lib.CeWeights of the weighted loss for a step over `global_batch` sequences (all ranks and micro-batches)."""
+        a_text, a_image = loss_coefficients(self.loss_weights, self.text_seq_len, self.image_seq_len, global_batch)
+        return L.make_ce_weights(self.S, self.text_seq_len - 1, a_text, a_image, self.z_loss)
+
+    def loss_part_scales(self, global_batch):
+        """Factors that turn the sums [1..3] of a weighted forward into the text-row mean CE, the image-row mean CE
+        and the mean z-term over all rows."""
+        n_text = max(self.text_seq_len - 1, 1)
+        return 1.0 / (global_batch * n_text), 1.0 / (global_batch * (self.image_seq_len + 1)), \
+            1.0 / (global_batch * self.S)
+
+    def forward(self, tokens, loss_accum=None, step=None, row0=0, global_batch=None):
         """tokens int32 [B,S] on the device.  Adds sum_t loss_rows[t] of this batch into the 1-element fp32 tensor
         `loss_accum` (default: the aux slot behind the gradients, which rides along with the gradient all-reduce)
         and returns it.  The mean over all positions (src/dalle_mtf/models.py:353-354) is that sum / (global B*S).
+
+        Weighted loss (loss_weights / z_loss): loss_rows[t] = CE_t + z lse_t^2 and loss_accum (4 floats, default aux
+        slots 0-3) receives (sum_t a_t loss_rows[t], text-row CE sum, image-row CE sum, z-term sum), with the
+        coefficients a_t of a step over `global_batch` sequences (default B): slot 0 then is this batch's share of the
+        loss itself.
 
         step: the global optimiser step of a training forward; with a step the dropout rates apply (mode "train"),
         without one they do not.  row0: global index of tokens[0] in the step's batch (rank and micro-batch offset),
@@ -467,6 +530,13 @@ class DalleEngine:
         ops.gemm(bufs["hf"], self.W("wout"), None, T, self.Vpad, self.d, a_mn=False, b_mn=True, mode=L.EPI_CE_STATS,
                  bias=self.P("bout"), labels=labels, part_max=bufs["part_max"], part_sum=bufs["part_sum"],
                  label_logit=bufs["label_logit"], n_valid=self.V)
+        if self.weighted_loss:
+            self._cew = self.ce_weights(B if global_batch is None else global_batch)
+            if loss_accum is None:
+                loss_accum = self.grads[self.aux_off:self.aux_off + 4]
+            ops.ce_finish_weighted(bufs["part_max"], bufs["part_sum"], bufs["label_logit"], bufs["lse_v"],
+                                   bufs["loss_rows"], loss_accum, self._cew)
+            return loss_accum
         if loss_accum is None:
             loss_accum = self.grads[self.aux_off:self.aux_off + 1]
         ops.ce_finish(bufs["part_max"], bufs["part_sum"], bufs["label_logit"], bufs["lse_v"], bufs["loss_rows"],
@@ -477,7 +547,7 @@ class DalleEngine:
         """fp32 logits [B,S,V] (return_logits=True path, src/dalle_mtf/models.py:412-415).  Test / eval use only:
         this materialises the tensor the training path never writes."""
         B, S = tokens.shape
-        self.forward(tokens, loss_accum=torch.zeros(1, dtype=F32, device=self.device))
+        self.forward(tokens, loss_accum=torch.zeros(4 if self.weighted_loss else 1, dtype=F32, device=self.device))
         T = B * S
         out = torch.empty(T, self.Vpad, dtype=F32, device=self.device)
         ops.gemm(self._bufs["hf"], self.W("wout"), out, T, self.Vpad, self.d, a_mn=False, b_mn=True,
@@ -578,16 +648,21 @@ class DalleEngine:
                             self._site("mlp_out", i - 1) if i > 0 else None)          # db2 of the layer below
 
     def backward(self, grad_scale, on_bucket_ready=None):
-        """Back-propagates d(sum(loss_rows) * grad_scale).  Gradients ACCUMULATE into self.grads.
+        """Back-propagates d(sum(loss_rows) * grad_scale); with the weighted loss d(sum_t a_t loss_rows[t] * grad_scale)
+        (the coefficients of the preceding forward).  Gradients ACCUMULATE into self.grads.
         on_bucket_ready(start, end) is called as soon as the flat range [start, end) is final (data-parallel hook)."""
         bufs = self._bufs
         tokens = self._tokens
         B, S = tokens.shape
         T, d = B * S, self.d
         labels = bufs["labels"].view(T)
+        cew = None
+        if self.weighted_loss:
+            c = self._cew
+            cew = L.make_ce_weights(c.period, c.text_rows, c.a_text * grad_scale, c.a_image * grad_scale, c.z_loss)
         ops.gemm(bufs["hf"], self.W("wout"), bufs["dlogits"], T, self.Vpad, d, a_mn=False, b_mn=True,
                  mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=self.P("bout"), labels=labels, lse=bufs["lse_v"],
-                 n_valid=self.V, colsum=self.G("bout"))                 # dlogits + fused d(bout) = colsum(dlogits)
+                 n_valid=self.V, colsum=self.G("bout"), ce_weights=cew)  # dlogits + fused d(bout) = colsum(dlogits)
         ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
         ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
         dx = bufs["dx_a"]

@@ -75,9 +75,12 @@ class Estimator:
             spec.train_op(features, labels)
             if spec.global_step % log_every == 0 or spec.global_step == max_steps:
                 loss = float(spec.loss_sum.item()) * spec.loss_scale      # the only host sync
+                parts = getattr(spec, "loss_parts", None)
+                parts = "" if parts is None else \
+                    " text_ce {:.5f} image_ce {:.5f} z_term {:.3g}".format(*parts.tolist())
                 dt = time.time() - t0
                 if spec.dp.rank == 0:
-                    self._log(f"step {spec.global_step} loss {loss:.5f} "
+                    self._log(f"step {spec.global_step} loss {loss:.5f}{parts} "
                               f"global_step/sec {(spec.global_step - s0) / max(dt, 1e-9):.3f}")
                 t0, s0 = time.time(), spec.global_step
             if ckpt_every and spec.global_step % ckpt_every == 0:

@@ -77,6 +77,19 @@ def make_dropout(rate, seed, step, site, row0):
     return d
 
 
+class CeWeights(ctypes.Structure):
+    """Mirror of ``struct db200_ce_weights`` (weighted cross-entropy: per-row class coefficients and the z-loss)."""
+    _fields_ = [("period", ctypes.c_int32), ("text_rows", ctypes.c_int32), ("a_text", c_f32), ("a_image", c_f32),
+                ("z_loss", c_f32)]
+
+
+def make_ce_weights(period, text_rows, a_text, a_image, z_loss):
+    w = CeWeights()
+    w.period, w.text_rows, w.a_text, w.a_image, w.z_loss = int(period), int(text_rows), float(a_text), \
+        float(a_image), float(z_loss)
+    return w
+
+
 class ConvDesc(ctypes.Structure):
     """Mirror of ``struct db200_conv_desc``."""
     _fields_ = [(n, ctypes.c_int32) for n in
@@ -109,6 +122,8 @@ _SIGNATURES = {
                         ctypes.POINTER(GemmEpilogue)],
     "db200_gemm_bf16_ex": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
                            ctypes.POINTER(GemmEpilogue), ctypes.POINTER(Dropout)],
+    "db200_gemm_bf16_ce_weighted": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
+                                    ctypes.POINTER(GemmEpilogue), ctypes.POINTER(CeWeights)],
     "db200_gemm_ce_tiles": [c_int],
     "db200_embed_fwd_at": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_attn_decode": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_f32],
@@ -133,6 +148,8 @@ _SIGNATURES = {
     "db200_tfrecord_index": [c_vp, c_u64, c_int, c_vp, c_vp, c_u64, c_vp],
     "db200_image_crop_resize_normalize": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_ce_finish": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
+    "db200_ce_finish_weighted": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, ctypes.POINTER(CeWeights),
+                                 c_vp, c_i64],
     "db200_attn_causal_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_causal_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_causal_fwd_ex": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32, ctypes.POINTER(Dropout)],
@@ -182,6 +199,7 @@ _WORKSPACE_QUERIES = {
     "db200_colsum_workspace_bytes": [c_int, c_int],
     "db200_sqnorm_workspace_bytes": [c_sz],
     "db200_ce_finish_workspace_bytes": [c_int],
+    "db200_ce_finish_weighted_workspace_bytes": [c_int],
     "db200_embed_bwd_workspace_bytes": [c_int, c_int],
 }
 EXPORTED_SYMBOLS = ["db200_last_error", "db200_launch_count"] + sorted(_SIGNATURES) + sorted(_WORKSPACE_QUERIES)

@@ -11,7 +11,7 @@ import torch
 
 from . import lib as L
 from . import ops
-from .dalle_engine import DalleEngine
+from .dalle_engine import DalleEngine, validate_loss_weights
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -41,6 +41,7 @@ class StepSpec:
         self.global_step = 0
         self.extra = extra or {}
         self.loss = None              # device scalar of the last step (read it only when logging: it syncs)
+        self.loss_parts = None        # weighted loss: device [3] = text-row mean CE, image-row mean CE, mean z-term
 
 
 def _to_device(t, dtype, device):
@@ -144,6 +145,14 @@ def caption_dropout(params):
     return rate, int(pad)
 
 
+def loss_weights(params):
+    """((w_text, w_image) or None, z_loss) of a DALL-E config: the extension keys text_loss_weight / image_loss_weight
+    (both or neither; finite reals >= 0 with a sum > 0) and z_loss (a finite real >= 0, default 0).  The loss is then
+    (w_t * mean text-row loss + w_i * mean image-row loss) / (w_t + w_i), each row's loss CE + z_loss * lse^2, the
+    means over the rows of the global batch (dalle_engine.loss_coefficients)."""
+    return validate_loss_weights(params.get("text_loss_weight"), params.get("image_loss_weight"), params.get("z_loss"))
+
+
 def dalle_model_fn(features, labels, mode, params):
     """src/model_fns.py:55-236.  features: images f32 [B,H,W,C] in [-1,1] (NHWC); labels: caption ids i32
     [B, text_seq_len].  (The reference's own comment has them swapped; the code uses them this way.)"""
@@ -152,6 +161,7 @@ def dalle_model_fn(features, labels, mode, params):
         raise NotImplementedError                                             # model_fns.py:135-136
     cap_rate, pad_id = caption_dropout(params)
     attention_types, local_radius = attention_layers(params)
+    weights, z_loss = loss_weights(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -182,7 +192,8 @@ def dalle_model_fn(features, labels, mode, params):
                         # what lets the d = 4096 configuration fit 80 GB GPUs in pure data parallelism
                         zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None,
                         dropout=rates, dropout_seed=params.get("seed") or 0,
-                        attention_types=attention_types, local_attention_radius=local_radius)   # models.py:229-301
+                        attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
+                        loss_weights=weights, z_loss=z_loss)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")
@@ -220,6 +231,16 @@ def dalle_model_fn(features, labels, mode, params):
         # sum of per-token losses over all ranks (all-reduced with the gradients) / global token count
         return model.grads[model.aux_off:model.aux_off + 1]
 
+    # weighted loss: the coefficients depend on the global batch only (not on the rank count, the micro-batch size or a
+    # resume), aux slot 0 holds the loss itself and slots 1-3 the sums the parts are formed from
+    weighted = model.weighted_loss
+    loss_scale = 1.0 if weighted else 1.0 / total_tokens_global
+    part_scales = torch.tensor(model.loss_part_scales(global_batch), dtype=torch.float32, device=device) \
+        if weighted else None
+
+    def loss_parts(sums):
+        return sums[1:4] * part_scales if weighted else None
+
     dp.hint_tokens_per_gpu(local_batch * S)
 
     def train_op(features, labels):
@@ -235,13 +256,15 @@ def dalle_model_fn(features, labels, mode, params):
         for i in range(num_microbatches):
             # dropout masks of the global step, indexed by the global sequence index of each row: the same masks
             # whatever the rank count or micro-batch size (models.py:198-323 apply them in mode "train" only)
-            model.forward(toks[i * mb:(i + 1) * mb], step=spec.global_step, row0=first_row + i * mb)
+            model.forward(toks[i * mb:(i + 1) * mb], step=spec.global_step, row0=first_row + i * mb,
+                          global_batch=global_batch)
             last = i == num_microbatches - 1
             if last:
                 dp.begin_overlap()
             # loss = mean over the GLOBAL batch (models.py:353-354): every rank back-props local_sum / (B*S) and the
-            # all-reduce SUMs the shard partials (mtf semantics, SURVEY.md §8e)
-            model.backward(1.0 / total_tokens_global, on_bucket_ready=hook if last else None)
+            # all-reduce SUMs the shard partials (mtf semantics, SURVEY.md §8e); the weighted loss carries its global
+            # normalisation in its coefficients
+            model.backward(1.0 if weighted else 1.0 / total_tokens_global, on_bucket_ready=hook if last else None)
         dp.wait()
         lr = opt.learning_rate(spec.global_step)                                # step counter before the increment
         model.optimizer_step(lr, beta1=opt.beta_1, beta2=opt.beta_2, eps=opt.epsilon,
@@ -249,16 +272,18 @@ def dalle_model_fn(features, labels, mode, params):
         spec.global_step += 1                                                   # model_fns.py:201
         spec.lr = lr
         spec.loss_sum = loss_value()
-        spec.loss_scale = 1.0 / total_tokens_global
+        spec.loss_scale = loss_scale
+        spec.loss_parts = loss_parts(model.grads[model.aux_off:model.aux_off + 4])
         return spec.loss_sum
 
     def eval_op(features, labels):
         toks = assemble(features, labels)
-        acc = torch.zeros(1, dtype=torch.float32, device=device)
-        model.forward(toks, loss_accum=acc)
+        acc = torch.zeros(4 if weighted else 1, dtype=torch.float32, device=device)
+        model.forward(toks, loss_accum=acc, global_batch=global_batch)
         dp.all_reduce_now(acc)
-        spec.loss_sum, spec.loss_scale = acc, 1.0 / total_tokens_global
-        return acc
+        spec.loss_sum, spec.loss_scale = acc[:1], loss_scale
+        spec.loss_parts = loss_parts(acc)
+        return spec.loss_sum
 
     def state_fn():
         st = {k: v for k, v in model.export_params().items()}

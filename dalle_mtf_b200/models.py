@@ -6,7 +6,7 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
-from .model_fns import attention_layers, dropout_rates
+from .model_fns import attention_layers, dropout_rates, loss_weights
 from .vae_engine import VaeEngine
 
 
@@ -22,6 +22,7 @@ class DALLE:
             raise NotImplementedError("incremental inference is stubbed in the reference too (src/model_fns.py:135)")
         params = params or {}
         attention_types, local_radius = attention_layers({**params, "n_layers": n_layers})
+        weights, z_loss = loss_weights(params)
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
@@ -32,7 +33,9 @@ class DALLE:
         self.engine = DalleEngine(n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len,
                                   image_seq_len, recompute_grad=bool(params.get("recompute_grad")) and mode == "train",
                                   dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0,
-                                  attention_types=attention_types, local_attention_radius=local_radius)
+                                  attention_types=attention_types, local_attention_radius=local_radius,
+                                  loss_weights=weights, z_loss=z_loss)
+        self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id
         self.engine.init_params(seed=params.get("seed") or 0)
@@ -40,18 +43,26 @@ class DALLE:
 
     def forward(self, features, return_loss=True, return_logits=False):
         """features = {"tokens": int [B, S]}.  Returns what the reference returns (models.py:397-416):
-        logits | (loss, loss_batch) | (loss, loss_batch, logits), as device tensors (loss fp32 scalar)."""
+        logits | (loss, loss_batch) | (loss, loss_batch, logits), as device tensors (loss fp32 scalar).
+        With params text_loss_weight / image_loss_weight / z_loss, loss is the weighted loss over this batch,
+        loss_batch holds CE + z_loss * lse^2 per position, and self.loss_parts the text-row mean CE, the image-row mean
+        CE and the mean z-term."""
         tokens = features["tokens"] if isinstance(features, dict) else features
         tokens = tokens.to(device=self.engine.device, dtype=torch.int32).contiguous()
         B, S = tokens.shape
         if not return_loss:
             return self.engine.logits(tokens)
-        acc = torch.zeros(1, dtype=torch.float32, device=self.engine.device)
+        e = self.engine
+        acc = torch.zeros(4 if e.weighted_loss else 1, dtype=torch.float32, device=e.device)
         step = None
         if self.mode == "train":   # dropout only in train mode (models.py:198, 215, 290, 312, 318)
             step, self._step = self._step, self._step + 1
-        self.engine.forward(tokens, loss_accum=acc, step=step)
-        loss = acc / float(B * S)   # reduce_mean over every position (models.py:353-354); scalar glue only
+        e.forward(tokens, loss_accum=acc, step=step)
+        if e.weighted_loss:         # slot 0 is the loss itself (coefficients of a batch of B sequences)
+            loss = acc[:1]
+            self.loss_parts = acc[1:4] * torch.tensor(e.loss_part_scales(B), dtype=torch.float32, device=e.device)
+        else:
+            loss = acc / float(B * S)   # reduce_mean over every position (models.py:353-354); scalar glue only
         loss_batch = self.engine._bufs["loss_rows"].view(B, S)
         if return_logits:
             return loss, loss_batch, self.engine.logits(tokens)

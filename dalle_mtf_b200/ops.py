@@ -45,11 +45,13 @@ def _nbytes(ws):
 
 def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=None, mode=L.EPI_STORE,
          alpha=1.0, bias=None, relu=False, residual=None, aux=None, split_k=1, labels=None, part_max=None,
-         part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None, dropout=None):
+         part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None, dropout=None, ce_weights=None):
     """D[M,N] = A[M,K] @ B[K,N] on wgmma.  a_mn / b_mn: operand is stored with M (resp. N) contiguous.
 
     a: [M,K] (k-major) or [K,M] (mn-major);  b: [N,K] (k-major) or [K,N] (mn-major).
     dropout (lib.Dropout, STORE only): D = residual + keep * scale * act(alpha * acc + bias).
+    ce_weights (lib.CeWeights, CE_GRAD only, a k-major / b mn-major): the weighted CE_GRAD epilogue, which takes its
+    per-row coefficients from the descriptor instead of alpha.
     """
     L.require_device()
     _chk(a, BF16, "gemm A")
@@ -88,7 +90,11 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-    if dropout is None:
+    if ce_weights is not None:
+        check(L.load().db200_gemm_bf16_ce_weighted(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb,
+                                                   ptr(out), ldd, M, N, K, ctypes.byref(e), ctypes.byref(ce_weights)),
+              "db200_gemm_bf16_ce_weighted")
+    elif dropout is None:
         check(L.load().db200_gemm_bf16(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out), ldd,
                                        M, N, K, ctypes.byref(e)), "db200_gemm_bf16")
     else:
@@ -134,6 +140,21 @@ def ce_finish(part_max, part_sum, label_logit, lse, loss_rows, loss_sum):
     check(L.load().db200_ce_finish(stream_ptr(), ptr(part_max), ptr(part_sum), ptr(label_logit), ptr(lse),
                                    ptr(loss_rows), ptr(loss_sum), M, n_tiles, ptr(ws), _nbytes(ws)),
           "db200_ce_finish")
+
+
+def ce_finish_weighted(part_max, part_sum, label_logit, lse, loss_rows, sums, weights):
+    """Weighted finish (lib.CeWeights): loss_rows = CE + z lse^2; sums[0..3] += (sum a loss_rows, text-row CE sum,
+    image-row CE sum, sum z lse^2)."""
+    L.require_device()
+    n_tiles, M = part_max.shape
+    _chk(sums, F32, "sums")
+    if sums.numel() < 4:
+        raise L.DB200Error("ce_finish_weighted: sums needs 4 elements")
+    ws = L.workspace(L.load().db200_ce_finish_weighted_workspace_bytes(M))
+    check(L.load().db200_ce_finish_weighted(stream_ptr(), ptr(part_max), ptr(part_sum), ptr(label_logit), ptr(lse),
+                                            ptr(loss_rows), ptr(sums), M, n_tiles, ctypes.byref(weights), ptr(ws),
+                                            _nbytes(ws)),
+          "db200_ce_finish_weighted")
 
 
 # ----------------------------------------------------------------------------------------------- row ops

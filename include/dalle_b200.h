@@ -183,6 +183,23 @@ int db200_gemm_bf16(db200_stream_t stream, const void* A, int a_mn_major, int64_
 int db200_gemm_bf16_ex(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
                        int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi,
                        const db200_dropout* dropout);
+/* Weighted cross-entropy (extension; the reference has no equivalent).  Row m of the vocabulary product is a text row
+ * iff m mod period < text_rows, else an image row; it carries the coefficient a = a_text or a_image and the z-loss
+ * z_loss * lse[m]^2 (mtf's z_loss).  The loss is sum_m a * (lse[m] - logit[m][label[m]] + z_loss * lse[m]^2).
+ * period > 0, 0 <= text_rows <= period, a_text, a_image, z_loss finite and >= 0; otherwise DB200_E_INVALID. */
+typedef struct db200_ce_weights {
+  int32_t period;     /* rows per sequence (S)                                                     */
+  int32_t text_rows;  /* rows per sequence whose target is a text token (text_seq_len - 1)        */
+  float a_text;       /* coefficient of a text row's loss                                         */
+  float a_image;      /* coefficient of an image row's loss (targets: image tokens and EOS)       */
+  float z_loss;       /* z >= 0                                                                   */
+} db200_ce_weights;
+/* weighted CE_GRAD: D(bf16) = a * ((1 + 2 z lse[m]) exp(acc+bias - lse[m]) - [n == label[m]]), 0 for n >= n_valid;
+ * epi->mode must be DB200_EPI_CE_GRAD (epi->alpha is not read), A k-major and B mn-major (DB200_E_UNSUPPORTED
+ * otherwise).  A row with a = 0 gets exact zeros; colsum / workspace as for CE_GRAD. */
+int db200_gemm_bf16_ce_weighted(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                                int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                                const db200_gemm_epilogue* epi, const db200_ce_weights* w);
 /* number of N tiles the CE_STATS epilogue writes per row for a given N (host helper for sizing part_max/part_sum) */
 int db200_gemm_ce_tiles(int N);
 /* epi->workspace size for this product: split-K slices (ATOMIC) or fused column sums (CE_GRAD / RELU_BWD with colsum) */
@@ -197,6 +214,13 @@ int db200_ce_finish(db200_stream_t stream, const float* part_max, const float* p
                     float* lse, float* loss_rows, float* loss_sum, int M, int n_tiles, void* workspace,
                     int64_t workspace_bytes);
 int64_t db200_ce_finish_workspace_bytes(int M);
+/* weighted finish (db200_ce_weights above): lse[m] as ce_finish; loss_rows[m] = lse[m] - label_logit[m] + z lse[m]^2;
+ * sums[0..3] += { sum_m a_m loss_rows[m],  sum over text rows of (lse - label_logit),  the same over image rows,
+ * sum_m z lse[m]^2 }.  Per-block partials added in block order: bit-reproducible. */
+int db200_ce_finish_weighted(db200_stream_t stream, const float* part_max, const float* part_sum,
+                             const float* label_logit, float* lse, float* loss_rows, float* sums, int M, int n_tiles,
+                             const db200_ce_weights* w, void* workspace, int64_t workspace_bytes);
+int64_t db200_ce_finish_weighted_workspace_bytes(int M);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * K4  causal flash attention on wgmma.  Replaces mtf_transformer.attention.attention with the [S,S] -1e10 mask:

@@ -61,6 +61,26 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
+def param_layout(d, n_layers, V, S):
+    """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
+    length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns."""
+    Vpad = _round_up(V, 64)
+    lay = ParamLayout()
+    lay.add("wte", (V, d))
+    lay.add("wpe", (S, d))
+    for i in range(n_layers):
+        p = f"l{i}."
+        lay.add(p + "ln1_g", (d,)); lay.add(p + "ln1_b", (d,))
+        lay.add(p + "wqkv", (d, 3 * d))
+        lay.add(p + "wo", (d, d)); lay.add(p + "o_b", (d,))
+        lay.add(p + "ln2_g", (d,)); lay.add(p + "ln2_b", (d,))
+        lay.add(p + "w1", (d, 4 * d)); lay.add(p + "b1", (4 * d,))
+        lay.add(p + "w2", (4 * d, d)); lay.add(p + "b2", (d,))
+    lay.add("lnf_g", (d,)); lay.add("lnf_b", (d,))
+    lay.add("wout", (d, Vpad)); lay.add("bout", (Vpad,))
+    return lay
+
+
 def layer_radii(attention_types, radius, n_layers):
     """Per-layer attention radius: None for a "global" layer, `radius` for a "local" one (attention_types None: every
     layer global)."""
@@ -169,20 +189,7 @@ class DalleEngine:
         self._cew = None             # lib.CeWeights of the current forward (weighted loss only)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
-        lay = ParamLayout()
-        lay.add("wte", (V, d))
-        lay.add("wpe", (S, d))
-        for i in range(Lyr):
-            p = f"l{i}."
-            lay.add(p + "ln1_g", (d,)); lay.add(p + "ln1_b", (d,))
-            lay.add(p + "wqkv", (d, 3 * d))
-            lay.add(p + "wo", (d, d)); lay.add(p + "o_b", (d,))
-            lay.add(p + "ln2_g", (d,)); lay.add(p + "ln2_b", (d,))
-            lay.add(p + "w1", (d, 4 * d)); lay.add(p + "b1", (4 * d,))
-            lay.add(p + "w2", (4 * d, d)); lay.add(p + "b2", (d,))
-        lay.add("lnf_g", (d,)); lay.add("lnf_b", (d,))
-        lay.add("wout", (d, self.Vpad)); lay.add("bout", (self.Vpad,))
-        self.layout = lay
+        self.layout = lay = param_layout(d, Lyr, V, S)
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
         #   [0] = sum of per-token losses of this rank (weighted loss: sum of a_t * loss_t)
@@ -414,6 +421,16 @@ class DalleEngine:
         if self.zero is not None:
             return self._refresh_vecs()
         ops.cast_f32_to_bf16(self.master[:self.n_params_padded], self.shadow[:self.n_params_padded])
+
+    def copy_params_from(self, src):
+        """Take over the current weights of `src`, an engine of the same model and rank (evaluation of the weights
+        being trained).  ZeRO-1: the fp32 master is only this rank's slice, so the full bf16 copy the kernels read is
+        copied too and the fp32 vector parameters are rebuilt from it."""
+        self.master.copy_(src.master)
+        if self.zero is None:
+            return self.refresh_shadow()
+        self.shadow.copy_(src.shadow)
+        self._refresh_vecs()
 
     # ------------------------------------------------------------------------------------------ buffers
     def _alloc(self, B):

@@ -97,9 +97,7 @@ class Estimator:
         spec = self._spec(EVAL, features, labels)
         train_spec = self._specs.get(TRAIN)
         if train_spec is not None:  # evaluate the weights being trained
-            spec.engine.master.copy_(train_spec.engine.master)
-            if hasattr(spec.engine, "refresh_shadow"):
-                spec.engine.refresh_shadow()
+            spec.engine.copy_params_from(train_spec.engine)
             spec.global_step = train_spec.global_step
         total = 0.0
         for i in range(steps):

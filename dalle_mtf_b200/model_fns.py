@@ -297,7 +297,14 @@ def dalle_model_fn(features, labels, mode, params):
 
     def load_fn(st):
         names = [k for k in st if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"]
+        if model.zero is not None and mode == TRAIN:
+            # restarting Adam's moments from zero at the full learning rate would silently change the run
+            raise L.DB200Error("optimizer_state_sharding: ZeRO-1 checkpoints hold no Adam slots (DESIGN.md §7) and "
+                               "resuming training needs them; such a checkpoint can be evaluated, exported or sampled")
         model.load_params({k: st[k] for k in names})                                # master + bf16 shadow
+        if model.zero is not None:      # evaluation: the parameters are all it needs
+            spec.global_step = int(st.get("global_step", 0))
+            return
         for suffix, flat in (("/adam_m", model.adam_m), ("/adam_v", model.adam_v)):
             model.load_flat(flat, {k: st[k + suffix] for k in names})
         spec.global_step = int(st.get("global_step", 0))

@@ -130,6 +130,12 @@ class VaeEngine:
         if self._cb_tc:
             ops.split_f32(self.P("codebook/codebook"), self.cb_hi, self.cb_lo)
 
+    def copy_params_from(self, src):
+        """Take over the current weights of `src`, an engine of the same model (evaluation of the weights being
+        trained)."""
+        self.master.copy_(src.master)
+        self.refresh_shadow()
+
     def _mm_split(self, a_parts, b_parts, out_f32, M, N, K, b_mn):
         """out = sum over the listed (a, b) pairs of a @ b on wgmma (first product stores, the rest red.add)."""
         first = True

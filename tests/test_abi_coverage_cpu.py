@@ -30,7 +30,6 @@ REACHED_THROUGH = {
     "db200_attn_decode_dev": ("sampling", "test_sampling_gpu.py"),
     "db200_sample_rows_at": ("sampling", "test_sampling_gpu.py"),
     "db200_incr_i32": ("sampling", "test_sampling_gpu.py"),
-    "db200_gather_cast_bf16_f32": ("dalle_engine", "test_dp_gpu.py"),
     "db200_crc32c": ("tfrecord", "test_data_cpu.py"),
     "db200_tfrecord_masked_crc": ("tfrecord", "test_data_cpu.py"),
     "db200_tfrecord_frame": ("tfrecord", "test_data_cpu.py"),

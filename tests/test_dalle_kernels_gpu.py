@@ -945,6 +945,36 @@ def _f32(x):
     return float(torch.tensor(x, dtype=F32))
 
 
+def check_adam_update(tag, inputs, outputs, lr, b1, b2, eps, wd, clip, gscale, bc, step):
+    """One db200_adam_step against the float64 restatement of oracle/optim.py (adam_mtf_step / adam_tf_step,
+    clip_by_global_norm) on the kernel's fp32 constants, with the bounds of the module docstring.  inputs = (p, m, v,
+    g, gnorm_sq) as the kernel read them (gnorm_sq unused without clipping), outputs = (p', m', v', bf16 shadow) as it
+    wrote them.  Returns whether the clip scaled the gradient down."""
+    p, m, v, gr, gn = inputs
+    pd, md, vd, p16 = outputs
+    B1, B2, EPS, LR, WD, CL, GS = map(_f32, (b1, b2, eps, lr, wd, clip, gscale))
+    gmul, clipped = GS, False
+    if clip:
+        gnorm = math.sqrt(float(gn)) * GS
+        gmul = GS * CL / max(gnorm, CL)
+        clipped = gnorm > CL
+    gs = gr.to(F64) * gmul
+    m2 = B1 * m.to(F64) + _f32(1 - B1) * gs
+    mA = B1 * m.to(F64).abs() + _f32(1 - B1) * gs.abs()
+    v2 = B2 * v.to(F64) + _f32(1 - B2) * gs * gs
+    den = torch.sqrt(v2) + EPS
+    lr_eff = _f32(LR * math.sqrt(1 - B2 ** step) / (1 - B1 ** step)) if bc else LR
+    upd = m2 / den + (WD * p.to(F64) if wd else 0.0)
+    ref_u = -lr_eff * upd
+    p_new = p.to(F64) + ref_u
+    check(f"adam m ({tag})", md, m2, mA, a=0.0, b=9 * U)
+    check(f"adam v ({tag})", vd, v2, v2, a=0.0, b=16 * U)
+    check(f"adam update p'-p ({tag})", pd.to(F64) - p.to(F64), ref_u,
+          lr_eff * (mA / den + WD * p.to(F64).abs()), a=3 * U, b=20 * U, floor=U * p_new.abs())
+    assert torch.equal(p16.view(torch.int16), pd.to(BF16).view(torch.int16)), "bf16 shadow is not RNE of the new p"
+    return clipped
+
+
 @pytest.mark.parametrize("case", ["clip active", "clip inactive", "bias correction", "weight decay", "zero_grad"])
 def test_sqnorm_and_adam_update(ops, case):
     n = 1_000_003
@@ -975,27 +1005,9 @@ def test_sqnorm_and_adam_update(ops, case):
     p16 = nan_like((n,), BF16)
     ops.adam_step(pd, md, vd, gd, p16, lr, b1, b2, eps, wd, gn if clip else None, clip, gscale, bc, step,
                   zero_grad=case == "zero_grad")
-    # float64 restatement of oracle/optim.py (adam_mtf_step / adam_tf_step, clip_by_global_norm) on fp32 constants
-    B1, B2, EPS, LR, WD, CL, GS = map(_f32, (b1, b2, eps, lr, wd, clip, gscale))
-    gmul = GS
-    if clip:
-        gnorm = math.sqrt(float(gn)) * GS
-        gmul = GS * CL / max(gnorm, CL)
-        assert (gnorm > CL) == (case == "clip active")
-    gs = gr.to(F64) * gmul
-    m2 = B1 * m.to(F64) + _f32(1 - B1) * gs
-    mA = B1 * m.to(F64).abs() + _f32(1 - B1) * gs.abs()
-    v2 = B2 * v.to(F64) + _f32(1 - B2) * gs * gs
-    den = torch.sqrt(v2) + EPS
-    lr_eff = _f32(LR * math.sqrt(1 - B2 ** step) / (1 - B1 ** step)) if bc else LR
-    upd = m2 / den + (WD * p.to(F64) if wd else 0.0)
-    ref_u = -lr_eff * upd
-    p_new = p.to(F64) + ref_u
-    check(f"adam m ({case})", md, m2, mA, a=0.0, b=9 * U)
-    check(f"adam v ({case})", vd, v2, v2, a=0.0, b=16 * U)
-    check(f"adam update p'-p ({case})", pd.to(F64) - p.to(F64), ref_u,
-          lr_eff * (mA / den + WD * p.to(F64).abs()), a=3 * U, b=20 * U, floor=U * p_new.abs())
-    assert torch.equal(p16.view(torch.int16), pd.to(BF16).view(torch.int16)), "bf16 shadow is not RNE of the new p"
+    clipped = check_adam_update(case, (p, m, v, gr, gn), (pd, md, vd, p16), lr, b1, b2, eps, wd, clip, gscale, bc,
+                                step)
+    assert clipped == (case == "clip active")
     if case == "zero_grad":
         assert (gd == 0).all()
     else:

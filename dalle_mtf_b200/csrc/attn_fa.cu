@@ -12,6 +12,16 @@
 // LOCAL (sliding-window attention, mtf local_attention_1d with fully_autoregressive=True, src/dalle_mtf/models.py:
 // 257-273): query i sees key j iff i - radius < j <= i.  The loops visit only the key (query) blocks that intersect that
 // band and the masks add the lower edge; the global (causal) instantiations compile without either.
+//
+// AXIAL (DALL-E's row and column attention, DALLE-pytorch's "axial_row" / "axial_col"): text length TL, image grid
+// W x W, position p >= TL is image token k = p - TL at row k / W, column k % W.  Text queries are causal; an image
+// query sees every text key and the image keys of its own row (column) at or before it.  The kernels walk the rows in
+// "kernel order" t: t = p for a row layer and for text rows; the image rows of a column layer are taken column-major,
+// u = t - TL, p = TL + (u % W) W + u / W.  In kernel order both layers are one mask: t_k <= t_q and (t_k < TL or
+// t_k >= the start TL + ((t_q - TL) / W) W of t_q's segment), i.e. a text prefix plus causal attention inside
+// segments of W rows.  Every global access (tile loads, stores, lse / delta) goes through the row map, so the tensor
+// layouts are those of the other instantiations; rows whose p >= S (a shorter prefill) are absent: zero-filled,
+// never stored, and a present query never sees one.
 #include "gemm_common.cuh"  // cp.async helpers
 #include "philox.cuh"
 #include "wgmma.cuh"
@@ -145,15 +155,81 @@ __device__ __forceinline__ void fa_store_rows(bf16* dst, long long ld, const flo
 template <int DH>
 constexpr size_t fa_smem(int tiles) { return 1024 + size_t(tiles) * FA_ROWS * DH * 2 + 2 * FA_ROWS * 4; }
 
+// ---- AXIAL: geometry and row map.  rows = kernel-order rows the grid covers (S for a row layer).
+struct FaAxial {
+  int text_len, grid_w, axis, rows;
+};
+// sequence position of kernel-order row t, or -1 when the row is absent
+__device__ __forceinline__ int fa_axial_pos(const FaAxial& a, int S, int t) {
+  if (t >= a.rows) return -1;
+  int p = t;
+  if (a.axis && t >= a.text_len) {
+    const int u = t - a.text_len;
+    p = a.text_len + (u % a.grid_w) * a.grid_w + u / a.grid_w;
+  }
+  return p < S ? p : -1;
+}
+// first kernel-order row of t's segment (0 for a text row: every key up to t)
+__device__ __forceinline__ int fa_axial_seg_start(const FaAxial& a, int t) {
+  return t < a.text_len ? 0 : a.text_len + (t - a.text_len) / a.grid_w * a.grid_w;
+}
+// fa_load_tile of kernel-order rows t0 .. t0 + 63: row t at base + p(t) * ld, absent rows zero-filled
+template <int DH>
+__device__ __forceinline__ void fa_load_tile_axial(uint32_t dst, const bf16* base, long long ld, const FaAxial& a,
+                                                   int S, int t0) {
+  constexpr int CPR = DH / 8;
+#pragma unroll
+  for (int i = 0; i < FA_ROWS * CPR / 128; ++i) {
+    const int idx = threadIdx.x + 128 * i;
+    const int r = idx / CPR, c = idx % CPR;
+    const int p = fa_axial_pos(a, S, t0 + r);
+    const bool ok = p >= 0;
+    const uint32_t off = (c >> 3) * (FA_ROWS * 128) + r * 128 + ((((c & 7) ^ (r & 7)) & 7) << 4);
+    cp_async16_zfill(dst + off, ok ? base + (long long)p * ld + c * 8 : base, ok);
+  }
+}
+// fa_store_rows of kernel-order rows t0 .. t0 + 63 to base + p(t) * ld (present rows only)
+template <int DH>
+__device__ __forceinline__ void fa_store_rows_axial(bf16* base, long long ld, const float* acc, const float (&mul)[2],
+                                                    const FaAxial& a, int S, int t0, const Frag& f) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int p = fa_axial_pos(a, S, t0 + f.fr + 8 * h);
+    if (p < 0) continue;
+    bf16* d = base + (long long)p * ld + f.fc;
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i)
+      *reinterpret_cast<uint32_t*>(d + 8 * i) = pack_bf16x2(acc[4 * i + 2 * h] * mul[h], acc[4 * i + 2 * h + 1] * mul[h]);
+  }
+}
+// key blocks of query block qb (forward, dQ): the text blocks [0, jt), then the blocks from js (the block of the segment
+// start of the block's first image query) to qb.  No block is visited twice.
+__device__ __forceinline__ void fa_axial_key_blocks(const FaAxial& a, int qb, int& jt, int& js) {
+  jt = (a.text_len + FA_ROWS - 1) / FA_ROWS;
+  const int t = max(qb * FA_ROWS, a.text_len);
+  js = t < (qb + 1) * FA_ROWS ? fa_axial_seg_start(a, t) / FA_ROWS : jt;
+}
+__device__ __forceinline__ int fa_axial_next(int j, int jt, int js) { return (j + 1 >= jt && j + 1 < js) ? js : j + 1; }
+// query blocks of key block kb (dK / dV): [kb, end).  A block holding a text key sees every later query; an image key
+// block the queries up to the end of the last segment it touches.
+__device__ __forceinline__ int fa_axial_query_end(const FaAxial& a, int kb) {
+  const int nq = (a.rows + FA_ROWS - 1) / FA_ROWS, k0 = kb * FA_ROWS;
+  if (k0 < a.text_len) return nq;
+  const int last = min(k0 + FA_ROWS - 1, a.rows - 1);
+  const int seg_end = fa_axial_seg_start(a, last) + a.grid_w - 1;
+  return min(nq, seg_end / FA_ROWS + 1);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
 // forward: grid (query blocks, B * H); online softmax in the exp2 domain
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL>
 __global__ void __launch_bounds__(128, 1)
 attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, const db200_dropout dr, int radius) {
+                float scale, const db200_dropout dr, int radius, const FaAxial ax) {
+  static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -165,16 +241,28 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
   const Frag f;
   const float sl2 = scale * kLog2e;
 
-  fa_load_tile<DH>(sQ, Q + q0 * ldq, ldq, S - q0);
+  if constexpr (AXIAL) fa_load_tile_axial<DH>(sQ, Q, ldq, ax, S, q0);
+  else fa_load_tile<DH>(sQ, Q + q0 * ldq, ldq, S - q0);
   float o[DH / 2], m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
-  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : 0;
-  for (int j = j0; j <= qb; ++j) {
+  int jt = 0, js = 0, slo[2] = {0, 0};  // AXIAL: key blocks and the segment start of each query row
+  if constexpr (AXIAL) {
+    fa_axial_key_blocks(ax, qb, jt, js);
+    slo[0] = fa_axial_seg_start(ax, q0 + f.fr);
+    slo[1] = fa_axial_seg_start(ax, q0 + f.fr + 8);
+  }
+  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : (AXIAL && jt == 0 ? js : 0);
+  for (int j = j0; j <= qb; j = AXIAL ? fa_axial_next(j, jt, js) : j + 1) {
     const int k0 = j * FA_ROWS;
     __syncthreads();  // the previous block's K / V tiles are no longer read
-    fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
-    fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
+    if constexpr (AXIAL) {
+      fa_load_tile_axial<DH>(sK, Q + (long long)H * DH, ldq, ax, S, k0);
+      fa_load_tile_axial<DH>(sV, Q + 2LL * H * DH, ldq, ax, S, k0);
+    } else {
+      fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
+      fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
+    }
     fa_tiles_ready();
     float s[32];
     fa_qk<DH>(s, sQ, sK);
@@ -187,7 +275,8 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
         for (int e = 0; e < 2; ++e) {
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           float& v = s[4 * i + 2 * hh + e];
-          v = (col <= row && col < S && (!LOCAL || col > row - radius)) ? v * sl2 : -INFINITY;
+          if constexpr (AXIAL) v = (col <= row && (col < ax.text_len || col >= slo[hh])) ? v * sl2 : -INFINITY;
+          else v = (col <= row && col < S && (!LOCAL || col > row - radius)) ? v * sl2 : -INFINITY;
           mx[hh] = fmaxf(mx[hh], v);
         }
     float alpha[2], mb[2];
@@ -225,20 +314,25 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
   for (int hh = 0; hh < 2; ++hh) {
     const float tot = quad_sum(l[hh]);
     inv[hh] = tot > 0.f ? 1.f / tot : 0.f;
-    const int row = q0 + f.fr + 8 * hh;
-    if ((f.fc == 0) && row < S) lse[((long long)b * H + h) * S + row] = (m[hh] + log2f(tot)) * kLn2;
+    const int row = AXIAL ? fa_axial_pos(ax, S, q0 + f.fr + 8 * hh) : q0 + f.fr + 8 * hh;
+    if ((f.fc == 0) && row < S && (!AXIAL || row >= 0))
+      lse[((long long)b * H + h) * S + row] = (m[hh] + log2f(tot)) * kLn2;
   }
-  fa_store_rows<DH>(out + ((long long)b * S + q0) * H * DH + (long long)h * DH, (long long)H * DH, o, inv, S - q0, f);
+  if constexpr (AXIAL)
+    fa_store_rows_axial<DH>(out + (long long)b * S * H * DH + (long long)h * DH, (long long)H * DH, o, inv, ax, S, q0, f);
+  else
+    fa_store_rows<DH>(out + ((long long)b * S + q0) * H * DH + (long long)h * DH, (long long)H * DH, o, inv, S - q0, f);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ: grid (query blocks, B * H).  P = exp(scale S - lse), dS = P (dO V^T - delta), dQ = scale dS K
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                    const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                   const db200_dropout dr, int radius) {
+                   const db200_dropout dr, int radius, const FaAxial ax) {
+  static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -250,25 +344,47 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
   const Frag f;
   const float sl2 = scale * kLog2e;
 
-  fa_load_tile<DH>(sQ, Q + q0 * ldq, ldq, S - q0);
-  fa_load_tile<DH>(sdO, dout + ((long long)b * S + q0) * ldo + (long long)h * DH, ldo, S - q0);
+  int slo[2] = {0, 0};  // AXIAL: segment start of each query row
+  if constexpr (AXIAL) {
+    fa_load_tile_axial<DH>(sQ, Q, ldq, ax, S, q0);
+    fa_load_tile_axial<DH>(sdO, dout + (long long)b * S * ldo + (long long)h * DH, ldo, ax, S, q0);
+  } else {
+    fa_load_tile<DH>(sQ, Q + q0 * ldq, ldq, S - q0);
+    fa_load_tile<DH>(sdO, dout + ((long long)b * S + q0) * ldo + (long long)h * DH, ldo, S - q0);
+  }
   float lse2[2], dl[2];
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int row = q0 + f.fr + 8 * hh;
-    const long long ix = ((long long)b * H + h) * S + (row < S ? row : S - 1);
-    lse2[hh] = lse[ix] * kLog2e;
-    dl[hh] = delta[ix];
+    if constexpr (AXIAL) {
+      // an absent row gets P = 0 (lse = +inf) and dS = 0
+      const int p = fa_axial_pos(ax, S, row);
+      const long long ix = ((long long)b * H + h) * S + (p >= 0 ? p : 0);
+      lse2[hh] = p >= 0 ? lse[ix] * kLog2e : INFINITY;
+      dl[hh] = p >= 0 ? delta[ix] : 0.f;
+      slo[hh] = fa_axial_seg_start(ax, row);
+    } else {
+      const long long ix = ((long long)b * H + h) * S + (row < S ? row : S - 1);
+      lse2[hh] = lse[ix] * kLog2e;
+      dl[hh] = delta[ix];
+    }
   }
   float dq[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) dq[i] = 0.f;
-  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : 0;
-  for (int j = j0; j <= qb; ++j) {
+  int jt = 0, js = 0;
+  if constexpr (AXIAL) fa_axial_key_blocks(ax, qb, jt, js);
+  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : (AXIAL && jt == 0 ? js : 0);
+  for (int j = j0; j <= qb; j = AXIAL ? fa_axial_next(j, jt, js) : j + 1) {
     const int k0 = j * FA_ROWS;
     __syncthreads();
-    fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
-    fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
+    if constexpr (AXIAL) {
+      fa_load_tile_axial<DH>(sK, Q + (long long)H * DH, ldq, ax, S, k0);
+      fa_load_tile_axial<DH>(sV, Q + 2LL * H * DH, ldq, ax, S, k0);
+    } else {
+      fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
+      fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
+    }
     fa_tiles_ready();
     float s[32], dp[32];
     fa_qk<DH>(s, sQ, sK);
@@ -283,25 +399,28 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
         for (int e = 0; e < 2; ++e) {
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           const int x = 4 * i + 2 * hh + e;
-          const bool vis = col <= row && col < S && row < S && (!LOCAL || col > row - radius);
+          const bool vis = AXIAL ? col <= row && (col < ax.text_len || col >= slo[hh])
+                                 : col <= row && col < S && row < S && (!LOCAL || col > row - radius);
           const float p = vis ? exp2f(s[x] * sl2 - lse2[hh]) : 0.f;
           s[x] = p * ((DROP ? dp[x] * fa_keep_mul(kb, x, dr.scale) : dp[x]) - dl[hh]);
         }
     fa_pv<DH>(dq, s, sK);
   }
   const float mul[2] = {scale, scale};
-  fa_store_rows<DH>(dqkv + ((long long)b * S + q0) * ldq + (long long)h * DH, ldq, dq, mul, S - q0, f);
+  if constexpr (AXIAL) fa_store_rows_axial<DH>(dqkv + (long long)b * S * ldq + (long long)h * DH, ldq, dq, mul, ax, S, q0, f);
+  else fa_store_rows<DH>(dqkv + ((long long)b * S + q0) * ldq + (long long)h * DH, ldq, dq, mul, S - q0, f);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dK / dV: grid (key blocks, B * H), transposed products so that the key index is the accumulator row.
 //   P^T = exp(scale K Q^T - lse), dV = P^T dO, dS^T = P^T (V dO^T - delta), dK = scale dS^T Q
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                     const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                    const db200_dropout dr, int radius) {
+                    const db200_dropout dr, int radius, const FaAxial ax) {
+  static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -315,24 +434,47 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
   const Frag f;
   const float sl2 = scale * kLog2e;
   // LOCAL: the last query that sees key k0 + 63 is k0 + 62 + radius
-  const int nqb = LOCAL ? min((S + FA_ROWS - 1) / FA_ROWS, (int)(((long long)k0 + 62 + radius) / FA_ROWS) + 1)
+  // AXIAL: fa_axial_query_end; a key row sees the queries up to the end of its segment (text keys: every later one)
+  const int nqb = AXIAL ? fa_axial_query_end(ax, kb)
+                : LOCAL ? min((S + FA_ROWS - 1) / FA_ROWS, (int)(((long long)k0 + 62 + radius) / FA_ROWS) + 1)
                         : (S + FA_ROWS - 1) / FA_ROWS;
-
-  fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
-  fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
+  int kend[2] = {0, 0};
+  if constexpr (AXIAL) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int key = k0 + f.fr + 8 * hh;
+      kend[hh] = key < ax.text_len ? INT_MAX : fa_axial_seg_start(ax, key) + ax.grid_w - 1;
+    }
+    fa_load_tile_axial<DH>(sK, Q + (long long)H * DH, ldq, ax, S, k0);
+    fa_load_tile_axial<DH>(sV, Q + 2LL * H * DH, ldq, ax, S, k0);
+  } else {
+    fa_load_tile<DH>(sK, Q + k0 * ldq + (long long)H * DH, ldq, S - k0);
+    fa_load_tile<DH>(sV, Q + k0 * ldq + 2LL * H * DH, ldq, S - k0);
+  }
   float dk[DH / 2], dv[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
   for (int i = kb; i < nqb; ++i) {
     const int q0 = i * FA_ROWS;
     __syncthreads();
-    fa_load_tile<DH>(sQ, Q + q0 * ldq, ldq, S - q0);
-    fa_load_tile<DH>(sdO, dout + ((long long)b * S + q0) * ldo + (long long)h * DH, ldo, S - q0);
-    if (threadIdx.x < FA_ROWS) {
-      const int q = q0 + threadIdx.x;
-      const long long ix = ((long long)b * H + h) * S + (q < S ? q : S - 1);
-      s_lse[threadIdx.x] = lse[ix] * kLog2e;
-      s_dl[threadIdx.x] = delta[ix];
+    if constexpr (AXIAL) {
+      fa_load_tile_axial<DH>(sQ, Q, ldq, ax, S, q0);
+      fa_load_tile_axial<DH>(sdO, dout + (long long)b * S * ldo + (long long)h * DH, ldo, ax, S, q0);
+      if (threadIdx.x < FA_ROWS) {  // an absent query gets P = 0 (lse = +inf) and dS = 0
+        const int p = fa_axial_pos(ax, S, q0 + threadIdx.x);
+        const long long ix = ((long long)b * H + h) * S + (p >= 0 ? p : 0);
+        s_lse[threadIdx.x] = p >= 0 ? lse[ix] * kLog2e : INFINITY;
+        s_dl[threadIdx.x] = p >= 0 ? delta[ix] : 0.f;
+      }
+    } else {
+      fa_load_tile<DH>(sQ, Q + q0 * ldq, ldq, S - q0);
+      fa_load_tile<DH>(sdO, dout + ((long long)b * S + q0) * ldo + (long long)h * DH, ldo, S - q0);
+      if (threadIdx.x < FA_ROWS) {
+        const int q = q0 + threadIdx.x;
+        const long long ix = ((long long)b * H + h) * S + (q < S ? q : S - 1);
+        s_lse[threadIdx.x] = lse[ix] * kLog2e;
+        s_dl[threadIdx.x] = delta[ix];
+      }
     }
     fa_tiles_ready();
     float st[32], dpt[32];
@@ -345,7 +487,8 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
         for (int e = 0; e < 2; ++e) {
           const int key = k0 + f.fr + 8 * hh, cq = 8 * ii + f.fc + e, q = q0 + cq;
           const int x = 4 * ii + 2 * hh + e;
-          const bool vis = key <= q && q < S && key < S && (!LOCAL || key > q - radius);
+          const bool vis = AXIAL ? key <= q && (key < ax.text_len || q <= kend[hh])
+                                 : key <= q && q < S && key < S && (!LOCAL || key > q - radius);
           st[x] = vis ? exp2f(st[x] * sl2 - s_lse[cq]) : 0.f;
         }
     // dropout: dV += (P keep scale)^T dO,  dS = P (dP keep scale - delta)
@@ -365,41 +508,51 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
     fa_pv<DH>(dk, st, sQ);
   }
   const float one[2] = {1.f, 1.f}, mul[2] = {scale, scale};
-  bf16* dst = dqkv + ((long long)b * S + k0) * ldq + (long long)h * DH;
-  fa_store_rows<DH>(dst + (long long)H * DH, ldq, dk, mul, S - k0, f);
-  fa_store_rows<DH>(dst + 2LL * H * DH, ldq, dv, one, S - k0, f);
+  if constexpr (AXIAL) {
+    bf16* dst = dqkv + (long long)b * S * ldq + (long long)h * DH;
+    fa_store_rows_axial<DH>(dst + (long long)H * DH, ldq, dk, mul, ax, S, k0, f);
+    fa_store_rows_axial<DH>(dst + 2LL * H * DH, ldq, dv, one, ax, S, k0, f);
+  } else {
+    bf16* dst = dqkv + ((long long)b * S + k0) * ldq + (long long)h * DH;
+    fa_store_rows<DH>(dst + (long long)H * DH, ldq, dk, mul, S - k0, f);
+    fa_store_rows<DH>(dst + 2LL * H * DH, ldq, dv, one, S - k0, f);
+  }
 }
 
-template <int DH, bool DROP, bool LOCAL = false>
+// AXIAL: the grid covers ax.rows kernel-order rows instead of S
+template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false>
 static int fa_fwd(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, float scale,
-                  const db200_dropout& dr, int radius = 0) {
+                  const db200_dropout& dr, int radius = 0, const FaAxial& ax = FaAxial{}) {
   constexpr size_t smem = fa_smem<DH>(3);
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL, AXIAL>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(attr_rc);
-  const dim3 grid((S + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_fwd_kernel<DH, DROP, LOCAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale, dr,
-                                                                radius);
+  const dim3 grid(((AXIAL ? ax.rows : S) + FA_ROWS - 1) / FA_ROWS, B * H);
+  attn_fwd_kernel<DH, DROP, LOCAL, AXIAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale,
+                                                                       dr, radius, ax);
   return check_launch("attn_fwd_kernel");
 }
 
-template <int DH, bool DROP, bool LOCAL = false>
+template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false>
 static int fa_bwd(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
-                  void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr, int radius = 0) {
+                  void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr, int radius = 0,
+                  const FaAxial& ax = FaAxial{}) {
   constexpr size_t smem = fa_smem<DH>(4);
-  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL>,
+  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL>,
+  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(rc1);
   DB200_CUDA(rc2);
-  const dim3 grid((S + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_bwd_dq_kernel<DH, DROP, LOCAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
-                                                                   (bf16*)dqkv, S, H, scale, dr, radius);
+  const dim3 grid(((AXIAL ? ax.rows : S) + FA_ROWS - 1) / FA_ROWS, B * H);
+  attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse,
+                                                                          delta, (bf16*)dqkv, S, H, scale, dr, radius,
+                                                                          ax);
   int rc = check_launch("attn_bwd_dq_kernel");
   if (rc != DB200_OK) return rc;
-  attn_bwd_dkv_kernel<DH, DROP, LOCAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse, delta,
-                                                                    (bf16*)dqkv, S, H, scale, dr, radius);
+  attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse,
+                                                                           delta, (bf16*)dqkv, S, H, scale, dr, radius,
+                                                                           ax);
   return check_launch("attn_bwd_dkv_kernel");
 }
 
@@ -437,6 +590,32 @@ int attn_local_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout
   const db200_dropout none{};
   return dh == 128 ? fa_bwd<128, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, radius)
                    : fa_bwd<64, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, radius);
+}
+
+// kernel-order rows of an axial layer of length S: S for a row layer (or without image rows); for a column layer, one
+// past the largest u = c W + r of the present image tokens k = r W + c < S - TL
+static int axial_rows(int S, int text_len, int grid_w, int axis) {
+  const int n = S - text_len;
+  if (!axis || n <= 0) return S;
+  const int umax = n >= grid_w ? (grid_w - 1) * grid_w + (n - grid_w) / grid_w : (n - 1) * grid_w;
+  return text_len + umax + 1;
+}
+
+// row (axis 0) or column (axis 1) attention over a text prefix of text_len and a grid_w x grid_w image; no dropout
+int attn_axial_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
+                          int text_len, int grid_w, int axis, float scale) {
+  const db200_dropout none{};
+  const FaAxial ax{text_len, grid_w, axis, axial_rows(S, text_len, grid_w, axis)};
+  return dh == 128 ? fa_fwd<128, false, false, true>(stream, qkv, out, lse, B, S, H, scale, none, 0, ax)
+                   : fa_fwd<64, false, false, true>(stream, qkv, out, lse, B, S, H, scale, none, 0, ax);
+}
+
+int attn_axial_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
+                          void* dqkv, int B, int S, int H, int dh, int text_len, int grid_w, int axis, float scale) {
+  const db200_dropout none{};
+  const FaAxial ax{text_len, grid_w, axis, axial_rows(S, text_len, grid_w, axis)};
+  return dh == 128 ? fa_bwd<128, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, ax)
+                   : fa_bwd<64, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, ax);
 }
 
 }  // namespace db200

@@ -7,6 +7,8 @@
 //   attn_decode    append this step's k,v to the cache at `pos`, then out[b,h,:] = softmax_{lo<=j<=pos}(scale q.k_j) v_j,
 //                  lo = max(0, pos - radius + 1) (radius >= S: every key <= pos; a local layer, models.py:257-273: its window)
 //                  fp32 scores / softmax, P rounded to bf16 for the PV product (same policy as attn.cu)
+//                  AXIAL (row / column layers): over a key list, the text run [0, min(pos, TL - 1)] followed, for an
+//                  image position (grid row r, column c), by row r's columns 0..c or column c's rows 0..r
 //   sample_rows    idx = lo + argmax_{lo<=c<hi}(logits[c] * inv_temp + gumbel(u[c-lo]))   (first maximum; u NULL = greedy)
 //   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
 //   sample_rows_guided     either of the two over the classifier-free-guidance mix u + s (c - u) of a conditional
@@ -37,10 +39,13 @@ __global__ void embed_at_kernel(const int* __restrict__ ids, const bf16* __restr
 // over `pos` keys of the first version made generation latency-bound (~100 us per call at pos ~ 1000).
 // Scores live in dynamic shared memory, indexed by j - lo (pos + 1 - lo floats, or min(S, radius) when the position is
 // read on the device).
-template <int DH>
+// AXIAL: scores are indexed by position in the key list: list entry j < n1 is key j (the text run), entry n1 + i is
+// key ist + i * istr (the image run of the position's row or column); at most text_len + grid_w entries.
+template <int DH, bool AXIAL = false>
 __global__ void __launch_bounds__(256)
 attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __restrict__ vc, bf16* __restrict__ out,
-                   int S, int H, int pos, float scale, const int* __restrict__ pos_dev, int radius) {
+                   int S, int H, int pos, float scale, const int* __restrict__ pos_dev, int radius, int text_len,
+                   int grid_w, int axis) {
   extern __shared__ float sc[];
   __shared__ float red[8];
   __shared__ float part[8][DH];
@@ -62,7 +67,20 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
 #pragma unroll
   for (int e = 0; e < EPL; ++e) qr[e] = __bfloat162float(q[lane * EPL + e]);
   __syncthreads();  // this block's own global writes are visible to it after the barrier
-  const int lo = max(0, pos - radius + 1), n = pos + 1 - lo;
+  const int lo = AXIAL ? 0 : max(0, pos - radius + 1);
+  int n = pos + 1 - lo, n1 = 0, ist = 0, istr = 0;
+  if constexpr (AXIAL) {
+    n1 = min(pos, text_len - 1) + 1;
+    n = n1;
+    if (pos >= text_len) {
+      const int k = pos - text_len, r = k / grid_w, c = k % grid_w;
+      ist = text_len + (axis ? c : r * grid_w);
+      istr = axis ? grid_w : 1;
+      n += (axis ? r : c) + 1;
+    }
+  }
+  // key row of list entry j
+  auto key = [&](int j) { return AXIAL ? (j < n1 ? j : ist + (j - n1) * istr) : j; };
   const bf16* kw = kcb + (long long)lo * rs;         // key / value rows of the window: j - lo = 0 .. n - 1
   const bf16* vw = vcb + (long long)lo * rs;
   auto load_row = [&](const bf16* base, int j, float* o) {
@@ -81,7 +99,7 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
     float kr[4][EPL], s[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u)
-      if (j0 + 8 * u < n) load_row(kw, j0 + 8 * u, kr[u]);
+      if (j0 + 8 * u < n) load_row(kw, key(j0 + 8 * u), kr[u]);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       s[u] = 0.f;
@@ -125,7 +143,7 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
     float vr[4][EPL];
 #pragma unroll
     for (int u = 0; u < 4; ++u)
-      if (j0 + 8 * u < n) load_row(vw, j0 + 8 * u, vr[u]);
+      if (j0 + 8 * u < n) load_row(vw, key(j0 + 8 * u), vr[u]);
 #pragma unroll
     for (int u = 0; u < 4; ++u)
       if (j0 + 8 * u < n) {
@@ -511,14 +529,26 @@ extern "C" int db200_incr_i32(db200_stream_t stream_, int32_t* p, int delta) {
 
 // pos_dev == NULL: position `pos` (scores need min(pos + 1, radius) floats of shared memory); else the position is read
 // on the device and shared memory is sized for min(S, radius) keys.  radius >= S: every key <= pos.
+// axis >= 0: an axial layer (attn_decode_kernel<DH, true>, radius unused): the key list of `pos` (text_len + grid_w
+// floats when the position is read on the device).
 static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k_cache, void* v_cache, void* out, int B,
-                              int S, int H, int dh, int pos, float scale, const int32_t* pos_dev, int radius) {
+                              int S, int H, int dh, int pos, float scale, const int32_t* pos_dev, int radius,
+                              int text_len = 0, int grid_w = 1, int axis = -1) {
   DB200_REQUIRE(qkv_step && k_cache && v_cache && out, DB200_E_INVALID, "attn_decode: null pointer");
   DB200_REQUIRE(B > 0 && H > 0 && S > 0 && pos >= 0 && pos < S, DB200_E_INVALID, "attn_decode: B %d H %d pos %d of %d",
                 B, H, pos, S);
   DB200_REQUIRE(radius >= 1, DB200_E_INVALID, "attn_decode: radius %d < 1", radius);
   DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn_decode: head_dim %d not in {64,128}", dh);
-  const size_t keys = (size_t)min(pos_dev ? S : pos + 1, radius);
+  const bool axial = axis >= 0;
+  size_t keys = (size_t)min(pos_dev ? S : pos + 1, radius);
+  if (axial) {
+    if (pos_dev) {
+      keys = (size_t)min((long long)S, (long long)text_len + grid_w);
+    } else {
+      const int k = pos - text_len;
+      keys = (size_t)(min(pos, text_len - 1) + 1) + (k >= 0 ? (size_t)((axis ? k / grid_w : k % grid_w) + 1) : 0);
+    }
+  }
   DB200_REQUIRE(keys * 4 <= 200 * 1024, DB200_E_UNSUPPORTED, "attn_decode: %zu keys exceed shared memory", keys);
   const size_t smem = keys * sizeof(float);
   dim3 grid(H, B);
@@ -526,16 +556,19 @@ static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k
                                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   static const cudaError_t a64 = cudaFuncSetAttribute(attn_decode_kernel<64>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  static const cudaError_t x128 = cudaFuncSetAttribute(attn_decode_kernel<128, true>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  static const cudaError_t x64 = cudaFuncSetAttribute(attn_decode_kernel<64, true>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   DB200_CUDA(a128);
   DB200_CUDA(a64);
-  if (dh == 128)
-    attn_decode_kernel<128><<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step),
-                                                         static_cast<bf16*>(k_cache), static_cast<bf16*>(v_cache),
-                                                         static_cast<bf16*>(out), S, H, pos, scale, pos_dev, radius);
-  else
-    attn_decode_kernel<64><<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step), static_cast<bf16*>(k_cache),
-                                                        static_cast<bf16*>(v_cache), static_cast<bf16*>(out), S, H, pos,
-                                                        scale, pos_dev, radius);
+  DB200_CUDA(x128);
+  DB200_CUDA(x64);
+  auto kernel = dh == 128 ? (axial ? attn_decode_kernel<128, true> : attn_decode_kernel<128>)
+                          : (axial ? attn_decode_kernel<64, true> : attn_decode_kernel<64>);
+  kernel<<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step), static_cast<bf16*>(k_cache),
+                                      static_cast<bf16*>(v_cache), static_cast<bf16*>(out), S, H, pos, scale, pos_dev,
+                                      radius, text_len, grid_w, axis);
   return check_launch("attn_decode_kernel");
 }
 
@@ -565,6 +598,36 @@ extern "C" int db200_attn_decode_local_dev(db200_stream_t stream_, const void* q
   DB200_REQUIRE(pos_dev, DB200_E_INVALID, "attn_decode_local_dev: null position pointer");
   return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
                             pos_dev, radius);
+}
+
+// axial layers (row: axis 0, column: axis 1): the query of `pos` attends to the text keys [0, min(pos, text_len - 1)]
+// and, at an image position (grid row r, column c), to row r's columns 0..c or column c's rows 0..r
+static int axial_decode_args_ok(const char* fn, int S, int text_len, int grid_w, int axis) {
+  DB200_REQUIRE(axis == 0 || axis == 1, DB200_E_INVALID, "%s: axis %d not 0 (row) or 1 (column)", fn, axis);
+  DB200_REQUIRE(grid_w >= 1 && text_len >= 0, DB200_E_INVALID, "%s: grid_w %d < 1 or text_len %d < 0", fn, grid_w,
+                text_len);
+  DB200_REQUIRE((long long)S <= (long long)text_len + (long long)grid_w * grid_w, DB200_E_INVALID,
+                "%s: S %d exceeds text_len %d + grid_w^2 (%d^2)", fn, S, text_len, grid_w);
+  return DB200_OK;
+}
+
+extern "C" int db200_attn_decode_axial(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
+                                       void* out, int B, int S, int H, int dh, int pos, int text_len, int grid_w,
+                                       int axis, float scale) {
+  const int rc = axial_decode_args_ok("attn_decode_axial", S, text_len, grid_w, axis);
+  if (rc != DB200_OK) return rc;
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, pos, scale,
+                            nullptr, S, text_len, grid_w, axis);
+}
+
+extern "C" int db200_attn_decode_axial_dev(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
+                                           void* out, int B, int S, int H, int dh, const int32_t* pos_dev,
+                                           int text_len, int grid_w, int axis, float scale) {
+  DB200_REQUIRE(pos_dev, DB200_E_INVALID, "attn_decode_axial_dev: null position pointer");
+  const int rc = axial_decode_args_ok("attn_decode_axial_dev", S, text_len, grid_w, axis);
+  if (rc != DB200_OK) return rc;
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
+                            pos_dev, S, text_len, grid_w, axis);
 }
 
 extern "C" int db200_sample_rows(db200_stream_t stream_, const float* logits, const float* u_or_null, int32_t* idx,

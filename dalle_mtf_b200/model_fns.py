@@ -11,7 +11,7 @@ import torch
 
 from . import lib as L
 from . import ops
-from .dalle_engine import DalleEngine, validate_loss_weights
+from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_loss_weights
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -102,8 +102,9 @@ def attention_layers(params):
 
     local_attention_radius: the reference's key (src/dalle_mtf/models.py:259, default 256), an integer >= 1.
     attention_types: per-layer attention types in GPT-Neo's form, e.g. [[["global", "local"], 3]]: each inner list is
-    repeated `count` times and the expansion must give "global" or "local" for exactly n_layers layers.  A missing or
-    null key is None: every layer global.  Returns the expanded list (or None) and the radius."""
+    repeated `count` times and the expansion must give "global", "local", "axial_row" or "axial_col" (DALL-E's row and
+    column attention over the image-token grid, DalleEngine) for exactly n_layers layers.  A missing or null key is
+    None: every layer global.  Returns the expanded list (or None) and the radius."""
     v = params.get("local_attention_radius")
     radius = 256 if v is None else v
     if isinstance(radius, bool) or not isinstance(radius, int) or radius < 1:
@@ -120,8 +121,8 @@ def attention_layers(params):
                 and isinstance(item[1], int) and not isinstance(item[1], bool) and item[1] >= 1):
             raise ValueError(f"attention_types item {item!r}: expected [[types...], count] with an integer count >= 1")
         for t in item[0]:
-            if t not in ("global", "local"):
-                raise ValueError(f"attention_types: unknown attention type {t!r} (expected 'global' or 'local')")
+            if t not in ATTENTION_TYPES:
+                raise ValueError(f"attention_types: unknown attention type {t!r} (expected one of {ATTENTION_TYPES})")
         types += list(item[0]) * item[1]
     if len(types) != n_layers:
         raise ValueError(f"attention_types expands to {len(types)} layers, but n_layers = {n_layers}")

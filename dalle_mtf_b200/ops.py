@@ -4,6 +4,7 @@ Every function enqueues on torch's current CUDA stream and returns without synch
 containers for device memory here; no torch arithmetic happens on the product path.
 """
 import ctypes
+import numbers
 
 import torch
 
@@ -288,7 +289,7 @@ def split_f32(src, hi, lo=None):
 # bench.py sets ATTN_PROFILE to a list to time every attention launch like GEMM_PROFILE: entries are
 # (start_event, end_event, causal-algorithmic flops, "fwd" | "bwd").  Forward = 2 products over the visible half of the
 # S x S logits: 4 S^2 dh B H / 2; backward = 2.5 x that (5 products).  A local launch counts the (query, key) pairs of
-# its band instead: sum_i min(i + 1, radius).
+# its band instead: sum_i min(i + 1, radius); an axial launch those of its mask (attn_pairs_axial).
 ATTN_PROFILE = None
 
 
@@ -300,7 +301,17 @@ def attn_pairs(S, radius=None):
     return r * (r + 1) / 2.0 + (S - r) * r
 
 
-def _attn_timed(kind, B, S, H, dh, call, radius=None):
+def attn_pairs_axial(S, text_len, grid_w, axis):
+    """(query, key) pairs an axial attention of length S computes: i + 1 for a text query i, text_len + c + 1 (row,
+    axis 0) or text_len + r + 1 (column, axis 1) for the image query at grid row r, column c."""
+    m, n = min(S, text_len), max(S - text_len, 0)
+    q, rem = divmod(n, grid_w)
+    image = q * grid_w * (grid_w + 1) // 2 + rem * (rem + 1) // 2 if axis == 0 else \
+        grid_w * q * (q + 1) // 2 + rem * (q + 1)
+    return float(m * (m + 1) // 2 + n * text_len + image)
+
+
+def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None):
     prof = ATTN_PROFILE
     if prof is None:
         return call()
@@ -308,7 +319,8 @@ def _attn_timed(kind, B, S, H, dh, call, radius=None):
     ev0.record()
     call()
     ev1.record()
-    prof.append((ev0, ev1, 4.0 * attn_pairs(S, radius) * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
+    pairs = attn_pairs_axial(S, *axial) if axial is not None else attn_pairs(S, radius)
+    prof.append((ev0, ev1, 4.0 * pairs * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
 
 
 def _radius(radius):
@@ -319,13 +331,30 @@ def _radius(radius):
     return int(radius)
 
 
-def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None):
+def _axial(axial, radius, dropout, what):
+    """Validated (text_len, grid_w, axis) of an axial launch, or None."""
+    if axial is None:
+        return None
+    if radius is not None or dropout is not None:
+        raise L.DB200Error(f"{what}: axial attention takes no radius and no dropout")
+    if len(axial) != 3 or any(not isinstance(v, numbers.Integral) or isinstance(v, bool) for v in axial):
+        raise L.DB200Error(f"{what}: axial must be three integers (text_len, grid_w, axis), got {axial!r}")
+    return tuple(int(v) for v in axial)
+
+
+def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, axial=None):
     """dropout: lib.Dropout of the attention-weights site (row0 = global index of sequence 0), or None.
-    radius: None = causal attention; else local attention, query i over keys (i - radius, i] (no dropout)."""
+    radius: None = causal attention; else local attention, query i over keys (i - radius, i] (no dropout).
+    axial: (text_len, grid_w, axis) = row (axis 0) or column (axis 1) attention of the image tokens of a text_len
+    caption and a grid_w x grid_w image (db200_attn_axial_fwd); excludes radius and dropout."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(lse, F32, "lse")
+    axial = _axial(axial, radius, dropout, "attn_fwd")
     radius = _radius(radius)
-    if radius is not None:
+    if axial is not None:
+        call = lambda: check(L.load().db200_attn_axial_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
+                                                           *axial, scale), "attn_axial_fwd")
+    elif radius is not None:
         if dropout is not None:
             raise L.DB200Error("attn_fwd: local attention has no dropout (src/dalle_mtf/models.py:270)")
         call = lambda: check(L.load().db200_attn_local_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
@@ -336,17 +365,23 @@ def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None):
     else:
         call = lambda: check(L.load().db200_attn_causal_fwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_fwd_ex")
-    _attn_timed("fwd", B, S, H, dh, call, radius)
+    _attn_timed("fwd", B, S, H, dh, call, radius, axial)
     return out
 
 
-def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None, radius=None):
-    """radius: as attn_fwd's (None = causal)."""
+def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None, radius=None,
+             axial=None):
+    """radius, axial: as attn_fwd's (None = causal)."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(dout, BF16, "dout"); _chk(dqkv, BF16, "dqkv")
     _chk(lse, F32, "lse"); _chk(dq_accum, F32, "dq_accum"); _chk(delta, F32, "delta")
+    axial = _axial(axial, radius, dropout, "attn_bwd")
     radius = _radius(radius)
-    if radius is not None:
+    if axial is not None:
+        call = lambda: check(L.load().db200_attn_axial_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
+                                                           ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, *axial,
+                                                           scale), "attn_axial_bwd")
+    elif radius is not None:
         if dropout is not None:
             raise L.DB200Error("attn_bwd: local attention has no dropout (src/dalle_mtf/models.py:270)")
         call = lambda: check(L.load().db200_attn_local_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
@@ -360,7 +395,7 @@ def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0,
         call = lambda: check(L.load().db200_attn_causal_bwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                                ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_bwd_ex")
-    _attn_timed("bwd", B, S, H, dh, call, radius)
+    _attn_timed("bwd", B, S, H, dh, call, radius, axial)
     return dqkv
 
 
@@ -549,14 +584,20 @@ def embed_fwd_at(ids, wte, wpe, out, pos):
     return out
 
 
-def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None):
+def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None, axial=None):
     """Append this position's k, v to the caches and attend with its q over keys <= pos (models.py:246-254, 281-299);
-    radius (local layer, models.py:257-273): over keys [max(0, pos - radius + 1), pos] only."""
+    radius (local layer, models.py:257-273): over keys [max(0, pos - radius + 1), pos] only; axial (text_len, grid_w,
+    axis) (row / column layer, attn_fwd's): over the text keys and pos's image row (axis 0) or column (axis 1)."""
     L.require_device()
     _chk(qkv_step, BF16, "qkv_step"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache"); _chk(out, BF16, "out")
     B, S, H, dh = k_cache.shape
     assert v_cache.shape == k_cache.shape and qkv_step.numel() == B * 3 * H * dh and out.numel() == B * H * dh
+    axial = _axial(axial, radius, None, "attn_decode")
     radius = _radius(radius)
+    if axial is not None:
+        check(L.load().db200_attn_decode_axial(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S,
+                                               H, dh, int(pos), *axial, float(scale)), "db200_attn_decode_axial")
+        return out
     if radius is not None:
         check(L.load().db200_attn_decode_local(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S,
                                                H, dh, int(pos), radius, float(scale)), "db200_attn_decode_local")
@@ -588,11 +629,17 @@ def embed_fwd_at_dev(tokens, wte, wpe, out, pos_dev):
     return out
 
 
-def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None):
+def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None, axial=None):
     """attn_decode with the position read on the device from pos_dev (graph replay)."""
     L.require_device()
     B, S, H, dh = k_cache.shape
+    axial = _axial(axial, radius, None, "attn_decode_dev")
     radius = _radius(radius)
+    if axial is not None:
+        check(L.load().db200_attn_decode_axial_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B,
+                                                   S, H, dh, ptr(pos_dev), *axial, float(scale)),
+              "db200_attn_decode_axial_dev")
+        return out
     if radius is not None:
         check(L.load().db200_attn_decode_local_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B,
                                                    S, H, dh, ptr(pos_dev), radius, float(scale)),

@@ -249,6 +249,18 @@ int db200_attn_local_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_
 int db200_attn_local_bwd(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
                          const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H, int dh,
                          int radius, float scale);
+/* Axial attention of DALL-E's image tokens (DALLE-pytorch's "axial_row" / "axial_col"): a text prefix of text_len
+ * positions followed by a grid_w x grid_w image, position p >= text_len being the image token at grid row
+ * r = (p - text_len) / grid_w, column c = (p - text_len) % grid_w.  A text query i attends causally to keys j <= i.  An
+ * image query attends to every text key and to the image keys of its own row at columns <= c (axis 0, row attention)
+ * or of its own column at rows <= r (axis 1, column attention).  S <= text_len + grid_w^2 (a prompt prefill may be
+ * shorter).  Layouts, workspaces and numerics as db200_attn_causal_fwd / _bwd.  No dropout.  axis not 0 or 1,
+ * grid_w < 1, text_len < 0 or S > text_len + grid_w^2: DB200_E_INVALID. */
+int db200_attn_axial_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, float* lse, int B, int S, int H,
+                         int dh, int text_len, int grid_w, int axis, float scale);
+int db200_attn_axial_bwd(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
+                         const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H, int dh,
+                         int text_len, int grid_w, int axis, float scale);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * small HBM-bound helpers
@@ -407,6 +419,16 @@ int db200_attn_decode_local(db200_stream_t stream, const void* qkv_step_bf16, vo
 int db200_attn_decode_local_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
                                 void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
                                 const int32_t* pos_dev, int radius, float scale);
+/* attn_decode / attn_decode_dev of an axial layer (db200_attn_axial_fwd's geometry): the query of position p attends
+ * to the text keys [0, min(p, text_len - 1)] and, when p is the image token at grid row r, column c, to keys
+ * text_len + r grid_w + c' for c' <= c (axis 0) or text_len + r' grid_w + c for r' <= r (axis 1).  The device-position
+ * variant sizes shared memory for min(S, text_len + grid_w) keys.  Invalid geometry as db200_attn_axial_fwd. */
+int db200_attn_decode_axial(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16, void* v_cache_bf16,
+                            void* out_bf16, int B, int S, int H, int dh, int pos, int text_len, int grid_w, int axis,
+                            float scale);
+int db200_attn_decode_axial_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
+                                void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
+                                const int32_t* pos_dev, int text_len, int grid_w, int axis, float scale);
 int db200_sample_rows_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
                          long long ld_tokens, int rows, long long ld, int lo, int hi, float inv_temp,
                          const int32_t* pos_dev);

@@ -27,6 +27,10 @@ int attn_axial_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float
                           int text_len, int grid_w, int axis, float scale);
 int attn_axial_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
                           void* dqkv, int B, int S, int H, int dh, int text_len, int grid_w, int axis, float scale);
+int attn_conv_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
+                         int text_len, int grid_w, int kernel, float scale);
+int attn_conv_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
+                         void* dqkv, int B, int S, int H, int dh, int text_len, int grid_w, int kernel, float scale);
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward: delta = rowsum(dO * O)
@@ -190,4 +194,47 @@ extern "C" int db200_attn_axial_bwd(db200_stream_t stream_, const void* qkv, con
   const int rc = attn_delta(stream, out, dout, delta, B, S, H, dh);
   if (rc != DB200_OK) return rc;
   return attn_axial_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, text_len, grid_w, axis, scale);
+}
+
+// ---- convolutional attention of DALL-E image tokens: text queries are causal; an image query at grid row r, column c
+// sees every text key and the image keys (r', c') with r - kernel < r' <= r and c - kernel < c' <= c.
+// S <= text_len + grid_w^2 (a prefill may be shorter).  No dropout.
+static int conv_args_ok(const char* fn, int S, int text_len, int grid_w, int kernel) {
+  DB200_REQUIRE(kernel >= 1, DB200_E_INVALID, "%s: kernel %d < 1", fn, kernel);
+  DB200_REQUIRE(grid_w >= 1 && text_len >= 0, DB200_E_INVALID, "%s: grid_w %d < 1 or text_len %d < 0", fn, grid_w,
+                text_len);
+  DB200_REQUIRE((long long)S <= (long long)text_len + (long long)grid_w * grid_w, DB200_E_INVALID,
+                "%s: S %d exceeds text_len %d + grid_w^2 (%d^2)", fn, S, text_len, grid_w);
+  return DB200_OK;
+}
+
+extern "C" int db200_attn_conv_fwd(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B, int S, int H,
+                                   int dh, int text_len, int grid_w, int kernel, float scale) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_conv_fwd: B,S,H must be positive");
+  const int arc = conv_args_ok("attn_conv_fwd", S, text_len, grid_w, kernel);
+  if (arc != DB200_OK) return arc;
+  DB200_REQUIRE(qkv && out && lse && aligned16(qkv) && aligned16(out), DB200_E_ALIGN,
+                "attn_conv_fwd: NULL or unaligned pointer");
+  DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_conv_fwd: scale must be > 0");
+  DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
+  return attn_conv_fwd_launch(stream, qkv, out, lse, B, S, H, dh, text_len, grid_w, kernel, scale);
+}
+
+extern "C" int db200_attn_conv_bwd(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
+                                   const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S, int H,
+                                   int dh, int text_len, int grid_w, int kernel, float scale) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  (void)dq_accum;
+  DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_conv_bwd: B,S,H must be positive");
+  const int arc = conv_args_ok("attn_conv_bwd", S, text_len, grid_w, kernel);
+  if (arc != DB200_OK) return arc;
+  DB200_REQUIRE(qkv && out && dout && lse && delta && dqkv && aligned16(qkv) && aligned16(out) && aligned16(dout) &&
+                    aligned16(dqkv),
+                DB200_E_ALIGN, "attn_conv_bwd: NULL or unaligned pointer");
+  DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_conv_bwd: scale must be > 0");
+  DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
+  const int rc = attn_delta(stream, out, dout, delta, B, S, H, dh);
+  if (rc != DB200_OK) return rc;
+  return attn_conv_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, text_len, grid_w, kernel, scale);
 }

@@ -22,6 +22,13 @@
 // segments of W rows.  Every global access (tile loads, stores, lse / delta) goes through the row map, so the tensor
 // layouts are those of the other instantiations; rows whose p >= S (a shorter prefill) are absent: zero-filled,
 // never stored, and a present query never sees one.
+//
+// CONV (DALL-E's convolutional attention, DALLE-pytorch's SparseConvCausalAttention at dilation 1): the grid of AXIAL,
+// kernel size k.  Text queries are causal; the image query at (r, c) sees every text key and the image keys (r', c')
+// with r - k < r' <= r and c - k < c' <= c, the k x k window above and to the left of it.  Rows stay in raster order
+// (no row map).  Every visible key precedes its query, but the mask is not a band: (r - 1, c + 1) is earlier and
+// outside the window.  The loops visit the text blocks and the band of blocks from the window's top row to the
+// query; each tile's mask tests the window from grid coordinates stepped along the thread's columns.
 #include "gemm_common.cuh"  // cp.async helpers
 #include "philox.cuh"
 #include "wgmma.cuh"
@@ -220,16 +227,81 @@ __device__ __forceinline__ int fa_axial_query_end(const FaAxial& a, int kb) {
   return min(nq, seg_end / FA_ROWS + 1);
 }
 
+// ---- CONV: geometry (kernel >= 1).  Rows are sequence positions.
+struct FaConv {
+  int text_len, grid_w, kernel;
+};
+// grid row / column of position p, or row -1 for a text position
+__device__ __forceinline__ void fa_conv_rc(const FaConv& c, int p, int& r, int& col) {
+  const int u = p - c.text_len;
+  r = u < 0 ? -1 : u / c.grid_w;
+  col = u < 0 ? 0 : u - (u / c.grid_w) * c.grid_w;
+}
+// Visible bits of this thread's 32 fragment elements of a 64 x 64 tile (bit x = element x, as fa_keep_bits) whose first
+// row / column are r0 / c0; rows and columns >= S are absent.  QROWS: rows are queries and columns keys (forward, dQ);
+// else rows are keys and columns queries (dK / dV).  rr / rc: grid row / column of the thread's two rows (fa_conv_rc).
+// The grid coordinates of the columns are stepped from one division per tile (floor division: a text column has a
+// negative row, and stepping carries it into the image rows).
+template <bool QROWS>
+__device__ __forceinline__ uint32_t fa_conv_vis_bits(const FaConv& cv, int S, int r0, int c0, const int (&rr)[2],
+                                                     const int (&rc)[2], const Frag& f) {
+  const int u0 = c0 + f.fc - cv.text_len;
+  int gr = u0 >= 0 ? u0 / cv.grid_w : -((cv.grid_w - 1 - u0) / cv.grid_w);
+  int gc = u0 - gr * cv.grid_w;
+  uint32_t bits = 0u;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int col = c0 + 8 * i + f.fc + e;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = r0 + f.fr + 8 * hh;
+        const bool vis =
+            QROWS ? row < S && col <= row &&
+                        (col < cv.text_len || (gr > rr[hh] - cv.kernel && gc <= rc[hh] && gc > rc[hh] - cv.kernel))
+                  : col < S && row <= col &&
+                        (row < cv.text_len || (gr - rr[hh] < cv.kernel && gc >= rc[hh] && gc - rc[hh] < cv.kernel));
+        bits |= (uint32_t)vis << (4 * i + 2 * hh + e);
+      }
+      gc += e == 0 ? 1 : 7;  // the next column: col + 1, then col + 7 = the next i's first
+      while (gc >= cv.grid_w) {
+        gc -= cv.grid_w;
+        ++gr;
+      }
+    }
+  return bits;
+}
+// key blocks of query block qb (forward, dQ): the text blocks [0, jt), then the blocks from js (the block holding the
+// first position of the window's top row, grid row max(0, r0 - k + 1), for the block's first image query at row r0) to
+// qb.  With fa_axial_next no block is visited twice.
+__device__ __forceinline__ void fa_conv_key_blocks(const FaConv& c, int qb, int& jt, int& js) {
+  jt = (c.text_len + FA_ROWS - 1) / FA_ROWS;
+  const int t = max(qb * FA_ROWS, c.text_len);
+  const int top = max(0, (t - c.text_len) / c.grid_w - c.kernel + 1);
+  js = t < (qb + 1) * FA_ROWS ? (c.text_len + top * c.grid_w) / FA_ROWS : jt;
+}
+// query blocks of key block kb (dK / dV): [kb, end).  A block holding a text key sees every later query; an image key
+// is seen up to (k - 1) rows and k - 1 columns later, i.e. at most min(k - 1, W - 1) (W + 1) positions after it.
+__device__ __forceinline__ int fa_conv_query_end(const FaConv& c, int S, int kb) {
+  const int nq = (S + FA_ROWS - 1) / FA_ROWS, k0 = kb * FA_ROWS;
+  if (k0 < c.text_len) return nq;
+  const long long last = min(k0 + FA_ROWS - 1, S - 1);
+  const long long reach = last + (long long)(min(c.kernel, c.grid_w) - 1) * (c.grid_w + 1);
+  return (int)min((long long)nq, reach / FA_ROWS + 1);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
 // forward: grid (query blocks, B * H); online softmax in the exp2 domain
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL, bool AXIAL>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV>
 __global__ void __launch_bounds__(128, 1)
 attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, const db200_dropout dr, int radius, const FaAxial ax) {
+                float scale, const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv) {
   static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
+  static_assert(!(CONV && (DROP || LOCAL || AXIAL)), "conv layers have no dropout, no window and no row map");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -247,13 +319,19 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
   int jt = 0, js = 0, slo[2] = {0, 0};  // AXIAL: key blocks and the segment start of each query row
+  int qr[2] = {0, 0}, qc[2] = {0, 0};   // CONV: grid row / column of each query row
   if constexpr (AXIAL) {
     fa_axial_key_blocks(ax, qb, jt, js);
     slo[0] = fa_axial_seg_start(ax, q0 + f.fr);
     slo[1] = fa_axial_seg_start(ax, q0 + f.fr + 8);
   }
-  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : (AXIAL && jt == 0 ? js : 0);
-  for (int j = j0; j <= qb; j = AXIAL ? fa_axial_next(j, jt, js) : j + 1) {
+  if constexpr (CONV) {
+    fa_conv_key_blocks(cv, qb, jt, js);
+    fa_conv_rc(cv, q0 + f.fr, qr[0], qc[0]);
+    fa_conv_rc(cv, q0 + f.fr + 8, qr[1], qc[1]);
+  }
+  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : ((AXIAL || CONV) && jt == 0 ? js : 0);
+  for (int j = j0; j <= qb; j = (AXIAL || CONV) ? fa_axial_next(j, jt, js) : j + 1) {
     const int k0 = j * FA_ROWS;
     __syncthreads();  // the previous block's K / V tiles are no longer read
     if constexpr (AXIAL) {
@@ -266,6 +344,7 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
     fa_tiles_ready();
     float s[32];
     fa_qk<DH>(s, sQ, sK);
+    const uint32_t vb = CONV ? fa_conv_vis_bits<true>(cv, S, q0, k0, qr, qc, f) : 0u;
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int i = 0; i < 8; ++i)
@@ -276,6 +355,7 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           float& v = s[4 * i + 2 * hh + e];
           if constexpr (AXIAL) v = (col <= row && (col < ax.text_len || col >= slo[hh])) ? v * sl2 : -INFINITY;
+          else if constexpr (CONV) v = ((vb >> (4 * i + 2 * hh + e)) & 1u) ? v * sl2 : -INFINITY;
           else v = (col <= row && col < S && (!LOCAL || col > row - radius)) ? v * sl2 : -INFINITY;
           mx[hh] = fmaxf(mx[hh], v);
         }
@@ -327,12 +407,13 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ: grid (query blocks, B * H).  P = exp(scale S - lse), dS = P (dO V^T - delta), dQ = scale dS K
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL, bool AXIAL>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                    const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                   const db200_dropout dr, int radius, const FaAxial ax) {
+                   const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv) {
   static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
+  static_assert(!(CONV && (DROP || LOCAL || AXIAL)), "conv layers have no dropout, no window and no row map");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -372,10 +453,15 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
   float dq[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) dq[i] = 0.f;
-  int jt = 0, js = 0;
+  int jt = 0, js = 0, qr[2] = {0, 0}, qc[2] = {0, 0};  // CONV: grid row / column of each query row
   if constexpr (AXIAL) fa_axial_key_blocks(ax, qb, jt, js);
-  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : (AXIAL && jt == 0 ? js : 0);
-  for (int j = j0; j <= qb; j = AXIAL ? fa_axial_next(j, jt, js) : j + 1) {
+  if constexpr (CONV) {
+    fa_conv_key_blocks(cv, qb, jt, js);
+    fa_conv_rc(cv, q0 + f.fr, qr[0], qc[0]);
+    fa_conv_rc(cv, q0 + f.fr + 8, qr[1], qc[1]);
+  }
+  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : ((AXIAL || CONV) && jt == 0 ? js : 0);
+  for (int j = j0; j <= qb; j = (AXIAL || CONV) ? fa_axial_next(j, jt, js) : j + 1) {
     const int k0 = j * FA_ROWS;
     __syncthreads();
     if constexpr (AXIAL) {
@@ -391,6 +477,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
     fa_qk<DH>(dp, sdO, sV);
     // dropout: dS = P (dP keep scale - delta)
     const uint32_t kb = DROP ? fa_keep_bits<true>(dr, b, h, H, (S + 1) >> 1, q0, k0, f) : 0u;
+    const uint32_t vb = CONV ? fa_conv_vis_bits<true>(cv, S, q0, k0, qr, qc, f) : 0u;
 #pragma unroll
     for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -400,6 +487,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           const int x = 4 * i + 2 * hh + e;
           const bool vis = AXIAL ? col <= row && (col < ax.text_len || col >= slo[hh])
+                         : CONV  ? ((vb >> x) & 1u) != 0u
                                  : col <= row && col < S && row < S && (!LOCAL || col > row - radius);
           const float p = vis ? exp2f(s[x] * sl2 - lse2[hh]) : 0.f;
           s[x] = p * ((DROP ? dp[x] * fa_keep_mul(kb, x, dr.scale) : dp[x]) - dl[hh]);
@@ -415,12 +503,13 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
 // backward, dK / dV: grid (key blocks, B * H), transposed products so that the key index is the accumulator row.
 //   P^T = exp(scale K Q^T - lse), dV = P^T dO, dS^T = P^T (V dO^T - delta), dK = scale dS^T Q
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL, bool AXIAL>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                     const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                    const db200_dropout dr, int radius, const FaAxial ax) {
+                    const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv) {
   static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
+  static_assert(!(CONV && (DROP || LOCAL || AXIAL)), "conv layers have no dropout, no window and no row map");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -435,9 +524,16 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
   const float sl2 = scale * kLog2e;
   // LOCAL: the last query that sees key k0 + 63 is k0 + 62 + radius
   // AXIAL: fa_axial_query_end; a key row sees the queries up to the end of its segment (text keys: every later one)
+  // CONV: fa_conv_query_end
   const int nqb = AXIAL ? fa_axial_query_end(ax, kb)
+                : CONV  ? fa_conv_query_end(cv, S, kb)
                 : LOCAL ? min((S + FA_ROWS - 1) / FA_ROWS, (int)(((long long)k0 + 62 + radius) / FA_ROWS) + 1)
                         : (S + FA_ROWS - 1) / FA_ROWS;
+  int kr[2] = {0, 0}, kc[2] = {0, 0};  // CONV: grid row / column of each key row
+  if constexpr (CONV) {
+    fa_conv_rc(cv, k0 + f.fr, kr[0], kc[0]);
+    fa_conv_rc(cv, k0 + f.fr + 8, kr[1], kc[1]);
+  }
   int kend[2] = {0, 0};
   if constexpr (AXIAL) {
 #pragma unroll
@@ -479,6 +575,7 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
     fa_tiles_ready();
     float st[32], dpt[32];
     fa_qk<DH>(st, sK, sQ);
+    const uint32_t vb = CONV ? fa_conv_vis_bits<false>(cv, S, k0, q0, kr, kc, f) : 0u;
 #pragma unroll
     for (int ii = 0; ii < 8; ++ii)
 #pragma unroll
@@ -488,6 +585,7 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
           const int key = k0 + f.fr + 8 * hh, cq = 8 * ii + f.fc + e, q = q0 + cq;
           const int x = 4 * ii + 2 * hh + e;
           const bool vis = AXIAL ? key <= q && (key < ax.text_len || q <= kend[hh])
+                         : CONV  ? ((vb >> x) & 1u) != 0u
                                  : key <= q && q < S && key < S && (!LOCAL || key > q - radius);
           st[x] = vis ? exp2f(st[x] * sl2 - s_lse[cq]) : 0.f;
         }
@@ -520,39 +618,40 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
 }
 
 // AXIAL: the grid covers ax.rows kernel-order rows instead of S
-template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false>
+template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false, bool CONV = false>
 static int fa_fwd(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, float scale,
-                  const db200_dropout& dr, int radius = 0, const FaAxial& ax = FaAxial{}) {
+                  const db200_dropout& dr, int radius = 0, const FaAxial& ax = FaAxial{},
+                  const FaConv& cv = FaConv{}) {
   constexpr size_t smem = fa_smem<DH>(3);
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL, AXIAL>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL, AXIAL, CONV>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(attr_rc);
   const dim3 grid(((AXIAL ? ax.rows : S) + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_fwd_kernel<DH, DROP, LOCAL, AXIAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H, scale,
-                                                                       dr, radius, ax);
+  attn_fwd_kernel<DH, DROP, LOCAL, AXIAL, CONV><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H,
+                                                                             scale, dr, radius, ax, cv);
   return check_launch("attn_fwd_kernel");
 }
 
-template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false>
+template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false, bool CONV = false>
 static int fa_bwd(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
                   void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr, int radius = 0,
-                  const FaAxial& ax = FaAxial{}) {
+                  const FaAxial& ax = FaAxial{}, const FaConv& cv = FaConv{}) {
   constexpr size_t smem = fa_smem<DH>(4);
-  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL>,
+  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL, CONV>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL>,
+  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL, CONV>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(rc1);
   DB200_CUDA(rc2);
   const dim3 grid(((AXIAL ? ax.rows : S) + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse,
-                                                                          delta, (bf16*)dqkv, S, H, scale, dr, radius,
-                                                                          ax);
+  attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL, CONV><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout,
+                                                                                lse, delta, (bf16*)dqkv, S, H, scale,
+                                                                                dr, radius, ax, cv);
   int rc = check_launch("attn_bwd_dq_kernel");
   if (rc != DB200_OK) return rc;
-  attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout, lse,
-                                                                           delta, (bf16*)dqkv, S, H, scale, dr, radius,
-                                                                           ax);
+  attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL, CONV><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout,
+                                                                                 lse, delta, (bf16*)dqkv, S, H, scale,
+                                                                                 dr, radius, ax, cv);
   return check_launch("attn_bwd_dkv_kernel");
 }
 
@@ -616,6 +715,24 @@ int attn_axial_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout
   const FaAxial ax{text_len, grid_w, axis, axial_rows(S, text_len, grid_w, axis)};
   return dh == 128 ? fa_bwd<128, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, ax)
                    : fa_bwd<64, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, ax);
+}
+
+// convolutional attention (k x k window) over a text prefix of text_len and a grid_w x grid_w image; no dropout
+int attn_conv_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, int dh,
+                         int text_len, int grid_w, int kernel, float scale) {
+  const db200_dropout none{};
+  const FaConv cv{text_len, grid_w, kernel};
+  return dh == 128 ? fa_fwd<128, false, false, false, true>(stream, qkv, out, lse, B, S, H, scale, none, 0, {}, cv)
+                   : fa_fwd<64, false, false, false, true>(stream, qkv, out, lse, B, S, H, scale, none, 0, {}, cv);
+}
+
+int attn_conv_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
+                         void* dqkv, int B, int S, int H, int dh, int text_len, int grid_w, int kernel, float scale) {
+  const db200_dropout none{};
+  const FaConv cv{text_len, grid_w, kernel};
+  return dh == 128
+             ? fa_bwd<128, false, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, {}, cv)
+             : fa_bwd<64, false, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, {}, cv);
 }
 
 }  // namespace db200

@@ -9,6 +9,8 @@
 //                  fp32 scores / softmax, P rounded to bf16 for the PV product (same policy as attn.cu)
 //                  AXIAL (row / column layers): over a key list, the text run [0, min(pos, TL - 1)] followed, for an
 //                  image position (grid row r, column c), by row r's columns 0..c or column c's rows 0..r
+//                  CONV (convolutional layers, kernel k): the text run followed by one run per row r' of the k x k
+//                  window, max(0, r - k + 1) <= r' <= r, each over columns max(0, c - k + 1) .. c
 //   sample_rows    idx = lo + argmax_{lo<=c<hi}(logits[c] * inv_temp + gumbel(u[c-lo]))   (first maximum; u NULL = greedy)
 //   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
 //   sample_rows_guided     either of the two over the classifier-free-guidance mix u + s (c - u) of a conditional
@@ -41,11 +43,14 @@ __global__ void embed_at_kernel(const int* __restrict__ ids, const bf16* __restr
 // read on the device).
 // AXIAL: scores are indexed by position in the key list: list entry j < n1 is key j (the text run), entry n1 + i is
 // key ist + i * istr (the image run of the position's row or column); at most text_len + grid_w entries.
-template <int DH, bool AXIAL = false>
+// CONV: the same text run; entry n1 + i is key ist + (i / m) grid_w + i % m (m window columns per row, ist the window's
+// top-left key); at most text_len + min(k, grid_w)^2 entries.
+template <int DH, bool AXIAL = false, bool CONV = false>
 __global__ void __launch_bounds__(256)
 attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __restrict__ vc, bf16* __restrict__ out,
                    int S, int H, int pos, float scale, const int* __restrict__ pos_dev, int radius, int text_len,
-                   int grid_w, int axis) {
+                   int grid_w, int axis, int kernel) {
+  static_assert(!(AXIAL && CONV), "one key list");
   extern __shared__ float sc[];
   __shared__ float red[8];
   __shared__ float part[8][DH];
@@ -67,8 +72,8 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
 #pragma unroll
   for (int e = 0; e < EPL; ++e) qr[e] = __bfloat162float(q[lane * EPL + e]);
   __syncthreads();  // this block's own global writes are visible to it after the barrier
-  const int lo = AXIAL ? 0 : max(0, pos - radius + 1);
-  int n = pos + 1 - lo, n1 = 0, ist = 0, istr = 0;
+  const int lo = (AXIAL || CONV) ? 0 : max(0, pos - radius + 1);
+  int n = pos + 1 - lo, n1 = 0, ist = 0, istr = 0, m = 1;
   if constexpr (AXIAL) {
     n1 = min(pos, text_len - 1) + 1;
     n = n1;
@@ -79,8 +84,22 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
       n += (axis ? r : c) + 1;
     }
   }
+  if constexpr (CONV) {
+    n1 = min(pos, text_len - 1) + 1;
+    n = n1;
+    if (pos >= text_len) {
+      const int k = pos - text_len, r = k / grid_w, c = k % grid_w;
+      const int r0 = max(0, r - kernel + 1), c0 = max(0, c - kernel + 1);
+      m = c - c0 + 1;
+      ist = text_len + r0 * grid_w + c0;
+      n += (r - r0 + 1) * m;
+    }
+  }
   // key row of list entry j
-  auto key = [&](int j) { return AXIAL ? (j < n1 ? j : ist + (j - n1) * istr) : j; };
+  auto key = [&](int j) {
+    if constexpr (CONV) return j < n1 ? j : ist + (j - n1) / m * grid_w + (j - n1) % m;
+    else return AXIAL ? (j < n1 ? j : ist + (j - n1) * istr) : j;
+  };
   const bf16* kw = kcb + (long long)lo * rs;         // key / value rows of the window: j - lo = 0 .. n - 1
   const bf16* vw = vcb + (long long)lo * rs;
   auto load_row = [&](const bf16* base, int j, float* o) {
@@ -531,16 +550,27 @@ extern "C" int db200_incr_i32(db200_stream_t stream_, int32_t* p, int delta) {
 // on the device and shared memory is sized for min(S, radius) keys.  radius >= S: every key <= pos.
 // axis >= 0: an axial layer (attn_decode_kernel<DH, true>, radius unused): the key list of `pos` (text_len + grid_w
 // floats when the position is read on the device).
+// kernel >= 1: a convolutional layer (attn_decode_kernel<DH, false, true>, radius and axis unused): the key list of
+// `pos` (text_len + kernel min(kernel, grid_w) floats when the position is read on the device).
 static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k_cache, void* v_cache, void* out, int B,
                               int S, int H, int dh, int pos, float scale, const int32_t* pos_dev, int radius,
-                              int text_len = 0, int grid_w = 1, int axis = -1) {
+                              int text_len = 0, int grid_w = 1, int axis = -1, int kernel = 0) {
   DB200_REQUIRE(qkv_step && k_cache && v_cache && out, DB200_E_INVALID, "attn_decode: null pointer");
   DB200_REQUIRE(B > 0 && H > 0 && S > 0 && pos >= 0 && pos < S, DB200_E_INVALID, "attn_decode: B %d H %d pos %d of %d",
                 B, H, pos, S);
   DB200_REQUIRE(radius >= 1, DB200_E_INVALID, "attn_decode: radius %d < 1", radius);
   DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn_decode: head_dim %d not in {64,128}", dh);
-  const bool axial = axis >= 0;
+  const bool axial = axis >= 0, conv = kernel >= 1;
   size_t keys = (size_t)min(pos_dev ? S : pos + 1, radius);
+  if (conv) {
+    if (pos_dev) {
+      keys = (size_t)min((long long)S, (long long)text_len + (long long)kernel * min(kernel, grid_w));
+    } else {
+      const int k = pos - text_len, r = k / grid_w, c = k % grid_w;
+      keys = (size_t)(min(pos, text_len - 1) + 1) +
+             (k >= 0 ? (size_t)(r - max(0, r - kernel + 1) + 1) * (size_t)(c - max(0, c - kernel + 1) + 1) : 0);
+    }
+  }
   if (axial) {
     if (pos_dev) {
       keys = (size_t)min((long long)S, (long long)text_len + grid_w);
@@ -562,13 +592,21 @@ static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   DB200_CUDA(a128);
   DB200_CUDA(a64);
+  static const cudaError_t c128 = cudaFuncSetAttribute(attn_decode_kernel<128, false, true>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  static const cudaError_t c64 = cudaFuncSetAttribute(attn_decode_kernel<64, false, true>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   DB200_CUDA(x128);
   DB200_CUDA(x64);
-  auto kernel = dh == 128 ? (axial ? attn_decode_kernel<128, true> : attn_decode_kernel<128>)
-                          : (axial ? attn_decode_kernel<64, true> : attn_decode_kernel<64>);
-  kernel<<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step), static_cast<bf16*>(k_cache),
-                                      static_cast<bf16*>(v_cache), static_cast<bf16*>(out), S, H, pos, scale, pos_dev,
-                                      radius, text_len, grid_w, axis);
+  DB200_CUDA(c128);
+  DB200_CUDA(c64);
+  auto fn = dh == 128 ? (conv ? attn_decode_kernel<128, false, true>
+                              : axial ? attn_decode_kernel<128, true> : attn_decode_kernel<128>)
+                      : (conv ? attn_decode_kernel<64, false, true>
+                              : axial ? attn_decode_kernel<64, true> : attn_decode_kernel<64>);
+  fn<<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step), static_cast<bf16*>(k_cache),
+                                  static_cast<bf16*>(v_cache), static_cast<bf16*>(out), S, H, pos, scale, pos_dev,
+                                  radius, text_len, grid_w, axis, kernel);
   return check_launch("attn_decode_kernel");
 }
 
@@ -628,6 +666,36 @@ extern "C" int db200_attn_decode_axial_dev(db200_stream_t stream_, const void* q
   if (rc != DB200_OK) return rc;
   return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
                             pos_dev, S, text_len, grid_w, axis);
+}
+
+// convolutional layers: the query of `pos` attends to the text keys [0, min(pos, text_len - 1)] and, at an image
+// position (grid row r, column c), to the k x k window of keys at rows (r - kernel, r] and columns (c - kernel, c]
+static int conv_decode_args_ok(const char* fn, int S, int text_len, int grid_w, int kernel) {
+  DB200_REQUIRE(kernel >= 1, DB200_E_INVALID, "%s: kernel %d < 1", fn, kernel);
+  DB200_REQUIRE(grid_w >= 1 && text_len >= 0, DB200_E_INVALID, "%s: grid_w %d < 1 or text_len %d < 0", fn, grid_w,
+                text_len);
+  DB200_REQUIRE((long long)S <= (long long)text_len + (long long)grid_w * grid_w, DB200_E_INVALID,
+                "%s: S %d exceeds text_len %d + grid_w^2 (%d^2)", fn, S, text_len, grid_w);
+  return DB200_OK;
+}
+
+extern "C" int db200_attn_decode_conv(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
+                                      void* out, int B, int S, int H, int dh, int pos, int text_len, int grid_w,
+                                      int kernel, float scale) {
+  const int rc = conv_decode_args_ok("attn_decode_conv", S, text_len, grid_w, kernel);
+  if (rc != DB200_OK) return rc;
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, pos, scale,
+                            nullptr, S, text_len, grid_w, -1, kernel);
+}
+
+extern "C" int db200_attn_decode_conv_dev(db200_stream_t stream_, const void* qkv_step, void* k_cache, void* v_cache,
+                                          void* out, int B, int S, int H, int dh, const int32_t* pos_dev, int text_len,
+                                          int grid_w, int kernel, float scale) {
+  DB200_REQUIRE(pos_dev, DB200_E_INVALID, "attn_decode_conv_dev: null position pointer");
+  const int rc = conv_decode_args_ok("attn_decode_conv_dev", S, text_len, grid_w, kernel);
+  if (rc != DB200_OK) return rc;
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
+                            pos_dev, S, text_len, grid_w, -1, kernel);
 }
 
 extern "C" int db200_sample_rows(db200_stream_t stream_, const float* logits, const float* u_or_null, int32_t* idx,

@@ -81,12 +81,12 @@ def param_layout(d, n_layers, V, S):
     return lay
 
 
-ATTENTION_TYPES = ("global", "local", "axial_row", "axial_col")
+ATTENTION_TYPES = ("global", "local", "axial_row", "axial_col", "conv")
 AXIAL_AXIS = {"axial_row": 0, "axial_col": 1}
 
 
 def layer_radii(attention_types, radius, n_layers):
-    """Per-layer attention radius: None for a "global" (or axial) layer, `radius` for a "local" one (attention_types
+    """Per-layer attention radius: None for a "global" (or axial, or conv) layer, `radius` for a "local" one (attention_types
     None: every layer global)."""
     if isinstance(radius, bool) or not isinstance(radius, numbers.Integral) or radius < 1:
         raise ValueError(f"local_attention_radius must be an integer >= 1, got {radius!r}")
@@ -112,6 +112,29 @@ def layer_axial(attention_types, text_seq_len, image_seq_len, n_layers):
         raise ValueError(f"axial attention layers need a square image-token grid, but image_seq_len = {image_seq_len} "
                          "is not a square")
     return [(int(text_seq_len), W, AXIAL_AXIS[t]) if t in AXIAL_AXIS else None for t in types]
+
+
+def validate_conv_kernel(kernel):
+    """The kernel size of convolutional attention layers: an integer >= 1."""
+    if isinstance(kernel, bool) or not isinstance(kernel, numbers.Integral) or kernel < 1:
+        raise ValueError(f"conv_attention_kernel must be an integer >= 1, got {kernel!r}")
+    return int(kernel)
+
+
+def layer_conv(attention_types, text_seq_len, image_seq_len, kernel, n_layers):
+    """Per-layer convolutional geometry: (text_seq_len, W, kernel) for a "conv" layer, where the image tokens form a
+    W x W grid (image_seq_len = W^2), and None for any other layer."""
+    kernel = validate_conv_kernel(kernel)
+    if attention_types is None:
+        return [None] * n_layers
+    types = list(attention_types)
+    if "conv" not in types:
+        return [None] * len(types)
+    W = math.isqrt(image_seq_len)
+    if W * W != image_seq_len:
+        raise ValueError(f"convolutional attention layers need a square image-token grid, but image_seq_len = "
+                         f"{image_seq_len} is not a square")
+    return [(int(text_seq_len), W, kernel) if t == "conv" else None for t in types]
 
 
 def _real(v):
@@ -154,21 +177,24 @@ class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lnf_g", "lnf_b", "bout")
+    conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
-                 dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0):
+                 dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
+                 conv_attention_kernel=5):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
 
-        attention_types: one "global", "local", "axial_row" or "axial_col" per layer (None: every layer global).  A
-        local layer attends from position i to positions (i - local_attention_radius, i] (src/dalle_mtf/models.py:
-        257-273).  Axial layers need image_seq_len = W^2: text positions attend causally, and the image token at grid
-        row r, column c attends to every text position and to the image tokens of row r at columns <= c (axial_row)
-        or of column c at rows <= r (axial_col).  Local and axial layers apply no attention dropout (the reference
-        passes local attention none, :270; the dropout site 2 + 3l of such a layer l is unused); their residual dropout
-        is unchanged.
+        attention_types: one "global", "local", "axial_row", "axial_col" or "conv" per layer (None: every layer
+        global).  A local layer attends from position i to positions (i - local_attention_radius, i]
+        (src/dalle_mtf/models.py:257-273).  Axial and conv layers need image_seq_len = W^2: text positions attend
+        causally, and the image token at grid row r, column c attends to every text position and to the image tokens
+        of row r at columns <= c (axial_row), of column c at rows <= r (axial_col), or at rows (r - k, r] and columns
+        (c - k, c] with k = conv_attention_kernel (conv, DALL-E's convolutional mask).  Local, axial and conv layers
+        apply no attention dropout (the reference passes local attention none, :270; the dropout site 2 + 3l of such a
+        layer l is unused); their residual dropout is unchanged.
 
         zero: a DataParallel with world > 1 turns on optimiser-state sharding (ZeRO-1, SURVEY.md §7 "12 B in pure
         DP"): fp32 master / Adam m / Adam v exist only for this rank's 1/N slice of the flat buffer, the bf16 compute
@@ -209,6 +235,9 @@ class DalleEngine:
         # per layer: None or the (text_len, grid_w, axis) of an axial layer, and the attention ops' keyword for it
         self.axial = layer_axial(attention_types, text_seq_len, image_seq_len, n_layers)
         self.axial_kw = [{} if a is None else {"axial": a} for a in self.axial]
+        # per layer: None or the (text_len, grid_w, kernel) of a conv layer, and the attention ops' keyword for it
+        self.conv = layer_conv(attention_types, text_seq_len, image_seq_len, conv_attention_kernel, n_layers)
+        self.conv_kw = [{} if c is None else {"conv": c} for c in self.conv]
         lw = (None, None) if loss_weights is None else tuple(loss_weights)
         self.loss_weights, self.z_loss = validate_loss_weights(*lw, z_loss)
         self.weighted_loss = self.loss_weights is not None or self.z_loss > 0
@@ -501,7 +530,9 @@ class DalleEngine:
         rows0 = row0 * self.S
         return {
             "wte": mk(emb, L.SITE_WTE, rows0), "wpe": mk(emb, L.SITE_WPE, 0),
-            "attn": [mk(att, L.dropout_site_attn(i), row0) if self.radii[i] is None and self.axial[i] is None else None
+            "attn": [mk(att, L.dropout_site_attn(i), row0)
+                     if self.radii[i] is None and self.axial[i] is None and (self.conv is None or self.conv[i] is None)
+                     else None
                      for i in range(self.L)],
             "attn_out": [mk(res, L.dropout_site_attn_out(i), rows0) for i in range(self.L)],
             "mlp_out": [mk(res, L.dropout_site_mlp_out(i), rows0) for i in range(self.L)],
@@ -519,7 +550,8 @@ class DalleEngine:
                           self.ln_eps)
         ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
         ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
-                     dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i])  # :257-299
+                     dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
+                     **self.conv_kw[i])  # :257-299
         ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in,
                        dropout=self._site("attn_out", i))                               # :303-314,330
         ops.layernorm_fwd(sv["xmid"], self.P(p + "ln2_g"), self.P(p + "ln2_b"), sv["ln2"], sv["mean2"], sv["rstd2"],
@@ -685,7 +717,7 @@ class DalleEngine:
         ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
         ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"], B,
                      self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i), radius=self.radii[i],
-                     **self.axial_kw[i])
+                     **self.axial_kw[i], **self.conv_kw[i])
         ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                      # dLN1 out
         ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
         return self._ln_bwd(bufs["dtmp"], x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,

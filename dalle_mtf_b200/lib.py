@@ -137,6 +137,10 @@ _SIGNATURES = {
                                 c_f32],
     "db200_attn_decode_axial_dev": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                     c_f32],
+    "db200_attn_decode_conv": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                               c_f32],
+    "db200_attn_decode_conv_dev": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
+                                   c_f32],
     "db200_sample_rows_at": [c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_i64, c_int, c_int, c_f32, c_vp],
     "db200_incr_i32": [c_vp, c_vp, c_int],
     "db200_sample_rows_filtered": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_int, c_int, c_f32, c_int, c_f32],
@@ -164,6 +168,9 @@ _SIGNATURES = {
     "db200_attn_axial_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_axial_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                              c_int, c_f32],
+    "db200_attn_conv_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f32],
+    "db200_attn_conv_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
+                            c_int, c_f32],
     "db200_colsum_bf16": [c_vp, c_vp, c_i64, c_int, c_int, c_vp, c_vp, c_i64],
     "db200_cast_f32_to_bf16": [c_vp, c_vp, c_vp, c_sz],
     "db200_cast_bf16_to_f32": [c_vp, c_vp, c_vp, c_sz],

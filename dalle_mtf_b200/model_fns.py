@@ -11,7 +11,7 @@ import torch
 
 from . import lib as L
 from . import ops
-from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_loss_weights
+from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_conv_kernel, validate_loss_weights
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -102,9 +102,10 @@ def attention_layers(params):
 
     local_attention_radius: the reference's key (src/dalle_mtf/models.py:259, default 256), an integer >= 1.
     attention_types: per-layer attention types in GPT-Neo's form, e.g. [[["global", "local"], 3]]: each inner list is
-    repeated `count` times and the expansion must give "global", "local", "axial_row" or "axial_col" (DALL-E's row and
-    column attention over the image-token grid, DalleEngine) for exactly n_layers layers.  A missing or null key is
-    None: every layer global.  Returns the expanded list (or None) and the radius."""
+    repeated `count` times and the expansion must give "global", "local", "axial_row", "axial_col" or "conv" (DALL-E's
+    row, column and convolutional attention over the image-token grid, DalleEngine) for exactly n_layers layers.  A
+    missing or null key is None: every layer global.  Returns the expanded list (or None) and the radius; the kernel
+    size of conv layers is conv_kernel's."""
     v = params.get("local_attention_radius")
     radius = 256 if v is None else v
     if isinstance(radius, bool) or not isinstance(radius, int) or radius < 1:
@@ -127,6 +128,16 @@ def attention_layers(params):
     if len(types) != n_layers:
         raise ValueError(f"attention_types expands to {len(types)} layers, but n_layers = {n_layers}")
     return types, radius
+
+
+def conv_kernel(params):
+    """conv_attention_kernel of a DALL-E config: the k of "conv" layers' k x k window (DalleEngine), an integer >= 1.
+    A missing or null key is 5, DALLE-pytorch's default."""
+    v = params.get("conv_attention_kernel")
+    try:
+        return validate_conv_kernel(5 if v is None else v)
+    except ValueError:
+        raise ValueError(f"conv_attention_kernel = {v!r}: must be an integer >= 1") from None
 
 
 def caption_dropout(params):
@@ -162,6 +173,7 @@ def dalle_model_fn(features, labels, mode, params):
         raise NotImplementedError                                             # model_fns.py:135-136
     cap_rate, pad_id = caption_dropout(params)
     attention_types, local_radius = attention_layers(params)
+    conv_k = conv_kernel(params)
     weights, z_loss = loss_weights(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
@@ -194,7 +206,7 @@ def dalle_model_fn(features, labels, mode, params):
                         zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None,
                         dropout=rates, dropout_seed=params.get("seed") or 0,
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
-                        loss_weights=weights, z_loss=z_loss)
+                        conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

@@ -6,7 +6,7 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
-from .model_fns import attention_layers, dropout_rates, loss_weights
+from .model_fns import attention_layers, conv_kernel, dropout_rates, loss_weights
 from .vae_engine import VaeEngine
 
 
@@ -22,6 +22,7 @@ class DALLE:
             raise NotImplementedError("incremental inference is stubbed in the reference too (src/model_fns.py:135)")
         params = params or {}
         attention_types, local_radius = attention_layers({**params, "n_layers": n_layers})
+        conv_k = conv_kernel(params)
         weights, z_loss = loss_weights(params)
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
@@ -34,7 +35,7 @@ class DALLE:
                                   image_seq_len, recompute_grad=bool(params.get("recompute_grad")) and mode == "train",
                                   dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0,
                                   attention_types=attention_types, local_attention_radius=local_radius,
-                                  loss_weights=weights, z_loss=z_loss)
+                                  conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

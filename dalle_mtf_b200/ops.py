@@ -289,7 +289,8 @@ def split_f32(src, hi, lo=None):
 # bench.py sets ATTN_PROFILE to a list to time every attention launch like GEMM_PROFILE: entries are
 # (start_event, end_event, causal-algorithmic flops, "fwd" | "bwd").  Forward = 2 products over the visible half of the
 # S x S logits: 4 S^2 dh B H / 2; backward = 2.5 x that (5 products).  A local launch counts the (query, key) pairs of
-# its band instead: sum_i min(i + 1, radius); an axial launch those of its mask (attn_pairs_axial).
+# its band instead: sum_i min(i + 1, radius); an axial (convolutional) launch those of its mask (attn_pairs_axial,
+# attn_pairs_conv).
 ATTN_PROFILE = None
 
 
@@ -311,7 +312,21 @@ def attn_pairs_axial(S, text_len, grid_w, axis):
     return float(m * (m + 1) // 2 + n * text_len + image)
 
 
-def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None):
+def attn_pairs_conv(S, text_len, grid_w, kernel):
+    """(query, key) pairs a convolutional attention of length S computes: i + 1 for a text query i, text_len +
+    min(kernel, r + 1) min(kernel, c + 1) for the image query at grid row r, column c."""
+    k = kernel
+
+    def run(n):   # sum_{i < n} min(k, i + 1)
+        return n * (n + 1) // 2 if n <= k else k * (k + 1) // 2 + (n - k) * k
+
+    m, n = min(S, text_len), max(S - text_len, 0)
+    q, rem = divmod(n, grid_w)
+    image = run(q) * run(grid_w) + min(k, q + 1) * run(rem)
+    return float(m * (m + 1) // 2 + n * text_len + image)
+
+
+def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None, conv=None):
     prof = ATTN_PROFILE
     if prof is None:
         return call()
@@ -319,7 +334,8 @@ def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None):
     ev0.record()
     call()
     ev1.record()
-    pairs = attn_pairs_axial(S, *axial) if axial is not None else attn_pairs(S, radius)
+    pairs = attn_pairs_axial(S, *axial) if axial is not None else \
+        attn_pairs_conv(S, *conv) if conv is not None else attn_pairs(S, radius)
     prof.append((ev0, ev1, 4.0 * pairs * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
 
 
@@ -342,16 +358,34 @@ def _axial(axial, radius, dropout, what):
     return tuple(int(v) for v in axial)
 
 
-def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, axial=None):
+def _conv(conv, radius, axial, dropout, what):
+    """Validated (text_len, grid_w, kernel) of a convolutional launch, or None."""
+    if conv is None:
+        return None
+    if radius is not None or axial is not None or dropout is not None:
+        raise L.DB200Error(f"{what}: convolutional attention takes no radius, no axial geometry and no dropout")
+    if len(conv) != 3 or any(not isinstance(v, numbers.Integral) or isinstance(v, bool) for v in conv):
+        raise L.DB200Error(f"{what}: conv must be three integers (text_len, grid_w, kernel), got {conv!r}")
+    return tuple(int(v) for v in conv)
+
+
+def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, axial=None, conv=None):
     """dropout: lib.Dropout of the attention-weights site (row0 = global index of sequence 0), or None.
     radius: None = causal attention; else local attention, query i over keys (i - radius, i] (no dropout).
     axial: (text_len, grid_w, axis) = row (axis 0) or column (axis 1) attention of the image tokens of a text_len
-    caption and a grid_w x grid_w image (db200_attn_axial_fwd); excludes radius and dropout."""
+    caption and a grid_w x grid_w image (db200_attn_axial_fwd); excludes radius and dropout.
+    conv: (text_len, grid_w, kernel) = convolutional attention over the same grid, the image query at (r, c) over the
+    caption and the kernel x kernel window of image tokens (r - kernel, r] x (c - kernel, c] (db200_attn_conv_fwd);
+    excludes radius, axial and dropout."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(lse, F32, "lse")
+    conv = _conv(conv, radius, axial, dropout, "attn_fwd")
     axial = _axial(axial, radius, dropout, "attn_fwd")
     radius = _radius(radius)
-    if axial is not None:
+    if conv is not None:
+        call = lambda: check(L.load().db200_attn_conv_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
+                                                          *conv, scale), "attn_conv_fwd")
+    elif axial is not None:
         call = lambda: check(L.load().db200_attn_axial_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                            *axial, scale), "attn_axial_fwd")
     elif radius is not None:
@@ -365,19 +399,24 @@ def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, a
     else:
         call = lambda: check(L.load().db200_attn_causal_fwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_fwd_ex")
-    _attn_timed("fwd", B, S, H, dh, call, radius, axial)
+    _attn_timed("fwd", B, S, H, dh, call, radius, axial, conv)
     return out
 
 
 def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None, radius=None,
-             axial=None):
-    """radius, axial: as attn_fwd's (None = causal)."""
+             axial=None, conv=None):
+    """radius, axial, conv: as attn_fwd's (None = causal)."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(dout, BF16, "dout"); _chk(dqkv, BF16, "dqkv")
     _chk(lse, F32, "lse"); _chk(dq_accum, F32, "dq_accum"); _chk(delta, F32, "delta")
+    conv = _conv(conv, radius, axial, dropout, "attn_bwd")
     axial = _axial(axial, radius, dropout, "attn_bwd")
     radius = _radius(radius)
-    if axial is not None:
+    if conv is not None:
+        call = lambda: check(L.load().db200_attn_conv_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
+                                                          ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, *conv,
+                                                          scale), "attn_conv_bwd")
+    elif axial is not None:
         call = lambda: check(L.load().db200_attn_axial_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                            ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, *axial,
                                                            scale), "attn_axial_bwd")
@@ -395,7 +434,7 @@ def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0,
         call = lambda: check(L.load().db200_attn_causal_bwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                                ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_bwd_ex")
-    _attn_timed("bwd", B, S, H, dh, call, radius, axial)
+    _attn_timed("bwd", B, S, H, dh, call, radius, axial, conv)
     return dqkv
 
 
@@ -584,16 +623,22 @@ def embed_fwd_at(ids, wte, wpe, out, pos):
     return out
 
 
-def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None, axial=None):
+def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None, axial=None, conv=None):
     """Append this position's k, v to the caches and attend with its q over keys <= pos (models.py:246-254, 281-299);
     radius (local layer, models.py:257-273): over keys [max(0, pos - radius + 1), pos] only; axial (text_len, grid_w,
-    axis) (row / column layer, attn_fwd's): over the text keys and pos's image row (axis 0) or column (axis 1)."""
+    axis) (row / column layer, attn_fwd's): over the text keys and pos's image row (axis 0) or column (axis 1); conv
+    (text_len, grid_w, kernel) (convolutional layer, attn_fwd's): over the text keys and pos's kernel x kernel window."""
     L.require_device()
     _chk(qkv_step, BF16, "qkv_step"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache"); _chk(out, BF16, "out")
     B, S, H, dh = k_cache.shape
     assert v_cache.shape == k_cache.shape and qkv_step.numel() == B * 3 * H * dh and out.numel() == B * H * dh
+    conv = _conv(conv, radius, axial, None, "attn_decode")
     axial = _axial(axial, radius, None, "attn_decode")
     radius = _radius(radius)
+    if conv is not None:
+        check(L.load().db200_attn_decode_conv(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S,
+                                              H, dh, int(pos), *conv, float(scale)), "db200_attn_decode_conv")
+        return out
     if axial is not None:
         check(L.load().db200_attn_decode_axial(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S,
                                                H, dh, int(pos), *axial, float(scale)), "db200_attn_decode_axial")
@@ -629,12 +674,18 @@ def embed_fwd_at_dev(tokens, wte, wpe, out, pos_dev):
     return out
 
 
-def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None, axial=None):
+def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None, axial=None, conv=None):
     """attn_decode with the position read on the device from pos_dev (graph replay)."""
     L.require_device()
     B, S, H, dh = k_cache.shape
+    conv = _conv(conv, radius, axial, None, "attn_decode_dev")
     axial = _axial(axial, radius, None, "attn_decode_dev")
     radius = _radius(radius)
+    if conv is not None:
+        check(L.load().db200_attn_decode_conv_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B,
+                                                  S, H, dh, ptr(pos_dev), *conv, float(scale)),
+              "db200_attn_decode_conv_dev")
+        return out
     if axial is not None:
         check(L.load().db200_attn_decode_axial_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B,
                                                    S, H, dh, ptr(pos_dev), *axial, float(scale)),

@@ -9,7 +9,7 @@ parameters and the same kernels' numerics as training:
   per position p:   x = wte[token] + wpe[p]                                     (embed_fwd_at)
   per layer:        q|k|v = LN1(x) Wqkv;  cache[p] = k, v;  a = softmax_{j<=p}(q.k_j) v_j   (attn_decode;
                     a local layer of radius r takes j > p - r only, models.py:257-273; an axial layer the text
-                    positions and p's image row or column)
+                    positions and p's image row or column; a conv layer the text positions and p's k x k window)
                     x = x + a Wo + o_b;  x = x + relu(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows)
   logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
 
@@ -77,7 +77,7 @@ class DalleSampler:
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
             ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
-                            **e.axial_kw[i])
+                            **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), relu=True)
@@ -99,7 +99,7 @@ class DalleSampler:
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
             ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
-                                radius=e.radii[i], **e.axial_kw[i])
+                                radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), relu=True)

@@ -17,7 +17,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
-from dalle_mtf_b200.model_fns import attention_layers, vae_checkpoint
+from dalle_mtf_b200.model_fns import attention_layers, conv_kernel, vae_checkpoint
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
 PADDING_ID = 50257   # GPT-2 vocabulary + <|padding|> (src/data/tokenizer_utils.py), what training pads captions with
@@ -150,6 +150,7 @@ def main(argv=None):
     ckpt, vae_ckpt = find_checkpoints(params, args.checkpoint)
     tl, tv, iv = params["text_seq_len"], params["text_vocab_size"], params["image_vocab_size"]
     attention_types, local_radius = attention_layers(params)    # the layer types the checkpoint was trained with
+    conv_k = conv_kernel(params)
     if args.guidance_scale is not None and not 0 <= padding_id(params) < tv:
         raise SystemExit(f"--guidance_scale: padding id {padding_id(params)} outside [0, {tv}); set padding_id in the "
                          "config")
@@ -183,7 +184,8 @@ def main(argv=None):
         raise SystemExit(f"VAE has {vae.K} codes but image_vocab_size is {iv}: a sampled id would index past the "
                          "codebook")
     eng = DalleEngine(params["n_embd"], params["n_layers"], params["n_heads"], tv, iv, tl, vae.image_seq_len,
-                      device=device, attention_types=attention_types, local_attention_radius=local_radius)
+                      device=device, attention_types=attention_types, local_attention_radius=local_radius,
+                      conv_attention_kernel=conv_k)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})

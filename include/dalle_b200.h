@@ -262,6 +262,19 @@ int db200_attn_axial_bwd(db200_stream_t stream, const void* qkv_bf16, const void
                          const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H, int dh,
                          int text_len, int grid_w, int axis, float scale);
 
+/* Convolutional attention of DALL-E's image tokens (DALLE-pytorch's SparseConvCausalAttention at dilation 1), over the
+ * grid of db200_attn_axial_fwd.  A text query i attends causally to keys j <= i.  The image query at grid row r,
+ * column c attends to every text key and to the image keys at rows r' and columns c' with r - kernel < r' <= r and
+ * c - kernel < c' <= c: the kernel x kernel window above and to the left of it, itself included (kernel >= grid_w: every
+ * image key at rows <= r and columns <= c).  S <= text_len + grid_w^2 (a prompt prefill may be shorter).  Layouts,
+ * workspaces and numerics as db200_attn_causal_fwd / _bwd.  No dropout.  kernel < 1, grid_w < 1, text_len < 0 or
+ * S > text_len + grid_w^2: DB200_E_INVALID. */
+int db200_attn_conv_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, float* lse, int B, int S, int H,
+                        int dh, int text_len, int grid_w, int kernel, float scale);
+int db200_attn_conv_bwd(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16, const void* dout_bf16,
+                        const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H, int dh,
+                        int text_len, int grid_w, int kernel, float scale);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * small HBM-bound helpers
  * ------------------------------------------------------------------------------------------------------------------ */
@@ -429,6 +442,17 @@ int db200_attn_decode_axial(db200_stream_t stream, const void* qkv_step_bf16, vo
 int db200_attn_decode_axial_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
                                 void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
                                 const int32_t* pos_dev, int text_len, int grid_w, int axis, float scale);
+/* attn_decode / attn_decode_dev of a convolutional layer (db200_attn_conv_fwd's geometry): the query of position p
+ * attends to the text keys [0, min(p, text_len - 1)] and, when p is the image token at grid row r, column c, to the
+ * keys text_len + r' grid_w + c' for max(0, r - kernel + 1) <= r' <= r and max(0, c - kernel + 1) <= c' <= c.  The
+ * device-position variant sizes shared memory for min(S, text_len + kernel min(kernel, grid_w)) keys.  Invalid
+ * geometry as db200_attn_conv_fwd. */
+int db200_attn_decode_conv(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16, void* v_cache_bf16,
+                           void* out_bf16, int B, int S, int H, int dh, int pos, int text_len, int grid_w, int kernel,
+                           float scale);
+int db200_attn_decode_conv_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
+                               void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
+                               const int32_t* pos_dev, int text_len, int grid_w, int kernel, float scale);
 int db200_sample_rows_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
                          long long ld_tokens, int rows, long long ld, int lo, int hi, float inv_temp,
                          const int32_t* pos_dev);

@@ -127,6 +127,21 @@ def kernel_order(S, text_len, grid_w, axis):
     return torch.where(t < text_len, t, text_len + (u % grid_w) * grid_w + u // grid_w)
 
 
+def key_blocks(S, text_len, grid_w, qb, rows=64):
+    """Kernel-order key blocks the forward / dQ kernels visit for query block qb (attn_fa.cu fa_axial_key_blocks and
+    fa_axial_next, restated for 64-row blocks): the text blocks, then the blocks from the one holding the segment start
+    of the block's first image query to qb."""
+    jt = -(-text_len // rows)
+    t = max(qb * rows, text_len)
+    seg = 0 if t < text_len else text_len + (t - text_len) // grid_w * grid_w
+    js = seg // rows if t < (qb + 1) * rows else jt
+    j, out = (js if jt == 0 else 0), []
+    while j <= qb:
+        out.append(j)
+        j = js if (jt <= j + 1 < js) else j + 1
+    return out
+
+
 def segment_hidden(S, text_len, grid_w):
     """[S,S] bool of the kernel-order mask: True unless t_k <= t_q and (t_k < text_len or t_k, t_q lie in the same
     segment of grid_w image rows)."""

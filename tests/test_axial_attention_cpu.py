@@ -117,6 +117,24 @@ def test_column_layer_is_the_segment_mask_in_kernel_order(TL, W):
     assert torch.equal(OA.axial_hidden(S, TL, W, 0), seg)
 
 
+@pytest.mark.parametrize("TL,W", [(256, 32), (100, 24), (64, 80), (7, 1), (0, 24), (0, 40), (0, 3)])
+def test_key_block_walk_covers_every_visible_pair(TL, W):
+    """axial_oracle.key_blocks (the forward / dQ walk) visits each key block once, never past the query block, and
+    every 64 x 64 tile of the kernel-order mask that holds a visible pair.  With TL = 0 and W = 24 query block 1 starts
+    its walk at block 0, where its rows 72..127 see nothing."""
+    S = TL + W * W
+    n = -(-S // 64)
+    pad = torch.zeros(n * 64, n * 64, dtype=torch.bool)
+    pad[:S, :S] = ~OA.segment_hidden(S, TL, W)
+    need = pad.view(n, 64, n, 64).any(3).any(1)
+    for qb in range(n):
+        blocks = OA.key_blocks(S, TL, W, qb)
+        assert len(set(blocks)) == len(blocks) and all(0 <= j <= qb for j in blocks)
+        assert set(need[qb].nonzero()[:, 0].tolist()) <= set(blocks), qb
+    if (TL, W) == (0, 24):
+        assert OA.key_blocks(S, 0, 24, 1) == [0, 1] and not pad[72:128, :64].any() and pad[64:72, 48:64].all()
+
+
 # ------------------------------------------------------------------------------------------------------- oracle
 def _case(types, seed=0, B=2, ts=5, isl=16, L=3, dtype=torch.float32):
     cfg = OA.AxialConfig(64, L, 2, 100, 30, ts, isl, attention_types=types, local_attention_radius=3)

@@ -51,7 +51,8 @@ def visible(S, TL, W, axis, shift=0):
 
 
 def masked_reference(q, k, v, do, o, scale, mask):
-    """test_local_attention_gpu.local_reference with an arbitrary [S,S] visibility mask (every row sees a key)."""
+    """test_local_attention_gpu.local_reference with an arbitrary [S,S] visibility mask (every row sees a key).
+    do = None: the forward only (O and lse; b_bwd is None)."""
     q, k, v = (t.to(F64).permute(0, 2, 1, 3) for t in (q, k, v))
     S, dh = q.shape[2], q.shape[3]
     s = (scale * q @ k.transpose(-1, -2)).masked_fill(~mask, -math.inf)
@@ -65,6 +66,10 @@ def masked_reference(q, k, v, do, o, scale, mask):
     eps_lse = eps_row + (S + 32) * U + (nblk + 4) * 2.0 ** -21 + 2 * U * lse.abs()
     out = {"O": (P @ v, P @ v.abs()), "lse": (lse, eps_lse)}
     b_fwd = UBF + 2 * eps_row + (2 * nblk + 2) * 2.0 ** -21 + (2 * S + 2 * nblk + 32) * UTC
+    if do is None:
+        out = {n: (x.permute(0, 2, 1, 3) if x.dim() == 4 else x, a.permute(0, 2, 1, 3) if a.dim() == 4 else a)
+               for n, (x, a) in out.items()}
+        return out, b_fwd.permute(0, 2, 1)[..., None], None
     do, o = do.to(F64).permute(0, 2, 1, 3), o.to(F64).permute(0, 2, 1, 3)
     dP, dPa = do @ v.transpose(-1, -2), do.abs() @ v.abs().transpose(-1, -2)
     delta, deltaa = (do * o).sum(-1, keepdim=True), (do * o).abs().sum(-1, keepdim=True)

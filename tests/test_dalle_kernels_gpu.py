@@ -182,7 +182,8 @@ def _describe(name, args, kw):
     if name in ("attn_fwd", "attn_bwd"):
         B, S, H, dh = args[3:7] if name == "attn_fwd" else args[7:11]
         scale = args[7] if name == "attn_fwd" and len(args) > 7 else (args[11] if len(args) > 11 else kw["scale"])
-        return (name, B, S, H, dh, float(scale), kw.get("dropout") is not None, kw.get("radius"))
+        return (name, B, S, H, dh, float(scale), kw.get("dropout") is not None, kw.get("radius"), kw.get("axial"),
+                kw.get("conv"))
     if name == "layernorm_fwd":
         return (name,) + tuple(args[0].shape)
     if name == "layernorm_bwd":
@@ -629,8 +630,9 @@ def test_attention_at_the_engine_shapes(ops, config):
     calls, _, _, _, S = engine_calls(ops, config)
     att = [c for c in calls if c[0] in ("attn_fwd", "attn_bwd")]
     assert {c[0] for c in att} == {"attn_fwd", "attn_bwd"} and len({c[1:] for c in att}) == 1
-    _, _, S_, H, dh, scale, dropout, radius = att[0]
-    assert not dropout and radius is None                 # the configurations' engines run causal attention
+    _, _, S_, H, dh, scale, dropout, radius, axial, conv = att[0]
+    # the configurations' engines run causal attention: no window, no axial and no conv geometry
+    assert not dropout and radius is None and axial is None and conv is None
     B = CONFIGS[config] // S
     qkv, dout = _qkv(B, S, H, dh, _gen(B * H))
     run_attention(ops, f"{config} attention B={B} S={S} H={H} dh={dh}", B, S, H, dh, scale, qkv, dout)

@@ -93,8 +93,8 @@ def sharp_engine(config, attention_types=None):
     """DalleEngine at the configuration's width, heads and vocabulary, with init_params weights sharpened as
     test_prefill_gpu.sharp_engine does: x4 on wte, wout and the layer kernels, biases and LayerNorm betas N(0, 0.02)
     (bout zero past V).  Attention is then peaked rather than uniform.  One layer, or one per entry of
-    attention_types (local layers at the configuration's local_attention_radius, default 256).  One engine lives at
-    a time."""
+    attention_types (local layers at the configuration's local_attention_radius, default 256; conv layers at
+    its conv_attention_kernel, default 5).  One engine lives at a time."""
     key = (config, None if attention_types is None else tuple(attention_types))
     if key in _ENGINE:
         return _ENGINE[key]
@@ -105,7 +105,8 @@ def sharp_engine(config, attention_types=None):
     n_layers = 1 if attention_types is None else len(attention_types)
     eng = DalleEngine(cfg["n_embd"], n_layers, cfg["n_heads"], cfg["text_vocab_size"], cfg["image_vocab_size"],
                       TEXT_LEN, IMAGE_LEN, attention_types=attention_types,
-                      local_attention_radius=cfg.get("local_attention_radius", 256))
+                      local_attention_radius=cfg.get("local_attention_radius", 256),
+                      conv_attention_kernel=cfg.get("conv_attention_kernel", 5))
     eng.init_params(seed=3)
     g = DK._gen(9)
     for n in ("wte", "wout") + tuple(f"l{i}.{w}" for i in range(n_layers) for w in ("wqkv", "wo", "w1", "w2")):
@@ -128,7 +129,7 @@ def describe(name, args, kw):
     if name in ("gemm", "layernorm_fwd", "attn_fwd", "embed_fwd"):
         return DK._describe(name, args, kw)
     if name in ("attn_decode", "attn_decode_dev"):
-        return (name,) + tuple(args[1].shape) + (float(args[5]), kw.get("radius"))
+        return (name,) + tuple(args[1].shape) + (float(args[5]), kw.get("radius"), kw.get("axial"), kw.get("conv"))
     if name == "embed_fwd_at":
         return (name, args[3].shape[0], args[1].shape[0], args[3].shape[1])
     if name == "embed_fwd_at_dev":
@@ -163,7 +164,8 @@ def generation_calls(ops, config, attention_types=None):
     """Distinct calls of (a) eager DalleSampler.step at STEP_ROWS rows and positions 0, 1, 256, and (b) complete() of
     REC_B prompts with a REC_N-code image prefix, REC_REP samples per prompt and guidance (the captured step at
     2 REC_B REC_REP rows and the prefill of 2 REC_B prompts), on sharp_engine(config, attention_types).  Also returns
-    the engine's dimensions and its per-layer radii (None: global)."""
+    the engine's dimensions, its per-layer radii (None: global) and its per-layer attention geometry
+    layers = ((radius, axial, conv), ...) as the attention ops take them (all None: causal)."""
     key = (config, None if attention_types is None else tuple(attention_types))
     if key in _CALLS:
         return _CALLS[key]
@@ -190,7 +192,7 @@ def generation_calls(ops, config, attention_types=None):
         torch.cuda.synchronize()
     assert out.shape == (REC_B * REC_REP, eng.S)
     dims = types.SimpleNamespace(d=eng.d, H=eng.H, dh=eng.dh, V=eng.V, Vpad=eng.Vpad, S=eng.S, scale=eng.attn_scale,
-                                 radii=tuple(eng.radii))
+                                 radii=tuple(eng.radii), layers=tuple(zip(eng.radii, eng.axial, eng.conv)))
     res = ({k: list(v) for k, v in seen.items()}, dims)
     del smp
     torch.cuda.empty_cache()
@@ -212,23 +214,24 @@ def step_products(M, dm):
 
 
 def expected_step_calls(rows, dm, graphed):
-    """The distinct calls of one step at `rows` rows: one attn_decode(_dev) shape per distinct layer radius."""
+    """The distinct calls of one step at `rows` rows: one attn_decode(_dev) shape per distinct layer geometry
+    (radius, axial, conv)."""
     s = set(step_products(rows, dm)) | {("layernorm_fwd", rows, dm.d)}
     if graphed:
-        s |= {("attn_decode_dev", rows, dm.S, dm.H, dm.dh, dm.scale, r) for r in dm.radii}
+        s |= {("attn_decode_dev", rows, dm.S, dm.H, dm.dh, dm.scale) + g for g in dm.layers}
         s |= {("embed_fwd_at_dev", rows, dm.V, dm.d, dm.S)}
     else:
-        s |= {("attn_decode", rows, dm.S, dm.H, dm.dh, dm.scale, r) for r in dm.radii}
+        s |= {("attn_decode", rows, dm.S, dm.H, dm.dh, dm.scale) + g for g in dm.layers}
         s |= {("embed_fwd_at", rows, dm.V, dm.d)}
     return s
 
 
 def expected_prefill_calls(dm):
     """The distinct calls complete() adds to its step's for the prefill of generation_calls: one attn_fwd shape per
-    distinct layer radius, at S = P."""
+    distinct layer geometry (radius, axial, conv), at S = P."""
     B2, P, R2 = 2 * REC_B, TEXT_LEN + REC_N, 2 * REC_B * REC_REP
     T = B2 * P
-    return set(step_products(T, dm)[:4]) | {("attn_fwd", B2, P, dm.H, dm.dh, dm.scale, False, r) for r in dm.radii} | {
+    return set(step_products(T, dm)[:4]) | {("attn_fwd", B2, P, dm.H, dm.dh, dm.scale, False) + g for g in dm.layers} | {
         ("layernorm_fwd", T, dm.d), ("embed_fwd", B2, P, False),
         ("kv_cache_fill", T, (R2, dm.S, dm.H, dm.dh), P, REC_REP), ("rows_repeat", (B2, dm.d), P * dm.d, REC_REP)}
 
@@ -239,7 +242,8 @@ def test_generation_call_set(ops, config):
     embed_fwd_at.  complete() adds the prefill: its embedding, LayerNorm, 4 GEMMs and attention at 2 REC_B prompts of
     P = 256 + REC_N, then kv_cache_fill, rows_repeat, the final LayerNorm and the logits GEMM at the step's rows."""
     calls, dm = generation_calls(ops, config)
-    assert dm.radii == (None,)                            # the configurations' samplers run causal attention
+    # the configurations' samplers run causal attention: no window, no axial and no conv geometry
+    assert dm.radii == (None,) and dm.layers == ((None, None, None),)
     assert set(calls["step"]) == expected_step_calls(STEP_ROWS, dm, graphed=False), calls["step"]
     R2 = 2 * REC_B * REC_REP
     assert set(calls["complete"]) == expected_step_calls(R2, dm, graphed=True) | expected_prefill_calls(dm), \

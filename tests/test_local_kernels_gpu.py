@@ -115,7 +115,8 @@ def test_engine_and_sampler_call_set(ops):
     is_att = lambda c: c[0] in ("attn_fwd", "attn_bwd")
     assert {c for c in calls if not is_att(c)} == {c for c in base if not is_att(c)}
     (scale,) = {c[5] for c in base if is_att(c)}
-    want = {("attn_fwd", 1, S, H, dh, scale, False, r), ("attn_bwd", 1, S, H, dh, scale, False, r)}
+    want = {("attn_fwd", 1, S, H, dh, scale, False, r, None, None),
+            ("attn_bwd", 1, S, H, dh, scale, False, r, None, None)}
     assert {c for c in calls if is_att(c)} == want, calls
     dropped = DK.engine_calls(ops, CONFIG, step=6, attention_types=["local"], local_attention_radius=r,
                               dropout=(0.1, 0.1, 0.1), dropout_seed=3)[0]
@@ -124,7 +125,7 @@ def test_engine_and_sampler_call_set(ops):
     print(f"[{TAG}] {CONFIG} one local layer: {len(calls)} distinct calls, attention {sorted(want)}")
 
     gen, dm = DEC.generation_calls(ops, CONFIG, ["global", "local"])
-    assert dm.radii == (None, r)
+    assert dm.radii == (None, r) and dm.layers == ((None, None, None), (r, None, None))
     assert set(gen["step"]) == DEC.expected_step_calls(DEC.STEP_ROWS, dm, graphed=False), gen["step"]
     R2 = 2 * DEC.REC_B * DEC.REC_REP
     assert set(gen["complete"]) == DEC.expected_step_calls(R2, dm, graphed=True) | DEC.expected_prefill_calls(dm), \

@@ -8,6 +8,9 @@ shapes the bench is quoted on, with the batch cut to what the CPU oracle finishe
   * CO   = configs[3] dalle_coco  @ BASELINE geometry: d1024 / H16 (dh64) / S = 1280 / recompute_grad, L cut to 2, B = 1;
   * EXL / COL = EX / CO with local (sliding-window) layers of radius 256: [global, local] x 3 / [global, local],
            against oracle/dalle_local.py under the same criteria;
+  * EXS / COS = EX with the sparse-transformer schedule of configs/dalle_example_conv_b200.json
+           ([axial_row, axial_col] x 2, axial_row, conv at k = 5) / CO with [axial_col, conv], against
+           tests/conv_oracle.py under the same criteria;
   * VC   = configs[2] vae_coco    @ BASELINE geometry: 256 px, convblocks [[2,128],[3,256],[5,512]], K = 8192 (bf16
            activations, fp32-split codebook GEMMs), B = 1;
   * TOK  = the bench's tokenizer config (vae_example_b200: 256 px, K = 512, bf16 tensor-core convolutions): token
@@ -54,8 +57,10 @@ def _randomise_small_params(params, g):
             params[k] = 1 + torch.randn(params[k].shape, generator=g) * 0.05
 
 
-def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed, attention_types=None, radius=256):
-    """attention_types: one "global" / "local" per layer (local layers of `radius`), against oracle/dalle_local.py."""
+def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed, attention_types=None, radius=256, kernel=5):
+    """attention_types: one "global" / "local" per layer (local layers of `radius`), against oracle/dalle_local.py;
+    with an "axial_row", "axial_col" or "conv" layer (conv layers of kernel size `kernel`) against
+    tests/conv_oracle.py."""
     from dalle_mtf_b200.dalle_engine import DalleEngine
     from oracle import dalle as O
     from oracle import dalle_local as OL
@@ -63,6 +68,11 @@ def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed, attention_
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     if attention_types is None:
         cfg, oracle = O.DalleConfig(d, L, H, tv, iv, ts, isl), O
+    elif set(attention_types) & {"axial_row", "axial_col", "conv"}:
+        import conv_oracle as OC
+        cfg = OC.ConvConfig(d, L, H, tv, iv, ts, isl, attention_types=tuple(attention_types),
+                            local_attention_radius=radius, conv_attention_kernel=kernel)
+        oracle = OC
     else:
         cfg = OL.LocalConfig(d, L, H, tv, iv, ts, isl, attention_types=tuple(attention_types),
                              local_attention_radius=radius)
@@ -80,7 +90,7 @@ def _dalle_parity(name, d, L, H, tv, iv, ts, isl, B, recompute, seed, attention_
     _, rows16, logits16, g16 = oracle.loss_and_grads(params, tokens, cfg, bf16=True)
 
     eng = DalleEngine(d, L, H, tv, iv, ts, isl, recompute_grad=recompute, attention_types=attention_types,
-                      local_attention_radius=radius)
+                      local_attention_radius=radius, conv_attention_kernel=kernel)
     eng.load_params(params)
     tok = tokens.to(torch.int32).to(DEV)
     T = tokens.numel()
@@ -152,6 +162,19 @@ def test_dalle_coco_geometry_with_a_local_layer_matches_oracle():
     """COL: the CO geometry (d1024 / H16 / S1280 / recompute_grad, L = 2) with layers [global, local] of radius 256."""
     _dalle_parity("COL d1024 L2 H16 S1280 V50771 B1 recompute global/local r256", 1024, 2, 16, 50258, 512, 256, 1024,
                   1, True, seed=15, attention_types=["global", "local"], radius=256)
+
+
+def test_dalle_example_with_the_sparse_schedule_matches_oracle():
+    """EXS: the EX shape with the layer schedule of configs/dalle_example_conv_b200.json, [axial_row, axial_col] x 2
+    then [axial_row, conv] at k = 5, against tests/conv_oracle.py."""
+    _dalle_parity("EXS d512 L6 H4 S1280 V50771 B2 row/col/row/col/row/conv k5", 512, 6, 4, 50258, 512, 256, 1024, 2,
+                  False, seed=16, attention_types=["axial_row", "axial_col"] * 2 + ["axial_row", "conv"], kernel=5)
+
+
+def test_dalle_coco_geometry_with_axial_and_conv_layers_matches_oracle():
+    """COS: the CO geometry (d1024 / H16 / S1280 / recompute_grad, L = 2) with layers [axial_col, conv] at k = 5."""
+    _dalle_parity("COS d1024 L2 H16 S1280 V50771 B1 recompute col/conv k5", 1024, 2, 16, 50258, 512, 256, 1024, 1,
+                  True, seed=17, attention_types=["axial_col", "conv"], kernel=5)
 
 
 def test_vae_coco_geometry_k8192_bf16_matches_oracle():

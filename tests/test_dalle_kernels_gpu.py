@@ -389,8 +389,9 @@ def test_gemm_products_of_the_engine(ops, config):
 
 
 # ------------------------------------------------------------------------------------------------------- cross-entropy
-def run_cross_entropy(ops, tag, T, K, V, Vpad, *, labels, h, W, bias, n_valid=None, alpha=None, colsum=True):
-    """CE_STATS -> ce_finish -> CE_GRAD as the engine runs them, checked per element in row slabs."""
+def run_cross_entropy(ops, tag, T, K, V, Vpad, *, labels, h, W, bias, n_valid=None, alpha=None, colsum=True, dl=None):
+    """CE_STATS -> ce_finish -> CE_GRAD as the engine runs them, checked per element in row slabs.  dl: the NaN-filled
+    [T, Vpad] bf16 gradient to write (default: a fresh one), for callers that read it afterwards."""
     from dalle_mtf_b200 import lib as L
     n_valid = V if n_valid is None else n_valid
     alpha = 1.0 / T if alpha is None else alpha
@@ -403,7 +404,7 @@ def run_cross_entropy(ops, tag, T, K, V, Vpad, *, labels, h, W, bias, n_valid=No
              part_max=pm, part_sum=ps, label_logit=ll, n_valid=n_valid)
     ops.ce_finish(pm, ps, ll, lse, lr, lsum)
     del pm, ps
-    dl = nan_like((T, Vpad), BF16)
+    dl = nan_like((T, Vpad), BF16) if dl is None else dl
     cs_base = torch.randn(Vpad, generator=_gen(T + Vpad), device=DEV) * 1e-3 if colsum else None
     cs = cs_base.clone() if colsum else None
     ops.gemm(h, W, dl, T, Vpad, K, a_mn=False, b_mn=True, mode=L.EPI_CE_GRAD, alpha=alpha, bias=bias, labels=labels,
@@ -492,6 +493,13 @@ def test_cross_entropy_at_the_real_vocabulary(ops, config):
 
 def real_vocabulary_cross_entropy(ops, config, T):
     """run_cross_entropy at the configuration's V / Vpad / width with T rows (see the test above)."""
+    K, V, Vpad, h, W, bias, labels = real_vocabulary_operands(ops, config, T)
+    return run_cross_entropy(ops, f"{config} CE T={T} V={V}", T, K, V, Vpad, labels=labels, h=h, W=W, bias=bias)
+
+
+def real_vocabulary_operands(ops, config, T):
+    """(K, V, Vpad, h, W, bias, labels) of the vocabulary head of `config` with T rows: ce_operands with dominating
+    logits at the edge columns, labels of the engine's shift_labels with edge columns on every 101st row."""
     cfg = _config(config)
     calls, _, V, Vpad, S = engine_calls(ops, config)
     assert any(c[0] == "gemm" and c[13] == V for c in calls)          # the engine's n_valid is V
@@ -510,8 +518,7 @@ def real_vocabulary_cross_entropy(ops, config, T):
     rows = torch.arange(7, T, 101, device=DEV)
     labels[rows] = torch.tensor(edge, dtype=I32, device=DEV)[torch.arange(rows.numel(), device=DEV) % len(edge)]
     labels[sel_rows] = torch.tensor(cols, dtype=I32, device=DEV)[torch.arange(sel_rows.numel(), device=DEV) % len(cols)]
-    return run_cross_entropy(ops, f"{config} CE T={T} V={V}", T, K, V, Vpad, labels=labels.contiguous(), h=h, W=W,
-                             bias=bias)
+    return K, V, Vpad, h, W, bias, labels.contiguous()
 
 
 @pytest.mark.parametrize("n_valid", [130, 1, 200])
@@ -881,26 +888,43 @@ def fixed_point_runs(ids, V):
     return torch.bincount(flat[start], minlength=V)
 
 
-def run_embedding(ops, tag, ids, V, d, dx_scale, g):
+def run_embedding(ops, tag, ids, V, d, dx_scale, g, wte_drop=None, wpe_drop=None):
+    """embed_fwd / embed_bwd against float64.  With the dropout descriptors (both or neither) every term carries its
+    keep mask * scale: the forward is then a bound (one fp32 rounding per product and one for the sum, then bf16)
+    instead of bit for bit, and the backward adds one rounding per masked gradient element (+ U)."""
+    from dalle_mtf_b200 import lib as L
     B, S = ids.shape
     wte = _randn(V, d, g=g, scale=0.02, dtype=BF16)
     wpe = _randn(S, d, g=g, scale=0.01, dtype=BF16)
+    mt = mp = None
+    if wte_drop is not None:
+        mt = torch.empty(B * S, d, dtype=torch.uint8, device=DEV)
+        ops.dropout_mask(wte_drop, L.DROPOUT_ELEMENTWISE, (B * S, d), mt)
+        mp = torch.empty(S, d, dtype=torch.uint8, device=DEV)
+        ops.dropout_mask(wpe_drop, L.DROPOUT_ELEMENTWISE, (S, d), mp)
+        mt = mt.view(B, S, d).to(F64) * _f32(wte_drop.scale)
+        mp = mp.to(F64) * _f32(wpe_drop.scale)
     out = nan_like((B, S, d), BF16)
-    ops.embed_fwd(ids, wte, wpe, out)
-    for b0 in range(0, B, 8):
-        ref = wte.to(F64)[ids[b0:b0 + 8].long()] + wpe.to(F64)[None]
-        assert torch.equal(out[b0:b0 + 8].view(torch.int16), bf16_rne(ref).view(torch.int16)), f"{tag} forward"
-    print(f"{float64_bounds.prefix()}[{TAG}] {tag} embed_fwd: bf16 RNE of the exact sum, bit for bit "
-          "(worst err/bound 0)")
+    ops.embed_fwd(ids, wte, wpe, out, wte_drop=wte_drop, wpe_drop=wpe_drop)
+    if mt is None:
+        for b0 in range(0, B, 8):
+            ref = wte.to(F64)[ids[b0:b0 + 8].long()] + wpe.to(F64)[None]
+            assert torch.equal(out[b0:b0 + 8].view(torch.int16), bf16_rne(ref).view(torch.int16)), f"{tag} forward"
+        print(f"{float64_bounds.prefix()}[{TAG}] {tag} embed_fwd: bf16 RNE of the exact sum, bit for bit "
+              "(worst err/bound 0)")
+    else:
+        a, p = wte.to(F64)[ids.long()] * mt, wpe.to(F64)[None] * mp[None]
+        check(f"{tag} embed_fwd", out, a + p, a.abs() + p.abs(), b=2 * U, bf16_out=True)
     dx = _randn(B, S, d, g=g, scale=dx_scale, dtype=BF16)
     base_t = _randn(V, d, g=g, scale=dx_scale)
     base_p = _randn(S, d, g=g, scale=dx_scale)
     dwte, dwpe = base_t.clone(), base_p.clone()
-    ops.embed_bwd(ids, dx, dwte, dwpe)
+    ops.embed_bwd(ids, dx, dwte, dwpe, wte_drop=wte_drop, wpe_drop=wpe_drop)
     flat = ids.reshape(-1).long()
-    dx2 = dx.reshape(-1, d).to(F64)
+    dx2 = (dx.to(F64) * (1.0 if mt is None else mt)).reshape(-1, d)
     runs = fixed_point_runs(ids, V).to(F64)
     share = torch.zeros(V, dtype=F64, device=DEV)        # the fixed-point term's share of the bound, per row
+    b_run = (31 if mt is None else 32) * U
     w = Worst(f"{tag} dwte")
     for v0, v1 in _slabs(V, d):
         sel = (flat >= v0) & (flat < v1)
@@ -908,8 +932,8 @@ def run_embedding(ops, tag, ids, V, d, dx_scale, g):
         ref = base_t[v0:v1].to(F64).index_add_(0, idx, rows)
         absref = base_t[v0:v1].abs().to(F64).index_add_(0, idx, rows.abs())
         fixed = runs[v0:v1, None] * 2.0 ** -41
-        w.add(dwte[v0:v1], ref, absref, a=2 * U, b=31 * U, floor=fixed)
-        fp32 = (31 * U * absref + 2 * U * ref.abs()).mean(1)
+        w.add(dwte[v0:v1], ref, absref, a=2 * U, b=b_run, floor=fixed)
+        fp32 = (b_run * absref + 2 * U * ref.abs()).mean(1)
         share[v0:v1] = fixed[:, 0] / (fixed[:, 0] + fp32).clamp_min(1e-300)
         del ref, absref, rows
     r = w.report()
@@ -919,9 +943,9 @@ def run_embedding(ops, tag, ids, V, d, dx_scale, g):
           f"the padding row ({int(runs[pad])} runs, {int((flat == pad).sum())} tokens), "
           f"median {share[touched].median().item():.4f}, max {share.max().item():.4f} over the {int(touched.sum())} "
           "rows hit")
-    dref = base_p.to(F64) + dx.to(F64).sum(0)
-    dabs = base_p.abs().to(F64) + dx.to(F64).abs().sum(0)
-    r = max(r, check(f"{tag} dwpe", dwpe, dref, dabs, a=2 * U, b=(B + 2) * U))
+    dref = base_p.to(F64) + dx.to(F64).sum(0) * (1.0 if mp is None else mp)
+    dabs = base_p.abs().to(F64) + dx.to(F64).abs().sum(0) * (1.0 if mp is None else mp)
+    r = max(r, check(f"{tag} dwpe", dwpe, dref, dabs, a=2 * U, b=(B + 2 + (mp is not None)) * U))
     return r
 
 

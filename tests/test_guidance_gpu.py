@@ -44,6 +44,13 @@ def first_argmax(x, mask):
 @pytest.mark.parametrize("rows,n", [(1, 512), (32, 512), (130, 512), (1, 8192), (32, 8192), (130, 8192),
                                     (1, 32768), (32, 32768), (130, 32768)])
 def test_guided_draws_match_the_float32_oracle(ops, rows, n):
+    check_guided_rows(ops, rows, n)
+
+
+def check_guided_rows(ops, rows, n):
+    """sample_rows_guided over n ids at lo = 7 of rows pairs with ld = lo + n + 5, for every guidance scale, two
+    temperatures and the filters: greedy draws are the oracle's first maximum of the kept set, kept counts equal the
+    oracle's, noisy draws the first Gumbel-max, both rows of a pair get the draw and no other column is written."""
     g = torch.Generator(device=DEV).manual_seed(rows * 13 + n)
     lo = 7
     hi, ld = lo + n, lo + n + 5

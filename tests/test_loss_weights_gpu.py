@@ -37,9 +37,10 @@ def ops():
 
 
 def run_weighted_ce(ops, tag, T, K, V, Vpad, S, TL, *, labels, h, W, bias, weights, z, global_batch=None,
-                    mutants=()):
+                    mutants=(), dl=None):
     """CE_STATS -> ce_finish_weighted -> weighted CE_GRAD, checked per element in row slabs; returns the worst
-    err/bound.  mutants: oracle.loss_weights LossQuirks whose dlogits must exceed the bound somewhere."""
+    err/bound.  mutants: oracle.loss_weights LossQuirks whose dlogits must exceed the bound somewhere.  dl: the
+    NaN-filled [T, Vpad] bf16 gradient to write (default: a fresh one)."""
     from dalle_mtf_b200 import lib as L
     from oracle import loss_weights as OW
     IL = S - TL
@@ -55,7 +56,7 @@ def run_weighted_ce(ops, tag, T, K, V, Vpad, S, TL, *, labels, h, W, bias, weigh
              part_max=pm, part_sum=ps, label_logit=ll, n_valid=V)
     ops.ce_finish_weighted(pm, ps, ll, lse, lr, sums, cew)
     del pm, ps
-    dl = nan_like((T, Vpad), BF16)
+    dl = nan_like((T, Vpad), BF16) if dl is None else dl
     cs_base = torch.randn(Vpad, generator=_gen(T + Vpad), device=DEV) * 1e-3
     cs = cs_base.clone()
     ops.gemm(h, W, dl, T, Vpad, K, a_mn=False, b_mn=True, mode=L.EPI_CE_GRAD, bias=bias, labels=labels, lse=lse,

@@ -51,6 +51,13 @@ def check_selection(idx, lo, mask, pert, rows_ok):
 @pytest.mark.parametrize("rows,n", [(1, 512), (32, 512), (130, 512), (1, 8192), (32, 8192), (130, 8192),
                                     (1, 32768), (32, 32768), (130, 32768)])
 def test_kept_set_and_selection_match_the_float64_oracle(ops, rows, n):
+    check_filtered_rows(ops, rows, n)
+
+
+def check_filtered_rows(ops, rows, n):
+    """sample_rows_filtered over n ids at lo = 5 of rows with ld = lo + n + 3, at three temperatures and a grid of
+    top_k / top_p: the kept counts equal the oracle's and every draw is the first Gumbel-max of the kept set, except on
+    rows whose top-p decision lies within MARGIN of a tie (at most a quarter of them)."""
     g = torch.Generator(device=DEV).manual_seed(rows * 7 + n)
     lo = 5
     hi, ld = lo + n, lo + n + 3

@@ -1,8 +1,11 @@
-// K13 — Gumbel-softmax (soft / hard straight-through), row argmax with the first-maximum tie rule, MSE loss.
+// K13 — Gumbel-softmax (soft / hard straight-through), row argmax with the first-maximum tie rule, MSE loss, and the
+// optional KL(q || Uniform(K)) term with its codebook-usage histogram.
 // fp32 row kernels, one warp per row, warp-shuffle reductions; HBM-bound (the [rows][K] tensors are read/written once
 // or twice).
 //
 // Reference: gumbel_softmax src/vae_tf/layers.py:4-21, mse_loss :24-25, tf.math.argmax src/model_fns.py:76.
+#include <cfloat>
+
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -70,9 +73,13 @@ gumbel_softmax_fwd_kernel(const float* __restrict__ logits, const float* __restr
   if (idx_out && lane == 0) idx_out[row] = mi;
 }
 
+// KL = false: the straight-through Gumbel-softmax backward.  KL = true adds the gradient of c * KL(q || Uniform(K)),
+// q = softmax(logits), in the same store: c q (l - lse - ent), with lse / ent of the row from vae_kl_stats_kernel.
+template <bool KL>
 __global__ void __launch_bounds__(128)
 gumbel_softmax_bwd_kernel(const float* __restrict__ y_soft, const float* __restrict__ dy, float* __restrict__ dlogits,
-                          int rows, int K, float inv_tau) {
+                          int rows, int K, float inv_tau, const float* __restrict__ logits,
+                          const float* __restrict__ lse, const float* __restrict__ ent, float c) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (row >= rows) return;
@@ -82,7 +89,123 @@ gumbel_softmax_bwd_kernel(const float* __restrict__ y_soft, const float* __restr
   for (int k = lane; k < K; k += 32) dot += y[k] * d[k];
   dot = warp_sum(dot);
   float* o = dlogits + (long long)row * K;
-  for (int k = lane; k < K; k += 32) o[k] = y[k] * (d[k] - dot) * inv_tau;
+  if (KL) {
+    const float* lr = logits + (long long)row * K;
+    const float ls = lse[row], en = ent[row];
+    for (int k = lane; k < K; k += 32) {
+      const float z = lr[k] - ls;              // log q, formed from the logit: q = 0 still gives a finite factor
+      o[k] = y[k] * (d[k] - dot) * inv_tau + c * expf(z) * (fmaxf(z, -FLT_MAX) - en);
+    }
+  } else {
+    for (int k = lane; k < K; k += 32) o[k] = y[k] * (d[k] - dot) * inv_tau;
+  }
+}
+
+// ---- KL(q || Uniform(K)) statistics of the encoder logits (the KL term of the DALL-E paper's ELB; the reference has
+// none).  One warp per row, KL_WARPS rows in flight per CTA, CTAs striding over the rows.  A single pass keeps, per lane,
+// the running maximum m, s = sum exp(l - m) and t = sum exp(l - m) (l - m), rescaled whenever m grows; then
+//   lse = m + log s,   ent = sum q (l - lse) = t / s - log s,   KL_r = ent + log K = t / s - log(s / K)
+// (the last form does not cancel log K against ent's -log K for near-uniform rows).  No log q is ever taken, so a q
+// that underflows to 0 contributes exactly 0.
+constexpr int KL_WARPS = 8;
+constexpr int KL_SMEM_HIST_MAX_K = 12000;     // K * 4 bytes + red[] within the 48 KB a CTA gets without an opt-in
+
+// (s, t) taken from maximum m to maximum mn >= m.  d is clamped so that an empty set (s = t = 0) stays 0, not 0 * -inf.
+__device__ __forceinline__ void kl_rescale(float& s, float& t, float m, float mn) {
+  const float a = expf(m - mn);
+  t = a * fmaf(fmaxf(m - mn, -FLT_MAX), s, t);
+  s = a * s;
+}
+
+// one logit l at index k into a lane's running (m, s, t), first maximum mi and NaN flag
+__device__ __forceinline__ void kl_visit(float l, int k, float& m, float& s, float& t, int& mi, bool& nan) {
+  nan |= l != l;
+  if (l > m) {
+    kl_rescale(s, t, m, l);
+    s += 1.f;        // the new maximum itself: exp(0) = 1, (l - m) = 0
+    m = l;
+    mi = k;
+  } else if (l != -INFINITY) {   // -inf has q = 0 and adds nothing; NaN falls through here and poisons s
+    const float z = l - m;
+    const float p = expf(z);
+    s += p;
+    t = fmaf(p, z, t);
+  }
+}
+
+// VEC4 (K % 4 == 0, 16-byte aligned logits): a lane reads 4 consecutive logits per load, so a warp keeps four times the
+// bytes in flight; a lane still visits its indices in increasing order, which keeps the first-maximum rule.
+template <bool SMEM_HIST, bool VEC4>
+__global__ void __launch_bounds__(KL_WARPS * 32)
+vae_kl_stats_kernel(const float* __restrict__ logits, float* __restrict__ lse, float* __restrict__ ent,
+                    int* __restrict__ hist, float* __restrict__ partials, int rows, int K, float Kf, float scale) {
+  extern __shared__ int sh_hist[];
+  __shared__ float red[KL_WARPS];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int* h = hist;
+  if (SMEM_HIST) {
+    for (int k = threadIdx.x; k < K; k += blockDim.x) sh_hist[k] = 0;
+    __syncthreads();
+    h = sh_hist;
+  }
+  float kl_sum = 0.f;   // this warp's rows, in row order
+  for (long long row = blockIdx.x * KL_WARPS + warp; row < rows; row += (long long)gridDim.x * KL_WARPS) {
+    const float* lr = logits + (long long)row * K;
+    float m = -INFINITY, s = 0.f, t = 0.f;
+    int mi = 0;          // first index of the maximum (argmax_rows' rule); stays 0 for a row of -inf
+    bool nan = false;
+    if (VEC4) {
+      const float4* lr4 = reinterpret_cast<const float4*>(lr);
+#pragma unroll 2
+      for (int j = lane; j < (K >> 2); j += 32) {
+        const float4 v = lr4[j];
+        kl_visit(v.x, 4 * j, m, s, t, mi, nan);
+        kl_visit(v.y, 4 * j + 1, m, s, t, mi, nan);
+        kl_visit(v.z, 4 * j + 2, m, s, t, mi, nan);
+        kl_visit(v.w, 4 * j + 3, m, s, t, mi, nan);
+      }
+    } else {
+#pragma unroll 4
+      for (int k = lane; k < K; k += 32) kl_visit(lr[k], k, m, s, t, mi, nan);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float om = __shfl_xor_sync(0xffffffffu, m, o);
+      const float os = __shfl_xor_sync(0xffffffffu, s, o);
+      const float ot = __shfl_xor_sync(0xffffffffu, t, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
+      const float mn = fmaxf(m, om);
+      if (mn != -INFINITY) {   // else both halves hold only -inf logits (or none): s = t = 0 on both
+        float s2 = os, t2 = ot;
+        kl_rescale(s, t, m, mn);
+        kl_rescale(s2, t2, om, mn);
+        s += s2;
+        t += t2;
+      }
+      if (om > m || (om == m && oi < mi)) mi = oi;
+      m = mn;
+    }
+    nan = __any_sync(0xffffffffu, nan);
+    const float ls = logf(s);
+    const float ts = t / s;
+    kl_sum += ts - logf(s / Kf);
+    if (lane == 0) {
+      lse[row] = m + ls;
+      ent[row] = ts - ls;
+      atomicAdd(&h[nan ? 0 : mi], 1);   // integer counts: exact in any order
+    }
+  }
+  if (lane == 0) red[warp] = kl_sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float v = 0.f;
+#pragma unroll
+    for (int w = 0; w < KL_WARPS; ++w) v += red[w];
+    partials[blockIdx.x] = v * scale;   // per-CTA partial, summed in CTA order by the launcher
+  }
+  if (SMEM_HIST)
+    for (int k = threadIdx.x; k < K; k += blockDim.x)
+      if (sh_hist[k]) atomicAdd(&hist[k], sh_hist[k]);
 }
 
 __global__ void __launch_bounds__(128)
@@ -170,8 +293,58 @@ extern "C" int db200_gumbel_softmax_bwd(db200_stream_t stream_, const float* y_s
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(y_soft && dy && dlogits && rows > 0 && K > 0 && tau > 0.f, DB200_E_INVALID,
                 "gumbel_softmax_bwd: bad arguments");
-  gumbel_softmax_bwd_kernel<<<(rows + 3) / 4, 128, 0, stream>>>(y_soft, dy, dlogits, rows, K, 1.f / tau);
+  gumbel_softmax_bwd_kernel<false><<<(rows + 3) / 4, 128, 0, stream>>>(y_soft, dy, dlogits, rows, K, 1.f / tau,
+                                                                       nullptr, nullptr, nullptr, 0.f);
   return check_launch("gumbel_softmax_bwd_kernel");
+}
+
+extern "C" int db200_gumbel_softmax_bwd_kl(db200_stream_t stream_, const float* y_soft, const float* dy,
+                                           const float* logits, const float* lse, const float* ent, float* dlogits,
+                                           int rows, int K, float tau, float c) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(y_soft && dy && logits && lse && ent && dlogits && rows > 0 && K > 0 && tau > 0.f && isfinite(c),
+                DB200_E_INVALID, "gumbel_softmax_bwd_kl: bad arguments");
+  gumbel_softmax_bwd_kernel<true><<<(rows + 3) / 4, 128, 0, stream>>>(y_soft, dy, dlogits, rows, K, 1.f / tau, logits,
+                                                                      lse, ent, c);
+  return check_launch("gumbel_softmax_bwd_kernel<KL>");
+}
+
+// One wave: as many CTAs as fit on the device at once (the shared histogram bounds it), each striding over the rows;
+// a second, part-empty wave would leave most SMs idle while it runs.
+static int kl_stats_blocks(int rows, int K) {
+  int per_sm = 1;   // the four instantiations use the same resources but for the shared histogram
+  if (K <= KL_SMEM_HIST_MAX_K)
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vae_kl_stats_kernel<true, true>, KL_WARPS * 32,
+                                                  (size_t)K * sizeof(int));
+  else
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vae_kl_stats_kernel<false, true>, KL_WARPS * 32, 0);
+  const long long need = ((long long)rows + KL_WARPS - 1) / KL_WARPS;
+  const long long cap = (long long)sm_count() * (per_sm > 0 ? per_sm : 1);
+  return (int)(need < cap ? need : cap);
+}
+
+extern "C" int64_t db200_vae_kl_stats_workspace_bytes(int rows, int K) {
+  return rows > 0 && K > 0 ? (int64_t)kl_stats_blocks(rows, K) * (int64_t)sizeof(float) : 0;
+}
+
+extern "C" int db200_vae_kl_stats(db200_stream_t stream_, const float* logits, float* lse, float* ent, int32_t* hist,
+                                  float* kl_accum, int rows, int K, float scale, void* workspace,
+                                  int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(logits && lse && ent && hist && kl_accum && rows > 0 && K > 0 && isfinite(scale), DB200_E_INVALID,
+                "vae_kl_stats: bad arguments");
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_vae_kl_stats_workspace_bytes(rows, K)),
+                DB200_E_INVALID, "vae_kl_stats: needs an aligned workspace of db200_vae_kl_stats_workspace_bytes() bytes");
+  const int blocks = kl_stats_blocks(rows, K);
+  float* ws = static_cast<float*>(workspace);
+  const bool vec4 = K % 4 == 0 && aligned16(logits);
+  const size_t smem = K <= KL_SMEM_HIST_MAX_K ? (size_t)K * sizeof(int) : 0;
+  auto kernel = K <= KL_SMEM_HIST_MAX_K ? (vec4 ? vae_kl_stats_kernel<true, true> : vae_kl_stats_kernel<true, false>)
+                                        : (vec4 ? vae_kl_stats_kernel<false, true> : vae_kl_stats_kernel<false, false>);
+  kernel<<<blocks, KL_WARPS * 32, smem, stream>>>(logits, lse, ent, hist, ws, rows, K, (float)K, scale);
+  const int rc = check_launch("vae_kl_stats_kernel");
+  if (rc != DB200_OK) return rc;
+  return reduce_rows_add(stream, ws, blocks, 1, kl_accum);
 }
 
 extern "C" int db200_argmax_rows_f32(db200_stream_t stream_, const float* x, int32_t* idx, int rows, int K) {

@@ -4,7 +4,7 @@ train_vae_tf.py:51-93): build once via model_fn, restore the latest checkpoint, 
 """
 import time
 
-from .model_fns import EVAL, TRAIN
+from .model_fns import DALLE_PARTS_FORMAT, EVAL, TRAIN
 from .utils import (latest_checkpoint, load_checkpoint, load_global_step_from_checkpoint_dir, save_checkpoint)
 
 
@@ -77,7 +77,11 @@ class Estimator:
                 loss = float(spec.loss_sum.item()) * spec.loss_scale      # the only host sync
                 parts = getattr(spec, "loss_parts", None)
                 parts = "" if parts is None else \
-                    " text_ce {:.5f} image_ce {:.5f} z_term {:.3g}".format(*parts.tolist())
+                    getattr(spec, "loss_parts_format", DALLE_PARTS_FORMAT).format(*parts.tolist())
+                usage = getattr(spec, "codebook_usage", None)
+                if usage is not None:   # a collective: every rank runs this branch
+                    codes_used, perplexity = usage()
+                    parts += f" codes_used {codes_used} perplexity {perplexity:.2f}"
                 dt = time.time() - t0
                 if spec.dp.rank == 0:
                     self._log(f"step {spec.global_step} loss {loss:.5f}{parts} "

@@ -7,6 +7,9 @@ ONCE (like the Estimator's graph build) and ``spec.train_op(features, labels)`` 
 batch (host or device tensors), returning the device scalar with the global-mean loss.  One process per GPU: each
 rank passes ITS shard of the global batch (rows rank*B/N..., the reference's "batch_dim:data" layout).
 """
+import math
+import numbers
+
 import torch
 
 from . import lib as L
@@ -15,7 +18,7 @@ from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_conv_kernel, va
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
-from .vae_engine import VaeEngine
+from .vae_engine import VaeEngine, codebook_usage
 
 TRAIN, EVAL, PREDICT = "train", "eval", "predict"   # tf.estimator.ModeKeys values
 
@@ -41,7 +44,14 @@ class StepSpec:
         self.global_step = 0
         self.extra = extra or {}
         self.loss = None              # device scalar of the last step (read it only when logging: it syncs)
-        self.loss_parts = None        # weighted loss: device [3] = text-row mean CE, image-row mean CE, mean z-term
+        self.loss_parts = None        # weighted loss: device [3] = text-row mean CE, image-row mean CE, mean z-term;
+                                      # VAE with KL: device [2] = reconstruction MSE, KL (global means)
+        self.loss_parts_format = DALLE_PARTS_FORMAT   # how a training log line shows loss_parts
+        self.codebook_usage = None    # VAE with KL: () -> (codes_used, perplexity) of the last batch (a collective)
+
+
+DALLE_PARTS_FORMAT = " text_ce {:.5f} image_ce {:.5f} z_term {:.3g}"
+VAE_PARTS_FORMAT = " recon_mse {:.5f} kl {:.5f}"
 
 
 def _to_device(t, dtype, device):
@@ -342,11 +352,48 @@ def vae_temperature(step, params):
     return 1.0 if t is None else t
 
 
+def validate_kl_weight(beta, anneal_steps=None):
+    """(beta, anneal_steps) of the VAE's KL term, or (None, None) without one.  beta: a finite real >= 0 (not a bool);
+    anneal_steps: None or an integer >= 1 (not a bool), only together with beta."""
+    if beta is None:
+        if anneal_steps is not None:
+            raise ValueError(f"kl_anneal_steps = {anneal_steps!r} without kl_loss_weight has no effect")
+        return None, None
+    if isinstance(beta, bool) or not isinstance(beta, numbers.Real) or not math.isfinite(beta) or beta < 0:
+        raise ValueError(f"kl_loss_weight = {beta!r}: must be a finite real >= 0")
+    if anneal_steps is not None and (isinstance(anneal_steps, bool) or not isinstance(anneal_steps, numbers.Integral)
+                                     or anneal_steps < 1):
+        raise ValueError(f"kl_anneal_steps = {anneal_steps!r}: must be an integer >= 1")
+    return float(beta), None if anneal_steps is None else int(anneal_steps)
+
+
+def kl_loss_weight(params):
+    """(beta, anneal_steps) of a VAE config's extension keys kl_loss_weight / kl_anneal_steps (validate_kl_weight).
+    The objective is then MSE + beta_t * KL, KL the mean over the latent rows of the global batch of
+    KL(softmax(logits) || Uniform(K)), beta_t = vae_kl_weight(step, params)."""
+    return validate_kl_weight(params.get("kl_loss_weight"), params.get("kl_anneal_steps"))
+
+
+def vae_kl_weight(step, params):
+    """beta_t of the KL term at global step `step`: beta * min(step / kl_anneal_steps, 1), or beta without the anneal
+    key (None without kl_loss_weight).  A function of the step alone, so a resumed run continues the schedule."""
+    beta, anneal = kl_loss_weight(params)
+    if beta is None:
+        return None
+    return beta * min(step / anneal, 1.0) if anneal else beta
+
+
 def vae_model_fn(features, labels, mode, params):
-    """src/model_fns_tf.py:9-114.  features = labels = images f32 [B,H,W,C] in [-1,1]."""
+    """src/model_fns_tf.py:9-114.  features = labels = images f32 [B,H,W,C] in [-1,1].
+
+    With the extension key kl_loss_weight (and optionally kl_anneal_steps), spec.loss_sum * spec.loss_scale is the
+    objective MSE + beta_t * KL, spec.loss_parts the device [2] (MSE, KL) of the global batch and
+    spec.codebook_usage() the (codes_used, perplexity) of its first-maximum codes."""
     mode_str = mode_to_str(mode)
     if mode == PREDICT:
         raise NotImplementedError                                             # model_fns_tf.py:29-30
+    kl_beta, _ = kl_loss_weight(params)
+    kl_on = kl_beta is not None
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -357,7 +404,7 @@ def vae_model_fn(features, labels, mode, params):
                       convblocks=params.get("convblocks") or [(3, 64), (3, 128), (3, 256)],
                       input_channels=params.get("input_channels") or 3,
                       recompute_grad=bool(params.get("recompute_grad")), use_bf16=bool(params.get("use_bf16")),
-                      stack_factor=params.get("stack_factor") or 1, device=device)
+                      stack_factor=params.get("stack_factor") or 1, device=device, kl=kl_on)
     model.init_params(seed=params.get("seed") or 0)
     if dp.rank == 0:
         print_n_params(model.n_params())
@@ -383,11 +430,27 @@ def vae_model_fn(features, labels, mode, params):
     def run(features, train):
         img = _to_device(features, torch.float32, device).view(local_batch, H, H, model.img_C)
         temp = vae_temperature(spec.global_step, params)
+        spec.kl_weight = vae_kl_weight(spec.global_step, params)
         u = params.get("_gumbel_u")
         u = draw_noise() if u is None else u
         model.zero_grads()
-        recon = model.forward(img, u, temp, hard)       # adds sum((img-out)^2)/local_numel into the aux slot
+        # adds sum((img-out)^2)/local_numel into aux slot 0 and, with the KL term, the local mean KL into slot 1
+        recon = model.forward(img, u, temp, hard, kl_weight=spec.kl_weight)
         return recon
+
+    def report(sums):
+        # sums: the all-reduced aux slots [MSE, KL], each the SUM over ranks of the local means
+        if kl_on:
+            spec.loss_parts = sums[:2] * (1.0 / dp.world)
+            spec.loss_sum, spec.loss_scale = sums[:1] + spec.kl_weight * sums[1:2], 1.0 / dp.world
+        else:
+            spec.loss_sum, spec.loss_scale = sums[:1], 1.0 / dp.world
+
+    def usage():
+        # code counts of the global batch: one all-reduce, only when asked (every rank must ask)
+        counts = model.code_counts().to(torch.float32)
+        dp.all_reduce_now(counts)
+        return codebook_usage(counts)
 
     def train_op(features, labels=None):
         run(features, True)
@@ -398,16 +461,16 @@ def vae_model_fn(features, labels, mode, params):
         dp.wait()
         spec.global_step += 1
         model.optimizer_step(params["lr"], spec.global_step, grad_scale=1.0 / dp.world)   # model_fns_tf.py:58-60
-        spec.loss_sum = model.grads[model.aux_off:model.aux_off + 1]
-        spec.loss_scale = 1.0 / dp.world    # each rank's aux slot holds its local mean; the SUM over ranks / N
+        # each rank's aux slots hold its local means, all-reduced with the decoder bucket; the SUM over ranks / N
+        report(model.grads[model.aux_off:model.aux_off + 2])
         return spec.loss_sum
 
     def eval_op(features, labels=None):
         run(features, False)
-        acc = model.grads[model.aux_off:model.aux_off + 1].clone()
+        acc = model.grads[model.aux_off:model.aux_off + (2 if kl_on else 1)].clone()
         dp.all_reduce_now(acc)
-        spec.loss_sum, spec.loss_scale = acc, 1.0 / dp.world
-        return acc
+        report(acc)
+        return spec.loss_sum
 
     def state_fn():
         st = {"vae/" + k: v for k, v in model.export_params().items()}
@@ -430,4 +493,8 @@ def vae_model_fn(features, labels, mode, params):
     spec.state_fn, spec.load_fn = state_fn, load_fn
     spec.images_per_step = global_batch
     spec.n_global = n_global
+    spec.kl_weight = None
+    if kl_on:
+        spec.loss_parts_format = VAE_PARTS_FORMAT
+        spec.codebook_usage = usage
     return spec

@@ -6,7 +6,7 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
-from .model_fns import attention_layers, conv_kernel, dropout_rates, loss_weights
+from .model_fns import attention_layers, conv_kernel, dropout_rates, loss_weights, validate_kl_weight
 from .vae_engine import VaeEngine
 
 
@@ -100,14 +100,19 @@ class DALLE:
 
 class DiscreteVAE:
     def __init__(self, num_tokens, dimensions, convblocks, dim=512, hidden_dim=64, input_channels=3,
-                 recompute_grad=False, use_bf16=False, stack_factor=1):
+                 recompute_grad=False, use_bf16=False, stack_factor=1, kl_loss_weight=None):
+        """kl_loss_weight (extension; None: the reference's objective): beta of the KL term, a finite real >= 0.  With
+        it, forward(..., return_recon_loss=True) returns MSE + beta * KL, KL the mean over the batch's latent rows of
+        KL(softmax(logits) || Uniform(K)), and leaves the device [2] (MSE, KL) in self.loss_parts."""
+        self.kl_loss_weight, _ = validate_kl_weight(kl_loss_weight)
+        self.loss_parts = None
         self.num_tokens, self.dim, self.hdim = num_tokens, dim, hidden_dim   # dim / hidden_dim have no effect (ref too)
         self.H = self.W = dimensions
         self.convblocks = convblocks
         self.num_ch = input_channels
         self.stack_factor = stack_factor
         self.engine = VaeEngine(num_tokens, dimensions, convblocks, input_channels, use_bf16, recompute_grad,
-                                stack_factor)
+                                stack_factor, kl=self.kl_loss_weight is not None)
         self.engine.init_params(0)
         self._gen = torch.Generator(device=self.engine.device).manual_seed(1234)
 
@@ -120,10 +125,15 @@ class DiscreteVAE:
             return e.encode_logits(img).view(B, e.hw, e.hw, e.K)
         rows = img.shape[0] * e.hw * e.hw
         u = torch.empty(rows, e.K, dtype=torch.float32, device=e.device).uniform_(1e-9, 1.0, generator=self._gen)
-        acc = torch.zeros(1, dtype=torch.float32, device=e.device)
-        out = e.forward(img, u, temperature, hard_gumbel, loss_accum=acc)
+        kl = self.kl_loss_weight is not None
+        acc = torch.zeros(2 if kl else 1, dtype=torch.float32, device=e.device)
+        out = e.forward(img, u, temperature, hard_gumbel, loss_accum=acc[:1], kl_weight=self.kl_loss_weight,
+                        kl_accum=acc[1:] if kl else None)
         if not return_recon_loss:
             return out
+        if kl:                     # scalar glue: the objective from the two device sums
+            self.loss_parts = acc
+            return acc[:1] + self.kl_loss_weight * acc[1:], out
         return acc, out
 
     def decode(self, image_token_ids, offset=0):

@@ -591,6 +591,26 @@ def argmax_rows(x, idx, rows, K):
     check(L.load().db200_argmax_rows_f32(stream_ptr(), ptr(x), ptr(idx), rows, K), "argmax_rows")
 
 
+def vae_kl_stats(logits, lse, ent, hist, kl_accum, rows, K, scale):
+    """KL(softmax(l) || Uniform(K)) statistics of f32 logits [rows, K]: lse / ent f32 [rows] (logsumexp, sum q (l - lse)),
+    hist int32 [K] += the first-maximum code counts, kl_accum[0] += scale * sum of the rows' KL."""
+    L.require_device()
+    _chk(logits, F32, "logits"); _chk(lse, F32, "lse"); _chk(ent, F32, "ent"); _chk(hist, I32, "hist")
+    _chk(kl_accum, F32, "kl_accum")
+    if logits.numel() < rows * K or lse.numel() < rows or ent.numel() < rows or hist.numel() < K:
+        raise L.DB200Error("vae_kl_stats: a buffer is smaller than rows x K")
+    ws = L.workspace(L.load().db200_vae_kl_stats_workspace_bytes(rows, K))
+    check(L.load().db200_vae_kl_stats(stream_ptr(), ptr(logits), ptr(lse), ptr(ent), ptr(hist), ptr(kl_accum), rows,
+                                      K, scale, ptr(ws), _nbytes(ws)), "db200_vae_kl_stats")
+
+
+def gumbel_softmax_bwd_kl(y_soft, dy, logits, lse, ent, dlogits, rows, K, tau, c):
+    """gumbel_softmax_bwd plus the gradient of c * KL: dlogits += c q (l - lse - ent), in the same pass."""
+    L.require_device()
+    check(L.load().db200_gumbel_softmax_bwd_kl(stream_ptr(), ptr(y_soft), ptr(dy), ptr(logits), ptr(lse), ptr(ent),
+                                               ptr(dlogits), rows, K, tau, c), "gumbel_softmax_bwd_kl")
+
+
 def mse_fwd_bwd(pred, target, dpred, loss_accum, scale):
     L.require_device()
     check(L.load().db200_mse_fwd_bwd(stream_ptr(), ptr(pred), ptr(target), ptr(dpred), ptr(loss_accum),

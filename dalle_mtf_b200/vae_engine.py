@@ -6,6 +6,9 @@ src/model_fns_tf.py:40-66.  Parameter names are the reference's TF variable name
 (SURVEY.md Appendix B): kernels HWIO, transposed-conv kernels [kh,kw,out,in], codebook [n_hid, K].
 Activations are NHWC, fp32 or bf16 (use_bf16, src/model_fns_tf.py:48-53); the codebook matmuls, Gumbel-softmax and
 the loss are always fp32 (src/vae_tf/models.py:115-116,157-158).
+
+Optional KL term (extension, kl=True; the reference has none): KL(q_r || Uniform(K)) of q_r = softmax(raw logits), the
+mean over the latent rows, with a first-maximum code histogram for codebook-usage readouts (DESIGN.md §4).
 """
 import math
 
@@ -20,7 +23,7 @@ BF16, F32, I32 = torch.bfloat16, torch.float32, torch.int32
 
 class VaeEngine:
     def __init__(self, num_tokens, image_size, convblocks, input_channels=3, use_bf16=False, recompute_grad=False,
-                 stack_factor=1, device="cuda"):
+                 stack_factor=1, device="cuda", kl=False):
         L.require_device()
         assert math.log2(stack_factor).is_integer()                      # src/vae_tf/models.py:78
         self.K = int(num_tokens)
@@ -41,6 +44,9 @@ class VaeEngine:
         # recomputing would add a forward pass of FLOPs for nothing.  Gradients are identical either way (the
         # recomputation is deterministic), so the flag only changes memory, never numbers; model_fns says so at start-up.
         self.recompute_grad = bool(recompute_grad)
+        # KL statistics buffers ([rows] lse / ent, [K] code counts) exist only when the KL term may be requested
+        self.kl = bool(kl)
+        self._kl_c = None
         self.device = torch.device(device)
         self.act = BF16 if self.use_bf16 else F32
         if self.H % (2 ** len(self.convblocks)) != 0:
@@ -234,6 +240,8 @@ class VaeEngine:
             "dy": e(rows, self.K, dtype=F32), "dlogits": e(rows, self.K, dtype=F32),
             "dz_f32": e(rows, self.n_hid, dtype=F32), "denc_f32": e(rows, self.n_hid, dtype=F32),
         })
+        if self.kl:
+            b.update({"kl_lse": e(rows, dtype=F32), "kl_ent": e(rows, dtype=F32), "kl_hist": e(self.K, dtype=I32)})
         if self.stack_factor > 1:
             b["img_packed"] = e(B, self.H, self.W, self.C, dtype=F32)
             b["recon_flat"] = e(B, self.img_H, self.img_W, self.img_C, dtype=F32)
@@ -370,14 +378,29 @@ class VaeEngine:
         self._codebook_lookup(B)
         return self._unpack(self._decode_from_z(B))
 
-    def forward(self, img, u, temperature=1.0, hard=True, loss_accum=None):
+    def forward(self, img, u, temperature=1.0, hard=True, loss_accum=None, kl_weight=None, kl_accum=None):
         """DiscreteVAE.forward(return_recon_loss=True) (src/vae_tf/models.py:165-184).  u: fp32 uniform noise
-        [B*h*w, K] in [1e-9, 1) or None (no noise).  Adds sum((img-out)^2)/numel into loss_accum; returns recon."""
+        [B*h*w, K] in [1e-9, 1) or None (no noise).  Adds sum((img-out)^2)/numel into loss_accum; returns recon.
+
+        kl_weight (engine built with kl=True; None = no KL statistics): also adds the mean over the B*h*w latent rows of
+        KL(softmax(logits) || Uniform(K)) into kl_accum (default: aux slot 1, behind the loss), counts the first-maximum
+        code of every row into code_counts(), and, when kl_weight > 0, makes backward add the gradient of
+        kl_weight * KL to the encoder logits'."""
         B = img.shape[0]
         logits = self.encode_logits(img, for_training=True)
         b = self._b
         rows = B * self.hw * self.hw
         self._tau = float(temperature)
+        self._kl_c = None
+        if kl_weight is not None:
+            if not self.kl:
+                raise L.DB200Error("VaeEngine.forward: kl_weight needs an engine built with kl=True")
+            if kl_accum is None:
+                kl_accum = self.grads[self.aux_off + 1:self.aux_off + 2]
+            b["kl_hist"].zero_()
+            ops.vae_kl_stats(logits, b["kl_lse"], b["kl_ent"], b["kl_hist"], kl_accum, rows, self.K, 1.0 / rows)
+            if kl_weight > 0:   # weight 0 monitors only: backward then runs exactly the plain kernels
+                self._kl_c = float(kl_weight) / rows
         ops.gumbel_softmax_fwd(logits, u, b["y_soft"], b["y_out"], b["idx"], rows, self.K, self._tau, hard)
         self._codebook_lookup(B)
         recon = self._decode_from_z(B)
@@ -474,7 +497,7 @@ class VaeEngine:
             dzb = dx.view(rows, self.n_hid)                                                       # exactly bf16
             ops.linear_wgrad(dzb, b["y_hi"], gcb); ops.linear_wgrad(dzb, b["y_lo"], gcb)          # d codebook (decode)
             self._mm_split([dzb, dzb], [self.cb_hi, self.cb_lo], b["dy"], rows, self.K, self.n_hid, b_mn=True)
-            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
+            self._gumbel_backward(rows)
             ops.split_f32(b["dlogits"], b["dl_hi"], b["dl_lo"])
             ops.linear_wgrad(self._enc_bf16, b["dl_hi"], gcb); ops.linear_wgrad(self._enc_bf16, b["dl_lo"], gcb)
             self._mm_split([b["dl_hi"], b["dl_hi"], b["dl_lo"]], [self.cb_hi, self.cb_lo, self.cb_hi],
@@ -483,9 +506,24 @@ class VaeEngine:
             dz = self._to_f32(dx.view(rows, self.n_hid), b["dz_f32"])
             ops.rowmatmul_tn(dz, b["y_out"], gcb, rows, self.n_hid, self.K)                       # d codebook (decode)
             ops.rowmatmul(dz, cb, b["dy"], rows, self.n_hid, self.K)                              # dy = dz @ C
-            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
+            self._gumbel_backward(rows)
             ops.rowmatmul_tn(self._enc_f32, b["dlogits"], gcb, rows, self.n_hid, self.K)
             ops.rowmatmul(b["dlogits"], cb, b["denc_f32"], rows, self.K, self.n_hid, b_transposed=True)
+
+    def _gumbel_backward(self, rows):
+        """b["dlogits"] from b["dy"]: the straight-through Gumbel-softmax backward, plus the gradient of
+        kl_weight * KL (kl_weight / rows * q (l - lse - ent)) in the same pass when forward was given kl_weight > 0."""
+        b = self._b
+        if self._kl_c is None:
+            ops.gumbel_softmax_bwd(b["y_soft"], b["dy"], b["dlogits"], rows, self.K, self._tau)   # straight-through
+        else:
+            ops.gumbel_softmax_bwd_kl(b["y_soft"], b["dy"], b["logits"], b["kl_lse"], b["kl_ent"], b["dlogits"], rows,
+                                      self.K, self._tau, self._kl_c)
+
+    def code_counts(self):
+        """int32 [K]: how many latent rows of the last forward with kl_weight had each code as the first maximum of
+        their logits (a row with a NaN counts as code 0)."""
+        return self._b["kl_hist"]
 
     # ------------------------------------------------------------------------------------------ optimiser
     def zero_grads(self):
@@ -506,3 +544,12 @@ class VaeEngine:
         self._grads_clean = True
         if self._cb_tc:
             ops.split_f32(self.P("codebook/codebook"), self.cb_hi, self.cb_lo)
+
+
+def codebook_usage(counts):
+    """(codes_used, perplexity) of a code histogram: the number of codes with a count > 0 and exp(-sum p log p),
+    p = counts / sum(counts).  Host values (reading a device histogram synchronises)."""
+    c = counts.detach().double().cpu()
+    n = c.sum()
+    p = c[c > 0] / n
+    return int((c > 0).sum()), float(torch.exp(-(p * p.log()).sum()))

@@ -371,6 +371,19 @@ int db200_gumbel_softmax_fwd(db200_stream_t stream, const float* logits, const f
 int db200_gumbel_softmax_bwd(db200_stream_t stream, const float* y_soft, const float* dy, float* dlogits, int rows,
                              int K, float tau);
 int db200_argmax_rows_f32(db200_stream_t stream, const float* x, int32_t* idx, int rows, int K);
+/* KL(q_r || Uniform(K)) of the encoder logits l_r, q_r = softmax(l_r) (extension: the KL term of the DALL-E paper's
+ * ELB, DALLE-pytorch's kl_div_loss_weight; the reference has neither).  All f32 except the int32 histogram.
+ *   vae_kl_stats: lse[r] = logsumexp(l_r);  ent[r] = sum_k q_rk (l_rk - lse[r]);  hist[argmax l_r] += 1 (first maximum,
+ *                 a row with a NaN counts as code 0);  *kl_accum += scale * sum_r (ent[r] + log K).  One read of the
+ *                 logits; per-CTA partials added in CTA order (bit-reproducible); a row with NaN / inf logits may get a
+ *                 NaN lse / ent / KL but writes nothing outside its row and a histogram index in [0, K).
+ *   gumbel_softmax_bwd_kl: dlogits = y (dy - sum(dy.*y)) / tau + c q (l - lse - ent)   (q recomputed from l and lse)
+ * scale and c must be finite. */
+int db200_vae_kl_stats(db200_stream_t stream, const float* logits, float* lse, float* ent, int32_t* hist,
+                       float* kl_accum, int rows, int K, float scale, void* workspace, int64_t workspace_bytes);
+int64_t db200_vae_kl_stats_workspace_bytes(int rows, int K);
+int db200_gumbel_softmax_bwd_kl(db200_stream_t stream, const float* y_soft, const float* dy, const float* logits,
+                                const float* lse, const float* ent, float* dlogits, int rows, int K, float tau, float c);
 /* mse:  *loss_accum += sum((a-b)^2) * scale;  dgrad: da = 2*(a-b)*scale */
 int db200_mse_fwd_bwd(db200_stream_t stream, const float* pred, const float* target, float* dpred_or_null,
                       float* loss_accum, size_t n, float scale);

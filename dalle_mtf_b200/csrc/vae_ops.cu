@@ -1,10 +1,12 @@
-// K13 — Gumbel-softmax (soft / hard straight-through), row argmax with the first-maximum tie rule, MSE loss, and the
-// optional KL(q || Uniform(K)) term with its codebook-usage histogram.
+// K13 — Gumbel-softmax (soft / hard straight-through), row argmax with the first-maximum tie rule, MSE loss, the
+// optional KL(q || Uniform(K)) term with its codebook-usage histogram, and the optional logit-Laplace reconstruction
+// loss.
 // fp32 row kernels, one warp per row, warp-shuffle reductions; HBM-bound (the [rows][K] tensors are read/written once
 // or twice).
 //
 // Reference: gumbel_softmax src/vae_tf/layers.py:4-21, mse_loss :24-25, tf.math.argmax src/model_fns.py:76.
 #include <cfloat>
+#include <type_traits>
 
 #include "common.cuh"
 #include "ptx.cuh"
@@ -242,6 +244,91 @@ mse_kernel(const float* __restrict__ pred, const float* __restrict__ target, flo
   }
 }
 
+// ---- logit-Laplace reconstruction loss (the DALL-E paper's dVAE likelihood; the reference has MSE only).  The decoder
+// emits stats[p][0, Cp) = mu and stats[p][Cp, 2 Cp) = ln b per pixel p; the target x in [-1, 1] maps to
+// y = clamp(eps + (1 - 2 eps)(x + 1) / 2, eps, 1 - eps) = clamp(0.4 x + 0.5, 0.1, 0.9), t = logit(y), and per subpixel
+//   nll = ln 2 + ln b + ln y + ln(1 - y) + |t - mu| exp(-ln b),
+//   d nll / d mu = -sign(t - mu) exp(-ln b),   d nll / d ln b = 1 - |t - mu| exp(-ln b),
+//   xhat = 2 clamp((sigmoid(mu) - eps) / (1 - 2 eps), 0, 1) - 1 = clamp(2.5 sigmoid(mu) - 1.25, -1, 1).
+// An item is V consecutive channels of one pixel (V = 4: 16-byte loads and stores).  One wave of CTAs strides over the
+// items; each thread carries its (pixel, group) pair forward by the stride instead of dividing a 64-bit index.
+constexpr int LL_THREADS = 256;
+
+__device__ __forceinline__ void ll_one(float mu, float lb, const float* x, float* dmu, float* dlb, float& xh,
+                                       float c, float& nll, float& se) {
+  xh = fminf(fmaxf(fmaf(2.5f, 1.f / (1.f + expf(-mu)), -1.25f), -1.f), 1.f);
+  if (x) {
+    const float y = fminf(fmaxf(fmaf(0.4f, *x, 0.5f), 0.1f), 0.9f);
+    const float ly = logf(y), l1y = logf(1.f - y);
+    const float d = (ly - l1y) - mu;
+    const float ib = expf(-lb);
+    const float a = fabsf(d) * ib;
+    nll += 0.69314718055994531f + lb + (ly + l1y) + a;
+    const float e = xh - *x;
+    se = fmaf(e, e, se);
+    *dmu = d > 0.f ? -c * ib : (d < 0.f ? c * ib : (d == 0.f ? 0.f : d));   // sign(NaN) stays NaN
+    *dlb = c * (1.f - a);
+  }
+}
+
+template <int V>
+__global__ void __launch_bounds__(LL_THREADS)
+logit_laplace_kernel(const float* __restrict__ stats, const float* __restrict__ target, float* __restrict__ dstats,
+                     float* __restrict__ recon, float* __restrict__ partials, long long n_pix, int Cp, float scale) {
+  using VT = typename std::conditional<V == 4, float4, float>::type;
+  __shared__ float red[2][LL_THREADS / 32];
+  const int G = Cp / V;                                     // items per pixel
+  const long long start = (long long)blockIdx.x * LL_THREADS + threadIdx.x;
+  const long long stride = (long long)gridDim.x * LL_THREADS;
+  const long long sp = stride / G;
+  const int sg = (int)(stride % G);
+  long long p = start / G;
+  int g = (int)(start % G);
+  float nll = 0.f, se = 0.f;
+  for (; p < n_pix;) {
+    const long long s0 = p * 2 * Cp + (long long)g * V;     // mu of this item; ln b is Cp further
+    const long long i0 = p * Cp + (long long)g * V;
+    const VT mu = *reinterpret_cast<const VT*>(stats + s0);
+    const VT lb = *reinterpret_cast<const VT*>(stats + s0 + Cp);
+    VT xh, dm, dl;
+    if (target) {
+      const VT x = *reinterpret_cast<const VT*>(target + i0);
+      const float* xs = reinterpret_cast<const float*>(&x);
+      const float* ms = reinterpret_cast<const float*>(&mu);
+      const float* ls = reinterpret_cast<const float*>(&lb);
+      float* hs = reinterpret_cast<float*>(&xh);
+      float* dms = reinterpret_cast<float*>(&dm);
+      float* dls = reinterpret_cast<float*>(&dl);
+#pragma unroll
+      for (int v = 0; v < V; ++v) ll_one(ms[v], ls[v], xs + v, dms + v, dls + v, hs[v], scale, nll, se);
+      *reinterpret_cast<VT*>(dstats + s0) = dm;
+      *reinterpret_cast<VT*>(dstats + s0 + Cp) = dl;
+    } else {
+      const float* ms = reinterpret_cast<const float*>(&mu);
+      float* hs = reinterpret_cast<float*>(&xh);
+#pragma unroll
+      for (int v = 0; v < V; ++v) ll_one(ms[v], 0.f, nullptr, nullptr, nullptr, hs[v], 0.f, nll, se);
+    }
+    *reinterpret_cast<VT*>(recon + i0) = xh;
+    p += sp;
+    g += sg;
+    if (g >= G) { g -= G; ++p; }
+  }
+  if (!target) return;
+  nll = warp_sum(nll);
+  se = warp_sum(se);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { red[0][warp] = nll; red[1][warp] = se; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float a = 0.f, b = 0.f;
+#pragma unroll
+    for (int w = 0; w < LL_THREADS / 32; ++w) { a += red[0][w]; b += red[1][w]; }
+    partials[blockIdx.x] = a * scale;               // per-CTA partials, summed in CTA order by the launcher
+    partials[gridDim.x + blockIdx.x] = b * scale;
+  }
+}
+
 // tf.space_to_depth / tf.depth_to_space (NHWC, block size s) used by stack_factor > 1 (src/vae_tf/models.py:85-86,
 // 155-161): deep[n, y, x, (dy*s + dx)*C + c] = flat[n, y*s + dy, x*s + dx, c].  One thread per element, coalesced on
 // the deep side (the flat side is read / written in runs of C consecutive floats).
@@ -362,4 +449,47 @@ extern "C" int db200_mse_fwd_bwd(db200_stream_t stream_, const float* pred, cons
   if (blocks > (size_t)sm_count() * 8) blocks = (size_t)sm_count() * 8;
   mse_kernel<<<(int)blocks, 256, 0, stream>>>(pred, target, dpred, loss_accum, n, scale);
   return check_launch("mse_kernel");
+}
+
+// One wave: as many CTAs as fit on the device at once, each striding over the items, but no more than the items need.
+static int logit_laplace_blocks(long long n_pix, int Cp) {
+  int per_sm = 1;   // both instantiations: 256 threads, the same small static shared memory
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, logit_laplace_kernel<1>, LL_THREADS, 0);
+  const long long items = n_pix * (Cp % 4 == 0 ? Cp / 4 : Cp);
+  const long long need = (items + LL_THREADS - 1) / LL_THREADS;
+  const long long cap = (long long)sm_count() * (per_sm > 0 ? per_sm : 1);
+  return (int)(need < cap ? need : cap);
+}
+
+extern "C" int64_t db200_logit_laplace_workspace_bytes(int64_t n_pix, int Cp) {
+  return n_pix > 0 && Cp > 0 ? 2 * (int64_t)logit_laplace_blocks(n_pix, Cp) * (int64_t)sizeof(float) : 0;
+}
+
+extern "C" int db200_logit_laplace_fwd_bwd(db200_stream_t stream_, const float* stats, const float* target,
+                                           float* dstats, float* recon_out, float* nll_accum, float* mse_accum,
+                                           int64_t n_pix, int Cp, float scale, void* workspace,
+                                           int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(stats && recon_out && n_pix > 0 && Cp > 0 && n_pix <= INT64_MAX / (2 * (int64_t)Cp) &&
+                isfinite(scale), DB200_E_INVALID, "logit_laplace: bad arguments");
+  DB200_REQUIRE(!target || (dstats && nll_accum && mse_accum), DB200_E_INVALID,
+                "logit_laplace: a target needs dstats, nll_accum and mse_accum");
+  const int blocks = logit_laplace_blocks(n_pix, Cp);
+  DB200_REQUIRE(!target || workspace_ok(workspace, workspace_bytes, 2 * (int64_t)blocks * (int64_t)sizeof(float)),
+                DB200_E_INVALID,
+                "logit_laplace: needs an aligned workspace of db200_logit_laplace_workspace_bytes() bytes");
+  float* ws = static_cast<float*>(workspace);
+  const bool vec4 = Cp % 4 == 0 && aligned16(stats) && aligned16(recon_out) &&
+                    (!target || (aligned16(target) && aligned16(dstats)));
+  if (vec4)
+    logit_laplace_kernel<4><<<blocks, LL_THREADS, 0, stream>>>(stats, target, dstats, recon_out, ws, n_pix, Cp,
+                                                              scale);
+  else
+    logit_laplace_kernel<1><<<blocks, LL_THREADS, 0, stream>>>(stats, target, dstats, recon_out, ws, n_pix, Cp,
+                                                              scale);
+  const int rc = check_launch("logit_laplace_kernel");
+  if (rc != DB200_OK || !target) return rc;
+  const int rc2 = reduce_rows_add(stream, ws, blocks, 1, nll_accum);
+  if (rc2 != DB200_OK) return rc2;
+  return reduce_rows_add(stream, ws + blocks, blocks, 1, mse_accum);
 }

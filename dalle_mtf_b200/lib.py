@@ -194,6 +194,7 @@ _SIGNATURES = {
     "db200_vae_kl_stats": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_vp, c_i64],
     "db200_gumbel_softmax_bwd_kl": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_f32],
     "db200_mse_fwd_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_f32],
+    "db200_logit_laplace_fwd_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_f32, c_vp, c_i64],
     "db200_gather_cast_bf16_f32": [c_vp, c_vp, c_vp, c_vp, c_int],
     "db200_space_to_depth_f32": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_comm_load_nccl": [ctypes.c_char_p],
@@ -218,6 +219,7 @@ _WORKSPACE_QUERIES = {
     "db200_ce_finish_weighted_workspace_bytes": [c_int],
     "db200_embed_bwd_workspace_bytes": [c_int, c_int],
     "db200_vae_kl_stats_workspace_bytes": [c_int, c_int],
+    "db200_logit_laplace_workspace_bytes": [c_i64, c_int],
 }
 EXPORTED_SYMBOLS = ["db200_last_error", "db200_launch_count"] + sorted(_SIGNATURES) + sorted(_WORKSPACE_QUERIES)
 

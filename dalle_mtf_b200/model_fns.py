@@ -18,7 +18,7 @@ from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_conv_kernel, va
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
-from .vae_engine import VaeEngine, codebook_usage
+from .vae_engine import RECONSTRUCTION_LOSSES, VaeEngine, codebook_usage
 
 TRAIN, EVAL, PREDICT = "train", "eval", "predict"   # tf.estimator.ModeKeys values
 
@@ -45,13 +45,16 @@ class StepSpec:
         self.extra = extra or {}
         self.loss = None              # device scalar of the last step (read it only when logging: it syncs)
         self.loss_parts = None        # weighted loss: device [3] = text-row mean CE, image-row mean CE, mean z-term;
-                                      # VAE with KL: device [2] = reconstruction MSE, KL (global means)
+                                      # VAE with KL: device [2] = reconstruction MSE, KL (global means);
+                                      # logit-Laplace VAE: device [2] = NLL, image-space MSE (+ KL with the KL term)
         self.loss_parts_format = DALLE_PARTS_FORMAT   # how a training log line shows loss_parts
         self.codebook_usage = None    # VAE with KL: () -> (codes_used, perplexity) of the last batch (a collective)
 
 
 DALLE_PARTS_FORMAT = " text_ce {:.5f} image_ce {:.5f} z_term {:.3g}"
 VAE_PARTS_FORMAT = " recon_mse {:.5f} kl {:.5f}"
+VAE_LL_PARTS_FORMAT = " recon_nll {:.5f} recon_mse {:.5f}"
+VAE_LL_KL_PARTS_FORMAT = " recon_nll {:.5f} recon_mse {:.5f} kl {:.5f}"
 
 
 def _to_device(t, dtype, device):
@@ -77,7 +80,8 @@ def load_vae_model(params, device):
     vae = VaeEngine(num_tokens=vae_params["num_tokens"], image_size=D, convblocks=convblocks,
                     input_channels=vae_params.get("input_channels") or 3,
                     use_bf16=bool(vae_params.get("use_bf16")),   # bf16 -> wgmma implicit-GEMM convolutions
-                    stack_factor=vae_params.get("stack_factor") or 1, device=device)
+                    stack_factor=vae_params.get("stack_factor") or 1, device=device,
+                    reconstruction_loss=reconstruction_loss(vae_params.get("reconstruction_loss")))
     return vae, vae_checkpoint(params)
 
 
@@ -383,17 +387,33 @@ def vae_kl_weight(step, params):
     return beta * min(step / anneal, 1.0) if anneal else beta
 
 
+def reconstruction_loss(value):
+    """The VAE's reconstruction term from its config key reconstruction_loss (an extension): None (absent, null) or
+    "mse" is the reference's MSE, "logit_laplace" the DALL-E paper's logit-Laplace NLL; anything else is rejected."""
+    if value is None:
+        return "mse"
+    if not isinstance(value, str) or value not in RECONSTRUCTION_LOSSES:
+        raise ValueError(f"reconstruction_loss = {value!r}: must be one of {RECONSTRUCTION_LOSSES} (or null)")
+    return value
+
+
 def vae_model_fn(features, labels, mode, params):
     """src/model_fns_tf.py:9-114.  features = labels = images f32 [B,H,W,C] in [-1,1].
 
     With the extension key kl_loss_weight (and optionally kl_anneal_steps), spec.loss_sum * spec.loss_scale is the
     objective MSE + beta_t * KL, spec.loss_parts the device [2] (MSE, KL) of the global batch and
-    spec.codebook_usage() the (codes_used, perplexity) of its first-maximum codes."""
+    spec.codebook_usage() the (codes_used, perplexity) of its first-maximum codes.
+
+    With reconstruction_loss "logit_laplace" the reconstruction term is the mean logit-Laplace NLL and spec.loss_parts
+    the device (NLL, image-space MSE) or, with the KL term, (NLL, image-space MSE, KL)."""
     mode_str = mode_to_str(mode)
     if mode == PREDICT:
         raise NotImplementedError                                             # model_fns_tf.py:29-30
     kl_beta, _ = kl_loss_weight(params)
     kl_on = kl_beta is not None
+    recon_loss = reconstruction_loss(params.get("reconstruction_loss"))
+    ll = recon_loss == "logit_laplace"
+    n_aux = 3 if ll else (2 if kl_on else 1)    # aux slots: [recon term, KL, image-space MSE]
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -404,7 +424,8 @@ def vae_model_fn(features, labels, mode, params):
                       convblocks=params.get("convblocks") or [(3, 64), (3, 128), (3, 256)],
                       input_channels=params.get("input_channels") or 3,
                       recompute_grad=bool(params.get("recompute_grad")), use_bf16=bool(params.get("use_bf16")),
-                      stack_factor=params.get("stack_factor") or 1, device=device, kl=kl_on)
+                      stack_factor=params.get("stack_factor") or 1, device=device, kl=kl_on,
+                      reconstruction_loss=recon_loss)
     model.init_params(seed=params.get("seed") or 0)
     if dp.rank == 0:
         print_n_params(model.n_params())
@@ -434,13 +455,19 @@ def vae_model_fn(features, labels, mode, params):
         u = params.get("_gumbel_u")
         u = draw_noise() if u is None else u
         model.zero_grads()
-        # adds sum((img-out)^2)/local_numel into aux slot 0 and, with the KL term, the local mean KL into slot 1
+        # adds sum((img-out)^2)/local_numel (logit-Laplace: the mean NLL) into aux slot 0, with the KL term the local
+        # mean KL into slot 1, and with logit-Laplace the image-space MSE into slot 2
         recon = model.forward(img, u, temp, hard, kl_weight=spec.kl_weight)
         return recon
 
     def report(sums):
-        # sums: the all-reduced aux slots [MSE, KL], each the SUM over ranks of the local means
-        if kl_on:
+        # sums: the all-reduced aux slots [recon term, KL, image-space MSE], each the SUM over ranks of the local means
+        if ll:
+            parts = [sums[:1], sums[2:3]] + ([sums[1:2]] if kl_on else [])
+            spec.loss_parts = torch.cat(parts) * (1.0 / dp.world)
+            spec.loss_sum = sums[:1] + spec.kl_weight * sums[1:2] if kl_on else sums[:1]
+            spec.loss_scale = 1.0 / dp.world
+        elif kl_on:
             spec.loss_parts = sums[:2] * (1.0 / dp.world)
             spec.loss_sum, spec.loss_scale = sums[:1] + spec.kl_weight * sums[1:2], 1.0 / dp.world
         else:
@@ -462,12 +489,12 @@ def vae_model_fn(features, labels, mode, params):
         spec.global_step += 1
         model.optimizer_step(params["lr"], spec.global_step, grad_scale=1.0 / dp.world)   # model_fns_tf.py:58-60
         # each rank's aux slots hold its local means, all-reduced with the decoder bucket; the SUM over ranks / N
-        report(model.grads[model.aux_off:model.aux_off + 2])
+        report(model.grads[model.aux_off:model.aux_off + n_aux])
         return spec.loss_sum
 
     def eval_op(features, labels=None):
         run(features, False)
-        acc = model.grads[model.aux_off:model.aux_off + (2 if kl_on else 1)].clone()
+        acc = model.grads[model.aux_off:model.aux_off + n_aux].clone()
         dp.all_reduce_now(acc)
         report(acc)
         return spec.loss_sum
@@ -497,4 +524,6 @@ def vae_model_fn(features, labels, mode, params):
     if kl_on:
         spec.loss_parts_format = VAE_PARTS_FORMAT
         spec.codebook_usage = usage
+    if ll:
+        spec.loss_parts_format = VAE_LL_KL_PARTS_FORMAT if kl_on else VAE_LL_PARTS_FORMAT
     return spec

@@ -7,6 +7,7 @@ import torch
 from . import lib as L
 from .dalle_engine import DalleEngine
 from .model_fns import attention_layers, conv_kernel, dropout_rates, loss_weights, validate_kl_weight
+from .model_fns import reconstruction_loss as _reconstruction_loss
 from .vae_engine import VaeEngine
 
 
@@ -100,11 +101,17 @@ class DALLE:
 
 class DiscreteVAE:
     def __init__(self, num_tokens, dimensions, convblocks, dim=512, hidden_dim=64, input_channels=3,
-                 recompute_grad=False, use_bf16=False, stack_factor=1, kl_loss_weight=None):
+                 recompute_grad=False, use_bf16=False, stack_factor=1, kl_loss_weight=None, reconstruction_loss=None):
         """kl_loss_weight (extension; None: the reference's objective): beta of the KL term, a finite real >= 0.  With
         it, forward(..., return_recon_loss=True) returns MSE + beta * KL, KL the mean over the batch's latent rows of
-        KL(softmax(logits) || Uniform(K)), and leaves the device [2] (MSE, KL) in self.loss_parts."""
+        KL(softmax(logits) || Uniform(K)), and leaves the device [2] (MSE, KL) in self.loss_parts.
+
+        reconstruction_loss (extension; None or "mse": the reference's MSE): "logit_laplace" makes the reconstruction
+        term the mean logit-Laplace NLL; forward then returns the image-space output and, with return_recon_loss, the
+        objective NLL (+ beta * KL), leaving the device (NLL, image-space MSE) or (NLL, image-space MSE, KL) in
+        self.loss_parts."""
         self.kl_loss_weight, _ = validate_kl_weight(kl_loss_weight)
+        self.reconstruction_loss = _reconstruction_loss(reconstruction_loss)
         self.loss_parts = None
         self.num_tokens, self.dim, self.hdim = num_tokens, dim, hidden_dim   # dim / hidden_dim have no effect (ref too)
         self.H = self.W = dimensions
@@ -112,7 +119,8 @@ class DiscreteVAE:
         self.num_ch = input_channels
         self.stack_factor = stack_factor
         self.engine = VaeEngine(num_tokens, dimensions, convblocks, input_channels, use_bf16, recompute_grad,
-                                stack_factor, kl=self.kl_loss_weight is not None)
+                                stack_factor, kl=self.kl_loss_weight is not None,
+                                reconstruction_loss=self.reconstruction_loss)
         self.engine.init_params(0)
         self._gen = torch.Generator(device=self.engine.device).manual_seed(1234)
 
@@ -126,11 +134,15 @@ class DiscreteVAE:
         rows = img.shape[0] * e.hw * e.hw
         u = torch.empty(rows, e.K, dtype=torch.float32, device=e.device).uniform_(1e-9, 1.0, generator=self._gen)
         kl = self.kl_loss_weight is not None
-        acc = torch.zeros(2 if kl else 1, dtype=torch.float32, device=e.device)
+        ll = e.logit_laplace
+        acc = torch.zeros(3 if ll else (2 if kl else 1), dtype=torch.float32, device=e.device)  # [recon, KL, MSE]
         out = e.forward(img, u, temperature, hard_gumbel, loss_accum=acc[:1], kl_weight=self.kl_loss_weight,
-                        kl_accum=acc[1:] if kl else None)
+                        kl_accum=acc[1:2] if kl else None, mse_accum=acc[2:3] if ll else None)
         if not return_recon_loss:
             return out
+        if ll:
+            self.loss_parts = torch.cat([acc[:1], acc[2:3]] + ([acc[1:2]] if kl else []))
+            return (acc[:1] + self.kl_loss_weight * acc[1:2] if kl else acc[:1]), out
         if kl:                     # scalar glue: the objective from the two device sums
             self.loss_parts = acc
             return acc[:1] + self.kl_loss_weight * acc[1:], out

@@ -617,6 +617,22 @@ def mse_fwd_bwd(pred, target, dpred, loss_accum, scale):
                                      pred.numel(), scale), "mse_fwd_bwd")
 
 
+def logit_laplace(stats, target, dstats, recon, nll_accum, mse_accum, n_pix, Cp, scale):
+    """Logit-Laplace loss of f32 decoder stats [n_pix, 2 Cp] (mu | ln b) against the packed f32 target [n_pix, Cp] in
+    [-1, 1]: recon [n_pix, Cp] = the image-space output, nll_accum[0] / mse_accum[0] += scale * the sums of the NLL and
+    of (recon - target)^2, dstats = scale * d(NLL) / d(stats).  target None (decoding): recon only."""
+    L.require_device()
+    _chk(stats, F32, "stats"); _chk(target, F32, "target"); _chk(dstats, F32, "dstats"); _chk(recon, F32, "recon")
+    _chk(nll_accum, F32, "nll_accum"); _chk(mse_accum, F32, "mse_accum")
+    if stats.numel() < n_pix * 2 * Cp or recon.numel() < n_pix * Cp or (
+            target is not None and (target.numel() < n_pix * Cp or dstats is None or dstats.numel() < n_pix * 2 * Cp)):
+        raise L.DB200Error("logit_laplace: a buffer is smaller than n_pix x Cp")
+    ws = None if target is None else L.workspace(L.load().db200_logit_laplace_workspace_bytes(n_pix, Cp))
+    check(L.load().db200_logit_laplace_fwd_bwd(stream_ptr(), ptr(stats), ptr(target), ptr(dstats), ptr(recon),
+                                               ptr(nll_accum), ptr(mse_accum), n_pix, Cp, scale, ptr(ws),
+                                               _nbytes(ws)), "db200_logit_laplace_fwd_bwd")
+
+
 # ----------------------------------------------------------------------------------------------- input pipeline (N2)
 def image_crop_resize_normalize(packed_u8, offsets_i64, heights_i32, widths_i32, boxes_f32, out_f32, channels, size):
     """decode_img's crop_and_resize + (x - 127.5) / 127.5 for a packed batch of decoded uint8 images (input_fns.py:4-21)."""

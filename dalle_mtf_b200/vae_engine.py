@@ -9,6 +9,11 @@ the loss are always fp32 (src/vae_tf/models.py:115-116,157-158).
 
 Optional KL term (extension, kl=True; the reference has none): KL(q_r || Uniform(K)) of q_r = softmax(raw logits), the
 mean over the latent rows, with a first-maximum code histogram for codebook-usage readouts (DESIGN.md §4).
+
+Optional logit-Laplace reconstruction loss (extension, reconstruction_loss="logit_laplace"; the reference has MSE only):
+the decoder's final 1x1 conv emits 2 C_p channels, mu then ln b in the packed channel order, the loss is the mean
+logit-Laplace NLL of the targets mapped into (0.1, 0.9), and the image-space output is
+2 clamp((sigmoid(mu) - 0.1) / 0.8, 0, 1) - 1 (DESIGN.md §4).
 """
 import math
 
@@ -19,11 +24,12 @@ from . import ops
 from .dalle_engine import ParamLayout
 
 BF16, F32, I32 = torch.bfloat16, torch.float32, torch.int32
+RECONSTRUCTION_LOSSES = ("mse", "logit_laplace")
 
 
 class VaeEngine:
     def __init__(self, num_tokens, image_size, convblocks, input_channels=3, use_bf16=False, recompute_grad=False,
-                 stack_factor=1, device="cuda", kl=False):
+                 stack_factor=1, device="cuda", kl=False, reconstruction_loss="mse"):
         L.require_device()
         assert math.log2(stack_factor).is_integer()                      # src/vae_tf/models.py:78
         self.K = int(num_tokens)
@@ -38,6 +44,7 @@ class VaeEngine:
         self.H = self.W = self.img_H // self.stack_factor
         self.convblocks = [(int(s), int(c)) for s, c in convblocks]
         self.C = self.img_C * self.stack_factor ** 2
+        self.out_C = 2 * self.C if reconstruction_loss == "logit_laplace" else self.C   # decoder output channels
         self.use_bf16 = bool(use_bf16)
         # src/vae_tf/models.py:8-43 re-runs every residual pair inside backward to save activation memory.  Here the
         # activations are simply kept: at vae_coco (256 px, 16 images per GPU, bf16) they take ~6 GB of the 80 GB, and
@@ -47,6 +54,10 @@ class VaeEngine:
         # KL statistics buffers ([rows] lse / ent, [K] code counts) exist only when the KL term may be requested
         self.kl = bool(kl)
         self._kl_c = None
+        if reconstruction_loss not in RECONSTRUCTION_LOSSES:
+            raise ValueError(f"reconstruction_loss = {reconstruction_loss!r}: must be one of {RECONSTRUCTION_LOSSES}")
+        self.reconstruction_loss = reconstruction_loss
+        self.logit_laplace = reconstruction_loss == "logit_laplace"
         self.device = torch.device(device)
         self.act = BF16 if self.use_bf16 else F32
         if self.H % (2 ** len(self.convblocks)) != 0:
@@ -84,7 +95,7 @@ class VaeEngine:
                         lay.add(pre + nm + "/kernel", (3, 3, ch, ch)); lay.add(pre + nm + "/bias", (ch,))
                     self.dec.append(("res", pre, ch, ch, res))
             cin = ch
-        lay.add("decoder/conv2d/kernel", (1, 1, cin, self.C)); lay.add("decoder/conv2d/bias", (self.C,))
+        lay.add("decoder/conv2d/kernel", (1, 1, cin, self.out_C)); lay.add("decoder/conv2d/bias", (self.out_C,))
         self._first_dec = next(n for n in lay.order if n.startswith("decoder/"))
         self.dec_out_cin = cin
         self.layout = lay
@@ -234,14 +245,17 @@ class VaeEngine:
         if self._cb_tc:
             b.update({"y_hi": e(rows, self.K, dtype=BF16), "y_lo": e(rows, self.K, dtype=BF16),
                       "dl_hi": e(rows, self.K, dtype=BF16), "dl_lo": e(rows, self.K, dtype=BF16)})
+        oc = self.out_C
         b.update({
-            "recon_act": e(B, self.H, self.W, self.C), "recon": e(B, self.H, self.W, self.C, dtype=F32),
-            "drecon": e(B, self.H, self.W, self.C, dtype=F32), "drecon_act": e(B, self.H, self.W, self.C),
+            "recon_act": e(B, self.H, self.W, oc), "recon": e(B, self.H, self.W, oc, dtype=F32),
+            "drecon": e(B, self.H, self.W, oc, dtype=F32), "drecon_act": e(B, self.H, self.W, oc),
             "dy": e(rows, self.K, dtype=F32), "dlogits": e(rows, self.K, dtype=F32),
             "dz_f32": e(rows, self.n_hid, dtype=F32), "denc_f32": e(rows, self.n_hid, dtype=F32),
         })
         if self.kl:
             b.update({"kl_lse": e(rows, dtype=F32), "kl_ent": e(rows, dtype=F32), "kl_hist": e(self.K, dtype=I32)})
+        if self.logit_laplace:
+            b["xhat"] = e(B, self.H, self.W, self.C, dtype=F32)      # image-space output, packed
         if self.stack_factor > 1:
             b["img_packed"] = e(B, self.H, self.W, self.C, dtype=F32)
             b["recon_flat"] = e(B, self.img_H, self.img_W, self.img_C, dtype=F32)
@@ -324,7 +338,8 @@ class VaeEngine:
         return self._b["idx"].view(img.shape[0], self.image_seq_len)
 
     def _decode_from_z(self, B):
-        """DiscreteVAE.decoder after the tied codebook matmul (src/vae_tf/models.py:129-163): b["z_f32"] -> recon fp32."""
+        """DiscreteVAE.decoder after the tied codebook matmul (src/vae_tf/models.py:129-163): b["z_f32"] -> recon fp32
+        (logit-Laplace: the packed stats, mu | ln b)."""
         b = self._b
         rows = B * self.hw * self.hw
         x = self._to_act(b["z_f32"], b["z"].view(rows, self.n_hid)).view(B, self.hw, self.hw, self.n_hid)
@@ -336,7 +351,7 @@ class VaeEngine:
             else:
                 x = self._res_fwd(B, name, ch, res, x, sv)
         self._dec_last = x
-        ops.conv2d_fwd(self._desc(B, self.H, self.dec_out_cin, self.C, 1, 1), x, self.P("decoder/conv2d/kernel"),
+        ops.conv2d_fwd(self._desc(B, self.H, self.dec_out_cin, self.out_C, 1, 1), x, self.P("decoder/conv2d/kernel"),
                        self.P("decoder/conv2d/bias"), None, b["recon_act"])                   # models.py:155
         return self._to_f32(b["recon_act"], b["recon"])
 
@@ -376,11 +391,20 @@ class VaeEngine:
         rows = B * self.hw * self.hw
         ops.onehot_rows(idx.reshape(rows).contiguous(), self._b["y_out"], offset)
         self._codebook_lookup(B)
-        return self._unpack(self._decode_from_z(B))
+        out = self._decode_from_z(B)
+        if self.logit_laplace:
+            n_pix = B * self.H * self.W
+            ops.logit_laplace(out, None, None, self._b["xhat"], None, None, n_pix, self.C, 0.0)
+            out = self._b["xhat"]
+        return self._unpack(out)
 
-    def forward(self, img, u, temperature=1.0, hard=True, loss_accum=None, kl_weight=None, kl_accum=None):
+    def forward(self, img, u, temperature=1.0, hard=True, loss_accum=None, kl_weight=None, kl_accum=None,
+                mse_accum=None):
         """DiscreteVAE.forward(return_recon_loss=True) (src/vae_tf/models.py:165-184).  u: fp32 uniform noise
         [B*h*w, K] in [1e-9, 1) or None (no noise).  Adds sum((img-out)^2)/numel into loss_accum; returns recon.
+
+        Logit-Laplace engine: adds the mean NLL into loss_accum (default aux slot 0) and the mean (xhat - img)^2 into
+        mse_accum (default aux slot 2), and returns the image-space output xhat.
 
         kl_weight (engine built with kl=True; None = no KL statistics): also adds the mean over the B*h*w latent rows of
         KL(softmax(logits) || Uniform(K)) into kl_accum (default: aux slot 1, behind the loss), counts the first-maximum
@@ -410,6 +434,12 @@ class VaeEngine:
         n = img.numel()
         self._loss_scale = 1.0 / n
         packed = self._b["img_packed"] if self.stack_factor > 1 else img   # written by encode_logits
+        if self.logit_laplace:
+            if mse_accum is None:
+                mse_accum = self.grads[self.aux_off + 2:self.aux_off + 3]
+            ops.logit_laplace(recon, packed, b["drecon"], b["xhat"], loss_accum, mse_accum, B * self.H * self.W,
+                              self.C, 1.0 / n)
+            return self._unpack(b["xhat"])
         ops.mse_fwd_bwd(recon, packed, b["drecon"], loss_accum, 1.0 / n)                       # layers.py:24-25
         return self._unpack(recon)
 
@@ -436,7 +466,7 @@ class VaeEngine:
         if grad_scale != 1.0:
             raise L.DB200Error("VaeEngine.backward: fold grad_scale into the Adam step (grad_scale argument there)")
         dx = self._to_act(b["drecon"], b["drecon_act"])
-        d1 = self._desc(B, self.H, self.dec_out_cin, self.C, 1, 1)
+        d1 = self._desc(B, self.H, self.dec_out_cin, self.out_C, 1, 1)
         ops.conv2d_wgrad(d1, self._dec_last, dx, self.G("decoder/conv2d/kernel"), self.G("decoder/conv2d/bias"))
         gs = b["gscratch"][tuple(self._dec_last.shape)]
         ops.conv2d_dgrad(d1, dx, self.P("decoder/conv2d/kernel"), None, None, gs[0])

@@ -384,6 +384,20 @@ int db200_vae_kl_stats(db200_stream_t stream, const float* logits, float* lse, f
 int64_t db200_vae_kl_stats_workspace_bytes(int rows, int K);
 int db200_gumbel_softmax_bwd_kl(db200_stream_t stream, const float* y_soft, const float* dy, const float* logits,
                                 const float* lse, const float* ent, float* dlogits, int rows, int K, float tau, float c);
+/* Logit-Laplace reconstruction loss (extension: the DALL-E paper's dVAE likelihood; the reference has MSE only).  f32,
+ * n_pix pixels of Cp packed channels.  stats [n_pix][2 Cp]: mu in channels [0, Cp), ln b in [Cp, 2 Cp).
+ * target [n_pix][Cp] in [-1, 1]: y = clamp(0.1 + 0.8 (x + 1) / 2, 0.1, 0.9), t = ln y - ln(1 - y).
+ *   recon_out = clamp(2.5 sigmoid(mu) - 1.25, -1, 1)   (always written)
+ * With a target (dstats, nll_accum, mse_accum and the workspace then required):
+ *   *nll_accum += scale * sum (ln 2 + ln b + ln y + ln(1 - y) + |t - mu| exp(-ln b));
+ *   *mse_accum += scale * sum (recon_out - target)^2;
+ *   dstats[mu] = -scale sign(t - mu) exp(-ln b) (sign(0) = 0);  dstats[ln b] = scale (1 - |t - mu| exp(-ln b)).
+ * target NULL (decoding): only recon_out is written.  Both sums are per-CTA partials added in CTA order
+ * (bit-reproducible); a non-finite stat stays in its own element.  scale must be finite. */
+int db200_logit_laplace_fwd_bwd(db200_stream_t stream, const float* stats, const float* target_or_null,
+                                float* dstats_or_null, float* recon_out, float* nll_accum, float* mse_accum,
+                                int64_t n_pix, int Cp, float scale, void* workspace, int64_t workspace_bytes);
+int64_t db200_logit_laplace_workspace_bytes(int64_t n_pix, int Cp);
 /* mse:  *loss_accum += sum((a-b)^2) * scale;  dgrad: da = 2*(a-b)*scale */
 int db200_mse_fwd_bwd(db200_stream_t stream, const float* pred, const float* target, float* dpred_or_null,
                       float* loss_accum, size_t n, float scale);

@@ -163,8 +163,10 @@ __global__ void embed_bwd_wpe_kernel(const bf16* __restrict__ dx, float* __restr
   if constexpr (DROP) {
     float m[8];
     dropout_mul8(dp, s, d, c, m);
+    // rounded on its own (__fmul_rn is never contracted with the add below into an fma): the call adds one fully
+    // formed contribution, so W ranks summed in rank order equal one rank running the same rows as W micro-batches
 #pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] *= m[j];
+    for (int j = 0; j < 8; ++j) acc[j] = __fmul_rn(acc[j], m[j]);
   }
   float* dst = dwpe + (long long)s * d + c;
 #pragma unroll

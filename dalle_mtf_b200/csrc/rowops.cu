@@ -191,21 +191,116 @@ __global__ void assemble_tokens_kernel(const int* __restrict__ text, const int* 
   out[i] = t < Tt ? text[b * Tt + t] : img[b * Ti + (t - Tt)] + offset;
 }
 
-// the same with caption dropout: row b's text positions all become `pad` when the Philox word of global sequence index
-// e = dr.row0 + b (elementwise layout with cols = 1: block e >> 2, word e & 3) is below dr.threshold
-__global__ void assemble_tokens_drop_kernel(const int* __restrict__ text, const int* __restrict__ img,
-                                            int* __restrict__ out, int B, int Tt, int Ti, int offset, int pad,
-                                            const db200_dropout dr) {
+// One token of the assembly with caption dropout or per-position pads.  DROP: caption dropout, row b's text positions
+// all become a pad when the Philox word of global sequence index e = dr.row0 + b (elementwise layout with cols = 1:
+// block e >> 2, word e & 3) is below dr.threshold.  PER_POS: the pad of text position t is pad_base + t, and a caption
+// id equal to `pad` becomes that per-position pad too (DALL-E's separate padding token for each text position); without
+// it a dropped caption is `pad` everywhere and caption ids pass through unchanged.
+template <bool DROP, bool PER_POS>
+__device__ __forceinline__ void assemble_one(const int* __restrict__ text, const int* __restrict__ img,
+                                             int* __restrict__ out, int B, int Tt, int Ti, int offset, int pad,
+                                             int pad_base, const db200_dropout& dr) {
   const int S = Tt + Ti;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * S) return;
   const int b = i / S, t = i - b * S;
   if (t < Tt) {
-    const uint4 words = dropout_block(dr, dropout_elem_block(dr, b, 1, 0));
-    const bool dropped = uint4_word(words, (int)((dr.row0 + b) & 3)) < dr.threshold;
-    out[i] = dropped ? pad : text[b * Tt + t];
+    bool dropped = false;
+    if constexpr (DROP) {
+      const uint4 words = dropout_block(dr, dropout_elem_block(dr, b, 1, 0));
+      dropped = uint4_word(words, (int)((dr.row0 + b) & 3)) < dr.threshold;
+    }
+    if constexpr (PER_POS) {
+      const int id = text[b * Tt + t];
+      out[i] = (dropped || id == pad) ? pad_base + t : id;
+    } else {
+      out[i] = dropped ? pad : text[b * Tt + t];
+    }
   } else {
     out[i] = img[b * Ti + (t - Tt)] + offset;
+  }
+}
+
+// assemble_tokens_kernel with caption dropout
+__global__ void assemble_tokens_drop_kernel(const int* __restrict__ text, const int* __restrict__ img,
+                                            int* __restrict__ out, int B, int Tt, int Ti, int offset, int pad,
+                                            const db200_dropout dr) {
+  assemble_one<true, false>(text, img, out, B, Tt, Ti, offset, pad, 0, dr);
+}
+
+// the same with per-position pads (DROP: and caption dropout)
+template <bool DROP>
+__global__ void assemble_tokens_pp_kernel(const int* __restrict__ text, const int* __restrict__ img,
+                                          int* __restrict__ out, int B, int Tt, int Ti, int offset, int pad,
+                                          int pad_base, const db200_dropout dr) {
+  assemble_one<DROP, true>(text, img, out, B, Tt, Ti, offset, pad, pad_base, dr);
+}
+
+// ------------------------------------------------------------------------------------------------ row / column positions
+// pos[p] = wpe[p] for p < TL, pos[TL + r W + c] = bf16_rn(float(row[r]) + float(col[c])): the [S][d] bf16 table the
+// embedding kernels read in place of an absolute wpe.  One thread per (position, 8 columns), 16-byte loads and stores.
+__global__ void __launch_bounds__(256)
+pos_compose_kernel(const bf16* __restrict__ wpe, const bf16* __restrict__ row, const bf16* __restrict__ col,
+                   bf16* __restrict__ out, int TL, int W, int d) {
+  const int vec_per_row = d >> 3;
+  const long long total = (long long)(TL + W * W) * vec_per_row;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int p = (int)(i / vec_per_row);
+    const int c = (int)(i - (long long)p * vec_per_row) << 3;
+    uint4 v;
+    if (p < TL) {
+      v = *reinterpret_cast<const uint4*>(wpe + (long long)p * d + c);
+    } else {
+      const int r = (p - TL) / W, k = (p - TL) - r * W;
+      float a[8], b[8];
+      unpack8(*reinterpret_cast<const uint4*>(row + (long long)r * d + c), a);
+      unpack8(*reinterpret_cast<const uint4*>(col + (long long)k * d + c), b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a[j] += b[j];
+      v = pack8(a);
+    }
+    *reinterpret_cast<uint4*>(out + (long long)p * d + c) = v;
+  }
+}
+
+// The transpose of pos_compose on fp32 gradients: dwpe[p] += dpos[p] (p < TL), drow[r] += sum_c dpos[TL + r W + c] with c
+// ascending, dcol[c] += sum_r dpos[TL + r W + c] with r ascending.  One thread per (output row, 8 columns): every sum
+// runs in registers in that fixed order and is added to the gradient once, so the result is bit-reproducible and a call
+// adds one fully formed contribution (W ranks summed in rank order equal one rank running W micro-batches).
+__global__ void __launch_bounds__(256)
+pos_fold_kernel(const float* __restrict__ dpos, float* __restrict__ dwpe, float* __restrict__ drow,
+                float* __restrict__ dcol, int TL, int W, int d) {
+  const int vec_per_row = d >> 3;
+  const long long total = (long long)(TL + 2 * W) * vec_per_row;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int o = (int)(i / vec_per_row);
+    const int c = (int)(i - (long long)o * vec_per_row) << 3;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float* dst;
+    long long p0, stride;
+    int n;
+    if (o < TL) {
+      dst = dwpe + (long long)o * d; p0 = o; stride = 0; n = 1;
+    } else if (o < TL + W) {
+      const int r = o - TL;
+      dst = drow + (long long)r * d; p0 = TL + (long long)r * W; stride = 1; n = W;
+    } else {
+      const int k = o - TL - W;
+      dst = dcol + (long long)k * d; p0 = TL + k; stride = W; n = W;
+    }
+    for (int j = 0; j < n; ++j) {
+      const float* src = dpos + (p0 + j * stride) * d + c;
+      const float4 u = *reinterpret_cast<const float4*>(src), w = *reinterpret_cast<const float4*>(src + 4);
+      acc[0] += u.x; acc[1] += u.y; acc[2] += u.z; acc[3] += u.w;
+      acc[4] += w.x; acc[5] += w.y; acc[6] += w.z; acc[7] += w.w;
+    }
+    float4* q = reinterpret_cast<float4*>(dst + c);
+    float4 u = q[0], w = q[1];
+    u.x += acc[0]; u.y += acc[1]; u.z += acc[2]; u.w += acc[3];
+    w.x += acc[4]; w.y += acc[5]; w.z += acc[6]; w.w += acc[7];
+    q[0] = u; q[1] = w;
   }
 }
 
@@ -785,6 +880,59 @@ extern "C" int db200_assemble_tokens_ex(db200_stream_t stream_, const int32_t* t
   assemble_tokens_drop_kernel<<<(n + 255) / 256, 256, 0, stream>>>(text_ids, image_idx, tokens, B, text_len, image_len,
                                                                   image_offset, pad_id, *caption_drop);
   return check_launch("assemble_tokens_drop_kernel");
+}
+
+extern "C" int db200_assemble_tokens_pp(db200_stream_t stream_, const int32_t* text_ids, const int32_t* image_idx,
+                                        int32_t* tokens, int B, int text_len, int image_len, int image_offset,
+                                        int32_t pad_id, int32_t pad_base, const db200_dropout* caption_drop) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(B > 0 && text_len >= 0 && image_len >= 0 && text_len + image_len > 0 && tokens &&
+                    (text_len == 0 || text_ids) && (image_len == 0 || image_idx),
+                DB200_E_INVALID, "assemble_tokens_pp: bad arguments");
+  DB200_REQUIRE(pad_id >= 0 && pad_base >= 0 && (long long)pad_base + text_len <= 2147483647LL, DB200_E_INVALID,
+                "assemble_tokens_pp: pad_id %d pad_base %d", pad_id, pad_base);
+  const bool drop = dropout_active(caption_drop);
+  DB200_REQUIRE(!drop || caption_drop->row0 >= 0, DB200_E_INVALID, "assemble_tokens_pp: row0 %lld",
+                (long long)caption_drop->row0);
+  const int n = B * (text_len + image_len);
+  if (drop) {
+    assemble_tokens_pp_kernel<true><<<(n + 255) / 256, 256, 0, stream>>>(text_ids, image_idx, tokens, B, text_len,
+                                                                         image_len, image_offset, pad_id, pad_base,
+                                                                         *caption_drop);
+  } else {
+    assemble_tokens_pp_kernel<false><<<(n + 255) / 256, 256, 0, stream>>>(text_ids, image_idx, tokens, B, text_len,
+                                                                          image_len, image_offset, pad_id, pad_base,
+                                                                          db200_dropout{});
+  }
+  return check_launch("assemble_tokens_pp_kernel");
+}
+
+extern "C" int db200_pos_compose(db200_stream_t stream_, const void* wpe, const void* image_row, const void* image_col,
+                                 void* pos, int text_len, int grid_w, int d) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(text_len >= 0 && grid_w > 0 && d > 0 && d % 8 == 0, DB200_E_INVALID,
+                "pos_compose: need text_len >= 0, grid_w > 0 and d %% 8 == 0 (got %d %d %d)", text_len, grid_w, d);
+  DB200_REQUIRE((text_len == 0 || aligned16(wpe)) && aligned16(image_row) && aligned16(image_col) && aligned16(pos),
+                DB200_E_ALIGN, "pos_compose: NULL or unaligned pointer");
+  const long long total = ((long long)text_len + (long long)grid_w * grid_w) * (d / 8);
+  const int blocks = (int)((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
+  pos_compose_kernel<<<blocks, 256, 0, stream>>>((const bf16*)wpe, (const bf16*)image_row, (const bf16*)image_col,
+                                                 (bf16*)pos, text_len, grid_w, d);
+  return check_launch("pos_compose_kernel");
+}
+
+extern "C" int db200_pos_fold(db200_stream_t stream_, const float* dpos, float* dwpe, float* dimage_row,
+                              float* dimage_col, int text_len, int grid_w, int d) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(text_len >= 0 && grid_w > 0 && d > 0 && d % 8 == 0, DB200_E_INVALID,
+                "pos_fold: need text_len >= 0, grid_w > 0 and d %% 8 == 0 (got %d %d %d)", text_len, grid_w, d);
+  DB200_REQUIRE(aligned16(dpos) && (text_len == 0 || aligned16(dwpe)) && aligned16(dimage_row) &&
+                    aligned16(dimage_col),
+                DB200_E_ALIGN, "pos_fold: NULL or unaligned pointer");
+  const long long total = ((long long)text_len + 2LL * grid_w) * (d / 8);
+  const int blocks = (int)((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
+  pos_fold_kernel<<<blocks, 256, 0, stream>>>(dpos, dwpe, dimage_row, dimage_col, text_len, grid_w, d);
+  return check_launch("pos_fold_kernel");
 }
 
 extern "C" int db200_layernorm_fwd(db200_stream_t stream_, const void* x, const float* g, const float* b, void* y,

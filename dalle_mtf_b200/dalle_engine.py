@@ -61,13 +61,19 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
-def param_layout(d, n_layers, V, S):
+def param_layout(d, n_layers, V, S, text_len=None, grid_w=None):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
-    length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns."""
+    length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
+    column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
+    the grid_w rows and columns of the image-token grid."""
     Vpad = _round_up(V, 64)
     lay = ParamLayout()
     lay.add("wte", (V, d))
-    lay.add("wpe", (S, d))
+    if grid_w is None:
+        lay.add("wpe", (S, d))
+    else:
+        lay.add("wpe", (text_len, d))
+        lay.add("image_row", (grid_w, d)); lay.add("image_col", (grid_w, d))
     for i in range(n_layers):
         p = f"l{i}."
         lay.add(p + "ln1_g", (d,)); lay.add(p + "ln1_b", (d,))
@@ -137,6 +143,38 @@ def layer_conv(attention_types, text_seq_len, image_seq_len, kernel, n_layers):
     return [(int(text_seq_len), W, kernel) if t == "conv" else None for t in types]
 
 
+POSITION_EMBEDDINGS = ("absolute", "row_col")
+
+
+def validate_position_embedding(value):
+    """The image_position_embedding scheme: None or "absolute" (a learned vector per position, the reference's wpe) ->
+    "absolute"; "row_col" (the DALL-E paper's row embedding + column embedding per image token); anything else is
+    rejected."""
+    if value is None:
+        return "absolute"
+    if not isinstance(value, str) or value not in POSITION_EMBEDDINGS:
+        raise ValueError(f"image_position_embedding = {value!r}: must be one of {POSITION_EMBEDDINGS} (or null)")
+    return value
+
+
+def validate_per_position_padding(value):
+    """per_position_padding: None or a bool (None: False)."""
+    if value is None:
+        return False
+    if not isinstance(value, bool):
+        raise ValueError(f"per_position_padding = {value!r}: must be true, false or null")
+    return value
+
+
+def image_grid_side(image_seq_len):
+    """W of the W x W image-token grid row / column position embeddings need (image_seq_len = W^2)."""
+    W = math.isqrt(image_seq_len)
+    if W * W != image_seq_len:
+        raise ValueError(f"row_col image position embeddings need a square image-token grid, but image_seq_len = "
+                         f"{image_seq_len} is not a square")
+    return W
+
+
 def _real(v):
     return isinstance(v, numbers.Real) and not isinstance(v, bool)
 
@@ -182,7 +220,7 @@ class DalleEngine:
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
-                 conv_attention_kernel=5):
+                 conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -204,7 +242,20 @@ class DalleEngine:
         loss_weights = (w_text, w_image) and z_loss: the weighted loss of loss_coefficients() with z_loss * lse^2 added
         to every row (validate_loss_weights).  With either active, forward() accumulates four sums (weighted loss,
         text-row CE, image-row CE, z-term) and backward() runs the weighted CE_GRAD epilogue; otherwise the step is
-        the reference's."""
+        the reference's.
+
+        image_position_embedding "row_col" (None / "absolute": the reference's wpe [S, d]): wpe holds the text
+        positions only and image token (r, c) of the W x W grid (image_seq_len = W^2) gets image_row[r] + image_col[c].
+        The engine composes one bf16 [S, d] table from the bf16 parameters (pos_table) wherever they are rewritten, and
+        every embedding kernel reads it as it reads wpe otherwise; backward folds the table's gradient into the three.
+
+        per_position_padding: the text vocabulary grows by text_seq_len padding tokens, token text_vocab_size + p
+        being text position p's pad (pad_base = text_vocab_size), and image code i becomes token image_offset + i with
+        image_offset = text_vocab_size + text_seq_len (otherwise text_vocab_size).  Captions are mapped by
+        ops.assemble_tokens_pp."""
+        self.row_col = validate_position_embedding(image_position_embedding) == "row_col"
+        self.grid_w = image_grid_side(image_seq_len) if self.row_col else None
+        self.per_position_padding = validate_per_position_padding(per_position_padding)
         L.require_device()
         self.d, self.L, self.H = n_embd, n_layers, n_heads
         assert n_embd % n_heads == 0, "n_state must be divisible by n_heads"  # src/dalle_mtf/models.py:232
@@ -216,7 +267,9 @@ class DalleEngine:
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
         self.S = text_seq_len + image_seq_len                       # models.py:153
-        self.V = text_vocab_size + image_vocab_size + 1             # models.py:157 (extra id = EOS)
+        self.pad_base = text_vocab_size if self.per_position_padding else None
+        self.image_offset = text_vocab_size + (text_seq_len if self.per_position_padding else 0)
+        self.V = self.image_offset + image_vocab_size + 1           # models.py:157 (extra id = EOS)
         self.eos_token_id = self.V - 1                              # models.py:158
         self.Vpad = _round_up(self.V, 64)
         self.device = torch.device(device)
@@ -244,7 +297,9 @@ class DalleEngine:
         self._cew = None             # lib.CeWeights of the current forward (weighted loss only)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
-        self.layout = lay = param_layout(d, Lyr, V, S)
+        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w) if self.row_col else \
+            param_layout(d, Lyr, V, S)
+        self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
         #   [0] = sum of per-token losses of this rank (weighted loss: sum of a_t * loss_t)
@@ -281,6 +336,9 @@ class DalleEngine:
                     off += _round_up(shp[0], 64)
             self.vec32 = torch.zeros(off, dtype=F32, device=dev)
             self._vec_table = torch.tensor(table, dtype=torch.int64, device=dev)
+        if self.row_col:   # the composed bf16 position table the embedding kernels read, and its fp32 gradient
+            self.pos_table = torch.zeros(S, d, dtype=BF16, device=dev)
+            self._dpos = torch.zeros(S, d, dtype=F32, device=dev)
         self.gnorm_sq = torch.zeros(1, dtype=F32, device=dev)
         self._grads_clean = False
         self._bufs = None
@@ -314,11 +372,29 @@ class DalleEngine:
     def G(self, name):  # fp32 gradient view
         return self._view(2, self.grads, name)
 
+    def pos_embedding(self):
+        """The bf16 [S, d] position table the embedding kernels read: wpe, or with row / column image positions the
+        table composed from wpe, image_row and image_col."""
+        return self.pos_table if self.row_col else self.W("wpe")
+
+    def _compose_pos(self):
+        """Rebuild the composed position table from the bf16 parameters (row / column image positions only)."""
+        if self.row_col:
+            ops.pos_compose(self.W("wpe"), self.W("image_row"), self.W("image_col"), self.pos_table)
+
     def n_params(self):
         """Trainable parameter count as the reference would print it (src/utils/utils.py:55-70)."""
         d, V, S, Lyr = self.d, self.V, self.S, self.L
-        return V * d + S * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d) + \
+        n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else S
+        return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d) + \
             2 * d + d * V + V
+
+    EMBED_REF_NAMES = {"wte": "embedding/wte", "wpe": "positional_embedding/wpe",
+                       "image_row": "positional_embedding/image_row", "image_col": "positional_embedding/image_col"}
+
+    def _ref_embed_name(self, name):
+        """Reference-style variable name of an embedding parameter (other names are returned unchanged)."""
+        return self.EMBED_REF_NAMES.get(name, name)
 
     @staticmethod
     def _ref_names(i):
@@ -339,6 +415,9 @@ class DalleEngine:
         """ZeRO-1: place a full fp32 parameter tensor: bf16 copy (full) + the part of it inside this rank's slice."""
         off, shape = self.layout.entries[name]
         dst16 = self.layout.view(self.shadow, name)
+        if cols is None and tuple(t.shape) != tuple(shape):
+            raise L.DB200Error(f"load_params: {self._ref_embed_name(name)}: expected {tuple(shape)}, got "
+                               f"{tuple(t.shape)}")
         if cols is not None:
             dst16 = dst16[:, :cols] if dst16.dim() == 2 else dst16[:cols]
         dst16.copy_(t)
@@ -351,7 +430,9 @@ class DalleEngine:
             self.master[a - lo:b - lo].copy_(full.view(-1)[a - off:b - off])
 
     def _refresh_vecs(self):
+        """ZeRO-1: rebuild what is derived from the full bf16 parameters (fp32 vector parameters, position table)."""
         ops.gather_cast(self.shadow, self.vec32, self._vec_table, self._vec_table.numel() // 3)
+        self._compose_pos()
 
     def load_flat(self, flat, named):
         """Fill one of the flat fp32 buffers (master | adam_m | adam_v) from a dict of reference-named tensors."""
@@ -361,8 +442,8 @@ class DalleEngine:
                 raise L.DB200Error("ZeRO-1 mode: loading sharded Adam slots is not implemented (throughput configuration)")
             self.master.zero_(); self.shadow.zero_()
             f32 = lambda x: x.to(device=dev, dtype=F32)
-            self._scatter_full("wte", f32(named["embedding/wte"]))
-            self._scatter_full("wpe", f32(named["positional_embedding/wpe"]))
+            for name in self.embed_names:
+                self._scatter_full(name, f32(named[self._ref_embed_name(name)]))
             for i in range(self.L):
                 p = f"l{i}."
                 for k, rn in self._ref_names(i).items():
@@ -383,11 +464,12 @@ class DalleEngine:
             dst = view(name)
             t = t.to(device=dev, dtype=F32)
             if tuple(t.shape) != tuple(dst.shape):
-                raise L.DB200Error(f"load_params: {name}: expected {tuple(dst.shape)}, got {tuple(t.shape)}")
+                raise L.DB200Error(f"load_params: {self._ref_embed_name(name)}: expected {tuple(dst.shape)}, got "
+                                   f"{tuple(t.shape)}")
             dst.copy_(t)
 
-        put("wte", named["embedding/wte"])
-        put("wpe", named["positional_embedding/wpe"])
+        for name in self.embed_names:
+            put(name, named[self._ref_embed_name(name)])
         for i in range(self.L):
             p = f"l{i}."
             ref = self._ref_names(i)
@@ -409,7 +491,7 @@ class DalleEngine:
             raise L.DB200Error("ZeRO-1 mode: the Adam slots are sharded across ranks")
         flat = self.master if source is None else source
         view = lambda n: self.layout.view(flat, n).detach().float().cpu().clone()
-        out = {"embedding/wte": view("wte"), "positional_embedding/wpe": view("wpe")}
+        out = {self._ref_embed_name(n): view(n) for n in self.embed_names}
         d = self.d
         for i in range(self.L):
             p = f"l{i}."
@@ -439,6 +521,8 @@ class DalleEngine:
             t.copy_(torch.randn(t.shape, generator=g, device=self.device, dtype=F32) * std)
 
         normal("wte", 0.02); normal("wpe", 0.01)
+        if self.row_col:
+            normal("image_row", 0.01); normal("image_col", 0.01)
         for i in range(Lyr):
             p = f"l{i}."
             self.P(p + "ln1_g").fill_(1.0); self.P(p + "ln2_g").fill_(1.0)
@@ -458,7 +542,9 @@ class DalleEngine:
         self.master.zero_(); self.shadow.zero_()
         rn = lambda shape, std: torch.randn(shape, generator=g, device=self.device, dtype=F32) * std
         ones = lambda n: torch.ones(n, dtype=F32, device=self.device)
-        self._scatter_full("wte", rn((self.V, d), 0.02)); self._scatter_full("wpe", rn((self.S, d), 0.01))
+        self._scatter_full("wte", rn((self.V, d), 0.02))
+        for name in self.embed_names[1:]:
+            self._scatter_full(name, rn(self.layout.entries[name][1], 0.01))
         for i in range(Lyr):
             p = f"l{i}."
             self._scatter_full(p + "ln1_g", ones(d)); self._scatter_full(p + "ln2_g", ones(d))
@@ -476,6 +562,7 @@ class DalleEngine:
         if self.zero is not None:
             return self._refresh_vecs()
         ops.cast_f32_to_bf16(self.master[:self.n_params_padded], self.shadow[:self.n_params_padded])
+        self._compose_pos()
 
     def copy_params_from(self, src):
         """Take over the current weights of `src`, an engine of the same model and rank (evaluation of the weights
@@ -592,10 +679,11 @@ class DalleEngine:
         self._tokens = tokens
         self._drop = self._dropout_descs(step, row0)
         if self._drop is not None:
-            ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), bufs["xs"][0].view(B, S, self.d),
+            ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(), bufs["xs"][0].view(B, S, self.d),
                           wte_drop=self._drop["wte"], wpe_drop=self._drop["wpe"])            # models.py:198-217
         else:
-            ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), bufs["xs"][0].view(B, S, self.d))  # models.py:399
+            ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(),
+                          bufs["xs"][0].view(B, S, self.d))                                   # models.py:399
         for i in range(self.L):
             sv = bufs["layers"][0 if self.recompute_grad else i]
             self._block_fwd(i, bufs["xs"][i], bufs["xs"][i + 1], sv, B)
@@ -667,7 +755,7 @@ class DalleEngine:
             raise ValueError(f"prefill: expected {self.L} k and v caches of shape {shape}")
         b = self._prefill_alloc(B, P, rep)
         d = self.d
-        ops.embed_fwd(tokens, self.W("wte"), self.W("wpe"), b["xs"][0].view(B, P, d))
+        ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(), b["xs"][0].view(B, P, d))
         drop, self._drop = self._drop, None        # restored below: backward() of a preceding forward() reads it
         try:
             x_in, x_out = b["xs"]
@@ -762,13 +850,18 @@ class DalleEngine:
             if on_bucket_ready:
                 s, e = self.layout.span(f"l{i}.ln1_g", f"l{i}.b2")
                 on_bucket_ready(s, e)
+        # row / column positions: the gradient of the composed table goes into a zeroed scratch, then is folded into
+        # wpe, image_row and image_col (one fully formed contribution per call, like the wpe gradient itself)
+        dpos = self._dpos.zero_() if self.row_col else self.G("wpe")
         if self._drop is not None:
-            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), self.G("wpe"), wte_drop=self._drop["wte"],
+            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos, wte_drop=self._drop["wte"],
                           wpe_drop=self._drop["wpe"])
         else:
-            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), self.G("wpe"))
+            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos)
+        if self.row_col:
+            ops.pos_fold(dpos, self.G("wpe"), self.G("image_row"), self.G("image_col"))
         if on_bucket_ready:
-            s, e = self.layout.span("wte", "wpe")
+            s, e = self.layout.span("wte", self.embed_names[-1])
             on_bucket_ready(s, e)
 
     # ------------------------------------------------------------------------------------------ optimiser
@@ -787,7 +880,8 @@ class DalleEngine:
         exclude_from_weight_decay=["norm", "bias"] (src/optimizers.py:84-88), i.e. every variable whose NAME contains
         "norm" or "bias" (LayerNorm g/b, all biases incl. compute_output_bias/o_b) is left undecayed."""
         if getattr(self, "_segs", None) is None:
-            decays = lambda n: n in ("wte", "wpe", "wout") or n.split(".")[-1] in ("wqkv", "wo", "w1", "w2")
+            decays = lambda n: n in ("wte", "wpe", "image_row", "image_col", "wout") or \
+                n.split(".")[-1] in ("wqkv", "wo", "w1", "w2")
             segs = []
             for name in self.layout.order:
                 s, e = self.layout.span(name, name)
@@ -824,7 +918,8 @@ class DalleEngine:
             ops.adam_step(self.master[:n], self.adam_m[:n], self.adam_v[:n], self.grads[:n], self.shadow[:n], lr,
                           beta1, beta2, eps, 0.0, gn, clip, 1.0, False, 0, zero_grad=True)
             self._grads_clean = True
-            return
+            return self._compose_pos()
         for s, e, d in self._decay_segments():     # `update += weight_decay * param` only on the kernels / embeddings
             ops.adam_step(self.master[s:e], self.adam_m[s:e], self.adam_v[s:e], self.grads[s:e], self.shadow[s:e], lr,
                           beta1, beta2, eps, weight_decay if d else 0.0, gn, clip, 1.0, False, 0)
+        self._compose_pos()

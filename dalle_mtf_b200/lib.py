@@ -111,6 +111,10 @@ _SIGNATURES = {
     "db200_assemble_tokens": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_assemble_tokens_ex": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, ctypes.c_int32,
                                  ctypes.POINTER(Dropout)],
+    "db200_assemble_tokens_pp": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, ctypes.c_int32, ctypes.c_int32,
+                                 ctypes.POINTER(Dropout)],
+    "db200_pos_compose": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int],
+    "db200_pos_fold": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_shift_labels": [c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_layernorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
     "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],

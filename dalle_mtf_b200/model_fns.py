@@ -14,7 +14,8 @@ import torch
 
 from . import lib as L
 from . import ops
-from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_conv_kernel, validate_loss_weights
+from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_conv_kernel, validate_loss_weights, \
+    validate_per_position_padding, validate_position_embedding
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -171,6 +172,26 @@ def caption_dropout(params):
     return rate, int(pad)
 
 
+def input_embedding(params):
+    """(image_position_embedding, per_position_padding, padding_id) of a DALL-E config: the DALL-E paper's input
+    embedding (extension keys; both absent: the reference's).
+
+    image_position_embedding: absent, null or "absolute" is the reference's learned vector per position (wpe [S, d]);
+    "row_col" gives each image token the sum of a row and a column embedding of the W x W token grid, wpe keeping the
+    text positions only (DalleEngine).  per_position_padding: absent, null or false is off; true gives every text
+    position p its own padding token text_vocab_size + p, used wherever the caption holds padding_id (which must then
+    be an integer in [0, text_vocab_size)) and for dropped or unconditional captions.  padding_id is None when it is
+    off.  Any other value is rejected."""
+    scheme = validate_position_embedding(params.get("image_position_embedding"))
+    per_pos = validate_per_position_padding(params.get("per_position_padding"))
+    if not per_pos:
+        return scheme, False, None
+    pad, tv = params.get("padding_id"), params.get("text_vocab_size")
+    if pad is None or isinstance(pad, bool) or int(pad) != pad or tv is None or not 0 <= pad < tv:
+        raise ValueError(f"per_position_padding needs padding_id in [0, text_vocab_size = {tv}), got {pad!r}")
+    return scheme, True, int(pad)
+
+
 def loss_weights(params):
     """((w_text, w_image) or None, z_loss) of a DALL-E config: the extension keys text_loss_weight / image_loss_weight
     (both or neither; finite reals >= 0 with a sum > 0) and z_loss (a finite real >= 0, default 0).  The loss is then
@@ -189,6 +210,7 @@ def dalle_model_fn(features, labels, mode, params):
     attention_types, local_radius = attention_layers(params)
     conv_k = conv_kernel(params)
     weights, z_loss = loss_weights(params)
+    pos_scheme, per_pos, pp_pad = input_embedding(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -220,7 +242,8 @@ def dalle_model_fn(features, labels, mode, params):
                         zero=dp if (params.get("optimizer_state_sharding") and dp.enabled) else None,
                         dropout=rates, dropout_seed=params.get("seed") or 0,
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
-                        conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss)
+                        conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
+                        image_position_embedding=pos_scheme, per_position_padding=per_pos)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")
@@ -250,8 +273,12 @@ def dalle_model_fn(features, labels, mode, params):
         img = _to_device(features, torch.float32, device).view(local_batch, vae.img_H, vae.img_W, vae.img_C)
         text = _to_device(labels, torch.int32, device).view(local_batch, params["text_seq_len"])
         img_ids = vae.encode_tokens(img)                                        # model_fns.py:72-77
-        ops.assemble_tokens(text, img_ids, tokens, model.text_vocab_size,       # model_fns.py:117-122
-                            caption_drop=caption_drop, pad_id=pad_id)
+        if per_pos:   # padding ids (and dropped captions) become the per-position pads
+            ops.assemble_tokens_pp(text, img_ids, tokens, model.image_offset, pp_pad, model.pad_base,
+                                   caption_drop=caption_drop)
+        else:
+            ops.assemble_tokens(text, img_ids, tokens, model.text_vocab_size,   # model_fns.py:117-122
+                                caption_drop=caption_drop, pad_id=pad_id)
         return tokens
 
     def loss_value():

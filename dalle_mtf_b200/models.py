@@ -6,7 +6,8 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
-from .model_fns import attention_layers, conv_kernel, dropout_rates, loss_weights, validate_kl_weight
+from .model_fns import attention_layers, conv_kernel, dropout_rates, input_embedding, loss_weights, \
+    validate_kl_weight
 from .model_fns import reconstruction_loss as _reconstruction_loss
 from .vae_engine import VaeEngine
 
@@ -25,18 +26,21 @@ class DALLE:
         attention_types, local_radius = attention_layers({**params, "n_layers": n_layers})
         conv_k = conv_kernel(params)
         weights, z_loss = loss_weights(params)
+        pos_scheme, per_pos, _ = input_embedding({**params, "text_vocab_size": text_vocab_size})
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
         self.total_seq_dim = text_seq_len + image_seq_len
-        self.total_tokens = text_vocab_size + image_vocab_size + 1
+        # per-position padding: text_seq_len padding tokens follow the text vocabulary
+        self.total_tokens = text_vocab_size + (text_seq_len if per_pos else 0) + image_vocab_size + 1
         self.eos_token_id = self.total_tokens - 1 if eos_token_id is None else eos_token_id
         self.batch_size, self.bf_16, self.mode = batch_size, bf_16, mode
         self.engine = DalleEngine(n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len,
                                   image_seq_len, recompute_grad=bool(params.get("recompute_grad")) and mode == "train",
                                   dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0,
                                   attention_types=attention_types, local_attention_radius=local_radius,
-                                  conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss)
+                                  conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
+                                  image_position_embedding=pos_scheme, per_position_padding=per_pos)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

@@ -205,6 +205,52 @@ def assemble_tokens(text_ids, image_idx, tokens, image_offset, caption_drop=None
     return tokens
 
 
+def assemble_tokens_pp(text_ids, image_idx, tokens, image_offset, pad_id, pad_base, caption_drop=None):
+    """assemble_tokens with per-position padding: text position t becomes pad_base + t where the caption id is pad_id
+    or the row's caption is dropped (caption_drop as in assemble_tokens).  image_idx None: captions alone (tokens
+    [B, text_len])."""
+    L.require_device()
+    _chk(text_ids, I32, "text_ids"); _chk(image_idx, I32, "image_idx"); _chk(tokens, I32, "tokens")
+    B, Tt = text_ids.shape
+    Ti = 0 if image_idx is None else image_idx.shape[1]
+    if tuple(tokens.shape) != (B, Tt + Ti):
+        raise L.DB200Error(f"assemble_tokens_pp: tokens must be [{B}, {Tt + Ti}], got {tuple(tokens.shape)}")
+    check(L.load().db200_assemble_tokens_pp(stream_ptr(), ptr(text_ids), ptr(image_idx), ptr(tokens), B, Tt, Ti,
+                                            int(image_offset), int(pad_id), int(pad_base), _ref(caption_drop)),
+          "assemble_tokens_pp")
+    return tokens
+
+
+def pos_compose(wpe, image_row, image_col, out):
+    """out bf16 [TL + W^2, d] = wpe [TL, d] followed by image_row[r] + image_col[c] at TL + r W + c (bf16, each sum
+    rounded to nearest even)."""
+    L.require_device()
+    _chk(wpe, BF16, "wpe"); _chk(image_row, BF16, "image_row"); _chk(image_col, BF16, "image_col"); _chk(out, BF16, "out")
+    TL, d = wpe.shape
+    W = image_row.shape[0]
+    if tuple(image_col.shape) != (W, d) or tuple(image_row.shape) != (W, d) or tuple(out.shape) != (TL + W * W, d):
+        raise L.DB200Error(f"pos_compose: shapes wpe {tuple(wpe.shape)} image_row {tuple(image_row.shape)} "
+                           f"image_col {tuple(image_col.shape)} out {tuple(out.shape)}")
+    check(L.load().db200_pos_compose(stream_ptr(), ptr(wpe), ptr(image_row), ptr(image_col), ptr(out), TL, W, d),
+          "pos_compose")
+    return out
+
+
+def pos_fold(dpos, dwpe, dimage_row, dimage_col):
+    """dwpe [TL, d] += dpos[:TL]; dimage_row[r] += sum_c dpos[TL + r W + c]; dimage_col[c] += sum_r (fp32, fixed
+    order)."""
+    L.require_device()
+    _chk(dpos, F32, "dpos"); _chk(dwpe, F32, "dwpe"); _chk(dimage_row, F32, "dimage_row")
+    _chk(dimage_col, F32, "dimage_col")
+    TL, d = dwpe.shape
+    W = dimage_row.shape[0]
+    if tuple(dimage_col.shape) != (W, d) or tuple(dimage_row.shape) != (W, d) or tuple(dpos.shape) != (TL + W * W, d):
+        raise L.DB200Error(f"pos_fold: shapes dpos {tuple(dpos.shape)} dwpe {tuple(dwpe.shape)} dimage_row "
+                           f"{tuple(dimage_row.shape)} dimage_col {tuple(dimage_col.shape)}")
+    check(L.load().db200_pos_fold(stream_ptr(), ptr(dpos), ptr(dwpe), ptr(dimage_row), ptr(dimage_col), TL, W, d),
+          "pos_fold")
+
+
 def shift_labels(ids, labels, eos_id):
     L.require_device()
     _chk(ids, I32, "ids"); _chk(labels, I32, "labels")

@@ -16,12 +16,14 @@ parameters and the same kernels' numerics as training:
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
 instead runs the whole prompt (text, optionally followed by the first rows of an image's codes) through the training
 forward kernels in one pass (DalleEngine.prefill) and continues from there with the same sampling step.  Image
-positions are restricted to the image-token id range [text_vocab_size, text_vocab_size + image_vocab_size), matching
-the ids training builds (src/model_fns.py:117-122).  `temperature == 0` (or None) is greedy decoding; `top_k` /
+positions are restricted to the image-token id range [image_offset, image_offset + image_vocab_size), matching the
+ids training builds (src/model_fns.py:117-122; image_offset = text_vocab_size, + text_seq_len with per-position
+padding).  `temperature == 0` (or None) is greedy decoding; `top_k` /
 `top_p` truncate the image-token distribution (after temperature) before the Gumbel-max draw.
 
 Classifier-free guidance (`guidance_scale` s, "condition scale"): every sampled row gets a twin whose caption is
-text_seq_len padding ids (the unconditional prompt a model trained with caption dropout has learned).  The 2R rows run
+text_seq_len padding ids (the unconditional prompt a model trained with caption dropout has learned; with
+per-position padding the text_seq_len per-position pads).  The 2R rows run
 through the same step kernels (R conditional rows, then R unconditional ones) and each image token is drawn once per
 pair from u + s (c - u) of the two logit rows (db200_sample_rows_guided), then fed to both.  s = 1 (or None) is the
 plain sampler: no twin rows, the same kernels, the same tokens.
@@ -47,6 +49,22 @@ class DalleSampler:
         self.padding_id = int(pad)
         self._B = None
 
+    def _captions(self, text_ids):
+        """The text positions of the prompt rows: text_ids, or with per-position padding text_ids with every padding_id
+        at position p replaced by p's padding token (the training mapping, db200_assemble_tokens_pp)."""
+        e = self.e
+        if not e.per_position_padding:
+            return text_ids
+        out = torch.empty(text_ids.shape, dtype=I32, device=e.device)
+        return ops.assemble_tokens_pp(text_ids.to(device=e.device, dtype=I32).contiguous(), None, out, 0,
+                                      self.padding_id, e.pad_base)
+
+    def _uncond(self, B):
+        """The text positions of B unconditional (guidance) rows: padding_id everywhere, or the per-position pads."""
+        if not self.e.per_position_padding:
+            return self.padding_id
+        return self._captions(torch.full((B, self.e.text_seq_len), self.padding_id, dtype=I32, device=self.e.device))
+
     def _alloc(self, B):
         if self._B == B:
             return
@@ -70,7 +88,7 @@ class DalleSampler:
     def step(self, tokens_b, pos):
         """One position for every row: tokens_b int32 [B] -> fp32 logits [B, Vpad] of the NEXT position."""
         e = self.e
-        ops.embed_fwd_at(tokens_b, e.W("wte"), e.W("wpe"), self.x[0], pos)
+        ops.embed_fwd_at(tokens_b, e.W("wte"), e.pos_embedding(), self.x[0], pos)
         x_in, x_out = self.x
         for i in range(e.L):
             p = f"l{i}."
@@ -92,7 +110,7 @@ class DalleSampler:
     def _step_dev(self, tokens):
         """self.step with the position (and the input token column) read on the device from self.pos_dev."""
         e = self.e
-        ops.embed_fwd_at_dev(tokens, e.W("wte"), e.W("wpe"), self.x[0], self.pos_dev)
+        ops.embed_fwd_at_dev(tokens, e.W("wte"), e.pos_embedding(), self.x[0], self.pos_dev)
         x_in, x_out = self.x
         for i in range(e.L):
             p = f"l{i}."
@@ -132,7 +150,7 @@ class DalleSampler:
 
     def _sample_guided(self, logits, u, tokens, inv_t, flt, gs, pos_dev=None):
         e = self.e
-        lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+        lo, hi = e.image_offset, e.image_offset + e.image_vocab_size
         ops.sample_rows_guided(logits, u, tokens, lo, hi, inv_t, gs, *(flt or (0, 1.0)), pos_dev=pos_dev)
 
     def _capture(self, B, greedy, inv_t, flt, gs=None):
@@ -146,7 +164,7 @@ class DalleSampler:
         dev = e.device
         self.tokens = torch.zeros(2 * B if gs is not None else B, e.S, dtype=I32, device=dev)
         self.pos_dev = torch.zeros(1, dtype=I32, device=dev)
-        lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+        lo, hi = e.image_offset, e.image_offset + e.image_vocab_size
 
         def sample(logits):
             if gs is not None:
@@ -194,9 +212,9 @@ class DalleSampler:
         inv_t = 1.0 if greedy else 1.0 / float(temperature)
         self._capture(B, greedy, inv_t, flt, gs)
         self.tokens.zero_()
-        self.tokens[:B, :TL] = text_ids
+        self.tokens[:B, :TL] = self._captions(text_ids)
         if gs is not None:
-            self.tokens[B:, :TL] = self.padding_id
+            self.tokens[B:, :TL] = self._uncond(B)
         self.pos_dev.zero_()
         for pos in range(e.S - 1):
             (self.g_prompt if pos + 1 < TL else self.g_sample).replay()
@@ -208,7 +226,7 @@ class DalleSampler:
         """Image completion: text_ids int32 [B, text_seq_len] (device) and optionally image_prefix int32 [B, n], the
         first n (0 < n < image_seq_len) VAE codes in [0, image_vocab_size) in the VAE's row-major token order (e.g.
         vae.encode_tokens(img)[:, :n]).  Returns int32 [B * samples_per_prompt, text_seq_len + image_seq_len]: row
-        b * samples_per_prompt + r is sample r of prompt b, the prompt (prefix offset by text_vocab_size) followed by
+        b * samples_per_prompt + r is sample r of prompt b, the prompt (prefix offset by image_offset) followed by
         sampled image-token ids.
 
         The whole prompt (P = text_seq_len + n positions) runs once per distinct prompt as one batched forward pass
@@ -248,13 +266,13 @@ class DalleSampler:
         self._capture(R, greedy, inv_t, flt, gs)
         torch.cuda.set_rng_state(rng, e.device)
         prompt = torch.empty(2 * B if gs is not None else B, P, dtype=I32, device=e.device)
-        prompt[:B, :TL] = text_ids
+        prompt[:B, :TL] = self._captions(text_ids)
         if gs is not None:
-            prompt[B:, :TL] = self.padding_id
+            prompt[B:, :TL] = self._uncond(B)
         if n:   # (with guidance the padding-caption prompts continue with the same image prefix)
-            prompt[:, TL:] = (image_prefix.to(device=e.device, dtype=I32) + e.text_vocab_size).repeat(len(prompt) // B, 1)
+            prompt[:, TL:] = (image_prefix.to(device=e.device, dtype=I32) + e.image_offset).repeat(len(prompt) // B, 1)
         logits = e.prefill(prompt, self.kc, self.vc, rep)
-        lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+        lo, hi = e.image_offset, e.image_offset + e.image_vocab_size
         if self.u is not None:
             self.u.uniform_(1e-9, 1.0)
         if gs is not None:
@@ -275,7 +293,7 @@ class DalleSampler:
     def generate(self, text_ids, temperature=1.0, generator=None, return_logits=False, top_k=None, top_p=None,
                  guidance_scale=None):
         """text_ids int32 [B, text_seq_len] (device) -> int32 [B, text_seq_len + image_seq_len]: the prompt followed by
-        image_seq_len sampled image-token ids (already offset by text_vocab_size, as in training).
+        image_seq_len sampled image-token ids (already offset by the engine's image_offset, as in training).
 
         top_k (>= 1) keeps the k most likely image tokens (all of a tie at the k-th), top_p (in (0, 1]) the smallest
         set of them whose probability mass after temperature reaches p (nucleus sampling); with both, top-k applies
@@ -292,10 +310,10 @@ class DalleSampler:
         rows = 2 * B if gs is not None else B
         self._alloc(rows)
         out = torch.empty(rows, e.S, dtype=I32, device=e.device)
-        out[:B, :TL] = text_ids
+        out[:B, :TL] = self._captions(text_ids)
         if gs is not None:
-            out[B:, :TL] = self.padding_id
-        lo, hi = e.text_vocab_size, e.text_vocab_size + e.image_vocab_size
+            out[B:, :TL] = self._uncond(B)
+        lo, hi = e.image_offset, e.image_offset + e.image_vocab_size
         greedy = temperature is None or temperature <= 0
         inv_t = 1.0 if greedy else 1.0 / float(temperature)
         kept = [] if return_logits else None

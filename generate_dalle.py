@@ -6,7 +6,8 @@ image tokens for each caption (optionally completing the top rows of a prompt im
         [--temperature T] [--top_k K] [--top_p P] [--guidance_scale G] [--batch_size B] [--seed S]
 
 Writes DIR/{caption:05d}_{sample:02d}.png and DIR/tokens.npy (int32 [captions * samples_per_prompt, S]: caption ids,
-then image-token ids offset by text_vocab_size, as in training).  One process, one GPU.
+then image-token ids offset as in training: by text_vocab_size, or with per_position_padding by text_vocab_size +
+text_seq_len, the caption's padding then shown as the per-position pad tokens the model saw).  One process, one GPU.
 """
 import argparse
 import math
@@ -17,7 +18,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
-from dalle_mtf_b200.model_fns import attention_layers, conv_kernel, vae_checkpoint
+from dalle_mtf_b200.model_fns import attention_layers, conv_kernel, input_embedding, vae_checkpoint
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
 PADDING_ID = 50257   # GPT-2 vocabulary + <|padding|> (src/data/tokenizer_utils.py), what training pads captions with
@@ -87,31 +88,31 @@ def find_checkpoints(params, checkpoint=None):
     return local_path(ckpt), local_path(vae_ckpt)
 
 
-def pad_captions(rows, text_seq_len, text_vocab_size):
-    """Captions (lists of ids) -> int32 [N, text_seq_len], padded / truncated as in training."""
+def pad_captions(rows, text_seq_len, text_vocab_size, pad=PADDING_ID):
+    """Captions (lists of ids) -> int32 [N, text_seq_len], padded with `pad` / truncated as in training."""
     if len(rows) == 0:
         raise SystemExit("no captions given")
-    out = np.stack([truncate_or_pad_label(r, text_seq_len, PADDING_ID) for r in rows])
+    out = np.stack([truncate_or_pad_label(r, text_seq_len, pad) for r in rows])
     if out.min() < 0 or out.max() >= text_vocab_size:
         raise SystemExit(f"caption ids must lie in [0, {text_vocab_size})")
     return out
 
 
-def load_caption_ids(path, text_seq_len, text_vocab_size):
+def load_caption_ids(path, text_seq_len, text_vocab_size, pad=PADDING_ID):
     ids = np.load(path)
     if ids.ndim == 1:
         ids = ids[None]
     if ids.ndim != 2 or not np.issubdtype(ids.dtype, np.integer):
         raise SystemExit(f"{path}: expected an integer array [N, <= {text_seq_len}], got {ids.dtype} {ids.shape}")
-    return pad_captions(list(ids), text_seq_len, text_vocab_size)
+    return pad_captions(list(ids), text_seq_len, text_vocab_size, pad)
 
 
-def encode_captions(lines, tokenizer, text_seq_len, text_vocab_size):
+def encode_captions(lines, tokenizer, text_seq_len, text_vocab_size, pad=PADDING_ID):
     try:
         rows = [tokenizer.encode(line) for line in lines]
     except NotImplementedError as err:
         raise SystemExit(f"cannot tokenise captions ({err}); pass pre-tokenised ids with --caption_ids") from None
-    return pad_captions(rows, text_seq_len, text_vocab_size)
+    return pad_captions(rows, text_seq_len, text_vocab_size, pad)
 
 
 def token_grid_side(params):
@@ -151,16 +152,20 @@ def main(argv=None):
     tl, tv, iv = params["text_seq_len"], params["text_vocab_size"], params["image_vocab_size"]
     attention_types, local_radius = attention_layers(params)    # the layer types the checkpoint was trained with
     conv_k = conv_kernel(params)
+    pos_scheme, per_pos, _ = input_embedding(params)   # the input embedding the checkpoint was trained with
+    # with per-position padding the captions are padded with the config's padding_id, which the sampler maps to the
+    # per-position pads as training does
+    pad = padding_id(params) if per_pos else PADDING_ID
     if args.guidance_scale is not None and not 0 <= padding_id(params) < tv:
         raise SystemExit(f"--guidance_scale: padding id {padding_id(params)} outside [0, {tv}); set padding_id in the "
                          "config")
     if args.caption_ids:
-        captions = load_caption_ids(args.caption_ids, tl, tv)
+        captions = load_caption_ids(args.caption_ids, tl, tv, pad)
     else:
         from dalle_mtf_b200.tokenizer import get_tokenizer
         with open(args.captions) as f:
             lines = [ln.rstrip("\n") for ln in f if ln.strip()]
-        captions = encode_captions(lines, get_tokenizer(params["tokenizer"]), tl, tv)
+        captions = encode_captions(lines, get_tokenizer(params["tokenizer"]), tl, tv, pad)
     N = len(captions)
     n = 0
     if args.image_prompt:
@@ -185,7 +190,8 @@ def main(argv=None):
                          "codebook")
     eng = DalleEngine(params["n_embd"], params["n_layers"], params["n_heads"], tv, iv, tl, vae.image_seq_len,
                       device=device, attention_types=attention_types, local_attention_radius=local_radius,
-                      conv_attention_kernel=conv_k)
+                      conv_attention_kernel=conv_k, image_position_embedding=pos_scheme,
+                      per_position_padding=per_pos)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})
@@ -195,7 +201,7 @@ def main(argv=None):
         prefix = encode_image_prompts(args.image_prompt, params, vae, device)[:, :n]
         if len(prefix) == 1:
             prefix = prefix.expand(N, n)
-    sampler = DalleSampler(eng, padding_id=padding_id(params) if args.guidance_scale is not None else None)
+    sampler = DalleSampler(eng, padding_id=padding_id(params) if (args.guidance_scale is not None or per_pos) else None)
     torch.manual_seed(args.seed)
     rep = args.samples_per_prompt
     bs = args.batch_size or params["predict_batch_size"] or 1
@@ -206,7 +212,7 @@ def main(argv=None):
         pre = prefix[c0:c0 + bs].contiguous() if prefix is not None else None
         toks = sampler.complete(text, pre, samples_per_prompt=rep, temperature=args.temperature, top_k=args.top_k,
                                 top_p=args.top_p, guidance_scale=args.guidance_scale)
-        imgs = to_uint8(vae.decode_tokens(toks[:, tl:].contiguous(), offset=tv).cpu().numpy())
+        imgs = to_uint8(vae.decode_tokens(toks[:, tl:].contiguous(), offset=eng.image_offset).cpu().numpy())
         for j, im in enumerate(imgs):
             c, s = c0 + j // rep, j % rep
             Image.fromarray(im if im.shape[-1] == 3 else im[..., 0]).save(

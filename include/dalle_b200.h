@@ -108,6 +108,26 @@ int db200_assemble_tokens(db200_stream_t stream, const int32_t* text_ids, const 
 int db200_assemble_tokens_ex(db200_stream_t stream, const int32_t* text_ids, const int32_t* image_idx, int32_t* tokens,
                              int B, int text_len, int image_len, int image_offset, int32_t pad_id,
                              const db200_dropout* caption_drop);
+/* with per-position padding (the DALL-E paper's separate padding token for each text position): text position t of
+ * row b becomes pad_base + t when its caption id equals pad_id or when the row's caption is dropped (caption_drop as in
+ * _ex; NULL or threshold 0: no dropout); other caption ids pass through and image positions are as above.  image_len
+ * may be 0 (captions alone, image_idx NULL).  pad_id < 0, pad_base < 0 or row0 < 0 -> DB200_E_INVALID. */
+int db200_assemble_tokens_pp(db200_stream_t stream, const int32_t* text_ids, const int32_t* image_idx, int32_t* tokens,
+                             int B, int text_len, int image_len, int image_offset, int32_t pad_id, int32_t pad_base,
+                             const db200_dropout* caption_drop);
+
+/* Row / column image positions (the DALL-E paper's input embedding).  The image tokens form a grid_w x grid_w grid.
+ *   pos_compose: pos bf16 [text_len + grid_w^2][d] from wpe [text_len][d], image_row / image_col [grid_w][d] (bf16):
+ *                pos[p] = wpe[p] for p < text_len, pos[text_len + r grid_w + c] = bf16_rn(float(image_row[r]) +
+ *                float(image_col[c])).  The embedding kernels read pos where they read an absolute wpe.
+ *   pos_fold:    its transpose on fp32 gradients, dpos [text_len + grid_w^2][d]: dwpe[p] += dpos[p],
+ *                dimage_row[r] += sum_c dpos[text_len + r grid_w + c] (c ascending), dimage_col[c] += sum_r (r
+ *                ascending).  Each sum is formed in fp32 in that order and added once: bit-reproducible.
+ * d % 8 == 0, 16-byte aligned pointers (wpe / dwpe may be NULL when text_len == 0). */
+int db200_pos_compose(db200_stream_t stream, const void* wpe_bf16, const void* image_row_bf16,
+                      const void* image_col_bf16, void* pos_bf16, int text_len, int grid_w, int d);
+int db200_pos_fold(db200_stream_t stream, const float* dpos, float* dwpe, float* dimage_row, float* dimage_col,
+                   int text_len, int grid_w, int d);
 
 /* label shift: labels[b][t] = ids[b][t+1], labels[b][S-1] = eos_id.  Replaces the pad + gather at
  * src/dalle_mtf/models.py:407-410 (pad op: src/dalle_mtf/ops.py:6-68). */

@@ -190,7 +190,14 @@ _SIGNATURES = {
     "db200_conv2d_first_fwd_fma": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_conv2d_dgrad": [c_vp, ctypes.POINTER(ConvDesc), c_vp, c_vp, c_vp, c_vp, c_vp],
     "db200_conv2d_wgrad": [c_vp, ctypes.POINTER(ConvDesc), c_vp, c_vp, c_vp, c_vp],
-    "db200_rowmatmul_f32": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_conv7x7_in_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
+    "db200_conv7x7_in_wgrad": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_i64],
+    "db200_maxpool2x2_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_maxpool2x2_bwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_upsample2x_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_upsample2x_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_residual_gain": [c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp, c_i64, c_int],
+    "db200_rowmatmul_f32":[c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_rowmatmul_tn_f32": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_gumbel_softmax_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_int],
     "db200_gumbel_softmax_bwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
@@ -224,6 +231,7 @@ _WORKSPACE_QUERIES = {
     "db200_embed_bwd_workspace_bytes": [c_int, c_int],
     "db200_vae_kl_stats_workspace_bytes": [c_int, c_int],
     "db200_logit_laplace_workspace_bytes": [c_i64, c_int],
+    "db200_conv7x7_in_wgrad_workspace_bytes": [c_int, c_int, c_int, c_int, c_int],
 }
 EXPORTED_SYMBOLS = ["db200_last_error", "db200_launch_count"] + sorted(_SIGNATURES) + sorted(_WORKSPACE_QUERIES)
 

@@ -20,6 +20,7 @@ from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
 from .vae_engine import RECONSTRUCTION_LOSSES, VaeEngine, codebook_usage
+from .vae_paper_engine import PaperVaeEngine, check_paper_geometry
 
 TRAIN, EVAL, PREDICT = "train", "eval", "predict"   # tf.estimator.ModeKeys values
 
@@ -77,12 +78,7 @@ def load_vae_model(params, device):
     vae_params = params.get("vae_params")
     assert vae_params is not None, "vae model config must be supplied"        # model_fns.py:38
     D = params["dataset"]["image_size"]
-    convblocks = vae_params.get("convblocks") or [(3, 64), (3, 128), (3, 256)]
-    vae = VaeEngine(num_tokens=vae_params["num_tokens"], image_size=D, convblocks=convblocks,
-                    input_channels=vae_params.get("input_channels") or 3,
-                    use_bf16=bool(vae_params.get("use_bf16")),   # bf16 -> wgmma implicit-GEMM convolutions
-                    stack_factor=vae_params.get("stack_factor") or 1, device=device,
-                    reconstruction_loss=reconstruction_loss(vae_params.get("reconstruction_loss")))
+    vae = build_vae_engine(vae_params, D, device)
     return vae, vae_checkpoint(params)
 
 
@@ -424,6 +420,58 @@ def reconstruction_loss(value):
     return value
 
 
+VAE_ARCHITECTURES = ("reference", "dalle_paper")
+PAPER_VAE_DEFAULTS = {"n_hid": 256, "n_blk_per_group": 2, "group_count": 4, "n_init": 128}
+
+
+def vae_architecture(params, image_size):
+    """The network of a VAE config: None for the reference's (key architecture absent, null or "reference"), else the
+    geometry dict {n_hid, n_blk_per_group, group_count, n_init} of the DALL-E paper's ("dalle_paper"; absent keys
+    take PAPER_VAE_DEFAULTS).  Raises ValueError for any other architecture, for convblocks or stack_factor > 1 with
+    the paper's network, and for a geometry it does not define (PaperVaeEngine)."""
+    arch = params.get("architecture")
+    if arch is None or arch == "reference":
+        return None
+    if arch != "dalle_paper":
+        raise ValueError(f"architecture = {arch!r}: must be one of {VAE_ARCHITECTURES} (or null)")
+    if params.get("convblocks") is not None:
+        raise ValueError("convblocks describes the reference network; architecture \"dalle_paper\" is sized by n_hid, "
+                         "n_blk_per_group, group_count and n_init")
+    sf = params.get("stack_factor")
+    if sf is not None and sf != 1:
+        raise ValueError(f"stack_factor = {sf!r}: architecture \"dalle_paper\" takes no stack_factor > 1")
+    geo = {k: (d if params.get(k) is None else params[k]) for k, d in PAPER_VAE_DEFAULTS.items()}
+    check_paper_geometry(image_size, **geo)
+    return geo
+
+
+def vae_grid_size(params, image_size):
+    """Side of a VAE config's token grid: image_size / 2^(group_count - 1) for the paper's network, image_size /
+    stack_factor / 2^len(convblocks) for the reference's."""
+    geo = vae_architecture(params, image_size)
+    if geo is not None:
+        return image_size // 2 ** (geo["group_count"] - 1)
+    convblocks = params.get("convblocks") or [(3, 64), (3, 128), (3, 256)]
+    return image_size // (params.get("stack_factor") or 1) // (2 ** len(convblocks))
+
+
+def build_vae_engine(params, image_size, device, kl=False):
+    """The VAE engine of a VAE config (vae_architecture picks the network)."""
+    recon = reconstruction_loss(params.get("reconstruction_loss"))
+    geo = vae_architecture(params, image_size)
+    if geo is not None:
+        return PaperVaeEngine(num_tokens=params["num_tokens"], image_size=image_size,
+                              input_channels=params.get("input_channels") or 3, use_bf16=bool(params.get("use_bf16")),
+                              recompute_grad=bool(params.get("recompute_grad")), device=device, kl=kl,
+                              reconstruction_loss=recon, **geo)
+    return VaeEngine(num_tokens=params["num_tokens"], image_size=image_size,
+                     convblocks=params.get("convblocks") or [(3, 64), (3, 128), (3, 256)],
+                     input_channels=params.get("input_channels") or 3,
+                     recompute_grad=bool(params.get("recompute_grad")),
+                     use_bf16=bool(params.get("use_bf16")),   # bf16 -> wgmma implicit-GEMM convolutions
+                     stack_factor=params.get("stack_factor") or 1, device=device, kl=kl, reconstruction_loss=recon)
+
+
 def vae_model_fn(features, labels, mode, params):
     """src/model_fns_tf.py:9-114.  features = labels = images f32 [B,H,W,C] in [-1,1].
 
@@ -440,6 +488,7 @@ def vae_model_fn(features, labels, mode, params):
     kl_on = kl_beta is not None
     recon_loss = reconstruction_loss(params.get("reconstruction_loss"))
     ll = recon_loss == "logit_laplace"
+    vae_architecture(params, params["dataset"]["image_size"])   # rejects an invalid network before any device work
     n_aux = 3 if ll else (2 if kl_on else 1)    # aux slots: [recon term, KL, image-space MSE]
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
@@ -447,12 +496,7 @@ def vae_model_fn(features, labels, mode, params):
     H = params["dataset"]["image_size"]                                       # model_fns_tf.py:13
     global_batch = params[f"{mode_str}_batch_size"]
     _, local_batch = dp.shard(global_batch)
-    model = VaeEngine(num_tokens=params["num_tokens"], image_size=H,
-                      convblocks=params.get("convblocks") or [(3, 64), (3, 128), (3, 256)],
-                      input_channels=params.get("input_channels") or 3,
-                      recompute_grad=bool(params.get("recompute_grad")), use_bf16=bool(params.get("use_bf16")),
-                      stack_factor=params.get("stack_factor") or 1, device=device, kl=kl_on,
-                      reconstruction_loss=recon_loss)
+    model = build_vae_engine(params, H, device, kl=kl_on)
     model.init_params(seed=params.get("seed") or 0)
     if dp.rank == 0:
         print_n_params(model.n_params())

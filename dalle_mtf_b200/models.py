@@ -8,8 +8,8 @@ from . import lib as L
 from .dalle_engine import DalleEngine
 from .model_fns import attention_layers, conv_kernel, dropout_rates, input_embedding, loss_weights, \
     validate_kl_weight
+from .model_fns import build_vae_engine, vae_architecture
 from .model_fns import reconstruction_loss as _reconstruction_loss
-from .vae_engine import VaeEngine
 
 
 class DALLE:
@@ -104,8 +104,9 @@ class DALLE:
 
 
 class DiscreteVAE:
-    def __init__(self, num_tokens, dimensions, convblocks, dim=512, hidden_dim=64, input_channels=3,
-                 recompute_grad=False, use_bf16=False, stack_factor=1, kl_loss_weight=None, reconstruction_loss=None):
+    def __init__(self, num_tokens, dimensions, convblocks=None, dim=512, hidden_dim=64, input_channels=3,
+                 recompute_grad=False, use_bf16=False, stack_factor=1, kl_loss_weight=None, reconstruction_loss=None,
+                 architecture=None, n_hid=None, n_blk_per_group=None, group_count=None, n_init=None):
         """kl_loss_weight (extension; None: the reference's objective): beta of the KL term, a finite real >= 0.  With
         it, forward(..., return_recon_loss=True) returns MSE + beta * KL, KL the mean over the batch's latent rows of
         KL(softmax(logits) || Uniform(K)), and leaves the device [2] (MSE, KL) in self.loss_parts.
@@ -113,8 +114,18 @@ class DiscreteVAE:
         reconstruction_loss (extension; None or "mse": the reference's MSE): "logit_laplace" makes the reconstruction
         term the mean logit-Laplace NLL; forward then returns the image-space output and, with return_recon_loss, the
         objective NLL (+ beta * KL), leaving the device (NLL, image-space MSE) or (NLL, image-space MSE, KL) in
-        self.loss_parts."""
+        self.loss_parts.
+
+        architecture (extension; None or "reference": the reference's network, sized by convblocks): "dalle_paper"
+        builds the DALL-E paper's network instead, sized by n_hid, n_blk_per_group, group_count and n_init (None:
+        256, 2, 4, 128); convblocks must then be None and stack_factor 1 (model_fns.vae_architecture)."""
         self.kl_loss_weight, _ = validate_kl_weight(kl_loss_weight)
+        cfg = {"architecture": architecture, "convblocks": convblocks, "stack_factor": stack_factor,
+               "n_hid": n_hid, "n_blk_per_group": n_blk_per_group, "group_count": group_count, "n_init": n_init,
+               "num_tokens": num_tokens, "input_channels": input_channels, "use_bf16": use_bf16,
+               "recompute_grad": recompute_grad, "reconstruction_loss": reconstruction_loss}
+        if vae_architecture(cfg, dimensions) is None and convblocks is None:
+            raise ValueError("DiscreteVAE: the reference network needs convblocks")
         self.reconstruction_loss = _reconstruction_loss(reconstruction_loss)
         self.loss_parts = None
         self.num_tokens, self.dim, self.hdim = num_tokens, dim, hidden_dim   # dim / hidden_dim have no effect (ref too)
@@ -122,9 +133,7 @@ class DiscreteVAE:
         self.convblocks = convblocks
         self.num_ch = input_channels
         self.stack_factor = stack_factor
-        self.engine = VaeEngine(num_tokens, dimensions, convblocks, input_channels, use_bf16, recompute_grad,
-                                stack_factor, kl=self.kl_loss_weight is not None,
-                                reconstruction_loss=self.reconstruction_loss)
+        self.engine = build_vae_engine(cfg, dimensions, "cuda", kl=self.kl_loss_weight is not None)
         self.engine.init_params(0)
         self._gen = torch.Generator(device=self.engine.device).manual_seed(1234)
 

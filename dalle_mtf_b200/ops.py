@@ -608,6 +608,88 @@ def conv2d_wgrad(c, x, dy, dw, dbias):
           "conv2d_wgrad")
 
 
+# the DALL-E paper's dVAE network (include/dalle_b200.h, K11p): activations NHWC, bf16 or f32 (all operands alike)
+def _act(t, name, *others):
+    """act_f32 flag of activation tensor t; every tensor in `others` must have its dtype."""
+    if t.dtype not in (BF16, F32):
+        raise L.DB200Error(f"{name}: activations must be bf16 or f32, got {t.dtype}")
+    for o in others:
+        _chk(o, t.dtype, name)
+    _chk(t, t.dtype, name)
+    return int(t.dtype == F32)
+
+
+def conv7x7_in_fwd(x_f32, w, bias, y):
+    """Encoder input conv: f32 image [N,H,W,C] (C <= 4) -> y [N,H,W,Cout] (bf16 or f32) = conv7x7(x, w) + bias
+    (SAME, stride 1), f32 FMAs of the f32 operands, the output rounded once."""
+    L.require_device()
+    _chk(x_f32, F32, "x"); _chk(w, F32, "w"); _chk(bias, F32, "bias")
+    N, H, W_, C = x_f32.shape
+    if tuple(w.shape) != (7, 7, C, y.shape[-1]) or tuple(y.shape[:3]) != (N, H, W_):
+        raise L.DB200Error(f"conv7x7_in_fwd: shapes x {tuple(x_f32.shape)} w {tuple(w.shape)} y {tuple(y.shape)}")
+    check(L.load().db200_conv7x7_in_fwd(stream_ptr(), ptr(x_f32), ptr(w), ptr(bias), ptr(y), N, H, W_, C,
+                                        y.shape[-1], _act(y, "y")), "conv7x7_in_fwd")
+    return y
+
+
+def conv7x7_in_wgrad(x_f32, dy, dw, dbias):
+    """dw [7,7,C,Cout] += the 7x7 input conv's kernel gradient, dbias [Cout] += sum dy (dbias may be None)."""
+    L.require_device()
+    _chk(x_f32, F32, "x"); _chk(dw, F32, "dw"); _chk(dbias, F32, "dbias")
+    N, H, W_, C = x_f32.shape
+    Cout = dy.shape[-1]
+    if tuple(dw.shape) != (7, 7, C, Cout) or tuple(dy.shape[:3]) != (N, H, W_):
+        raise L.DB200Error(f"conv7x7_in_wgrad: shapes x {tuple(x_f32.shape)} dy {tuple(dy.shape)} dw {tuple(dw.shape)}")
+    ws = L.workspace(L.load().db200_conv7x7_in_wgrad_workspace_bytes(N, H, W_, C, Cout))
+    check(L.load().db200_conv7x7_in_wgrad(stream_ptr(), ptr(x_f32), ptr(dy), ptr(dw), ptr(dbias), N, H, W_, C, Cout,
+                                          _act(dy, "dy"), ptr(ws), _nbytes(ws)), "conv7x7_in_wgrad")
+
+
+def maxpool2x2_fwd(x, y):
+    """y [N,H/2,W/2,C] = 2x2 stride-2 max-pool of x [N,H,W,C]."""
+    L.require_device()
+    N, H, W_, C = x.shape
+    check(L.load().db200_maxpool2x2_fwd(stream_ptr(), ptr(x), ptr(y), N, H, W_, C, _act(x, "maxpool2x2_fwd", y)),
+          "maxpool2x2_fwd")
+    return y
+
+
+def maxpool2x2_bwd(x, dy, dx):
+    """dx [N,H,W,C] = dy at each window's first maximum of x (raster order), 0 elsewhere."""
+    L.require_device()
+    N, H, W_, C = x.shape
+    check(L.load().db200_maxpool2x2_bwd(stream_ptr(), ptr(x), ptr(dy), ptr(dx), N, H, W_, C,
+                                        _act(x, "maxpool2x2_bwd", dy, dx)), "maxpool2x2_bwd")
+    return dx
+
+
+def upsample2x_fwd(x, y):
+    """y [N,2H,2W,C] = nearest-neighbour 2x upsampling of x [N,H,W,C]."""
+    L.require_device()
+    N, H, W_, C = x.shape
+    check(L.load().db200_upsample2x_fwd(stream_ptr(), ptr(x), ptr(y), N, H, W_, C, _act(x, "upsample2x_fwd", y)),
+          "upsample2x_fwd")
+    return y
+
+
+def upsample2x_bwd(dy, dx):
+    """dx [N,H,W,C] = the f32 sum of each 2x2 block of dy [N,2H,2W,C]."""
+    L.require_device()
+    N, H, W_, C = dx.shape
+    check(L.load().db200_upsample2x_bwd(stream_ptr(), ptr(dy), ptr(dx), N, H, W_, C, _act(dx, "upsample2x_bwd", dy)),
+          "upsample2x_bwd")
+    return dx
+
+
+def residual_gain(r, gain=1.0, id=None, mask=None, y=None, relu_y=None):
+    """v = gain * r + id (id None: gain * r), 0 where mask <= 0; y = v (activation dtype), relu_y = max(y, 0)."""
+    L.require_device()
+    act = _act(r, "residual_gain", id, mask, y, relu_y)
+    check(L.load().db200_residual_gain(stream_ptr(), ptr(id), ptr(r), ptr(mask), float(gain), ptr(y), ptr(relu_y),
+                                       r.numel(), act), "residual_gain")
+    return y if y is not None else relu_y
+
+
 def rowmatmul(a, b, out, rows, K, N, b_transposed=False, accumulate=False):
     L.require_device()
     check(L.load().db200_rowmatmul_f32(stream_ptr(), ptr(a), ptr(b), ptr(out), rows, K, N, int(b_transposed),

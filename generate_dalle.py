@@ -18,7 +18,8 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
-from dalle_mtf_b200.model_fns import attention_layers, conv_kernel, input_embedding, vae_checkpoint
+from dalle_mtf_b200.model_fns import attention_layers, conv_kernel, input_embedding, vae_checkpoint, \
+    vae_grid_size
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
 PADDING_ID = 50257   # GPT-2 vocabulary + <|padding|> (src/data/tokenizer_utils.py), what training pads captions with
@@ -116,10 +117,9 @@ def encode_captions(lines, tokenizer, text_seq_len, text_vocab_size, pad=PADDING
 
 
 def token_grid_side(params):
-    """Side of the VAE's token grid: image_size / stack_factor / 2^len(convblocks)."""
-    vp = params["vae_params"]
-    convblocks = vp.get("convblocks") or [(3, 64), (3, 128), (3, 256)]
-    return params["dataset"]["image_size"] // (vp.get("stack_factor") or 1) // (2 ** len(convblocks))
+    """Side of the VAE's token grid: image_size / 2^(group_count - 1) for the DALL-E paper's network, image_size /
+    stack_factor / 2^len(convblocks) for the reference's."""
+    return vae_grid_size(params["vae_params"], params["dataset"]["image_size"])
 
 
 def prefix_length(params, prompt_rows):

@@ -375,6 +375,45 @@ int db200_conv2d_wgrad(db200_stream_t stream, const db200_conv_desc* c, const vo
                        float* dbias_or_null);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * K11p  the DALL-E paper's discrete-VAE network (extension, architecture "dalle_paper"; the reference has none): the
+ *     pieces its encoder and decoder need beyond K11's convolutions.  NHWC activations, bf16 (act_f32 = 0) or f32
+ *     (act_f32 = 1); 64-bit element counts and offsets throughout.
+ *   conv7x7_in_fwd:   the encoder's input conv, y = conv7x7(x, w, stride 1, SAME) + bias, x the f32 image [N][H][W][C]
+ *                     (1 <= C <= 4), w f32 [7][7][C][Cout], y [N][H][W][Cout] (Cout % 8 == 0; bf16 or f32).
+ *                     Precision: the products and sums are f32 FMAs of the f32 image and the f32 kernel (no bf16
+ *                     rounding of either operand, 49 C taps in kh, kw, c order); only the stored output is rounded.
+ *   conv7x7_in_wgrad: dw [7][7][C][Cout] += sum over pixels of x[p + tap] dy[p], dbias [Cout] += sum dy (dbias may be
+ *                     NULL); dy bf16 or f32.  Per-CTA partials go through the workspace and are added in a fixed
+ *                     order: bit-reproducible.  The image's own gradient is never needed and has no kernel.
+ *   maxpool2x2_fwd:   y[n][i][j][c] = max of x[n][2i + a][2j + b][c] over the window, H and W even.
+ *   maxpool2x2_bwd:   dx = dy at the window's FIRST maximum in raster order (0,0), (0,1), (1,0), (1,1) (a later
+ *                     element wins only if strictly greater), 0 at the other three; every dx element is written.  The
+ *                     arg-max is recomputed from x (no index tensor).  A NaN only wins as the window's first element.
+ *   upsample2x_fwd:   y[n][2i + a][2j + b][c] = x[n][i][j][c] (nearest neighbour); x is [N][H][W][C].
+ *   upsample2x_bwd:   dx[n][i][j][c] = ((dy(0,0) + dy(0,1)) + dy(1,0)) + dy(1,1), summed in f32, rounded once.
+ *   residual_gain:    v = gain * r + id (one f32 FMA; id NULL: gain * r), then v = 0 where mask <= 0 (mask NULL: no
+ *                     mask); y = v rounded to the activation type, relu_y = max(y, 0).  Either output may be NULL,
+ *                     not both; y may alias r or id.  A residual block's output x + gain (conv_4 + bias) with the
+ *                     ReLU its successor reads, the ReLU alone (id NULL, gain 1), the gradient of the gain-scaled
+ *                     path (gain dy) and the ReLU's backward (mask = the ReLU's input).
+ * Unsupported geometry (odd H or W for the pool, C outside [1, 4] or Cout % 8 != 0 for the 7x7 conv) returns
+ * DB200_E_UNSUPPORTED; there is no fallback.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int db200_conv7x7_in_fwd(db200_stream_t stream, const float* x, const float* w, const float* bias_or_null, void* y,
+                         int N, int H, int W, int C, int Cout, int act_f32);
+int db200_conv7x7_in_wgrad(db200_stream_t stream, const float* x, const void* dy, float* dw, float* dbias_or_null,
+                           int N, int H, int W, int C, int Cout, int act_f32, void* workspace,
+                           int64_t workspace_bytes);
+int64_t db200_conv7x7_in_wgrad_workspace_bytes(int N, int H, int W, int C, int Cout);
+int db200_maxpool2x2_fwd(db200_stream_t stream, const void* x, void* y, int N, int H, int W, int C, int act_f32);
+int db200_maxpool2x2_bwd(db200_stream_t stream, const void* x, const void* dy, void* dx, int N, int H, int W, int C,
+                         int act_f32);
+int db200_upsample2x_fwd(db200_stream_t stream, const void* x, void* y, int N, int H, int W, int C, int act_f32);
+int db200_upsample2x_bwd(db200_stream_t stream, const void* dy, void* dx, int N, int H, int W, int C, int act_f32);
+int db200_residual_gain(db200_stream_t stream, const void* id_or_null, const void* r, const void* mask_or_null,
+                        float gain, void* y_or_null, void* relu_y_or_null, int64_t n, int act_f32);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * K12/K13  codebook matmul + Gumbel-softmax + argmax  (src/vae_tf/models.py:111-120,124-127; src/vae_tf/layers.py:4-21;
  *          src/model_fns.py:76).  All f32, rows = N*h*w positions, K codes.
  *   rowmatmul:        out[r][n] = sum_k a[r][k] * b[k][n]   (or b^T) — small-K f32 matmul used for the codebook

@@ -7,8 +7,8 @@
 //   warps 4-11 : two MMA warpgroups.  Warpgroup g issues wgmma m64 x BN x 16 for rows [64g, 64g+64) of the tile and at
 //                the end of the tile writes its accumulators to a shared-memory accumulator tile.
 //   warps 12-15: the epilogue warpgroup.  Warp e owns rows [32e, 32e+32) of the accumulator tile, one row per thread,
-//                and runs the epilogue on it half tile by half tile -> bias / ReLU / residual / split-K reduction /
-//                cross-entropy statistics and gradient.
+//                and runs the epilogue on it half tile by half tile -> bias / ReLU / GELU / residual / split-K
+//                reduction / cross-entropy statistics and gradient.
 //
 // The accumulator tile is single-buffered and handed over through two named barriers (FULL: written by the MMA
 // warpgroups; EMPTY: read by the epilogue).  The MMA warpgroups run the next tile's mainloop while the epilogue works
@@ -43,8 +43,10 @@ static_assert(128 * G_REGS_PRODUCER + 256 * G_REGS_MMA + 128 * G_REGS_EPI <= 655
 constexpr int G_BAR_FULL = 1, G_BAR_EMPTY = 2, G_BAR_HANDOFF_THREADS = 384;
 
 // operand majors (1 = MN-major), compile-time for wgmma; DROP: dropout in the STORE epilogue; WCE: the weighted CE_GRAD
-// epilogue (instantiated for the vocabulary product only: A K-major, B MN-major)
-template <int TA, int TB, bool DROP, bool WCE = false>
+// epilogue (instantiated for the vocabulary product only: A K-major, B MN-major); GELU: the GELU MLP's epilogues,
+// G_GELU_FWD (the W1 forward: A K-major, B MN-major) or G_GELU_BWD (its dgrad: both K-major)
+constexpr int G_GELU_FWD = 1, G_GELU_BWD = 2;
+template <int TA, int TB, bool DROP, bool WCE = false, int GELU = 0>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr int BN = GBN;
@@ -189,6 +191,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           epi_ce_grad_weighted<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane);
           continue;
         }
+        if constexpr (GELU == G_GELU_FWD) {
+          epi_gelu_store<CH>(p, t_addr, cbase, stg, row0, lane);
+          continue;
+        }
+        if constexpr (GELU == G_GELU_BWD) {
+          epi_gelu_bwd<CH>(p, t_addr, cbase, stg, row0, lane);
+          continue;
+        }
         switch (p.mode) {
           case DB200_EPI_STORE:    epi_store<CH, DROP>(p, t_addr, row, row_ok, cbase, stg, row0, lane); break;
           case DB200_EPI_ATOMIC:
@@ -206,15 +216,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
-template <int TA, int TB, bool DROP, bool WCE = false>
+template <int TA, int TB, bool DROP, bool WCE = false, int GELU = 0>
 static int launch_gemm(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP, WCE>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP, WCE, GELU>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                           (int)G_SMEM_BYTES);  // once, thread-safe (magic static)
   DB200_CUDA(attr_rc);
   const int total = p.m_tiles * p.n_tiles * p.splits;
   const int grid = total < sm_count() ? total : sm_count();
-  gemm_tc_kernel<TA, TB, DROP, WCE><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_tc_kernel<TA, TB, DROP, WCE, GELU><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
   return check_launch("gemm_tc_kernel");
 }
 
@@ -257,10 +267,13 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
   return db200_gemm_bf16_ex(stream_, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr);
 }
 
-// every product: cew != NULL selects the weighted CE_GRAD epilogue (validated by db200_gemm_bf16_ce_weighted)
+// every product: cew != NULL selects the weighted CE_GRAD epilogue (validated by db200_gemm_bf16_ce_weighted), gelu the
+// GELU MLP's store (G_GELU_FWD, pre-activation output z / ldz) or dgrad (G_GELU_BWD) epilogue (validated by
+// db200_gemm_bf16_gelu / db200_gemm_bf16_gelu_bwd)
 static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
                     int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi,
-                    const db200_dropout* dropout, const db200_ce_weights* cew) {
+                    const db200_dropout* dropout, const db200_ce_weights* cew, int gelu = 0, void* z = nullptr,
+                    int64_t ldz = 0) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   DB200_REQUIRE(epi != nullptr, DB200_E_INVALID, "gemm: epilogue descriptor is NULL");
   const bool drop = dropout_active(dropout);
@@ -332,6 +345,8 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   p.colsum = (mode == DB200_EPI_CE_GRAD || mode == DB200_EPI_RELU_BWD) ? epi->colsum : nullptr;
   p.drop = drop ? *dropout : db200_dropout{};
   p.cew = cew ? *cew : db200_ce_weights{};
+  p.zout = reinterpret_cast<bf16*>(z);
+  p.ldz = ldz;
 
   p.n_tiles = (N + GBN - 1) / GBN;
   p.n_parts = 2 * p.n_tiles;
@@ -370,7 +385,13 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   } else if (colsum_out) {
     p.colsum = static_cast<float*>(epi->workspace);
   }
-  if (cew)     // the vocabulary product: A k-major, B mn-major
+  if (gelu == G_GELU_FWD)   // the MLP's W1 forward: A k-major, B mn-major
+    rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, false, G_GELU_FWD>(stream, tmA, tmB, p)
+                             : set_error(DB200_E_UNSUPPORTED, "gemm_gelu: needs a k-major A and an mn-major B");
+  else if (gelu == G_GELU_BWD)   // its dgrad dH = dbranch W2^T: both k-major
+    rc = (!p.a_mn && !p.b_mn) ? launch_gemm<0, 0, false, false, G_GELU_BWD>(stream, tmA, tmB, p)
+                              : set_error(DB200_E_UNSUPPORTED, "gemm_gelu_bwd: needs k-major A and B");
+  else if (cew)     // the vocabulary product: A k-major, B mn-major
     rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, true>(stream, tmA, tmB, p)
                              : set_error(DB200_E_UNSUPPORTED, "gemm: weighted CE_GRAD needs a k-major A and an mn-major B");
   else if (drop)    // residual dropout runs in forward products only: A k-major, B mn-major
@@ -398,4 +419,26 @@ extern "C" int db200_gemm_bf16_ce_weighted(db200_stream_t stream, const void* A,
   const int rc = ce_weights_check(w, "gemm_ce_weighted");
   if (rc != DB200_OK) return rc;
   return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, w);
+}
+
+extern "C" int db200_gemm_bf16_gelu(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                                    int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                                    const db200_gemm_epilogue* epi, void* z, int64_t ldz) {
+  DB200_REQUIRE(epi != nullptr && epi->mode == DB200_EPI_STORE, DB200_E_INVALID,
+                "gemm_gelu: needs an epilogue descriptor with mode DB200_EPI_STORE");
+  DB200_REQUIRE(!epi->out_f32 && !epi->relu && !epi->residual, DB200_E_INVALID,
+                "gemm_gelu: bf16 output only, without relu or a residual");
+  if (z) DB200_REQUIRE(aligned16(z) && ldz % 8 == 0 && ldz >= N, DB200_E_ALIGN,
+                       "gemm_gelu: z must be 16-byte aligned with ldz %% 8 == 0 and ldz >= N (got ldz=%lld)",
+                       (long long)ldz);
+  return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, nullptr, G_GELU_FWD,
+                  z, z ? ldz : 0);
+}
+
+extern "C" int db200_gemm_bf16_gelu_bwd(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda,
+                                        const void* B, int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N,
+                                        int K, const db200_gemm_epilogue* epi) {
+  DB200_REQUIRE(epi != nullptr && epi->mode == DB200_EPI_RELU_BWD, DB200_E_INVALID,
+                "gemm_gelu_bwd: needs an epilogue descriptor with mode DB200_EPI_RELU_BWD (aux = z)");
+  return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, nullptr, G_GELU_BWD);
 }

@@ -39,6 +39,8 @@ struct GemmParams {
   float* colsum;  // CE_GRAD / RELU_BWD: workspace [M/32 row blocks][N] of column sums (bias gradient), or NULL
   db200_dropout drop;  // STORE with dropout (kernel instantiated with DROP = true): elementwise mask over [M][N]
   db200_ce_weights cew;  // weighted CE_GRAD (kernel instantiated with WCE = true): per-row class coefficients and z
+  bf16* zout;            // GELU store: pre-activation z [M][ldz] (bf16), or NULL (inference: only h is written)
+  long long ldz;
 };
 
 struct TileCoord {
@@ -361,6 +363,103 @@ __device__ __forceinline__ void epi_relu_bwd(const GemmParams& p, uint32_t t_add
     stage_flush<2>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
   }
   (void)row; (void)row_ok;
+}
+
+// mtf's tanh GELU: gelu(x) = 0.5 x (1 + tanh(u)) = x s with s = sigma(2u) = 1 / (1 + 2^(-2 log2(e) u)) and
+// u = sqrt(2/pi) (x + 0.044715 x^3).  ex2.approx and rcp.approx keep s within a few fp32 ulps *relative* over the whole
+// range (tanh.approx's absolute error of ~2^-11 would be a large relative error in the negative tail); an exponent
+// argument t carries a relative error of ~|t| ln2 2^-24 into s.  Where 1 + 2^t overflows or rcp underflows (z below
+// about -10.1, where |gelu| < 2^-126 |z|), s is 0 and h is (-)0.  Large |x| overflows x^3 to +-inf, which gives s = 1
+// or 0 exactly: finite z always yields a finite h.  +inf -> +inf; -inf and NaN -> NaN.
+constexpr float kGeluA = 0.044715f;
+constexpr float kGeluC2 = 1.5957691216057308f;    // 2 sqrt(2/pi)
+constexpr float kGeluT = -2.3022082088626627f;    // -2 log2(e) sqrt(2/pi)
+__device__ __forceinline__ float fast_rcp(float x) {
+  float y;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ float gelu_s(float x) {
+  return fast_rcp(1.f + fast_exp2(kGeluT * fmaf(kGeluA * x, x * x, x)));
+}
+// gelu'(x) = s + x s (1 - s) 2 sqrt(2/pi) (1 + 3 * 0.044715 x^2).  Where s is exactly 0 or 1, s (1 - s) = 0 and the
+// result is exactly s (no 0 * inf from the overflowing x^2 term); 0 * x turns +-inf into NaN, as torch's float64 does.
+__device__ __forceinline__ float gelu_grad(float x) {
+  const float s = gelu_s(x);
+  const float q = s * (1.f - s);
+  return q == 0.f ? fmaf(0.f, x, s) : fmaf(x * q, kGeluC2 * fmaf(3.f * kGeluA, x * x, 1.f), s);
+}
+
+// GELU forward store: z = bf16(alpha acc + bias) is staged (and written to zout when it is given), read back as the
+// rounded value and replaced in place by h = bf16(gelu(z)) evaluated in fp32, which goes to D.
+template <int CH>
+__device__ __forceinline__ void epi_gelu_store(const GemmParams& p, uint32_t t_addr, int cbase, uint32_t stg, int row0,
+                                               int lane) {
+#pragma unroll 1
+  for (int pc = 0; pc < CH / 2; ++pc) {
+    const int colp = cbase + pc * 64;
+    if (colp >= p.N) break;  // warp-uniform
+    uint32_t rr2[2][32];
+    acc_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
+    acc_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int col0 = colp + h * 32;
+      float o[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) o[j] = __uint_as_float(rr2[h][j]) * p.alpha;
+      if (p.bias && col0 + 32 <= p.N) {
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          float b[8];
+          load8(p.bias + col0 + g * 8, b);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[g * 8 + j] += b[j];
+        }
+      } else if (p.bias) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+          if (col0 + j < p.N) o[j] += __ldg(p.bias + col0 + j);
+      }
+      stage_put_bf16(stg, lane, h, o);
+    }
+    if (p.zout) stage_flush<2>(stg, p.zout, p.ldz, row0, colp, p.M, p.N, lane);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float z[32];
+      stage_get_bf16(stg, lane, h, z);  // this lane's own row: no exchange between lanes
+#pragma unroll
+      for (int j = 0; j < 32; ++j) z[j] *= gelu_s(z[j]);
+      stage_put_bf16(stg, lane, h, z);
+    }
+    stage_flush<2>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
+  }
+}
+
+// GELU backward (dgrad of the MLP's first product): dZ = bf16(alpha acc * gelu'(z)), z read from aux; fused column
+// sums as in RELU_BWD.  Rows and columns past the matrix read z = 0 and acc = 0, so they stage zeros.
+template <int CH>
+__device__ __forceinline__ void epi_gelu_bwd(const GemmParams& p, uint32_t t_addr, int cbase, uint32_t stg, int row0,
+                                             int lane) {
+#pragma unroll 1
+  for (int pc = 0; pc < CH / 2; ++pc) {
+    const int colp = cbase + pc * 64;
+    if (colp >= p.N) break;
+    uint32_t rr2[2][32];
+    acc_ld_x32(t_addr + (pc * 2) * 32, rr2[0]);
+    acc_ld_x32(t_addr + (pc * 2 + 1) * 32, rr2[1]);
+    stage_fetch_bf16(stg, p.aux, p.ldaux, row0, colp, p.M, p.N, lane);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float o[32];
+      stage_get_bf16(stg, lane, h, o);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) o[j] = __uint_as_float(rr2[h][j]) * p.alpha * gelu_grad(o[j]);
+      stage_put_bf16(stg, lane, h, o);  // in place: this lane overwrites the slots it just read
+    }
+    if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, lane);
+    stage_flush<2>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
+  }
 }
 
 // per (row, half-tile): running max and sum exp of (acc + bias) over the valid vocabulary columns; label logit

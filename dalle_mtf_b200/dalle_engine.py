@@ -211,6 +211,17 @@ def loss_coefficients(loss_weights, text_seq_len, image_seq_len, global_batch):
     return a_text, wi / ((wt + wi) * global_batch * n_image)
 
 
+ACTIVATIONS = ("relu", "gelu")
+
+
+def validate_activation(activation):
+    """The MLP nonlinearity: "relu" (the reference's default, mtf.relu) or "gelu" (mtf's tanh GELU); anything else
+    (other spellings, booleans, numbers) is a ValueError."""
+    if not isinstance(activation, str) or activation not in ACTIVATIONS:
+        raise ValueError(f"activation must be one of {ACTIVATIONS}, got {activation!r}")
+    return activation
+
+
 class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
@@ -220,7 +231,8 @@ class DalleEngine:
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
-                 conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False):
+                 conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
+                 activation="relu"):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -252,7 +264,14 @@ class DalleEngine:
         per_position_padding: the text vocabulary grows by text_seq_len padding tokens, token text_vocab_size + p
         being text position p's pad (pad_base = text_vocab_size), and image code i becomes token image_offset + i with
         image_offset = text_vocab_size + text_seq_len (otherwise text_vocab_size).  Captions are mapped by
-        ops.assemble_tokens_pp."""
+        ops.assemble_tokens_pp.
+
+        activation: the MLP nonlinearity (validate_activation).  "gelu" makes the MLP gelu(LN2(x) W1 + b1) W2 + b2 with
+        mtf's tanh GELU, fused into the W1 product's epilogue (which also keeps the pre-activation z for backward: one
+        more bf16 [T, 4d] per saved layer) and into its dgrad's; no parameter changes."""
+        self.activation = validate_activation(activation)
+        self.gelu = self.activation == "gelu"
+        self.mlp_act = {"gelu": True} if self.gelu else {"relu": True}   # linear_fwd keywords of an inference W1
         self.row_col = validate_position_embedding(image_position_embedding) == "row_col"
         self.grid_w = image_grid_side(image_seq_len) if self.row_col else None
         self.per_position_padding = validate_per_position_padding(per_position_padding)
@@ -589,7 +608,7 @@ class DalleEngine:
                 "ln1": e(T, d), "mean1": e(T, dtype=F32), "rstd1": e(T, dtype=F32),
                 "qkv": e(T, 3 * d), "attn": e(T, d), "lse": e(B, self.H, S, dtype=F32),
                 "xmid": e(T, d), "ln2": e(T, d), "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32),
-                "h1": e(T, 4 * d),
+                "h1": e(T, 4 * d), **({"z1": e(T, 4 * d)} if self.gelu else {}),
             } for _ in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
             "labels": e(B, S, dtype=I32),
@@ -643,7 +662,11 @@ class DalleEngine:
                        dropout=self._site("attn_out", i))                               # :303-314,330
         ops.layernorm_fwd(sv["xmid"], self.P(p + "ln2_g"), self.P(p + "ln2_b"), sv["ln2"], sv["mean2"], sv["rstd2"],
                           self.ln_eps)
-        ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), relu=True)     # :320
+        if self.gelu:   # h1 = gelu(z1), z1 = LN2 W1 + b1 kept for backward (the prefill's sv has none: not written)
+            ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), gelu=True,
+                           z_out=sv.get("z1"))
+        else:
+            ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), relu=True)     # :320
         ops.linear_fwd(sv["h1"], self.W(p + "w2"), x_out, bias=self.P(p + "b2"), residual=sv["xmid"],
                        dropout=self._site("mlp_out", i))                                # :321-323,333
 
@@ -791,8 +814,11 @@ class DalleEngine:
         same for the layer below."""
         p = f"l{i}."
         # ---- MLP
-        ops.linear_dgrad(dbranch, self.W(p + "w2"), bufs["dh1"], relu_mask_of=sv["h1"],
-                         colsum=self.G(p + "b1"))                                       # dH = (dx W2^T)*[h1>0]; db1
+        if self.gelu:   # dZ = (dx W2^T) * gelu'(z1); db1
+            ops.linear_dgrad(dbranch, self.W(p + "w2"), bufs["dh1"], gelu_grad_of=sv["z1"], colsum=self.G(p + "b1"))
+        else:
+            ops.linear_dgrad(dbranch, self.W(p + "w2"), bufs["dh1"], relu_mask_of=sv["h1"],
+                             colsum=self.G(p + "b1"))                                   # dH = (dx W2^T)*[h1>0]; db1
         ops.linear_wgrad(sv["h1"], dbranch, self.G(p + "w2"))
         ops.linear_dgrad(bufs["dh1"], self.W(p + "w1"), bufs["dtmp"])                         # dLN2 out
         ops.linear_wgrad(sv["ln2"], bufs["dh1"], self.G(p + "w1"))

@@ -128,6 +128,10 @@ _SIGNATURES = {
                            ctypes.POINTER(GemmEpilogue), ctypes.POINTER(Dropout)],
     "db200_gemm_bf16_ce_weighted": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
                                     ctypes.POINTER(GemmEpilogue), ctypes.POINTER(CeWeights)],
+    "db200_gemm_bf16_gelu": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
+                             ctypes.POINTER(GemmEpilogue), c_vp, c_i64],
+    "db200_gemm_bf16_gelu_bwd": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
+                                 ctypes.POINTER(GemmEpilogue)],
     "db200_gemm_ce_tiles": [c_int],
     "db200_embed_fwd_at": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_attn_decode": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_f32],

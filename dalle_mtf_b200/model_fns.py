@@ -14,8 +14,8 @@ import torch
 
 from . import lib as L
 from . import ops
-from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_conv_kernel, validate_loss_weights, \
-    validate_per_position_padding, validate_position_embedding
+from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
+    validate_loss_weights, validate_per_position_padding, validate_position_embedding
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -141,6 +141,17 @@ def attention_layers(params):
     return types, radius
 
 
+def activation_function(params):
+    """The MLP nonlinearity of a DALL-E config, GPT-Neo's key activation_function: absent, null or "relu" is the
+    reference's ReLU, "gelu" mtf's tanh GELU (DalleEngine).  Any other value (other spellings such as "GELU",
+    "swish", booleans, numbers) is rejected.  No parameter depends on it, so checkpoints keep their layout."""
+    v = params.get("activation_function")
+    try:
+        return validate_activation("relu" if v is None else v)
+    except ValueError:
+        raise ValueError(f"activation_function = {v!r}: expected null, \"relu\" or \"gelu\"") from None
+
+
 def conv_kernel(params):
     """conv_attention_kernel of a DALL-E config: the k of "conv" layers' k x k window (DalleEngine), an integer >= 1.
     A missing or null key is 5, DALLE-pytorch's default."""
@@ -207,6 +218,7 @@ def dalle_model_fn(features, labels, mode, params):
     conv_k = conv_kernel(params)
     weights, z_loss = loss_weights(params)
     pos_scheme, per_pos, pp_pad = input_embedding(params)
+    activation = activation_function(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -239,7 +251,8 @@ def dalle_model_fn(features, labels, mode, params):
                         dropout=rates, dropout_seed=params.get("seed") or 0,
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
-                        image_position_embedding=pos_scheme, per_position_padding=per_pos)
+                        image_position_embedding=pos_scheme, per_position_padding=per_pos,
+                        activation=activation)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

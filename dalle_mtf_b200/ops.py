@@ -46,13 +46,16 @@ def _nbytes(ws):
 
 def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=None, mode=L.EPI_STORE,
          alpha=1.0, bias=None, relu=False, residual=None, aux=None, split_k=1, labels=None, part_max=None,
-         part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None, dropout=None, ce_weights=None):
+         part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None, dropout=None, ce_weights=None, gelu=None,
+         z=None):
     """D[M,N] = A[M,K] @ B[K,N] on wgmma.  a_mn / b_mn: operand is stored with M (resp. N) contiguous.
 
     a: [M,K] (k-major) or [K,M] (mn-major);  b: [N,K] (k-major) or [K,N] (mn-major).
     dropout (lib.Dropout, STORE only): D = residual + keep * scale * act(alpha * acc + bias).
     ce_weights (lib.CeWeights, CE_GRAD only, a k-major / b mn-major): the weighted CE_GRAD epilogue, which takes its
     per-row coefficients from the descriptor instead of alpha.
+    gelu "fwd" (STORE, a k-major / b mn-major): D = gelu(bf16(alpha * acc + bias)), and z (bf16, or None) receives the
+    rounded pre-activation; gelu "bwd" (RELU_BWD, both k-major): D = alpha * acc * gelu'(aux), aux = the stored z.
     """
     L.require_device()
     _chk(a, BF16, "gemm A")
@@ -78,6 +81,9 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     e.part_max, e.part_sum, e.label_logit, e.lse = ptr(part_max), ptr(part_sum), ptr(label_logit), ptr(lse)
     e.n_valid = n_valid
     _chk(colsum, F32, "gemm colsum")
+    _chk(z, BF16, "gemm z")
+    if z is not None and gelu != "fwd":
+        raise L.DB200Error("gemm: a pre-activation output needs the GELU forward epilogue")
     e.colsum = ptr(colsum)
     if out is not None:
         if mode == L.EPI_ATOMIC:
@@ -91,7 +97,16 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-    if ce_weights is not None:
+    if gelu == "fwd":
+        check(L.load().db200_gemm_bf16_gelu(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out),
+                                            ldd, M, N, K, ctypes.byref(e), ptr(z), z.stride(0) if z is not None else 0),
+              "db200_gemm_bf16_gelu")
+    elif gelu == "bwd":
+        check(L.load().db200_gemm_bf16_gelu_bwd(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out),
+                                                ldd, M, N, K, ctypes.byref(e)), "db200_gemm_bf16_gelu_bwd")
+    elif gelu is not None:
+        raise ValueError(f"gemm: gelu must be None, 'fwd' or 'bwd', got {gelu!r}")
+    elif ce_weights is not None:
         check(L.load().db200_gemm_bf16_ce_weighted(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb,
                                                    ptr(out), ldd, M, N, K, ctypes.byref(e), ctypes.byref(ce_weights)),
               "db200_gemm_bf16_ce_weighted")
@@ -107,17 +122,32 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     return out
 
 
-def linear_fwd(x, w, out, bias=None, relu=False, residual=None, dropout=None):
-    """out[T,N] = dropout(act(x[T,K] @ w[K,N] + bias)) + residual      (forward: A k-major, B mn-major)."""
+def linear_fwd(x, w, out, bias=None, relu=False, residual=None, dropout=None, gelu=False, z_out=None):
+    """out[T,N] = dropout(act(x[T,K] @ w[K,N] + bias)) + residual      (forward: A k-major, B mn-major).
+
+    gelu: out = gelu(z) with z = bf16(x @ w + bias) (mtf's tanh GELU, no residual or dropout); z_out [T,N] bf16
+    receives z for the backward, or is None (inference)."""
     T, K = x.shape
     N = w.shape[1]
+    if gelu:
+        if relu or residual is not None or dropout is not None:
+            raise L.DB200Error("linear_fwd: the GELU epilogue takes no relu, residual or dropout")
+        return gemm(x, w, out, T, N, K, a_mn=False, b_mn=True, bias=bias, gelu="fwd", z=z_out)
+    if z_out is not None:
+        raise L.DB200Error("linear_fwd: z_out needs gelu=True")
     return gemm(x, w, out, T, N, K, a_mn=False, b_mn=True, bias=bias, relu=relu, residual=residual, dropout=dropout)
 
 
-def linear_dgrad(dy, w, out, relu_mask_of=None, colsum=None):
-    """out[T,K] = dy[T,N] @ w[K,N]^T  (optionally masked by relu_mask_of > 0; colsum[k] += sum_t out[t,k])."""
+def linear_dgrad(dy, w, out, relu_mask_of=None, colsum=None, gelu_grad_of=None):
+    """out[T,K] = dy[T,N] @ w[K,N]^T  (optionally masked by relu_mask_of > 0, or multiplied by gelu'(gelu_grad_of),
+    the stored pre-activation z; colsum[k] += sum_t out[t,k])."""
     T, N = dy.shape
     K = w.shape[0]
+    if relu_mask_of is not None and gelu_grad_of is not None:
+        raise L.DB200Error("linear_dgrad: relu_mask_of and gelu_grad_of are exclusive")
+    if gelu_grad_of is not None:
+        return gemm(dy, w, out, T, K, N, a_mn=False, b_mn=False, mode=L.EPI_RELU_BWD, aux=gelu_grad_of,
+                    colsum=colsum, gelu="bwd")
     if relu_mask_of is not None:
         return gemm(dy, w, out, T, K, N, a_mn=False, b_mn=False, mode=L.EPI_RELU_BWD, aux=relu_mask_of, colsum=colsum)
     return gemm(dy, w, out, T, K, N, a_mn=False, b_mn=False)

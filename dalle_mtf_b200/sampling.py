@@ -10,7 +10,8 @@ parameters and the same kernels' numerics as training:
   per layer:        q|k|v = LN1(x) Wqkv;  cache[p] = k, v;  a = softmax_{j<=p}(q.k_j) v_j   (attn_decode;
                     a local layer of radius r takes j > p - r only, models.py:257-273; an axial layer the text
                     positions and p's image row or column; a conv layer the text positions and p's k x k window)
-                    x = x + a Wo + o_b;  x = x + relu(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows)
+                    x = x + a Wo + o_b;  x = x + act(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows;
+                    act = ReLU, or GELU without a pre-activation output)
   logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
 
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
@@ -98,7 +99,7 @@ class DalleSampler:
                             **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
-            ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), relu=True)
+            ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             ops.linear_fwd(self.h1, e.W(p + "w2"), x_out, bias=e.P(p + "b2"), residual=self.xmid)
             x_in, x_out = x_out, x_in
         ops.layernorm_fwd(x_in, e.P("lnf_g"), e.P("lnf_b"), self.ln, self.mean, self.rstd, e.ln_eps)
@@ -120,7 +121,7 @@ class DalleSampler:
                                 radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
-            ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), relu=True)
+            ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             ops.linear_fwd(self.h1, e.W(p + "w2"), x_out, bias=e.P(p + "b2"), residual=self.xmid)
             x_in, x_out = x_out, x_in
         ops.layernorm_fwd(x_in, e.P("lnf_g"), e.P("lnf_b"), self.ln, self.mean, self.rstd, e.ln_eps)

@@ -220,9 +220,27 @@ typedef struct db200_ce_weights {
 int db200_gemm_bf16_ce_weighted(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
                                 int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
                                 const db200_gemm_epilogue* epi, const db200_ce_weights* w);
+/* GELU MLP (extension; the reference's DALLE(activation_fn=...) hook, src/dalle_mtf/models.py:146,177-179,320).
+ * mtf's tanh GELU, gelu(x) = x sigma(2u) with u = sqrt(2/pi) (x + 0.044715 x^3), evaluated in fp32.
+ * Forward store (the W1 product): z = bf16(alpha*acc + bias[n]); D(bf16) = bf16(gelu(z)); z is also written to
+ *   z[M][ldz] (bf16) when z != NULL (training keeps it for backward; inference passes NULL).  epi->mode must be
+ *   DB200_EPI_STORE with out_f32 = 0, relu = 0 and no residual; A k-major and B mn-major (DB200_E_UNSUPPORTED
+ *   otherwise); N, ldd and ldz multiples of 8 and z 16-byte aligned (DB200_E_ALIGN).
+ * Backward (the dgrad dH = dbranch W2^T): D(bf16) = bf16(alpha*acc * gelu'(aux[m,n])) with aux = the stored z;
+ *   epi->mode must be DB200_EPI_RELU_BWD (aux, colsum and workspace exactly as for RELU_BWD, so
+ *   db200_gemm_workspace_bytes sizes its column-sum workspace); A and B k-major.
+ * Finite z gives finite h and gelu'; where sigma is exactly 0 or 1 in fp32, gelu' is exactly 0 or 1.  z = +inf gives
+ * h = +inf, z = -inf or NaN gives h = NaN; gelu' of a non-finite z is NaN. */
+int db200_gemm_bf16_gelu(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                         int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                         const db200_gemm_epilogue* epi, void* z, int64_t ldz);
+int db200_gemm_bf16_gelu_bwd(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                             int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                             const db200_gemm_epilogue* epi);
 /* number of N tiles the CE_STATS epilogue writes per row for a given N (host helper for sizing part_max/part_sum) */
 int db200_gemm_ce_tiles(int N);
-/* epi->workspace size for this product: split-K slices (ATOMIC) or fused column sums (CE_GRAD / RELU_BWD with colsum) */
+/* epi->workspace size for this product: split-K slices (ATOMIC) or fused column sums (CE_GRAD / RELU_BWD, which includes
+ * the GELU backward, with colsum) */
 int64_t db200_gemm_workspace_bytes(int M, int N, int K, const db200_gemm_epilogue* epi);
 
 /* ------------------------------------------------------------------------------------------------------------------

@@ -33,8 +33,9 @@ millions of outputs some lie within b * absref of a rounding midpoint, where the
 
 The wgmma convolutions run at the geometry of the two VAE configurations, at a batch chosen so that every launch has at
 least twice as many work tiles as the device has SMs (the persistent CTAs then walk several tiles each), and at edge
-geometries: ragged spatial sizes, several images packed into one tile, 64-wide and ragged channel tiles, and a wgrad
-with fewer pixel tiles than the split count the host rule asks for.
+geometries: ragged spatial sizes, several images packed into one tile, 64-wide and ragged channel tiles, 1x1 kernels
+(one k-block per tile at 64 input channels), and a wgrad with fewer pixel tiles than the split count the host rule
+asks for.  Each check also runs a mutated reference that must fail (run_conv).
 """
 import functools
 import json
@@ -147,14 +148,45 @@ def conv_refs(x, w, dy, stride, transposed):
     return out
 
 
-def run_conv(ops, tag, N, H, Cin, Cout, k, stride, transposed, *, dgrad=True, res_block=False, act_f32=False,
-             seed=0):
+FWD_VARIANTS = ("plain", "relu", "res")
+DGRAD_VARIANTS = ("plain", "mask", "dres", "dres in place", "mask dres in place")
+WGRAD_REL = 2.0 ** -12
+
+
+def must_fail(name, got, wrong_ref, absref, **bound):
+    """A reference with one deliberate mistake (a mutation) must be told apart from the kernel's output."""
+    r = float64_bounds.worst_ratio(name, got, wrong_ref, absref, **bound)
+    assert r >= 1.0, f"{name}: the mutated reference passes too (worst err/bound {r:.4f})"
+
+
+def _mask_operand(shape, g, dtype):
+    """A ReLU mask as the engine passes it: a post-ReLU activation or a block input, with exact zeros and
+    negatives (only > 0 keeps the gradient)."""
+    m = _randn(*shape, g=g, dtype=dtype)
+    m.view(-1)[::5] = 0
+    return m
+
+
+def run_conv(ops, tag, N, H, Cin, Cout, k, stride, transposed, *, dgrad=True, wgrad=True, res_block=False,
+             act_f32=False, seed=0, fwd_variants=None, dgrad_variants=None, line_tag="vae-kernels"):
     """Forward, dgrad and wgrad (+ bias gradient) of one convolution through the kernels VaeEngine picks for it,
     with the arguments the engine passes: a residual block's conv_in runs with the fused ReLU, its conv_out with the
     residual add; their dgrads with the ReLU mask (conv_out) and the residual gradient (conv_in), which the engine
-    reads from and writes to the same buffer (VaeEngine._res_bwd)."""
+    reads from and writes to the same buffer (VaeEngine._res_bwd).  PaperVaeEngine also passes the mask and the
+    in-place residual gradient in one launch (_block_bwd).  fwd_variants / dgrad_variants (names from FWD_VARIANTS /
+    DGRAD_VARIANTS) replace those sets by the ones an engine was seen to launch; wgrad=False skips the weight
+    gradient (a forward-only launch).
+
+    Every check also runs a mutated reference that must fail: the mask or the residual gradient dropped, a 1x1
+    output compared one pixel over, the weight gradient without its base."""
     g = _gen(seed)
     act = F32 if act_f32 else BF16
+    chk = functools.partial(float64_bounds.check, tag=line_tag)
+    if fwd_variants is None:
+        fwd_variants = ("relu", "res") if res_block else ("plain",)
+    if dgrad_variants is None:
+        dgrad_variants = ("mask", "dres", "dres in place", "mask dres in place") if res_block else ("plain",)
+    assert set(fwd_variants) <= set(FWD_VARIANTS) and set(dgrad_variants) <= set(DGRAD_VARIANTS)
     Ho = out_res(H, stride, transposed)
     wshape = (k, k, Cout, Cin) if transposed else (k, k, Cin, Cout)
     x = _randn(N, H, H, Cin, g=g, dtype=act)
@@ -179,10 +211,9 @@ def run_conv(ops, tag, N, H, Cin, Cout, k, stride, transposed, *, dgrad=True, re
     ratios = []
 
     # ---- forward
-    variants = [("", None, False)]
-    if res_block:
-        variants = [(" relu", None, True), (" +res", _randn(N, Ho, Ho, Cout, g=g, dtype=act), False)]
-    for label, res, relu in variants:
+    for label in fwd_variants:
+        relu = label == "relu"
+        res = _randn(N, Ho, Ho, Cout, g=g, dtype=act) if label == "res" else None
         y = nan_like((N, Ho, Ho, Cout), act)
         cc = c_relu if relu else c
         if fwd_tc:
@@ -196,34 +227,43 @@ def run_conv(ops, tag, N, H, Cin, Cout, k, stride, transposed, *, dgrad=True, re
         if res is not None:
             ref = ref + res.to(F64)
             absref = absref + res.abs().to(F64)
-        ratios.append(check(f"{tag} fwd{label} [{'wgmma' if fwd_tc else 'direct'} {kind}]", y, ref, absref,
-                            b=L_f * u_acc + 8 * U, bf16_out=not act_f32))
+        name = f"{tag} fwd {label} [{'wgmma' if fwd_tc else 'direct'} {kind}]"
+        bound = dict(b=L_f * u_acc + 8 * U, bf16_out=not act_f32)
+        ratios.append(chk(name, y, ref, absref, **bound))
+        if k == 1:
+            must_fail(name + " one pixel over", y, ref.roll(1, 2), absref.roll(1, 2), **bound)
 
     # ---- dgrad
-    if dgrad:
-        variants = [("", None, None, False)]
-        if res_block:
-            variants = [(" mask", _randn(N, H, H, Cin, g=g, dtype=act), None, False),
-                        (" +dres", None, _randn(N, H, H, Cin, g=g, dtype=act), False),
-                        (" +dres in place", None, _randn(N, H, H, Cin, g=g, dtype=act), True)]
-        for label, mask, dres, in_place in variants:
-            dx = dres.clone() if in_place else nan_like((N, H, H, Cin), act)
-            dres_arg = dx if in_place else dres
-            if dg_tc:
-                ops.conv2d_dgrad_tc(c, dy, w16, mask, dres_arg, dx)
-            else:
-                ops.conv2d_dgrad(c, dy, w, mask, dres_arg, dx)
-            ref, absref = dx64, dxa
-            if mask is not None:
-                keep = (mask > 0).to(F64)
-                ref, absref = ref * keep, absref * keep
-            if dres is not None:
-                ref, absref = ref + dres.to(F64), absref + dres.abs().to(F64)
-            ratios.append(check(f"{tag} dgrad{label} [{'wgmma' if dg_tc else 'direct'} {kind}]", dx, ref, absref,
-                                b=L_d * u_acc + 8 * U, bf16_out=not act_f32))
+    for label in dgrad_variants if dgrad else ():
+        mask = _mask_operand((N, H, H, Cin), g, act) if "mask" in label else None
+        dres = _randn(N, H, H, Cin, g=g, dtype=act) if "dres" in label else None
+        in_place = "in place" in label
+        dx = dres.clone() if in_place else nan_like((N, H, H, Cin), act)
+        dres_arg = dx if in_place else dres
+        if dg_tc:
+            ops.conv2d_dgrad_tc(c, dy, w16, mask, dres_arg, dx)
+        else:
+            ops.conv2d_dgrad(c, dy, w, mask, dres_arg, dx)
+        ref, absref = dx64, dxa
+        keep = (mask > 0).to(F64) if mask is not None else 1.0
+        add, add_abs = (dres.to(F64), dres.abs().to(F64)) if dres is not None else (0.0, 0.0)
+        name = f"{tag} dgrad {label} [{'wgmma' if dg_tc else 'direct'} {kind}]"
+        bound = dict(b=L_d * u_acc + 8 * U, bf16_out=not act_f32)
+        ratios.append(chk(name, dx, ref * keep + add, absref * keep + add_abs, **bound))
+        if mask is not None:
+            must_fail(name + " mask dropped", dx, ref + add, absref + add_abs, **bound)
+        if dres is not None:
+            must_fail(name + " dres dropped", dx, ref * keep, absref * keep, **bound)
 
-    # ---- wgrad + bias gradient, accumulated onto non-zero bases
-    base_w = _randn(*wshape, g=g, scale=math.sqrt(L_w))
+    # ---- wgrad + bias gradient, accumulated onto non-zero bases.  The componentwise bound grows as L_w while the
+    # gradient grows as sqrt(L_w): past L_w ~ 2^16 it exceeds the gradient itself.  So the base is made larger than the
+    # bound (a kernel that drops it still fails), and the gradient (dw - base) is also held to a relative Frobenius
+    # error of WGRAD_REL, which a lost pixel tile or split exceeds.
+    if not wgrad:        # a forward-only launch (the tokenizer)
+        return ratios
+    b_w = (L_w + 64) * u_acc + 8 * U
+    assert b_w < 0.5, (tag, L_w)
+    base_w = _randn(*wshape, g=g, scale=max(math.sqrt(L_w), 4 * b_w * float(dwa.max()) / (1 - b_w)))
     base_b = _randn(Cout, g=g, scale=math.sqrt(L_w))
     dw, db = base_w.clone(), base_b.clone()
     if wg_tc:
@@ -232,12 +272,15 @@ def run_conv(ops, tag, N, H, Cin, Cout, k, stride, transposed, *, dgrad=True, re
     else:
         ops.conv2d_wgrad(c, x, dy, dw, db)
     wlabel = "wgmma" if wg_tc else "direct"
-    ratios.append(check(f"{tag} wgrad [{wlabel} {kind}]", dw, base_w.to(F64) + dw64, base_w.abs().to(F64) + dwa,
-                        b=(L_w + 64) * u_acc + 8 * U))
+    name = f"{tag} wgrad [{wlabel} {kind}]"
+    ratios.append(chk(name, dw, base_w.to(F64) + dw64, base_w.abs().to(F64) + dwa, b=b_w))
+    must_fail(name + " without its base", dw, dw64, base_w.abs().to(F64) + dwa, b=b_w)
+    rel = ((dw.to(F64) - base_w.to(F64) - dw64).norm() / dw64.norm().clamp_min(1e-300)).item()
+    assert rel < WGRAD_REL, f"{name}: relative Frobenius error {rel:.3g} of dw - base"
     dy64 = dy.to(F64).reshape(-1, Cout)
-    ratios.append(check(f"{tag} dbias [{'colsum' if wg_tc else 'direct'} {kind}]", db,
-                        base_b.to(F64) + dy64.sum(0), base_b.abs().to(F64) + dy64.abs().sum(0),
-                        b=(L_w + 64) * 2 * U + 8 * U))
+    ratios.append(chk(f"{tag} dbias [{'colsum' if wg_tc else 'direct'} {kind}]", db,
+                      base_b.to(F64) + dy64.sum(0), base_b.abs().to(F64) + dy64.abs().sum(0),
+                      b=(L_w + 64) * 2 * U + 8 * U))
     return ratios
 
 
@@ -330,6 +373,10 @@ EDGE_GEOMETRIES = [
     (7, 4, 64, 64, 4, 2, True),        # conv-transpose from 4 px: eight images per tile, N = 7
     (1, 8, 64, 64, 3, 1, False),       # wgrad: one pixel tile, fewer than the splits the SM count asks for
     (3, 8, 128, 128, 4, 2, False),     # wgrad over 4 px outputs, 3 images per 8-image tile
+    (6, 16, 64, 256, 1, 1, False),     # 1x1, Cin 64: one k-block per tile, the stage ring wraps every four tiles
+    (3, 12, 192, 192, 1, 1, False),    # 1x1, 12 px; 192 channels: ragged last channel tile on both sides
+    (3, 32, 128, 64, 1, 1, False),     # 1x1 at 32 px (the token grid): 64-wide output channel tile
+    (13, 4, 64, 128, 1, 1, False),     # 1x1 at 4 px: eight images per tile, N = 13
 ]
 
 

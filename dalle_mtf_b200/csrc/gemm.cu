@@ -216,6 +216,177 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 }
 
+// ----------------------------------------------------------------------------------------------------------------------
+// The ping-pong kernel for short contractions (gemm_run picks it by K and epilogue).  With K <= 1024 a tile's mainloop
+// is at most 16 k-blocks, and the hand-off above (128 x 128 fp32 through shared memory, both MMA warpgroups storing at
+// once, one epilogue warp per SM sub-partition) costs about as much as the mainloop.  Here each of the two consumer
+// warpgroups owns a whole 128 x 128 tile: two m64n128 chains per k-step against the same B descriptor, 128 accumulators
+// per thread.  The CTA's tiles alternate between the warpgroups, a pair of named barriers gives the tensor cores to one
+// warpgroup at a time, and a warpgroup runs its epilogue from its registers (gemm_common.cuh: fragment epilogues) while
+// the other multiplies.  The shared memory the accumulator tile took goes to the operand ring.
+//
+//   warp 0     : TMA producer, filling stages in consumption order (the tiles of warpgroup 0 and 1 interleaved)
+//   warps 1-3  : idle (they hand their registers to the consumers and exit)
+//   warps 4-7  : consumer warpgroup 0: entries 0, 2, 4, ... of the CTA's tile list
+//   warps 8-11 : consumer warpgroup 1: entries 1, 3, 5, ...
+// ----------------------------------------------------------------------------------------------------------------------
+constexpr int PP_THREADS = 384;
+constexpr int PP_STAGES = 6;
+constexpr size_t PP_SMEM_BYTES =
+    1024 /*align slack*/ + size_t(PP_STAGES) * G_STAGE_BYTES + 256 /*barriers*/ + 8 * STG_BYTES;
+static_assert(PP_SMEM_BYTES <= 227 * 1024, "ping-pong GEMM shared memory exceeds the H100 per-block limit");
+// 384 threads compile to 168 registers each; the producer warpgroup's share goes to the consumers (128 accumulators)
+constexpr int PP_REGS_PRODUCER = 40, PP_REGS_MMA = 232;
+static_assert(128 * PP_REGS_PRODUCER + 256 * PP_REGS_MMA <= 384 * 168, "ping-pong GEMM register budget");
+// named barriers: PP_BAR_TURN + g admits warpgroup g to the tensor cores (its 128 threads wait, the other warpgroup's
+// 128 arrive); PP_BAR_PAIR + 2 g + {0, 1}: the two warp pairs of warpgroup g around their staging blocks
+constexpr int PP_BAR_TURN = 1, PP_BAR_PAIR = 3;
+
+// The epilogues of gemm_pp_kernel: STORE without dropout, RELU_BWD and plain CE_GRAD, whose per-element results do not
+// depend on which thread holds an element.  CE_STATS sums a row's exponentials in column order, which a thread of the
+// accumulator fragment cannot do (it holds two columns in eight), so it stays with the row-per-thread epilogue: lse,
+// and with it every gradient behind it, keeps its bits.
+static bool pp_has_epilogue(int mode, bool drop, bool wce, int gelu) {
+  return !drop && !wce && !gelu && (mode == DB200_EPI_STORE || mode == DB200_EPI_RELU_BWD || mode == DB200_EPI_CE_GRAD);
+}
+// Up to this many k-blocks per tile a product runs on gemm_pp_kernel (K <= 1024).  -DDB200_PP_MAX_KB=<n> moves the
+// rule in a side build, for measuring both kernels at one K (tools/bench_gemm_shapes.py).
+#ifndef DB200_PP_MAX_KB
+#define DB200_PP_MAX_KB 16
+#endif
+constexpr int PP_MAX_KB = DB200_PP_MAX_KB;
+
+template <int TA, int TB>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  constexpr int BN = GBN;
+  constexpr int STAGES = PP_STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t sA = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024-byte alignment
+  const uint32_t sB = sA + STAGES * A_BYTES;
+  const uint32_t bars = sA + STAGES * G_STAGE_BYTES;
+  const uint32_t full_bar = bars;                // STAGES x 8 B
+  const uint32_t empty_bar = bars + 8 * STAGES;  // STAGES x 8 B
+  const uint32_t stg_base = bars + 256;          // 2 warpgroups x 4 x STG_BYTES, 256-byte aligned
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+  }
+  if (warp == 1 && lane == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(full_bar + 8 * i, 1);
+      mbar_init(empty_bar + 8 * i, 1);  // a stage is read by one warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int total_tiles = p.m_tiles * p.n_tiles;  // never split-K: every tile has p.kb_total k-blocks
+
+  if (warp < 4) {
+    setmaxnreg_dec<PP_REGS_PRODUCER>();
+    if (warp != 0) return;
+    // ------------------------------------------------------------------ TMA producer (as in gemm_tc_kernel)
+    uint32_t stage = 0, phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
+      const int m0 = t.m_blk * BM, n0 = t.n_blk * BN;
+      for (int kb = 0; kb < p.kb_total; ++kb) {
+        mbar_wait_mma(empty_bar + 8 * stage, phase ^ 1);
+        const uint32_t fb = full_bar + 8 * stage;
+        if (elect_one_sync()) {
+          mbar_expect_tx(fb, G_STAGE_BYTES);
+          const int k0 = kb * BK;
+          const uint32_t a_dst = sA + stage * A_BYTES;
+          const uint32_t b_dst = sB + stage * G_B_BYTES;
+          if (p.a_3d) {
+            tma_load_3d(a_dst, &tmA, fb, 0, k0, m0 >> 6);
+          } else if (p.a_mn) {
+#pragma unroll
+            for (int s = 0; s < BM / 64; ++s) tma_load_2d(a_dst + s * SLAB_BYTES, &tmA, fb, m0 + 64 * s, k0);
+          } else {
+            tma_load_2d(a_dst, &tmA, fb, k0, m0);
+          }
+          if (p.b_3d) {
+            tma_load_3d(b_dst, &tmB, fb, 0, k0, n0 >> 6);
+          } else if (p.b_mn) {
+#pragma unroll
+            for (int s = 0; s < BN / 64; ++s) tma_load_2d(b_dst + s * SLAB_BYTES, &tmB, fb, n0 + 64 * s, k0);
+          } else {
+            tma_load_2d(b_dst, &tmB, fb, k0, n0);
+          }
+        }
+        __syncwarp();
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    // ------------------------------------------------------------------ consumer warpgroups
+    setmaxnreg_inc<PP_REGS_MMA>();
+    const int wg = (warp - 4) >> 2;
+    const FragCtx f = frag_ctx(stg_base + wg * 4 * STG_BYTES, threadIdx.x & 127, PP_BAR_PAIR + 2 * wg);
+    constexpr uint64_t astep = TA ? 128u : 2u, bstep = TB ? 128u : 2u;
+    constexpr uint32_t a_chain = TA ? SLAB_BYTES : 64u * 128u;  // rows 64-127 of the A stage
+    float d[2 * (BN / 2)];
+    for (int j = wg; blockIdx.x + (long long)j * gridDim.x < total_tiles; j += 2) {
+      const int tile = blockIdx.x + j * gridDim.x;
+      const TileCoord t = decode_tile(p, tile);
+      // ring position of this tile's first k-block: the other warpgroup consumed the tiles in between
+      const uint32_t it = (uint32_t)j * (uint32_t)p.kb_total;
+      uint32_t stage = it % STAGES, phase = (it / STAGES) & 1u, prev_stage = 0;
+#pragma unroll
+      for (int i = 0; i < 2 * (BN / 2); ++i) d[i] = 0.f;
+      // the other warpgroup has issued the last MMA of the tile before this one
+      if (j > 0) named_bar_sync(PP_BAR_TURN + wg, 256);
+      for (int kb = 0; kb < p.kb_total; ++kb) {
+        mbar_wait_mma(full_bar + 8 * stage, phase);
+        const uint64_t ad0 = smem_desc_sw128(sA + stage * A_BYTES, TA ? SLAB_BYTES : 0u, 1024);
+        const uint64_t ad1 = smem_desc_sw128(sA + stage * A_BYTES + a_chain, TA ? SLAB_BYTES : 0u, 1024);
+        const uint64_t bd0 = smem_desc_sw128(sB + stage * G_B_BYTES, TB ? SLAB_BYTES : 0u, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          wgmma_m64n128<TA, TB>(d, ad0 + k * astep, bd0 + k * bstep, 1u);
+          wgmma_m64n128<TA, TB>(d + BN / 2, ad1 + k * astep, bd0 + k * bstep, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      // one arrival per wait: only when the other warpgroup has a tile after this one
+      if (tile + (int)gridDim.x < total_tiles) named_bar_arrive(PP_BAR_TURN + (wg ^ 1), 256);
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+      const int m0 = t.m_blk * BM, n0 = t.n_blk * BN;
+      switch (p.mode) {
+        case DB200_EPI_STORE:    frag_store(p, d, f, m0, n0); break;
+        case DB200_EPI_RELU_BWD: frag_relu_bwd(p, d, f, m0, n0); break;
+        case DB200_EPI_CE_GRAD:  frag_ce_grad(p, d, f, m0, n0); break;
+        default: break;
+      }
+    }
+  }
+}
+
+template <int TA, int TB>
+static int launch_gemm_pp(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_pp_kernel<TA, TB>,
+                                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                          (int)PP_SMEM_BYTES);  // once, thread-safe (magic static)
+  DB200_CUDA(attr_rc);
+  const int total = p.m_tiles * p.n_tiles;
+  const int grid = total < sm_count() ? total : sm_count();
+  gemm_pp_kernel<TA, TB><<<grid, PP_THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  return check_launch("gemm_pp_kernel");
+}
+
 template <int TA, int TB, bool DROP, bool WCE = false, int GELU = 0>
 static int launch_gemm(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
   static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP, WCE, GELU>,
@@ -385,7 +556,12 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   } else if (colsum_out) {
     p.colsum = static_cast<float*>(epi->workspace);
   }
-  if (gelu == G_GELU_FWD)   // the MLP's W1 forward: A k-major, B mn-major
+  // Short contractions with a fragment epilogue run on the ping-pong kernel.  The rule reads the epilogue, K and the
+  // operand majors only, never M: prefill (M = B P) and training (M = B S) must take the same path, bit for bit.
+  if (kb_total <= PP_MAX_KB && pp_has_epilogue(mode, drop, cew != nullptr, gelu)) {
+    if (p.a_mn) rc = p.b_mn ? launch_gemm_pp<1, 1>(stream, tmA, tmB, p) : launch_gemm_pp<1, 0>(stream, tmA, tmB, p);
+    else        rc = p.b_mn ? launch_gemm_pp<0, 1>(stream, tmA, tmB, p) : launch_gemm_pp<0, 0>(stream, tmA, tmB, p);
+  } else if (gelu == G_GELU_FWD)   // the MLP's W1 forward: A k-major, B mn-major
     rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, false, G_GELU_FWD>(stream, tmA, tmB, p)
                              : set_error(DB200_E_UNSUPPORTED, "gemm_gelu: needs a k-major A and an mn-major B");
   else if (gelu == G_GELU_BWD)   // its dgrad dH = dbranch W2^T: both k-major

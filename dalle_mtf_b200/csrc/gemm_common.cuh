@@ -1,5 +1,6 @@
 // GEMM kernel parameters, tile decoding and the epilogue routines that turn the shared-memory accumulator tile
-// (wgmma.cuh: acc_store_smem / acc_ld_x32) into global-memory results; the convolutions reuse the staging helpers.
+// (wgmma.cuh: acc_store_smem / acc_ld_x32) of gemm_tc_kernel, or the accumulator fragments of gemm_pp_kernel, into
+// global-memory results; the convolutions reuse the staging helpers.
 #pragma once
 #include "common.cuh"
 #include "philox.cuh"
@@ -633,6 +634,233 @@ __device__ __forceinline__ void epi_ce_grad_weighted(const GemmParams& p, uint32
     }
     if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, lane);
     stage_flush<2, true>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// fragment epilogues (gemm_pp_kernel).  A warpgroup holds a whole 128 x 128 tile as two m64n128 accumulator fragments
+// (wgmma.cuh): thread t keeps, for chain c, 8-column group i and row half h, the pair d[frag_idx(c, i, h) + {0, 1}] =
+// tile row 64 c + 16 (t / 32) + 8 h + (t % 32) / 4, columns 8 i + 2 (t % 4) + {0, 1}.  The elementwise math runs on
+// those registers in place, with the per-element expressions of the row-per-thread epilogues above, so both kernels
+// round identically.  Global traffic keeps the staging discipline: rows [32 b, 32 b + 32) of the tile live in the
+// two warps 2 (b % 2), 2 (b % 2) + 1 of chain b / 2, which fill that row block's [32 rows][128 B] staging block
+// together (a 64-thread named barrier around it); one of the two then runs the unchanged stage_fetch_bf16 /
+// stage_colsum_bf16 / stage_flush on it.  A warp pair serves two blocks (one per chain) and each warp owns one.
+// ------------------------------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int frag_idx(int c, int i, int h) { return c * 64 + 4 * i + 2 * h; }
+
+struct FragCtx {
+  uint32_t own_stg;  // the staging block this warp fetches, sums and flushes (its pair's block of chain `own`)
+  uint32_t a[2];    // this thread's 4-byte word in row half 0 of each block at column group 0 (swizzle folded in)
+  int lane, q;      // q = lane % 4: the thread's column pair inside every 8-column group
+  int row;          // tile row of (chain 0, half 0): 16 (t / 32) + (t % 32) / 4
+  int own_row0;     // first tile row of that block
+  int bar;          // named barrier of the warp pair
+};
+__device__ __forceinline__ FragCtx frag_ctx(uint32_t stg_wg, int wg_thread, int bar0) {
+  FragCtx f;
+  const int w = wg_thread >> 5;
+  f.lane = wg_thread & 31;
+  f.q = f.lane & 3;
+  f.row = 16 * w + (f.lane >> 2);
+  f.own_row0 = 64 * (w & 1) + 32 * (w >> 1);
+  f.own_stg = stg_wg + (2 * (w & 1) + (w >> 1)) * STG_BYTES;
+  f.bar = bar0 + (w >> 1);
+  const int r = 16 * (w & 1) + (f.lane >> 2);  // row inside the block; r % 8 == lane / 4 for both row halves
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    f.a[c] = stg_wg + (2 * c + (w >> 1)) * STG_BYTES + r * 128 + ((f.lane >> 2) << 4) + 4 * f.q;
+  }
+  return f;
+}
+__device__ __forceinline__ void pair_sync(const FragCtx& f) { named_bar_sync(f.bar, 64); }
+// 16-byte slot `slot` of the thread's row (half h): the row's XOR swizzle is already in f.a, blocks are 128 B aligned
+__device__ __forceinline__ uint32_t frag_addr(const FragCtx& f, int c, int h, int slot) {
+  return (f.a[c] + h * 1024) ^ (slot << 4);
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+// columns [64 hp, 64 hp + 64) of the tile as bf16 into both blocks
+__device__ __forceinline__ void frag_put_bf16(const FragCtx& f, const float (&d)[128], int hp) {
+#pragma unroll
+  for (int c = 0; c < 2; ++c)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int k = frag_idx(c, 8 * hp + i, h);
+        st_shared_u32(frag_addr(f, c, h, i), pack_bf16x2(d[k], d[k + 1]));
+      }
+}
+// columns [32 s, 32 s + 32) of the tile as fp32 into both blocks: column 8 i + 2 q is word 2 q of slots 2 i, 2 i + 1
+__device__ __forceinline__ void frag_put_f32(const FragCtx& f, const float (&d)[128], int s) {
+#pragma unroll
+  for (int c = 0; c < 2; ++c)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int k = frag_idx(c, 4 * s + i, h);
+        const uint32_t row_base = (f.a[c] + h * 1024 - 4 * f.q) ^ ((2 * i + (f.q >> 1)) << 4);
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(row_base + 8 * (f.q & 1)), "f"(d[k]), "f"(d[k + 1])
+                     : "memory");
+      }
+}
+// bias of the thread's column pairs in columns [col0, col0 + 64), zero at and past `limit` (even or odd)
+__device__ __forceinline__ void frag_bias(const float* bias, int col0, int q, int limit, float2 (&b)[8]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int col = col0 + 8 * i + 2 * q;
+    b[i] = make_float2(0.f, 0.f);
+    if (!bias) continue;
+    if (col + 1 < limit) b[i] = __ldg(reinterpret_cast<const float2*>(bias + col));
+    else if (col < limit) b[i].x = __ldg(bias + col);
+  }
+}
+// the owner's work on its staged bf16 block: fused column sums (when asked for) and the flush to D
+template <bool STREAM>
+__device__ __forceinline__ void frag_flush_bf16(const GemmParams& p, const FragCtx& f, int m0, int colp, bool colsum) {
+  const int row0 = m0 + f.own_row0;
+  if (colsum) stage_colsum_bf16(f.own_stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, f.lane);
+  stage_flush<2, STREAM>(f.own_stg, p.D, p.ldd, row0, colp, p.M, p.N, f.lane);
+}
+
+__device__ __forceinline__ void frag_store(const GemmParams& p, float (&d)[128], const FragCtx& f, int m0, int n0) {
+#pragma unroll
+  for (int hp = 0; hp < 2; ++hp) {
+    const int colp = n0 + hp * 64;
+    if (colp >= p.N) break;  // uniform over the tile
+    if (p.residual) {
+      stage_fetch_bf16(f.own_stg, p.residual, p.ldr, m0 + f.own_row0, colp, p.M, p.N, f.lane);
+      pair_sync(f);
+    }
+    float2 b[8];
+    frag_bias(p.bias, colp, f.q, p.N, b);
+#pragma unroll
+    for (int c = 0; c < 2; ++c)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int k = frag_idx(c, 8 * hp + i, h);
+          d[k] = d[k] * p.alpha;
+          d[k + 1] = d[k + 1] * p.alpha;
+        }
+        if (p.bias) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int k = frag_idx(c, 8 * hp + i, h);
+            d[k] += b[i].x;
+            d[k + 1] += b[i].y;
+          }
+        }
+        if (p.relu) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int k = frag_idx(c, 8 * hp + i, h);
+            d[k] = fmaxf(d[k], 0.f);
+            d[k + 1] = fmaxf(d[k + 1], 0.f);
+          }
+        }
+        if (p.residual) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int k = frag_idx(c, 8 * hp + i, h);
+            const float2 r = unpack_bf16x2(ld_shared_u32(frag_addr(f, c, h, i)));
+            d[k] += r.x;
+            d[k + 1] += r.y;
+          }
+        }
+      }
+    if (!p.out_f32) {  // in place: every thread overwrites the residual words it has just read
+      frag_put_bf16(f, d, hp);
+      pair_sync(f);
+      frag_flush_bf16<false>(p, f, m0, colp, false);
+      pair_sync(f);
+    } else {
+      if (p.residual) pair_sync(f);  // fp32 words land on other threads' residual words
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        frag_put_f32(f, d, 2 * hp + s);
+        pair_sync(f);
+        stage_flush<4>(f.own_stg, p.D, p.ldd, m0 + f.own_row0, colp + 32 * s, p.M, p.N, f.lane);
+        pair_sync(f);
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ void frag_relu_bwd(const GemmParams& p, float (&d)[128], const FragCtx& f, int m0, int n0) {
+#pragma unroll
+  for (int hp = 0; hp < 2; ++hp) {
+    const int colp = n0 + hp * 64;
+    if (colp >= p.N) break;
+    stage_fetch_bf16(f.own_stg, p.aux, p.ldaux, m0 + f.own_row0, colp, p.M, p.N, f.lane);
+    pair_sync(f);
+#pragma unroll
+    for (int c = 0; c < 2; ++c)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int k = frag_idx(c, 8 * hp + i, h);
+          const uint32_t addr = frag_addr(f, c, h, i);
+          const float2 am = unpack_bf16x2(ld_shared_u32(addr));
+          const float o0 = am.x > 0.f ? d[k] * p.alpha : 0.f;
+          const float o1 = am.y > 0.f ? d[k + 1] * p.alpha : 0.f;
+          st_shared_u32(addr, pack_bf16x2(o0, o1));  // in place: the word this thread has just read
+        }
+    pair_sync(f);
+    frag_flush_bf16<false>(p, f, m0, colp, p.colsum != nullptr);
+    pair_sync(f);
+  }
+}
+
+__device__ __forceinline__ void frag_ce_grad(const GemmParams& p, float (&d)[128], const FragCtx& f, int m0, int n0) {
+  int label[2][2];
+  float l2[2][2];
+  bool row_ok[2][2];
+#pragma unroll
+  for (int c = 0; c < 2; ++c)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = m0 + 64 * c + 8 * h + f.row;
+      row_ok[c][h] = row < p.M;
+      label[c][h] = row_ok[c][h] ? p.labels[row] : -1;
+      l2[c][h] = row_ok[c][h] ? fmaf(p.lse[row], kLog2e, -log2f(p.alpha)) : 0.f;
+    }
+#pragma unroll
+  for (int hp = 0; hp < 2; ++hp) {
+    const int colp = n0 + hp * 64;
+    if (colp >= p.N) break;
+    float2 b[8];
+    frag_bias(p.bias, colp, f.q, p.n_valid, b);
+#pragma unroll
+    for (int c = 0; c < 2; ++c)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int k = frag_idx(c, 8 * hp + i, h);
+          const int col = colp + 8 * i + 2 * f.q;
+          float o0 = col < p.n_valid ? fast_exp2(fmaf(d[k] + b[i].x, kLog2e, -l2[c][h])) : 0.f;
+          float o1 = col + 1 < p.n_valid ? fast_exp2(fmaf(d[k + 1] + b[i].y, kLog2e, -l2[c][h])) : 0.f;
+          if (col == label[c][h]) o0 -= p.alpha;
+          if (col + 1 == label[c][h]) o1 -= p.alpha;
+          // rows past M: zeros (they are not stored, but the fused column sums read the staged block)
+          d[k] = row_ok[c][h] ? o0 : 0.f;
+          d[k + 1] = row_ok[c][h] ? o1 : 0.f;
+        }
+    frag_put_bf16(f, d, hp);
+    pair_sync(f);
+    frag_flush_bf16<true>(p, f, m0, colp, p.colsum != nullptr);  // 4 GB of dlogits: stream past L2
+    pair_sync(f);
   }
 }
 

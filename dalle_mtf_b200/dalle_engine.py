@@ -166,6 +166,15 @@ def validate_per_position_padding(value):
     return value
 
 
+def validate_logits_mask(value):
+    """logits_mask: None or a bool (None: False)."""
+    if value is None:
+        return False
+    if not isinstance(value, bool):
+        raise ValueError(f"logits_mask = {value!r}: must be true, false or null")
+    return value
+
+
 def image_grid_side(image_seq_len):
     """W of the W x W image-token grid row / column position embeddings need (image_seq_len = W^2)."""
     W = math.isqrt(image_seq_len)
@@ -232,7 +241,7 @@ class DalleEngine:
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
-                 activation="relu"):
+                 activation="relu", logits_mask=False):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -268,7 +277,16 @@ class DalleEngine:
 
         activation: the MLP nonlinearity (validate_activation).  "gelu" makes the MLP gelu(LN2(x) W1 + b1) W2 + b2 with
         mtf's tanh GELU, fused into the W1 product's epilogue (which also keeps the pre-activation z for backward: one
-        more bf16 [T, 4d] per saved layer) and into its dgrad's; no parameter changes."""
+        more bf16 [T, 4d] per saved layer) and into its dgrad's; no parameter changes.
+
+        logits_mask (DALLE-pytorch's logits_mask): a text row (position p < text_seq_len - 1, whose target is a text
+        token) normalises over the ids [0, image_offset), an image row (target an image code or EOS) over
+        [image_offset, V); each row's loss is lse_window - logit[label] (+ z_loss lse_window^2) and its gradient is 0
+        outside the window.  The step gathers each class into one block of rows and runs the vocabulary products on
+        that block's columns only (_masked_forward / _masked_backward); logits() returns -inf outside the windows.  A
+        label outside its row's window is undefined, as a label >= V is: assemble_tokens(_pp) keeps every label in its
+        window as long as the caption ids are < text_vocab_size and the codes < image_vocab_size.  No parameter
+        changes; prefill and decoding are unchanged (image draws already see only image ids)."""
         self.activation = validate_activation(activation)
         self.gelu = self.activation == "gelu"
         self.mlp_act = {"gelu": True} if self.gelu else {"relu": True}   # linear_fwd keywords of an inference W1
@@ -291,6 +309,14 @@ class DalleEngine:
         self.V = self.image_offset + image_vocab_size + 1           # models.py:157 (extra id = EOS)
         self.eos_token_id = self.V - 1                              # models.py:158
         self.Vpad = _round_up(self.V, 64)
+        self.logits_mask = validate_logits_mask(logits_mask)
+        # windows of the masked vocabulary products: the text block over columns [0, mask_text_cols) (n_valid =
+        # image_offset), the image block over [mask_c0, mask_c0 + mask_image_cols) (n_valid = V - mask_c0), with
+        # mask_c0 = image_offset rounded down to 8 columns so that the operand base stays 16-byte aligned for TMA
+        self.text_rows = text_seq_len - 1
+        self.mask_c0 = self.image_offset // 8 * 8
+        self.mask_text_cols = _round_up(self.image_offset, 8)
+        self.mask_image_cols = _round_up(self.V - self.mask_c0, 8)
         self.device = torch.device(device)
         self.recompute_grad = bool(recompute_grad)
         self.attn_scale = float(attn_scale)
@@ -313,7 +339,8 @@ class DalleEngine:
         lw = (None, None) if loss_weights is None else tuple(loss_weights)
         self.loss_weights, self.z_loss = validate_loss_weights(*lw, z_loss)
         self.weighted_loss = self.loss_weights is not None or self.z_loss > 0
-        self._cew = None             # lib.CeWeights of the current forward (weighted loss only)
+        self._cew = None             # lib.CeWeights of the current forward (weighted loss only; logits mask: a
+                                     # (text block, image block) pair)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w) if self.row_col else \
@@ -611,16 +638,30 @@ class DalleEngine:
                 "h1": e(T, 4 * d), **({"z1": e(T, 4 * d)} if self.gelu else {}),
             } for _ in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
-            "labels": e(B, S, dtype=I32),
-            "part_max": e(nt, T, dtype=F32), "part_sum": e(nt, T, dtype=F32),
-            "label_logit": e(T, dtype=F32), "lse_v": e(T, dtype=F32), "loss_rows": e(T, dtype=F32),
-            "dlogits": e(T, self.Vpad),
+            "labels": e(B, S, dtype=I32), "loss_rows": e(T, dtype=F32),
             # backward scratch
             "dx_a": e(T, d), "dx_b": e(T, d), "dtmp": e(T, d), "dh1": e(T, 4 * d), "dqkv": e(T, 3 * d),
             "delta": e(B, self.H, S, dtype=F32), "dq_acc": e(1, dtype=F32),
         }
         if self.dropout[2] > 0:   # gradient of a branch output before its residual dropout
             b["dxm"] = e(T, d)
+        if not self.logits_mask:
+            b.update({"part_max": e(nt, T, dtype=F32), "part_sum": e(nt, T, dtype=F32), "label_logit": e(T, dtype=F32),
+                      "lse_v": e(T, dtype=F32), "dlogits": e(T, self.Vpad)})
+        else:   # one set of vocabulary-product buffers per row block, sized to its window
+            b["bias_image"] = e(self.mask_image_cols, dtype=F32)
+            b["blocks"] = []
+            n_image = B * (S - self.text_rows)
+            for rows, N in ((B * self.text_rows, self.mask_text_cols), (n_image, self.mask_image_cols)):
+                if rows == 0:   # text_seq_len 1: no text rows
+                    b["blocks"].append(None)
+                    continue
+                nb = ops.ce_tiles(N)
+                b["blocks"].append({
+                    "rows": rows, "N": N, "hf": e(rows, d), "labels": e(rows, dtype=I32),
+                    "part_max": e(nb, rows, dtype=F32), "part_sum": e(nb, rows, dtype=F32),
+                    "label_logit": e(rows, dtype=F32), "lse_v": e(rows, dtype=F32), "loss_rows": e(rows, dtype=F32),
+                    "dlogits": e(rows, N), "dx": e(rows, d)})
         self._bufs, self._buf_key = b, key
         return b
 
@@ -714,6 +755,8 @@ class DalleEngine:
                           bufs["rstdf"], self.ln_eps)                                            # models.py:393
         ops.shift_labels(tokens, bufs["labels"], self.eos_token_id)                                # models.py:407-410
         labels = bufs["labels"].view(T)
+        if self.logits_mask:
+            return self._masked_forward(bufs, B, loss_accum, global_batch)
         ops.gemm(bufs["hf"], self.W("wout"), None, T, self.Vpad, self.d, a_mn=False, b_mn=True, mode=L.EPI_CE_STATS,
                  bias=self.P("bout"), labels=labels, part_max=bufs["part_max"], part_sum=bufs["part_sum"],
                  label_logit=bufs["label_logit"], n_valid=self.V)
@@ -730,16 +773,87 @@ class DalleEngine:
                       loss_accum)
         return loss_accum
 
+    # ------------------------------------------------------------------------------------------ logits mask
+    def _mask_windows(self):
+        """(first column, n_valid) of the text and the image block's vocabulary window; the image block's labels are
+        relative to its first column."""
+        c0 = self.mask_c0
+        return ((0, self.image_offset), (c0, self.V - c0))
+
+    def _masked_forward(self, bufs, B, loss_accum, global_batch):
+        """The vocabulary products of forward() with the logits mask: partition hf and the labels into the text and
+        image blocks, CE_STATS + finish on each block over its window (text block first: fixed order), scatter the
+        row losses back into [B*S] order."""
+        S, d = self.S, self.d
+        text, image = bufs["blocks"]
+        ops.logits_mask_partition(bufs["hf"], bufs["labels"].view(-1), self.P("bout"),
+                                  text["hf"] if text else None, image["hf"], text["labels"] if text else None,
+                                  image["labels"], bufs["bias_image"], B, S, self.text_rows, self.mask_c0,
+                                  self.image_offset, self.V)
+        if self.weighted_loss:
+            a_text, a_image = loss_coefficients(self.loss_weights, self.text_seq_len, self.image_seq_len,
+                                                B if global_batch is None else global_batch)
+            self._cew = (L.make_ce_weights(1, 1, a_text, a_image, self.z_loss),
+                         L.make_ce_weights(1, 0, a_text, a_image, self.z_loss))
+            if loss_accum is None:
+                loss_accum = self.grads[self.aux_off:self.aux_off + 4]
+        elif loss_accum is None:
+            loss_accum = self.grads[self.aux_off:self.aux_off + 1]
+        biases = (self.P("bout"), bufs["bias_image"])
+        for k, ((c0, n_valid), blk) in enumerate(zip(self._mask_windows(), bufs["blocks"])):
+            if blk is None:
+                continue
+            ops.gemm(blk["hf"], self.W("wout")[:, c0:c0 + blk["N"]], None, blk["rows"], blk["N"], d, a_mn=False,
+                     b_mn=True, mode=L.EPI_CE_STATS, bias=biases[k], labels=blk["labels"], part_max=blk["part_max"],
+                     part_sum=blk["part_sum"], label_logit=blk["label_logit"], n_valid=n_valid)
+            if self.weighted_loss:
+                ops.ce_finish_weighted(blk["part_max"], blk["part_sum"], blk["label_logit"], blk["lse_v"],
+                                       blk["loss_rows"], loss_accum, self._cew[k])
+            else:
+                ops.ce_finish(blk["part_max"], blk["part_sum"], blk["label_logit"], blk["lse_v"], blk["loss_rows"],
+                              loss_accum)
+        ops.logits_mask_scatter(B, S, self.text_rows, loss_text=text["loss_rows"] if text else None,
+                                loss_image=image["loss_rows"], loss_rows=bufs["loss_rows"])
+        return loss_accum
+
+    def _masked_backward(self, bufs, B, grad_scale):
+        """The vocabulary products of backward() with the logits mask: per block (text first) the CE_GRAD product with
+        its fused bias gradient, the wout wgrad and the dgrad, all over the block's window and accumulating into
+        G("wout") / G("bout") at its column offset; then the two dgrads are scattered into bufs["dtmp"]."""
+        d = self.d
+        biases = (self.P("bout"), bufs["bias_image"])
+        for k, ((c0, n_valid), blk) in enumerate(zip(self._mask_windows(), bufs["blocks"])):
+            if blk is None:
+                continue
+            N = blk["N"]
+            cew = None
+            if self.weighted_loss:
+                c = self._cew[k]
+                cew = L.make_ce_weights(c.period, c.text_rows, c.a_text * grad_scale, c.a_image * grad_scale, c.z_loss)
+            ops.gemm(blk["hf"], self.W("wout")[:, c0:c0 + N], blk["dlogits"], blk["rows"], N, d, a_mn=False, b_mn=True,
+                     mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=biases[k], labels=blk["labels"], lse=blk["lse_v"],
+                     n_valid=n_valid, colsum=self.G("bout")[c0:c0 + N], ce_weights=cew)
+            ops.linear_wgrad(blk["hf"], blk["dlogits"], self.G("wout")[:, c0:c0 + N])
+            ops.linear_dgrad(blk["dlogits"], self.W("wout")[:, c0:c0 + N], blk["dx"])
+        text, image = bufs["blocks"]
+        ops.logits_mask_scatter(B, self.S, self.text_rows, dx_text=text["dx"] if text else None, dx_image=image["dx"],
+                                dx=bufs["dtmp"])
+
     def logits(self, tokens):
         """fp32 logits [B,S,V] (return_logits=True path, src/dalle_mtf/models.py:412-415).  Test / eval use only:
-        this materialises the tensor the training path never writes."""
+        this materialises the tensor the training path never writes.  With the logits mask, -inf outside each row's
+        window, so that softmax(logits) is the model's distribution."""
         B, S = tokens.shape
         self.forward(tokens, loss_accum=torch.zeros(4 if self.weighted_loss else 1, dtype=F32, device=self.device))
         T = B * S
         out = torch.empty(T, self.Vpad, dtype=F32, device=self.device)
         ops.gemm(self._bufs["hf"], self.W("wout"), out, T, self.Vpad, self.d, a_mn=False, b_mn=True,
                  bias=self.P("bout"))
-        return out.view(B, S, self.Vpad)[:, :, :self.V]
+        logits = out.view(B, S, self.Vpad)[:, :, :self.V]
+        if self.logits_mask:
+            logits[:, :self.text_rows, self.image_offset:] = -math.inf
+            logits[:, self.text_rows:, :self.image_offset] = -math.inf
+        return logits
 
     # ------------------------------------------------------------------------------------------ prompt prefill
     def _prefill_alloc(self, B, P, rep):
@@ -846,16 +960,19 @@ class DalleEngine:
         tokens = self._tokens
         B, S = tokens.shape
         T, d = B * S, self.d
-        labels = bufs["labels"].view(T)
-        cew = None
-        if self.weighted_loss:
-            c = self._cew
-            cew = L.make_ce_weights(c.period, c.text_rows, c.a_text * grad_scale, c.a_image * grad_scale, c.z_loss)
-        ops.gemm(bufs["hf"], self.W("wout"), bufs["dlogits"], T, self.Vpad, d, a_mn=False, b_mn=True,
-                 mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=self.P("bout"), labels=labels, lse=bufs["lse_v"],
-                 n_valid=self.V, colsum=self.G("bout"), ce_weights=cew)  # dlogits + fused d(bout) = colsum(dlogits)
-        ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
-        ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
+        if self.logits_mask:
+            self._masked_backward(bufs, B, grad_scale)
+        else:
+            labels = bufs["labels"].view(T)
+            cew = None
+            if self.weighted_loss:
+                c = self._cew
+                cew = L.make_ce_weights(c.period, c.text_rows, c.a_text * grad_scale, c.a_image * grad_scale, c.z_loss)
+            ops.gemm(bufs["hf"], self.W("wout"), bufs["dlogits"], T, self.Vpad, d, a_mn=False, b_mn=True,
+                     mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=self.P("bout"), labels=labels, lse=bufs["lse_v"],
+                     n_valid=self.V, colsum=self.G("bout"), ce_weights=cew)  # dlogits + fused d(bout) = colsum(dlogits)
+            ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
+            ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
         dx = bufs["dx_a"]
         dbranch = self._ln_bwd(bufs["dtmp"], bufs["xs"][self.L], self.P("lnf_g"), bufs["meanf"], bufs["rstdf"], None,
                                dx, self.G("lnf_g"), self.G("lnf_b"), self.G(f"l{self.L - 1}.b2"),

@@ -166,6 +166,9 @@ _SIGNATURES = {
     "db200_ce_finish": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
     "db200_ce_finish_weighted": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, ctypes.POINTER(CeWeights),
                                  c_vp, c_i64],
+    "db200_logits_mask_partition": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int,
+                                    c_int, c_int, c_int],
+    "db200_logits_mask_scatter": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_attn_causal_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_causal_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_causal_fwd_ex": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32, ctypes.POINTER(Dropout)],

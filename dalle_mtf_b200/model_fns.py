@@ -15,7 +15,7 @@ import torch
 from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
-    validate_loss_weights, validate_per_position_padding, validate_position_embedding
+    validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -207,6 +207,16 @@ def loss_weights(params):
     return validate_loss_weights(params.get("text_loss_weight"), params.get("image_loss_weight"), params.get("z_loss"))
 
 
+def logits_mask(params):
+    """The extension key logits_mask of a DALL-E config (DALLE-pytorch's logits_mask): absent, null or false is the
+    reference's objective; true makes text rows (positions p < text_seq_len - 1) normalise over the text ids [0,
+    image_offset) only and image rows (image codes and EOS) over [image_offset, V) only (DalleEngine).  Any other value
+    is rejected.  Every label must lie in its row's window, which assemble_tokens(_pp) guarantees when the caption ids
+    are < text_vocab_size and the VAE codes < image_vocab_size; the loss of a row whose label lies outside is undefined.
+    No parameter depends on it, so a checkpoint loads with or without the key."""
+    return validate_logits_mask(params.get("logits_mask"))
+
+
 def dalle_model_fn(features, labels, mode, params):
     """src/model_fns.py:55-236.  features: images f32 [B,H,W,C] in [-1,1] (NHWC); labels: caption ids i32
     [B, text_seq_len].  (The reference's own comment has them swapped; the code uses them this way.)"""
@@ -219,6 +229,7 @@ def dalle_model_fn(features, labels, mode, params):
     weights, z_loss = loss_weights(params)
     pos_scheme, per_pos, pp_pad = input_embedding(params)
     activation = activation_function(params)
+    mask = logits_mask(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -252,7 +263,7 @@ def dalle_model_fn(features, labels, mode, params):
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
-                        activation=activation)
+                        activation=activation, logits_mask=mask)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

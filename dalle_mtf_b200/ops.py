@@ -188,6 +188,48 @@ def ce_finish_weighted(part_max, part_sum, label_logit, lse, loss_rows, sums, we
           "db200_ce_finish_weighted")
 
 
+def logits_mask_partition(hf, labels, bias, hf_text, hf_image, labels_text, labels_image, bias_image, B, S, text_rows,
+                          c0, image_offset, V):
+    """Row partition of the modality logits mask (include/dalle_b200.h): hf [B*S, d] -> hf_text [B*text_rows, d] and
+    hf_image [B*(S - text_rows), d]; labels -> labels_text and labels_image - c0; bias_image [round_up(V - c0, 8)] =
+    -inf on [c0, image_offset), bias[image_offset:V], then 0.  With text_rows 0 the text blocks may be None."""
+    L.require_device()
+    _chk(hf, BF16, "hf"); _chk(hf_text, BF16, "hf_text"); _chk(hf_image, BF16, "hf_image")
+    _chk(labels, I32, "labels"); _chk(labels_text, I32, "labels_text"); _chk(labels_image, I32, "labels_image")
+    _chk(bias, F32, "bias"); _chk(bias_image, F32, "bias_image")
+    d = hf.shape[1]
+    ni = S - text_rows
+    n_bias = (V - c0 + 7) // 8 * 8
+    if tuple(hf.shape) != (B * S, d) or labels.numel() != B * S or tuple(hf_image.shape) != (B * ni, d) or \
+            labels_image.numel() != B * ni or bias_image.numel() < n_bias or bias.numel() < V or \
+            (text_rows and (tuple(hf_text.shape) != (B * text_rows, d) or labels_text.numel() != B * text_rows)):
+        raise L.DB200Error(f"logits_mask_partition: block shapes do not match B={B} S={S} text_rows={text_rows} d={d}")
+    check(L.load().db200_logits_mask_partition(stream_ptr(), ptr(hf), ptr(labels), ptr(bias), ptr(hf_text),
+                                               ptr(hf_image), ptr(labels_text), ptr(labels_image), ptr(bias_image), B,
+                                               S, text_rows, d, int(c0), int(image_offset), int(V)),
+          "logits_mask_partition")
+
+
+def logits_mask_scatter(B, S, text_rows, dx_text=None, dx_image=None, dx=None, loss_text=None, loss_image=None,
+                        loss_rows=None):
+    """Inverse of logits_mask_partition on row data: dx [B*S, d] from the blocks' dgrads dx_text / dx_image and
+    loss_rows [B*S] from loss_text / loss_image (either part skipped when dx, resp. loss_rows, is None)."""
+    L.require_device()
+    _chk(dx_text, BF16, "dx_text"); _chk(dx_image, BF16, "dx_image"); _chk(dx, BF16, "dx")
+    _chk(loss_text, F32, "loss_text"); _chk(loss_image, F32, "loss_image"); _chk(loss_rows, F32, "loss_rows")
+    ni = S - text_rows
+    d = dx.shape[1] if dx is not None else 0
+    if dx is not None and (tuple(dx.shape) != (B * S, d) or tuple(dx_image.shape) != (B * ni, d) or
+                           (text_rows and tuple(dx_text.shape) != (B * text_rows, d))):
+        raise L.DB200Error(f"logits_mask_scatter: dx block shapes do not match B={B} S={S} text_rows={text_rows}")
+    if loss_rows is not None and (loss_rows.numel() != B * S or loss_image.numel() != B * ni or
+                                  (text_rows and loss_text.numel() != B * text_rows)):
+        raise L.DB200Error(f"logits_mask_scatter: loss block sizes do not match B={B} S={S} text_rows={text_rows}")
+    check(L.load().db200_logits_mask_scatter(stream_ptr(), ptr(dx_text), ptr(dx_image), ptr(dx), ptr(loss_text),
+                                             ptr(loss_image), ptr(loss_rows), B, S, text_rows, d),
+          "logits_mask_scatter")
+
+
 # ----------------------------------------------------------------------------------------------- row ops
 def embed_fwd(ids, wte, wpe, out, wte_drop=None, wpe_drop=None):
     """out = wte[ids] + wpe[s]; with embedding dropout (lib.Dropout descriptors of the wte / wpe sites) each term is

@@ -260,6 +260,26 @@ int db200_ce_finish_weighted(db200_stream_t stream, const float* part_max, const
                              const db200_ce_weights* w, void* workspace, int64_t workspace_bytes);
 int64_t db200_ce_finish_weighted_workspace_bytes(int M);
 
+/* Modality logits mask (extension; DALLE-pytorch's logits_mask).  Row p of each S-row sequence is a text row iff
+ * p < text_rows (text_seq_len - 1: its target is a text token) and normalises over vocabulary ids [0, image_offset);
+ * the others are image rows (image codes and EOS) and normalise over [image_offset, V).  The vocabulary products run on
+ * each class as one contiguous block of rows, the image block over the columns [c0, c0 + round_up(V - c0, 8)) with
+ * c0 = image_offset rounded down to a multiple of 8 (a 16-byte aligned TMA base).
+ *   partition: hf bf16 [B*S][d] -> hf_text [B*text_rows][d] (rows b*S + p, p < text_rows, in order) and hf_image
+ *              [B*(S-text_rows)][d] (the other rows, in order); labels [B*S] -> labels_text (unchanged) and
+ *              labels_image (label - c0); bias_image [round_up(V - c0, 8)] = -inf on [c0, image_offset), bias[c] on
+ *              [image_offset, V), 0 past V (the -inf columns drop out of every CE epilogue's max, sum and gradient).
+ *   scatter:   its inverse on row data: dx bf16 [B*S][d] from dx_text / dx_image and loss_rows [B*S] from loss_text /
+ *              loss_image; either triple may be skipped by passing dx (resp. loss_rows) NULL.
+ * 0 <= text_rows < S; with text_rows == 0 the text pointers may be NULL.  d % 8 == 0, bf16 pointers 16-byte aligned;
+ * 0 <= c0 <= image_offset < V, c0 % 8 == 0.  Row indices are 64-bit; grids are sized from the usable SMs. */
+int db200_logits_mask_partition(db200_stream_t stream, const void* hf_bf16, const int32_t* labels, const float* bias,
+                                void* hf_text_bf16, void* hf_image_bf16, int32_t* labels_text, int32_t* labels_image,
+                                float* bias_image, int B, int S, int text_rows, int d, int c0, int image_offset, int V);
+int db200_logits_mask_scatter(db200_stream_t stream, const void* dx_text_bf16, const void* dx_image_bf16,
+                              void* dx_bf16, const float* loss_text, const float* loss_image, float* loss_rows, int B,
+                              int S, int text_rows, int d);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * K4  causal flash attention on wgmma.  Replaces mtf_transformer.attention.attention with the [S,S] -1e10 mask:
  *     src/dalle_mtf/models.py:221-227, 287-299.   qkv: bf16 [B][S][3][H][dh] (output of the fused q|k|v GEMM),

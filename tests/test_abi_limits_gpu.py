@@ -274,9 +274,7 @@ def test_sqnorm_and_adam_past_2_31_elements(ops):
     for _, a, b in flat_slabs(n):
         sq += (bufs["g"].out[a:b].to(F64) ** 2).sum()
     sq = gn_base + sq
-    blocks = min(-(-(n // 4) // 256), 8 * DK._sm())
-    depth = 4 * -(-(n // 4) // (blocks * 256)) + 5 + 8 + blocks + 8
-    DK.check("sqnorm n=2^31+37", gn, sq.reshape(1), sq.reshape(1), a=0.0, b=depth * U)
+    DK.check("sqnorm n=2^31+37", gn, sq.reshape(1), sq.reshape(1), a=0.0, b=DK.sqnorm_depth(n) * U)
     p16 = guarded((n,), BF16)
     lr, b1, b2, eps, wd, clip = 1e-3, 0.9, 0.999, 1e-6, 0.01, 1.0
     ops.adam_step(bufs["p"].out, bufs["m"].out, bufs["v"].out, bufs["g"].out, p16.out, lr, b1, b2, eps, wd, gn, clip,

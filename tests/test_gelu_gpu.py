@@ -143,22 +143,23 @@ def _epilogue_case(ops, name, M, d, N, seed):
     x64, w164 = x.to(F64), w1.to(F64)
     zref = x64 @ w164 + b1.to(F64)
     zabs = x64.abs() @ w164.abs() + b1.to(F64).abs()
-    FB.check(f"{name} z", z, zref, zabs, b=(d + 8) * UTC, bf16_out=True, tag=TAG)
+    r = FB.check(f"{name} z", z, zref, zabs, b=(d + 8) * UTC, bf16_out=True, tag=TAG)
     del zref, zabs, x64, w164
-    check_h(f"{name} h", h, z)
+    r = max(r, check_h(f"{name} h", h, z))
     # backward on the stored z: dZ and the fused column sums
     dy64, w264 = dy.to(F64), w2.to(F64)
     acc = dy64 @ w264.T
     absref = dy64.abs() @ w264.abs().T
-    check_dz(f"{name} dZ", dz, acc, absref, z, d)
+    r = max(r, check_dz(f"{name} dZ", dz, acc, absref, z, d))
     del acc, absref, dy64, w264
     dz64 = dz.to(F64)
     cref = base.to(F64) + dz64.sum(0)
-    FB.check(f"{name} colsum", colsum, cref, base.to(F64).abs() + dz64.abs().sum(0), b=(32 + M / 32 + 8) * U,
-             tag=TAG)
+    r = max(r, FB.check(f"{name} colsum", colsum, cref, base.to(F64).abs() + dz64.abs().sum(0),
+                        b=(32 + M / 32 + 8) * U, tag=TAG))
     sat = ((z.float() > -1) & (z.float() < 1)).float().mean().item()
     print(f"[{TAG}] {name} M={M} K={d} N={N}: fraction of z in (-1, 1) {sat:.3f}, z range "
           f"[{z.float().min().item():.2f}, {z.float().max().item():.2f}]")
+    return r
 
 
 @pytest.mark.parametrize("name,M,d,N", SHAPES, ids=[s[0] for s in SHAPES])

@@ -28,7 +28,6 @@ On an H100 80GB HBM3 (132 SMs, 700 W power limit) the module takes 30 s (pytest'
 8 x 256^2 included.
 """
 import functools
-import inspect
 import math
 
 import pytest
@@ -38,6 +37,7 @@ import float64_bounds
 import test_vae_kernels_gpu as VK
 import test_vae_paper_gpu as VP
 from float64_bounds import DEV, U, UTC, nan_like
+from launch_census import OpsRecorder
 
 pytestmark = pytest.mark.gpu
 
@@ -164,49 +164,14 @@ def weight_names(eng):
     return names
 
 
-class Recorder:
-    """Context manager that wraps every public function of dalle_mtf_b200.ops.  Each call at the outermost level (a
-    wrapper calling another, as linear_wgrad calls gemm, counts once) is described and appended to `launches`;
-    before(entry, args) / after(entry, args, state) run around it with the bound arguments."""
+class Recorder(OpsRecorder):
+    """OpsRecorder of the outermost ops calls (a wrapper calling another, as linear_wgrad calls gemm, counts once),
+    each described as a Launch with the engine's weight names."""
 
     def __init__(self, eng, before=None, after=None):
         self.names = weight_names(eng)
-        self.before, self.after = before, after
-        self.launches = []
-        self._depth = 0
-
-    def __enter__(self):
-        from dalle_mtf_b200 import ops
-        self._mp = pytest.MonkeyPatch()
-        for name, fn in list(vars(ops).items()):
-            if inspect.isfunction(fn) and fn.__module__ == ops.__name__ and not name.startswith("_") \
-                    and name not in HOST_ONLY:
-                self._mp.setattr(ops, name, self._wrap(name, fn))
-        return self
-
-    def __exit__(self, *exc):
-        self._mp.undo()
-
-    def _wrap(self, entry, fn):
-        sig = inspect.signature(fn)
-
-        def call(*a, **k):
-            if self._depth:
-                return fn(*a, **k)
-            ba = sig.bind(*a, **k)
-            ba.apply_defaults()
-            A = dict(ba.arguments)
-            self.launches.append(describe(entry, A, self.names))
-            state = self.before(entry, A) if self.before else None
-            self._depth += 1
-            try:
-                out = fn(*a, **k)
-            finally:
-                self._depth -= 1
-            if self.after:
-                self.after(entry, A, state)
-            return out
-        return call
+        super().__init__(lambda entry, A: (describe(entry, A, self.names), None), skip=HOST_ONLY, before=before,
+                         after=after)
 
 
 def distinct(launches):

@@ -25,6 +25,11 @@ from .dalle_engine import ParamLayout
 
 BF16, F32, I32 = torch.bfloat16, torch.float32, torch.int32
 RECONSTRUCTION_LOSSES = ("mse", "logit_laplace")
+# decode_tokens allocates every per-image buffer of the training step (_alloc), ~0.45 GiB per 256^2 image for vae_coco
+# and ~1.4 GiB for the paper network, so 128 images in one pass would need 58 and 182 GiB.  Generation holds the DALL-E
+# engine, its KV cache and the sampler at the same time, so decoding takes at most a fifth of an 80 GB device: passes
+# of 35 and 11 images, each still thousands of pixel tiles per convolution.
+DECODE_PASS_BYTES = 16 << 30
 
 
 class VaeEngine:
@@ -222,9 +227,25 @@ class VaeEngine:
     def _alloc(self, B):
         if self._B == B:
             return
-        dev, act = self.device, self.act
-        e = lambda *shape, dtype=act: torch.empty(*shape, dtype=dtype, device=dev)
+        self._B = self._b = None            # the previous batch's buffers go before the new ones are allocated
+        self._b = self._buffers(B, self.device)
         self._B = B
+
+    def buffer_bytes(self, B):
+        """Bytes of the buffers _alloc(B) allocates (counted on the meta device, nothing is allocated)."""
+        def size(v):
+            if isinstance(v, torch.Tensor):
+                return v.numel() * v.element_size()
+            return sum(size(x) for x in (v.values() if isinstance(v, dict) else v))
+        return size(self._buffers(B, torch.device("meta")))
+
+    def decode_pass_images(self):
+        """The most images decode_tokens runs through the network at once: DECODE_PASS_BYTES of buffers."""
+        return max(1, DECODE_PASS_BYTES // self.buffer_bytes(1))
+
+    def _buffers(self, B, dev):
+        act = self.act
+        e = lambda *shape, dtype=act: torch.empty(*shape, dtype=dtype, device=dev)
         rows = B * self.hw * self.hw
         b = {"x_in": e(B, self.H, self.W, self.C), "enc": [], "dec": []}
         for kind, _, cin, ch, res in self.enc:
@@ -266,7 +287,7 @@ class VaeEngine:
                 shapes[tuple(d["out"].shape)] = None
         shapes[(B, self.hw, self.hw, self.n_hid)] = None
         b["gscratch"] = {s: [e(*s), e(*s)] for s in shapes}
-        self._b = b
+        return b
 
     def _desc(self, B, res, cin, cout, k, stride, transposed=False, relu=False):
         key = (B, res, cin, cout, k, stride, transposed, relu)
@@ -385,7 +406,20 @@ class VaeEngine:
 
     def decode_tokens(self, idx, offset=0):
         """Image-token ids int32 [B, image_seq_len] (minus `offset`) -> reconstruction fp32 NHWC [B,H,W,C] in [-1,1]-ish:
-        one-hot codes through the tied codebook and the decoder — the generation-side counterpart of encode_tokens."""
+        one-hot codes through the tied codebook and the decoder — the generation-side counterpart of encode_tokens.
+
+        Runs in passes of at most decode_pass_images() images, each written into one output tensor; every decode launch
+        computes an image from that image's codes alone, so the result does not depend on the pass size."""
+        B = idx.shape[0]
+        n = self.decode_pass_images()
+        if B <= n:
+            return self._decode_pass(idx, offset)
+        out = torch.empty(B, self.img_H, self.img_W, self.img_C, dtype=F32, device=self.device)
+        for i in range(0, B, n):
+            out[i:i + n].copy_(self._decode_pass(idx[i:i + n], offset))
+        return out
+
+    def _decode_pass(self, idx, offset):
         B = idx.shape[0]
         self._alloc(B)
         rows = B * self.hw * self.hw

@@ -154,11 +154,13 @@ class PaperVaeEngine(VaeEngine):
 
     # ------------------------------------------------------------------------------------------ buffers
     def _alloc(self, B):
-        if self._B == B:
-            return
-        dev, act = self.device, self.act
+        if self._B != B:
+            self._pool = {}
+        super()._alloc(B)
+
+    def _buffers(self, B, dev):
+        act = self.act
         e = lambda *shape, dtype=act: torch.empty(*shape, dtype=dtype, device=dev)
-        self._B = B
         rows = B * self.hw * self.hw
         b = {"x0": e(B, self.H, self.W, self.base_width), "enc": [], "dec": []}
         for side in ("enc", "dec"):
@@ -190,8 +192,7 @@ class PaperVaeEngine(VaeEngine):
             b.update({"kl_lse": e(rows, dtype=F32), "kl_ent": e(rows, dtype=F32), "kl_hist": e(K, dtype=I32)})
         if self.logit_laplace:
             b["xhat"] = e(B, self.H, self.W, self.C, dtype=F32)
-        self._b = b
-        self._pool = {}
+        return b
 
     def _scratch(self, shape, avoid=()):
         """A gradient buffer of `shape` (activation dtype) other than the tensors in `avoid`; the pool grows to the

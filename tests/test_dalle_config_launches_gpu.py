@@ -6,8 +6,10 @@ by the same helpers) at its per-GPU batch (the global batch over the data mesh a
 distinct attention type of its schedule (products do not depend on the layer count), its recompute_grad, and a
 random-init VAE stand-in of 1024 tokens.  One train_op, one eval_op, then DalleSampler on that engine: eager generate
 and generate_graphed with top-k / top-p filtering at the per-GPU batch, and complete() with an image prefix, 2 samples
-per prompt and guidance (prefill and hand-off).  Recording pauses inside the VAE's encode_tokens, whose launches the
-VAE modules own.  GEMMs are recorded at ops.gemm, everything else at its outermost ops call.
+per prompt and guidance (prefill and hand-off).  Recording pauses inside the VAE's encode_tokens: the tokenizer's
+launches are recorded at each configuration's real VAE and batch by test_vae_config_launches_gpu.py (the convolutional
+network) and test_vae_paper_kernels_gpu.py (the DALL-E paper's network).  GEMMs are recorded at ops.gemm, everything
+else at its outermost ops call.
 
 Classes.  A GEMM class carries M, N, K, the operand majors, the mode, the output dtype, alpha != 1, every epilogue
 input (bias, relu, residual, aux, colsum, dropout, ce_weights, gelu, z), split_k, n_valid < N, whether each of A, B
@@ -541,6 +543,20 @@ def _place(t, off):
     return v
 
 
+def replay_plain_gemm(ops, c, info, seed, tag=TAG):
+    """One plain product class (is_plain_gemm) at its recorded shape through DK's operands and check_gemm, its
+    operands at the recorded storage alignment.  Returns (worst err/bound, case name)."""
+    f = LC.fields(c)
+    desc = _dk_desc(c)
+    splits = DK.gemm_splits(f["M"], f["N"], f["K"], f["mode"], f["split_k"], DK._sm())
+    o = DK.gemm_operands(ops, desc, f["M"], f["K"], seed=seed, dropout=info.get("dropout"))
+    o.a, o.b, o.out = _place(o.a, f["a_off"]), _place(o.b, f["b_off"]), _place(o.out, f["d_off"])
+    DK.run_gemm(ops, o)
+    tiles = -(-f["M"] // 128) * -(-f["N"] // 128) * splits
+    name = DK.gemm_case_name(desc, f["M"], f["N"], f["K"], splits, tiles, info.get("dropout"))
+    return DK.check_gemm(f"{tag} {name}", o, splits), name
+
+
 def test_plain_gemm_classes(ops, census):
     """Every plain product (training, eval, decode, prefill) at its recorded shape through DK's operands and
     check_gemm, its operands at the recorded storage alignment."""
@@ -553,16 +569,8 @@ def test_plain_gemm_classes(ops, census):
         for i, (c, info) in enumerate(want.items()):
             case_peak()
             held = torch.cuda.memory_allocated()
-            f = LC.fields(c)
-            desc = _dk_desc(c)
-            splits = DK.gemm_splits(f["M"], f["N"], f["K"], f["mode"], f["split_k"], DK._sm())
-            o = DK.gemm_operands(ops, desc, f["M"], f["K"], seed=i, dropout=info.get("dropout"))
-            o.a, o.b, o.out = _place(o.a, f["a_off"]), _place(o.b, f["b_off"]), _place(o.out, f["d_off"])
-            DK.run_gemm(ops, o)
-            tiles = -(-f["M"] // 128) * -(-f["N"] // 128) * splits
-            name = DK.gemm_case_name(desc, f["M"], f["N"], f["K"], splits, tiles, info.get("dropout"))
-            worst = max(worst, note("GEMM", [c], DK.check_gemm(f"{TAG} {name}", o, splits)))
-            del o
+            r, name = replay_plain_gemm(ops, c, info, seed=i)
+            worst = max(worst, note("GEMM", [c], r))
             torch.cuda.synchronize()
             peaks.append((torch.cuda.max_memory_allocated(), name, held))
     assert_covered("plain GEMM", want, replayed(run))

@@ -11,7 +11,9 @@ bf16 ulp at |ref| instead of a |ref|).  One `[vae-paper-kernels] ...: worst err/
      the gemm inside it): its entry point, descriptor and which of bias / mask / residual it passes, and whether the
      residual gradient is the output buffer.  It runs at the vae_paper_b200 geometry (256^2, n_hid 256, 2 blocks x 4
      groups, n_init 128, K 8192, bf16, logit-Laplace, KL on, soft Gumbel): one training step at 8 images per GPU
-     (64 over data:8), encode_tokens and decode_tokens at 16 (dalle_coco_paper_vae_b200 tokenises 128 over data:8).
+     (64 over data:8), encode_tokens at 16 (dalle_coco_paper_vae_b200 tokenises 128 over data:8) and decode_tokens at
+     dalle_coco_paper_vae_b200's predict_batch_size, the images generate_dalle.py decodes in one call (the engine
+     runs them in passes of at most decode_pass_images()).
   2. Every recorded launch class is replayed at its recorded batch (convolutions through VK.run_conv with exactly the
      recorded flag sets), checked on the engine's own operands (the projections), or named in EXEMPT with the test
      that pins its class at equal or larger size.  Anything else fails test_every_recorded_launch_is_checked.
@@ -49,6 +51,7 @@ must_fail = VK.must_fail
 PAPER = dict(n_hid=256, n_blk_per_group=2, group_count=4, n_init=128)
 K_PAPER, SIZE = 8192, 256
 TRAIN_B, TOKENIZE_B = 8, 16          # vae_paper_b200: 64 over data:8; dalle_coco_paper_vae_b200: 128 over data:8
+DECODE_B = VK._config("dalle_coco_paper_vae_b200")["predict_batch_size"]
 TAU, BETA = 0.7, 0.034375
 
 CONV_ENTRIES = ("conv2d_fwd", "conv2d_fwd_tc", "conv2d_dgrad", "conv2d_dgrad_tc", "conv2d_wgrad", "conv2d_wgrad_tc")
@@ -74,7 +77,7 @@ EXEMPT = {
     "logit_laplace": ("test_vae_logit_laplace_gpu.py::test_logit_laplace_kernel_against_float64[1048576-3] and "
                       "test_logit_laplace_decode_mode_writes_only_the_image[1048576-3]",
                       "16 x 256^2 pixels of 3 channels (the vae_coco rows), the recorded training step's 8 x 256^2 "
-                      "and the decode's 16 x 256^2"),
+                      "and the decode passes of at most 16 x 256^2"),
 }
 
 
@@ -229,8 +232,9 @@ PROJ_PARAMS = ("encoder/output/conv/kernel", "encoder/output/conv/bias", "decode
 
 @pytest.fixture(scope="module")
 def paper_run(ops):
-    """Launches of the vae_paper_b200 step at B = 8 and of the tokenizer at B = 16, and the B = 8 step's projection
-    operands and results (a second step with the projection gradients seeded with bases sized from the first)."""
+    """Launches of the vae_paper_b200 step at B = 8, of encode_tokens at B = 16 and of decode_tokens at DECODE_B, and
+    the B = 8 step's projection operands and results (a second step with the projection gradients seeded with bases
+    sized from the first)."""
     eng = paper_engine()
     img, u = step_inputs(eng, TRAIN_B, 1)
     cap = {}
@@ -270,12 +274,21 @@ def paper_run(ops):
     keep.update({"param/" + n: eng.P(n).clone() for n in PROJ_PARAMS})
     keep["bases"] = bases
     keep["hw"], keep["n_hid"], keep["n_init"] = eng.hw, eng.n_hid, eng.n_init
-    # the tokenizer's launches at 16 images
+    # the tokenizer's launches at 16 images, decoding at DECODE_B
     img16, _ = step_inputs(eng, TOKENIZE_B, 2)
     with Recorder(eng) as rec:
         tokens = eng.encode_tokens(img16).clone()
-        eng.decode_tokens(tokens)
+        codes = tokens.repeat(_cdiv(DECODE_B, TOKENIZE_B), 1)[:DECODE_B].contiguous()
         torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        held = torch.cuda.memory_allocated()
+        images = eng.decode_tokens(codes)
+        torch.cuda.synchronize()
+    assert images.shape == (DECODE_B, SIZE, SIZE, 3) and torch.isfinite(images).all()
+    print(f"[{TAG}] decode_tokens B={DECODE_B} in passes of {eng.decode_pass_images()}: peak allocation "
+          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB, {held / 2 ** 30:.1f} GiB of it held before the call "
+          f"(the engine with its 16-image tokenizer buffers, which the first pass replaces)")
+    del images, codes
     token_launches = list(rec.launches)
     del eng
     torch.cuda.empty_cache()

@@ -220,6 +220,38 @@ def loss_coefficients(loss_weights, text_seq_len, image_seq_len, global_batch):
     return a_text, wi / ((wt + wi) * global_batch * n_image)
 
 
+LAYERNORM_WIDTHS = (256, 512, 768, 1024, 2048, 4096)   # the d db200_layernorm_fwd / _bwd_ex dispatch (csrc/rowops.cu)
+HEAD_DIMS = (64, 128)                                  # the head dims of the attention and decoding kernels
+
+
+def _count(v):
+    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+
+def validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size, n_layers=1):
+    """The head dim n_embd // n_heads of a model the kernels can run, or an error naming the knob: ValueError for a
+    malformed value, L.DB200Error for a width or head dim no kernel implements.
+
+    n_embd must be one of LAYERNORM_WIDTHS and n_embd / n_heads one of HEAD_DIMS.  Every count must be an integer >= 1.
+    text_seq_len >= 1 because the first image token is predicted at the last text position: without one, no row
+    predicts it and generation has no position to draw it from.  text_vocab_size >= 1 because the caption padding id
+    and the text window of the logits mask are text ids."""
+    for name, v in (("n_embd", n_embd), ("n_heads", n_heads), ("n_layers", n_layers), ("text_seq_len", text_seq_len),
+                    ("image_seq_len", image_seq_len), ("text_vocab_size", text_vocab_size),
+                    ("image_vocab_size", image_vocab_size)):
+        if not _count(v) or v < 1:
+            raise ValueError(f"{name} must be an integer >= 1, got {v!r}")
+    if n_embd % n_heads != 0:   # src/dalle_mtf/models.py:232
+        raise ValueError(f"n_embd {n_embd} must be divisible by n_heads {n_heads}")
+    if n_embd not in LAYERNORM_WIDTHS:
+        raise L.DB200Error(f"n_embd {n_embd} unsupported by the LayerNorm kernels (one of {LAYERNORM_WIDTHS})")
+    dh = n_embd // n_heads
+    if dh not in HEAD_DIMS:
+        raise L.DB200Error(f"head_dim {dh} = n_embd {n_embd} / n_heads {n_heads} unsupported by the attention kernels "
+                           f"(one of {HEAD_DIMS})")
+    return dh
+
+
 ACTIVATIONS = ("relu", "gelu")
 
 
@@ -287,6 +319,8 @@ class DalleEngine:
         label outside its row's window is undefined, as a label >= V is: assemble_tokens(_pp) keeps every label in its
         window as long as the caption ids are < text_vocab_size and the codes < image_vocab_size.  No parameter
         changes; prefill and decoding are unchanged (image draws already see only image ids)."""
+        self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
+                                    n_layers)
         self.activation = validate_activation(activation)
         self.gelu = self.activation == "gelu"
         self.mlp_act = {"gelu": True} if self.gelu else {"relu": True}   # linear_fwd keywords of an inference W1
@@ -295,12 +329,6 @@ class DalleEngine:
         self.per_position_padding = validate_per_position_padding(per_position_padding)
         L.require_device()
         self.d, self.L, self.H = n_embd, n_layers, n_heads
-        assert n_embd % n_heads == 0, "n_state must be divisible by n_heads"  # src/dalle_mtf/models.py:232
-        self.dh = n_embd // n_heads
-        if self.dh not in (64, 128):
-            raise L.DB200Error(f"head_dim {self.dh} unsupported by the attention kernels (64 or 128)")
-        if n_embd % 256 != 0:
-            raise L.DB200Error(f"n_embd {n_embd} must be a multiple of 256 (LayerNorm kernels)")
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
         self.S = text_seq_len + image_seq_len                       # models.py:153

@@ -38,6 +38,10 @@ from . import ops
 
 BF16, F32, I32 = torch.bfloat16, torch.float32, torch.int32
 
+# ids one filtered (top-k / top-p) draw can hold: db200_sample_rows_filtered keeps a row in one CTA's shared memory,
+# SF_MAX_N = SF_SMEM_BYTES / 4 in csrc/decode.cu.  Draws without a filter, guided or not, have no such limit.
+FILTER_MAX_IDS = 51200
+
 
 class DalleSampler:
     def __init__(self, engine, padding_id=None):
@@ -137,7 +141,12 @@ class DalleSampler:
             raise ValueError(f"top_p must lie in (0, 1] (or be None), got {top_p!r}")
         k = 0 if top_k is None or top_k >= self.e.image_vocab_size else int(top_k)
         p = 1.0 if top_p is None else float(top_p)
-        return None if (k == 0 and p == 1.0) else (k, p)
+        if k == 0 and p == 1.0:
+            return None
+        if self.e.image_vocab_size > FILTER_MAX_IDS:
+            raise ValueError(f"top_k / top_p filter at most {FILTER_MAX_IDS} image tokens, but image_vocab_size = "
+                             f"{self.e.image_vocab_size}; sample without a filter")
+        return k, p
 
     @staticmethod
     def _guidance(scale):

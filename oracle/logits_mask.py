@@ -64,15 +64,20 @@ def dlogits(logits, labels, text_seq_len, image_seq_len, image_offset, weights=N
 
 
 def loss_and_grads(params, tokens, cfg, image_offset, weights=None, z=0.0, global_batch=None, quirks=None,
-                   forward=None):
+                   forward=None, mask=True):
     """Autograd of masked_loss on top of a forward pass: (loss, rows, parts, logits, grads).  forward(leaves, tokens)
-    returns (loss, loss_batch, logits) (default oracle.dalle.forward with cfg); cfg.eos_token_id is the last id."""
+    returns (loss, loss_batch, logits) (default oracle.dalle.forward with cfg); cfg.eos_token_id is the last id.
+    mask False: the same with every row over the whole vocabulary (oracle.loss_weights.weighted_loss of the logits)."""
     leaves = {k: v.clone().requires_grad_(True) for k, v in params.items()}
     fwd = forward or (lambda p, t: O.forward(p, t, cfg))
     _, _, logits = fwd(leaves, tokens)
     labels = O.shift_labels(tokens, logits.shape[-1] - 1)
-    loss, rows, parts = masked_loss(logits, labels, cfg.text_seq_len, cfg.image_seq_len, image_offset, weights, z,
-                                    global_batch, quirks)
+    if mask:
+        loss, rows, parts = masked_loss(logits, labels, cfg.text_seq_len, cfg.image_seq_len, image_offset, weights, z,
+                                        global_batch, quirks)
+    else:
+        loss, rows, parts = OW.weighted_loss(logits, labels, cfg.text_seq_len, cfg.image_seq_len, weights, z,
+                                             global_batch)
     loss.backward()
     grads = {k: (v.grad if v.grad is not None else torch.zeros_like(v)) for k, v in leaves.items()}
     return loss.detach(), rows.detach(), tuple(p.detach() for p in parts), logits.detach(), grads

@@ -30,11 +30,15 @@ SHAPES = [(256, 2, 2, 300, 64, 24, 40, 3, 29), (256, 2, 4, 500, 100, 70, 90, 2, 
 
 
 def sharp_engine(d, L, H, tv, iv, ts, isl, **kw):
-    """Oracle-initialised engine with sharpened weights (clear arg-maxima), as in test_sampling_gpu.py."""
+    """Oracle-initialised engine with sharpened weights (clear arg-maxima), as in test_sampling_gpu.py.  With the
+    image_position_embedding / per_position_padding keywords the parameters are oracle/dalle_input.py's."""
     from dalle_mtf_b200.dalle_engine import DalleEngine
     from oracle import dalle as O
+    from oracle import dalle_input as I
     cfg = O.DalleConfig(d, L, H, tv, iv, ts, isl)
-    params = O.init_params(cfg, 3)
+    pp = bool(kw.get("per_position_padding"))
+    inp = I.InputConfig(kw.get("image_position_embedding") or "absolute", pp, tv - 1 if pp else None)
+    params = I.init_params(cfg, inp, 3)
     g = torch.Generator().manual_seed(9)
     for k in params:
         if k.endswith("/b") or k.endswith("bias") or k.endswith("o_b"):
@@ -157,12 +161,15 @@ def test_prefill_between_forward_and_backward_leaves_the_gradients_alone():
 def greedy_agrees_with_full_forward(eng, out, P):
     """Every sampled token equals the full forward pass's argmax wherever its top-2 margin is clear (the criterion of
     test_sampling_gpu.py)."""
-    tv, iv, S = eng.text_vocab_size, eng.image_vocab_size, eng.S
+    io, iv, S = eng.image_offset, eng.image_vocab_size, eng.S
     full = eng.logits(out)
-    rng = full[:, P - 1:S - 1, tv:tv + iv]
+    if iv == 1:   # one image code: every draw is it
+        assert (out[:, P:] == io).all()
+        return
+    rng = full[:, P - 1:S - 1, io:io + iv]
     top2 = rng.topk(2, -1).values
     clear = (top2[..., 0] - top2[..., 1]) > 0.05 * rng.abs().max()
-    same = (rng.argmax(-1) + tv) == out[:, P:]
+    same = (rng.argmax(-1) + io) == out[:, P:]
     assert (same | ~clear).all() and clear.float().mean() > 0.2 and same.float().mean() > 0.8
 
 

@@ -329,7 +329,7 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // ------------------------------------------------------------------ consumer warpgroups
     setmaxnreg_inc<PP_REGS_MMA>();
     const int wg = (warp - 4) >> 2;
-    const FragCtx f = frag_ctx(stg_base + wg * 4 * STG_BYTES, threadIdx.x & 127, PP_BAR_PAIR + 2 * wg);
+    const FragCtx f = frag_ctx<0>(stg_base + wg * 4 * STG_BYTES, threadIdx.x & 127, PP_BAR_PAIR + 2 * wg);
     constexpr uint64_t astep = TA ? 128u : 2u, bstep = TB ? 128u : 2u;
     constexpr uint32_t a_chain = TA ? SLAB_BYTES : 64u * 128u;  // rows 64-127 of the A stage
     float d[2 * (BN / 2)];
@@ -366,8 +366,8 @@ gemm_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
       const int m0 = t.m_blk * BM, n0 = t.n_blk * BN;
       switch (p.mode) {
-        case DB200_EPI_STORE:    frag_store(p, d, f, m0, n0); break;
-        case DB200_EPI_RELU_BWD: frag_relu_bwd(p, d, f, m0, n0); break;
+        case DB200_EPI_STORE:    frag_store<0>(p, d, f, m0, n0); break;
+        case DB200_EPI_RELU_BWD: frag_relu_bwd<0>(p, d, f, m0, n0); break;
         case DB200_EPI_CE_GRAD:  frag_ce_grad(p, d, f, m0, n0); break;
         default: break;
       }
@@ -385,6 +385,168 @@ static int launch_gemm_pp(cudaStream_t stream, const CUtensorMap& tmA, const CUt
   const int grid = total < sm_count() ? total : sm_count();
   gemm_pp_kernel<TA, TB><<<grid, PP_THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p);
   return check_launch("gemm_pp_kernel");
+}
+
+// ----------------------------------------------------------------------------------------------------------------------
+// The wide kernel for long contractions (gemm_run picks it by K, epilogue and tile count).  A 128 x 128 tile loads
+// (128 + 128) x K bf16 operands from L2 for 2 x 128 x 128 x K FLOP; a 128 x 256 tile loads (128 + 256) x K for twice
+// the FLOP, a quarter less L2 -> shared-memory traffic per FLOP, and the long-K products on 128 x 128 tiles level off
+// near 10 TB/s of it (DESIGN.md §3).  Warpgroup g issues wgmma m64n256 for rows [64 g, 64 g + 64) of the tile (128
+// accumulators per thread) and, when the tile's mainloop is done, runs its epilogue from those registers
+// (gemm_common.cuh: fragment epilogues, chains side by side).  The epilogue overlaps only the producer's loads for
+// the next tile, not its MMAs.  Each element gets the k16 steps of gemm_tc_kernel in the same k-block order and the
+// same per-element epilogue expression.
+//
+//   warp 0     : TMA producer              smem ring: W_STAGES x {A 128x64, B 256x64} bf16 (48 KiB per stage)
+//   warps 1-3  : idle (they hand their registers to the consumers and exit)
+//   warps 4-11 : two MMA warpgroups, rows [64 g, 64 g + 64) of every tile of the CTA
+// ----------------------------------------------------------------------------------------------------------------------
+constexpr int WBN = 256;
+constexpr int W_STAGES = 4;
+constexpr uint32_t W_B_BYTES = WBN * BK * 2;
+constexpr uint32_t W_STAGE_BYTES = A_BYTES + W_B_BYTES;
+constexpr size_t W_SMEM_BYTES =
+    1024 /*align slack*/ + size_t(W_STAGES) * W_STAGE_BYTES + 256 /*barriers*/ + 8 * STG_BYTES;
+static_assert(W_SMEM_BYTES <= 227 * 1024, "wide GEMM shared memory exceeds the H100 per-block limit");
+// named barriers: W_BAR_PAIR + 2 g + {0, 1}: the two warp pairs of warpgroup g around their staging blocks
+constexpr int W_BAR_PAIR = 1;
+
+// STORE without dropout and RELU_BWD.  The single-split ATOMIC vocabulary wgrad (both operands MN-major) measured
+// no faster on 128 x 256 tiles, and split-K, CE, GELU and dropout products stay with their kernels.
+static bool wide_has_epilogue(int mode, bool drop, bool wce, int gelu) {
+  return !drop && !wce && !gelu && (mode == DB200_EPI_STORE || mode == DB200_EPI_RELU_BWD);
+}
+// A product needs at least this many 128 x 256 tiles per SM for the wide kernel: at one tile per SM it measured as
+// fast as the 128 x 128 kernel, from two on 1.15x and more.  -DDB200_WIDE_MIN_TILES=<n> moves the rule in a side
+// build (tools/bench_gemm_shapes.py --sweep).
+#ifndef DB200_WIDE_MIN_TILES
+#define DB200_WIDE_MIN_TILES 2
+#endif
+constexpr int WIDE_MIN_TILES = DB200_WIDE_MIN_TILES;
+
+template <int TA, int TB>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  constexpr int STAGES = W_STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t sA = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024-byte alignment
+  const uint32_t sB = sA + STAGES * A_BYTES;
+  const uint32_t bars = sA + STAGES * W_STAGE_BYTES;
+  const uint32_t full_bar = bars;                // STAGES x 8 B
+  const uint32_t empty_bar = bars + 8 * STAGES;  // STAGES x 8 B
+  const uint32_t stg_base = bars + 256;          // 2 warpgroups x 4 x STG_BYTES, 256-byte aligned
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+  }
+  if (warp == 1 && lane == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(full_bar + 8 * i, 1);
+      mbar_init(empty_bar + 8 * i, 2);  // one arrive per MMA warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int total_tiles = p.m_tiles * p.n_tiles;  // n_tiles counts 256-wide tiles; never split-K
+
+  if (warp < 4) {
+    setmaxnreg_dec<PP_REGS_PRODUCER>();
+    if (warp != 0) return;
+    // ------------------------------------------------------------------ TMA producer
+    // the tensor maps are gemm_tc_kernel's (B boxes of 128 rows or 2 slabs): a 256-wide B stage takes two of them
+    uint32_t stage = 0, phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
+      const int m0 = t.m_blk * BM, n0 = t.n_blk * WBN;
+      for (int kb = 0; kb < p.kb_total; ++kb) {
+        mbar_wait_mma(empty_bar + 8 * stage, phase ^ 1);
+        const uint32_t fb = full_bar + 8 * stage;
+        if (elect_one_sync()) {
+          mbar_expect_tx(fb, W_STAGE_BYTES);
+          const int k0 = kb * BK;
+          const uint32_t a_dst = sA + stage * A_BYTES;
+          const uint32_t b_dst = sB + stage * W_B_BYTES;
+          if (p.a_3d) {
+            tma_load_3d(a_dst, &tmA, fb, 0, k0, m0 >> 6);
+          } else if (p.a_mn) {
+#pragma unroll
+            for (int s = 0; s < BM / 64; ++s) tma_load_2d(a_dst + s * SLAB_BYTES, &tmA, fb, m0 + 64 * s, k0);
+          } else {
+            tma_load_2d(a_dst, &tmA, fb, k0, m0);
+          }
+          if (p.b_3d) {
+#pragma unroll
+            for (int s = 0; s < WBN / GBN; ++s)
+              tma_load_3d(b_dst + s * G_B_BYTES, &tmB, fb, 0, k0, (n0 >> 6) + s * (GBN / 64));
+          } else if (p.b_mn) {
+#pragma unroll
+            for (int s = 0; s < WBN / 64; ++s) tma_load_2d(b_dst + s * SLAB_BYTES, &tmB, fb, n0 + 64 * s, k0);
+          } else {
+#pragma unroll
+            for (int s = 0; s < WBN / GBN; ++s) tma_load_2d(b_dst + s * G_B_BYTES, &tmB, fb, k0, n0 + GBN * s);
+          }
+        }
+        __syncwarp();
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    // ------------------------------------------------------------------ MMA warpgroups
+    setmaxnreg_inc<PP_REGS_MMA>();
+    const int wg = (warp - 4) >> 2;  // rows [64 wg, 64 wg + 64) of every tile
+    const FragCtx f = frag_ctx<WBN / 2>(stg_base + wg * 4 * STG_BYTES, threadIdx.x & 127, W_BAR_PAIR + 2 * wg);
+    constexpr uint64_t astep = TA ? 128u : 2u, bstep = TB ? 128u : 2u;
+    const uint32_t a_wg = wg * (TA ? SLAB_BYTES : 64u * 128u);
+    float d[WBN / 2];
+    uint32_t stage = 0, phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
+      uint32_t prev_stage = 0;
+#pragma unroll
+      for (int i = 0; i < WBN / 2; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < p.kb_total; ++kb) {
+        mbar_wait_mma(full_bar + 8 * stage, phase);
+        const uint64_t ad0 = smem_desc_sw128(sA + stage * A_BYTES + a_wg, TA ? SLAB_BYTES : 0u, 1024);
+        const uint64_t bd0 = smem_desc_sw128(sB + stage * W_B_BYTES, TB ? SLAB_BYTES : 0u, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_m64n256<TA, TB>(d, ad0 + k * astep, bd0 + k * bstep, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+      const int m0 = t.m_blk * BM + 64 * wg, n0 = t.n_blk * WBN;
+      switch (p.mode) {
+        case DB200_EPI_STORE:    frag_store<WBN / 2>(p, d, f, m0, n0); break;
+        case DB200_EPI_RELU_BWD: frag_relu_bwd<WBN / 2>(p, d, f, m0, n0); break;
+        default: break;
+      }
+    }
+  }
+}
+
+template <int TA, int TB>
+static int launch_gemm_wide(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p) {
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_wide_kernel<TA, TB>,
+                                                          cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                          (int)W_SMEM_BYTES);  // once, thread-safe (magic static)
+  DB200_CUDA(attr_rc);
+  p.n_tiles = (p.N + WBN - 1) / WBN;
+  const int total = p.m_tiles * p.n_tiles;
+  const int grid = total < sm_count() ? total : sm_count();
+  gemm_wide_kernel<TA, TB><<<grid, PP_THREADS, W_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  return check_launch("gemm_wide_kernel");
 }
 
 template <int TA, int TB, bool DROP, bool WCE = false, int GELU = 0>
@@ -558,9 +720,15 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   }
   // Short contractions with a fragment epilogue run on the ping-pong kernel.  The rule reads the epilogue, K and the
   // operand majors only, never M: prefill (M = B P) and training (M = B S) must take the same path, bit for bit.
+  // Long ones with enough tiles run on the wide kernel, which gives every element gemm_tc_kernel's bits.
+  const int wide_tiles = p.m_tiles * ((N + WBN - 1) / WBN);
   if (kb_total <= PP_MAX_KB && pp_has_epilogue(mode, drop, cew != nullptr, gelu)) {
     if (p.a_mn) rc = p.b_mn ? launch_gemm_pp<1, 1>(stream, tmA, tmB, p) : launch_gemm_pp<1, 0>(stream, tmA, tmB, p);
     else        rc = p.b_mn ? launch_gemm_pp<0, 1>(stream, tmA, tmB, p) : launch_gemm_pp<0, 0>(stream, tmA, tmB, p);
+  } else if (kb_total > PP_MAX_KB && wide_has_epilogue(mode, drop, cew != nullptr, gelu) &&
+             wide_tiles >= WIDE_MIN_TILES * sm_count()) {
+    if (p.a_mn) rc = p.b_mn ? launch_gemm_wide<1, 1>(stream, tmA, tmB, p) : launch_gemm_wide<1, 0>(stream, tmA, tmB, p);
+    else        rc = p.b_mn ? launch_gemm_wide<0, 1>(stream, tmA, tmB, p) : launch_gemm_wide<0, 0>(stream, tmA, tmB, p);
   } else if (gelu == G_GELU_FWD)   // the MLP's W1 forward: A k-major, B mn-major
     rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, false, G_GELU_FWD>(stream, tmA, tmB, p)
                              : set_error(DB200_E_UNSUPPORTED, "gemm_gelu: needs a k-major A and an mn-major B");

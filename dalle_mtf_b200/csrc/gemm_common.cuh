@@ -646,6 +646,10 @@ __device__ __forceinline__ void epi_ce_grad_weighted(const GemmParams& p, uint32
 // two warps 2 (b % 2), 2 (b % 2) + 1 of chain b / 2, which fill that row block's [32 rows][128 B] staging block
 // together (a 64-thread named barrier around it); one of the two then runs the unchanged stage_fetch_bf16 /
 // stage_colsum_bf16 / stage_flush on it.  A warp pair serves two blocks (one per chain) and each warp owns one.
+// gemm_wide_kernel's warpgroups hold a 64 x 256 slice as one m64n256 fragment, whose two halves are the m64n128
+// fragments of columns [0, 128) and [128, 256): the same registers with the chains side by side instead of stacked.
+// Template parameter CW says which: 0 (chain c at rows 64 c) or 128 (chain c at columns 128 c); warp pair b / 2 of a
+// wide warpgroup then stages rows [32 b, 32 b + 32) of its slice for both column halves.
 // ------------------------------------------------------------------------------------------------------------------
 __host__ __device__ constexpr int frag_idx(int c, int i, int h) { return c * 64 + 4 * i + 2 * h; }
 
@@ -655,15 +659,19 @@ struct FragCtx {
   int lane, q;      // q = lane % 4: the thread's column pair inside every 8-column group
   int row;          // tile row of (chain 0, half 0): 16 (t / 32) + (t % 32) / 4
   int own_row0;     // first tile row of that block
+  int own_col;      // its first column, relative to the chain 0 column of the same 64-column group
   int bar;          // named barrier of the warp pair
 };
+template <int CW>
 __device__ __forceinline__ FragCtx frag_ctx(uint32_t stg_wg, int wg_thread, int bar0) {
+  static_assert(CW == 0 || CW == 128, "chains stacked in rows or side by side in columns");
   FragCtx f;
   const int w = wg_thread >> 5;
   f.lane = wg_thread & 31;
   f.q = f.lane & 3;
   f.row = 16 * w + (f.lane >> 2);
-  f.own_row0 = 64 * (w & 1) + 32 * (w >> 1);
+  f.own_row0 = (CW ? 0 : 64 * (w & 1)) + 32 * (w >> 1);
+  f.own_col = CW * (w & 1);
   f.own_stg = stg_wg + (2 * (w & 1) + (w >> 1)) * STG_BYTES;
   f.bar = bar0 + (w >> 1);
   const int r = 16 * (w & 1) + (f.lane >> 2);  // row inside the block; r % 8 == lane / 4 for both row halves
@@ -726,22 +734,26 @@ __device__ __forceinline__ void frag_bias(const float* bias, int col0, int q, in
 // the owner's work on its staged bf16 block: fused column sums (when asked for) and the flush to D
 template <bool STREAM>
 __device__ __forceinline__ void frag_flush_bf16(const GemmParams& p, const FragCtx& f, int m0, int colp, bool colsum) {
-  const int row0 = m0 + f.own_row0;
-  if (colsum) stage_colsum_bf16(f.own_stg, p.colsum + (long long)(row0 >> 5) * p.N, colp, p.N, f.lane);
-  stage_flush<2, STREAM>(f.own_stg, p.D, p.ldd, row0, colp, p.M, p.N, f.lane);
+  const int row0 = m0 + f.own_row0, col0 = colp + f.own_col;
+  if (colsum) stage_colsum_bf16(f.own_stg, p.colsum + (long long)(row0 >> 5) * p.N, col0, p.N, f.lane);
+  stage_flush<2, STREAM>(f.own_stg, p.D, p.ldd, row0, col0, p.M, p.N, f.lane);
 }
 
+// m0, n0: the fragment's first row and column (chain 0).  Side-by-side chains past N stage values the bounded
+// fetches, sums and flushes then ignore.
+template <int CW>
 __device__ __forceinline__ void frag_store(const GemmParams& p, float (&d)[128], const FragCtx& f, int m0, int n0) {
 #pragma unroll
   for (int hp = 0; hp < 2; ++hp) {
     const int colp = n0 + hp * 64;
     if (colp >= p.N) break;  // uniform over the tile
     if (p.residual) {
-      stage_fetch_bf16(f.own_stg, p.residual, p.ldr, m0 + f.own_row0, colp, p.M, p.N, f.lane);
+      stage_fetch_bf16(f.own_stg, p.residual, p.ldr, m0 + f.own_row0, colp + f.own_col, p.M, p.N, f.lane);
       pair_sync(f);
     }
-    float2 b[8];
-    frag_bias(p.bias, colp, f.q, p.N, b);
+    float2 b[CW ? 2 : 1][8];
+#pragma unroll
+    for (int c = 0; c < (CW ? 2 : 1); ++c) frag_bias(p.bias, colp + CW * c, f.q, p.N, b[c]);
 #pragma unroll
     for (int c = 0; c < 2; ++c)
 #pragma unroll
@@ -756,8 +768,8 @@ __device__ __forceinline__ void frag_store(const GemmParams& p, float (&d)[128],
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int k = frag_idx(c, 8 * hp + i, h);
-            d[k] += b[i].x;
-            d[k + 1] += b[i].y;
+            d[k] += b[CW ? c : 0][i].x;
+            d[k + 1] += b[CW ? c : 0][i].y;
           }
         }
         if (p.relu) {
@@ -789,19 +801,20 @@ __device__ __forceinline__ void frag_store(const GemmParams& p, float (&d)[128],
       for (int s = 0; s < 2; ++s) {
         frag_put_f32(f, d, 2 * hp + s);
         pair_sync(f);
-        stage_flush<4>(f.own_stg, p.D, p.ldd, m0 + f.own_row0, colp + 32 * s, p.M, p.N, f.lane);
+        stage_flush<4>(f.own_stg, p.D, p.ldd, m0 + f.own_row0, colp + f.own_col + 32 * s, p.M, p.N, f.lane);
         pair_sync(f);
       }
     }
   }
 }
 
+template <int CW>
 __device__ __forceinline__ void frag_relu_bwd(const GemmParams& p, float (&d)[128], const FragCtx& f, int m0, int n0) {
 #pragma unroll
   for (int hp = 0; hp < 2; ++hp) {
     const int colp = n0 + hp * 64;
     if (colp >= p.N) break;
-    stage_fetch_bf16(f.own_stg, p.aux, p.ldaux, m0 + f.own_row0, colp, p.M, p.N, f.lane);
+    stage_fetch_bf16(f.own_stg, p.aux, p.ldaux, m0 + f.own_row0, colp + f.own_col, p.M, p.N, f.lane);
     pair_sync(f);
 #pragma unroll
     for (int c = 0; c < 2; ++c)

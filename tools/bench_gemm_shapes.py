@@ -11,11 +11,19 @@ The products (shape, operand majors, epilogue and its inputs) are recorded from 
   --sweep                       also the MLP's W1 forward (STORE, bias + ReLU, M x 4K x K) at K = 512, 1024, 2048 and
                                 4096 with M K = 40 960 x 512: the contraction lengths around the rule that picks the
                                 ping-pong kernel (K <= 1024).  A build with -DDB200_PP_MAX_KB=<k-blocks> moves the rule.
+                                And the MLP's W2 forward shape (STORE, bias, M x 512 x 2048) at M = 64 t SMs rows,
+                                t = 1 .. 5 tiles of 128 x 256 per SM: the counts around the rule that picks the wide
+                                kernel (t >= 2).  A build with -DDB200_WIDE_MIN_TILES=<t> moves the rule.
+
+For every build a line also names the GEMM kernel the product ran on (read from one profiled launch) and the operand
+bytes its tile shape moves from L2 into shared memory: every 128 x BN output tile loads (128 + BN) K bf16 values
+(BN = 256 on gemm_wide_kernel, 128 otherwise), divided by the kernel time.  Split-K products load the same total.
 
 Every line carries the GPU's name, its power limit and SM clocks, read in the same run.  Fails without a GPU."""
 import argparse
 import json
 import os
+import re
 import subprocess
 import sys
 
@@ -140,11 +148,34 @@ def timed(fn, n):
     return e0.elapsed_time(e1) / n
 
 
+def gemm_kernel(fn):
+    """Name of the GEMM kernel one launch of fn runs (its split-K or column-sum reductions aside)."""
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    names = {m.group(0) for e in prof.events() if e.device_type == DeviceType.CUDA
+             for m in [re.search(r"gemm_(tc|pp|wide)_kernel", e.name)] if m}
+    if len(names) != 1:
+        raise SystemExit(f"expected one GEMM kernel per launch, saw {sorted(names) or 'none'}")
+    return names.pop()
+
+
+def l2_operand_bytes(M, N, K, kernel):
+    """Bytes the product's 128 x BN tiles load from L2 into shared memory: (128 + BN) K bf16 values per tile."""
+    bn = 256 if kernel == "gemm_wide_kernel" else 128
+    tiles = -(-M // 128) * -(-N // bn)
+    return bn, tiles * (128 + bn) * K * 2
+
+
 def bench(name, shape, fn, libs, launches, rounds, info, family):
     M, N, K = shape
-    for lib in libs.values():
+    kernels = {}
+    for k, lib in libs.items():
         L._lib = lib
         timed(fn, 3)
+        kernels[k] = gemm_kernel(fn)
     ms = {k: [] for k in libs}
     clocks = []
     for _ in range(rounds):
@@ -155,8 +186,10 @@ def bench(name, shape, fn, libs, launches, rounds, info, family):
     row = {"bench": family, "product": name, "M": M, "N": N, "K": K, "launches": launches,
            "sm_clock_after_rounds": clocks, **info}
     for k, v in ms.items():
+        bn, l2_bytes = l2_operand_bytes(M, N, K, kernels[k])
         row[k] = {"ms_min": round(min(v), 4), "tflops": round(2.0 * M * N * K / min(v) / 1e9, 1),
-                  "ms_rounds": [round(x, 4) for x in v]}
+                  "ms_rounds": [round(x, 4) for x in v], "kernel": kernels[k], "tile": f"128x{bn}",
+                  "l2_operand_gb": round(l2_bytes / 1e9, 2), "l2_operand_tbps": round(l2_bytes / min(v) / 1e9, 2)}
     names = list(libs)
     if len(names) > 1:
         base = names[0]
@@ -188,6 +221,13 @@ def main():
             key = (T * 512 // K, 4 * K, K, False, True, L.EPI_STORE, False, True, True, False, False, 1, 0, False)
             name, shape, fn = make_call(key)
             bench(name, shape, fn, libs, args.launches, args.rounds, info, "w1_forward_by_K")
+            del fn
+            torch.cuda.empty_cache()
+        sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+        for t in (1, 2, 3, 4, 5):
+            key = (64 * t * sms, 512, 2048, False, True, L.EPI_STORE, False, True, False, False, False, 1, 0, False)
+            name, shape, fn = make_call(key)
+            bench(name, shape, fn, libs, args.launches, args.rounds, info, "w2_forward_by_wide_tiles_per_sm")
             del fn
             torch.cuda.empty_cache()
 

@@ -263,6 +263,31 @@ def validate_activation(activation):
     return activation
 
 
+def validate_rotary(rotary_dim, rotary_base, head_dim):
+    """(r, base) of rotary position embeddings, or None without them.  rotary_dim None: off (rotary_base must then be
+    None too); otherwise an even integer 2 <= r <= head_dim.  rotary_base None is 10000, else a finite real > 1."""
+    if rotary_dim is None:
+        if rotary_base is not None:
+            raise ValueError(f"rotary_base = {rotary_base!r} given without rotary_dim")
+        return None
+    if not _count(rotary_dim) or rotary_dim % 2 or not 2 <= rotary_dim <= head_dim:
+        raise ValueError(f"rotary_dim = {rotary_dim!r}: must be an even integer with 2 <= rotary_dim <= head_dim "
+                         f"{head_dim} (or null)")
+    base = 10000.0 if rotary_base is None else rotary_base
+    if not (_real(base) and math.isfinite(base) and base > 1):
+        raise ValueError(f"rotary_base = {rotary_base!r}: must be a finite number > 1")
+    return int(rotary_dim), float(base)
+
+
+def rope_table(n_pos, rotary_dim, base):
+    """The fp32 [n_pos, 2, rotary_dim / 2] table of the rotary kernels: position p's cos(p theta_j), then its
+    sin(p theta_j), theta_j = base^(-2j / rotary_dim), each evaluated in float64 and rounded once to fp32."""
+    h = rotary_dim // 2
+    theta = torch.tensor([base ** (-2.0 * j / rotary_dim) for j in range(h)], dtype=torch.float64)
+    angle = torch.arange(n_pos, dtype=torch.float64)[:, None] * theta[None, :]
+    return torch.stack([torch.cos(angle), torch.sin(angle)], dim=1).to(F32)
+
+
 class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
@@ -273,7 +298,7 @@ class DalleEngine:
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
-                 activation="relu", logits_mask=False):
+                 activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -318,9 +343,17 @@ class DalleEngine:
         that block's columns only (_masked_forward / _masked_backward); logits() returns -inf outside the windows.  A
         label outside its row's window is undefined, as a label >= V is: assemble_tokens(_pp) keeps every label in its
         window as long as the caption ids are < text_vocab_size and the codes < image_vocab_size.  No parameter
-        changes; prefill and decoding are unchanged (image draws already see only image ids)."""
+        changes; prefill and decoding are unchanged (image draws already see only image ids).
+
+        rotary_dim r (None: off) and rotary_base (None: 10000): rotary position embeddings, GPT-NeoX's rotate_half
+        layout with partial rotary (validate_rotary).  After the q|k|v product, the pair (x_j, x_{j+r/2}) of the first r
+        dims of every q and k head of every layer is rotated by p theta_j, p the token's sequence index and theta_j =
+        base^(-2j/r), in fp32 and rounded to bf16 (ops.rope_fwd); backward applies the transpose to dq and dk, and the
+        decoder rotates each step's q and k before they reach the cache.  v, the attention scale and the learned
+        position embeddings are unchanged, and no parameter is added."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
+        self.rotary = validate_rotary(rotary_dim, rotary_base, self.dh)
         self.activation = validate_activation(activation)
         self.gelu = self.activation == "gelu"
         self.mlp_act = {"gelu": True} if self.gelu else {"relu": True}   # linear_fwd keywords of an inference W1
@@ -414,6 +447,9 @@ class DalleEngine:
             self.pos_table = torch.zeros(S, d, dtype=BF16, device=dev)
             self._dpos = torch.zeros(S, d, dtype=F32, device=dev)
         self.gnorm_sq = torch.zeros(1, dtype=F32, device=dev)
+        # rotary position embeddings: r (None: off) and the cos / sin table of every position, built once
+        self.rotary_dim = self.rotary[0] if self.rotary else None
+        self.rope_table = rope_table(S, *self.rotary).to(dev) if self.rotary else None
         self._grads_clean = False
         self._bufs = None
         self._buf_key = None
@@ -724,6 +760,8 @@ class DalleEngine:
         ops.layernorm_fwd(x_in, self.P(p + "ln1_g"), self.P(p + "ln1_b"), sv["ln1"], sv["mean1"], sv["rstd1"],
                           self.ln_eps)
         ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
+        if self.rotary:
+            ops.rope_fwd(sv["qkv"], self.rope_table, S or self.S, self.H, self.dh, self.rotary_dim)
         ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
                      dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
                      **self.conv_kw[i])  # :257-299
@@ -974,6 +1012,8 @@ class DalleEngine:
         ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"], B,
                      self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i), radius=self.radii[i],
                      **self.axial_kw[i], **self.conv_kw[i])
+        if self.rotary:   # d(q|k|v) before the rotation
+            ops.rope_bwd(bufs["dqkv"], self.rope_table, self.S, self.H, self.dh, self.rotary_dim)
         ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                      # dLN1 out
         ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
         return self._ln_bwd(bufs["dtmp"], x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,

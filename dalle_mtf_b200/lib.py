@@ -158,6 +158,10 @@ _SIGNATURES = {
                                  c_f32, c_vp],
     "db200_kv_cache_fill": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_rows_repeat": [c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int],
+    "db200_rope_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_rope_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_rope_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
+    "db200_rope_decode_dev": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
     "db200_crc32c": [c_vp, c_u64, c_vp],
     "db200_tfrecord_masked_crc": [c_vp, c_u64, c_vp],
     "db200_tfrecord_frame": [c_vp, c_u64, c_vp],

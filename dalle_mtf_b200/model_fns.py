@@ -15,7 +15,8 @@ import torch
 from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
-    validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding
+    validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
+    validate_rotary
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -217,6 +218,20 @@ def logits_mask(params):
     return validate_logits_mask(params.get("logits_mask"))
 
 
+def rotary_embedding(params, n_embd=None, n_heads=None):
+    """(rotary_dim, rotary_base) of a DALL-E config's rotary position embeddings (extension keys; DalleEngine): both
+    (None, None) when rotary_dim is absent or null.  rotary_dim must be an even integer with 2 <= rotary_dim <= the
+    head dim n_embd / n_heads (taken from params unless given), rotary_base a finite number > 1 (absent or null:
+    10000); rotary_base without rotary_dim, and any other value, is rejected.  No parameter depends on them, so
+    checkpoints keep their layout."""
+    n_embd = params.get("n_embd") if n_embd is None else n_embd
+    n_heads = params.get("n_heads") if n_heads is None else n_heads
+    count = lambda v: isinstance(v, numbers.Integral) and not isinstance(v, bool)   # noqa: E731
+    dh = n_embd // n_heads if count(n_embd) and count(n_heads) and n_heads > 0 else 0
+    rot = validate_rotary(params.get("rotary_dim"), params.get("rotary_base"), dh)
+    return (None, None) if rot is None else rot
+
+
 def dalle_model_fn(features, labels, mode, params):
     """src/model_fns.py:55-236.  features: images f32 [B,H,W,C] in [-1,1] (NHWC); labels: caption ids i32
     [B, text_seq_len].  (The reference's own comment has them swapped; the code uses them this way.)"""
@@ -230,6 +245,7 @@ def dalle_model_fn(features, labels, mode, params):
     pos_scheme, per_pos, pp_pad = input_embedding(params)
     activation = activation_function(params)
     mask = logits_mask(params)
+    rotary_dim, rotary_base = rotary_embedding(params)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -263,7 +279,7 @@ def dalle_model_fn(features, labels, mode, params):
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
-                        activation=activation, logits_mask=mask)
+                        activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

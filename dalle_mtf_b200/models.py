@@ -7,7 +7,7 @@ import torch
 from . import lib as L
 from .dalle_engine import DalleEngine
 from .model_fns import activation_function, attention_layers, conv_kernel, dropout_rates, input_embedding, \
-    logits_mask, loss_weights, validate_kl_weight
+    logits_mask, loss_weights, rotary_embedding, validate_kl_weight
 from .model_fns import build_vae_engine, vae_architecture
 from .model_fns import reconstruction_loss as _reconstruction_loss
 
@@ -30,6 +30,7 @@ class DALLE:
         pos_scheme, per_pos, _ = input_embedding({**params, "text_vocab_size": text_vocab_size})
         activation = activation_function(params)
         mask = logits_mask(params)
+        rotary_dim, rotary_base = rotary_embedding(params, n_embd, n_heads)
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
@@ -44,7 +45,8 @@ class DALLE:
                                   attention_types=attention_types, local_attention_radius=local_radius,
                                   conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                                   image_position_embedding=pos_scheme, per_position_padding=per_pos,
-                                  activation=activation, logits_mask=mask)
+                                  activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
+                                  rotary_base=rotary_base)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

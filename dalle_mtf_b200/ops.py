@@ -1008,6 +1008,50 @@ def kv_cache_fill(qkv, k_cache, v_cache, P, rep=1):
                                        int(rep)), "db200_kv_cache_fill")
 
 
+def _rope_args(qkv, table, H, dh, r, what):
+    """(rows, table positions) of a rotary call after the dtype / shape checks."""
+    L.require_device()
+    _chk(qkv, BF16, what); _chk(table, F32, "table")
+    if not qkv.is_contiguous() or qkv.dim() != 2 or qkv.shape[1] != 3 * H * dh:
+        raise L.DB200Error(f"{what}: expected a contiguous [rows, {3 * H * dh}] q|k|v buffer, got {tuple(qkv.shape)}")
+    if not table.is_contiguous() or table.dim() != 3 or tuple(table.shape[1:]) != (2, r // 2):
+        raise L.DB200Error(f"{what}: expected a contiguous [n_pos, 2, {r // 2}] table, got {tuple(table.shape)}")
+    return qkv.shape[0], table.shape[0]
+
+
+def rope_fwd(qkv, table, S, H, dh, r):
+    """Rotary position embedding in place on the q and k columns of qkv [rows, 3*H*dh] (bf16), row t at position
+    t mod S, with the first r dims of each head rotated by the fp32 cos / sin table [n_pos >= S, 2, r/2]
+    (include/dalle_b200.h)."""
+    rows, n_pos = _rope_args(qkv, table, H, dh, r, "rope_fwd")
+    if S > n_pos:
+        raise L.DB200Error(f"rope_fwd: period S {S} exceeds the table's {n_pos} positions")
+    check(L.load().db200_rope_fwd(stream_ptr(), ptr(qkv), ptr(table), rows, int(S), H, dh, int(r)), "db200_rope_fwd")
+
+
+def rope_bwd(dqkv, table, S, H, dh, r):
+    """The transpose of rope_fwd in place on the dq and dk columns of dqkv [rows, 3*H*dh] (bf16)."""
+    rows, n_pos = _rope_args(dqkv, table, H, dh, r, "rope_bwd")
+    if S > n_pos:
+        raise L.DB200Error(f"rope_bwd: period S {S} exceeds the table's {n_pos} positions")
+    check(L.load().db200_rope_bwd(stream_ptr(), ptr(dqkv), ptr(table), rows, int(S), H, dh, int(r)), "db200_rope_bwd")
+
+
+def rope_decode(qkv, table, pos, H, dh, r):
+    """rope_fwd of one decoding step: every row of qkv [rows, 3*H*dh] at position pos (0 <= pos < n_pos)."""
+    rows, n_pos = _rope_args(qkv, table, H, dh, r, "rope_decode")
+    check(L.load().db200_rope_decode(stream_ptr(), ptr(qkv), ptr(table), rows, n_pos, H, dh, int(r), int(pos)),
+          "db200_rope_decode")
+
+
+def rope_decode_dev(qkv, table, pos_dev, H, dh, r):
+    """rope_decode with the position read on the device from pos_dev (graph replay)."""
+    rows, n_pos = _rope_args(qkv, table, H, dh, r, "rope_decode_dev")
+    _chk(pos_dev, I32, "pos_dev")
+    check(L.load().db200_rope_decode_dev(stream_ptr(), ptr(qkv), ptr(table), rows, n_pos, H, dh, int(r), ptr(pos_dev)),
+          "db200_rope_decode_dev")
+
+
 def rows_repeat(src, dst, rep=1):
     """dst[b*rep + r] = src[b] for a [B, d] view src (rows may be strided, e.g. x.view(B, P, d)[:, P - 1])."""
     L.require_device()

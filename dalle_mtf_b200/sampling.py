@@ -11,7 +11,8 @@ parameters and the same kernels' numerics as training:
                     a local layer of radius r takes j > p - r only, models.py:257-273; an axial layer the text
                     positions and p's image row or column; a conv layer the text positions and p's k x k window)
                     x = x + a Wo + o_b;  x = x + act(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows;
-                    act = ReLU, or GELU without a pre-activation output)
+                    act = ReLU, or GELU without a pre-activation output); with rotary embeddings q and k are
+                    rotated to position p (rope_decode) before k enters the cache
   logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
 
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
@@ -99,6 +100,8 @@ class DalleSampler:
             p = f"l{i}."
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
+            if e.rotary:
+                ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
             ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
                             **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
@@ -121,6 +124,8 @@ class DalleSampler:
             p = f"l{i}."
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
+            if e.rotary:
+                ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
             ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
                                 radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)

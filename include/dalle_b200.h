@@ -630,6 +630,24 @@ int db200_kv_cache_fill(db200_stream_t stream, const void* qkv_bf16, void* k_cac
 int db200_rows_repeat(db200_stream_t stream, const void* src_bf16, long long ld_src, void* dst_bf16, int B, int d,
                       int rep);
 
+/* Rotary position embeddings (extension; GPT-NeoX's rotate_half layout with partial rotary r = rotary_dim).  qkv is
+ * bf16 [rows][3][H][dh], rotated in place: for every q and k head of row t at position p, with h = r / 2 and j < h,
+ *   x_j' = bf16(x_j c - x_{j+h} s),  x_{j+h}' = bf16(x_{j+h} c + x_j s),  c = table[p][0][j], s = table[p][1][j],
+ * every product and sum rounded separately in fp32 (no FMA contraction).  v and the dims r .. dh-1 are unchanged.
+ * table: fp32 [n_pos][2][h], position p's cosines then its sines of p theta_j (theta_j = base^(-2j/r)).
+ *   rope_fwd        : p = t mod S; the table holds at least S positions.
+ *   rope_bwd        : the transpose rotation (s -> -s) of rope_fwd, applied to the dq and dk columns of dqkv.
+ *   rope_decode     : every row at position pos, 0 <= pos < S (the table's, and the cache's, length).
+ *   rope_decode_dev : every row at position *pos_dev (graph replay); a position outside [0, S) leaves qkv unchanged.
+ * r even with 2 <= r <= dh, rows, S, H, dh > 0 and non-NULL pointers, else DB200_E_INVALID; when h % 8 == 0 and
+ * dh % 8 == 0 (16-byte vectors) qkv and the table must be 16-byte aligned (DB200_E_ALIGN). */
+int db200_rope_fwd(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh, int r);
+int db200_rope_bwd(db200_stream_t stream, void* dqkv_bf16, const float* table, int rows, int S, int H, int dh, int r);
+int db200_rope_decode(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh, int r,
+                      int pos);
+int db200_rope_decode_dev(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh,
+                          int r, const int32_t* pos_dev);
+
 /* Segmented bf16 -> f32 gather (one launch): segment i copies table[3i+2] elements from src + table[3i] to
  * dst + table[3i+1]; `table_dev` is an int64 array in device memory.  ZeRO-1 mode: rebuilds the compact fp32 copy of the
  * vector parameters (LayerNorm g/b, biases) from the all-gathered bf16 parameters (mtf casts every variable to the

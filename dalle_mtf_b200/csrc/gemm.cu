@@ -43,10 +43,14 @@ static_assert(128 * G_REGS_PRODUCER + 256 * G_REGS_MMA + 128 * G_REGS_EPI <= 655
 constexpr int G_BAR_FULL = 1, G_BAR_EMPTY = 2, G_BAR_HANDOFF_THREADS = 384;
 
 // operand majors (1 = MN-major), compile-time for wgmma; DROP: dropout in the STORE epilogue; WCE: the weighted CE_GRAD
-// epilogue (instantiated for the vocabulary product only: A K-major, B MN-major); GELU: the GELU MLP's epilogues,
-// G_GELU_FWD (the W1 forward: A K-major, B MN-major) or G_GELU_BWD (its dgrad: both K-major)
+// epilogue (instantiated for the vocabulary product only: A K-major, B MN-major); MLP: the GELU MLP's epilogues,
+// G_GELU_FWD (the W1 forward: A K-major, B MN-major) or G_GELU_BWD (its dgrad: both K-major), or the gated MLP's,
+// G_GLU_*_FWD (the W1 forward, whose B operand is the [K][2N] value | gate weight) or G_GLU_*_BWD (its dgrad)
 constexpr int G_GELU_FWD = 1, G_GELU_BWD = 2;
-template <int TA, int TB, bool DROP, bool WCE = false, int GELU = 0>
+constexpr int G_GLU_RELU_FWD = 3, G_GLU_GELU_FWD = 4, G_GLU_RELU_BWD = 5, G_GLU_GELU_BWD = 6;
+__host__ __device__ constexpr bool glu_fwd(int mlp) { return mlp == G_GLU_RELU_FWD || mlp == G_GLU_GELU_FWD; }
+__host__ __device__ constexpr bool glu_bwd(int mlp) { return mlp == G_GLU_RELU_BWD || mlp == G_GLU_GELU_BWD; }
+template <int TA, int TB, bool DROP, bool WCE = false, int MLP = 0>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr int BN = GBN;
@@ -88,7 +92,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint32_t stage = 0, phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile);
-      const int m0 = t.m_blk * BM, n0 = t.n_blk * BN;
+      // a GLU forward tile covers 64 output columns: its value slab at n0 and its gate slab at N + n0
+      const int m0 = t.m_blk * BM, n0 = t.n_blk * (glu_fwd(MLP) ? 64 : BN);
       for (int kb = t.kb0; kb < t.kb1; ++kb) {
         mbar_wait_mma(empty_bar + 8 * stage, phase ^ 1);
         const uint32_t fb = full_bar + 8 * stage;
@@ -105,7 +110,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           } else {
             tma_load_2d(a_dst, &tmA, fb, k0, m0);
           }
-          if (p.b_3d) {
+          if constexpr (glu_fwd(MLP)) {  // the 2D map of B spans all 2N columns
+            tma_load_2d(b_dst, &tmB, fb, n0, k0);
+            tma_load_2d(b_dst + SLAB_BYTES, &tmB, fb, p.N + n0, k0);
+          } else if (p.b_3d) {
             tma_load_3d(b_dst, &tmB, fb, 0, k0, n0 >> 6);
           } else if (p.b_mn) {
 #pragma unroll
@@ -191,12 +199,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           epi_ce_grad_weighted<CH>(p, t_addr, row, row_ok, cbase, stg, row0, lane);
           continue;
         }
-        if constexpr (GELU == G_GELU_FWD) {
+        if constexpr (MLP == G_GELU_FWD) {
           epi_gelu_store<CH>(p, t_addr, cbase, stg, row0, lane);
           continue;
         }
-        if constexpr (GELU == G_GELU_BWD) {
+        if constexpr (MLP == G_GELU_BWD) {
           epi_gelu_bwd<CH>(p, t_addr, cbase, stg, row0, lane);
+          continue;
+        }
+        if constexpr (glu_fwd(MLP)) {  // the whole tile at once: value and gate halves of the same 64 columns
+          if (half == 0) epi_glu_store<MLP == G_GLU_GELU_FWD>(p, t_addr, t.n_blk * 64, stg, row0, lane);
+          continue;
+        }
+        if constexpr (glu_bwd(MLP)) {
+          epi_glu_bwd<MLP == G_GLU_GELU_BWD>(p, t_addr, cbase, stg, row0, lane);
           continue;
         }
         switch (p.mode) {
@@ -549,15 +565,15 @@ static int launch_gemm_wide(cudaStream_t stream, const CUtensorMap& tmA, const C
   return check_launch("gemm_wide_kernel");
 }
 
-template <int TA, int TB, bool DROP, bool WCE = false, int GELU = 0>
+template <int TA, int TB, bool DROP, bool WCE = false, int MLP = 0>
 static int launch_gemm(cudaStream_t stream, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p) {
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP, WCE, GELU>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(gemm_tc_kernel<TA, TB, DROP, WCE, MLP>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                           (int)G_SMEM_BYTES);  // once, thread-safe (magic static)
   DB200_CUDA(attr_rc);
   const int total = p.m_tiles * p.n_tiles * p.splits;
   const int grid = total < sm_count() ? total : sm_count();
-  gemm_tc_kernel<TA, TB, DROP, WCE, GELU><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_tc_kernel<TA, TB, DROP, WCE, MLP><<<grid, GEMM_THREADS, G_SMEM_BYTES, stream>>>(tmA, tmB, p);
   return check_launch("gemm_tc_kernel");
 }
 
@@ -602,7 +618,8 @@ extern "C" int db200_gemm_bf16(db200_stream_t stream_, const void* A, int a_mn_m
 
 // every product: cew != NULL selects the weighted CE_GRAD epilogue (validated by db200_gemm_bf16_ce_weighted), gelu the
 // GELU MLP's store (G_GELU_FWD, pre-activation output z / ldz) or dgrad (G_GELU_BWD) epilogue (validated by
-// db200_gemm_bf16_gelu / db200_gemm_bf16_gelu_bwd)
+// db200_gemm_bf16_gelu / db200_gemm_bf16_gelu_bwd), or the gated MLP's (G_GLU_*, validated by db200_gemm_bf16_glu /
+// db200_gemm_bf16_glu_bwd; N is the h width, B of the forward and D / aux / colsum of the backward are 2N wide)
 static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
                     int64_t ldb, void* D, int64_t ldd, int M, int N, int K, const db200_gemm_epilogue* epi,
                     const db200_dropout* dropout, const db200_ce_weights* cew, int gelu = 0, void* z = nullptr,
@@ -648,7 +665,8 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
                 "gemm: split_k > 1 is only valid with DB200_EPI_ATOMIC");
   const int splits = gemm_splits(M, N, K, epi);
   const int kb_total = (K + BK - 1) / BK;
-  DB200_REQUIRE(workspace_ok(epi->workspace, epi->workspace_bytes, db200_gemm_workspace_bytes(M, N, K, epi)),
+  const int n_sums = glu_bwd(gelu) ? 2 * N : N;  // columns of the fused column sums
+  DB200_REQUIRE(workspace_ok(epi->workspace, epi->workspace_bytes, db200_gemm_workspace_bytes(M, n_sums, K, epi)),
                 DB200_E_INVALID, "gemm: needs an aligned epi->workspace of db200_gemm_workspace_bytes() bytes");
 
   GemmParams p;
@@ -681,13 +699,13 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   p.zout = reinterpret_cast<bf16*>(z);
   p.ldz = ldz;
 
-  p.n_tiles = (N + GBN - 1) / GBN;
+  p.n_tiles = glu_fwd(gelu) ? N / 64 : (N + GBN - 1) / GBN;
   p.n_parts = 2 * p.n_tiles;
 
   // MN-major operands whose MN extent is a multiple of 64: one rank-3 map {64, K, MN/64} (stride of the slab index =
   // 128 bytes) fetches every 64-wide slab of a stage with a single TMA instruction instead of one per slab.
   p.a_3d = (p.a_mn && M % 64 == 0) ? 1 : 0;
-  p.b_3d = (p.b_mn && N % 64 == 0) ? 1 : 0;
+  p.b_3d = (p.b_mn && N % 64 == 0 && !glu_fwd(gelu)) ? 1 : 0;
   CUtensorMap tmA, tmB;
   int rc;
   if (p.a_3d) {
@@ -703,7 +721,9 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
     uint64_t str[2] = {(uint64_t)ldb * 2, 128};
     uint32_t box[3] = {64, BK, GBN / 64};
     rc = make_tmap_bf16(&tmB, B, 3, dims, str, box);
-  } else if (p.b_mn) rc = make_tmap_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, 64, BK);
+  } else if (p.b_mn) {  // a GLU forward's B holds 2N columns: value slabs, then gate slabs
+    rc = make_tmap_2d(&tmB, B, (uint64_t)(glu_fwd(gelu) ? 2 * N : N), (uint64_t)K, (uint64_t)ldb, 64, BK);
+  }
   else               rc = make_tmap_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BK, GBN);
   if (rc != DB200_OK) return rc;
 
@@ -735,6 +755,14 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   else if (gelu == G_GELU_BWD)   // its dgrad dH = dbranch W2^T: both k-major
     rc = (!p.a_mn && !p.b_mn) ? launch_gemm<0, 0, false, false, G_GELU_BWD>(stream, tmA, tmB, p)
                               : set_error(DB200_E_UNSUPPORTED, "gemm_gelu_bwd: needs k-major A and B");
+  else if (glu_fwd(gelu))   // the gated MLP's W1 forward: A k-major, B mn-major
+    rc = (p.a_mn || !p.b_mn) ? set_error(DB200_E_UNSUPPORTED, "gemm_glu: needs a k-major A and an mn-major B")
+         : gelu == G_GLU_GELU_FWD ? launch_gemm<0, 1, false, false, G_GLU_GELU_FWD>(stream, tmA, tmB, p)
+                                  : launch_gemm<0, 1, false, false, G_GLU_RELU_FWD>(stream, tmA, tmB, p);
+  else if (glu_bwd(gelu))   // its dgrad dh = dbranch W2^T: both k-major
+    rc = (p.a_mn || p.b_mn) ? set_error(DB200_E_UNSUPPORTED, "gemm_glu_bwd: needs k-major A and B")
+         : gelu == G_GLU_GELU_BWD ? launch_gemm<0, 0, false, false, G_GLU_GELU_BWD>(stream, tmA, tmB, p)
+                                  : launch_gemm<0, 0, false, false, G_GLU_RELU_BWD>(stream, tmA, tmB, p);
   else if (cew)     // the vocabulary product: A k-major, B mn-major
     rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, true>(stream, tmA, tmB, p)
                              : set_error(DB200_E_UNSUPPORTED, "gemm: weighted CE_GRAD needs a k-major A and an mn-major B");
@@ -745,7 +773,7 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
   else             rc = p.b_mn ? launch_gemm<0, 1, false>(stream, tmA, tmB, p) : launch_gemm<0, 0, false>(stream, tmA, tmB, p);
   if (rc != DB200_OK) return rc;
   if (p.splits > 1) return reduce_splits_add(stream, static_cast<const float*>(p.D), p.splits, M, N, d_out, ldd);
-  if (colsum_out) return reduce_rows_add(stream, p.colsum, row_blocks, N, colsum_out);
+  if (colsum_out) return reduce_rows_add(stream, p.colsum, row_blocks, n_sums, colsum_out);
   return DB200_OK;
 }
 
@@ -785,4 +813,49 @@ extern "C" int db200_gemm_bf16_gelu_bwd(db200_stream_t stream, const void* A, in
   DB200_REQUIRE(epi != nullptr && epi->mode == DB200_EPI_RELU_BWD, DB200_E_INVALID,
                 "gemm_gelu_bwd: needs an epilogue descriptor with mode DB200_EPI_RELU_BWD (aux = z)");
   return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, nullptr, G_GELU_BWD);
+}
+
+// the gated MLP: act 0 = ReGLU, 1 = GEGLU (DB200_ACT_*); N = the h width, a multiple of 64
+static int glu_check(const void* A, const void* B, const void* D, int N, int act, const char* fn) {
+  DB200_REQUIRE(act == DB200_ACT_RELU || act == DB200_ACT_GELU, DB200_E_INVALID,
+                "%s: act must be DB200_ACT_RELU or DB200_ACT_GELU (got %d)", fn, act);
+  DB200_REQUIRE(A && B && D, DB200_E_INVALID, "%s: NULL operand or output", fn);
+  DB200_REQUIRE(N > 0 && N % 64 == 0, DB200_E_INVALID, "%s: N must be a positive multiple of 64 (got %d)", fn, N);
+  return DB200_OK;
+}
+
+extern "C" int db200_gemm_bf16_glu(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                                   int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                                   const db200_gemm_epilogue* epi, int act, void* z, int64_t ldz) {
+  DB200_REQUIRE(epi != nullptr && epi->mode == DB200_EPI_STORE, DB200_E_INVALID,
+                "gemm_glu: needs an epilogue descriptor with mode DB200_EPI_STORE");
+  DB200_REQUIRE(!epi->out_f32 && !epi->relu && !epi->residual, DB200_E_INVALID,
+                "gemm_glu: bf16 output only, without relu or a residual");
+  const int rc = glu_check(A, B, D, N, act, "gemm_glu");
+  if (rc != DB200_OK) return rc;
+  DB200_REQUIRE(!a_mn_major && b_mn_major, DB200_E_UNSUPPORTED, "gemm_glu: needs a k-major A and an mn-major B");
+  DB200_REQUIRE(ldb >= 2 * (int64_t)N, DB200_E_INVALID,
+                "gemm_glu: B holds the value and gate columns: ldb must be >= 2N (got ldb=%lld, N=%d)", (long long)ldb, N);
+  if (z) DB200_REQUIRE(aligned16(z) && ldz % 8 == 0 && ldz >= 2 * (int64_t)N, DB200_E_ALIGN,
+                       "gemm_glu: z must be 16-byte aligned with ldz %% 8 == 0 and ldz >= 2N (got ldz=%lld, N=%d)",
+                       (long long)ldz, N);
+  return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, nullptr,
+                  act == DB200_ACT_GELU ? G_GLU_GELU_FWD : G_GLU_RELU_FWD, z, z ? ldz : 0);
+}
+
+extern "C" int db200_gemm_bf16_glu_bwd(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda,
+                                       const void* B, int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N,
+                                       int K, const db200_gemm_epilogue* epi, int act) {
+  DB200_REQUIRE(epi != nullptr && epi->mode == DB200_EPI_RELU_BWD, DB200_E_INVALID,
+                "gemm_glu_bwd: needs an epilogue descriptor with mode DB200_EPI_RELU_BWD (aux = z)");
+  const int rc = glu_check(A, B, D, N, act, "gemm_glu_bwd");
+  if (rc != DB200_OK) return rc;
+  DB200_REQUIRE(!a_mn_major && !b_mn_major, DB200_E_UNSUPPORTED, "gemm_glu_bwd: needs k-major A and B");
+  DB200_REQUIRE(ldd >= 2 * (int64_t)N, DB200_E_INVALID,
+                "gemm_glu_bwd: D is [M][2N] (dzv | dzg): ldd must be >= 2N (got ldd=%lld, N=%d)", (long long)ldd, N);
+  DB200_REQUIRE(epi->aux && aligned16(epi->aux) && epi->ldaux % 8 == 0 && epi->ldaux >= 2 * (int64_t)N, DB200_E_ALIGN,
+                "gemm_glu_bwd: aux = z [M][2N] must be 16-byte aligned with ldaux %% 8 == 0 and ldaux >= 2N (got %lld)",
+                (long long)epi->ldaux);
+  return gemm_run(stream, A, a_mn_major, lda, B, b_mn_major, ldb, D, ldd, M, N, K, epi, nullptr, nullptr,
+                  act == DB200_ACT_GELU ? G_GLU_GELU_BWD : G_GLU_RELU_BWD);
 }

@@ -463,6 +463,123 @@ __device__ __forceinline__ void epi_gelu_bwd(const GemmParams& p, uint32_t t_add
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Gated MLP (GLU).  z = [zv | zg] is [M][2N] (value half first: DALLE-pytorch's chunk order), h = zv * act(zg) is
+// [M][N].  The gate's nonlinearity a = bf16(act(zg)): GEGLU's zg s(zg) exactly as the GELU store evaluates it;
+// ReGLU's zg > 0 ? zg : 0, which maps NaN (and -0) to +0 as the ReLU store's fmaxf does NaN.  h = bf16(zv a): the
+// product of two bf16 values is exact in fp32 unless it leaves the normal range.
+// ------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+template <bool GELU>
+__device__ __forceinline__ float glu_act(float zg) {
+  if constexpr (GELU) return round_bf16(zg * gelu_s(zg));
+  else return zg > 0.f ? zg : 0.f;
+}
+
+// GLU forward store (the W1 product, N = the h width).  Tile n_blk holds value columns [64 n_blk, 64 n_blk + 64) in
+// accumulator columns 0-63 and the matching gate columns N + 64 n_blk .. in 64-127 (the producer loads the two B
+// slabs from there), so each thread has both halves of its row.  zv and zg = bf16(alpha acc + bias) go through the
+// staging block (and to zout at their two offsets when it is given); zv stays in registers as the 32 packed words
+// it was staged as while the block takes zg, then a and h = bf16(zv a) replace zg in place and h goes to D.
+template <bool GELU>
+__device__ __forceinline__ void epi_glu_store(const GemmParams& p, uint32_t t_addr, int colp, uint32_t stg, int row0,
+                                              int lane) {
+  uint32_t zv[32];  // columns 2 k, 2 k + 1 of this lane's value row
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {  // 0: value, 1: gate
+    const int zcol = half * p.N + colp;   // bias and z column of the half
+    uint32_t rr2[2][32];
+    acc_ld_x32(t_addr + half * 64, rr2[0]);
+    acc_ld_x32(t_addr + half * 64 + 32, rr2[1]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float o[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) o[j] = __uint_as_float(rr2[h][j]) * p.alpha;
+      if (p.bias) {  // N % 64 == 0: whole chunks
+#pragma unroll
+        for (int g = 0; g < 4; ++g) {
+          float b[8];
+          load8(p.bias + zcol + h * 32 + g * 8, b);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[g * 8 + j] += b[j];
+        }
+      }
+      stage_put_bf16(stg, lane, h, o);
+    }
+    if (p.zout) stage_flush<2>(stg, p.zout, p.ldz, row0, zcol, p.M, 2 * p.N, lane);
+    if (half == 0) {
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {  // this lane's own row: no exchange between lanes
+        const uint4 q = ld_shared_v4u(stg_addr(stg, lane, g));
+        zv[4 * g] = q.x; zv[4 * g + 1] = q.y; zv[4 * g + 2] = q.z; zv[4 * g + 3] = q.w;
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float o[32];
+    stage_get_bf16(stg, lane, h, o);  // zg
+#pragma unroll
+    for (int j = 0; j < 32; j += 2) {
+      const float2 v = unpack_bf16x2(zv[h * 16 + j / 2]);
+      o[j] = v.x * glu_act<GELU>(o[j]);
+      o[j + 1] = v.y * glu_act<GELU>(o[j + 1]);
+    }
+    stage_put_bf16(stg, lane, h, o);
+  }
+  stage_flush<2>(stg, p.D, p.ldd, row0, colp, p.M, p.N, lane);
+}
+
+// GLU backward (the dgrad dh = dbranch W2^T, N = the h width; D and aux are [M][2N]).  Half tile [colp, colp + 64) of
+// dh = alpha acc (fp32, not rounded) reads zg, then zv, from the stored z and writes
+//   dzv = bf16(dh a)                 a = bf16(act(zg)) as in the forward
+//   dzg = bf16((dh act'(zg)) zv)     multiplied in this order; ReGLU's dh act'(zg) is zg > 0 ? dh : 0 (RELU_BWD's
+//                                    mask convention), GEGLU's dh gelu'(zg)
+// each through the staging block with its fused column sums (workspace rows of 2N columns).  Rows past M read z = 0
+// and acc = 0, so they stage zeros.
+template <bool GELU>
+__device__ __forceinline__ void epi_glu_bwd(const GemmParams& p, uint32_t t_addr, int colp, uint32_t stg, int row0,
+                                            int lane) {
+  if (colp >= p.N) return;  // warp-uniform
+  const int N2 = 2 * p.N;
+  float dh[2][32];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint32_t r[32];
+    acc_ld_x32(t_addr + h * 32, r);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) dh[h][j] = __uint_as_float(r[j]) * p.alpha;
+  }
+  stage_fetch_bf16(stg, p.aux, p.ldaux, row0, p.N + colp, p.M, N2, lane);  // zg
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float o[32];
+    stage_get_bf16(stg, lane, h, o);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const float zg = o[j];
+      o[j] = dh[h][j] * glu_act<GELU>(zg);
+      if constexpr (GELU) dh[h][j] *= gelu_grad(zg);
+      else dh[h][j] = zg > 0.f ? dh[h][j] : 0.f;
+    }
+    stage_put_bf16(stg, lane, h, o);  // in place: this lane overwrites the slots it just read
+  }
+  if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * N2, colp, N2, lane);
+  stage_flush<2>(stg, p.D, p.ldd, row0, colp, p.M, N2, lane);
+  stage_fetch_bf16(stg, p.aux, p.ldaux, row0, colp, p.M, N2, lane);  // zv
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float o[32];
+    stage_get_bf16(stg, lane, h, o);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) o[j] = dh[h][j] * o[j];
+    stage_put_bf16(stg, lane, h, o);
+  }
+  if (p.colsum) stage_colsum_bf16(stg, p.colsum + (long long)(row0 >> 5) * N2, p.N + colp, N2, lane);
+  stage_flush<2>(stg, p.D, p.ldd, row0, p.N + colp, p.M, N2, lane);
+}
+
 // per (row, half-tile): running max and sum exp of (acc + bias) over the valid vocabulary columns; label logit
 template <int CH>
 __device__ __forceinline__ void epi_ce_stats(const GemmParams& p, uint32_t t_addr, int row, bool row_ok, int cbase,

@@ -61,11 +61,13 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
-def param_layout(d, n_layers, V, S, text_len=None, grid_w=None):
+def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
     length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
     column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
-    the grid_w rows and columns of the image-token grid."""
+    the grid_w rows and columns of the image-token grid.  gated_mlp: w1 is [d, 8d] and b1 [8d], the value columns
+    first and the gate columns second."""
+    w1_cols = 8 * d if gated_mlp else 4 * d
     Vpad = _round_up(V, 64)
     lay = ParamLayout()
     lay.add("wte", (V, d))
@@ -80,7 +82,7 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None):
         lay.add(p + "wqkv", (d, 3 * d))
         lay.add(p + "wo", (d, d)); lay.add(p + "o_b", (d,))
         lay.add(p + "ln2_g", (d,)); lay.add(p + "ln2_b", (d,))
-        lay.add(p + "w1", (d, 4 * d)); lay.add(p + "b1", (4 * d,))
+        lay.add(p + "w1", (d, w1_cols)); lay.add(p + "b1", (w1_cols,))
         lay.add(p + "w2", (4 * d, d)); lay.add(p + "b2", (d,))
     lay.add("lnf_g", (d,)); lay.add("lnf_b", (d,))
     lay.add("wout", (d, Vpad)); lay.add("bout", (Vpad,))
@@ -263,6 +265,14 @@ def validate_activation(activation):
     return activation
 
 
+def validate_gated_mlp(gated_mlp):
+    """The gated MLP switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
+    handled by model_fns.gated_mlp)."""
+    if not isinstance(gated_mlp, bool):
+        raise ValueError(f"gated_mlp must be a bool, got {gated_mlp!r}")
+    return gated_mlp
+
+
 def validate_rotary(rotary_dim, rotary_base, head_dim):
     """(r, base) of rotary position embeddings, or None without them.  rotary_dim None: off (rotary_base must then be
     None too); otherwise an even integer 2 <= r <= head_dim.  rotary_base None is 10000, else a finite real > 1."""
@@ -293,12 +303,13 @@ class DalleEngine:
 
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lnf_g", "lnf_b", "bout")
     conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
+    gated_mlp = False   # the gated MLP (validate_gated_mlp), set by the constructor
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
-                 activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None):
+                 activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -350,13 +361,21 @@ class DalleEngine:
         dims of every q and k head of every layer is rotated by p theta_j, p the token's sequence index and theta_j =
         base^(-2j/r), in fp32 and rounded to bf16 (ops.rope_fwd); backward applies the transpose to dq and dk, and the
         decoder rotates each step's q and k before they reach the cache.  v, the attention scale and the learned
-        position embeddings are unchanged, and no parameter is added."""
+        position embeddings are unchanged, and no parameter is added.
+
+        gated_mlp (validate_gated_mlp): the MLP becomes DALLE-pytorch's gated FeedForward, y = LN2(x) W1 + b1 with W1
+        [d, 8d], zv, zg = bf16(y[:, :4d]), bf16(y[:, 4d:]), h = bf16(zv bf16(act(zg))), out = h W2 + b2, with act the
+        `activation` (ReGLU or GEGLU).  The gate is fused into the W1 product's epilogue, which keeps z = [zv | zg]
+        ([T, 8d] bf16 per saved layer) for backward, and into its dgrad's."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.rotary = validate_rotary(rotary_dim, rotary_base, self.dh)
         self.activation = validate_activation(activation)
-        self.gelu = self.activation == "gelu"
-        self.mlp_act = {"gelu": True} if self.gelu else {"relu": True}   # linear_fwd keywords of an inference W1
+        self.gated_mlp = validate_gated_mlp(gated_mlp)
+        self.glu = self.activation if self.gated_mlp else None   # the gate's nonlinearity, or None: no gate
+        self.gelu = self.activation == "gelu" and not self.gated_mlp    # the ungated GELU MLP
+        # linear_fwd keywords of an inference W1
+        self.mlp_act = {"glu": self.glu} if self.gated_mlp else {"gelu": True} if self.gelu else {"relu": True}
         self.row_col = validate_position_embedding(image_position_embedding) == "row_col"
         self.grid_w = image_grid_side(image_seq_len) if self.row_col else None
         self.per_position_padding = validate_per_position_padding(per_position_padding)
@@ -404,8 +423,8 @@ class DalleEngine:
                                      # (text block, image block) pair)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
-        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w) if self.row_col else \
-            param_layout(d, Lyr, V, S)
+        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, gated_mlp=self.gated_mlp) \
+            if self.row_col else param_layout(d, Lyr, V, S, gated_mlp=self.gated_mlp)
         self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
@@ -496,8 +515,9 @@ class DalleEngine:
         """Trainable parameter count as the reference would print it (src/utils/utils.py:55-70)."""
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else S
-        return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d) + \
-            2 * d + d * V + V
+        gate = (4 * d * d + 4 * d) if self.gated_mlp else 0   # the gate half of W1 and b1
+        return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d +
+                                          gate) + 2 * d + d * V + V
 
     EMBED_REF_NAMES = {"wte": "embedding/wte", "wpe": "positional_embedding/wpe",
                        "image_row": "positional_embedding/image_row", "image_col": "positional_embedding/image_col"}
@@ -662,7 +682,7 @@ class DalleEngine:
             wkv = torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5)
             self._scatter_full(p + "wqkv", torch.cat([wq, wkv], dim=1))
             self._scatter_full(p + "wo", rn((d, d), (H * dh) ** -0.5))
-            self._scatter_full(p + "w1", rn((d, 4 * d), 0.02))
+            self._scatter_full(p + "w1", rn(self.layout.entries[p + "w1"][1], 0.02))
             self._scatter_full(p + "w2", rn((4 * d, d), 0.02 / math.sqrt(Lyr)))
         self._scatter_full("lnf_g", ones(d))
         self._scatter_full("wout", rn((d, self.V), 0.02), cols=self.V)
@@ -700,6 +720,7 @@ class DalleEngine:
                 "qkv": e(T, 3 * d), "attn": e(T, d), "lse": e(B, self.H, S, dtype=F32),
                 "xmid": e(T, d), "ln2": e(T, d), "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32),
                 "h1": e(T, 4 * d), **({"z1": e(T, 4 * d)} if self.gelu else {}),
+                **({"z1": e(T, 8 * d)} if self.gated_mlp else {}),
             } for _ in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
             "labels": e(B, S, dtype=I32), "loss_rows": e(T, dtype=F32),
@@ -709,6 +730,8 @@ class DalleEngine:
         }
         if self.dropout[2] > 0:   # gradient of a branch output before its residual dropout
             b["dxm"] = e(T, d)
+        if self.gated_mlp:        # [dzv | dzg], the gradient of z1
+            b["dz1"] = e(T, 8 * d)
         if not self.logits_mask:
             b.update({"part_max": e(nt, T, dtype=F32), "part_sum": e(nt, T, dtype=F32), "label_logit": e(T, dtype=F32),
                       "lse_v": e(T, dtype=F32), "dlogits": e(T, self.Vpad)})
@@ -769,7 +792,10 @@ class DalleEngine:
                        dropout=self._site("attn_out", i))                               # :303-314,330
         ops.layernorm_fwd(sv["xmid"], self.P(p + "ln2_g"), self.P(p + "ln2_b"), sv["ln2"], sv["mean2"], sv["rstd2"],
                           self.ln_eps)
-        if self.gelu:   # h1 = gelu(z1), z1 = LN2 W1 + b1 kept for backward (the prefill's sv has none: not written)
+        if self.gated_mlp:   # h1 = zv * act(zg), z1 = [zv | zg] = LN2 W1 + b1 kept for backward (prefill: not written)
+            ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), glu=self.glu,
+                           z_out=sv.get("z1"))
+        elif self.gelu:   # h1 = gelu(z1), z1 = LN2 W1 + b1 kept for backward (the prefill's sv has none: not written)
             ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), gelu=True,
                            z_out=sv.get("z1"))
         else:
@@ -994,14 +1020,17 @@ class DalleEngine:
         same for the layer below."""
         p = f"l{i}."
         # ---- MLP
-        if self.gelu:   # dZ = (dx W2^T) * gelu'(z1); db1
+        dz = bufs["dz1"] if self.gated_mlp else bufs["dh1"]   # the gradient of W1's output
+        if self.gated_mlp:   # dh = dx W2^T -> dz1 = [dh a | dh act'(zg) zv]; db1 = colsum(dz1)
+            ops.linear_dgrad(dbranch, self.W(p + "w2"), dz, glu_grad_of=sv["z1"], glu=self.glu, colsum=self.G(p + "b1"))
+        elif self.gelu:   # dZ = (dx W2^T) * gelu'(z1); db1
             ops.linear_dgrad(dbranch, self.W(p + "w2"), bufs["dh1"], gelu_grad_of=sv["z1"], colsum=self.G(p + "b1"))
         else:
             ops.linear_dgrad(dbranch, self.W(p + "w2"), bufs["dh1"], relu_mask_of=sv["h1"],
                              colsum=self.G(p + "b1"))                                   # dH = (dx W2^T)*[h1>0]; db1
         ops.linear_wgrad(sv["h1"], dbranch, self.G(p + "w2"))
-        ops.linear_dgrad(bufs["dh1"], self.W(p + "w1"), bufs["dtmp"])                         # dLN2 out
-        ops.linear_wgrad(sv["ln2"], bufs["dh1"], self.G(p + "w1"))
+        ops.linear_dgrad(dz, self.W(p + "w1"), bufs["dtmp"])                                  # dLN2 out
+        ops.linear_wgrad(sv["ln2"], dz, self.G(p + "w1"))
         dx_mid = bufs["dx_b"] if dx_out is bufs["dx_a"] else bufs["dx_a"]
         da = self._ln_bwd(bufs["dtmp"], sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
                           self.G(p + "ln2_g"), self.G(p + "ln2_b"), self.G(p + "o_b"),

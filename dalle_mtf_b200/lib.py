@@ -21,6 +21,7 @@ c_sz = ctypes.c_size_t
 c_u64 = ctypes.c_uint64
 
 EPI_STORE, EPI_ATOMIC, EPI_RELU_BWD, EPI_CE_STATS, EPI_CE_GRAD = 0, 1, 2, 3, 4
+ACT_RELU, ACT_GELU = 0, 1            # the gated MLP's gate nonlinearity (db200_gemm_bf16_glu*)
 
 
 class GemmEpilogue(ctypes.Structure):
@@ -132,6 +133,10 @@ _SIGNATURES = {
                              ctypes.POINTER(GemmEpilogue), c_vp, c_i64],
     "db200_gemm_bf16_gelu_bwd": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
                                  ctypes.POINTER(GemmEpilogue)],
+    "db200_gemm_bf16_glu": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
+                            ctypes.POINTER(GemmEpilogue), c_int, c_vp, c_i64],
+    "db200_gemm_bf16_glu_bwd": [c_vp, c_vp, c_int, c_i64, c_vp, c_int, c_i64, c_vp, c_i64, c_int, c_int, c_int,
+                                ctypes.POINTER(GemmEpilogue), c_int],
     "db200_gemm_ce_tiles": [c_int],
     "db200_embed_fwd_at": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_attn_decode": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_f32],

@@ -153,6 +153,18 @@ def activation_function(params):
         raise ValueError(f"activation_function = {v!r}: expected null, \"relu\" or \"gelu\"") from None
 
 
+def gated_mlp(params):
+    """gated_mlp of a DALL-E config: absent, null or false keeps the MLP act(LN2(x) W1 + b1) W2 + b2; true makes it
+    DALLE-pytorch's gated FeedForward with the activation_function as the gate's nonlinearity (ReGLU or GEGLU) and W1
+    [d, 8d] (DalleEngine).  Only a JSON bool is accepted: 1, "true" or a list is rejected."""
+    v = params.get("gated_mlp")
+    if v is None:
+        return False
+    if not isinstance(v, bool):
+        raise ValueError(f"gated_mlp = {v!r}: expected null, true or false")
+    return v
+
+
 def conv_kernel(params):
     """conv_attention_kernel of a DALL-E config: the k of "conv" layers' k x k window (DalleEngine), an integer >= 1.
     A missing or null key is 5, DALLE-pytorch's default."""
@@ -244,6 +256,7 @@ def dalle_model_fn(features, labels, mode, params):
     weights, z_loss = loss_weights(params)
     pos_scheme, per_pos, pp_pad = input_embedding(params)
     activation = activation_function(params)
+    gated = gated_mlp(params)
     mask = logits_mask(params)
     rotary_dim, rotary_base = rotary_embedding(params)
     L.require_device()
@@ -279,7 +292,8 @@ def dalle_model_fn(features, labels, mode, params):
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
-                        activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base)
+                        activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
+                        gated_mlp=gated)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

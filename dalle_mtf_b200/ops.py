@@ -47,7 +47,7 @@ def _nbytes(ws):
 def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=None, mode=L.EPI_STORE,
          alpha=1.0, bias=None, relu=False, residual=None, aux=None, split_k=1, labels=None, part_max=None,
          part_sum=None, label_logit=None, lse=None, n_valid=0, colsum=None, dropout=None, ce_weights=None, gelu=None,
-         z=None):
+         z=None, glu=None, glu_act=None):
     """D[M,N] = A[M,K] @ B[K,N] on wgmma.  a_mn / b_mn: operand is stored with M (resp. N) contiguous.
 
     a: [M,K] (k-major) or [K,M] (mn-major);  b: [N,K] (k-major) or [K,N] (mn-major).
@@ -56,6 +56,9 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     per-row coefficients from the descriptor instead of alpha.
     gelu "fwd" (STORE, a k-major / b mn-major): D = gelu(bf16(alpha * acc + bias)), and z (bf16, or None) receives the
     rounded pre-activation; gelu "bwd" (RELU_BWD, both k-major): D = alpha * acc * gelu'(aux), aux = the stored z.
+    glu "fwd" / "bwd" with glu_act "relu" or "gelu": the gated MLP's W1 store (STORE, a k-major / b mn-major, b = the
+    [K, 2N] value | gate weight, N the width of D = h; z [M, 2N] or None) and its dgrad (RELU_BWD, both k-major, N the
+    width of dh, D [M, 2N], aux = the stored z, colsum 2N entries); include/dalle_b200.h states their arithmetic.
     """
     L.require_device()
     _chk(a, BF16, "gemm A")
@@ -82,8 +85,11 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     e.n_valid = n_valid
     _chk(colsum, F32, "gemm colsum")
     _chk(z, BF16, "gemm z")
-    if z is not None and gelu != "fwd":
-        raise L.DB200Error("gemm: a pre-activation output needs the GELU forward epilogue")
+    if z is not None and gelu != "fwd" and glu != "fwd":
+        raise L.DB200Error("gemm: a pre-activation output needs the GELU or GLU forward epilogue")
+    if glu is not None and (gelu is not None or glu not in ("fwd", "bwd") or glu_act not in ("relu", "gelu")):
+        raise ValueError(f"gemm: glu must be 'fwd' or 'bwd' with glu_act 'relu' or 'gelu' and no gelu, got "
+                         f"{glu!r}, {glu_act!r}, gelu={gelu!r}")
     e.colsum = ptr(colsum)
     if out is not None:
         if mode == L.EPI_ATOMIC:
@@ -91,13 +97,24 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
         ldd = ldd if ldd is not None else out.stride(0)
     else:
         ldd = 0
-    ws = L.workspace(L.load().db200_gemm_workspace_bytes(M, N, K, ctypes.byref(e)))
+    # the GLU backward's fused column sums span its 2N output columns
+    ws = L.workspace(L.load().db200_gemm_workspace_bytes(M, 2 * N if glu == "bwd" else N, K, ctypes.byref(e)))
     e.workspace, e.workspace_bytes = ptr(ws), (ws.numel() if ws is not None else 0)
     prof = GEMM_PROFILE
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-    if gelu == "fwd":
+    if glu is not None:
+        act = L.ACT_GELU if glu_act == "gelu" else L.ACT_RELU
+        if glu == "fwd":
+            check(L.load().db200_gemm_bf16_glu(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out),
+                                               ldd, M, N, K, ctypes.byref(e), act, ptr(z),
+                                               z.stride(0) if z is not None else 0), "db200_gemm_bf16_glu")
+        else:
+            check(L.load().db200_gemm_bf16_glu_bwd(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb,
+                                                   ptr(out), ldd, M, N, K, ctypes.byref(e), act),
+                  "db200_gemm_bf16_glu_bwd")
+    elif gelu == "fwd":
         check(L.load().db200_gemm_bf16_gelu(stream_ptr(), ptr(a), int(a_mn), lda, ptr(b), int(b_mn), ldb, ptr(out),
                                             ldd, M, N, K, ctypes.byref(e), ptr(z), z.stride(0) if z is not None else 0),
               "db200_gemm_bf16_gelu")
@@ -122,29 +139,45 @@ def gemm(a, b, out, M, N, K, *, a_mn=False, b_mn=False, lda=None, ldb=None, ldd=
     return out
 
 
-def linear_fwd(x, w, out, bias=None, relu=False, residual=None, dropout=None, gelu=False, z_out=None):
+def linear_fwd(x, w, out, bias=None, relu=False, residual=None, dropout=None, gelu=False, z_out=None, glu=None):
     """out[T,N] = dropout(act(x[T,K] @ w[K,N] + bias)) + residual      (forward: A k-major, B mn-major).
 
     gelu: out = gelu(z) with z = bf16(x @ w + bias) (mtf's tanh GELU, no residual or dropout); z_out [T,N] bf16
-    receives z for the backward, or is None (inference)."""
+    receives z for the backward, or is None (inference).
+    glu "relu" / "gelu" (the gated MLP): w is [K, 2N'] and z = bf16(x @ w + bias) = [zv | zg]; out [T, N'] =
+    bf16(zv * bf16(act(zg))); z_out [T, 2N'] receives z, or is None."""
     T, K = x.shape
     N = w.shape[1]
+    if glu is not None:
+        if relu or gelu or residual is not None or dropout is not None:
+            raise L.DB200Error("linear_fwd: the GLU epilogue takes no relu, gelu, residual or dropout")
+        if N % 2:
+            raise L.DB200Error(f"linear_fwd: a GLU weight holds value and gate columns: even width, got {N}")
+        return gemm(x, w, out, T, N // 2, K, a_mn=False, b_mn=True, bias=bias, glu="fwd", glu_act=glu, z=z_out)
     if gelu:
         if relu or residual is not None or dropout is not None:
             raise L.DB200Error("linear_fwd: the GELU epilogue takes no relu, residual or dropout")
         return gemm(x, w, out, T, N, K, a_mn=False, b_mn=True, bias=bias, gelu="fwd", z=z_out)
     if z_out is not None:
-        raise L.DB200Error("linear_fwd: z_out needs gelu=True")
+        raise L.DB200Error("linear_fwd: z_out needs gelu=True or glu")
     return gemm(x, w, out, T, N, K, a_mn=False, b_mn=True, bias=bias, relu=relu, residual=residual, dropout=dropout)
 
 
-def linear_dgrad(dy, w, out, relu_mask_of=None, colsum=None, gelu_grad_of=None):
+def linear_dgrad(dy, w, out, relu_mask_of=None, colsum=None, gelu_grad_of=None, glu_grad_of=None, glu=None):
     """out[T,K] = dy[T,N] @ w[K,N]^T  (optionally masked by relu_mask_of > 0, or multiplied by gelu'(gelu_grad_of),
-    the stored pre-activation z; colsum[k] += sum_t out[t,k])."""
+    the stored pre-activation z; colsum[k] += sum_t out[t,k]).
+
+    glu_grad_of = the stored z [T, 2K] of a gated MLP and glu = its nonlinearity ("relu" / "gelu"): dh = dy @ w^T is
+    the gradient of h and out [T, 2K] receives [dzv | dzg] (include/dalle_b200.h), colsum 2K entries."""
     T, N = dy.shape
     K = w.shape[0]
-    if relu_mask_of is not None and gelu_grad_of is not None:
-        raise L.DB200Error("linear_dgrad: relu_mask_of and gelu_grad_of are exclusive")
+    if sum(v is not None for v in (relu_mask_of, gelu_grad_of, glu_grad_of)) > 1:
+        raise L.DB200Error("linear_dgrad: relu_mask_of, gelu_grad_of and glu_grad_of are exclusive")
+    if (glu_grad_of is None) != (glu is None):
+        raise L.DB200Error("linear_dgrad: glu_grad_of and glu go together")
+    if glu_grad_of is not None:
+        return gemm(dy, w, out, T, K, N, a_mn=False, b_mn=False, mode=L.EPI_RELU_BWD, aux=glu_grad_of,
+                    colsum=colsum, glu="bwd", glu_act=glu)
     if gelu_grad_of is not None:
         return gemm(dy, w, out, T, K, N, a_mn=False, b_mn=False, mode=L.EPI_RELU_BWD, aux=gelu_grad_of,
                     colsum=colsum, gelu="bwd")

@@ -237,6 +237,26 @@ int db200_gemm_bf16_gelu(db200_stream_t stream, const void* A, int a_mn_major, i
 int db200_gemm_bf16_gelu_bwd(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
                              int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
                              const db200_gemm_epilogue* epi);
+/* Gated MLP (extension; DALLE-pytorch's FeedForward: Linear(d, 2*4d), x, gates = chunk(2), x * act(gates)).  N is
+ * the width of h (4d); z = [zv | zg] is [M][2N], value columns first.  act: DB200_ACT_RELU (ReGLU) or DB200_ACT_GELU
+ * (GEGLU, mtf's tanh GELU evaluated as in db200_gemm_bf16_gelu).
+ * Forward store (the W1 product, B = the [K][2N] weight, mn-major, ldb >= 2N): zv = bf16(alpha*acc + bias[n]) over
+ *   columns n < N and zg = bf16(alpha*acc + bias[N + n]) over columns N + n; a = bf16(act(zg)) with ReLU's
+ *   zg > 0 ? zg : 0 (NaN and -0 give +0); D(bf16) [M][N] = bf16(zv * a); z [M][ldz] (ldz >= 2N) receives zv | zg
+ *   when z != NULL.  bias (when given) has 2N entries.  epi->mode must be DB200_EPI_STORE with out_f32 = 0,
+ *   relu = 0 and no residual; A k-major and B mn-major (DB200_E_UNSUPPORTED otherwise); N a multiple of 64.
+ * Backward (the dgrad dh = dbranch W2^T, A and B k-major, N = the dh width): epi->mode must be DB200_EPI_RELU_BWD
+ *   with aux = the stored z (ldaux >= 2N); dh = alpha*acc in fp32, and D(bf16) [M][ldd >= 2N] receives
+ *   dzv = bf16(dh * a) in columns n and dzg = bf16((dh * act'(zg)) * zv) in columns N + n, multiplied in that
+ *   order, with ReGLU's dh * act'(zg) = zg > 0 ? dh : 0 (the RELU_BWD mask) and GEGLU's dh * gelu'(zg).  colsum (bias gradient, 2N entries) gets the column sums of D as for
+ *   RELU_BWD; its workspace is db200_gemm_workspace_bytes(M, 2N, K, epi). */
+enum { DB200_ACT_RELU = 0, DB200_ACT_GELU = 1 };
+int db200_gemm_bf16_glu(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                        int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                        const db200_gemm_epilogue* epi, int act, void* z, int64_t ldz);
+int db200_gemm_bf16_glu_bwd(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
+                            int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
+                            const db200_gemm_epilogue* epi, int act);
 /* number of N tiles the CE_STATS epilogue writes per row for a given N (host helper for sizing part_max/part_sum) */
 int db200_gemm_ce_tiles(int N);
 /* epi->workspace size for this product: split-K slices (ATOMIC) or fused column sums (CE_GRAD / RELU_BWD, which includes

@@ -289,6 +289,17 @@ def validate_rotary(rotary_dim, rotary_base, head_dim):
     return int(rotary_dim), float(base)
 
 
+def validate_shift_tokens(shift_tokens, image_seq_len):
+    """The token-shift switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
+    handled by model_fns.shift_tokens).  On, it needs a square image-token grid (image_seq_len = W^2)."""
+    if not isinstance(shift_tokens, bool):
+        raise ValueError(f"shift_tokens must be a bool, got {shift_tokens!r}")
+    if shift_tokens and math.isqrt(image_seq_len) ** 2 != image_seq_len:
+        raise ValueError(f"shift_tokens needs a square image-token grid, but image_seq_len = {image_seq_len} is not "
+                         f"a square")
+    return shift_tokens
+
+
 def rope_table(n_pos, rotary_dim, base):
     """The fp32 [n_pos, 2, rotary_dim / 2] table of the rotary kernels: position p's cos(p theta_j), then its
     sin(p theta_j), theta_j = base^(-2j / rotary_dim), each evaluated in float64 and rounded once to fp32."""
@@ -304,12 +315,14 @@ class DalleEngine:
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lnf_g", "lnf_b", "bout")
     conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
     gated_mlp = False   # the gated MLP (validate_gated_mlp), set by the constructor
+    shift_tokens = False   # the token shift (validate_shift_tokens), set by the constructor
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
-                 activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False):
+                 activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False,
+                 shift_tokens=False):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -366,9 +379,19 @@ class DalleEngine:
         gated_mlp (validate_gated_mlp): the MLP becomes DALLE-pytorch's gated FeedForward, y = LN2(x) W1 + b1 with W1
         [d, 8d], zv, zg = bf16(y[:, :4d]), bf16(y[:, 4d:]), h = bf16(zv bf16(act(zg))), out = h W2 + b2, with act the
         `activation` (ReGLU or GEGLU).  The gate is fused into the W1 product's epilogue, which keeps z = [zv | zg]
-        ([T, 8d] bf16 per saved layer) for backward, and into its dgrad's."""
+        ([T, 8d] bf16 per saved layer) for backward, and into its dgrad's.
+
+        shift_tokens (validate_shift_tokens): DALLE-pytorch's token shift after both LayerNorms of every layer (its
+        PreNorm(PreShiftToken(...))).  With c = d / 4, a text position's columns [0, 2c) come from the position before
+        it, an image token's [0, c) from the token one grid row above and [c, 2c) from the token to its left, zeros
+        where there is none; [2c, d) are kept (ops.shift_tokens_fwd, exact copies).  The LayerNorm writes a scratch
+        [T, d] and the shift writes the ln1 / ln2 buffers the q|k|v and W1 products and their wgrads read; backward
+        applies the transpose to d(LN out) before the LayerNorm backward, and the decoder keeps a [rows, S, d/2] cache
+        of unshifted outputs per layer and LayerNorm.  No parameter is added."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
+        self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
+        self.shift_w = math.isqrt(image_seq_len) if self.shift_tokens else None   # the grid side W
         self.rotary = validate_rotary(rotary_dim, rotary_base, self.dh)
         self.activation = validate_activation(activation)
         self.gated_mlp = validate_gated_mlp(gated_mlp)
@@ -713,6 +736,10 @@ class DalleEngine:
         e = lambda *shape, dtype=BF16: torch.empty(*shape, dtype=dtype, device=dev)
         nt = ops.ce_tiles(self.Vpad)
         n_saved = 1 if self.recompute_grad else self.L
+        # token shift: one scratch shared by every layer, the unshifted LayerNorm output in forward and the gradient
+        # of the LayerNorm output in backward
+        scratch = e(T, d) if self.shift_tokens else None
+        raw = {"ln1_raw": scratch, "ln2_raw": scratch} if self.shift_tokens else {}
         b = {
             "xs": [e(T, d) for _ in range(self.L + 1)],        # residual stream at every layer boundary
             "layers": [{
@@ -720,7 +747,7 @@ class DalleEngine:
                 "qkv": e(T, 3 * d), "attn": e(T, d), "lse": e(B, self.H, S, dtype=F32),
                 "xmid": e(T, d), "ln2": e(T, d), "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32),
                 "h1": e(T, 4 * d), **({"z1": e(T, 4 * d)} if self.gelu else {}),
-                **({"z1": e(T, 8 * d)} if self.gated_mlp else {}),
+                **({"z1": e(T, 8 * d)} if self.gated_mlp else {}), **raw,
             } for _ in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
             "labels": e(B, S, dtype=I32), "loss_rows": e(T, dtype=F32),
@@ -776,12 +803,21 @@ class DalleEngine:
         return self._drop[kind][i] if self._drop is not None else None
 
     # ------------------------------------------------------------------------------------------ forward
+    def _layernorm_fwd(self, x, p, k, sv, S):
+        """LayerNorm k (1 or 2) of layer prefix p into sv["ln<k>"]; with the token shift the LayerNorm writes
+        sv["ln<k>_raw"] and sv["ln<k>"] receives its shift (rows at position row mod S)."""
+        ln = sv[f"ln{k}"]
+        out = sv[f"ln{k}_raw"] if self.shift_tokens else ln
+        ops.layernorm_fwd(x, self.P(f"{p}ln{k}_g"), self.P(f"{p}ln{k}_b"), out, sv[f"mean{k}"], sv[f"rstd{k}"],
+                          self.ln_eps)
+        if self.shift_tokens:
+            ops.shift_tokens_fwd(out, ln, S, self.text_seq_len, self.shift_w)
+
     def _block_fwd(self, i, x_in, x_out, sv, B, S=None):
         """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x)).
         S: sequence length of the rows (default the model's; prefill runs a shorter prompt)."""
         p = f"l{i}."
-        ops.layernorm_fwd(x_in, self.P(p + "ln1_g"), self.P(p + "ln1_b"), sv["ln1"], sv["mean1"], sv["rstd1"],
-                          self.ln_eps)
+        self._layernorm_fwd(x_in, p, 1, sv, S or self.S)
         ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
         if self.rotary:
             ops.rope_fwd(sv["qkv"], self.rope_table, S or self.S, self.H, self.dh, self.rotary_dim)
@@ -790,8 +826,7 @@ class DalleEngine:
                      **self.conv_kw[i])  # :257-299
         ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in,
                        dropout=self._site("attn_out", i))                               # :303-314,330
-        ops.layernorm_fwd(sv["xmid"], self.P(p + "ln2_g"), self.P(p + "ln2_b"), sv["ln2"], sv["mean2"], sv["rstd2"],
-                          self.ln_eps)
+        self._layernorm_fwd(sv["xmid"], p, 2, sv, S or self.S)
         if self.gated_mlp:   # h1 = zv * act(zg), z1 = [zv | zg] = LN2 W1 + b1 kept for backward (prefill: not written)
             ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), glu=self.glu,
                            z_out=sv.get("z1"))
@@ -959,19 +994,24 @@ class DalleEngine:
             "xs": [e(T, d), e(T, d)],
             "sv": {"ln1": e(T, d), "mean1": e(T, dtype=F32), "rstd1": e(T, dtype=F32), "qkv": e(T, 3 * d),
                    "attn": e(T, d), "lse": e(B, self.H, P, dtype=F32), "xmid": e(T, d), "ln2": e(T, d),
-                   "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32), "h1": e(T, 4 * d)},
+                   "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32), "h1": e(T, 4 * d),
+                   # token shift: both unshifted LayerNorm outputs stay until the layer's caches are filled
+                   **({"ln1_raw": e(T, d), "ln2_raw": e(T, d)} if self.shift_tokens else {})},
             "x_last": e(B * rep, d), "hf": e(B * rep, d), "meanf": e(B * rep, dtype=F32),
             "rstdf": e(B * rep, dtype=F32), "logits": e(B * rep, self.Vpad, dtype=F32),
         }
         self._pf_key = key
         return self._pf
 
-    def prefill(self, tokens, k_caches, v_caches, rep=1):
+    def prefill(self, tokens, k_caches, v_caches, rep=1, shift_caches=None):
         """Runs a whole prompt, tokens int32 [B, P] (1 <= P < S), through the training forward kernels in one pass
         and hands it to the decoder: every layer's k / v of positions < P go into k_caches[i] / v_caches[i] (bf16
         [B*rep, S, H, dh], rows b*rep .. b*rep + rep - 1 all receive prompt b), and the result is the fp32 logits
         [B*rep, Vpad] of position P for each replica.  No dropout (inference); the training buffers and the state a
-        pending backward() reads are left untouched."""
+        pending backward() reads are left untouched.
+
+        shift_caches (required with the token shift, else None): 2 L bf16 [B*rep, S, d/2] caches, layer i's LN1 at
+        2i and its LN2 at 2i + 1; positions < P receive the first d/2 columns of the unshifted LayerNorm outputs."""
         B, P = tokens.shape
         if not 1 <= P < self.S:
             raise ValueError(f"prefill: prompt length {P} outside [1, {self.S})")
@@ -982,6 +1022,13 @@ class DalleEngine:
         if len(k_caches) != self.L or len(v_caches) != self.L or \
                 any(tuple(c.shape) != shape for c in list(k_caches) + list(v_caches)):
             raise ValueError(f"prefill: expected {self.L} k and v caches of shape {shape}")
+        if self.shift_tokens:
+            sshape = (B * rep, self.S, self.d // 2)
+            if shift_caches is None or len(shift_caches) != 2 * self.L or \
+                    any(tuple(c.shape) != sshape for c in shift_caches):
+                raise ValueError(f"prefill: the token shift needs {2 * self.L} shift caches of shape {sshape}")
+        elif shift_caches is not None:
+            raise ValueError("prefill: shift_caches given to an engine without the token shift")
         b = self._prefill_alloc(B, P, rep)
         d = self.d
         ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(), b["xs"][0].view(B, P, d))
@@ -991,6 +1038,9 @@ class DalleEngine:
             for i in range(self.L):
                 self._block_fwd(i, x_in, x_out, b["sv"], B, S=P)
                 ops.kv_cache_fill(b["sv"]["qkv"], k_caches[i], v_caches[i], P, rep)
+                if self.shift_tokens:
+                    ops.shift_cache_fill(b["sv"]["ln1_raw"], shift_caches[2 * i], P, rep)
+                    ops.shift_cache_fill(b["sv"]["ln2_raw"], shift_caches[2 * i + 1], P, rep)
                 x_in, x_out = x_out, x_in
         finally:
             self._drop = drop
@@ -1012,6 +1062,11 @@ class DalleEngine:
         ops.layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=dxsum, dxm=dxm, dropout=site)
         return dxm
 
+    def _shift_bwd(self, dshifted, out):
+        """The token shift's transpose: the gradient of the unshifted LayerNorm output, written to `out`."""
+        ops.shift_tokens_bwd(dshifted, out, self.S, self.text_seq_len, self.shift_w)
+        return out
+
     def _block_bwd(self, i, x_in, sv, dx_out, dx_in, bufs, B, dxsum_below, dbranch):
         """Backward of one block.  Bias gradients are column sums of activation gradients; they are produced by the
         kernel that WRITES that gradient (LayerNorm-backward / ReLU-mask epilogue) instead of separate passes:
@@ -1031,8 +1086,9 @@ class DalleEngine:
         ops.linear_wgrad(sv["h1"], dbranch, self.G(p + "w2"))
         ops.linear_dgrad(dz, self.W(p + "w1"), bufs["dtmp"])                                  # dLN2 out
         ops.linear_wgrad(sv["ln2"], dz, self.G(p + "w1"))
+        dln = self._shift_bwd(bufs["dtmp"], sv["ln2_raw"]) if self.shift_tokens else bufs["dtmp"]
         dx_mid = bufs["dx_b"] if dx_out is bufs["dx_a"] else bufs["dx_a"]
-        da = self._ln_bwd(bufs["dtmp"], sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
+        da = self._ln_bwd(dln, sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
                           self.G(p + "ln2_g"), self.G(p + "ln2_b"), self.G(p + "o_b"),
                           self._site("attn_out", i))                                    # do_b = colsum(da)
         # ---- attention
@@ -1045,7 +1101,8 @@ class DalleEngine:
             ops.rope_bwd(bufs["dqkv"], self.rope_table, self.S, self.H, self.dh, self.rotary_dim)
         ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                      # dLN1 out
         ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
-        return self._ln_bwd(bufs["dtmp"], x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
+        dln = self._shift_bwd(bufs["dtmp"], sv["ln1_raw"]) if self.shift_tokens else bufs["dtmp"]
+        return self._ln_bwd(dln, x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
                             self.G(p + "ln1_g"), self.G(p + "ln1_b"), dxsum_below,
                             self._site("mlp_out", i - 1) if i > 0 else None)          # db2 of the layer below
 

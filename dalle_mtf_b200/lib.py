@@ -167,6 +167,11 @@ _SIGNATURES = {
     "db200_rope_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_rope_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_rope_decode_dev": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
+    "db200_shift_tokens_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_shift_tokens_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_shift_tokens_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
+    "db200_shift_tokens_decode_dev": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
+    "db200_shift_cache_fill": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_crc32c": [c_vp, c_u64, c_vp],
     "db200_tfrecord_masked_crc": [c_vp, c_u64, c_vp],
     "db200_tfrecord_frame": [c_vp, c_u64, c_vp],

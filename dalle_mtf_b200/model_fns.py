@@ -16,7 +16,7 @@ from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
     validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
-    validate_rotary
+    validate_rotary, validate_shift_tokens
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -165,6 +165,19 @@ def gated_mlp(params):
     return v
 
 
+def shift_tokens(params, image_seq_len=None):
+    """shift_tokens of a DALL-E config: absent, null or false is off; true turns on DALLE-pytorch's token shift after
+    both LayerNorms of every layer (DalleEngine), which needs a square image-token grid (checked here when
+    image_seq_len is given, and by the engine).  Only a JSON bool is accepted: 1, "true" or a list is rejected.  No
+    parameter depends on it, so checkpoints keep their layout."""
+    v = params.get("shift_tokens")
+    if v is None:
+        return False
+    if not isinstance(v, bool):
+        raise ValueError(f"shift_tokens = {v!r}: expected null, true or false")
+    return v if image_seq_len is None else validate_shift_tokens(v, image_seq_len)
+
+
 def conv_kernel(params):
     """conv_attention_kernel of a DALL-E config: the k of "conv" layers' k x k window (DalleEngine), an integer >= 1.
     A missing or null key is 5, DALLE-pytorch's default."""
@@ -257,6 +270,7 @@ def dalle_model_fn(features, labels, mode, params):
     pos_scheme, per_pos, pp_pad = input_embedding(params)
     activation = activation_function(params)
     gated = gated_mlp(params)
+    shift = shift_tokens(params)
     mask = logits_mask(params)
     rotary_dim, rotary_base = rotary_embedding(params)
     L.require_device()
@@ -293,7 +307,7 @@ def dalle_model_fn(features, labels, mode, params):
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
                         activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
-                        gated_mlp=gated)
+                        gated_mlp=gated, shift_tokens=shift)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

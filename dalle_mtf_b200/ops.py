@@ -1085,6 +1085,73 @@ def rope_decode_dev(qkv, table, pos_dev, H, dh, r):
           "db200_rope_decode_dev")
 
 
+def _shift_rows(y, what):
+    """(rows, d) of a contiguous bf16 [rows, d] operand of the token-shift kernels."""
+    L.require_device()
+    _chk(y, BF16, what)
+    if not y.is_contiguous() or y.dim() != 2:
+        raise L.DB200Error(f"{what}: expected a contiguous [rows, d] tensor, got {tuple(y.shape)}")
+    return y.shape
+
+
+def _shift_cache(cache, rows, d, what):
+    """The length S of a token-shift cache bf16 [rows, S, d/2]."""
+    _chk(cache, BF16, what)
+    if not cache.is_contiguous() or cache.dim() != 3 or cache.shape[0] != rows or cache.shape[2] * 2 != d:
+        raise L.DB200Error(f"{what}: expected a contiguous [{rows}, S, {d // 2}] cache, got {tuple(cache.shape)}")
+    return cache.shape[1]
+
+
+def shift_tokens_fwd(y, out, S, text_len, grid_w):
+    """Token shift out = shift(y) of bf16 [rows, d] LayerNorm outputs, row t at position t mod S: the first d/4
+    columns from the token above (image) or before (text), the next d/4 from the token to the left (image) or before
+    (text), zeros where there is none (include/dalle_b200.h)."""
+    rows, d = _shift_rows(y, "y")
+    if tuple(_shift_rows(out, "out")) != (rows, d):
+        raise L.DB200Error(f"shift_tokens_fwd: out {tuple(out.shape)} does not match y {(rows, d)}")
+    check(L.load().db200_shift_tokens_fwd(stream_ptr(), ptr(y), ptr(out), rows, int(S), d, int(text_len),
+                                          int(grid_w)), "db200_shift_tokens_fwd")
+
+
+def shift_tokens_bwd(dout, dy, S, text_len, grid_w):
+    """The transpose of shift_tokens_fwd: dy = shift^T(dout), bf16 [rows, d]."""
+    rows, d = _shift_rows(dout, "dout")
+    if tuple(_shift_rows(dy, "dy")) != (rows, d):
+        raise L.DB200Error(f"shift_tokens_bwd: dy {tuple(dy.shape)} does not match dout {(rows, d)}")
+    check(L.load().db200_shift_tokens_bwd(stream_ptr(), ptr(dout), ptr(dy), rows, int(S), d, int(text_len),
+                                          int(grid_w)), "db200_shift_tokens_bwd")
+
+
+def shift_tokens_decode(y, cache, pos, text_len, grid_w):
+    """One decoding step of the token shift at position pos, in place on y bf16 [rows, d]: y's first d/2 columns go
+    into cache[:, pos] (bf16 [rows, S, d/2]) and are replaced by the shifted chunks read from the cache."""
+    rows, d = _shift_rows(y, "y")
+    S = _shift_cache(cache, rows, d, "cache")
+    check(L.load().db200_shift_tokens_decode(stream_ptr(), ptr(y), ptr(cache), rows, S, d, int(text_len), int(grid_w),
+                                             int(pos)), "db200_shift_tokens_decode")
+
+
+def shift_tokens_decode_dev(y, cache, pos_dev, text_len, grid_w):
+    """shift_tokens_decode with the position read on the device from pos_dev (graph replay)."""
+    rows, d = _shift_rows(y, "y")
+    S = _shift_cache(cache, rows, d, "cache")
+    _chk(pos_dev, I32, "pos_dev")
+    check(L.load().db200_shift_tokens_decode_dev(stream_ptr(), ptr(y), ptr(cache), rows, S, d, int(text_len),
+                                                 int(grid_w), ptr(pos_dev)), "db200_shift_tokens_decode_dev")
+
+
+def shift_cache_fill(y, cache, P, rep=1):
+    """Prefill hand-off of the token shift: y bf16 [B*P, d], the unshifted LayerNorm outputs of B prompts of P
+    positions -> cache bf16 [B*rep, S, d/2], cache[b*rep + r, p] = y[b*P + p, :d/2] (kv_cache_fill's replica order)."""
+    rows, d = _shift_rows(y, "y")
+    if P < 1 or rows % P:
+        raise L.DB200Error(f"shift_cache_fill: {rows} rows are not a whole number of {P}-position prompts")
+    B = rows // P
+    S = _shift_cache(cache, B * int(rep), d, "cache")
+    check(L.load().db200_shift_cache_fill(stream_ptr(), ptr(y), ptr(cache), B, int(P), d, S, int(rep)),
+          "db200_shift_cache_fill")
+
+
 def rows_repeat(src, dst, rep=1):
     """dst[b*rep + r] = src[b] for a [B, d] view src (rows may be strided, e.g. x.view(B, P, d)[:, P - 1])."""
     L.require_device()

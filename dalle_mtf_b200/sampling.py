@@ -12,7 +12,9 @@ parameters and the same kernels' numerics as training:
                     positions and p's image row or column; a conv layer the text positions and p's k x k window)
                     x = x + a Wo + o_b;  x = x + act(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows;
                     act = ReLU, or GELU without a pre-activation output); with rotary embeddings q and k are
-                    rotated to position p (rope_decode) before k enters the cache
+                    rotated to position p (rope_decode) before k enters the cache; with the token shift each
+                    LayerNorm output's first d/2 columns enter a per-layer cache and are replaced by the shifted
+                    chunks of positions p - 1 and p - W (shift_tokens_decode)
   logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
 
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
@@ -80,6 +82,8 @@ class DalleSampler:
         mk = lambda *shape, dtype=BF16: torch.empty(*shape, dtype=dtype, device=dev)
         self.kc = [mk(B, e.S, e.H, e.dh) for _ in range(e.L)]
         self.vc = [mk(B, e.S, e.H, e.dh) for _ in range(e.L)]
+        # token shift: the unshifted first d/2 columns of every position's LN1 (2i) and LN2 (2i + 1) output of layer i
+        self.sc = [mk(B, e.S, d // 2) for _ in range(2 * e.L)] if e.shift_tokens else None
         self.x = [mk(B, d), mk(B, d)]
         self.ln = mk(B, d)
         self.qkv = mk(B, 3 * d)
@@ -99,6 +103,8 @@ class DalleSampler:
         for i in range(e.L):
             p = f"l{i}."
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
+            if e.shift_tokens:
+                ops.shift_tokens_decode(self.ln, self.sc[2 * i], pos, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
             if e.rotary:
                 ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
@@ -106,6 +112,8 @@ class DalleSampler:
                             **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
+            if e.shift_tokens:
+                ops.shift_tokens_decode(self.ln, self.sc[2 * i + 1], pos, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             ops.linear_fwd(self.h1, e.W(p + "w2"), x_out, bias=e.P(p + "b2"), residual=self.xmid)
             x_in, x_out = x_out, x_in
@@ -123,6 +131,8 @@ class DalleSampler:
         for i in range(e.L):
             p = f"l{i}."
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
+            if e.shift_tokens:
+                ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i], self.pos_dev, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
             if e.rotary:
                 ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
@@ -130,6 +140,8 @@ class DalleSampler:
                                 radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
             ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
+            if e.shift_tokens:
+                ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i + 1], self.pos_dev, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             ops.linear_fwd(self.h1, e.W(p + "w2"), x_out, bias=e.P(p + "b2"), residual=self.xmid)
             x_in, x_out = x_out, x_in
@@ -286,7 +298,7 @@ class DalleSampler:
             prompt[B:, :TL] = self._uncond(B)
         if n:   # (with guidance the padding-caption prompts continue with the same image prefix)
             prompt[:, TL:] = (image_prefix.to(device=e.device, dtype=I32) + e.image_offset).repeat(len(prompt) // B, 1)
-        logits = e.prefill(prompt, self.kc, self.vc, rep)
+        logits = e.prefill(prompt, self.kc, self.vc, rep, shift_caches=self.sc)
         lo, hi = e.image_offset, e.image_offset + e.image_vocab_size
         if self.u is not None:
             self.u.uniform_(1e-9, 1.0)

@@ -668,6 +668,35 @@ int db200_rope_decode(db200_stream_t stream, void* qkv_bf16, const float* table,
 int db200_rope_decode_dev(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh,
                           int r, const int32_t* pos_dev);
 
+/* Token shift (extension; DALLE-pytorch's PreShiftToken) on a bf16 [rows][d] LayerNorm output y, c = d / 4.  Position
+ * p < text_len (TL) is a text token, p >= TL the image token u = p - TL at grid row u / grid_w, column u % grid_w.
+ * shift(y)[p] keeps y[p][2c, d) and replaces
+ *   text p       : [0, 2c) by y[p-1][0, 2c)                                 (zeros at p = 0)
+ *   image (r, k) : [0, c) by y[p - grid_w][0, c) if r >= 1, [c, 2c) by y[p-1][c, 2c) if k >= 1, zeros otherwise
+ * Pure copies (16-byte vectors, 64-bit offsets): exact.
+ *   shift_tokens_fwd        : out = shift(y), row t at position t mod S (out of place).
+ *   shift_tokens_bwd        : dy = shift^T(dout): text p gets dout[p+1][0, 2c) if p + 1 < TL; image (r, k) gets
+ *                             dout[p + grid_w][0, c) if r + 1 < grid_w and dout[p+1][c, 2c) if k + 1 < grid_w
+ *                             (sources at positions >= S excluded); [2c, d) is copied.
+ *   shift_tokens_decode     : one decoding step at position pos, in place on y [rows][d] with the cache bf16
+ *                             [rows][S][d/2]: cache[b][pos] = y[b][0, 2c), then y[b][0, 2c) = the shifted chunks read
+ *                             from cache[b][pos-1] / cache[b][pos-grid_w] (or zeros).  0 <= pos < S.
+ *   shift_tokens_decode_dev : the same at position *pos_dev (graph replay); a position outside [0, S) changes nothing.
+ *   shift_cache_fill        : prefill hand-off, y bf16 [B][P][d] -> cache [B*rep][S_cache][d/2]: cache[b*rep + r][p] =
+ *                             y[b][p][0, 2c) for p < P, r < rep (kv_cache_fill's replica order).
+ * rows, S, d, grid_w > 0, text_len >= 0, S <= text_len + grid_w^2, d % 32 == 0, non-NULL and non-overlapping buffers,
+ * else DB200_E_INVALID; pointers not 16-byte aligned -> DB200_E_ALIGN. */
+int db200_shift_tokens_fwd(db200_stream_t stream, const void* y_bf16, void* out_bf16, int rows, int S, int d,
+                           int text_len, int grid_w);
+int db200_shift_tokens_bwd(db200_stream_t stream, const void* dout_bf16, void* dy_bf16, int rows, int S, int d,
+                           int text_len, int grid_w);
+int db200_shift_tokens_decode(db200_stream_t stream, void* y_bf16, void* cache_bf16, int rows, int S, int d,
+                              int text_len, int grid_w, int pos);
+int db200_shift_tokens_decode_dev(db200_stream_t stream, void* y_bf16, void* cache_bf16, int rows, int S, int d,
+                                  int text_len, int grid_w, const int32_t* pos_dev);
+int db200_shift_cache_fill(db200_stream_t stream, const void* y_bf16, void* cache_bf16, int B, int P, int d,
+                           int S_cache, int rep);
+
 /* Segmented bf16 -> f32 gather (one launch): segment i copies table[3i+2] elements from src + table[3i] to
  * dst + table[3i+1]; `table_dev` is an int64 array in device memory.  ZeRO-1 mode: rebuilds the compact fp32 copy of the
  * vector parameters (LayerNorm g/b, biases) from the all-gathered bf16 parameters (mtf casts every variable to the

@@ -305,12 +305,22 @@ pos_fold_kernel(const float* __restrict__ dpos, float* __restrict__ dwpe, float*
 }
 
 // ------------------------------------------------------------------------------------------------ LayerNorm
+// o[j] = r[j] + o[j] for the 8 bf16 residual values at r (the sandwich LayerNorm's residual add, in fp32)
+__device__ __forceinline__ void ln_add_res8(const bf16* r, float* o) {
+  float rv[8];
+  unpack8(*reinterpret_cast<const uint4*>(r), rv);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = rv[j] + o[j];
+}
+
 // One warp per row; the row lives in registers (NCH 16-byte chunks per lane, d = NCH * 256).
-template <int NCH>
+// RES (sandwich LayerNorm): y = bf16(res + (x - mean) * rstd * g + b), one rounding; the statistics are the same
+// instructions as without it.  `res` is a trailing parameter so that the RES = false kernels keep their code.
+template <int NCH, bool RES = false>
 __global__ void __launch_bounds__(128)
 layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, const float* __restrict__ b,
                      bf16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows,
-                     float eps) {
+                     float eps, const bf16* __restrict__ res = nullptr) {
   constexpr int d = NCH * 256;
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -349,6 +359,7 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, co
     float o[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean) * rstd * gg[j] + bb[j];
+    if constexpr (RES) ln_add_res8(res + (long long)row * d + col, o);
     *reinterpret_cast<uint4*>(yr + col) = pack8(o);
   }
 }
@@ -473,11 +484,11 @@ __device__ __forceinline__ float2 block128_sum2(float a, float b, float* red /*[
   return make_float2(red[0] + red[1] + red[2] + red[3], red[4] + red[5] + red[6] + red[7]);
 }
 
-template <int NCW>
+template <int NCW, bool RES = false>
 __global__ void __launch_bounds__(128)
 layernorm_fwd_wide_kernel(const bf16* __restrict__ x, const float* __restrict__ g, const float* __restrict__ b,
                           bf16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows,
-                          float eps) {
+                          float eps, const bf16* __restrict__ res = nullptr) {
   constexpr int d = NCW * 1024;
   __shared__ float red[8];
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
@@ -515,6 +526,7 @@ layernorm_fwd_wide_kernel(const bf16* __restrict__ x, const float* __restrict__ 
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean) * rstd * gg[j] + bb[j];
+      if constexpr (RES) ln_add_res8(res + (long long)row * d + col, o);
       *reinterpret_cast<uint4*>(yr + col) = pack8(o);
     }
   }
@@ -955,6 +967,31 @@ extern "C" int db200_layernorm_fwd(db200_stream_t stream_, const void* x, const 
       return set_error(DB200_E_UNSUPPORTED, "layernorm: d=%d not in {256,512,768,1024,2048,4096}", d);
   }
   return check_launch("layernorm_fwd_kernel");
+}
+
+extern "C" int db200_layernorm_residual_fwd(db200_stream_t stream_, const void* o, const void* x_res, const float* g,
+                                            const float* b, void* y, float* mean, float* rstd, int rows, int d,
+                                            float eps) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(rows > 0, DB200_E_INVALID, "layernorm_residual_fwd: rows must be positive");
+  DB200_REQUIRE(o && x_res && y && g && b && mean && rstd, DB200_E_INVALID, "layernorm_residual_fwd: NULL pointer");
+  DB200_REQUIRE(aligned16(o) && aligned16(x_res) && aligned16(y) && aligned16(g) && aligned16(b), DB200_E_ALIGN,
+                "layernorm_residual_fwd: unaligned pointer");
+  const int grid = (rows + 3) / 4;
+  const bf16* op = (const bf16*)o;
+  const bf16* rp = (const bf16*)x_res;
+  bf16* yp = (bf16*)y;
+  switch (d) {
+    case 256:  layernorm_fwd_kernel<1, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp); break;
+    case 512:  layernorm_fwd_kernel<2, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp); break;
+    case 768:  layernorm_fwd_kernel<3, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp); break;
+    case 1024: layernorm_fwd_kernel<4, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp); break;
+    case 2048: layernorm_fwd_kernel<8, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp); break;
+    case 4096: layernorm_fwd_wide_kernel<4, true><<<min(rows, sm_count() * 16), 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp); break;
+    default:
+      return set_error(DB200_E_UNSUPPORTED, "layernorm_residual_fwd: d=%d not in {256,512,768,1024,2048,4096}", d);
+  }
+  return check_launch("layernorm_residual_fwd_kernel");
 }
 
 static int layernorm_bwd_grid(int rows, int d) {

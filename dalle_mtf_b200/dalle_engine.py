@@ -61,12 +61,13 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
-def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False):
+def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
     length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
     column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
     the grid_w rows and columns of the image-token grid.  gated_mlp: w1 is [d, 8d] and b1 [8d], the value columns
-    first and the gate columns second."""
+    first and the gate columns second.  sandwich_norm: each layer ends with its two output LayerNorms, lna_g / lna_b
+    (attention branch) and lnm_g / lnm_b (MLP branch), inside the layer's span l{i}.ln1_g .. layer_last(i)."""
     w1_cols = 8 * d if gated_mlp else 4 * d
     Vpad = _round_up(V, 64)
     lay = ParamLayout()
@@ -84,6 +85,9 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False)
         lay.add(p + "ln2_g", (d,)); lay.add(p + "ln2_b", (d,))
         lay.add(p + "w1", (d, w1_cols)); lay.add(p + "b1", (w1_cols,))
         lay.add(p + "w2", (4 * d, d)); lay.add(p + "b2", (d,))
+        if sandwich_norm:
+            lay.add(p + "lna_g", (d,)); lay.add(p + "lna_b", (d,))
+            lay.add(p + "lnm_g", (d,)); lay.add(p + "lnm_b", (d,))
     lay.add("lnf_g", (d,)); lay.add("lnf_b", (d,))
     lay.add("wout", (d, Vpad)); lay.add("bout", (Vpad,))
     return lay
@@ -289,6 +293,14 @@ def validate_rotary(rotary_dim, rotary_base, head_dim):
     return int(rotary_dim), float(base)
 
 
+def validate_sandwich_norm(sandwich_norm):
+    """The sandwich LayerNorm switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
+    handled by model_fns.sandwich_norm)."""
+    if not isinstance(sandwich_norm, bool):
+        raise ValueError(f"sandwich_norm must be a bool, got {sandwich_norm!r}")
+    return sandwich_norm
+
+
 def validate_shift_tokens(shift_tokens, image_seq_len):
     """The token-shift switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
     handled by model_fns.shift_tokens).  On, it needs a square image-token grid (image_seq_len = W^2)."""
@@ -312,17 +324,19 @@ def rope_table(n_pos, rotary_dim, base):
 class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
-    VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lnf_g", "lnf_b", "bout")
+    VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lna_g", "lna_b", "lnm_g", "lnm_b", "lnf_g",
+                     "lnf_b", "bout")
     conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
     gated_mlp = False   # the gated MLP (validate_gated_mlp), set by the constructor
     shift_tokens = False   # the token shift (validate_shift_tokens), set by the constructor
+    sandwich_norm = False   # the sandwich LayerNorm (validate_sandwich_norm), set by the constructor
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
                  activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False,
-                 shift_tokens=False):
+                 shift_tokens=False, sandwich_norm=False):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -387,11 +401,19 @@ class DalleEngine:
         where there is none; [2c, d) are kept (ops.shift_tokens_fwd, exact copies).  The LayerNorm writes a scratch
         [T, d] and the shift writes the ln1 / ln2 buffers the q|k|v and W1 products and their wgrads read; backward
         applies the transpose to d(LN out) before the LayerNorm backward, and the decoder keeps a [rows, S, d/2] cache
-        of unshifted outputs per layer and LayerNorm.  No parameter is added."""
+        of unshifted outputs per layer and LayerNorm.  No parameter is added.
+
+        sandwich_norm (validate_sandwich_norm): CogView's Sandwich-LN as DALLE-pytorch's PreNorm(..., sandwich=True)
+        builds it.  Each branch output after its residual dropout, oa = drop(a Wo + o_b) and om = drop(h W2 + b2), is
+        normalised by its own LayerNorm before the residual add: xmid = x + LNa(oa), xout = xmid + LNm(om), one
+        rounding each (ops.layernorm_residual_fwd); LNa / LNm are the parameters lna_g / lna_b and lnm_g / lnm_b
+        (layer_i/attn/norm_out and layer_i/mlp/norm_out), g = 1 and b = 0 at initialisation, not weight-decayed.  oa,
+        om and their statistics are kept per saved layer (two bf16 [T, d] and four fp32 [T])."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
         self.shift_w = math.isqrt(image_seq_len) if self.shift_tokens else None   # the grid side W
+        self.sandwich_norm = validate_sandwich_norm(sandwich_norm)
         self.rotary = validate_rotary(rotary_dim, rotary_base, self.dh)
         self.activation = validate_activation(activation)
         self.gated_mlp = validate_gated_mlp(gated_mlp)
@@ -446,8 +468,9 @@ class DalleEngine:
                                      # (text block, image block) pair)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
-        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, gated_mlp=self.gated_mlp) \
-            if self.row_col else param_layout(d, Lyr, V, S, gated_mlp=self.gated_mlp)
+        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, gated_mlp=self.gated_mlp,
+                                         sandwich_norm=self.sandwich_norm) \
+            if self.row_col else param_layout(d, Lyr, V, S, gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm)
         self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
@@ -539,8 +562,9 @@ class DalleEngine:
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else S
         gate = (4 * d * d + 4 * d) if self.gated_mlp else 0   # the gate half of W1 and b1
+        sandwich = 4 * d if self.sandwich_norm else 0         # LNa and LNm: g and b each
         return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d +
-                                          gate) + 2 * d + d * V + V
+                                          gate + sandwich) + 2 * d + d * V + V
 
     EMBED_REF_NAMES = {"wte": "embedding/wte", "wpe": "positional_embedding/wpe",
                        "image_row": "positional_embedding/image_row", "image_col": "positional_embedding/image_col"}
@@ -550,14 +574,37 @@ class DalleEngine:
         return self.EMBED_REF_NAMES.get(name, name)
 
     @staticmethod
-    def _ref_names(i):
+    def _ref_names(i, sandwich_norm=False):
         pre = f"layer_{i}/"
-        return {
+        names = {
             "ln1_g": pre + "norm_1/g", "ln1_b": pre + "norm_1/b", "wo": pre + "attn/o",
             "o_b": pre + "attn/compute_output_bias/o_b", "ln2_g": pre + "norm_2/g", "ln2_b": pre + "norm_2/b",
             "w1": pre + "mlp/mlp_linear_1/kernel", "b1": pre + "mlp/mlp_linear_1/bias",
             "w2": pre + "mlp/mlp_linear_2/kernel", "b2": pre + "mlp/mlp_linear_2/bias",
         }
+        if sandwich_norm:
+            names.update({"lna_g": pre + "attn/norm_out/g", "lna_b": pre + "attn/norm_out/b",
+                          "lnm_g": pre + "mlp/norm_out/g", "lnm_b": pre + "mlp/norm_out/b"})
+        return names
+
+    def _layer_ref_names(self, i):
+        """Reference names of layer i's parameters other than q / k / v (with this engine's sandwich_norm)."""
+        return self._ref_names(i, self.sandwich_norm)
+
+    def _check_sandwich_names(self, named):
+        """Refuse a checkpoint of the other sandwich_norm kind: one without a sandwich LayerNorm this model has, or
+        with one this model does not have (which would otherwise be ignored and leave a different model).  The error
+        names the first such variable."""
+        want = [rn for i in range(self.L) for rn in self._ref_names(i, True).values() if "/norm_out/" in rn] \
+            if self.sandwich_norm else []
+        for rn in want:   # layer order: layer_i/attn/norm_out/g, /b, layer_i/mlp/norm_out/g, /b
+            if rn not in named:
+                raise L.DB200Error(f"load_params: {rn}: missing from the checkpoint of a sandwich_norm model")
+        extra = [k for k in named if k.startswith("layer_") and "/norm_out/" in k and k not in want]
+        if extra:
+            k = min(extra, key=lambda n: (n.split("/")[0], n.split("/")[1] != "attn", n.endswith("/b")))
+            raise L.DB200Error(f"load_params: {k}: a sandwich LayerNorm variable, but this model has "
+                               f"sandwich_norm = {self.sandwich_norm}")
 
     def load_params(self, named):
         """Load a dict keyed by the reference's variable names (SURVEY.md Appendix B); CPU or CUDA fp32 tensors."""
@@ -590,6 +637,7 @@ class DalleEngine:
     def load_flat(self, flat, named):
         """Fill one of the flat fp32 buffers (master | adam_m | adam_v) from a dict of reference-named tensors."""
         dev = self.device
+        self._check_sandwich_names(named)
         if self.zero is not None:
             if flat is not self.master:
                 raise L.DB200Error("ZeRO-1 mode: loading sharded Adam slots is not implemented (throughput configuration)")
@@ -599,7 +647,7 @@ class DalleEngine:
                 self._scatter_full(name, f32(named[self._ref_embed_name(name)]))
             for i in range(self.L):
                 p = f"l{i}."
-                for k, rn in self._ref_names(i).items():
+                for k, rn in self._layer_ref_names(i).items():
                     self._scatter_full(p + k, f32(named[rn]))
                 pre = f"layer_{i}/attn/"
                 self._scatter_full(p + "wqkv", torch.cat([f32(named[pre + "q"]), f32(named[pre + "k"]),
@@ -625,7 +673,7 @@ class DalleEngine:
             put(name, named[self._ref_embed_name(name)])
         for i in range(self.L):
             p = f"l{i}."
-            ref = self._ref_names(i)
+            ref = self._layer_ref_names(i)
             for k, rn in ref.items():
                 put(p + k, named[rn])
             pre = f"layer_{i}/attn/"
@@ -648,7 +696,7 @@ class DalleEngine:
         d = self.d
         for i in range(self.L):
             p = f"l{i}."
-            for k, rn in self._ref_names(i).items():
+            for k, rn in self._layer_ref_names(i).items():
                 out[rn] = view(p + k)
             wqkv = view(p + "wqkv")
             pre = f"layer_{i}/attn/"
@@ -679,6 +727,8 @@ class DalleEngine:
         for i in range(Lyr):
             p = f"l{i}."
             self.P(p + "ln1_g").fill_(1.0); self.P(p + "ln2_g").fill_(1.0)
+            if self.sandwich_norm:
+                self.P(p + "lna_g").fill_(1.0); self.P(p + "lnm_g").fill_(1.0)
             wqkv = self.P(p + "wqkv")
             wqkv[:, :d].copy_(torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5))
             wqkv[:, d:].copy_(torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5))
@@ -701,6 +751,8 @@ class DalleEngine:
         for i in range(Lyr):
             p = f"l{i}."
             self._scatter_full(p + "ln1_g", ones(d)); self._scatter_full(p + "ln2_g", ones(d))
+            if self.sandwich_norm:
+                self._scatter_full(p + "lna_g", ones(d)); self._scatter_full(p + "lnm_g", ones(d))
             wq = torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5)
             wkv = torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5)
             self._scatter_full(p + "wqkv", torch.cat([wq, wkv], dim=1))
@@ -740,6 +792,9 @@ class DalleEngine:
         # of the LayerNorm output in backward
         scratch = e(T, d) if self.shift_tokens else None
         raw = {"ln1_raw": scratch, "ln2_raw": scratch} if self.shift_tokens else {}
+        # sandwich LayerNorm: both branch outputs and the statistics of their LayerNorms, for backward
+        sand = (lambda: {"oa": e(T, d), "om": e(T, d), "meana": e(T, dtype=F32), "rstda": e(T, dtype=F32),
+                         "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)}) if self.sandwich_norm else dict
         b = {
             "xs": [e(T, d) for _ in range(self.L + 1)],        # residual stream at every layer boundary
             "layers": [{
@@ -747,7 +802,7 @@ class DalleEngine:
                 "qkv": e(T, 3 * d), "attn": e(T, d), "lse": e(B, self.H, S, dtype=F32),
                 "xmid": e(T, d), "ln2": e(T, d), "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32),
                 "h1": e(T, 4 * d), **({"z1": e(T, 4 * d)} if self.gelu else {}),
-                **({"z1": e(T, 8 * d)} if self.gated_mlp else {}), **raw,
+                **({"z1": e(T, 8 * d)} if self.gated_mlp else {}), **raw, **sand(),
             } for _ in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
             "labels": e(B, S, dtype=I32), "loss_rows": e(T, dtype=F32),
@@ -813,8 +868,20 @@ class DalleEngine:
         if self.shift_tokens:
             ops.shift_tokens_fwd(out, ln, S, self.text_seq_len, self.shift_w)
 
+    def _branch_out(self, p, norm, x, w, bias, x_res, out, site, sv):
+        """The output projection of a branch of layer prefix p and its residual add: out = x_res + drop(x w + bias),
+        or with the sandwich LayerNorm sv["o<norm>"] = drop(x w + bias) and out = x_res + LN<norm>(sv["o<norm>"])
+        (norm "a": the attention branch's, "m": the MLP's)."""
+        if not self.sandwich_norm:
+            return ops.linear_fwd(x, w, out, bias=bias, residual=x_res, dropout=site)
+        o = sv["o" + norm]
+        ops.linear_fwd(x, w, o, bias=bias, dropout=site)
+        ops.layernorm_residual_fwd(o, x_res, self.P(f"{p}ln{norm}_g"), self.P(f"{p}ln{norm}_b"), out, sv["mean" + norm],
+                                   sv["rstd" + norm], self.ln_eps)
+
     def _block_fwd(self, i, x_in, x_out, sv, B, S=None):
-        """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x)).
+        """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x)); with the
+        sandwich LayerNorm x += LNa(drop(attn(LN1 x))); x += LNm(drop(mlp(LN2 x))).
         S: sequence length of the rows (default the model's; prefill runs a shorter prompt)."""
         p = f"l{i}."
         self._layernorm_fwd(x_in, p, 1, sv, S or self.S)
@@ -824,8 +891,8 @@ class DalleEngine:
         ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
                      dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
                      **self.conv_kw[i])  # :257-299
-        ops.linear_fwd(sv["attn"], self.W(p + "wo"), sv["xmid"], bias=self.P(p + "o_b"), residual=x_in,
-                       dropout=self._site("attn_out", i))                               # :303-314,330
+        self._branch_out(p, "a", sv["attn"], self.W(p + "wo"), self.P(p + "o_b"), x_in, sv["xmid"],
+                         self._site("attn_out", i), sv)                         # :303-314,330
         self._layernorm_fwd(sv["xmid"], p, 2, sv, S or self.S)
         if self.gated_mlp:   # h1 = zv * act(zg), z1 = [zv | zg] = LN2 W1 + b1 kept for backward (prefill: not written)
             ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), glu=self.glu,
@@ -835,8 +902,8 @@ class DalleEngine:
                            z_out=sv.get("z1"))
         else:
             ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), relu=True)     # :320
-        ops.linear_fwd(sv["h1"], self.W(p + "w2"), x_out, bias=self.P(p + "b2"), residual=sv["xmid"],
-                       dropout=self._site("mlp_out", i))                                # :321-323,333
+        self._branch_out(p, "m", sv["h1"], self.W(p + "w2"), self.P(p + "b2"), sv["xmid"], x_out,
+                         self._site("mlp_out", i), sv)                          # :321-323,333
 
     def ce_weights(self, global_batch):
         """lib.CeWeights of the weighted loss for a step over `global_batch` sequences (all ranks and micro-batches)."""
@@ -996,7 +1063,10 @@ class DalleEngine:
                    "attn": e(T, d), "lse": e(B, self.H, P, dtype=F32), "xmid": e(T, d), "ln2": e(T, d),
                    "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32), "h1": e(T, 4 * d),
                    # token shift: both unshifted LayerNorm outputs stay until the layer's caches are filled
-                   **({"ln1_raw": e(T, d), "ln2_raw": e(T, d)} if self.shift_tokens else {})},
+                   **({"ln1_raw": e(T, d), "ln2_raw": e(T, d)} if self.shift_tokens else {}),
+                   # sandwich LayerNorm: the branch outputs and their LayerNorms' statistics
+                   **({"oa": e(T, d), "om": e(T, d), "meana": e(T, dtype=F32), "rstda": e(T, dtype=F32),
+                       "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)} if self.sandwich_norm else {})},
             "x_last": e(B * rep, d), "hf": e(B * rep, d), "meanf": e(B * rep, dtype=F32),
             "rstdf": e(B * rep, dtype=F32), "logits": e(B * rep, self.Vpad, dtype=F32),
         }
@@ -1072,8 +1142,17 @@ class DalleEngine:
         kernel that WRITES that gradient (LayerNorm-backward / ReLU-mask epilogue) instead of separate passes:
         db2 (= colsum of this block's output gradient) was already accumulated by whoever produced dx_out.
         dbranch: gradient of the MLP output before its residual dropout (dx_out itself without dropout).  Returns the
-        same for the layer below."""
+        same for the layer below.
+
+        Sandwich LayerNorm: the branch gradients are the backward of LNm on dx_out and of LNa on dx_mid (without a
+        residual term, their dropout and the b2 / o_b column sums fused), so dbranch and dxsum_below are None and the
+        LayerNorms that produce dx_mid and dx_in fuse neither.  dx_in may be dx_out's storage: LNa's gradient goes
+        there once dx_out is consumed, and LN1's backward overwrites it last."""
         p = f"l{i}."
+        sand = self.sandwich_norm
+        if sand:   # d om = LNm'(dx_out); dbranch = d om * keep * scale, db2 = colsum(dbranch)
+            dbranch = self._ln_bwd(dx_out, sv["om"], self.P(p + "lnm_g"), sv["meanm"], sv["rstdm"], None, bufs["dtmp"],
+                                   self.G(p + "lnm_g"), self.G(p + "lnm_b"), self.G(p + "b2"), self._site("mlp_out", i))
         # ---- MLP
         dz = bufs["dz1"] if self.gated_mlp else bufs["dh1"]   # the gradient of W1's output
         if self.gated_mlp:   # dh = dx W2^T -> dz1 = [dh a | dh act'(zg) zv]; db1 = colsum(dz1)
@@ -1089,8 +1168,11 @@ class DalleEngine:
         dln = self._shift_bwd(bufs["dtmp"], sv["ln2_raw"]) if self.shift_tokens else bufs["dtmp"]
         dx_mid = bufs["dx_b"] if dx_out is bufs["dx_a"] else bufs["dx_a"]
         da = self._ln_bwd(dln, sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
-                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), self.G(p + "o_b"),
-                          self._site("attn_out", i))                                    # do_b = colsum(da)
+                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), None if sand else self.G(p + "o_b"),
+                          None if sand else self._site("attn_out", i))                  # do_b = colsum(da)
+        if sand:   # d oa = LNa'(dx_mid); da = d oa * keep * scale, do_b = colsum(da)
+            da = self._ln_bwd(dx_mid, sv["oa"], self.P(p + "lna_g"), sv["meana"], sv["rstda"], None, dx_in,
+                              self.G(p + "lna_g"), self.G(p + "lna_b"), self.G(p + "o_b"), self._site("attn_out", i))
         # ---- attention
         ops.linear_dgrad(da, self.W(p + "wo"), bufs["dtmp"])                                  # d(attn out)
         ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
@@ -1104,7 +1186,7 @@ class DalleEngine:
         dln = self._shift_bwd(bufs["dtmp"], sv["ln1_raw"]) if self.shift_tokens else bufs["dtmp"]
         return self._ln_bwd(dln, x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
                             self.G(p + "ln1_g"), self.G(p + "ln1_b"), dxsum_below,
-                            self._site("mlp_out", i - 1) if i > 0 else None)          # db2 of the layer below
+                            self._site("mlp_out", i - 1) if i > 0 and not sand else None)   # db2 of the layer below
 
     def backward(self, grad_scale, on_bucket_ready=None):
         """Back-propagates d(sum(loss_rows) * grad_scale); with the weighted loss d(sum_t a_t loss_rows[t] * grad_scale)
@@ -1128,9 +1210,10 @@ class DalleEngine:
             ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
             ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
         dx = bufs["dx_a"]
+        sand = self.sandwich_norm   # the sandwich LayerNorm's backward fuses db2 and the mlp_out dropout instead
         dbranch = self._ln_bwd(bufs["dtmp"], bufs["xs"][self.L], self.P("lnf_g"), bufs["meanf"], bufs["rstdf"], None,
-                               dx, self.G("lnf_g"), self.G("lnf_b"), self.G(f"l{self.L - 1}.b2"),
-                               self._site("mlp_out", self.L - 1))                          # db2 of the last block
+                               dx, self.G("lnf_g"), self.G("lnf_b"), None if sand else self.G(f"l{self.L - 1}.b2"),
+                               None if sand else self._site("mlp_out", self.L - 1))     # db2 of the last block
         if on_bucket_ready:
             s, e = self.layout.span("lnf_g", "bout")
             on_bucket_ready(s, e + 64)  # + the aux scalars (loss) that sit behind the last parameter
@@ -1143,9 +1226,9 @@ class DalleEngine:
             # dx (grad w.r.t. the block output) is dead once dx_mid has been formed in the other buffer, so the
             # block's input gradient is written back into the same storage.
             dbranch = self._block_bwd(i, bufs["xs"][i], sv, dx, dx, bufs, B,
-                                      self.G(f"l{i - 1}.b2") if i > 0 else None, dbranch)
+                                      self.G(f"l{i - 1}.b2") if i > 0 and not sand else None, dbranch)
             if on_bucket_ready:
-                s, e = self.layout.span(f"l{i}.ln1_g", f"l{i}.b2")
+                s, e = self.layout.span(f"l{i}.ln1_g", f"l{i}.lnm_b" if sand else f"l{i}.b2")
                 on_bucket_ready(s, e)
         # row / column positions: the gradient of the composed table goes into a zeroed scratch, then is folded into
         # wpe, image_row and image_col (one fully formed contribution per call, like the wpe gradient itself)

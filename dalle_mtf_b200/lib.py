@@ -118,6 +118,7 @@ _SIGNATURES = {
     "db200_pos_fold": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_shift_labels": [c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_layernorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
+    "db200_layernorm_residual_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
     "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
     "db200_layernorm_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp,
                                c_i64],

@@ -16,7 +16,7 @@ from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
     validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
-    validate_rotary, validate_shift_tokens
+    validate_rotary, validate_sandwich_norm, validate_shift_tokens
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -165,6 +165,19 @@ def gated_mlp(params):
     return v
 
 
+def sandwich_norm(params):
+    """sandwich_norm of a DALL-E config: absent, null or false is off; true normalises each branch output before its
+    residual add with a LayerNorm of its own (CogView's Sandwich-LN, DalleEngine), which adds the variables
+    layer_i/attn/norm_out/{g,b} and layer_i/mlp/norm_out/{g,b}.  Only a JSON bool is accepted: 1, "true" or a list is
+    rejected."""
+    v = params.get("sandwich_norm")
+    if v is None:
+        return False
+    if not isinstance(v, bool):
+        raise ValueError(f"sandwich_norm = {v!r}: expected null, true or false")
+    return validate_sandwich_norm(v)
+
+
 def shift_tokens(params, image_seq_len=None):
     """shift_tokens of a DALL-E config: absent, null or false is off; true turns on DALLE-pytorch's token shift after
     both LayerNorms of every layer (DalleEngine), which needs a square image-token grid (checked here when
@@ -271,6 +284,7 @@ def dalle_model_fn(features, labels, mode, params):
     activation = activation_function(params)
     gated = gated_mlp(params)
     shift = shift_tokens(params)
+    sandwich = sandwich_norm(params)
     mask = logits_mask(params)
     rotary_dim, rotary_base = rotary_embedding(params)
     L.require_device()
@@ -307,7 +321,7 @@ def dalle_model_fn(features, labels, mode, params):
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
                         activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
-                        gated_mlp=gated, shift_tokens=shift)
+                        gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

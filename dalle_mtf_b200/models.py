@@ -7,7 +7,8 @@ import torch
 from . import lib as L
 from .dalle_engine import DalleEngine
 from .model_fns import activation_function, attention_layers, conv_kernel, dropout_rates, gated_mlp, \
-    input_embedding, logits_mask, loss_weights, rotary_embedding, shift_tokens, validate_kl_weight
+    input_embedding, logits_mask, loss_weights, rotary_embedding, sandwich_norm, shift_tokens, \
+    validate_kl_weight
 from .model_fns import build_vae_engine, vae_architecture
 from .model_fns import reconstruction_loss as _reconstruction_loss
 
@@ -31,6 +32,7 @@ class DALLE:
         activation = activation_function(params)
         gated = gated_mlp(params)
         shift = shift_tokens(params, image_seq_len)
+        sandwich = sandwich_norm(params)
         mask = logits_mask(params)
         rotary_dim, rotary_base = rotary_embedding(params, n_embd, n_heads)
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
@@ -48,7 +50,8 @@ class DALLE:
                                   conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                                   image_position_embedding=pos_scheme, per_position_padding=per_pos,
                                   activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
-                                  rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift)
+                                  rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift,
+                                  sandwich_norm=sandwich)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

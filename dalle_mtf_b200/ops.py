@@ -374,6 +374,21 @@ def layernorm_fwd(x, g, b, y, mean, rstd, eps=1e-5):
     return y
 
 
+def layernorm_residual_fwd(o, x_res, g, b, y, mean, rstd, eps=1e-5):
+    """Sandwich LayerNorm: y = bf16(x_res + LN(o) * g + b) with LN's statistics of o into mean / rstd (fp32)."""
+    L.require_device()
+    _chk(o, BF16, "o"); _chk(x_res, BF16, "x_res"); _chk(y, BF16, "y"); _chk(g, F32, "g"); _chk(b, F32, "b")
+    _chk(mean, F32, "mean"); _chk(rstd, F32, "rstd")
+    rows, d = o.shape
+    if tuple(x_res.shape) != (rows, d) or tuple(y.shape) != (rows, d) or mean.numel() < rows or rstd.numel() < rows \
+            or g.numel() != d or b.numel() != d:
+        raise L.DB200Error(f"layernorm_residual_fwd: o, x_res and y must be [{rows}, {d}], g and b [{d}], mean and "
+                           f"rstd >= {rows} entries")
+    check(L.load().db200_layernorm_residual_fwd(stream_ptr(), ptr(o), ptr(x_res), ptr(g), ptr(b), ptr(y), ptr(mean),
+                                                ptr(rstd), rows, d, eps), "layernorm_residual_fwd")
+    return y
+
+
 def layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=None, dxm=None, dropout=None):
     """dxsum (optional, f32 [d]): += column sums of the produced dx (fused bias gradient of the layer below).
     dxm (with `dropout`, the residual-dropout site of the branch below): also writes dxm = dx * keep * scale, and dxsum

@@ -14,7 +14,8 @@ parameters and the same kernels' numerics as training:
                     act = ReLU, or GELU without a pre-activation output); with rotary embeddings q and k are
                     rotated to position p (rope_decode) before k enters the cache; with the token shift each
                     LayerNorm output's first d/2 columns enter a per-layer cache and are replaced by the shifted
-                    chunks of positions p - 1 and p - W (shift_tokens_decode)
+                    chunks of positions p - 1 and p - W (shift_tokens_decode); with the sandwich LayerNorm each
+                    branch output is normalised before its residual add (layernorm_residual_fwd)
   logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
 
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
@@ -90,10 +91,21 @@ class DalleSampler:
         self.att = mk(B, d)
         self.xmid = mk(B, d)
         self.h1 = mk(B, 4 * d)
+        self.ob = mk(B, d) if e.sandwich_norm else None   # sandwich LayerNorm: a branch output before its LayerNorm
         self.mean, self.rstd = mk(B, dtype=F32), mk(B, dtype=F32)
         self.logit = mk(B, e.Vpad, dtype=F32)
         self.tok = mk(B, dtype=I32)
         self._B = B
+
+    def _branch_out(self, p, norm, x, w, bias, x_res, out):
+        """out = x_res + x w + bias, or with the sandwich LayerNorm out = x_res + LN<norm>(x w + bias) (norm "a": the
+        attention branch's LayerNorm, "m": the MLP's)."""
+        e = self.e
+        if not e.sandwich_norm:
+            return ops.linear_fwd(x, w, out, bias=bias, residual=x_res)
+        ops.linear_fwd(x, w, self.ob, bias=bias)
+        ops.layernorm_residual_fwd(self.ob, x_res, e.P(f"{p}ln{norm}_g"), e.P(f"{p}ln{norm}_b"), out, self.mean,
+                                   self.rstd, e.ln_eps)
 
     def step(self, tokens_b, pos):
         """One position for every row: tokens_b int32 [B] -> fp32 logits [B, Vpad] of the NEXT position."""
@@ -110,12 +122,12 @@ class DalleSampler:
                 ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
             ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
                             **e.axial_kw[i], **e.conv_kw[i])
-            ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
+            self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
                 ops.shift_tokens_decode(self.ln, self.sc[2 * i + 1], pos, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
-            ops.linear_fwd(self.h1, e.W(p + "w2"), x_out, bias=e.P(p + "b2"), residual=self.xmid)
+            self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
         ops.layernorm_fwd(x_in, e.P("lnf_g"), e.P("lnf_b"), self.ln, self.mean, self.rstd, e.ln_eps)
         B = tokens_b.shape[0]
@@ -138,12 +150,12 @@ class DalleSampler:
                 ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
             ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
                                 radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
-            ops.linear_fwd(self.att, e.W(p + "wo"), self.xmid, bias=e.P(p + "o_b"), residual=x_in)
+            self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
                 ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i + 1], self.pos_dev, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
-            ops.linear_fwd(self.h1, e.W(p + "w2"), x_out, bias=e.P(p + "b2"), residual=self.xmid)
+            self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
         ops.layernorm_fwd(x_in, e.P("lnf_g"), e.P("lnf_b"), self.ln, self.mean, self.rstd, e.ln_eps)
         ops.gemm(self.ln, e.W("wout"), self.logit, tokens.shape[0], e.Vpad, e.d, a_mn=False, b_mn=True, bias=e.P("bout"))

@@ -19,7 +19,7 @@ import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
 from dalle_mtf_b200.model_fns import activation_function, attention_layers, conv_kernel, gated_mlp, \
-    input_embedding, logits_mask, rotary_embedding, shift_tokens, vae_checkpoint, vae_grid_size
+    input_embedding, logits_mask, rotary_embedding, sandwich_norm, shift_tokens, vae_checkpoint, vae_grid_size
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
 PADDING_ID = 50257   # GPT-2 vocabulary + <|padding|> (src/data/tokenizer_utils.py), what training pads captions with
@@ -156,6 +156,7 @@ def main(argv=None):
     activation = activation_function(params)           # and its MLP nonlinearity
     gated = gated_mlp(params)                           # and whether that MLP is gated
     shift = shift_tokens(params)                        # and whether its LayerNorm outputs are token-shifted
+    sandwich = sandwich_norm(params)                    # and whether its branch outputs are normalised
     mask = logits_mask(params)                         # and its objective (sampling draws image ids either way)
     rotary_dim, rotary_base = rotary_embedding(params)  # and its rotary position embeddings
     # with per-position padding the captions are padded with the config's padding_id, which the sampler maps to the
@@ -197,7 +198,7 @@ def main(argv=None):
                       device=device, attention_types=attention_types, local_attention_radius=local_radius,
                       conv_attention_kernel=conv_k, image_position_embedding=pos_scheme,
                       per_position_padding=per_pos, activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
-                      rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift)
+                      rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})

@@ -150,6 +150,13 @@ int db200_layernorm_bwd_ex(db200_stream_t stream, const void* dy_bf16, const voi
                            float* dg, float* db, float* dxsum_or_null, int rows, int d, void* workspace,
                            int64_t workspace_bytes);
 int64_t db200_layernorm_bwd_workspace_bytes(int rows, int d);
+/* sandwich LayerNorm (CogView's Sandwich-LN): the branch output o is normalised and added to the residual stream x,
+ *     y = bf16(x + (o - mean) * rstd * g + b)            (fp32, one rounding; the normalised o is never rounded alone)
+ * mean / rstd of o are computed by the same instructions as db200_layernorm_fwd's, so they are bit-identical to it on
+ * the same o.  Same d as db200_layernorm_fwd, any rows > 0.  Backward: db200_layernorm_bwd(_dropout) on o with
+ * dres = NULL (the residual's gradient is dy itself). */
+int db200_layernorm_residual_fwd(db200_stream_t stream, const void* o_bf16, const void* x_res_bf16, const float* g,
+                                 const float* b, void* y_bf16, float* mean, float* rstd, int rows, int d, float eps);
 /* backward of LayerNorm whose input x = r + dropout(branch): also writes dxm = dx * keep * scale (the gradient of the
  * branch output before its residual dropout, elementwise mask of `drop` over [rows][d]) and dxsum[c] += sum_rows dxm */
 int db200_layernorm_bwd_dropout(db200_stream_t stream, const void* dy_bf16, const void* x_bf16, const float* g,

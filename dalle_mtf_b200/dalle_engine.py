@@ -61,13 +61,15 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
-def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False):
+def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False, mlp_layers=None):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
     length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
     column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
     the grid_w rows and columns of the image-token grid.  gated_mlp: w1 is [d, 8d] and b1 [8d], the value columns
     first and the gate columns second.  sandwich_norm: each layer ends with its two output LayerNorms, lna_g / lna_b
-    (attention branch) and lnm_g / lnm_b (MLP branch), inside the layer's span l{i}.ln1_g .. layer_last(i)."""
+    (attention branch) and lnm_g / lnm_b (MLP branch), inside the layer's span l{i}.ln1_g .. layer_last(i).
+    mlp_layers: per layer, True for a gMLP token-mixing layer, whose gm_win [d, 4d], gm_bin [4d], sgu_g / sgu_b [2d],
+    sgu_w [S, S], sgu_c [S], gm_wout [2d, d] and gm_bout [d] take the place of wqkv, wo and o_b."""
     w1_cols = 8 * d if gated_mlp else 4 * d
     Vpad = _round_up(V, 64)
     lay = ParamLayout()
@@ -80,8 +82,14 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     for i in range(n_layers):
         p = f"l{i}."
         lay.add(p + "ln1_g", (d,)); lay.add(p + "ln1_b", (d,))
-        lay.add(p + "wqkv", (d, 3 * d))
-        lay.add(p + "wo", (d, d)); lay.add(p + "o_b", (d,))
+        if mlp_layers is not None and mlp_layers[i]:
+            lay.add(p + "gm_win", (d, 4 * d)); lay.add(p + "gm_bin", (4 * d,))
+            lay.add(p + "sgu_g", (2 * d,)); lay.add(p + "sgu_b", (2 * d,))
+            lay.add(p + "sgu_w", (S, S)); lay.add(p + "sgu_c", (S,))
+            lay.add(p + "gm_wout", (2 * d, d)); lay.add(p + "gm_bout", (d,))
+        else:
+            lay.add(p + "wqkv", (d, 3 * d))
+            lay.add(p + "wo", (d, d)); lay.add(p + "o_b", (d,))
         lay.add(p + "ln2_g", (d,)); lay.add(p + "ln2_b", (d,))
         lay.add(p + "w1", (d, w1_cols)); lay.add(p + "b1", (w1_cols,))
         lay.add(p + "w2", (4 * d, d)); lay.add(p + "b2", (d,))
@@ -93,7 +101,7 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     return lay
 
 
-ATTENTION_TYPES = ("global", "local", "axial_row", "axial_col", "conv")
+ATTENTION_TYPES = ("global", "local", "axial_row", "axial_col", "conv", "mlp")
 AXIAL_AXIS = {"axial_row": 0, "axial_col": 1}
 
 
@@ -109,6 +117,23 @@ def layer_radii(attention_types, radius, n_layers):
         raise ValueError(f"attention_types must list one of {ATTENTION_TYPES} for each of the {n_layers} layers, got "
                          f"{attention_types!r}")
     return [int(radius) if t == "local" else None for t in types]
+
+
+def layer_mlp(attention_types, n_layers, seq_len, n_embd):
+    """Per-layer flag of the gMLP token-mixing layers ("mlp"), refusing a geometry their kernels cannot run: the
+    sequence length must be a multiple of 64 (tile-aligned per-sequence rows for TMA) and 2 n_embd, the width of the
+    spatial gating unit's LayerNorm, one of LAYERNORM_WIDTHS."""
+    if attention_types is None:
+        return [False] * n_layers
+    flags = [t == "mlp" for t in attention_types]
+    if any(flags):
+        if seq_len % 64:
+            raise L.DB200Error(f"attention_types 'mlp': text_seq_len + image_seq_len = {seq_len} must be a multiple of "
+                               "64")
+        if 2 * n_embd not in LAYERNORM_WIDTHS:
+            raise L.DB200Error(f"attention_types 'mlp': n_embd {n_embd} gives a spatial gating unit of width "
+                               f"{2 * n_embd}, which the LayerNorm kernels do not implement (one of {LAYERNORM_WIDTHS})")
+    return flags
 
 
 def layer_axial(attention_types, text_seq_len, image_seq_len, n_layers):
@@ -325,11 +350,12 @@ class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lna_g", "lna_b", "lnm_g", "lnm_b", "lnf_g",
-                     "lnf_b", "bout")
+                     "lnf_b", "bout", "gm_bin", "sgu_g", "sgu_b", "sgu_c", "gm_bout")
     conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
     gated_mlp = False   # the gated MLP (validate_gated_mlp), set by the constructor
     shift_tokens = False   # the token shift (validate_shift_tokens), set by the constructor
     sandwich_norm = False   # the sandwich LayerNorm (validate_sandwich_norm), set by the constructor
+    mlp = ()   # per-layer flags of the gMLP token-mixing layers (layer_mlp), set by the constructor; () none
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
@@ -408,7 +434,16 @@ class DalleEngine:
         normalised by its own LayerNorm before the residual add: xmid = x + LNa(oa), xout = xmid + LNm(om), one
         rounding each (ops.layernorm_residual_fwd); LNa / LNm are the parameters lna_g / lna_b and lnm_g / lnm_b
         (layer_i/attn/norm_out and layer_i/mlp/norm_out), g = 1 and b = 0 at initialisation, not weight-decayed.  oa,
-        om and their statistics are kept per saved layer (two bf16 [T, d] and four fp32 [T])."""
+        om and their statistics are kept per saved layer (two bf16 [T, d] and four fp32 [T]).
+
+        An "mlp" entry of attention_types makes that layer a gMLP block (DALLE-pytorch's gMLPBlock with dim_ff = 4d,
+        causal, one head) in place of attention: u = gelu(LN1(x) W_in + b_in) (bf16, mtf's tanh GELU; the GELU
+        epilogue keeps z), res, gate = u[:, :2d], u[:, 2d:], gn = bf16(LN_sgu(gate)), mixed_i = sum_{j <= i} W_sgu[i, j]
+        gn_j + c_sgu[i] in fp32 per sequence, h = bf16(mixed res), and x += drop(h W_out + b_out) (with the sandwich
+        LayerNorm, LNa of it).  W_sgu [S, S] is lower triangular: its strict upper triangle starts, and stays, exactly
+        0 (its gradient there is never written) and a checkpoint with a non-zero one is refused.  Rotary embeddings and
+        attention dropout do not apply to the layer; residual dropout does.  Kept per saved layer: res, gate, their z,
+        gn, mixed and h (seven bf16 [T, 2d]) and the SGU LayerNorm's statistics."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
@@ -461,6 +496,8 @@ class DalleEngine:
         # per layer: None or the (text_len, grid_w, kernel) of a conv layer, and the attention ops' keyword for it
         self.conv = layer_conv(attention_types, text_seq_len, image_seq_len, conv_attention_kernel, n_layers)
         self.conv_kw = [{} if c is None else {"conv": c} for c in self.conv]
+        # per layer: True for a gMLP token-mixing layer
+        self.mlp = layer_mlp(attention_types, n_layers, self.S, n_embd)
         lw = (None, None) if loss_weights is None else tuple(loss_weights)
         self.loss_weights, self.z_loss = validate_loss_weights(*lw, z_loss)
         self.weighted_loss = self.loss_weights is not None or self.z_loss > 0
@@ -468,9 +505,11 @@ class DalleEngine:
                                      # (text block, image block) pair)
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
+        mlp_layers = self.mlp if any(self.mlp) else None
         self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, gated_mlp=self.gated_mlp,
-                                         sandwich_norm=self.sandwich_norm) \
-            if self.row_col else param_layout(d, Lyr, V, S, gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm)
+                                         sandwich_norm=self.sandwich_norm, mlp_layers=mlp_layers) \
+            if self.row_col else param_layout(d, Lyr, V, S, gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm,
+                                              mlp_layers=mlp_layers)
         self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
@@ -563,8 +602,11 @@ class DalleEngine:
         n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else S
         gate = (4 * d * d + 4 * d) if self.gated_mlp else 0   # the gate half of W1 and b1
         sandwich = 4 * d if self.sandwich_norm else 0         # LNa and LNm: g and b each
+        n_mlp = sum(self.mlp)
+        # a gMLP layer: W_in + b_in, the SGU norm, W_sgu + c_sgu and W_out + b_out in place of q, k, v, o and o_b
+        gmlp = 4 * d * d + 4 * d + 4 * d + S * S + S + 2 * d * d + d - (4 * d * d + d)
         return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d +
-                                          gate + sandwich) + 2 * d + d * V + V
+                                          gate + sandwich) + n_mlp * gmlp + 2 * d + d * V + V
 
     EMBED_REF_NAMES = {"wte": "embedding/wte", "wpe": "positional_embedding/wpe",
                        "image_row": "positional_embedding/image_row", "image_col": "positional_embedding/image_col"}
@@ -573,8 +615,12 @@ class DalleEngine:
         """Reference-style variable name of an embedding parameter (other names are returned unchanged)."""
         return self.EMBED_REF_NAMES.get(name, name)
 
+    GMLP_REF_NAMES = {"gm_win": "gmlp/proj_in/kernel", "gm_bin": "gmlp/proj_in/bias", "sgu_g": "gmlp/sgu/norm/g",
+                      "sgu_b": "gmlp/sgu/norm/b", "sgu_w": "gmlp/sgu/weight", "sgu_c": "gmlp/sgu/bias",
+                      "gm_wout": "gmlp/proj_out/kernel", "gm_bout": "gmlp/proj_out/bias"}
+
     @staticmethod
-    def _ref_names(i, sandwich_norm=False):
+    def _ref_names(i, sandwich_norm=False, mlp=False):
         pre = f"layer_{i}/"
         names = {
             "ln1_g": pre + "norm_1/g", "ln1_b": pre + "norm_1/b", "wo": pre + "attn/o",
@@ -582,14 +628,47 @@ class DalleEngine:
             "w1": pre + "mlp/mlp_linear_1/kernel", "b1": pre + "mlp/mlp_linear_1/bias",
             "w2": pre + "mlp/mlp_linear_2/kernel", "b2": pre + "mlp/mlp_linear_2/bias",
         }
+        if mlp:   # a gMLP layer: its token-mixing variables replace attn/o and o_b (and q, k, v)
+            del names["wo"], names["o_b"]
+            names.update({k: pre + v for k, v in DalleEngine.GMLP_REF_NAMES.items()})
         if sandwich_norm:
             names.update({"lna_g": pre + "attn/norm_out/g", "lna_b": pre + "attn/norm_out/b",
                           "lnm_g": pre + "mlp/norm_out/g", "lnm_b": pre + "mlp/norm_out/b"})
         return names
 
+    def _is_mlp(self, i):
+        """Whether layer i is a gMLP token-mixing layer."""
+        return bool(self.mlp) and self.mlp[i]
+
     def _layer_ref_names(self, i):
-        """Reference names of layer i's parameters other than q / k / v (with this engine's sandwich_norm)."""
-        return self._ref_names(i, self.sandwich_norm)
+        """Reference names of layer i's parameters other than q / k / v (with this engine's sandwich_norm and layer
+        kind)."""
+        return self._ref_names(i, self.sandwich_norm, self._is_mlp(i))
+
+    def _check_layer_kinds(self, named):
+        """Refuse a checkpoint whose layer kinds differ from this model's: an attention layer's variables where this
+        model has a gMLP layer, or the reverse; and a gMLP mixing weight whose strict upper triangle is not zero (the
+        layer's causality).  The error names the first such variable."""
+        for i in range(self.L):
+            pre = f"layer_{i}/"
+            if self._is_mlp(i):
+                for rn in [pre + "attn/q", pre + "attn/k", pre + "attn/v", pre + "attn/o"]:
+                    if rn in named:
+                        raise L.DB200Error(f"load_params: {rn}: an attention variable, but layer {i} of this model is "
+                                           "a gMLP ('mlp') layer")
+                for v in self.GMLP_REF_NAMES.values():
+                    if pre + v not in named:
+                        raise L.DB200Error(f"load_params: {pre + v}: missing from the checkpoint of a model whose layer "
+                                           f"{i} is a gMLP ('mlp') layer")
+                w = named[pre + "gmlp/sgu/weight"]
+                if tuple(w.shape) == (self.S, self.S) and bool(torch.triu(w, diagonal=1).ne(0).any()):
+                    raise L.DB200Error(f"load_params: {pre}gmlp/sgu/weight: the strict upper triangle of the causal "
+                                       "mixing weight must be exactly 0")
+            else:
+                extra = sorted(k for k in named if k.startswith(pre + "gmlp/"))
+                if extra:
+                    raise L.DB200Error(f"load_params: {extra[0]}: a gMLP variable, but layer {i} of this model is an "
+                                       "attention layer")
 
     def _check_sandwich_names(self, named):
         """Refuse a checkpoint of the other sandwich_norm kind: one without a sandwich LayerNorm this model has, or
@@ -638,6 +717,7 @@ class DalleEngine:
         """Fill one of the flat fp32 buffers (master | adam_m | adam_v) from a dict of reference-named tensors."""
         dev = self.device
         self._check_sandwich_names(named)
+        self._check_layer_kinds(named)
         if self.zero is not None:
             if flat is not self.master:
                 raise L.DB200Error("ZeRO-1 mode: loading sharded Adam slots is not implemented (throughput configuration)")
@@ -649,6 +729,8 @@ class DalleEngine:
                 p = f"l{i}."
                 for k, rn in self._layer_ref_names(i).items():
                     self._scatter_full(p + k, f32(named[rn]))
+                if self._is_mlp(i):
+                    continue
                 pre = f"layer_{i}/attn/"
                 self._scatter_full(p + "wqkv", torch.cat([f32(named[pre + "q"]), f32(named[pre + "k"]),
                                                           f32(named[pre + "v"])], dim=1))
@@ -676,6 +758,8 @@ class DalleEngine:
             ref = self._layer_ref_names(i)
             for k, rn in ref.items():
                 put(p + k, named[rn])
+            if self._is_mlp(i):
+                continue
             pre = f"layer_{i}/attn/"
             put(p + "wqkv", torch.cat([named[pre + "q"], named[pre + "k"], named[pre + "v"]], dim=1))
         put("lnf_g", named["to_logits/layer_norm/g"]); put("lnf_b", named["to_logits/layer_norm/b"])
@@ -698,6 +782,8 @@ class DalleEngine:
             p = f"l{i}."
             for k, rn in self._layer_ref_names(i).items():
                 out[rn] = view(p + k)
+            if self._is_mlp(i):
+                continue
             wqkv = view(p + "wqkv")
             pre = f"layer_{i}/attn/"
             out[pre + "q"], out[pre + "k"], out[pre + "v"] = wqkv[:, :d].clone(), wqkv[:, d:2 * d].clone(), \
@@ -729,15 +815,31 @@ class DalleEngine:
             self.P(p + "ln1_g").fill_(1.0); self.P(p + "ln2_g").fill_(1.0)
             if self.sandwich_norm:
                 self.P(p + "lna_g").fill_(1.0); self.P(p + "lnm_g").fill_(1.0)
-            wqkv = self.P(p + "wqkv")
-            wqkv[:, :d].copy_(torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5))
-            wqkv[:, d:].copy_(torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5))
-            normal(p + "wo", (H * dh) ** -0.5)
+            if self._is_mlp(i):
+                w_in, w_sgu, w_out = self._gmlp_init(g, 0.02 / math.sqrt(Lyr))
+                self.P(p + "gm_win").copy_(w_in); self.P(p + "sgu_w").copy_(w_sgu); self.P(p + "gm_wout").copy_(w_out)
+                self.P(p + "sgu_g").fill_(1.0); self.P(p + "sgu_c").fill_(1.0)
+            else:
+                wqkv = self.P(p + "wqkv")
+                wqkv[:, :d].copy_(torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5))
+                wqkv[:, d:].copy_(torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5))
+                normal(p + "wo", (H * dh) ** -0.5)
             normal(p + "w1", 0.02)
             normal(p + "w2", 0.02 / math.sqrt(Lyr))
         self.P("lnf_g").fill_(1.0)
         normal("wout", 0.02, cols=self.V)
         self.refresh_shadow()
+
+    def _gmlp_init(self, g, out_std):
+        """(W_in, W_sgu, W_out) of a gMLP layer from the generator g, in this order: W_in ~ N(0, 0.02), W_sgu ~
+        U(-1e-3 / S, 1e-3 / S) with the strict upper triangle exactly 0 (gMLP's initialisation, so that the block
+        starts near h = res with c_sgu = 1), W_out ~ N(0, out_std)."""
+        d, S, dev = self.d, self.S, self.device
+        w_in = torch.randn(d, 4 * d, generator=g, device=dev, dtype=F32) * 0.02
+        eps = 1e-3 / S
+        w_sgu = torch.tril((torch.rand(S, S, generator=g, device=dev, dtype=F32) * 2 - 1) * eps)
+        w_out = torch.randn(2 * d, d, generator=g, device=dev, dtype=F32) * out_std
+        return w_in, w_sgu, w_out
 
     def _init_params_sharded(self, g):
         """Same initialisers and the same random stream as init_params, one tensor at a time (ZeRO-1: no full fp32 buffer)."""
@@ -753,6 +855,14 @@ class DalleEngine:
             self._scatter_full(p + "ln1_g", ones(d)); self._scatter_full(p + "ln2_g", ones(d))
             if self.sandwich_norm:
                 self._scatter_full(p + "lna_g", ones(d)); self._scatter_full(p + "lnm_g", ones(d))
+            if self._is_mlp(i):
+                w_in, w_sgu, w_out = self._gmlp_init(g, 0.02 / math.sqrt(Lyr))
+                self._scatter_full(p + "gm_win", w_in); self._scatter_full(p + "sgu_w", w_sgu)
+                self._scatter_full(p + "gm_wout", w_out)
+                self._scatter_full(p + "sgu_g", ones(2 * d)); self._scatter_full(p + "sgu_c", ones(self.S))
+                self._scatter_full(p + "w1", rn(self.layout.entries[p + "w1"][1], 0.02))
+                self._scatter_full(p + "w2", rn((4 * d, d), 0.02 / math.sqrt(Lyr)))
+                continue
             wq = torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5)
             wkv = torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5)
             self._scatter_full(p + "wqkv", torch.cat([wq, wkv], dim=1))
@@ -795,15 +905,20 @@ class DalleEngine:
         # sandwich LayerNorm: both branch outputs and the statistics of their LayerNorms, for backward
         sand = (lambda: {"oa": e(T, d), "om": e(T, d), "meana": e(T, dtype=F32), "rstda": e(T, dtype=F32),
                          "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)}) if self.sandwich_norm else dict
+        # the token mixer's buffers of a saved layer: attention's, a gMLP layer's, or (recompute_grad's one slot) both
+        attn_slot = (lambda i: not all(self.mlp)) if self.recompute_grad else (lambda i: not self._is_mlp(i))
+        gmlp_slot = (lambda i: any(self.mlp)) if self.recompute_grad else (lambda i: self._is_mlp(i))
+        mixer = lambda i: {
+            **({"qkv": e(T, 3 * d), "attn": e(T, d), "lse": e(B, self.H, S, dtype=F32)} if attn_slot(i) else {}),
+            **(self._gmlp_bufs(T, e, train=True) if gmlp_slot(i) else {})}
         b = {
             "xs": [e(T, d) for _ in range(self.L + 1)],        # residual stream at every layer boundary
             "layers": [{
-                "ln1": e(T, d), "mean1": e(T, dtype=F32), "rstd1": e(T, dtype=F32),
-                "qkv": e(T, 3 * d), "attn": e(T, d), "lse": e(B, self.H, S, dtype=F32),
+                "ln1": e(T, d), "mean1": e(T, dtype=F32), "rstd1": e(T, dtype=F32), **mixer(i),
                 "xmid": e(T, d), "ln2": e(T, d), "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32),
                 "h1": e(T, 4 * d), **({"z1": e(T, 4 * d)} if self.gelu else {}),
                 **({"z1": e(T, 8 * d)} if self.gated_mlp else {}), **raw, **sand(),
-            } for _ in range(n_saved)],
+            } for i in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
             "labels": e(B, S, dtype=I32), "loss_rows": e(T, dtype=F32),
             # backward scratch
@@ -812,6 +927,8 @@ class DalleEngine:
         }
         if self.dropout[2] > 0:   # gradient of a branch output before its residual dropout
             b["dxm"] = e(T, d)
+        if any(self.mlp):         # gMLP backward: dh (then d gate), dmixed and dgn
+            b["g_dh"], b["g_dm"], b["g_dgn"] = e(T, 2 * d), e(T, 2 * d), e(T, 2 * d)
         if self.gated_mlp:        # [dzv | dzg], the gradient of z1
             b["dz1"] = e(T, 8 * d)
         if not self.logits_mask:
@@ -834,6 +951,16 @@ class DalleEngine:
         self._bufs, self._buf_key = b, key
         return b
 
+    def _gmlp_bufs(self, T, e, train):
+        """A gMLP layer's activations over T rows: res and gate (the two GELU halves of proj_in), gn = LN_sgu(gate) and
+        its statistics, h; training also keeps both pre-activations z and mixed for the backward."""
+        C = 2 * self.d
+        b = {"res": e(T, C), "gate": e(T, C), "gn": e(T, C), "meang": e(T, dtype=F32), "rstdg": e(T, dtype=F32),
+             "h": e(T, C)}
+        if train:
+            b.update({"zres": e(T, C), "zgate": e(T, C), "mixed": e(T, C)})
+        return b
+
     # ------------------------------------------------------------------------------------------ dropout
     def _dropout_descs(self, step, row0):
         """Descriptors of every dropout site for one forward of sequences [row0, row0 + B) of the global batch at
@@ -848,7 +975,7 @@ class DalleEngine:
             "wte": mk(emb, L.SITE_WTE, rows0), "wpe": mk(emb, L.SITE_WPE, 0),
             "attn": [mk(att, L.dropout_site_attn(i), row0)
                      if self.radii[i] is None and self.axial[i] is None and (self.conv is None or self.conv[i] is None)
-                     else None
+                     and not self._is_mlp(i) else None
                      for i in range(self.L)],
             "attn_out": [mk(res, L.dropout_site_attn_out(i), rows0) for i in range(self.L)],
             "mlp_out": [mk(res, L.dropout_site_mlp_out(i), rows0) for i in range(self.L)],
@@ -885,14 +1012,19 @@ class DalleEngine:
         S: sequence length of the rows (default the model's; prefill runs a shorter prompt)."""
         p = f"l{i}."
         self._layernorm_fwd(x_in, p, 1, sv, S or self.S)
-        ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                       # q|k|v, no bias (:242-244)
-        if self.rotary:
-            ops.rope_fwd(sv["qkv"], self.rope_table, S or self.S, self.H, self.dh, self.rotary_dim)
-        ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
-                     dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
-                     **self.conv_kw[i])  # :257-299
-        self._branch_out(p, "a", sv["attn"], self.W(p + "wo"), self.P(p + "o_b"), x_in, sv["xmid"],
-                         self._site("attn_out", i), sv)                         # :303-314,330
+        if self._is_mlp(i):   # gMLP token mixing in place of attention
+            self._gmlp_fwd(p, sv, B, S or self.S)
+            self._branch_out(p, "a", sv["h"], self.W(p + "gm_wout"), self.P(p + "gm_bout"), x_in, sv["xmid"],
+                             self._site("attn_out", i), sv)
+        else:
+            ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                   # q|k|v, no bias (:242-244)
+            if self.rotary:
+                ops.rope_fwd(sv["qkv"], self.rope_table, S or self.S, self.H, self.dh, self.rotary_dim)
+            ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
+                         dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
+                         **self.conv_kw[i])  # :257-299
+            self._branch_out(p, "a", sv["attn"], self.W(p + "wo"), self.P(p + "o_b"), x_in, sv["xmid"],
+                             self._site("attn_out", i), sv)                     # :303-314,330
         self._layernorm_fwd(sv["xmid"], p, 2, sv, S or self.S)
         if self.gated_mlp:   # h1 = zv * act(zg), z1 = [zv | zg] = LN2 W1 + b1 kept for backward (prefill: not written)
             ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), glu=self.glu,
@@ -904,6 +1036,18 @@ class DalleEngine:
             ops.linear_fwd(sv["ln2"], self.W(p + "w1"), sv["h1"], bias=self.P(p + "b1"), relu=True)     # :320
         self._branch_out(p, "m", sv["h1"], self.W(p + "w2"), self.P(p + "b2"), sv["xmid"], x_out,
                          self._site("mlp_out", i), sv)                          # :321-323,333
+
+    def _gmlp_fwd(self, p, sv, B, n):
+        """The token mixing of a gMLP layer over B sequences of n rows: res | gate = gelu(ln1 W_in + b_in) (two GELU
+        products, one per half, so that the gate is contiguous for its LayerNorm; z kept when sv has room for it),
+        gn = LN_sgu(gate), h = bf16((W_sgu gn + c_sgu) res) (mixed kept likewise)."""
+        C = 2 * self.d
+        w_in, b_in = self.W(p + "gm_win"), self.P(p + "gm_bin")
+        ops.linear_fwd(sv["ln1"], w_in[:, :C], sv["res"], bias=b_in[:C], gelu=True, z_out=sv.get("zres"))
+        ops.linear_fwd(sv["ln1"], w_in[:, C:], sv["gate"], bias=b_in[C:], gelu=True, z_out=sv.get("zgate"))
+        ops.layernorm_fwd(sv["gate"], self.P(p + "sgu_g"), self.P(p + "sgu_b"), sv["gn"], sv["meang"], sv["rstdg"],
+                          self.ln_eps)
+        ops.sgu_mix_fwd(self.W(p + "sgu_w"), sv["gn"], sv["res"], self.P(p + "sgu_c"), sv["h"], sv.get("mixed"), B, n)
 
     def ce_weights(self, global_batch):
         """lib.CeWeights of the weighted loss for a step over `global_batch` sequences (all ranks and micro-batches)."""
@@ -1066,7 +1210,9 @@ class DalleEngine:
                    **({"ln1_raw": e(T, d), "ln2_raw": e(T, d)} if self.shift_tokens else {}),
                    # sandwich LayerNorm: the branch outputs and their LayerNorms' statistics
                    **({"oa": e(T, d), "om": e(T, d), "meana": e(T, dtype=F32), "rstda": e(T, dtype=F32),
-                       "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)} if self.sandwich_norm else {})},
+                       "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)} if self.sandwich_norm else {}),
+                   # gMLP layers: their activations without what only a backward reads
+                   **(self._gmlp_bufs(T, e, train=False) if any(self.mlp) else {})},
             "x_last": e(B * rep, d), "hf": e(B * rep, d), "meanf": e(B * rep, dtype=F32),
             "rstdf": e(B * rep, dtype=F32), "logits": e(B * rep, self.Vpad, dtype=F32),
         }
@@ -1081,7 +1227,10 @@ class DalleEngine:
         pending backward() reads are left untouched.
 
         shift_caches (required with the token shift, else None): 2 L bf16 [B*rep, S, d/2] caches, layer i's LN1 at
-        2i and its LN2 at 2i + 1; positions < P receive the first d/2 columns of the unshifted LayerNorm outputs."""
+        2i and its LN2 at 2i + 1; positions < P receive the first d/2 columns of the unshifted LayerNorm outputs.
+
+        A gMLP layer i has no k / v: k_caches[i] is its bf16 [B*rep, S, 2d] cache of the SGU LayerNorm outputs gn
+        (positions < P filled, same replica order) and v_caches[i] is None."""
         B, P = tokens.shape
         if not 1 <= P < self.S:
             raise ValueError(f"prefill: prompt length {P} outside [1, {self.S})")
@@ -1089,9 +1238,13 @@ class DalleEngine:
             raise ValueError(f"prefill: rep must be an integer >= 1, got {rep!r}")
         rep = int(rep)
         shape = (B * rep, self.S, self.H, self.dh)
+        gshape = (B * rep, self.S, 2 * self.d)
         if len(k_caches) != self.L or len(v_caches) != self.L or \
-                any(tuple(c.shape) != shape for c in list(k_caches) + list(v_caches)):
-            raise ValueError(f"prefill: expected {self.L} k and v caches of shape {shape}")
+                any((tuple(k.shape) != gshape or v is not None) if m else
+                    (k is None or v is None or tuple(k.shape) != shape or tuple(v.shape) != shape)
+                    for k, v, m in zip(k_caches, v_caches, [self._is_mlp(i) for i in range(self.L)])):
+            raise ValueError(f"prefill: expected {self.L} k and v caches of shape {shape} (a gMLP layer: its SGU cache "
+                             f"{gshape} and None)")
         if self.shift_tokens:
             sshape = (B * rep, self.S, self.d // 2)
             if shift_caches is None or len(shift_caches) != 2 * self.L or \
@@ -1107,7 +1260,10 @@ class DalleEngine:
             x_in, x_out = b["xs"]
             for i in range(self.L):
                 self._block_fwd(i, x_in, x_out, b["sv"], B, S=P)
-                ops.kv_cache_fill(b["sv"]["qkv"], k_caches[i], v_caches[i], P, rep)
+                if self._is_mlp(i):
+                    ops.sgu_cache_fill(b["sv"]["gn"], k_caches[i], P, rep)
+                else:
+                    ops.kv_cache_fill(b["sv"]["qkv"], k_caches[i], v_caches[i], P, rep)
                 if self.shift_tokens:
                     ops.shift_cache_fill(b["sv"]["ln1_raw"], shift_caches[2 * i], P, rep)
                     ops.shift_cache_fill(b["sv"]["ln2_raw"], shift_caches[2 * i + 1], P, rep)
@@ -1150,6 +1306,7 @@ class DalleEngine:
         there once dx_out is consumed, and LN1's backward overwrites it last."""
         p = f"l{i}."
         sand = self.sandwich_norm
+        ob = p + ("gm_bout" if self._is_mlp(i) else "o_b")   # the token mixer's output bias
         if sand:   # d om = LNm'(dx_out); dbranch = d om * keep * scale, db2 = colsum(dbranch)
             dbranch = self._ln_bwd(dx_out, sv["om"], self.P(p + "lnm_g"), sv["meanm"], sv["rstdm"], None, bufs["dtmp"],
                                    self.G(p + "lnm_g"), self.G(p + "lnm_b"), self.G(p + "b2"), self._site("mlp_out", i))
@@ -1168,25 +1325,46 @@ class DalleEngine:
         dln = self._shift_bwd(bufs["dtmp"], sv["ln2_raw"]) if self.shift_tokens else bufs["dtmp"]
         dx_mid = bufs["dx_b"] if dx_out is bufs["dx_a"] else bufs["dx_a"]
         da = self._ln_bwd(dln, sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
-                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), None if sand else self.G(p + "o_b"),
+                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), None if sand else self.G(ob),
                           None if sand else self._site("attn_out", i))                  # do_b = colsum(da)
         if sand:   # d oa = LNa'(dx_mid); da = d oa * keep * scale, do_b = colsum(da)
             da = self._ln_bwd(dx_mid, sv["oa"], self.P(p + "lna_g"), sv["meana"], sv["rstda"], None, dx_in,
-                              self.G(p + "lna_g"), self.G(p + "lna_b"), self.G(p + "o_b"), self._site("attn_out", i))
-        # ---- attention
-        ops.linear_dgrad(da, self.W(p + "wo"), bufs["dtmp"])                                  # d(attn out)
-        ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
-        ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"], B,
-                     self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i), radius=self.radii[i],
-                     **self.axial_kw[i], **self.conv_kw[i])
-        if self.rotary:   # d(q|k|v) before the rotation
-            ops.rope_bwd(bufs["dqkv"], self.rope_table, self.S, self.H, self.dh, self.rotary_dim)
-        ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                      # dLN1 out
-        ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
+                              self.G(p + "lna_g"), self.G(p + "lna_b"), self.G(ob), self._site("attn_out", i))
+        if self._is_mlp(i):   # ---- gMLP token mixing
+            self._gmlp_bwd(p, sv, da, bufs, B)
+        else:             # ---- attention
+            ops.linear_dgrad(da, self.W(p + "wo"), bufs["dtmp"])                              # d(attn out)
+            ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
+            ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"],
+                         B, self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i),
+                         radius=self.radii[i], **self.axial_kw[i], **self.conv_kw[i])
+            if self.rotary:   # d(q|k|v) before the rotation
+                ops.rope_bwd(bufs["dqkv"], self.rope_table, self.S, self.H, self.dh, self.rotary_dim)
+            ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                  # dLN1 out
+            ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
         dln = self._shift_bwd(bufs["dtmp"], sv["ln1_raw"]) if self.shift_tokens else bufs["dtmp"]
         return self._ln_bwd(dln, x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
                             self.G(p + "ln1_g"), self.G(p + "ln1_b"), dxsum_below,
                             self._site("mlp_out", i - 1) if i > 0 and not sand else None)   # db2 of the layer below
+
+    def _gmlp_bwd(self, p, sv, da, bufs, B):
+        """Backward of a gMLP layer's token mixing from da, the gradient of the branch output before its bias: into
+        bufs["dtmp"] (the gradient of the LN1 output) and the layer's W_out, c_sgu, W_sgu, SGU norm, W_in and b_in
+        gradients.  du = [du_res | du_gate] is formed in bufs["dh1"] (free once the MLP branch is done)."""
+        C, S = 2 * self.d, self.S
+        dh, dm, dgn, du = bufs["g_dh"], bufs["g_dm"], bufs["g_dgn"], bufs["dh1"]
+        ops.linear_dgrad(da, self.W(p + "gm_wout"), dh)                                      # dh
+        ops.linear_wgrad(sv["h"], da, self.G(p + "gm_wout"))
+        # dmixed = dh res, du_res = dh mixed gelu'(z_res), dc_sgu
+        ops.sgu_bwd(dh, sv["mixed"], sv["res"], sv["zres"], dm, du[:, :C], self.G(p + "sgu_c"), B, S)
+        ops.sgu_mix_dgrad(self.W(p + "sgu_w"), dm, dgn, B, S)                                # dgn = W^T dmixed
+        ops.sgu_mix_wgrad(dm, sv["gn"], self.G(p + "sgu_w"), B, S)                           # dW (lower triangle)
+        ops.layernorm_bwd(dgn, sv["gate"], self.P(p + "sgu_g"), sv["meang"], sv["rstdg"], None, dh,
+                          self.G(p + "sgu_g"), self.G(p + "sgu_b"))                          # d gate (into dh)
+        ops.sgu_gate_bwd(dh, sv["zgate"], du[:, C:])                                        # du_gate
+        ops.colsum(du, self.G(p + "gm_bin"))                                                 # db_in
+        ops.linear_dgrad(du, self.W(p + "gm_win"), bufs["dtmp"])                             # dLN1 out
+        ops.linear_wgrad(sv["ln1"], du, self.G(p + "gm_win"))
 
     def backward(self, grad_scale, on_bucket_ready=None):
         """Back-propagates d(sum(loss_rows) * grad_scale); with the weighted loss d(sum_t a_t loss_rows[t] * grad_scale)
@@ -1261,7 +1439,7 @@ class DalleEngine:
         "norm" or "bias" (LayerNorm g/b, all biases incl. compute_output_bias/o_b) is left undecayed."""
         if getattr(self, "_segs", None) is None:
             decays = lambda n: n in ("wte", "wpe", "image_row", "image_col", "wout") or \
-                n.split(".")[-1] in ("wqkv", "wo", "w1", "w2")
+                n.split(".")[-1] in ("wqkv", "wo", "w1", "w2", "gm_win", "sgu_w", "gm_wout")
             segs = []
             for name in self.layout.order:
                 s, e = self.layout.span(name, name)

@@ -173,6 +173,14 @@ _SIGNATURES = {
     "db200_shift_tokens_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_shift_tokens_decode_dev": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
     "db200_shift_cache_fill": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_sgu_mix_fwd": [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int],
+    "db200_sgu_mix_dgrad": [c_vp, c_vp, c_i64, c_vp, c_vp, c_int, c_int, c_int],
+    "db200_sgu_mix_wgrad": [c_vp, c_vp, c_vp, c_vp, c_i64, c_int, c_int, c_int],
+    "db200_sgu_bwd": [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int],
+    "db200_sgu_gate_bwd": [c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_int, c_int],
+    "db200_sgu_decode": [c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
+    "db200_sgu_decode_dev": [c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_vp],
+    "db200_sgu_cache_fill": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_crc32c": [c_vp, c_u64, c_vp],
     "db200_tfrecord_masked_crc": [c_vp, c_u64, c_vp],
     "db200_tfrecord_frame": [c_vp, c_u64, c_vp],

@@ -1189,3 +1189,135 @@ def onehot_rows(idx, y, offset=0):
     rows, K = y.shape
     check(L.load().db200_onehot_rows_f32(stream_ptr(), ptr(idx), ptr(y), rows, K, int(offset)), "db200_onehot_rows_f32")
     return y
+
+
+# ----------------------------------------------------------------------------------------------- gMLP token mixing
+def _sgu_act(t, what, C=None):
+    """(rows, C) of a bf16 [rows, C] operand of the SGU kernels (rows may be strided, channels contiguous)."""
+    L.require_device()
+    _chk(t, BF16, what)
+    if t.dim() != 2 or (C is not None and t.shape[1] != C):
+        raise L.DB200Error(f"{what}: expected a [rows, {C if C is not None else 'C'}] tensor, got {tuple(t.shape)}")
+    return t.shape
+
+
+def _sgu_weight(w, n, what):
+    _chk(w, BF16, what)
+    if w.dim() != 2 or w.shape[0] < n or w.shape[1] < n:
+        raise L.DB200Error(f"{what}: expected a [>= {n}, >= {n}] mixing weight, got {tuple(w.shape)}")
+
+
+def sgu_mix_fwd(w, gn, res, c, h, mixed, B, n):
+    """The SGU's token mixing over B sequences of n positions (include/dalle_b200.h): m = W[:n, :n] gn_b + c[i] in
+    fp32, h = bf16(m * res), mixed = bf16(m) (or None).  gn, h, mixed contiguous bf16 [B n, C]; res [B n, C] with any
+    row pitch (the first half of the proj_in output); w the bf16 weight, read through its pitch; c fp32 [>= n]."""
+    rows, C = _sgu_act(gn, "gn")
+    _sgu_act(res, "res", C); _sgu_act(h, "h", C); _chk(c, F32, "c")
+    if mixed is not None:
+        _sgu_act(mixed, "mixed", C)
+    _sgu_weight(w, n, "w")
+    if rows != B * n or not gn.is_contiguous() or not h.is_contiguous() or res.shape[0] != rows or \
+            h.shape[0] != rows or (mixed is not None and (not mixed.is_contiguous() or mixed.shape[0] != rows)) or \
+            c.numel() < n:
+        raise L.DB200Error(f"sgu_mix_fwd: gn, h, mixed must be contiguous [{B * n}, {C}], res [{B * n}, {C}], c >= {n}")
+    check(L.load().db200_sgu_mix_fwd(stream_ptr(), ptr(w), w.stride(0), ptr(gn), ptr(res), res.stride(0), ptr(c),
+                                     ptr(h), ptr(mixed), B, n, C), "db200_sgu_mix_fwd")
+    return h
+
+
+def sgu_mix_dgrad(w, dmixed, dgn, B, n):
+    """dgn_b = W[:n, :n]^T dmixed_b (bf16 [B n, C] contiguous)."""
+    rows, C = _sgu_act(dmixed, "dmixed")
+    _sgu_act(dgn, "dgn", C)
+    _sgu_weight(w, n, "w")
+    if rows != B * n or dgn.shape[0] != rows or not dmixed.is_contiguous() or not dgn.is_contiguous():
+        raise L.DB200Error(f"sgu_mix_dgrad: dmixed and dgn must be contiguous [{B * n}, {C}]")
+    check(L.load().db200_sgu_mix_dgrad(stream_ptr(), ptr(w), w.stride(0), ptr(dmixed), ptr(dgn), B, n, C),
+          "db200_sgu_mix_dgrad")
+    return dgn
+
+
+def sgu_mix_wgrad(dmixed, gn, dw, B, n):
+    """dw[i, j] (fp32 [n, n] view, any row pitch) += sum_b sum_c dmixed_b[i, c] gn_b[j, c] for j <= i; the strict upper
+    triangle is never written."""
+    rows, C = _sgu_act(dmixed, "dmixed")
+    _sgu_act(gn, "gn", C)
+    _chk(dw, F32, "dw")
+    if rows != B * n or gn.shape[0] != rows or not dmixed.is_contiguous() or not gn.is_contiguous() or \
+            dw.dim() != 2 or dw.shape[0] < n or dw.shape[1] < n:
+        raise L.DB200Error(f"sgu_mix_wgrad: dmixed and gn must be contiguous [{B * n}, {C}], dw [>= {n}, >= {n}]")
+    check(L.load().db200_sgu_mix_wgrad(stream_ptr(), ptr(dmixed), ptr(gn), ptr(dw), dw.stride(0), B, n, C),
+          "db200_sgu_mix_wgrad")
+    return dw
+
+
+def sgu_bwd(dh, mixed, res, z_res, dmixed, du_res, dc, B, n):
+    """The SGU's elementwise backward: dmixed = bf16(dh res), du_res = bf16(dh mixed gelu'(z_res)) (the res half of the
+    proj_in gradient, any row pitch), dc[i] += sum over sequences and channels of dmixed at position i."""
+    rows, C = _sgu_act(dh, "dh")
+    for t, nm in ((mixed, "mixed"), (res, "res"), (z_res, "z_res"), (dmixed, "dmixed"), (du_res, "du_res")):
+        _sgu_act(t, nm, C)
+        if t.shape[0] != rows:
+            raise L.DB200Error(f"sgu_bwd: {nm} has {t.shape[0]} rows, expected {rows}")
+    _chk(dc, F32, "dc")
+    if rows != B * n or dc.numel() < n or not (dh.is_contiguous() and mixed.is_contiguous() and dmixed.is_contiguous()):
+        raise L.DB200Error(f"sgu_bwd: dh, mixed, dmixed must be contiguous [{B * n}, {C}], dc >= {n} entries")
+    check(L.load().db200_sgu_bwd(stream_ptr(), ptr(dh), ptr(mixed), ptr(res), res.stride(0), ptr(z_res),
+                                 z_res.stride(0), ptr(dmixed), ptr(du_res), du_res.stride(0), ptr(dc), B, n, C),
+          "db200_sgu_bwd")
+
+
+def sgu_gate_bwd(dgate, z_gate, du_gate):
+    """du_gate = bf16(dgate gelu'(z_gate)): the gate half of the proj_in gradient (z_gate and du_gate any row pitch)."""
+    rows, C = _sgu_act(dgate, "dgate")
+    _sgu_act(z_gate, "z_gate", C); _sgu_act(du_gate, "du_gate", C)
+    if not dgate.is_contiguous() or z_gate.shape[0] != rows or du_gate.shape[0] != rows:
+        raise L.DB200Error(f"sgu_gate_bwd: dgate must be contiguous [{rows}, {C}], z_gate and du_gate [{rows}, {C}]")
+    check(L.load().db200_sgu_gate_bwd(stream_ptr(), ptr(dgate), ptr(z_gate), z_gate.stride(0), ptr(du_gate),
+                                      du_gate.stride(0), rows, C), "db200_sgu_gate_bwd")
+
+
+def _sgu_decode_args(gn, res, w, c, cache, h):
+    rows, C = _sgu_act(gn, "gn")
+    _sgu_act(res, "res", C); _sgu_act(h, "h", C); _chk(c, F32, "c"); _chk(cache, BF16, "cache"); _chk(w, BF16, "w")
+    if not cache.is_contiguous() or cache.dim() != 3 or cache.shape[0] != rows or cache.shape[2] != C:
+        raise L.DB200Error(f"sgu_decode: expected a contiguous [{rows}, S, {C}] cache, got {tuple(cache.shape)}")
+    S = cache.shape[1]
+    if not gn.is_contiguous() or not h.is_contiguous() or res.shape[0] != rows or h.shape[0] != rows or \
+            c.numel() < S or w.dim() != 2 or w.shape[0] < S or w.shape[1] < S:
+        raise L.DB200Error(f"sgu_decode: gn and h contiguous [{rows}, {C}], res [{rows}, {C}], w [>= {S}, >= {S}], "
+                           f"c >= {S} entries")
+    return rows, S, C
+
+
+def sgu_decode(gn, res, w, c, cache, h, pos):
+    """One decoding step of the SGU at position pos: cache[:, pos] = gn, then h = bf16((sum_{j <= pos} w[pos, j]
+    cache[:, j] + c[pos]) res) with the sum in fp32 in j order."""
+    rows, S, C = _sgu_decode_args(gn, res, w, c, cache, h)
+    check(L.load().db200_sgu_decode(stream_ptr(), ptr(gn), ptr(res), res.stride(0), ptr(w), w.stride(0), ptr(c),
+                                    ptr(cache), ptr(h), rows, S, C, int(pos)), "db200_sgu_decode")
+    return h
+
+
+def sgu_decode_dev(gn, res, w, c, cache, h, pos_dev):
+    """sgu_decode with the position read on the device from pos_dev (graph replay)."""
+    rows, S, C = _sgu_decode_args(gn, res, w, c, cache, h)
+    _chk(pos_dev, I32, "pos_dev")
+    check(L.load().db200_sgu_decode_dev(stream_ptr(), ptr(gn), ptr(res), res.stride(0), ptr(w), w.stride(0), ptr(c),
+                                        ptr(cache), ptr(h), rows, S, C, ptr(pos_dev)), "db200_sgu_decode_dev")
+    return h
+
+
+def sgu_cache_fill(gn, cache, P, rep=1):
+    """Prefill hand-off of the SGU: gn bf16 [B*P, C] -> cache bf16 [B*rep, S, C], cache[b*rep + r, p] = gn[b*P + p]
+    (kv_cache_fill's replica order)."""
+    rows, C = _sgu_act(gn, "gn")
+    _chk(cache, BF16, "cache")
+    if P < 1 or rows % P or not gn.is_contiguous():
+        raise L.DB200Error(f"sgu_cache_fill: {rows} contiguous rows are not a whole number of {P}-position prompts")
+    B = rows // P
+    if not cache.is_contiguous() or cache.dim() != 3 or cache.shape[0] != B * int(rep) or cache.shape[2] != C:
+        raise L.DB200Error(f"sgu_cache_fill: expected a contiguous [{B * int(rep)}, S, {C}] cache, got "
+                           f"{tuple(cache.shape)}")
+    check(L.load().db200_sgu_cache_fill(stream_ptr(), ptr(gn), ptr(cache), B, int(P), C, cache.shape[1], int(rep)),
+          "db200_sgu_cache_fill")

@@ -81,8 +81,12 @@ class DalleSampler:
         e = self.e
         dev, d = e.device, e.d
         mk = lambda *shape, dtype=BF16: torch.empty(*shape, dtype=dtype, device=dev)
-        self.kc = [mk(B, e.S, e.H, e.dh) for _ in range(e.L)]
-        self.vc = [mk(B, e.S, e.H, e.dh) for _ in range(e.L)]
+        # per layer: the k / v caches, or for a gMLP layer its cache of SGU LayerNorm outputs (same bytes per token as
+        # a global layer's k + v) and None
+        self.kc = [mk(B, e.S, 2 * d) if e.mlp[i] else mk(B, e.S, e.H, e.dh) for i in range(e.L)]
+        self.vc = [None if e.mlp[i] else mk(B, e.S, e.H, e.dh) for i in range(e.L)]
+        if any(e.mlp):   # a gMLP layer's step: res | gate, gn, h
+            self.g_res, self.g_gate, self.g_gn, self.g_h = mk(B, 2 * d), mk(B, 2 * d), mk(B, 2 * d), mk(B, 2 * d)
         # token shift: the unshifted first d/2 columns of every position's LN1 (2i) and LN2 (2i + 1) output of layer i
         self.sc = [mk(B, e.S, d // 2) for _ in range(2 * e.L)] if e.shift_tokens else None
         self.x = [mk(B, d), mk(B, d)]
@@ -107,6 +111,21 @@ class DalleSampler:
         ops.layernorm_residual_fwd(self.ob, x_res, e.P(f"{p}ln{norm}_g"), e.P(f"{p}ln{norm}_b"), out, self.mean,
                                    self.rstd, e.ln_eps)
 
+    def _gmlp_step(self, p, i, pos=None, pos_dev=None):
+        """A gMLP layer's token mixing for one position of every row, from self.ln into self.g_h: the training
+        forward's two GELU products and SGU LayerNorm, then sgu_decode(_dev) over the layer's cache."""
+        e, C = self.e, 2 * self.e.d
+        w_in, b_in = e.W(p + "gm_win"), e.P(p + "gm_bin")
+        ops.linear_fwd(self.ln, w_in[:, :C], self.g_res, bias=b_in[:C], gelu=True)
+        ops.linear_fwd(self.ln, w_in[:, C:], self.g_gate, bias=b_in[C:], gelu=True)
+        ops.layernorm_fwd(self.g_gate, e.P(p + "sgu_g"), e.P(p + "sgu_b"), self.g_gn, self.mean, self.rstd, e.ln_eps)
+        if pos_dev is None:
+            ops.sgu_decode(self.g_gn, self.g_res, e.W(p + "sgu_w"), e.P(p + "sgu_c"), self.kc[i], self.g_h, pos)
+        else:
+            ops.sgu_decode_dev(self.g_gn, self.g_res, e.W(p + "sgu_w"), e.P(p + "sgu_c"), self.kc[i], self.g_h,
+                               pos_dev)
+        return self.g_h
+
     def step(self, tokens_b, pos):
         """One position for every row: tokens_b int32 [B] -> fp32 logits [B, Vpad] of the NEXT position."""
         e = self.e
@@ -117,12 +136,16 @@ class DalleSampler:
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
                 ops.shift_tokens_decode(self.ln, self.sc[2 * i], pos, e.text_seq_len, e.shift_w)
-            ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
-            if e.rotary:
-                ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
-            ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
-                            **e.axial_kw[i], **e.conv_kw[i])
-            self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
+            if e.mlp[i]:
+                self._branch_out(p, "a", self._gmlp_step(p, i, pos=pos), e.W(p + "gm_wout"), e.P(p + "gm_bout"), x_in,
+                                 self.xmid)
+            else:
+                ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
+                if e.rotary:
+                    ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
+                ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
+                                **e.axial_kw[i], **e.conv_kw[i])
+                self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
                 ops.shift_tokens_decode(self.ln, self.sc[2 * i + 1], pos, e.text_seq_len, e.shift_w)
@@ -145,12 +168,16 @@ class DalleSampler:
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
                 ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i], self.pos_dev, e.text_seq_len, e.shift_w)
-            ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
-            if e.rotary:
-                ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
-            ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
-                                radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
-            self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
+            if e.mlp[i]:
+                self._branch_out(p, "a", self._gmlp_step(p, i, pos_dev=self.pos_dev), e.W(p + "gm_wout"),
+                                 e.P(p + "gm_bout"), x_in, self.xmid)
+            else:
+                ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
+                if e.rotary:
+                    ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
+                ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
+                                    radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
+                self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
                 ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i + 1], self.pos_dev, e.text_seq_len, e.shift_w)

@@ -704,6 +704,45 @@ int db200_shift_tokens_decode_dev(db200_stream_t stream, void* y_bf16, void* cac
 int db200_shift_cache_fill(db200_stream_t stream, const void* y_bf16, void* cache_bf16, int B, int P, int d,
                            int S_cache, int rep);
 
+/* gMLP token mixing (extension; the spatial gating unit of "Pay Attention to MLPs", DALLE-pytorch's attention type
+ * 'mlp').  B sequences of n positions are rows b n .. b n + n - 1 of bf16 [B n][C] activations; W is the bf16
+ * [n][ldw] top-left block of the layer's causal mixing weight, whose strict upper triangle is zero.  Sums are fp32
+ * over wgmma (bf16 products, fp32 accumulation); one launch per call.
+ *   sgu_mix_fwd   : acc[b][i][c] = sum_{j <= i} W[i][j] gn[b n + j][c]; m = acc + c_sgu[i] (fp32);
+ *                   h = bf16(m res[b n + i][c]) (res: pitch ldres); mixed (or NULL) = bf16(m).  Any n >= 1.
+ *   sgu_mix_dgrad : dgn[b n + j][c] = bf16(sum_{i >= j} W[i][j] dmixed[b n + i][c]).  n % 64 == 0.
+ *   sgu_mix_wgrad : dW[i][j] (fp32, pitch ldw) += sum_b sum_c dmixed[b n + i][c] gn[b n + j][c] for j <= i only;
+ *                   elements with j > i are never written.  n % 64 == 0.
+ *   sgu_bwd       : dmixed = bf16(dh res); du_res (pitch ldu) = bf16(dh mixed gelu'(z_res)) with mtf's tanh GELU;
+ *                   dc[i] += sum over b, then c, of dmixed[b n + i][c] (fixed order).
+ *   sgu_gate_bwd  : du_gate[t][c] (pitch ldu) = bf16(dgate[t][c] gelu'(z_gate[t][c])), dgate contiguous [rows][C].
+ *   sgu_decode    : one decoding step at position pos for every row r, cache bf16 [rows][S][C]: cache[r][pos] = gn[r],
+ *                   then h[r][c] = bf16((sum_{j <= pos} W[pos][j] cache[r][j][c] + c_sgu[pos]) res[r][c]), the sum in
+ *                   fp32 in j order.  0 <= pos < S <= 12288.
+ *   sgu_decode_dev: the same at position *pos_dev (graph replay); a position outside [0, S) changes nothing.
+ *   sgu_cache_fill: prefill hand-off, gn bf16 [B P][C] -> cache [B rep][S_cache][C]: cache[b rep + r][p] = gn[b P + p].
+ * C % 64 == 0 (mixing products) or even (elementwise, C % 8 == 0 for the cache fill), ldw >= n, ldw % 8 == 0 and
+ * non-NULL pointers, else DB200_E_INVALID / DB200_E_ALIGN. */
+int db200_sgu_mix_fwd(db200_stream_t stream, const void* w_bf16, int64_t ldw, const void* gn_bf16, const void* res_bf16,
+                      int64_t ldres, const float* c, void* h_bf16, void* mixed_bf16, int B, int n, int C);
+int db200_sgu_mix_dgrad(db200_stream_t stream, const void* w_bf16, int64_t ldw, const void* dmixed_bf16,
+                        void* dgn_bf16, int B, int n, int C);
+int db200_sgu_mix_wgrad(db200_stream_t stream, const void* dmixed_bf16, const void* gn_bf16, float* dw, int64_t ldw,
+                        int B, int n, int C);
+int db200_sgu_bwd(db200_stream_t stream, const void* dh_bf16, const void* mixed_bf16, const void* res_bf16,
+                  int64_t ldres, const void* z_bf16, int64_t ldz, void* dmixed_bf16, void* du_bf16, int64_t ldu,
+                  float* dc, int B, int n, int C);
+int db200_sgu_gate_bwd(db200_stream_t stream, const void* dgate_bf16, const void* z_bf16, int64_t ldz, void* du_bf16,
+                       int64_t ldu, int rows, int C);
+int db200_sgu_decode(db200_stream_t stream, const void* gn_bf16, const void* res_bf16, int64_t ldres,
+                     const void* w_bf16, int64_t ldw, const float* c, void* cache_bf16, void* h_bf16, int rows, int S,
+                     int C, int pos);
+int db200_sgu_decode_dev(db200_stream_t stream, const void* gn_bf16, const void* res_bf16, int64_t ldres,
+                         const void* w_bf16, int64_t ldw, const float* c, void* cache_bf16, void* h_bf16, int rows,
+                         int S, int C, const int32_t* pos_dev);
+int db200_sgu_cache_fill(db200_stream_t stream, const void* gn_bf16, void* cache_bf16, int B, int P, int C,
+                         int S_cache, int rep);
+
 /* Segmented bf16 -> f32 gather (one launch): segment i copies table[3i+2] elements from src + table[3i] to
  * dst + table[3i+1]; `table_dev` is an int64 array in device memory.  ZeRO-1 mode: rebuilds the compact fp32 copy of the
  * vector parameters (LayerNorm g/b, biases) from the all-gathered bf16 parameters (mtf casts every variable to the

@@ -86,12 +86,13 @@ constexpr double EMB_FIX_SCALE = 1099511627776.0;  // 2^40: resolution 9.1e-13, 
 __device__ __forceinline__ void fixed_add(unsigned long long* dst, float v) {
   atomicAdd(dst, static_cast<unsigned long long>(__double2ll_rn(static_cast<double>(v) * EMB_FIX_SCALE)));
 }
-// DROP: dx[t] is multiplied by the wte keep mask first.
+// DROP: dx[t] is multiplied by the wte keep mask first.  SCALE (the stable embedding's gradient shrink): then by
+// alpha, rounded on its own in fp32 before it is summed.
 constexpr int EMB_STRIP = 32;
-template <bool DROP>
+template <bool DROP, bool SCALE = false>
 __global__ void __launch_bounds__(256)
 embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, unsigned long long* __restrict__ acc64,
-                     int T, int d, int V, const db200_dropout dw) {
+                     int T, int d, int V, const db200_dropout dw, float alpha = 1.f) {
   const int vec_per_row = d >> 3;
   const long long total = (long long)((T + EMB_STRIP - 1) / EMB_STRIP) * vec_per_row;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
@@ -124,6 +125,10 @@ embed_bwd_wte_kernel(const int* __restrict__ ids, const bf16* __restrict__ dx, u
 #pragma unroll
         for (int j = 0; j < 8; ++j) g[j] *= m[j];
       }
+      if constexpr (SCALE) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) g[j] = __fmul_rn(g[j], alpha);
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] += g[j];
     }
@@ -143,10 +148,10 @@ embed_fixed_flush_kernel(const unsigned long long* __restrict__ acc64, float* __
 }
 
 // one thread owns (s, 8 columns): dwpe[s][c..c+8) += sum_b dx[b][s][c..c+8)   (DROP: times the wpe keep mask of s,
-// which every sequence shares)
-template <bool DROP>
+// which every sequence shares; SCALE: each dx element times alpha, rounded on its own, before it is summed)
+template <bool DROP, bool SCALE = false>
 __global__ void embed_bwd_wpe_kernel(const bf16* __restrict__ dx, float* __restrict__ dwpe, int B, int S, int d,
-                                     const db200_dropout dp) {
+                                     const db200_dropout dp, float alpha = 1.f) {
   const int vec_per_row = d >> 3;
   const int total = S * vec_per_row;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -157,6 +162,10 @@ __global__ void embed_bwd_wpe_kernel(const bf16* __restrict__ dx, float* __restr
   for (int b = 0; b < B; ++b) {
     float g[8];
     unpack8(*reinterpret_cast<const uint4*>(dx + ((long long)b * S + s) * d + c), g);
+    if constexpr (SCALE) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) g[j] = __fmul_rn(g[j], alpha);
+    }
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] += g[j];
   }
@@ -312,15 +321,28 @@ __device__ __forceinline__ void ln_add_res8(const bf16* r, float* o) {
 #pragma unroll
   for (int j = 0; j < 8; ++j) o[j] = rv[j] + o[j];
 }
+// o[j] = r[j] + s[j] * o[j] (LayerScale on the sandwich LayerNorm's output, in fp32) for the 8 columns at r / s
+__device__ __forceinline__ void ln_add_scaled_res8(const bf16* r, const float* s, float* o) {
+  float rv[8];
+  unpack8(*reinterpret_cast<const uint4*>(r), rv);
+  const float4 s0 = *reinterpret_cast<const float4*>(s), s1 = *reinterpret_cast<const float4*>(s + 4);
+  const float ss[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = rv[j] + ss[j] * o[j];
+}
 
 // One warp per row; the row lives in registers (NCH 16-byte chunks per lane, d = NCH * 256).
 // RES (sandwich LayerNorm): y = bf16(res + (x - mean) * rstd * g + b), one rounding; the statistics are the same
 // instructions as without it.  `res` is a trailing parameter so that the RES = false kernels keep their code.
-template <int NCH, bool RES = false>
+// SCALE (with RES, LayerScale): y = bf16(res + scale * ((x - mean) * rstd * g + b)), one rounding.
+// DIVMAX (the stable final LayerNorm's DivideMax): the row is first divided by its maximum m (written to m_out), u =
+// x / m in fp32 (IEEE division), and the LayerNorm is that of u.
+template <int NCH, bool RES = false, bool SCALE = false, bool DIVMAX = false>
 __global__ void __launch_bounds__(128)
 layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, const float* __restrict__ b,
                      bf16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows,
-                     float eps, const bf16* __restrict__ res = nullptr) {
+                     float eps, const bf16* __restrict__ res = nullptr, const float* __restrict__ scale = nullptr,
+                     float* __restrict__ m_out = nullptr) {
   constexpr int d = NCH * 256;
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -328,11 +350,30 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, co
   const bf16* xr = x + (long long)row * d;
   float v[NCH][8];
   float sum = 0.f;
+  if constexpr (DIVMAX) {
+    float mx = -INFINITY;
 #pragma unroll
-  for (int c = 0; c < NCH; ++c) {
-    unpack8(*reinterpret_cast<const uint4*>(xr + (c * 32 + lane) * 8), v[c]);
+    for (int c = 0; c < NCH; ++c) {
+      unpack8(*reinterpret_cast<const uint4*>(xr + (c * 32 + lane) * 8), v[c]);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) sum += v[c][j];
+      for (int j = 0; j < 8; ++j) mx = fmaxf(mx, v[c][j]);
+    }
+    mx = warp_max(mx);
+    if (lane == 0) m_out[row] = mx;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        v[c][j] = __fdiv_rn(v[c][j], mx);
+        sum += v[c][j];
+      }
+  } else {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+      unpack8(*reinterpret_cast<const uint4*>(xr + (c * 32 + lane) * 8), v[c]);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sum += v[c][j];
+    }
   }
   const float mean = warp_sum(sum) * (1.f / d);
   float sq = 0.f;
@@ -359,7 +400,8 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ g, co
     float o[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean) * rstd * gg[j] + bb[j];
-    if constexpr (RES) ln_add_res8(res + (long long)row * d + col, o);
+    if constexpr (SCALE) ln_add_scaled_res8(res + (long long)row * d + col, scale + col, o);
+    else if constexpr (RES) ln_add_res8(res + (long long)row * d + col, o);
     *reinterpret_cast<uint4*>(yr + col) = pack8(o);
   }
 }
@@ -391,13 +433,15 @@ __device__ __forceinline__ void ln_bwd_store8(const float* o, bf16* dx, bf16* dx
 
 // Each warp walks rows with a grid stride, keeps per-lane partial dg/db in registers, then one block-level
 // reduction through shared memory and one partial row of dg / db (/ dxsum) per block, summed in block order afterwards.
-template <int NCH, bool DROP>
+// DIVMAX (the DivideMax LayerNorm): the normalised row is u = x / m with the row's m_in (the same IEEE division as
+// the forward) and the gradient is divided by m, dx = LN'(u)^T dy / m, before the residual term and the store.
+template <int NCH, bool DROP, bool DIVMAX = false>
 __global__ void __launch_bounds__(128)
 layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ g,
                      const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                      const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ dg,
                      float* __restrict__ db, float* __restrict__ dxsum, int rows, bf16* __restrict__ dxm,
-                     const db200_dropout dr) {
+                     const db200_dropout dr, const float* __restrict__ m_in = nullptr) {
   constexpr int d = NCH * 256;
   __shared__ float red[4][d];  // NCH <= 8 -> <= 32 KiB
   const int lane = threadIdx.x & 31;
@@ -425,6 +469,10 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
       float xv[8], dv[8];
       unpack8(*reinterpret_cast<const uint4*>(xr + col), xv);
       unpack8(*reinterpret_cast<const uint4*>(dyr + col), dv);
+      if constexpr (DIVMAX) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) xv[j] = __fdiv_rn(xv[j], m_in[row]);
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float h = (xv[j] - mean) * rstd;
@@ -444,6 +492,10 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (dg_[c][j] - c1 - xh[c][j] * c2) * rstd;
+      if constexpr (DIVMAX) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = __fdiv_rn(o[j], m_in[row]);
+      }
       if (dres) {
         float r[8];
         unpack8(*reinterpret_cast<const uint4*>(dres + (long long)row * d + col), r);
@@ -483,23 +535,50 @@ __device__ __forceinline__ float2 block128_sum2(float a, float b, float* red /*[
   __syncthreads();
   return make_float2(red[0] + red[1] + red[2] + red[3], red[4] + red[5] + red[6] + red[7]);
 }
+__device__ __forceinline__ float block128_max(float a, float* red /*[8]*/) {
+  a = warp_max(a);
+  __syncthreads();  // previous use of `red` is over
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = a;
+  __syncthreads();
+  return fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
+}
 
-template <int NCW, bool RES = false>
+template <int NCW, bool RES = false, bool SCALE = false, bool DIVMAX = false>
 __global__ void __launch_bounds__(128)
 layernorm_fwd_wide_kernel(const bf16* __restrict__ x, const float* __restrict__ g, const float* __restrict__ b,
                           bf16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int rows,
-                          float eps, const bf16* __restrict__ res = nullptr) {
+                          float eps, const bf16* __restrict__ res = nullptr,
+                          const float* __restrict__ scale = nullptr, float* __restrict__ m_out = nullptr) {
   constexpr int d = NCW * 1024;
   __shared__ float red[8];
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
     const bf16* xr = x + (long long)row * d;
     float v[NCW][8];
     float sum = 0.f;
+    if constexpr (DIVMAX) {
+      float mx = -INFINITY;
 #pragma unroll
-    for (int c = 0; c < NCW; ++c) {
-      unpack8(*reinterpret_cast<const uint4*>(xr + (c * 128 + threadIdx.x) * 8), v[c]);
+      for (int c = 0; c < NCW; ++c) {
+        unpack8(*reinterpret_cast<const uint4*>(xr + (c * 128 + threadIdx.x) * 8), v[c]);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) sum += v[c][j];
+        for (int j = 0; j < 8; ++j) mx = fmaxf(mx, v[c][j]);
+      }
+      mx = block128_max(mx, red);
+      if (threadIdx.x == 0) m_out[row] = mx;
+#pragma unroll
+      for (int c = 0; c < NCW; ++c)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          v[c][j] = __fdiv_rn(v[c][j], mx);
+          sum += v[c][j];
+        }
+    } else {
+#pragma unroll
+      for (int c = 0; c < NCW; ++c) {
+        unpack8(*reinterpret_cast<const uint4*>(xr + (c * 128 + threadIdx.x) * 8), v[c]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) sum += v[c][j];
+      }
     }
     const float mean = block128_sum2(sum, 0.f, red).x * (1.f / d);
     float sq = 0.f;
@@ -526,19 +605,20 @@ layernorm_fwd_wide_kernel(const bf16* __restrict__ x, const float* __restrict__ 
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean) * rstd * gg[j] + bb[j];
-      if constexpr (RES) ln_add_res8(res + (long long)row * d + col, o);
+      if constexpr (SCALE) ln_add_scaled_res8(res + (long long)row * d + col, scale + col, o);
+      else if constexpr (RES) ln_add_res8(res + (long long)row * d + col, o);
       *reinterpret_cast<uint4*>(yr + col) = pack8(o);
     }
   }
 }
 
-template <int NCW, bool DROP>
+template <int NCW, bool DROP, bool DIVMAX = false>
 __global__ void __launch_bounds__(128)
 layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ g,
                           const float* __restrict__ mean_in, const float* __restrict__ rstd_in,
                           const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ dg,
                           float* __restrict__ db, float* __restrict__ dxsum, int rows, bf16* __restrict__ dxm,
-                          const db200_dropout dr) {
+                          const db200_dropout dr, const float* __restrict__ m_in = nullptr) {
   constexpr int d = NCW * 1024;
   __shared__ float red[8];
   float gg[NCW][8], adg[NCW][8], adb[NCW][8], adx[NCW][8];
@@ -563,6 +643,10 @@ layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ 
       float xv[8], dv[8];
       unpack8(*reinterpret_cast<const uint4*>(xr + col), xv);
       unpack8(*reinterpret_cast<const uint4*>(dyr + col), dv);
+      if constexpr (DIVMAX) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) xv[j] = __fdiv_rn(xv[j], m_in[row]);
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float h = (xv[j] - mean) * rstd;
@@ -583,6 +667,10 @@ layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ 
       float o[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (dg_[c][j] - c1 - xh[c][j] * c2) * rstd;
+      if constexpr (DIVMAX) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = __fdiv_rn(o[j], m_in[row]);
+      }
       if (dres) {
         float r[8];
         unpack8(*reinterpret_cast<const uint4*>(dres + (long long)row * d + col), r);
@@ -602,6 +690,86 @@ layernorm_bwd_wide_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ 
       db[o] = adb[c][j];
       if (dxsum) dxsum[o] = adx[c][j];
     }
+}
+
+// ------------------------------------------------------------------------------------------------ LayerScale
+// y = bf16(x + s[c] * o), one 16-byte vector (8 columns) per thread and grid-stride step; nv = d / 8.
+__global__ void __launch_bounds__(256)
+layer_scale_residual_fwd_kernel(const bf16* __restrict__ o, const bf16* __restrict__ x, const float* __restrict__ s,
+                                bf16* __restrict__ y, long long total, int nv) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int col = (int)(i % nv) << 3;
+    float ov[8];
+    unpack8(reinterpret_cast<const uint4*>(o)[i], ov);
+    ln_add_scaled_res8(x + i * 8, s + col, ov);
+    reinterpret_cast<uint4*>(y)[i] = pack8(ov);
+  }
+}
+
+// dv = bf16(s * dy (* keep * scale)), ds += colsum(dy * v), db += colsum(dv as stored).  grid (d / 256, row splits):
+// lane -> 8 columns of the block's 256, the 8 warps stride over rows; one partial row of ds (and db) per block, summed
+// in block order by reduce_rows_add.  SAND: v = (o - mean) * rstd * g + b from the stored o, the expression of
+// layernorm_fwd_kernel.
+template <bool SAND, bool DROP>
+__global__ void __launch_bounds__(256)
+layer_scale_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ v, const float* __restrict__ s,
+                       const float* __restrict__ g, const float* __restrict__ b, const float* __restrict__ mean_in,
+                       const float* __restrict__ rstd_in, bf16* __restrict__ dv, float* __restrict__ ds_part,
+                       float* __restrict__ db_part, int rows, int d, const db200_dropout dr) {
+  __shared__ float red[8][256];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int col = blockIdx.x * 256 + lane * 8;
+  float ss[8], gg[8], bb[8], ads[8], adb[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    ss[j] = s[col + j];
+    gg[j] = SAND ? g[col + j] : 1.f;
+    bb[j] = SAND ? b[col + j] : 0.f;
+    ads[j] = adb[j] = 0.f;
+  }
+  for (int r = blockIdx.y * 8 + warp; r < rows; r += gridDim.y * 8) {
+    const long long off = (long long)r * d + col;
+    float dyv[8], vv[8], o[8];
+    unpack8(*reinterpret_cast<const uint4*>(dy + off), dyv);
+    unpack8(*reinterpret_cast<const uint4*>(v + off), vv);
+    if constexpr (SAND) {
+      const float mean = mean_in[r], rstd = rstd_in[r];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) vv[j] = (vv[j] - mean) * rstd * gg[j] + bb[j];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      ads[j] += dyv[j] * vv[j];
+      o[j] = ss[j] * dyv[j];
+    }
+    if constexpr (DROP) {
+      float m[8];
+      dropout_mul8(dr, r, d, col, m);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] *= m[j];
+    }
+    const uint4 packed = pack8(o);
+    *reinterpret_cast<uint4*>(dv + off) = packed;
+    if (db_part) {
+      unpack8(packed, o);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) adb[j] += o[j];
+    }
+  }
+  const int npass = db_part ? 2 : 1;
+#pragma unroll 1
+  for (int pass = 0; pass < npass; ++pass) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) red[warp][lane * 8 + j] = pass == 0 ? ads[j] : adb[j];
+    __syncthreads();
+    const int c = threadIdx.x;
+    float t = red[0][c];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) t += red[w][c];
+    (pass == 0 ? ds_part : db_part)[(long long)blockIdx.y * d + blockIdx.x * 256 + c] = t;
+    __syncthreads();
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ column sums
@@ -827,10 +995,11 @@ extern "C" int db200_embed_bwd(db200_stream_t stream_, const int32_t* ids, const
   return db200_embed_bwd_ex(stream_, ids, dx, dwte, dwpe, B, S, d, V, workspace, workspace_bytes, nullptr, nullptr);
 }
 
-extern "C" int db200_embed_bwd_ex(db200_stream_t stream_, const int32_t* ids, const void* dx, float* dwte,
-                                  float* dwpe, int B, int S, int d, int V, void* workspace, int64_t workspace_bytes,
-                                  const db200_dropout* wte_drop, const db200_dropout* wpe_drop) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// SCALE: every dx element times alpha before it is summed (db200_embed_bwd_scaled)
+template <bool SCALE>
+static int embed_bwd_impl(cudaStream_t stream, const int32_t* ids, const void* dx, float* dwte, float* dwpe, int B,
+                          int S, int d, int V, void* workspace, int64_t workspace_bytes, const db200_dropout* wte_drop,
+                          const db200_dropout* wpe_drop, float alpha) {
   const db200_dropout* dw = dropout_active(wte_drop) ? wte_drop : nullptr;
   const db200_dropout* dp = dropout_active(wpe_drop) ? wpe_drop : nullptr;
   DB200_REQUIRE(B > 0 && S > 0 && d > 0 && V > 0 && d % 8 == 0, DB200_E_INVALID,
@@ -843,8 +1012,8 @@ extern "C" int db200_embed_bwd_ex(db200_stream_t stream_, const int32_t* ids, co
                 "embed_bwd: needs an aligned workspace of db200_embed_bwd_workspace_bytes() bytes");
   auto* acc64 = static_cast<unsigned long long*>(workspace);
   DB200_CUDA(cudaMemsetAsync(acc64, 0, (size_t)n_wte * sizeof(unsigned long long), stream));
-  if (dw) embed_bwd_wte_kernel<true><<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V, *dw);
-  else    embed_bwd_wte_kernel<false><<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V, db200_dropout{});
+  if (dw) embed_bwd_wte_kernel<true, SCALE><<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V, *dw, alpha);
+  else    embed_bwd_wte_kernel<false, SCALE><<<blocks, 256, 0, stream>>>(ids, (const bf16*)dx, acc64, B * S, d, V, db200_dropout{}, alpha);
   int rc = check_launch("embed_bwd_wte_kernel");
   if (rc != DB200_OK) return rc;
   const long long fblocks = (n_wte + 255) / 256 < sm_count() * 16 ? (n_wte + 255) / 256 : sm_count() * 16;
@@ -852,9 +1021,23 @@ extern "C" int db200_embed_bwd_ex(db200_stream_t stream_, const int32_t* ids, co
   rc = check_launch("embed_fixed_flush_kernel");
   if (rc != DB200_OK) return rc;
   const int total_pe = S * (d / 8);
-  if (dp) embed_bwd_wpe_kernel<true><<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d, *dp);
-  else    embed_bwd_wpe_kernel<false><<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d, db200_dropout{});
+  if (dp) embed_bwd_wpe_kernel<true, SCALE><<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d, *dp, alpha);
+  else    embed_bwd_wpe_kernel<false, SCALE><<<(total_pe + 127) / 128, 128, 0, stream>>>((const bf16*)dx, dwpe, B, S, d, db200_dropout{}, alpha);
   return check_launch("embed_bwd_wpe_kernel");
+}
+
+extern "C" int db200_embed_bwd_ex(db200_stream_t stream_, const int32_t* ids, const void* dx, float* dwte,
+                                  float* dwpe, int B, int S, int d, int V, void* workspace, int64_t workspace_bytes,
+                                  const db200_dropout* wte_drop, const db200_dropout* wpe_drop) {
+  return embed_bwd_impl<false>(reinterpret_cast<cudaStream_t>(stream_), ids, dx, dwte, dwpe, B, S, d, V, workspace,
+                               workspace_bytes, wte_drop, wpe_drop, 1.f);
+}
+
+extern "C" int db200_embed_bwd_scaled(db200_stream_t stream_, const int32_t* ids, const void* dx, float* dwte,
+                                      float* dwpe, int B, int S, int d, int V, void* workspace, int64_t workspace_bytes,
+                                      const db200_dropout* wte_drop, const db200_dropout* wpe_drop, float alpha) {
+  return embed_bwd_impl<true>(reinterpret_cast<cudaStream_t>(stream_), ids, dx, dwte, dwpe, B, S, d, V, workspace,
+                              workspace_bytes, wte_drop, wpe_drop, alpha);
 }
 
 extern "C" int db200_shift_labels(db200_stream_t stream_, const int32_t* ids, int32_t* labels, int B, int S,
@@ -994,6 +1177,121 @@ extern "C" int db200_layernorm_residual_fwd(db200_stream_t stream_, const void* 
   return check_launch("layernorm_residual_fwd_kernel");
 }
 
+extern "C" int db200_layernorm_scale_residual_fwd(db200_stream_t stream_, const void* o, const void* x_res,
+                                                  const float* g, const float* b, const float* s, void* y, float* mean,
+                                                  float* rstd, int rows, int d, float eps) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(rows > 0, DB200_E_INVALID, "layernorm_scale_residual_fwd: rows must be positive");
+  DB200_REQUIRE(o && x_res && y && g && b && s && mean && rstd, DB200_E_INVALID,
+                "layernorm_scale_residual_fwd: NULL pointer");
+  DB200_REQUIRE(aligned16(o) && aligned16(x_res) && aligned16(y) && aligned16(g) && aligned16(b) && aligned16(s),
+                DB200_E_ALIGN, "layernorm_scale_residual_fwd: unaligned pointer");
+  const int grid = (rows + 3) / 4;
+  const bf16* op = (const bf16*)o;
+  const bf16* rp = (const bf16*)x_res;
+  bf16* yp = (bf16*)y;
+  switch (d) {
+    case 256:  layernorm_fwd_kernel<1, true, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp, s); break;
+    case 512:  layernorm_fwd_kernel<2, true, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp, s); break;
+    case 768:  layernorm_fwd_kernel<3, true, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp, s); break;
+    case 1024: layernorm_fwd_kernel<4, true, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp, s); break;
+    case 2048: layernorm_fwd_kernel<8, true, true><<<grid, 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp, s); break;
+    case 4096: layernorm_fwd_wide_kernel<4, true, true><<<min(rows, sm_count() * 16), 128, 0, stream>>>(op, g, b, yp, mean, rstd, rows, eps, rp, s); break;
+    default:
+      return set_error(DB200_E_UNSUPPORTED, "layernorm_scale_residual_fwd: d=%d not in {256,512,768,1024,2048,4096}",
+                       d);
+  }
+  return check_launch("layernorm_scale_residual_fwd_kernel");
+}
+
+extern "C" int db200_layernorm_divmax_fwd(db200_stream_t stream_, const void* x, const float* g, const float* b,
+                                          void* y, float* mean, float* rstd, float* m, int rows, int d, float eps) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(rows > 0, DB200_E_INVALID, "layernorm_divmax_fwd: rows must be positive");
+  DB200_REQUIRE(x && y && g && b && mean && rstd && m, DB200_E_INVALID, "layernorm_divmax_fwd: NULL pointer");
+  DB200_REQUIRE(aligned16(x) && aligned16(y) && aligned16(g) && aligned16(b), DB200_E_ALIGN,
+                "layernorm_divmax_fwd: unaligned pointer");
+  const int grid = (rows + 3) / 4;
+  const bf16* xp = (const bf16*)x;
+  bf16* yp = (bf16*)y;
+  switch (d) {
+    case 256:  layernorm_fwd_kernel<1, false, false, true><<<grid, 128, 0, stream>>>(xp, g, b, yp, mean, rstd, rows, eps, nullptr, nullptr, m); break;
+    case 512:  layernorm_fwd_kernel<2, false, false, true><<<grid, 128, 0, stream>>>(xp, g, b, yp, mean, rstd, rows, eps, nullptr, nullptr, m); break;
+    case 768:  layernorm_fwd_kernel<3, false, false, true><<<grid, 128, 0, stream>>>(xp, g, b, yp, mean, rstd, rows, eps, nullptr, nullptr, m); break;
+    case 1024: layernorm_fwd_kernel<4, false, false, true><<<grid, 128, 0, stream>>>(xp, g, b, yp, mean, rstd, rows, eps, nullptr, nullptr, m); break;
+    case 2048: layernorm_fwd_kernel<8, false, false, true><<<grid, 128, 0, stream>>>(xp, g, b, yp, mean, rstd, rows, eps, nullptr, nullptr, m); break;
+    case 4096: layernorm_fwd_wide_kernel<4, false, false, true><<<min(rows, sm_count() * 16), 128, 0, stream>>>(xp, g, b, yp, mean, rstd, rows, eps, nullptr, nullptr, m); break;
+    default:
+      return set_error(DB200_E_UNSUPPORTED, "layernorm_divmax_fwd: d=%d not in {256,512,768,1024,2048,4096}", d);
+  }
+  return check_launch("layernorm_divmax_fwd_kernel");
+}
+
+extern "C" int db200_layer_scale_residual_fwd(db200_stream_t stream_, const void* o, const void* x_res, const float* s,
+                                              void* y, int rows, int d) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(rows > 0 && d > 0 && d % 8 == 0, DB200_E_INVALID,
+                "layer_scale_residual_fwd: need rows > 0 and d a positive multiple of 8 (got rows=%d d=%d)", rows, d);
+  DB200_REQUIRE(o && x_res && s && y, DB200_E_INVALID, "layer_scale_residual_fwd: NULL pointer");
+  DB200_REQUIRE(aligned16(o) && aligned16(x_res) && aligned16(s) && aligned16(y), DB200_E_ALIGN,
+                "layer_scale_residual_fwd: unaligned pointer");
+  const long long total = (long long)rows * (d / 8);
+  const long long want = (total + 255) / 256;
+  const int grid = (int)(want < (long long)sm_count() * 16 ? want : (long long)sm_count() * 16);
+  layer_scale_residual_fwd_kernel<<<grid, 256, 0, stream>>>((const bf16*)o, (const bf16*)x_res, s, (bf16*)y, total,
+                                                            d / 8);
+  return check_launch("layer_scale_residual_fwd_kernel");
+}
+
+static int layer_scale_bwd_splits(int rows, int d) {
+  const int gx = d / 256;
+  int gy = (sm_count() * 4 + gx - 1) / gx;
+  if (gy > (rows + 7) / 8) gy = (rows + 7) / 8;
+  return gy < 1 ? 1 : gy;
+}
+
+extern "C" int64_t db200_layer_scale_bwd_workspace_bytes(int rows, int d) {
+  if (rows <= 0 || d <= 0 || d % 256) return 0;
+  return (int64_t)2 * layer_scale_bwd_splits(rows, d) * d * (int64_t)sizeof(float);
+}
+
+extern "C" int db200_layer_scale_bwd(db200_stream_t stream_, const void* dy, const void* v, const float* s,
+                                     const float* g, const float* b, const float* mean, const float* rstd, void* dv,
+                                     float* ds, float* db, const db200_dropout* drop, int rows, int d, void* workspace,
+                                     int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(rows > 0 && d > 0 && d % 256 == 0, DB200_E_INVALID,
+                "layer_scale_bwd: need rows > 0 and d a positive multiple of 256 (got rows=%d d=%d)", rows, d);
+  DB200_REQUIRE(dy && v && s && dv && ds, DB200_E_INVALID, "layer_scale_bwd: NULL pointer");
+  DB200_REQUIRE(aligned16(dy) && aligned16(v) && aligned16(dv), DB200_E_ALIGN, "layer_scale_bwd: unaligned pointer");
+  const bool sand = g != nullptr;
+  DB200_REQUIRE(!sand || (b && mean && rstd), DB200_E_INVALID,
+                "layer_scale_bwd: the sandwich form (g given) needs b, mean and rstd");
+  DB200_REQUIRE(!(sand && dropout_active(drop)), DB200_E_INVALID,
+                "layer_scale_bwd: the sandwich form takes no dropout (the LayerNorm backward applies it)");
+  const int gy = layer_scale_bwd_splits(rows, d);
+  DB200_REQUIRE(workspace_ok(workspace, workspace_bytes, db200_layer_scale_bwd_workspace_bytes(rows, d)),
+                DB200_E_INVALID, "layer_scale_bwd: needs an aligned workspace of db200_layer_scale_bwd_workspace_bytes() bytes");
+  float* ds_part = static_cast<float*>(workspace);
+  float* db_part = db ? ds_part + (size_t)gy * d : nullptr;
+  const dim3 grid(d / 256, gy);
+  const bf16 *dyp = (const bf16*)dy, *vp = (const bf16*)v;
+  bf16* dvp = (bf16*)dv;
+  if (sand)
+    layer_scale_bwd_kernel<true, false><<<grid, 256, 0, stream>>>(dyp, vp, s, g, b, mean, rstd, dvp, ds_part, db_part,
+                                                                  rows, d, db200_dropout{});
+  else if (dropout_active(drop))
+    layer_scale_bwd_kernel<false, true><<<grid, 256, 0, stream>>>(dyp, vp, s, g, b, mean, rstd, dvp, ds_part, db_part,
+                                                                  rows, d, *drop);
+  else
+    layer_scale_bwd_kernel<false, false><<<grid, 256, 0, stream>>>(dyp, vp, s, g, b, mean, rstd, dvp, ds_part, db_part,
+                                                                   rows, d, db200_dropout{});
+  int rc = check_launch("layer_scale_bwd_kernel");
+  if (rc == DB200_OK) rc = reduce_rows_add(stream, ds_part, gy, d, ds);
+  if (rc == DB200_OK && db) rc = reduce_rows_add(stream, db_part, gy, d, db);
+  return rc;
+}
+
 static int layernorm_bwd_grid(int rows, int d) {
   int grid = d == 4096 ? rows : (rows + 3) / 4;
   if (grid > sm_count() * 4) grid = sm_count() * 4;
@@ -1004,11 +1302,32 @@ extern "C" int64_t db200_layernorm_bwd_workspace_bytes(int rows, int d) {
   return (int64_t)3 * layernorm_bwd_grid(rows, d) * d * (int64_t)sizeof(float);
 }
 
+// the DivideMax LayerNorm backward's launch (layernorm_bwd_impl<DROP, true>); its d = 2048 rows run on the
+// one-CTA-per-row kernel, which keeps the row in registers without spilling
 template <bool DROP>
+static int layernorm_divmax_bwd_launch(cudaStream_t stream, int grid, int d, const bf16* dyp, const bf16* xp,
+                                       const float* g, const float* mean, const float* rstd, const bf16* drp, bf16* dxp,
+                                       float* dg, float* db, float* dxsum, int rows, bf16* dxmp,
+                                       const db200_dropout& dr, const float* m) {
+  switch (d) {
+    case 256:  layernorm_bwd_kernel<1, DROP, true><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr, m); break;
+    case 512:  layernorm_bwd_kernel<2, DROP, true><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr, m); break;
+    case 768:  layernorm_bwd_kernel<3, DROP, true><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr, m); break;
+    case 1024: layernorm_bwd_kernel<4, DROP, true><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr, m); break;
+    case 2048: layernorm_bwd_wide_kernel<2, DROP, true><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr, m); break;
+    case 4096: layernorm_bwd_wide_kernel<4, DROP, true><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr, m); break;
+    default:
+      return set_error(DB200_E_UNSUPPORTED, "layernorm: d=%d not in {256,512,768,1024,2048,4096}", d);
+  }
+  return DB200_OK;
+}
+
+// DIVMAX: the DivideMax LayerNorm's backward (m: the rows' maxima, layernorm_divmax_bwd_launch).
+template <bool DROP, bool DIVMAX = false>
 static int layernorm_bwd_impl(cudaStream_t stream, const void* dy, const void* x, const float* g, const float* mean,
                               const float* rstd, const void* dres, void* dx, float* dg, float* db, float* dxsum,
                               int rows, int d, void* workspace, int64_t workspace_bytes, void* dxm,
-                              const db200_dropout& dr) {
+                              const db200_dropout& dr, const float* m = nullptr) {
   DB200_REQUIRE(rows > 0, DB200_E_INVALID, "layernorm_bwd: rows must be positive");
   DB200_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx) && aligned16(g) && mean && rstd && dg && db &&
                     aligned16(dres),
@@ -1026,15 +1345,21 @@ static int layernorm_bwd_impl(cudaStream_t stream, const void* dy, const void* x
   dg = ws;
   db = ws + (size_t)grid * d;
   dxsum = dxsum_out ? ws + (size_t)2 * grid * d : nullptr;
-  switch (d) {
-    case 256:  layernorm_bwd_kernel<1, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
-    case 512:  layernorm_bwd_kernel<2, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
-    case 768:  layernorm_bwd_kernel<3, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
-    case 1024: layernorm_bwd_kernel<4, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
-    case 2048: layernorm_bwd_kernel<8, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
-    case 4096: layernorm_bwd_wide_kernel<4, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
-    default:
-      return set_error(DB200_E_UNSUPPORTED, "layernorm: d=%d not in {256,512,768,1024,2048,4096}", d);
+  if constexpr (DIVMAX) {
+    const int rc0 = layernorm_divmax_bwd_launch<DROP>(stream, grid, d, dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum,
+                                                      rows, dxmp, dr, m);
+    if (rc0 != DB200_OK) return rc0;
+  } else {
+    switch (d) {
+      case 256:  layernorm_bwd_kernel<1, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+      case 512:  layernorm_bwd_kernel<2, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+      case 768:  layernorm_bwd_kernel<3, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+      case 1024: layernorm_bwd_kernel<4, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+      case 2048: layernorm_bwd_kernel<8, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+      case 4096: layernorm_bwd_wide_kernel<4, DROP><<<grid, 128, 0, stream>>>(dyp, xp, g, mean, rstd, drp, dxp, dg, db, dxsum, rows, dxmp, dr); break;
+      default:
+        return set_error(DB200_E_UNSUPPORTED, "layernorm: d=%d not in {256,512,768,1024,2048,4096}", d);
+    }
   }
   int rc = check_launch("layernorm_bwd_kernel");
   if (rc == DB200_OK) rc = reduce_rows_add(stream, dg, grid, d, dg_out);
@@ -1066,6 +1391,20 @@ extern "C" int db200_layernorm_bwd_dropout(db200_stream_t stream_, const void* d
   }
   return layernorm_bwd_impl<true>(stream, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, rows, d, workspace,
                                   workspace_bytes, dxm, *drop);
+}
+
+extern "C" int db200_layernorm_divmax_bwd(db200_stream_t stream_, const void* dy, const void* x, const float* g,
+                                          const float* mean, const float* rstd, const float* m, const void* dres,
+                                          void* dx, void* dxm, float* dg, float* db, float* dxsum, int rows, int d,
+                                          const db200_dropout* drop, void* workspace, int64_t workspace_bytes) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(m, DB200_E_INVALID, "layernorm_divmax_bwd: NULL m");
+  if (!dropout_active(drop))
+    return layernorm_bwd_impl<false, true>(stream, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, rows, d, workspace,
+                                           workspace_bytes, nullptr, db200_dropout{}, m);
+  DB200_REQUIRE(aligned16(dxm) && dxm, DB200_E_ALIGN, "layernorm_divmax_bwd: NULL or unaligned dxm");
+  return layernorm_bwd_impl<true, true>(stream, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, rows, d, workspace,
+                                        workspace_bytes, dxm, *drop, m);
 }
 
 extern "C" int db200_layernorm_bwd(db200_stream_t stream_, const void* dy, const void* x, const float* g,

@@ -61,7 +61,8 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
-def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False, mlp_layers=None):
+def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False, mlp_layers=None,
+                 layer_scale=False):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
     length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
     column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
@@ -69,7 +70,9 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     first and the gate columns second.  sandwich_norm: each layer ends with its two output LayerNorms, lna_g / lna_b
     (attention branch) and lnm_g / lnm_b (MLP branch), inside the layer's span l{i}.ln1_g .. layer_last(i).
     mlp_layers: per layer, True for a gMLP token-mixing layer, whose gm_win [d, 4d], gm_bin [4d], sgu_g / sgu_b [2d],
-    sgu_w [S, S], sgu_c [S], gm_wout [2d, d] and gm_bout [d] take the place of wqkv, wo and o_b."""
+    sgu_w [S, S], sgu_c [S], gm_wout [2d, d] and gm_bout [d] take the place of wqkv, wo and o_b.  layer_scale: each
+    layer ends with its two LayerScale vectors, lsa (the token mixer's branch) and lsm (the MLP's), after the sandwich
+    LayerNorms."""
     w1_cols = 8 * d if gated_mlp else 4 * d
     Vpad = _round_up(V, 64)
     lay = ParamLayout()
@@ -96,6 +99,8 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
         if sandwich_norm:
             lay.add(p + "lna_g", (d,)); lay.add(p + "lna_b", (d,))
             lay.add(p + "lnm_g", (d,)); lay.add(p + "lnm_b", (d,))
+        if layer_scale:
+            lay.add(p + "lsa", (d,)); lay.add(p + "lsm", (d,))
     lay.add("lnf_g", (d,)); lay.add("lnf_b", (d,))
     lay.add("wout", (d, Vpad)); lay.add("bout", (Vpad,))
     return lay
@@ -326,6 +331,40 @@ def validate_sandwich_norm(sandwich_norm):
     return sandwich_norm
 
 
+def validate_layer_scale(layer_scale):
+    """The LayerScale setting: None or False -> None (off); True -> True (DALLE-pytorch's depth schedule,
+    layer_scale_init); a finite real > 0 -> that float for every layer.  Anything else is a ValueError: in particular a
+    bool is never read as the number 1 or 0."""
+    if layer_scale is None or layer_scale is False:
+        return None
+    if layer_scale is True:
+        return True
+    if not (_real(layer_scale) and math.isfinite(layer_scale) and layer_scale > 0):
+        raise ValueError(f"layer_scale = {layer_scale!r}: must be true, false, null or a finite number > 0")
+    return float(layer_scale)
+
+
+def layer_scale_init(layer_scale, i):
+    """The initial value of layer i's (0-based) LayerScale vectors: a number as given, or for True DALLE-pytorch's
+    schedule by depth n = i + 1: 0.1 for n <= 18, 1e-5 for 18 < n <= 24, 1e-6 beyond."""
+    if layer_scale is not True:
+        return float(layer_scale)
+    n = i + 1
+    return 0.1 if n <= 18 else 1e-5 if n <= 24 else 1e-6
+
+
+STABLE_ALPHA = 0.1   # the stable option's embedding gradient shrink: tokens * 0.1 + tokens.detach() * 0.9
+
+
+def validate_stable(stable):
+    """The stable switch: None (off) or a bool; numbers, strings and other values are a ValueError."""
+    if stable is None:
+        return False
+    if not isinstance(stable, bool):
+        raise ValueError(f"stable must be a bool or None, got {stable!r}")
+    return stable
+
+
 def validate_shift_tokens(shift_tokens, image_seq_len):
     """The token-shift switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
     handled by model_fns.shift_tokens).  On, it needs a square image-token grid (image_seq_len = W^2)."""
@@ -350,19 +389,21 @@ class DalleEngine:
     """One data-parallel replica of the DALL-E decoder (src/dalle_mtf/models.py:141-416)."""
 
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lna_g", "lna_b", "lnm_g", "lnm_b", "lnf_g",
-                     "lnf_b", "bout", "gm_bin", "sgu_g", "sgu_b", "sgu_c", "gm_bout")
+                     "lnf_b", "bout", "gm_bin", "sgu_g", "sgu_b", "sgu_c", "gm_bout", "lsa", "lsm")
     conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
     gated_mlp = False   # the gated MLP (validate_gated_mlp), set by the constructor
     shift_tokens = False   # the token shift (validate_shift_tokens), set by the constructor
     sandwich_norm = False   # the sandwich LayerNorm (validate_sandwich_norm), set by the constructor
     mlp = ()   # per-layer flags of the gMLP token-mixing layers (layer_mlp), set by the constructor; () none
+    layer_scale = None   # LayerScale (validate_layer_scale), set by the constructor; None: off
+    stable = False   # DALLE-pytorch's stable option (validate_stable), set by the constructor
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
                  activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False,
-                 shift_tokens=False, sandwich_norm=False):
+                 shift_tokens=False, sandwich_norm=False, layer_scale=None, stable=False):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -443,12 +484,30 @@ class DalleEngine:
         LayerNorm, LNa of it).  W_sgu [S, S] is lower triangular: its strict upper triangle starts, and stays, exactly
         0 (its gradient there is never written) and a checkpoint with a non-zero one is refused.  Rotary embeddings and
         attention dropout do not apply to the layer; residual dropout does.  Kept per saved layer: res, gate, their z,
-        gn, mixed and h (seven bf16 [T, 2d]) and the SGU LayerNorm's statistics."""
+        gn, mixed and h (seven bf16 [T, 2d]) and the SGU LayerNorm's statistics.
+
+        layer_scale (validate_layer_scale): DALLE-pytorch's LayerScale around both branches of every layer.  The branch
+        output after its residual dropout (with the sandwich LayerNorm: that LayerNorm's output) is multiplied per
+        channel by a learned vector before the residual add, xmid = bf16(x + s_a oa), xout = bf16(xmid + s_m om), one
+        rounding each in fp32 (ops.layer_scale_residual_fwd, ops.layernorm_scale_residual_fwd).  s_a and s_m are the
+        parameters lsa and lsm (layer_i/attn/layer_scale, or layer_i/gmlp/layer_scale in a gMLP layer, and
+        layer_i/mlp/layer_scale), initialised by layer_scale_init and not weight-decayed.  Without the sandwich
+        LayerNorm oa and om are kept per saved layer (two bf16 [T, d]); with it they are already kept.
+
+        stable (validate_stable): DALLE-pytorch's stable option.  (1) The embedding's gradient shrinks: its forward is
+        unchanged and every embedding table's gradient is STABLE_ALPHA times what it was (tokens * alpha +
+        tokens.detach() * (1 - alpha)).  (2) DivideMax before the final LayerNorm, wherever it runs (training, the
+        prefill, the decoder, logits()): per row m = max_c x[c] (held constant in backward), u = x / m in fp32 and
+        hf = bf16(LN_f(u)) (ops.layernorm_divmax_fwd); one more fp32 [T] keeps m.  (3) Its stable softmax is the
+        softmax every attention kernel already computes (the row maximum subtracted in fp32).  No parameter is
+        added."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
         self.shift_w = math.isqrt(image_seq_len) if self.shift_tokens else None   # the grid side W
         self.sandwich_norm = validate_sandwich_norm(sandwich_norm)
+        self.layer_scale = validate_layer_scale(layer_scale)
+        self.stable = validate_stable(stable)
         self.rotary = validate_rotary(rotary_dim, rotary_base, self.dh)
         self.activation = validate_activation(activation)
         self.gated_mlp = validate_gated_mlp(gated_mlp)
@@ -506,10 +565,10 @@ class DalleEngine:
 
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         mlp_layers = self.mlp if any(self.mlp) else None
-        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, gated_mlp=self.gated_mlp,
-                                         sandwich_norm=self.sandwich_norm, mlp_layers=mlp_layers) \
-            if self.row_col else param_layout(d, Lyr, V, S, gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm,
-                                              mlp_layers=mlp_layers)
+        kw = dict(gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm, mlp_layers=mlp_layers,
+                  layer_scale=self.layer_scale is not None)
+        self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, **kw) if self.row_col else \
+            param_layout(d, Lyr, V, S, **kw)
         self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
@@ -602,11 +661,12 @@ class DalleEngine:
         n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else S
         gate = (4 * d * d + 4 * d) if self.gated_mlp else 0   # the gate half of W1 and b1
         sandwich = 4 * d if self.sandwich_norm else 0         # LNa and LNm: g and b each
+        scales = 2 * d if self.layer_scale is not None else 0  # the two LayerScale vectors
         n_mlp = sum(self.mlp)
         # a gMLP layer: W_in + b_in, the SGU norm, W_sgu + c_sgu and W_out + b_out in place of q, k, v, o and o_b
         gmlp = 4 * d * d + 4 * d + 4 * d + S * S + S + 2 * d * d + d - (4 * d * d + d)
         return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d +
-                                          gate + sandwich) + n_mlp * gmlp + 2 * d + d * V + V
+                                          gate + sandwich + scales) + n_mlp * gmlp + 2 * d + d * V + V
 
     EMBED_REF_NAMES = {"wte": "embedding/wte", "wpe": "positional_embedding/wpe",
                        "image_row": "positional_embedding/image_row", "image_col": "positional_embedding/image_col"}
@@ -620,7 +680,7 @@ class DalleEngine:
                       "gm_wout": "gmlp/proj_out/kernel", "gm_bout": "gmlp/proj_out/bias"}
 
     @staticmethod
-    def _ref_names(i, sandwich_norm=False, mlp=False):
+    def _ref_names(i, sandwich_norm=False, mlp=False, layer_scale=False):
         pre = f"layer_{i}/"
         names = {
             "ln1_g": pre + "norm_1/g", "ln1_b": pre + "norm_1/b", "wo": pre + "attn/o",
@@ -634,16 +694,30 @@ class DalleEngine:
         if sandwich_norm:
             names.update({"lna_g": pre + "attn/norm_out/g", "lna_b": pre + "attn/norm_out/b",
                           "lnm_g": pre + "mlp/norm_out/g", "lnm_b": pre + "mlp/norm_out/b"})
+        if layer_scale:
+            names.update({"lsa": pre + ("gmlp" if mlp else "attn") + "/layer_scale", "lsm": pre + "mlp/layer_scale"})
         return names
+
+    @property
+    def split_branch(self):
+        """Whether each branch output is stored before its residual add (sandwich LayerNorm or LayerScale), its
+        gradient then coming from the branch's own backward rather than from the LayerNorm that forms the residual
+        gradient."""
+        return self.sandwich_norm or self.layer_scale is not None
+
+    def layer_last(self, i):
+        """The last entry of layer i in the layout: the end of its data-parallel bucket."""
+        p = f"l{i}."
+        return p + ("lsm" if self.layer_scale is not None else "lnm_b" if self.sandwich_norm else "b2")
 
     def _is_mlp(self, i):
         """Whether layer i is a gMLP token-mixing layer."""
         return bool(self.mlp) and self.mlp[i]
 
     def _layer_ref_names(self, i):
-        """Reference names of layer i's parameters other than q / k / v (with this engine's sandwich_norm and layer
-        kind)."""
-        return self._ref_names(i, self.sandwich_norm, self._is_mlp(i))
+        """Reference names of layer i's parameters other than q / k / v (with this engine's sandwich_norm, layer kind
+        and layer_scale)."""
+        return self._ref_names(i, self.sandwich_norm, self._is_mlp(i), self.layer_scale is not None)
 
     def _check_layer_kinds(self, named):
         """Refuse a checkpoint whose layer kinds differ from this model's: an attention layer's variables where this
@@ -685,6 +759,22 @@ class DalleEngine:
             raise L.DB200Error(f"load_params: {k}: a sandwich LayerNorm variable, but this model has "
                                f"sandwich_norm = {self.sandwich_norm}")
 
+    def _check_layer_scale_names(self, named):
+        """Refuse a checkpoint of the other layer_scale kind: one without a LayerScale vector this model has, or with
+        one it does not have.  The error names the first such variable (layer order, the token mixer's first)."""
+        want = [rn for i in range(self.L) for k, rn in self._layer_ref_names(i).items() if k in ("lsa", "lsm")]
+        for rn in want:
+            if rn not in named:
+                raise L.DB200Error(f"load_params: {rn}: missing from the checkpoint of a layer_scale model")
+        extra = [k for k in named if k.startswith("layer_") and k.endswith("/layer_scale") and k not in want]
+        if extra:
+            def order(n):   # layer index (a malformed one last), the token mixer's before the MLP's
+                i = n.split("/")[0][6:]
+                return (int(i) if i.isdigit() else math.inf, n.split("/")[1] == "mlp", n)
+            k = min(extra, key=order)
+            raise L.DB200Error(f"load_params: {k}: a LayerScale variable, but this model has layer_scale = "
+                               f"{self.layer_scale}")
+
     def load_params(self, named):
         """Load a dict keyed by the reference's variable names (SURVEY.md Appendix B); CPU or CUDA fp32 tensors."""
         self.load_flat(self.master, named)
@@ -718,6 +808,7 @@ class DalleEngine:
         dev = self.device
         self._check_sandwich_names(named)
         self._check_layer_kinds(named)
+        self._check_layer_scale_names(named)
         if self.zero is not None:
             if flat is not self.master:
                 raise L.DB200Error("ZeRO-1 mode: loading sharded Adam slots is not implemented (throughput configuration)")
@@ -815,6 +906,9 @@ class DalleEngine:
             self.P(p + "ln1_g").fill_(1.0); self.P(p + "ln2_g").fill_(1.0)
             if self.sandwich_norm:
                 self.P(p + "lna_g").fill_(1.0); self.P(p + "lnm_g").fill_(1.0)
+            if self.layer_scale is not None:
+                v = layer_scale_init(self.layer_scale, i)
+                self.P(p + "lsa").fill_(v); self.P(p + "lsm").fill_(v)
             if self._is_mlp(i):
                 w_in, w_sgu, w_out = self._gmlp_init(g, 0.02 / math.sqrt(Lyr))
                 self.P(p + "gm_win").copy_(w_in); self.P(p + "sgu_w").copy_(w_sgu); self.P(p + "gm_wout").copy_(w_out)
@@ -855,6 +949,9 @@ class DalleEngine:
             self._scatter_full(p + "ln1_g", ones(d)); self._scatter_full(p + "ln2_g", ones(d))
             if self.sandwich_norm:
                 self._scatter_full(p + "lna_g", ones(d)); self._scatter_full(p + "lnm_g", ones(d))
+            if self.layer_scale is not None:
+                v = layer_scale_init(self.layer_scale, i)
+                self._scatter_full(p + "lsa", ones(d) * v); self._scatter_full(p + "lsm", ones(d) * v)
             if self._is_mlp(i):
                 w_in, w_sgu, w_out = self._gmlp_init(g, 0.02 / math.sqrt(Lyr))
                 self._scatter_full(p + "gm_win", w_in); self._scatter_full(p + "sgu_w", w_sgu)
@@ -902,9 +999,8 @@ class DalleEngine:
         # of the LayerNorm output in backward
         scratch = e(T, d) if self.shift_tokens else None
         raw = {"ln1_raw": scratch, "ln2_raw": scratch} if self.shift_tokens else {}
-        # sandwich LayerNorm: both branch outputs and the statistics of their LayerNorms, for backward
-        sand = (lambda: {"oa": e(T, d), "om": e(T, d), "meana": e(T, dtype=F32), "rstda": e(T, dtype=F32),
-                         "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)}) if self.sandwich_norm else dict
+        # sandwich LayerNorm or LayerScale: both branch outputs (and the statistics of their LayerNorms), for backward
+        sand = lambda: self._branch_bufs(T, e)
         # the token mixer's buffers of a saved layer: attention's, a gMLP layer's, or (recompute_grad's one slot) both
         attn_slot = (lambda i: not all(self.mlp)) if self.recompute_grad else (lambda i: not self._is_mlp(i))
         gmlp_slot = (lambda i: any(self.mlp)) if self.recompute_grad else (lambda i: self._is_mlp(i))
@@ -920,6 +1016,7 @@ class DalleEngine:
                 **({"z1": e(T, 8 * d)} if self.gated_mlp else {}), **raw, **sand(),
             } for i in range(n_saved)],
             "hf": e(T, d), "meanf": e(T, dtype=F32), "rstdf": e(T, dtype=F32),
+            "mf": e(T, dtype=F32) if self.stable else None,   # DivideMax: the rows' maxima
             "labels": e(B, S, dtype=I32), "loss_rows": e(T, dtype=F32),
             # backward scratch
             "dx_a": e(T, d), "dx_b": e(T, d), "dtmp": e(T, d), "dh1": e(T, 4 * d), "dqkv": e(T, 3 * d),
@@ -949,6 +1046,15 @@ class DalleEngine:
                     "label_logit": e(rows, dtype=F32), "lse_v": e(rows, dtype=F32), "loss_rows": e(rows, dtype=F32),
                     "dlogits": e(rows, N), "dx": e(rows, d)})
         self._bufs, self._buf_key = b, key
+        return b
+
+    def _branch_bufs(self, T, e):
+        """The branch outputs oa and om that the sandwich LayerNorm or LayerScale keeps before the residual add, and
+        with the sandwich LayerNorm its statistics (nothing without either)."""
+        b = {"oa": e(T, self.d), "om": e(T, self.d)} if self.split_branch else {}
+        if self.sandwich_norm:
+            b.update({"meana": e(T, dtype=F32), "rstda": e(T, dtype=F32), "meanm": e(T, dtype=F32),
+                      "rstdm": e(T, dtype=F32)})
         return b
 
     def _gmlp_bufs(self, T, e, train):
@@ -998,13 +1104,24 @@ class DalleEngine:
     def _branch_out(self, p, norm, x, w, bias, x_res, out, site, sv):
         """The output projection of a branch of layer prefix p and its residual add: out = x_res + drop(x w + bias),
         or with the sandwich LayerNorm sv["o<norm>"] = drop(x w + bias) and out = x_res + LN<norm>(sv["o<norm>"])
-        (norm "a": the attention branch's, "m": the MLP's)."""
-        if not self.sandwich_norm:
+        (norm "a": the attention branch's, "m": the MLP's).  LayerScale multiplies what is added by s<norm>."""
+        if not self.split_branch:
             return ops.linear_fwd(x, w, out, bias=bias, residual=x_res, dropout=site)
         o = sv["o" + norm]
         ops.linear_fwd(x, w, o, bias=bias, dropout=site)
-        ops.layernorm_residual_fwd(o, x_res, self.P(f"{p}ln{norm}_g"), self.P(f"{p}ln{norm}_b"), out, sv["mean" + norm],
-                                   sv["rstd" + norm], self.ln_eps)
+        self.branch_add(p, norm, o, x_res, out, sv.get("mean" + norm), sv.get("rstd" + norm))
+
+    def branch_add(self, p, norm, o, x_res, out, mean, rstd):
+        """The residual add of a stored branch output o (sandwich LayerNorm or LayerScale) of layer prefix p and branch
+        norm: out = x_res + v with v = o, or with the sandwich LayerNorm LN<norm>(o) (its statistics into mean / rstd),
+        times s<norm> under LayerScale; one rounding.  The decoder's step runs it too."""
+        s = self.P(f"{p}ls{norm}") if self.layer_scale is not None else None
+        if not self.sandwich_norm:
+            return ops.layer_scale_residual_fwd(o, x_res, s, out)
+        g, b = self.P(f"{p}ln{norm}_g"), self.P(f"{p}ln{norm}_b")
+        if s is None:
+            return ops.layernorm_residual_fwd(o, x_res, g, b, out, mean, rstd, self.ln_eps)
+        return ops.layernorm_scale_residual_fwd(o, x_res, g, b, s, out, mean, rstd, self.ln_eps)
 
     def _block_fwd(self, i, x_in, x_out, sv, B, S=None):
         """DALLE.block (src/dalle_mtf/models.py:326-335): x += drop(attn(LN1 x)); x += drop(mlp(LN2 x)); with the
@@ -1089,8 +1206,7 @@ class DalleEngine:
         for i in range(self.L):
             sv = bufs["layers"][0 if self.recompute_grad else i]
             self._block_fwd(i, bufs["xs"][i], bufs["xs"][i + 1], sv, B)
-        ops.layernorm_fwd(bufs["xs"][self.L], self.P("lnf_g"), self.P("lnf_b"), bufs["hf"], bufs["meanf"],
-                          bufs["rstdf"], self.ln_eps)                                            # models.py:393
+        self.final_ln(bufs["xs"][self.L], bufs["hf"], bufs["meanf"], bufs["rstdf"], bufs["mf"])  # models.py:393
         ops.shift_labels(tokens, bufs["labels"], self.eos_token_id)                                # models.py:407-410
         labels = bufs["labels"].view(T)
         if self.logits_mask:
@@ -1110,6 +1226,13 @@ class DalleEngine:
         ops.ce_finish(bufs["part_max"], bufs["part_sum"], bufs["label_logit"], bufs["lse_v"], bufs["loss_rows"],
                       loss_accum)
         return loss_accum
+
+    def final_ln(self, x, hf, mean, rstd, m):
+        """hf = LN_f(x) (statistics into mean / rstd); with `stable` LN_f(x / max(x)) per row, the maxima into m.  The
+        prefill and the decoder's step run it too."""
+        if self.stable:
+            return ops.layernorm_divmax_fwd(x, self.P("lnf_g"), self.P("lnf_b"), hf, mean, rstd, m, self.ln_eps)
+        return ops.layernorm_fwd(x, self.P("lnf_g"), self.P("lnf_b"), hf, mean, rstd, self.ln_eps)
 
     # ------------------------------------------------------------------------------------------ logits mask
     def _mask_windows(self):
@@ -1208,13 +1331,13 @@ class DalleEngine:
                    "mean2": e(T, dtype=F32), "rstd2": e(T, dtype=F32), "h1": e(T, 4 * d),
                    # token shift: both unshifted LayerNorm outputs stay until the layer's caches are filled
                    **({"ln1_raw": e(T, d), "ln2_raw": e(T, d)} if self.shift_tokens else {}),
-                   # sandwich LayerNorm: the branch outputs and their LayerNorms' statistics
-                   **({"oa": e(T, d), "om": e(T, d), "meana": e(T, dtype=F32), "rstda": e(T, dtype=F32),
-                       "meanm": e(T, dtype=F32), "rstdm": e(T, dtype=F32)} if self.sandwich_norm else {}),
+                   # sandwich LayerNorm or LayerScale: the branch outputs (and their LayerNorms' statistics)
+                   **self._branch_bufs(T, e),
                    # gMLP layers: their activations without what only a backward reads
                    **(self._gmlp_bufs(T, e, train=False) if any(self.mlp) else {})},
             "x_last": e(B * rep, d), "hf": e(B * rep, d), "meanf": e(B * rep, dtype=F32),
             "rstdf": e(B * rep, dtype=F32), "logits": e(B * rep, self.Vpad, dtype=F32),
+            "mf": e(B * rep, dtype=F32) if self.stable else None,
         }
         self._pf_key = key
         return self._pf
@@ -1271,16 +1394,20 @@ class DalleEngine:
         finally:
             self._drop = drop
         ops.rows_repeat(x_in.view(B, P, d)[:, P - 1], b["x_last"], rep)
-        ops.layernorm_fwd(b["x_last"], self.P("lnf_g"), self.P("lnf_b"), b["hf"], b["meanf"], b["rstdf"], self.ln_eps)
+        self.final_ln(b["x_last"], b["hf"], b["meanf"], b["rstdf"], b["mf"])
         ops.gemm(b["hf"], self.W("wout"), b["logits"], B * rep, self.Vpad, d, a_mn=False, b_mn=True,
                  bias=self.P("bout"))
         return b["logits"]
 
     # ------------------------------------------------------------------------------------------ backward
-    def _ln_bwd(self, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, site):
+    def _ln_bwd(self, dy, x, g, mean, rstd, dres, dx, dg, db, dxsum, site, m=None):
         """LayerNorm backward; when `site` (the residual-dropout site of the branch whose output x sums) is active it
         also writes bufs["dxm"] = dx * keep * scale, and dxsum is colsum(dxm).  Returns the gradient of that branch
-        output (dxm, or dx without dropout)."""
+        output (dxm, or dx without dropout).  m: the rows' maxima of a DivideMax LayerNorm (final_ln with `stable`)."""
+        if m is not None:
+            dxm = None if site is None else self._bufs["dxm"]
+            ops.layernorm_divmax_bwd(dy, x, g, mean, rstd, m, dres, dx, dg, db, dxsum=dxsum, dxm=dxm, dropout=site)
+            return dx if dxm is None else dxm
         if site is None:
             ops.layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=dxsum)
             return dx
@@ -1300,16 +1427,16 @@ class DalleEngine:
         dbranch: gradient of the MLP output before its residual dropout (dx_out itself without dropout).  Returns the
         same for the layer below.
 
-        Sandwich LayerNorm: the branch gradients are the backward of LNm on dx_out and of LNa on dx_mid (without a
-        residual term, their dropout and the b2 / o_b column sums fused), so dbranch and dxsum_below are None and the
-        LayerNorms that produce dx_mid and dx_in fuse neither.  dx_in may be dx_out's storage: LNa's gradient goes
-        there once dx_out is consumed, and LN1's backward overwrites it last."""
+        Sandwich LayerNorm or LayerScale (split_branch): the branch gradients come from _branch_bwd on dx_out and on
+        dx_mid, which fuses their dropout and the b2 / o_b column sums, so dbranch and dxsum_below are None and the
+        LayerNorms that produce dx_mid and dx_in fuse neither.  dx_in may be dx_out's storage: the token mixer's branch
+        gradient goes there once dx_out is consumed, and LN1's backward overwrites it last."""
         p = f"l{i}."
-        sand = self.sandwich_norm
+        split = self.split_branch
         ob = p + ("gm_bout" if self._is_mlp(i) else "o_b")   # the token mixer's output bias
-        if sand:   # d om = LNm'(dx_out); dbranch = d om * keep * scale, db2 = colsum(dbranch)
-            dbranch = self._ln_bwd(dx_out, sv["om"], self.P(p + "lnm_g"), sv["meanm"], sv["rstdm"], None, bufs["dtmp"],
-                                   self.G(p + "lnm_g"), self.G(p + "lnm_b"), self.G(p + "b2"), self._site("mlp_out", i))
+        if split:   # dbranch = d om * keep * scale, db2 = colsum(dbranch)
+            dbranch = self._branch_bwd(p, "m", dx_out, sv, bufs, bufs["dtmp"], self.G(p + "b2"),
+                                       self._site("mlp_out", i))
         # ---- MLP
         dz = bufs["dz1"] if self.gated_mlp else bufs["dh1"]   # the gradient of W1's output
         if self.gated_mlp:   # dh = dx W2^T -> dz1 = [dh a | dh act'(zg) zv]; db1 = colsum(dz1)
@@ -1325,11 +1452,10 @@ class DalleEngine:
         dln = self._shift_bwd(bufs["dtmp"], sv["ln2_raw"]) if self.shift_tokens else bufs["dtmp"]
         dx_mid = bufs["dx_b"] if dx_out is bufs["dx_a"] else bufs["dx_a"]
         da = self._ln_bwd(dln, sv["xmid"], self.P(p + "ln2_g"), sv["mean2"], sv["rstd2"], dx_out, dx_mid,
-                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), None if sand else self.G(ob),
-                          None if sand else self._site("attn_out", i))                  # do_b = colsum(da)
-        if sand:   # d oa = LNa'(dx_mid); da = d oa * keep * scale, do_b = colsum(da)
-            da = self._ln_bwd(dx_mid, sv["oa"], self.P(p + "lna_g"), sv["meana"], sv["rstda"], None, dx_in,
-                              self.G(p + "lna_g"), self.G(p + "lna_b"), self.G(ob), self._site("attn_out", i))
+                          self.G(p + "ln2_g"), self.G(p + "ln2_b"), None if split else self.G(ob),
+                          None if split else self._site("attn_out", i))                 # do_b = colsum(da)
+        if split:   # da = d oa * keep * scale, do_b = colsum(da)
+            da = self._branch_bwd(p, "a", dx_mid, sv, bufs, dx_in, self.G(ob), self._site("attn_out", i))
         if self._is_mlp(i):   # ---- gMLP token mixing
             self._gmlp_bwd(p, sv, da, bufs, B)
         else:             # ---- attention
@@ -1345,7 +1471,24 @@ class DalleEngine:
         dln = self._shift_bwd(bufs["dtmp"], sv["ln1_raw"]) if self.shift_tokens else bufs["dtmp"]
         return self._ln_bwd(dln, x_in, self.P(p + "ln1_g"), sv["mean1"], sv["rstd1"], dx_mid, dx_in,
                             self.G(p + "ln1_g"), self.G(p + "ln1_b"), dxsum_below,
-                            self._site("mlp_out", i - 1) if i > 0 and not sand else None)   # db2 of the layer below
+                            self._site("mlp_out", i - 1) if i > 0 and not split else None)   # db2 of the layer below
+
+    def _branch_bwd(self, p, norm, dy, sv, bufs, out, dbias, site):
+        """The gradient of branch output o<norm> of layer prefix p before its residual dropout `site`, from dy, the
+        gradient of the residual sum it was added to: into `out` (bufs["dxm"] with dropout under the sandwich
+        LayerNorm), with dbias += its column sum.  LayerScale: d(s<norm>) += colsum(dy v) and the scaled gradient is
+        s dy; with the sandwich LayerNorm that goes through a [T, d] prefix of bufs["dh1"] (free until the MLP's
+        dgrad writes it) into LN<norm>'s backward."""
+        if self.layer_scale is not None:
+            s, ds = self.P(f"{p}ls{norm}"), self.G(f"{p}ls{norm}")
+            if not self.sandwich_norm:
+                return ops.layer_scale_bwd(dy, sv["o" + norm], s, out, ds, db=dbias, dropout=site)
+            dv = bufs["dh1"].view(-1)[:dy.numel()].view(dy.shape)
+            ops.layer_scale_bwd(dy, sv["o" + norm], s, dv, ds, norm=(self.P(f"{p}ln{norm}_g"), self.P(f"{p}ln{norm}_b"),
+                                                                     sv["mean" + norm], sv["rstd" + norm]))
+            dy = dv
+        return self._ln_bwd(dy, sv["o" + norm], self.P(f"{p}ln{norm}_g"), sv["mean" + norm], sv["rstd" + norm], None,
+                            out, self.G(f"{p}ln{norm}_g"), self.G(f"{p}ln{norm}_b"), dbias, site)
 
     def _gmlp_bwd(self, p, sv, da, bufs, B):
         """Backward of a gMLP layer's token mixing from da, the gradient of the branch output before its bias: into
@@ -1388,10 +1531,11 @@ class DalleEngine:
             ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
             ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
         dx = bufs["dx_a"]
-        sand = self.sandwich_norm   # the sandwich LayerNorm's backward fuses db2 and the mlp_out dropout instead
+        split = self.split_branch   # the branch's own backward fuses db2 and the mlp_out dropout instead
         dbranch = self._ln_bwd(bufs["dtmp"], bufs["xs"][self.L], self.P("lnf_g"), bufs["meanf"], bufs["rstdf"], None,
-                               dx, self.G("lnf_g"), self.G("lnf_b"), None if sand else self.G(f"l{self.L - 1}.b2"),
-                               None if sand else self._site("mlp_out", self.L - 1))     # db2 of the last block
+                               dx, self.G("lnf_g"), self.G("lnf_b"), None if split else self.G(f"l{self.L - 1}.b2"),
+                               None if split else self._site("mlp_out", self.L - 1),    # db2 of the last block
+                               bufs["mf"])
         if on_bucket_ready:
             s, e = self.layout.span("lnf_g", "bout")
             on_bucket_ready(s, e + 64)  # + the aux scalars (loss) that sit behind the last parameter
@@ -1404,18 +1548,19 @@ class DalleEngine:
             # dx (grad w.r.t. the block output) is dead once dx_mid has been formed in the other buffer, so the
             # block's input gradient is written back into the same storage.
             dbranch = self._block_bwd(i, bufs["xs"][i], sv, dx, dx, bufs, B,
-                                      self.G(f"l{i - 1}.b2") if i > 0 and not sand else None, dbranch)
+                                      self.G(f"l{i - 1}.b2") if i > 0 and not split else None, dbranch)
             if on_bucket_ready:
-                s, e = self.layout.span(f"l{i}.ln1_g", f"l{i}.lnm_b" if sand else f"l{i}.b2")
+                s, e = self.layout.span(f"l{i}.ln1_g", self.layer_last(i))
                 on_bucket_ready(s, e)
         # row / column positions: the gradient of the composed table goes into a zeroed scratch, then is folded into
         # wpe, image_row and image_col (one fully formed contribution per call, like the wpe gradient itself)
         dpos = self._dpos.zero_() if self.row_col else self.G("wpe")
+        alpha = {"alpha": STABLE_ALPHA} if self.stable else {}   # pos_fold is linear: it carries the shrink along
         if self._drop is not None:
             ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos, wte_drop=self._drop["wte"],
-                          wpe_drop=self._drop["wpe"])
+                          wpe_drop=self._drop["wpe"], **alpha)
         else:
-            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos)
+            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos, **alpha)
         if self.row_col:
             ops.pos_fold(dpos, self.G("wpe"), self.G("image_row"), self.G("image_col"))
         if on_bucket_ready:

@@ -119,6 +119,15 @@ _SIGNATURES = {
     "db200_shift_labels": [c_vp, c_vp, c_vp, c_int, c_int, c_int],
     "db200_layernorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
     "db200_layernorm_residual_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
+    "db200_layernorm_scale_residual_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
+    "db200_layer_scale_residual_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int],
+    "db200_layernorm_divmax_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
+    "db200_layernorm_divmax_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
+                                   c_int, c_vp, c_vp, c_i64],
+    "db200_embed_bwd_scaled": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64, c_vp, c_vp,
+                               c_f32],
+    "db200_layer_scale_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int,
+                              c_vp, c_i64],
     "db200_layernorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp, c_i64],
     "db200_layernorm_bwd_ex": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_vp,
                                c_i64],
@@ -254,6 +263,7 @@ _SIGNATURES = {
 _WORKSPACE_QUERIES = {
     "db200_gemm_workspace_bytes": [c_int, c_int, c_int, ctypes.POINTER(GemmEpilogue)],
     "db200_layernorm_bwd_workspace_bytes": [c_int, c_int],
+    "db200_layer_scale_bwd_workspace_bytes": [c_int, c_int],
     "db200_colsum_workspace_bytes": [c_int, c_int],
     "db200_sqnorm_workspace_bytes": [c_sz],
     "db200_ce_finish_workspace_bytes": [c_int],

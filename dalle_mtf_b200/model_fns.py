@@ -16,7 +16,7 @@ from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
     validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
-    validate_rotary, validate_sandwich_norm, validate_shift_tokens
+    validate_layer_scale, validate_rotary, validate_sandwich_norm, validate_shift_tokens, validate_stable
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -178,6 +178,27 @@ def sandwich_norm(params):
     return validate_sandwich_norm(v)
 
 
+def layer_scale(params):
+    """layer_scale of a DALL-E config: absent, null or false is off (None); true is DALLE-pytorch's LayerScale with its
+    initial values by depth (dalle_engine.layer_scale_init); a finite number > 0 is LayerScale starting at that value
+    in every layer.  Either adds the variables layer_i/attn/layer_scale (layer_i/gmlp/layer_scale in an 'mlp' layer)
+    and layer_i/mlp/layer_scale.  true is never read as the number 1; 0, negative, non-finite, string or list values
+    are rejected."""
+    return validate_layer_scale(params.get("layer_scale"))
+
+
+def stable(params):
+    """stable of a DALL-E config: absent, null or false is off; true is DALLE-pytorch's stable option (DalleEngine):
+    the embedding gradients shrink by 0.1 and the final LayerNorm sees each row divided by its maximum.  It adds no
+    variable.  Only a JSON bool is accepted: 1, "true" or a list is rejected."""
+    v = params.get("stable")
+    if v is None:
+        return False
+    if not isinstance(v, bool):
+        raise ValueError(f"stable = {v!r}: expected null, true or false")
+    return validate_stable(v)
+
+
 def shift_tokens(params, image_seq_len=None):
     """shift_tokens of a DALL-E config: absent, null or false is off; true turns on DALLE-pytorch's token shift after
     both LayerNorms of every layer (DalleEngine), which needs a square image-token grid (checked here when
@@ -285,6 +306,8 @@ def dalle_model_fn(features, labels, mode, params):
     gated = gated_mlp(params)
     shift = shift_tokens(params)
     sandwich = sandwich_norm(params)
+    scale = layer_scale(params)
+    stab = stable(params)
     mask = logits_mask(params)
     rotary_dim, rotary_base = rotary_embedding(params)
     L.require_device()
@@ -321,7 +344,8 @@ def dalle_model_fn(features, labels, mode, params):
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
                         activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
-                        gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich)
+                        gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich, layer_scale=scale,
+                        stable=stab)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

@@ -279,13 +279,19 @@ def embed_fwd(ids, wte, wpe, out, wte_drop=None, wpe_drop=None):
     return out
 
 
-def embed_bwd(ids, dx, dwte, dwpe, wte_drop=None, wpe_drop=None):
+def embed_bwd(ids, dx, dwte, dwpe, wte_drop=None, wpe_drop=None, alpha=None):
+    """alpha (the stable option's gradient shrink, None: off): every dx element is multiplied by alpha in fp32 before
+    it is summed into dwte / dwpe."""
     L.require_device()
     _chk(ids, I32, "ids"); _chk(dx, BF16, "dx"); _chk(dwte, F32, "dwte"); _chk(dwpe, F32, "dwpe")
     B, S = ids.shape
     V, d = dwte.shape
     ws = L.workspace(L.load().db200_embed_bwd_workspace_bytes(d, V))
-    if wte_drop is None and wpe_drop is None:
+    if alpha is not None:
+        check(L.load().db200_embed_bwd_scaled(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V,
+                                              ptr(ws), _nbytes(ws), _ref(wte_drop), _ref(wpe_drop), float(alpha)),
+              "embed_bwd_scaled")
+    elif wte_drop is None and wpe_drop is None:
         check(L.load().db200_embed_bwd(stream_ptr(), ptr(ids), ptr(dx), ptr(dwte), ptr(dwpe), B, S, d, V, ptr(ws),
                                        _nbytes(ws)), "embed_bwd")
     else:
@@ -387,6 +393,100 @@ def layernorm_residual_fwd(o, x_res, g, b, y, mean, rstd, eps=1e-5):
     check(L.load().db200_layernorm_residual_fwd(stream_ptr(), ptr(o), ptr(x_res), ptr(g), ptr(b), ptr(y), ptr(mean),
                                                 ptr(rstd), rows, d, eps), "layernorm_residual_fwd")
     return y
+
+
+def _rows_like(what, rows, d, *tensors):
+    for t in tensors:
+        if t is not None and (tuple(t.shape) != (rows, d) or not t.is_contiguous()):
+            raise L.DB200Error(f"{what}: every [rows, d] operand must be contiguous [{rows}, {d}]")
+
+
+def layernorm_scale_residual_fwd(o, x_res, g, b, s, y, mean, rstd, eps=1e-5):
+    """Sandwich LayerNorm under LayerScale: y = bf16(x_res + s * (LN(o) * g + b)) with LN's statistics of o into mean /
+    rstd (fp32), the same values layernorm_fwd writes."""
+    L.require_device()
+    _chk(o, BF16, "o"); _chk(x_res, BF16, "x_res"); _chk(y, BF16, "y"); _chk(g, F32, "g"); _chk(b, F32, "b")
+    _chk(s, F32, "s"); _chk(mean, F32, "mean"); _chk(rstd, F32, "rstd")
+    rows, d = o.shape
+    _rows_like("layernorm_scale_residual_fwd", rows, d, o, x_res, y)
+    if mean.numel() < rows or rstd.numel() < rows or g.numel() != d or b.numel() != d or s.numel() != d:
+        raise L.DB200Error(f"layernorm_scale_residual_fwd: g, b and s must have {d} entries, mean and rstd >= {rows}")
+    check(L.load().db200_layernorm_scale_residual_fwd(stream_ptr(), ptr(o), ptr(x_res), ptr(g), ptr(b), ptr(s), ptr(y),
+                                                      ptr(mean), ptr(rstd), rows, d, eps),
+          "layernorm_scale_residual_fwd")
+    return y
+
+
+def layernorm_divmax_fwd(x, g, b, y, mean, rstd, m, eps=1e-5):
+    """DivideMax LayerNorm: per row m = max(x) (into m), u = x / m in fp32, y = bf16(LN(u) g + b) with u's statistics
+    into mean / rstd."""
+    L.require_device()
+    _chk(x, BF16, "x"); _chk(y, BF16, "y"); _chk(g, F32, "g"); _chk(b, F32, "b"); _chk(mean, F32, "mean")
+    _chk(rstd, F32, "rstd"); _chk(m, F32, "m")
+    rows, d = x.shape
+    _rows_like("layernorm_divmax_fwd", rows, d, x, y)
+    if min(mean.numel(), rstd.numel(), m.numel()) < rows or g.numel() != d or b.numel() != d:
+        raise L.DB200Error(f"layernorm_divmax_fwd: g and b must have {d} entries, mean, rstd and m >= {rows}")
+    check(L.load().db200_layernorm_divmax_fwd(stream_ptr(), ptr(x), ptr(g), ptr(b), ptr(y), ptr(mean), ptr(rstd),
+                                              ptr(m), rows, d, eps), "layernorm_divmax_fwd")
+    return y
+
+
+def layernorm_divmax_bwd(dy, x, g, mean, rstd, m, dres, dx, dg, db, dxsum=None, dxm=None, dropout=None):
+    """Backward of layernorm_divmax_fwd with m constant: dx = LN'(x / m)^T dy / m (+ dres); dg, db, and the fusions of
+    layernorm_bwd (dxsum; dxm and the dropout site)."""
+    L.require_device()
+    _chk(dy, BF16, "dy"); _chk(x, BF16, "x"); _chk(dres, BF16, "dres"); _chk(dx, BF16, "dx"); _chk(m, F32, "m")
+    _chk(g, F32, "g"); _chk(dg, F32, "dg"); _chk(db, F32, "db"); _chk(dxsum, F32, "dxsum"); _chk(dxm, BF16, "dxm")
+    _chk(mean, F32, "mean"); _chk(rstd, F32, "rstd")
+    rows, d = x.shape
+    _rows_like("layernorm_divmax_bwd", rows, d, dy, x, dres, dx, dxm)
+    if min(mean.numel(), rstd.numel(), m.numel()) < rows or g.numel() != d or dg.numel() != d or db.numel() != d \
+            or (dxsum is not None and dxsum.numel() != d):
+        raise L.DB200Error(f"layernorm_divmax_bwd: mean, rstd and m must have >= {rows} entries, g, dg, db and dxsum "
+                           f"{d}")
+    ws = L.workspace(L.load().db200_layernorm_bwd_workspace_bytes(rows, d))
+    check(L.load().db200_layernorm_divmax_bwd(stream_ptr(), ptr(dy), ptr(x), ptr(g), ptr(mean), ptr(rstd), ptr(m),
+                                              ptr(dres), ptr(dx), ptr(dxm), ptr(dg), ptr(db), ptr(dxsum), rows, d,
+                                              _ref(dropout), ptr(ws), _nbytes(ws)), "layernorm_divmax_bwd")
+    return dx
+
+
+def layer_scale_residual_fwd(o, x_res, s, y):
+    """LayerScale: y = bf16(x_res + s * o), s fp32 [d] per channel."""
+    L.require_device()
+    _chk(o, BF16, "o"); _chk(x_res, BF16, "x_res"); _chk(y, BF16, "y"); _chk(s, F32, "s")
+    rows, d = o.shape
+    _rows_like("layer_scale_residual_fwd", rows, d, o, x_res, y)
+    if s.numel() != d:
+        raise L.DB200Error(f"layer_scale_residual_fwd: s must have {d} entries")
+    check(L.load().db200_layer_scale_residual_fwd(stream_ptr(), ptr(o), ptr(x_res), ptr(s), ptr(y), rows, d),
+          "layer_scale_residual_fwd")
+    return y
+
+
+def layer_scale_bwd(dy, v, s, dv, ds, db=None, dropout=None, norm=None):
+    """LayerScale backward from the residual gradient dy: dv = bf16(s * dy) (times the keep mask and scale of the
+    residual-dropout site `dropout`), ds += colsum(dy * v), db (optional) += colsum(dv).  norm = (g, b, mean, rstd):
+    v is a sandwich LayerNorm's input o and the scaled value is LN(o) * g + b, recomputed in fp32 (no dropout then)."""
+    L.require_device()
+    _chk(dy, BF16, "dy"); _chk(v, BF16, "v"); _chk(dv, BF16, "dv"); _chk(s, F32, "s"); _chk(ds, F32, "ds")
+    _chk(db, F32, "db")
+    rows, d = v.shape
+    _rows_like("layer_scale_bwd", rows, d, dy, v, dv)
+    g = b = mean = rstd = None
+    if norm is not None:
+        g, b, mean, rstd = norm
+        _chk(g, F32, "g"); _chk(b, F32, "b"); _chk(mean, F32, "mean"); _chk(rstd, F32, "rstd")
+        if g.numel() != d or b.numel() != d or mean.numel() < rows or rstd.numel() < rows:
+            raise L.DB200Error(f"layer_scale_bwd: g and b must have {d} entries, mean and rstd >= {rows}")
+    if s.numel() != d or ds.numel() != d or (db is not None and db.numel() != d):
+        raise L.DB200Error(f"layer_scale_bwd: s, ds and db must have {d} entries")
+    ws = L.workspace(L.load().db200_layer_scale_bwd_workspace_bytes(rows, d))
+    check(L.load().db200_layer_scale_bwd(stream_ptr(), ptr(dy), ptr(v), ptr(s), ptr(g), ptr(b), ptr(mean), ptr(rstd),
+                                         ptr(dv), ptr(ds), ptr(db), _ref(dropout), rows, d, ptr(ws), _nbytes(ws)),
+          "layer_scale_bwd")
+    return dv
 
 
 def layernorm_bwd(dy, x, g, mean, rstd, dres, dx, dg, db, dxsum=None, dxm=None, dropout=None):

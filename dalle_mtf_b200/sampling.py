@@ -15,8 +15,10 @@ parameters and the same kernels' numerics as training:
                     rotated to position p (rope_decode) before k enters the cache; with the token shift each
                     LayerNorm output's first d/2 columns enter a per-layer cache and are replaced by the shifted
                     chunks of positions p - 1 and p - W (shift_tokens_decode); with the sandwich LayerNorm each
-                    branch output is normalised before its residual add (layernorm_residual_fwd)
-  logits = LN_f(x) Wout + bout (fp32); next token = argmax over the allowed id range of logits / T + Gumbel noise
+                    branch output is normalised before its residual add (layernorm_residual_fwd); with LayerScale
+                    what a branch adds is multiplied by its per-channel scale (DalleEngine.branch_add)
+  logits = LN_f(x) Wout + bout (fp32), with the stable option LN_f(x / max(x)) (DalleEngine.final_ln);
+  next token = argmax over the allowed id range of logits / T + Gumbel noise
 
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
 instead runs the whole prompt (text, optionally followed by the first rows of an image's codes) through the training
@@ -95,21 +97,22 @@ class DalleSampler:
         self.att = mk(B, d)
         self.xmid = mk(B, d)
         self.h1 = mk(B, 4 * d)
-        self.ob = mk(B, d) if e.sandwich_norm else None   # sandwich LayerNorm: a branch output before its LayerNorm
+        self.ob = mk(B, d) if e.split_branch else None    # sandwich LayerNorm / LayerScale: a branch output
         self.mean, self.rstd = mk(B, dtype=F32), mk(B, dtype=F32)
+        self.mf = mk(B, dtype=F32) if e.stable else None   # stable: the DivideMax row maxima of the final LayerNorm
         self.logit = mk(B, e.Vpad, dtype=F32)
         self.tok = mk(B, dtype=I32)
         self._B = B
 
     def _branch_out(self, p, norm, x, w, bias, x_res, out):
         """out = x_res + x w + bias, or with the sandwich LayerNorm out = x_res + LN<norm>(x w + bias) (norm "a": the
-        attention branch's LayerNorm, "m": the MLP's)."""
+        attention branch's LayerNorm, "m": the MLP's), what is added times s<norm> under LayerScale
+        (DalleEngine.branch_add)."""
         e = self.e
-        if not e.sandwich_norm:
+        if not e.split_branch:
             return ops.linear_fwd(x, w, out, bias=bias, residual=x_res)
         ops.linear_fwd(x, w, self.ob, bias=bias)
-        ops.layernorm_residual_fwd(self.ob, x_res, e.P(f"{p}ln{norm}_g"), e.P(f"{p}ln{norm}_b"), out, self.mean,
-                                   self.rstd, e.ln_eps)
+        e.branch_add(p, norm, self.ob, x_res, out, self.mean, self.rstd)
 
     def _gmlp_step(self, p, i, pos=None, pos_dev=None):
         """A gMLP layer's token mixing for one position of every row, from self.ln into self.g_h: the training
@@ -152,7 +155,7 @@ class DalleSampler:
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
-        ops.layernorm_fwd(x_in, e.P("lnf_g"), e.P("lnf_b"), self.ln, self.mean, self.rstd, e.ln_eps)
+        e.final_ln(x_in, self.ln, self.mean, self.rstd, self.mf)
         B = tokens_b.shape[0]
         ops.gemm(self.ln, e.W("wout"), self.logit, B, e.Vpad, e.d, a_mn=False, b_mn=True, bias=e.P("bout"))
         return self.logit
@@ -184,7 +187,7 @@ class DalleSampler:
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
-        ops.layernorm_fwd(x_in, e.P("lnf_g"), e.P("lnf_b"), self.ln, self.mean, self.rstd, e.ln_eps)
+        e.final_ln(x_in, self.ln, self.mean, self.rstd, self.mf)
         ops.gemm(self.ln, e.W("wout"), self.logit, tokens.shape[0], e.Vpad, e.d, a_mn=False, b_mn=True, bias=e.P("bout"))
         return self.logit
 

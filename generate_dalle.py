@@ -19,7 +19,8 @@ import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
 from dalle_mtf_b200.model_fns import activation_function, attention_layers, conv_kernel, gated_mlp, \
-    input_embedding, logits_mask, rotary_embedding, sandwich_norm, shift_tokens, vae_checkpoint, vae_grid_size
+    input_embedding, layer_scale, logits_mask, rotary_embedding, sandwich_norm, shift_tokens, stable, \
+    vae_checkpoint, vae_grid_size
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
 PADDING_ID = 50257   # GPT-2 vocabulary + <|padding|> (src/data/tokenizer_utils.py), what training pads captions with
@@ -157,6 +158,8 @@ def main(argv=None):
     gated = gated_mlp(params)                           # and whether that MLP is gated
     shift = shift_tokens(params)                        # and whether its LayerNorm outputs are token-shifted
     sandwich = sandwich_norm(params)                    # and whether its branch outputs are normalised
+    scale = layer_scale(params)                         # and whether they are LayerScaled
+    stab = stable(params)                               # and whether its final LayerNorm divides by the row maximum
     mask = logits_mask(params)                         # and its objective (sampling draws image ids either way)
     rotary_dim, rotary_base = rotary_embedding(params)  # and its rotary position embeddings
     # with per-position padding the captions are padded with the config's padding_id, which the sampler maps to the
@@ -198,7 +201,8 @@ def main(argv=None):
                       device=device, attention_types=attention_types, local_attention_radius=local_radius,
                       conv_attention_kernel=conv_k, image_position_embedding=pos_scheme,
                       per_position_padding=per_pos, activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
-                      rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich)
+                      rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich,
+                      layer_scale=scale, stable=stab)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})

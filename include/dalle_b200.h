@@ -97,6 +97,12 @@ int db200_embed_fwd_ex(db200_stream_t stream, const int32_t* ids, const void* wt
 int db200_embed_bwd_ex(db200_stream_t stream, const int32_t* ids, const void* dx_bf16, float* dwte, float* dwpe, int B,
                        int S, int d, int V, void* workspace, int64_t workspace_bytes, const db200_dropout* wte_drop,
                        const db200_dropout* wpe_drop);
+/* same, with every dx element multiplied by alpha in fp32 (rounded on its own) before it is summed: the embedding
+ * gradient shrink of the `stable` option, tokens * alpha + tokens.detach() * (1 - alpha), whose forward is
+ * unchanged. */
+int db200_embed_bwd_scaled(db200_stream_t stream, const int32_t* ids, const void* dx_bf16, float* dwte, float* dwpe,
+                           int B, int S, int d, int V, void* workspace, int64_t workspace_bytes,
+                           const db200_dropout* wte_drop_or_null, const db200_dropout* wpe_drop_or_null, float alpha);
 
 /* T0 token assembly: tokens[b] = concat(text_ids[b], image_idx[b] + image_offset).  Replaces tf.concat at
  * src/model_fns.py:117-122 (image_offset = text_vocab_size). */
@@ -163,6 +169,46 @@ int db200_layernorm_bwd_dropout(db200_stream_t stream, const void* dy_bf16, cons
                                 const float* mean, const float* rstd, const void* dres_bf16_or_null, void* dx_bf16,
                                 void* dxm_bf16, float* dg, float* db, float* dxsum_or_null, int rows, int d,
                                 const db200_dropout* drop, void* workspace, int64_t workspace_bytes);
+/* LayerScale (DALLE-pytorch's LayerScale around every branch): the branch output o is scaled per channel by s before
+ * the residual add,
+ *     y = bf16(x + s[c] * o)                               (fp32, one rounding)
+ * any rows > 0, d % 8 == 0, 16-byte aligned operands. */
+int db200_layer_scale_residual_fwd(db200_stream_t stream, const void* o_bf16, const void* x_res_bf16, const float* s,
+                                   void* y_bf16, int rows, int d);
+/* LayerScale on a sandwich LayerNorm's output:
+ *     y = bf16(x + s[c] * ((o - mean) * rstd * g + b))       (fp32, one rounding)
+ * with mean / rstd of o from the same instructions as db200_layernorm_fwd's.  Same d as db200_layernorm_fwd. */
+int db200_layernorm_scale_residual_fwd(db200_stream_t stream, const void* o_bf16, const void* x_res_bf16,
+                                       const float* g, const float* b, const float* s, void* y_bf16, float* mean,
+                                       float* rstd, int rows, int d, float eps);
+/* LayerScale backward from the residual gradient dy and the branch value v the scale multiplied:
+ *     dv[r][c]  = bf16(s[c] * dy[r][c] * keep * scale)     (keep * scale: the mask of `drop`, NULL or inactive: 1)
+ *     ds[c]    += sum_r dy[r][c] * v[r][c]                 (fp32)
+ *     db[c]    += sum_r dv[r][c]                           (the stored bf16 values; db may be NULL)
+ * v is the bf16 branch output, or with g != NULL the sandwich LayerNorm output recomputed in fp32 from the stored o,
+ * v = (o - mean[r]) * rstd[r] * g[c] + b[c] (b, mean and rstd then required; `drop` must be NULL or inactive, the
+ * LayerNorm backward applies it).  Sums go through per-block partial rows of the workspace, added in a fixed order:
+ * the result is bit-reproducible.  d % 256 == 0. */
+int db200_layer_scale_bwd(db200_stream_t stream, const void* dy_bf16, const void* v_bf16, const float* s,
+                          const float* g_or_null, const float* b_or_null, const float* mean_or_null,
+                          const float* rstd_or_null, void* dv_bf16, float* ds, float* db_or_null,
+                          const db200_dropout* drop_or_null, int rows, int d, void* workspace,
+                          int64_t workspace_bytes);
+int64_t db200_layer_scale_bwd_workspace_bytes(int rows, int d);
+/* DivideMax before a LayerNorm (the `stable` option's final LayerNorm): per row m = max_c x[c] over the bf16 values,
+ * u = x / m in fp32 (IEEE division, never rounded to bf16), y = bf16((u - mean) * rstd * g + b) with mean / rstd of u.
+ * Writes y, mean, rstd and m (fp32 [rows]).  m = 0 gives the non-finite values of the division.  Same d as
+ * db200_layernorm_fwd, any rows > 0. */
+int db200_layernorm_divmax_fwd(db200_stream_t stream, const void* x_bf16, const float* g, const float* b, void* y_bf16,
+                               float* mean, float* rstd, float* m, int rows, int d, float eps);
+/* its backward with m held constant: dx = LN'(u)^T dy / m (+ dres), dg / db / dxsum as db200_layernorm_bwd_ex; with an
+ * active `drop` also dxm = dx * keep * scale and dxsum sums dxm, as db200_layernorm_bwd_dropout.  Workspace:
+ * db200_layernorm_bwd_workspace_bytes(rows, d). */
+int db200_layernorm_divmax_bwd(db200_stream_t stream, const void* dy_bf16, const void* x_bf16, const float* g,
+                               const float* mean, const float* rstd, const float* m, const void* dres_bf16_or_null,
+                               void* dx_bf16, void* dxm_bf16_or_null, float* dg, float* db, float* dxsum_or_null,
+                               int rows, int d, const db200_dropout* drop_or_null, void* workspace,
+                               int64_t workspace_bytes);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * K3/K5/K6/K8  bf16 GEMM on wgmma (TMA-fed, register accumulators, fp32 accumulate):   D[M,N] = A[M,K] * B[K,N]

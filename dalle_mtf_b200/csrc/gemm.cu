@@ -763,9 +763,9 @@ static int gemm_run(db200_stream_t stream_, const void* A, int a_mn_major, int64
     rc = (p.a_mn || p.b_mn) ? set_error(DB200_E_UNSUPPORTED, "gemm_glu_bwd: needs k-major A and B")
          : gelu == G_GLU_GELU_BWD ? launch_gemm<0, 0, false, false, G_GLU_GELU_BWD>(stream, tmA, tmB, p)
                                   : launch_gemm<0, 0, false, false, G_GLU_RELU_BWD>(stream, tmA, tmB, p);
-  else if (cew)     // the vocabulary product: A k-major, B mn-major
-    rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, false, true>(stream, tmA, tmB, p)
-                             : set_error(DB200_E_UNSUPPORTED, "gemm: weighted CE_GRAD needs a k-major A and an mn-major B");
+  else if (cew)     // the vocabulary product: A k-major, B mn-major (wout) or k-major (a tied wte)
+    rc = p.a_mn ? set_error(DB200_E_UNSUPPORTED, "gemm: weighted CE_GRAD needs a k-major A (and a B of either major)")
+         : p.b_mn ? launch_gemm<0, 1, false, true>(stream, tmA, tmB, p) : launch_gemm<0, 0, false, true>(stream, tmA, tmB, p);
   else if (drop)    // residual dropout runs in forward products only: A k-major, B mn-major
     rc = (!p.a_mn && p.b_mn) ? launch_gemm<0, 1, true>(stream, tmA, tmB, p)
                              : set_error(DB200_E_UNSUPPORTED, "gemm: dropout needs a k-major A and an mn-major B");

@@ -29,11 +29,13 @@ def _round_up(x, m):
 
 
 class ParamLayout:
-    """name -> (offset, shape) inside the flat buffers.  Every offset is a multiple of 64 elements."""
+    """name -> (offset, shape) inside the flat buffers.  Every offset is a multiple of 64 elements.  An alias (a shared
+    module's name in a layer that does not own it) has its owner's entry but no place in `order` and no size."""
 
     def __init__(self):
         self.entries = {}
         self.order = []
+        self.aliases = {}
         self.size = 0
 
     def add(self, name, shape):
@@ -43,6 +45,11 @@ class ParamLayout:
         self.entries[name] = (self.size, tuple(shape))
         self.order.append(name)
         self.size += _round_up(n, 64)
+
+    def alias(self, name, owner):
+        """Make `name` a second name of the existing entry `owner` (same offset, same storage)."""
+        self.entries[name] = self.entries[owner]
+        self.aliases[name] = owner
 
     def view(self, flat, name):
         off, shape = self.entries[name]
@@ -61,8 +68,13 @@ class ParamLayout:
         return o0, o1 + _round_up(n, 64)
 
 
+ATTN_MODULE = ("wqkv", "wo", "o_b")                 # an attention layer's token mixer
+GMLP_MODULE = ("gm_win", "gm_bin", "sgu_g", "sgu_b", "sgu_w", "sgu_c", "gm_wout", "gm_bout")   # a gMLP layer's
+FF_MODULE = ("w1", "b1", "w2", "b2")                 # the MLP
+
+
 def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False, mlp_layers=None,
-                 layer_scale=False):
+                 layer_scale=False, tied=False, attn_owner=None, ff_owner=None):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
     length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
     column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
@@ -72,37 +84,54 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     mlp_layers: per layer, True for a gMLP token-mixing layer, whose gm_win [d, 4d], gm_bin [4d], sgu_g / sgu_b [2d],
     sgu_w [S, S], sgu_c [S], gm_wout [2d, d] and gm_bout [d] take the place of wqkv, wo and o_b.  layer_scale: each
     layer ends with its two LayerScale vectors, lsa (the token mixer's branch) and lsm (the MLP's), after the sandwich
-    LayerNorms."""
+    LayerNorms.
+    tied (share_input_output_emb): wte is [Vpad, d], its pad rows exactly zero, and is also the vocabulary projection;
+    there is no wout.  attn_owner / ff_owner (shared_attn_ids / shared_ff_ids): per layer, the layer whose token mixer
+    (ATTN_MODULE or GMLP_MODULE) / MLP (FF_MODULE) it uses.  A layer that is not its module's owner gets aliases of the
+    owner's entries, so that layer i's own entries still run contiguously from l{i}.ln1_g."""
     w1_cols = 8 * d if gated_mlp else 4 * d
     Vpad = _round_up(V, 64)
+    attn_owner = list(range(n_layers)) if attn_owner is None else attn_owner
+    ff_owner = list(range(n_layers)) if ff_owner is None else ff_owner
     lay = ParamLayout()
-    lay.add("wte", (V, d))
+    lay.add("wte", (Vpad if tied else V, d))
     if grid_w is None:
         lay.add("wpe", (S, d))
     else:
         lay.add("wpe", (text_len, d))
         lay.add("image_row", (grid_w, d)); lay.add("image_col", (grid_w, d))
+
+    def module(i, owner, names, add):
+        if owner[i] == i:
+            return add()
+        for k in names:
+            lay.alias(f"l{i}.{k}", f"l{owner[i]}.{k}")
+
     for i in range(n_layers):
         p = f"l{i}."
         lay.add(p + "ln1_g", (d,)); lay.add(p + "ln1_b", (d,))
         if mlp_layers is not None and mlp_layers[i]:
-            lay.add(p + "gm_win", (d, 4 * d)); lay.add(p + "gm_bin", (4 * d,))
-            lay.add(p + "sgu_g", (2 * d,)); lay.add(p + "sgu_b", (2 * d,))
-            lay.add(p + "sgu_w", (S, S)); lay.add(p + "sgu_c", (S,))
-            lay.add(p + "gm_wout", (2 * d, d)); lay.add(p + "gm_bout", (d,))
+            module(i, attn_owner, GMLP_MODULE, lambda: (
+                lay.add(p + "gm_win", (d, 4 * d)), lay.add(p + "gm_bin", (4 * d,)),
+                lay.add(p + "sgu_g", (2 * d,)), lay.add(p + "sgu_b", (2 * d,)),
+                lay.add(p + "sgu_w", (S, S)), lay.add(p + "sgu_c", (S,)),
+                lay.add(p + "gm_wout", (2 * d, d)), lay.add(p + "gm_bout", (d,))))
         else:
-            lay.add(p + "wqkv", (d, 3 * d))
-            lay.add(p + "wo", (d, d)); lay.add(p + "o_b", (d,))
+            module(i, attn_owner, ATTN_MODULE, lambda: (
+                lay.add(p + "wqkv", (d, 3 * d)), lay.add(p + "wo", (d, d)), lay.add(p + "o_b", (d,))))
         lay.add(p + "ln2_g", (d,)); lay.add(p + "ln2_b", (d,))
-        lay.add(p + "w1", (d, w1_cols)); lay.add(p + "b1", (w1_cols,))
-        lay.add(p + "w2", (4 * d, d)); lay.add(p + "b2", (d,))
+        module(i, ff_owner, FF_MODULE, lambda: (
+            lay.add(p + "w1", (d, w1_cols)), lay.add(p + "b1", (w1_cols,)),
+            lay.add(p + "w2", (4 * d, d)), lay.add(p + "b2", (d,))))
         if sandwich_norm:
             lay.add(p + "lna_g", (d,)); lay.add(p + "lna_b", (d,))
             lay.add(p + "lnm_g", (d,)); lay.add(p + "lnm_b", (d,))
         if layer_scale:
             lay.add(p + "lsa", (d,)); lay.add(p + "lsm", (d,))
     lay.add("lnf_g", (d,)); lay.add("lnf_b", (d,))
-    lay.add("wout", (d, Vpad)); lay.add("bout", (Vpad,))
+    if not tied:
+        lay.add("wout", (d, Vpad))
+    lay.add("bout", (Vpad,))
     return lay
 
 
@@ -365,6 +394,50 @@ def validate_stable(stable):
     return stable
 
 
+def validate_share_input_output_emb(value):
+    """share_input_output_emb: None or a bool (None: False); numbers, strings and other values are a ValueError."""
+    if value is None:
+        return False
+    if not isinstance(value, bool):
+        raise ValueError(f"share_input_output_emb must be a bool or None, got {value!r}")
+    return value
+
+
+def validate_shared_ids(ids, n_layers, name):
+    """shared_attn_ids / shared_ff_ids (`name`): None (every layer its own module) or a non-empty list of integers >= 0,
+    cycled to n_layers as DALLE-pytorch's cycle() does ([0, 1] at 6 layers: 0 1 0 1 0 1).  Returns the per-layer ids or
+    None.  Bools, non-integers, negative ids, an empty list and anything but a list or tuple are a ValueError."""
+    if ids is None:
+        return None
+    if not isinstance(ids, (list, tuple)) or not ids or any(not _count(v) or v < 0 for v in ids):
+        raise ValueError(f"{name} = {ids!r}: must be null or a non-empty list of integers >= 0")
+    return [int(ids[i % len(ids)]) for i in range(n_layers)]
+
+
+def shared_owners(ids, n_layers):
+    """Per layer, the owner of its shared module: the lowest layer with the same id (every layer its own without
+    ids)."""
+    if ids is None:
+        return list(range(n_layers))
+    first = {}
+    return [first.setdefault(v, i) for i, v in enumerate(ids)]
+
+
+def sharing_owners(shared_attn_ids, shared_ff_ids, n_layers, attention_types=None):
+    """(attn_owner, ff_owner): per layer, the owner of its token mixer and of its MLP (shared_owners of the validated,
+    cycled ids).  Layers that share an attention id must have the same attention type (DALLE-pytorch refuses it
+    too): a ValueError names the first such pair."""
+    attn_ids = validate_shared_ids(shared_attn_ids, n_layers, "shared_attn_ids")
+    ff_ids = validate_shared_ids(shared_ff_ids, n_layers, "shared_ff_ids")
+    attn_owner = shared_owners(attn_ids, n_layers)
+    types = ["global"] * n_layers if attention_types is None else list(attention_types)
+    for i, o in enumerate(attn_owner):
+        if len(types) == n_layers and types[i] != types[o]:
+            raise ValueError(f"shared_attn_ids: layers {o} and {i} share attention id {attn_ids[i]} but have different "
+                             f"attention types ({types[o]!r}, {types[i]!r})")
+    return attn_owner, shared_owners(ff_ids, n_layers)
+
+
 def validate_shift_tokens(shift_tokens, image_seq_len):
     """The token-shift switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
     handled by model_fns.shift_tokens).  On, it needs a square image-token grid (image_seq_len = W^2)."""
@@ -397,13 +470,15 @@ class DalleEngine:
     mlp = ()   # per-layer flags of the gMLP token-mixing layers (layer_mlp), set by the constructor; () none
     layer_scale = None   # LayerScale (validate_layer_scale), set by the constructor; None: off
     stable = False   # DALLE-pytorch's stable option (validate_stable), set by the constructor
+    tied = False   # share_input_output_emb (validate_share_input_output_emb), set by the constructor
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
                  dropout_seed=0, attention_types=None, local_attention_radius=256, loss_weights=None, z_loss=0.0,
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
                  activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False,
-                 shift_tokens=False, sandwich_norm=False, layer_scale=None, stable=False):
+                 shift_tokens=False, sandwich_norm=False, layer_scale=None, stable=False, share_input_output_emb=False,
+                 shared_attn_ids=None, shared_ff_ids=None):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -500,7 +575,20 @@ class DalleEngine:
         prefill, the decoder, logits()): per row m = max_c x[c] (held constant in backward), u = x / m in fp32 and
         hf = bf16(LN_f(u)) (ops.layernorm_divmax_fwd); one more fp32 [T] keeps m.  (3) Its stable softmax is the
         softmax every attention kernel already computes (the row maximum subtracted in fp32).  No parameter is
-        added."""
+        added.
+
+        share_input_output_emb (validate_share_input_output_emb): DALLE-pytorch's tied embedding.  wte [Vpad, d] is
+        both the input embedding and the vocabulary projection, logits = hf wte^T + bout; wout does not exist
+        (to_logits/linear_out/kernel is not a variable), bout stays and so does the EOS row of wte.  The vocabulary
+        products read wte as a K-major B operand; wte's gradient is the sum of the vocabulary wgrad and the embedding
+        gather's (which alone `stable` shrinks).  wte's pad rows V..Vpad-1 start and stay exactly 0.
+
+        shared_attn_ids / shared_ff_ids (validate_shared_ids): DALLE-pytorch's parameter sharing.  Layers with the same
+        (cycled) attention id use one token mixer (wqkv, wo, o_b, or a gMLP layer's GMLP_MODULE), layers with the same
+        ff id one MLP (w1, b1, w2, b2).  LayerNorms, sandwich LayerNorms, LayerScale and decode caches stay per layer.
+        A shared module belongs to its lowest user (attn_owner / ff_owner): it is initialised and checkpointed there,
+        and the other users' names are layout aliases of its entries, so their gradients add into its slot.  Layers
+        sharing an attention id must have the same attention type."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
@@ -518,6 +606,8 @@ class DalleEngine:
         self.row_col = validate_position_embedding(image_position_embedding) == "row_col"
         self.grid_w = image_grid_side(image_seq_len) if self.row_col else None
         self.per_position_padding = validate_per_position_padding(per_position_padding)
+        self.tied = validate_share_input_output_emb(share_input_output_emb)
+        self.attn_owner, self.ff_owner = sharing_owners(shared_attn_ids, shared_ff_ids, n_layers, attention_types)
         L.require_device()
         self.d, self.L, self.H = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
@@ -566,7 +656,8 @@ class DalleEngine:
         d, V, S, Lyr = self.d, self.V, self.S, self.L
         mlp_layers = self.mlp if any(self.mlp) else None
         kw = dict(gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm, mlp_layers=mlp_layers,
-                  layer_scale=self.layer_scale is not None)
+                  layer_scale=self.layer_scale is not None, tied=self.tied, attn_owner=self.attn_owner,
+                  ff_owner=self.ff_owner)
         self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, **kw) if self.row_col else \
             param_layout(d, Lyr, V, S, **kw)
         self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
@@ -604,6 +695,9 @@ class DalleEngine:
                     self._vec_off[name] = (off, shp)
                     table += [o, off, shp[0]]
                     off += _round_up(shp[0], 64)
+            for name, owner in lay.aliases.items():   # a shared vector reads its owner's slot
+                if owner in self._vec_off:
+                    self._vec_off[name] = self._vec_off[owner]
             self.vec32 = torch.zeros(off, dtype=F32, device=dev)
             self._vec_table = torch.tensor(table, dtype=torch.int64, device=dev)
         if self.row_col:   # the composed bf16 position table the embedding kernels read, and its fp32 gradient
@@ -645,6 +739,45 @@ class DalleEngine:
     def G(self, name):  # fp32 gradient view
         return self._view(2, self.grads, name)
 
+    def wte_rows(self, flat):
+        """The [V, d] embedding rows of wte in the flat buffer `flat` (a tied wte has Vpad rows, the last ones pad)."""
+        v = self.layout.view(flat, "wte")
+        return v[:self.V] if self.tied else v
+
+    def embed_table(self):
+        """The bf16 [V, d] table the embedding kernels gather from."""
+        return self.W("wte")[:self.V] if self.tied else self.W("wte")
+
+    # The vocabulary products over the columns [c0, c0 + n) of the logits (default: all Vpad).  Untied, the B operand
+    # is wout's [d, n] column window, MN-major; tied, it is wte's [n, d] row window, K-major (ldb = d).
+    def _vocab_b(self, c0, n):
+        if self.tied:
+            w = self.W("wte")
+            return (w if n is None else w[c0:c0 + n]), False
+        w = self.W("wout")
+        return (w if n is None else w[:, c0:c0 + n]), True
+
+    def vocab_gemm(self, hf, out, c0=0, n=None, **kw):
+        """logits (or a vocabulary epilogue over them) of the rows hf [M, d] against the columns [c0, c0 + n)."""
+        b, b_mn = self._vocab_b(c0, n)
+        return ops.gemm(hf, b, out, hf.shape[0], self.Vpad if n is None else n, self.d, a_mn=False, b_mn=b_mn, **kw)
+
+    def vocab_wgrad(self, hf, dlogits, c0=0, n=None):
+        """The vocabulary weight's gradient += from dlogits [M, n]: G(wout)[:, window] += hf^T dlogits, or tied
+        G(wte)[window] += dlogits^T hf (the same both-MN-major product with M and N swapped)."""
+        if self.tied:
+            g = self.G("wte")
+            return ops.linear_wgrad(dlogits, hf, g if n is None else g[c0:c0 + n])
+        g = self.G("wout")
+        return ops.linear_wgrad(hf, dlogits, g if n is None else g[:, c0:c0 + n])
+
+    def vocab_dgrad(self, dlogits, out, c0=0, n=None):
+        """out [M, d] = dlogits [M, n] times the vocabulary weight's window transposed (tied: wte[window], MN-major)."""
+        b, b_mn = self._vocab_b(c0, n)
+        if self.tied:
+            return ops.linear_fwd(dlogits, b, out)
+        return ops.linear_dgrad(dlogits, b, out)
+
     def pos_embedding(self):
         """The bf16 [S, d] position table the embedding kernels read: wpe, or with row / column image positions the
         table composed from wpe, image_row and image_col."""
@@ -665,8 +798,17 @@ class DalleEngine:
         n_mlp = sum(self.mlp)
         # a gMLP layer: W_in + b_in, the SGU norm, W_sgu + c_sgu and W_out + b_out in place of q, k, v, o and o_b
         gmlp = 4 * d * d + 4 * d + 4 * d + S * S + S + 2 * d * d + d - (4 * d * d + d)
-        return V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d +
-                                          gate + sandwich + scales) + n_mlp * gmlp + 2 * d + d * V + V
+        n = V * d + n_pos * d + Lyr * (2 * d + 3 * d * d + d * d + d + 2 * d + 4 * d * d + 4 * d + 4 * d * d + d +
+                                       gate + sandwich + scales) + n_mlp * gmlp + 2 * d + d * V + V
+        if self.tied:   # no wout
+            n -= d * V
+        w1_cols = 8 * d if self.gated_mlp else 4 * d
+        for i in range(Lyr):   # a shared module counts once, at its owner
+            if not self._owns_mixer(i):
+                n -= gmlp + 4 * d * d + d if self._is_mlp(i) else 4 * d * d + d
+            if not self._owns_ff(i):
+                n -= d * w1_cols + w1_cols + 4 * d * d + d
+        return n
 
     EMBED_REF_NAMES = {"wte": "embedding/wte", "wpe": "positional_embedding/wpe",
                        "image_row": "positional_embedding/image_row", "image_col": "positional_embedding/image_col"}
@@ -706,18 +848,63 @@ class DalleEngine:
         return self.sandwich_norm or self.layer_scale is not None
 
     def layer_last(self, i):
-        """The last entry of layer i in the layout: the end of its data-parallel bucket."""
+        """The last entry layer i owns in the layout: the end of its data-parallel bucket (a shared MLP's b2 belongs to
+        its owner's bucket)."""
         p = f"l{i}."
-        return p + ("lsm" if self.layer_scale is not None else "lnm_b" if self.sandwich_norm else "b2")
+        return p + ("lsm" if self.layer_scale is not None else "lnm_b" if self.sandwich_norm else
+                    "b2" if self._owns_ff(i) else "ln2_b")
 
     def _is_mlp(self, i):
         """Whether layer i is a gMLP token-mixing layer."""
         return bool(self.mlp) and self.mlp[i]
 
+    attn_owner = ff_owner = None   # per layer, the owner of its token mixer / MLP (sharing_owners); None: itself
+
+    def _owns_mixer(self, i):
+        """Whether layer i owns its token mixer (no shared_attn_ids, or the lowest layer of its id)."""
+        return self.attn_owner is None or self.attn_owner[i] == i
+
+    def _owns_ff(self, i):
+        """Whether layer i owns its MLP (no shared_ff_ids, or the lowest layer of its id)."""
+        return self.ff_owner is None or self.ff_owner[i] == i
+
     def _layer_ref_names(self, i):
         """Reference names of layer i's parameters other than q / k / v (with this engine's sandwich_norm, layer kind
-        and layer_scale)."""
-        return self._ref_names(i, self.sandwich_norm, self._is_mlp(i), self.layer_scale is not None)
+        and layer_scale), without those of a shared module layer i does not own."""
+        names = self._ref_names(i, self.sandwich_norm, self._is_mlp(i), self.layer_scale is not None)
+        drop = (() if self._owns_mixer(i) else ATTN_MODULE + GMLP_MODULE) + (() if self._owns_ff(i) else FF_MODULE)
+        return {k: v for k, v in names.items() if k not in drop}
+
+    def _module_ref_names(self, i):
+        """[(owner, what, reference names)] of layer i's token mixer and MLP, whatever layer owns them."""
+        pre = f"layer_{i}/"
+        ref = self._ref_names(i, mlp=self._is_mlp(i))
+        mixer = [ref[k] for k in GMLP_MODULE] if self._is_mlp(i) else \
+            [pre + "attn/q", pre + "attn/k", pre + "attn/v", ref["wo"], ref["o_b"]]
+        return [(self.attn_owner[i] if self.attn_owner else i, "token mixer (shared_attn_ids)", mixer),
+                (self.ff_owner[i] if self.ff_owner else i, "MLP (shared_ff_ids)", [ref[k] for k in FF_MODULE])]
+
+    OUT_KERNEL = "to_logits/linear_out/kernel"
+
+    def _check_sharing_names(self, named):
+        """Refuse a checkpoint of another tying or sharing kind: an output projection kernel in the checkpoint of a
+        tied model or none in an untied one's, a variable of a module the layer does not own, a missing one of a
+        module it owns.  The error names the first such variable (layer order, the token mixer's first)."""
+        if self.tied and self.OUT_KERNEL in named:
+            raise L.DB200Error(f"load_params: {self.OUT_KERNEL}: an output projection, but this model ties it to "
+                               "embedding/wte (share_input_output_emb)")
+        if not self.tied and self.OUT_KERNEL not in named:
+            raise L.DB200Error(f"load_params: {self.OUT_KERNEL}: missing from the checkpoint of a model without "
+                               "share_input_output_emb")
+        for i in range(self.L):
+            for owner, what, names in self._module_ref_names(i):
+                for rn in names:
+                    if owner == i and rn not in named:
+                        raise L.DB200Error(f"load_params: {rn}: missing from the checkpoint, and layer {i} owns its "
+                                           f"{what}")
+                    if owner != i and rn in named:
+                        raise L.DB200Error(f"load_params: {rn}: layer {i} uses the {what} of layer {owner} and has "
+                                           "no variable of its own")
 
     def _check_layer_kinds(self, named):
         """Refuse a checkpoint whose layer kinds differ from this model's: an attention layer's variables where this
@@ -730,6 +917,8 @@ class DalleEngine:
                     if rn in named:
                         raise L.DB200Error(f"load_params: {rn}: an attention variable, but layer {i} of this model is "
                                            "a gMLP ('mlp') layer")
+                if not self._owns_mixer(i):   # its gMLP variables are its owner's (_check_sharing_names)
+                    continue
                 for v in self.GMLP_REF_NAMES.values():
                     if pre + v not in named:
                         raise L.DB200Error(f"load_params: {pre + v}: missing from the checkpoint of a model whose layer "
@@ -780,18 +969,25 @@ class DalleEngine:
         self.load_flat(self.master, named)
         self.refresh_shadow()
 
-    def _scatter_full(self, name, t, cols=None):
-        """ZeRO-1: place a full fp32 parameter tensor: bf16 copy (full) + the part of it inside this rank's slice."""
+    def _scatter_full(self, name, t, cols=None, rows=None):
+        """ZeRO-1: place a full fp32 parameter tensor: bf16 copy (full) + the part of it inside this rank's slice.
+        cols / rows: t fills only the first cols columns (a vector: entries) / rows rows of the entry, the rest 0."""
         off, shape = self.layout.entries[name]
         dst16 = self.layout.view(self.shadow, name)
-        if cols is None and tuple(t.shape) != tuple(shape):
+        if cols is None and rows is None and tuple(t.shape) != tuple(shape):
             raise L.DB200Error(f"load_params: {self._ref_embed_name(name)}: expected {tuple(shape)}, got "
                                f"{tuple(t.shape)}")
-        if cols is not None:
-            dst16 = dst16[:, :cols] if dst16.dim() == 2 else dst16[:cols]
-        dst16.copy_(t)
+        if rows is not None and tuple(t.shape) != (rows,) + tuple(shape[1:]):
+            raise L.DB200Error(f"load_params: {self._ref_embed_name(name)}: expected {(rows,) + tuple(shape[1:])}, "
+                               f"got {tuple(t.shape)}")
+        part = lambda x: x[:, :cols] if x.dim() == 2 else x[:cols]   # noqa: E731
+        if rows is not None:
+            part = lambda x: x[:rows]   # noqa: E731
+        elif cols is None:
+            part = lambda x: x   # noqa: E731
+        part(dst16).copy_(t)
         full = torch.zeros(shape, dtype=F32, device=self.device)
-        (full[:, :cols] if (cols is not None and full.dim() == 2) else (full[:cols] if cols is not None else full)).copy_(t)
+        part(full).copy_(t)
         lo, hi = self.shard
         n = full.numel()
         a, b = max(lo, off), min(hi, off + n)
@@ -809,25 +1005,28 @@ class DalleEngine:
         self._check_sandwich_names(named)
         self._check_layer_kinds(named)
         self._check_layer_scale_names(named)
+        self._check_sharing_names(named)
         if self.zero is not None:
             if flat is not self.master:
                 raise L.DB200Error("ZeRO-1 mode: loading sharded Adam slots is not implemented (throughput configuration)")
             self.master.zero_(); self.shadow.zero_()
             f32 = lambda x: x.to(device=dev, dtype=F32)
             for name in self.embed_names:
-                self._scatter_full(name, f32(named[self._ref_embed_name(name)]))
+                self._scatter_full(name, f32(named[self._ref_embed_name(name)]),
+                                   rows=self.V if name == "wte" and self.tied else None)
             for i in range(self.L):
                 p = f"l{i}."
                 for k, rn in self._layer_ref_names(i).items():
                     self._scatter_full(p + k, f32(named[rn]))
-                if self._is_mlp(i):
+                if self._is_mlp(i) or not self._owns_mixer(i):
                     continue
                 pre = f"layer_{i}/attn/"
                 self._scatter_full(p + "wqkv", torch.cat([f32(named[pre + "q"]), f32(named[pre + "k"]),
                                                           f32(named[pre + "v"])], dim=1))
             self._scatter_full("lnf_g", f32(named["to_logits/layer_norm/g"]))
             self._scatter_full("lnf_b", f32(named["to_logits/layer_norm/b"]))
-            self._scatter_full("wout", f32(named["to_logits/linear_out/kernel"]), cols=self.V)
+            if not self.tied:
+                self._scatter_full("wout", f32(named[self.OUT_KERNEL]), cols=self.V)
             self._scatter_full("bout", f32(named["to_logits/linear_out/bias"]), cols=self.V)
             self._refresh_vecs()
             return
@@ -835,7 +1034,7 @@ class DalleEngine:
         view = lambda n: self.layout.view(flat, n)
 
         def put(name, t):
-            dst = view(name)
+            dst = self.wte_rows(flat) if name == "wte" else view(name)
             t = t.to(device=dev, dtype=F32)
             if tuple(t.shape) != tuple(dst.shape):
                 raise L.DB200Error(f"load_params: {self._ref_embed_name(name)}: expected {tuple(dst.shape)}, got "
@@ -849,12 +1048,13 @@ class DalleEngine:
             ref = self._layer_ref_names(i)
             for k, rn in ref.items():
                 put(p + k, named[rn])
-            if self._is_mlp(i):
+            if self._is_mlp(i) or not self._owns_mixer(i):
                 continue
             pre = f"layer_{i}/attn/"
             put(p + "wqkv", torch.cat([named[pre + "q"], named[pre + "k"], named[pre + "v"]], dim=1))
         put("lnf_g", named["to_logits/layer_norm/g"]); put("lnf_b", named["to_logits/layer_norm/b"])
-        view("wout")[:, :self.V].copy_(named["to_logits/linear_out/kernel"].to(device=dev, dtype=F32))
+        if not self.tied:
+            view("wout")[:, :self.V].copy_(named[self.OUT_KERNEL].to(device=dev, dtype=F32))
         view("bout")[:self.V].copy_(named["to_logits/linear_out/bias"].to(device=dev, dtype=F32))
 
     def export_params(self, source=None):
@@ -866,21 +1066,22 @@ class DalleEngine:
         elif self.zero is not None and source is not self.grads:
             raise L.DB200Error("ZeRO-1 mode: the Adam slots are sharded across ranks")
         flat = self.master if source is None else source
-        view = lambda n: self.layout.view(flat, n).detach().float().cpu().clone()
+        view = lambda n: (self.wte_rows(flat) if n == "wte" else self.layout.view(flat, n)).detach().float().cpu().clone()
         out = {self._ref_embed_name(n): view(n) for n in self.embed_names}
         d = self.d
         for i in range(self.L):
             p = f"l{i}."
             for k, rn in self._layer_ref_names(i).items():
                 out[rn] = view(p + k)
-            if self._is_mlp(i):
+            if self._is_mlp(i) or not self._owns_mixer(i):
                 continue
             wqkv = view(p + "wqkv")
             pre = f"layer_{i}/attn/"
             out[pre + "q"], out[pre + "k"], out[pre + "v"] = wqkv[:, :d].clone(), wqkv[:, d:2 * d].clone(), \
                 wqkv[:, 2 * d:].clone()
         out["to_logits/layer_norm/g"], out["to_logits/layer_norm/b"] = view("lnf_g"), view("lnf_b")
-        out["to_logits/linear_out/kernel"] = view("wout")[:, :self.V].clone()
+        if not self.tied:
+            out[self.OUT_KERNEL] = view("wout")[:, :self.V].clone()
         out["to_logits/linear_out/bias"] = view("bout")[:self.V].clone()
         return out
 
@@ -892,13 +1093,15 @@ class DalleEngine:
             return self._init_params_sharded(g)
         self.master.zero_()
 
-        def normal(name, std, cols=None):
+        def normal(name, std, cols=None, rows=None):
             t = self.P(name)
             if cols is not None:
                 t = t[:, :cols] if t.dim() == 2 else t[:cols]
+            if rows is not None:
+                t = t[:rows]
             t.copy_(torch.randn(t.shape, generator=g, device=self.device, dtype=F32) * std)
 
-        normal("wte", 0.02); normal("wpe", 0.01)
+        normal("wte", 0.02, rows=self.V); normal("wpe", 0.01)
         if self.row_col:
             normal("image_row", 0.01); normal("image_col", 0.01)
         for i in range(Lyr):
@@ -909,7 +1112,9 @@ class DalleEngine:
             if self.layer_scale is not None:
                 v = layer_scale_init(self.layer_scale, i)
                 self.P(p + "lsa").fill_(v); self.P(p + "lsm").fill_(v)
-            if self._is_mlp(i):
+            if not self._owns_mixer(i):   # a shared module is drawn once, at its owner
+                pass
+            elif self._is_mlp(i):
                 w_in, w_sgu, w_out = self._gmlp_init(g, 0.02 / math.sqrt(Lyr))
                 self.P(p + "gm_win").copy_(w_in); self.P(p + "sgu_w").copy_(w_sgu); self.P(p + "gm_wout").copy_(w_out)
                 self.P(p + "sgu_g").fill_(1.0); self.P(p + "sgu_c").fill_(1.0)
@@ -918,10 +1123,12 @@ class DalleEngine:
                 wqkv[:, :d].copy_(torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5))
                 wqkv[:, d:].copy_(torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5))
                 normal(p + "wo", (H * dh) ** -0.5)
-            normal(p + "w1", 0.02)
-            normal(p + "w2", 0.02 / math.sqrt(Lyr))
+            if self._owns_ff(i):
+                normal(p + "w1", 0.02)
+                normal(p + "w2", 0.02 / math.sqrt(Lyr))
         self.P("lnf_g").fill_(1.0)
-        normal("wout", 0.02, cols=self.V)
+        if not self.tied:
+            normal("wout", 0.02, cols=self.V)
         self.refresh_shadow()
 
     def _gmlp_init(self, g, out_std):
@@ -941,7 +1148,7 @@ class DalleEngine:
         self.master.zero_(); self.shadow.zero_()
         rn = lambda shape, std: torch.randn(shape, generator=g, device=self.device, dtype=F32) * std
         ones = lambda n: torch.ones(n, dtype=F32, device=self.device)
-        self._scatter_full("wte", rn((self.V, d), 0.02))
+        self._scatter_full("wte", rn((self.V, d), 0.02), rows=self.V if self.tied else None)
         for name in self.embed_names[1:]:
             self._scatter_full(name, rn(self.layout.entries[name][1], 0.01))
         for i in range(Lyr):
@@ -952,22 +1159,24 @@ class DalleEngine:
             if self.layer_scale is not None:
                 v = layer_scale_init(self.layer_scale, i)
                 self._scatter_full(p + "lsa", ones(d) * v); self._scatter_full(p + "lsm", ones(d) * v)
-            if self._is_mlp(i):
+            if not self._owns_mixer(i):   # a shared module is drawn once, at its owner
+                pass
+            elif self._is_mlp(i):
                 w_in, w_sgu, w_out = self._gmlp_init(g, 0.02 / math.sqrt(Lyr))
                 self._scatter_full(p + "gm_win", w_in); self._scatter_full(p + "sgu_w", w_sgu)
                 self._scatter_full(p + "gm_wout", w_out)
                 self._scatter_full(p + "sgu_g", ones(2 * d)); self._scatter_full(p + "sgu_c", ones(self.S))
+            else:
+                wq = torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5)
+                wkv = torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5)
+                self._scatter_full(p + "wqkv", torch.cat([wq, wkv], dim=1))
+                self._scatter_full(p + "wo", rn((d, d), (H * dh) ** -0.5))
+            if self._owns_ff(i):
                 self._scatter_full(p + "w1", rn(self.layout.entries[p + "w1"][1], 0.02))
                 self._scatter_full(p + "w2", rn((4 * d, d), 0.02 / math.sqrt(Lyr)))
-                continue
-            wq = torch.randn(d, d, generator=g, device=self.device) * (d ** -0.5 * dh ** -0.5)
-            wkv = torch.randn(d, 2 * d, generator=g, device=self.device) * (d ** -0.5)
-            self._scatter_full(p + "wqkv", torch.cat([wq, wkv], dim=1))
-            self._scatter_full(p + "wo", rn((d, d), (H * dh) ** -0.5))
-            self._scatter_full(p + "w1", rn(self.layout.entries[p + "w1"][1], 0.02))
-            self._scatter_full(p + "w2", rn((4 * d, d), 0.02 / math.sqrt(Lyr)))
         self._scatter_full("lnf_g", ones(d))
-        self._scatter_full("wout", rn((d, self.V), 0.02), cols=self.V)
+        if not self.tied:
+            self._scatter_full("wout", rn((d, self.V), 0.02), cols=self.V)
         self._refresh_vecs()
 
     def refresh_shadow(self):
@@ -1198,10 +1407,10 @@ class DalleEngine:
         self._tokens = tokens
         self._drop = self._dropout_descs(step, row0)
         if self._drop is not None:
-            ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(), bufs["xs"][0].view(B, S, self.d),
+            ops.embed_fwd(tokens, self.embed_table(), self.pos_embedding(), bufs["xs"][0].view(B, S, self.d),
                           wte_drop=self._drop["wte"], wpe_drop=self._drop["wpe"])            # models.py:198-217
         else:
-            ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(),
+            ops.embed_fwd(tokens, self.embed_table(), self.pos_embedding(),
                           bufs["xs"][0].view(B, S, self.d))                                   # models.py:399
         for i in range(self.L):
             sv = bufs["layers"][0 if self.recompute_grad else i]
@@ -1211,9 +1420,9 @@ class DalleEngine:
         labels = bufs["labels"].view(T)
         if self.logits_mask:
             return self._masked_forward(bufs, B, loss_accum, global_batch)
-        ops.gemm(bufs["hf"], self.W("wout"), None, T, self.Vpad, self.d, a_mn=False, b_mn=True, mode=L.EPI_CE_STATS,
-                 bias=self.P("bout"), labels=labels, part_max=bufs["part_max"], part_sum=bufs["part_sum"],
-                 label_logit=bufs["label_logit"], n_valid=self.V)
+        self.vocab_gemm(bufs["hf"], None, mode=L.EPI_CE_STATS, bias=self.P("bout"), labels=labels,
+                        part_max=bufs["part_max"], part_sum=bufs["part_sum"], label_logit=bufs["label_logit"],
+                        n_valid=self.V)
         if self.weighted_loss:
             self._cew = self.ce_weights(B if global_batch is None else global_batch)
             if loss_accum is None:
@@ -1264,9 +1473,9 @@ class DalleEngine:
         for k, ((c0, n_valid), blk) in enumerate(zip(self._mask_windows(), bufs["blocks"])):
             if blk is None:
                 continue
-            ops.gemm(blk["hf"], self.W("wout")[:, c0:c0 + blk["N"]], None, blk["rows"], blk["N"], d, a_mn=False,
-                     b_mn=True, mode=L.EPI_CE_STATS, bias=biases[k], labels=blk["labels"], part_max=blk["part_max"],
-                     part_sum=blk["part_sum"], label_logit=blk["label_logit"], n_valid=n_valid)
+            self.vocab_gemm(blk["hf"], None, c0, blk["N"], mode=L.EPI_CE_STATS, bias=biases[k], labels=blk["labels"],
+                            part_max=blk["part_max"], part_sum=blk["part_sum"], label_logit=blk["label_logit"],
+                            n_valid=n_valid)
             if self.weighted_loss:
                 ops.ce_finish_weighted(blk["part_max"], blk["part_sum"], blk["label_logit"], blk["lse_v"],
                                        blk["loss_rows"], loss_accum, self._cew[k])
@@ -1291,11 +1500,11 @@ class DalleEngine:
             if self.weighted_loss:
                 c = self._cew[k]
                 cew = L.make_ce_weights(c.period, c.text_rows, c.a_text * grad_scale, c.a_image * grad_scale, c.z_loss)
-            ops.gemm(blk["hf"], self.W("wout")[:, c0:c0 + N], blk["dlogits"], blk["rows"], N, d, a_mn=False, b_mn=True,
-                     mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=biases[k], labels=blk["labels"], lse=blk["lse_v"],
-                     n_valid=n_valid, colsum=self.G("bout")[c0:c0 + N], ce_weights=cew)
-            ops.linear_wgrad(blk["hf"], blk["dlogits"], self.G("wout")[:, c0:c0 + N])
-            ops.linear_dgrad(blk["dlogits"], self.W("wout")[:, c0:c0 + N], blk["dx"])
+            self.vocab_gemm(blk["hf"], blk["dlogits"], c0, N, mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=biases[k],
+                            labels=blk["labels"], lse=blk["lse_v"], n_valid=n_valid, colsum=self.G("bout")[c0:c0 + N],
+                            ce_weights=cew)
+            self.vocab_wgrad(blk["hf"], blk["dlogits"], c0, N)
+            self.vocab_dgrad(blk["dlogits"], blk["dx"], c0, N)
         text, image = bufs["blocks"]
         ops.logits_mask_scatter(B, self.S, self.text_rows, dx_text=text["dx"] if text else None, dx_image=image["dx"],
                                 dx=bufs["dtmp"])
@@ -1308,8 +1517,7 @@ class DalleEngine:
         self.forward(tokens, loss_accum=torch.zeros(4 if self.weighted_loss else 1, dtype=F32, device=self.device))
         T = B * S
         out = torch.empty(T, self.Vpad, dtype=F32, device=self.device)
-        ops.gemm(self._bufs["hf"], self.W("wout"), out, T, self.Vpad, self.d, a_mn=False, b_mn=True,
-                 bias=self.P("bout"))
+        self.vocab_gemm(self._bufs["hf"], out, bias=self.P("bout"))
         logits = out.view(B, S, self.Vpad)[:, :, :self.V]
         if self.logits_mask:
             logits[:, :self.text_rows, self.image_offset:] = -math.inf
@@ -1377,7 +1585,7 @@ class DalleEngine:
             raise ValueError("prefill: shift_caches given to an engine without the token shift")
         b = self._prefill_alloc(B, P, rep)
         d = self.d
-        ops.embed_fwd(tokens, self.W("wte"), self.pos_embedding(), b["xs"][0].view(B, P, d))
+        ops.embed_fwd(tokens, self.embed_table(), self.pos_embedding(), b["xs"][0].view(B, P, d))
         drop, self._drop = self._drop, None        # restored below: backward() of a preceding forward() reads it
         try:
             x_in, x_out = b["xs"]
@@ -1395,8 +1603,7 @@ class DalleEngine:
             self._drop = drop
         ops.rows_repeat(x_in.view(B, P, d)[:, P - 1], b["x_last"], rep)
         self.final_ln(b["x_last"], b["hf"], b["meanf"], b["rstdf"], b["mf"])
-        ops.gemm(b["hf"], self.W("wout"), b["logits"], B * rep, self.Vpad, d, a_mn=False, b_mn=True,
-                 bias=self.P("bout"))
+        self.vocab_gemm(b["hf"], b["logits"], bias=self.P("bout"))
         return b["logits"]
 
     # ------------------------------------------------------------------------------------------ backward
@@ -1525,11 +1732,11 @@ class DalleEngine:
             if self.weighted_loss:
                 c = self._cew
                 cew = L.make_ce_weights(c.period, c.text_rows, c.a_text * grad_scale, c.a_image * grad_scale, c.z_loss)
-            ops.gemm(bufs["hf"], self.W("wout"), bufs["dlogits"], T, self.Vpad, d, a_mn=False, b_mn=True,
-                     mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=self.P("bout"), labels=labels, lse=bufs["lse_v"],
-                     n_valid=self.V, colsum=self.G("bout"), ce_weights=cew)  # dlogits + fused d(bout) = colsum(dlogits)
-            ops.linear_wgrad(bufs["hf"], bufs["dlogits"], self.G("wout"))
-            ops.linear_dgrad(bufs["dlogits"], self.W("wout"), bufs["dtmp"])
+            self.vocab_gemm(bufs["hf"], bufs["dlogits"], mode=L.EPI_CE_GRAD, alpha=grad_scale, bias=self.P("bout"),
+                            labels=labels, lse=bufs["lse_v"], n_valid=self.V, colsum=self.G("bout"),
+                            ce_weights=cew)  # dlogits + fused d(bout) = colsum(dlogits)
+            self.vocab_wgrad(bufs["hf"], bufs["dlogits"])
+            self.vocab_dgrad(bufs["dlogits"], bufs["dtmp"])
         dx = bufs["dx_a"]
         split = self.split_branch   # the branch's own backward fuses db2 and the mlp_out dropout instead
         dbranch = self._ln_bwd(bufs["dtmp"], bufs["xs"][self.L], self.P("lnf_g"), bufs["meanf"], bufs["rstdf"], None,
@@ -1555,12 +1762,13 @@ class DalleEngine:
         # row / column positions: the gradient of the composed table goes into a zeroed scratch, then is folded into
         # wpe, image_row and image_col (one fully formed contribution per call, like the wpe gradient itself)
         dpos = self._dpos.zero_() if self.row_col else self.G("wpe")
+        dwte = self.wte_rows(self.grads)   # tied: after the vocabulary wgrad, in this fixed order
         alpha = {"alpha": STABLE_ALPHA} if self.stable else {}   # pos_fold is linear: it carries the shrink along
         if self._drop is not None:
-            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos, wte_drop=self._drop["wte"],
+            ops.embed_bwd(tokens, dx.view(B, S, d), dwte, dpos, wte_drop=self._drop["wte"],
                           wpe_drop=self._drop["wpe"], **alpha)
         else:
-            ops.embed_bwd(tokens, dx.view(B, S, d), self.G("wte"), dpos, **alpha)
+            ops.embed_bwd(tokens, dx.view(B, S, d), dwte, dpos, **alpha)
         if self.row_col:
             ops.pos_fold(dpos, self.G("wpe"), self.G("image_row"), self.G("image_col"))
         if on_bucket_ready:

@@ -16,7 +16,8 @@ from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
     validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
-    validate_layer_scale, validate_rotary, validate_sandwich_norm, validate_shift_tokens, validate_stable
+    validate_layer_scale, validate_rotary, validate_sandwich_norm, validate_share_input_output_emb, \
+    validate_shared_ids, validate_shift_tokens, validate_stable
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -199,6 +200,39 @@ def stable(params):
     return validate_stable(v)
 
 
+def share_input_output_emb(params):
+    """share_input_output_emb of a DALL-E config: absent, null or false keeps the output projection
+    to_logits/linear_out/kernel; true ties it to the input embedding, logits = hf wte^T + bout (DalleEngine), and the
+    checkpoint has no to_logits/linear_out/kernel.  Only a JSON bool is accepted: 1, "true" or a list is rejected."""
+    v = params.get("share_input_output_emb")
+    if v is None:
+        return False
+    if not isinstance(v, bool):
+        raise ValueError(f"share_input_output_emb = {v!r}: expected null, true or false")
+    return validate_share_input_output_emb(v)
+
+
+def shared_attn_ids(params):
+    """shared_attn_ids of a DALL-E config: absent or null gives every layer its own token mixer; a non-empty list of
+    integers >= 0, cycled to n_layers, makes the layers with the same id share one (DalleEngine).  The shared module's
+    variables are those of its lowest layer.  Returned as given (the engine cycles it); bools, other numbers,
+    negative ids and empty lists are rejected."""
+    return _shared_ids(params, "shared_attn_ids")
+
+
+def shared_ff_ids(params):
+    """shared_ff_ids of a DALL-E config: as shared_attn_ids, for the MLPs (w1, b1, w2, b2)."""
+    return _shared_ids(params, "shared_ff_ids")
+
+
+def _shared_ids(params, key):
+    v = params.get(key)
+    if v is None:
+        return None
+    validate_shared_ids(v, 1, key)
+    return list(v)
+
+
 def shift_tokens(params, image_seq_len=None):
     """shift_tokens of a DALL-E config: absent, null or false is off; true turns on DALLE-pytorch's token shift after
     both LayerNorms of every layer (DalleEngine), which needs a square image-token grid (checked here when
@@ -308,6 +342,8 @@ def dalle_model_fn(features, labels, mode, params):
     sandwich = sandwich_norm(params)
     scale = layer_scale(params)
     stab = stable(params)
+    tied = share_input_output_emb(params)
+    attn_ids, ff_ids = shared_attn_ids(params), shared_ff_ids(params)
     mask = logits_mask(params)
     rotary_dim, rotary_base = rotary_embedding(params)
     L.require_device()
@@ -345,7 +381,7 @@ def dalle_model_fn(features, labels, mode, params):
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
                         activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
                         gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich, layer_scale=scale,
-                        stable=stab)
+                        stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

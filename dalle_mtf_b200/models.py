@@ -7,8 +7,8 @@ import torch
 from . import lib as L
 from .dalle_engine import DalleEngine
 from .model_fns import activation_function, attention_layers, conv_kernel, dropout_rates, gated_mlp, \
-    input_embedding, layer_scale, logits_mask, loss_weights, rotary_embedding, sandwich_norm, shift_tokens, stable, \
-    validate_kl_weight
+    input_embedding, layer_scale, logits_mask, loss_weights, rotary_embedding, sandwich_norm, share_input_output_emb, \
+    shared_attn_ids, shared_ff_ids, shift_tokens, stable, validate_kl_weight
 from .model_fns import build_vae_engine, vae_architecture
 from .model_fns import reconstruction_loss as _reconstruction_loss
 
@@ -35,6 +35,8 @@ class DALLE:
         sandwich = sandwich_norm(params)
         scale = layer_scale(params)
         stab = stable(params)
+        tied = share_input_output_emb(params)
+        attn_ids, ff_ids = shared_attn_ids(params), shared_ff_ids(params)
         mask = logits_mask(params)
         rotary_dim, rotary_base = rotary_embedding(params, n_embd, n_heads)
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
@@ -53,7 +55,8 @@ class DALLE:
                                   image_position_embedding=pos_scheme, per_position_padding=per_pos,
                                   activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
                                   rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift,
-                                  sandwich_norm=sandwich, layer_scale=scale, stable=stab)
+                                  sandwich_norm=sandwich, layer_scale=scale, stable=stab,
+                                  share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

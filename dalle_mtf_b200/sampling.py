@@ -17,7 +17,8 @@ parameters and the same kernels' numerics as training:
                     chunks of positions p - 1 and p - W (shift_tokens_decode); with the sandwich LayerNorm each
                     branch output is normalised before its residual add (layernorm_residual_fwd); with LayerScale
                     what a branch adds is multiplied by its per-channel scale (DalleEngine.branch_add)
-  logits = LN_f(x) Wout + bout (fp32), with the stable option LN_f(x / max(x)) (DalleEngine.final_ln);
+  logits = LN_f(x) Wout + bout (fp32), with the stable option LN_f(x / max(x)) (DalleEngine.final_ln), with a tied
+           embedding LN_f(x) wte^T + bout (DalleEngine.vocab_gemm);
   next token = argmax over the allowed id range of logits / T + Gumbel noise
 
 In generate / generate_graphed, prompt (text) positions are teacher-forced through the same step function; complete
@@ -132,7 +133,7 @@ class DalleSampler:
     def step(self, tokens_b, pos):
         """One position for every row: tokens_b int32 [B] -> fp32 logits [B, Vpad] of the NEXT position."""
         e = self.e
-        ops.embed_fwd_at(tokens_b, e.W("wte"), e.pos_embedding(), self.x[0], pos)
+        ops.embed_fwd_at(tokens_b, e.embed_table(), e.pos_embedding(), self.x[0], pos)
         x_in, x_out = self.x
         for i in range(e.L):
             p = f"l{i}."
@@ -156,15 +157,14 @@ class DalleSampler:
             self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
         e.final_ln(x_in, self.ln, self.mean, self.rstd, self.mf)
-        B = tokens_b.shape[0]
-        ops.gemm(self.ln, e.W("wout"), self.logit, B, e.Vpad, e.d, a_mn=False, b_mn=True, bias=e.P("bout"))
+        e.vocab_gemm(self.ln, self.logit, bias=e.P("bout"))
         return self.logit
 
     # -------------------------------------------------------------------------------------------- CUDA-graph path
     def _step_dev(self, tokens):
         """self.step with the position (and the input token column) read on the device from self.pos_dev."""
         e = self.e
-        ops.embed_fwd_at_dev(tokens, e.W("wte"), e.pos_embedding(), self.x[0], self.pos_dev)
+        ops.embed_fwd_at_dev(tokens, e.embed_table(), e.pos_embedding(), self.x[0], self.pos_dev)
         x_in, x_out = self.x
         for i in range(e.L):
             p = f"l{i}."
@@ -188,7 +188,7 @@ class DalleSampler:
             self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
         e.final_ln(x_in, self.ln, self.mean, self.rstd, self.mf)
-        ops.gemm(self.ln, e.W("wout"), self.logit, tokens.shape[0], e.Vpad, e.d, a_mn=False, b_mn=True, bias=e.P("bout"))
+        e.vocab_gemm(self.ln, self.logit, bias=e.P("bout"))
         return self.logit
 
     def _filter(self, top_k, top_p):

@@ -19,7 +19,8 @@ import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
 from dalle_mtf_b200.model_fns import activation_function, attention_layers, conv_kernel, gated_mlp, \
-    input_embedding, layer_scale, logits_mask, rotary_embedding, sandwich_norm, shift_tokens, stable, \
+    input_embedding, layer_scale, logits_mask, rotary_embedding, sandwich_norm, share_input_output_emb, \
+    shared_attn_ids, shared_ff_ids, shift_tokens, stable, \
     vae_checkpoint, vae_grid_size
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
@@ -160,6 +161,8 @@ def main(argv=None):
     sandwich = sandwich_norm(params)                    # and whether its branch outputs are normalised
     scale = layer_scale(params)                         # and whether they are LayerScaled
     stab = stable(params)                               # and whether its final LayerNorm divides by the row maximum
+    tied = share_input_output_emb(params)               # and whether its output projection is the embedding
+    attn_ids, ff_ids = shared_attn_ids(params), shared_ff_ids(params)   # and which layers share their modules
     mask = logits_mask(params)                         # and its objective (sampling draws image ids either way)
     rotary_dim, rotary_base = rotary_embedding(params)  # and its rotary position embeddings
     # with per-position padding the captions are padded with the config's padding_id, which the sampler maps to the
@@ -202,7 +205,8 @@ def main(argv=None):
                       conv_attention_kernel=conv_k, image_position_embedding=pos_scheme,
                       per_position_padding=per_pos, activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
                       rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich,
-                      layer_scale=scale, stable=stab)
+                      layer_scale=scale, stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids,
+                      shared_ff_ids=ff_ids)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})

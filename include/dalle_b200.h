@@ -268,8 +268,9 @@ typedef struct db200_ce_weights {
   float z_loss;       /* z >= 0                                                                   */
 } db200_ce_weights;
 /* weighted CE_GRAD: D(bf16) = a * ((1 + 2 z lse[m]) exp(acc+bias - lse[m]) - [n == label[m]]), 0 for n >= n_valid;
- * epi->mode must be DB200_EPI_CE_GRAD (epi->alpha is not read), A k-major and B mn-major (DB200_E_UNSUPPORTED
- * otherwise).  A row with a = 0 gets exact zeros; colsum / workspace as for CE_GRAD. */
+ * epi->mode must be DB200_EPI_CE_GRAD (epi->alpha is not read), A k-major (DB200_E_UNSUPPORTED otherwise) and B of
+ * either major (mn-major: an untied [d][Vpad] projection; k-major: a tied [Vpad][d] embedding).  A row with a = 0
+ * gets exact zeros; colsum / workspace as for CE_GRAD. */
 int db200_gemm_bf16_ce_weighted(db200_stream_t stream, const void* A, int a_mn_major, int64_t lda, const void* B,
                                 int b_mn_major, int64_t ldb, void* D, int64_t ldd, int M, int N, int K,
                                 const db200_gemm_epilogue* epi, const db200_ce_weights* w);

@@ -31,6 +31,11 @@ int attn_conv_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float*
                          int text_len, int grid_w, int kernel, float scale);
 int attn_conv_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
                          void* dqkv, int B, int S, int H, int dh, int text_len, int grid_w, int kernel, float scale);
+int attn_block_sparse_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H,
+                                 int dh, const uint16_t* mask, int pitch, float scale);
+int attn_block_sparse_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse,
+                                 const float* delta, void* dqkv, int B, int S, int H, int dh, const uint16_t* mask,
+                                 int pitch, float scale);
 
 // ------------------------------------------------------------------------------------------------------------------
 // backward: delta = rowsum(dO * O)
@@ -237,4 +242,37 @@ extern "C" int db200_attn_conv_bwd(db200_stream_t stream_, const void* qkv, cons
   const int rc = attn_delta(stream, out, dout, delta, B, S, H, dh);
   if (rc != DB200_OK) return rc;
   return attn_conv_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, text_len, grid_w, kernel, scale);
+}
+
+// ---- block-sparse attention: the 16-bit tile masks of a [>= ceil(S / 64)] x pitch table (attn_fa.cu, SPARSE) under
+// the causal mask.  No dropout.
+extern "C" int db200_attn_block_sparse_fwd(db200_stream_t stream_, const void* qkv, void* out, float* lse, int B, int S,
+                                           int H, int dh, const uint16_t* tile_mask, int mask_pitch, float scale) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_block_sparse_fwd: B,S,H must be positive");
+  DB200_REQUIRE(tile_mask && mask_pitch >= (S + 63) / 64, DB200_E_INVALID,
+                "attn_block_sparse_fwd: NULL tile mask or pitch %d < ceil(S / 64) for S %d", mask_pitch, S);
+  DB200_REQUIRE(qkv && out && lse && aligned16(qkv) && aligned16(out), DB200_E_ALIGN,
+                "attn_block_sparse_fwd: NULL or unaligned pointer");
+  DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_block_sparse_fwd: scale must be > 0");
+  DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
+  return attn_block_sparse_fwd_launch(stream, qkv, out, lse, B, S, H, dh, tile_mask, mask_pitch, scale);
+}
+
+extern "C" int db200_attn_block_sparse_bwd(db200_stream_t stream_, const void* qkv, const void* out, const void* dout,
+                                           const float* lse, float* dq_accum, float* delta, void* dqkv, int B, int S,
+                                           int H, int dh, const uint16_t* tile_mask, int mask_pitch, float scale) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  (void)dq_accum;
+  DB200_REQUIRE(B > 0 && S > 0 && H > 0, DB200_E_INVALID, "attn_block_sparse_bwd: B,S,H must be positive");
+  DB200_REQUIRE(tile_mask && mask_pitch >= (S + 63) / 64, DB200_E_INVALID,
+                "attn_block_sparse_bwd: NULL tile mask or pitch %d < ceil(S / 64) for S %d", mask_pitch, S);
+  DB200_REQUIRE(qkv && out && dout && lse && delta && dqkv && aligned16(qkv) && aligned16(out) && aligned16(dout) &&
+                    aligned16(dqkv),
+                DB200_E_ALIGN, "attn_block_sparse_bwd: NULL or unaligned pointer");
+  DB200_REQUIRE(scale > 0.f, DB200_E_INVALID, "attn_block_sparse_bwd: scale must be > 0");
+  DB200_REQUIRE(dh == 64 || dh == 128, DB200_E_UNSUPPORTED, "attn: head_dim %d not in {64,128}", dh);
+  const int rc = attn_delta(stream, out, dout, delta, B, S, H, dh);
+  if (rc != DB200_OK) return rc;
+  return attn_block_sparse_bwd_launch(stream, qkv, dout, lse, delta, dqkv, B, S, H, dh, tile_mask, mask_pitch, scale);
 }

@@ -29,6 +29,14 @@
 // (no row map).  Every visible key precedes its query, but the mask is not a band: (r - 1, c + 1) is earlier and
 // outside the window.  The loops visit the text blocks and the band of blocks from the window's top row to the
 // query; each tile's mask tests the window from grid coordinates stepped along the thread's columns.
+//
+// SPARSE (DeepSpeed-style block-sparse attention, DALLE-pytorch's SparseAttention): a per-layer table of 16-bit tile
+// masks, mask[qt * pitch + kt] for the 64 x 64 tile of query block qt and key block kt <= qt.  Bit 4 a + c set: the 16
+// queries 64 qt + 16 a .. + 15 see the 16 keys 64 kt + 16 c .. + 15, under the causal mask (key <= query, key < S).
+// The forward and dQ kernels visit, in ascending order, the key blocks whose mask is non-zero; the dK / dV kernel the
+// query blocks.  Warp w of the warpgroup holds the fragment rows 16 w .. 16 w + 15 and element i of a row lies in
+// column block i / 2, so each thread tests one nibble of the mask.  The table's pitch is independent of S, so that a
+// prefill shorter than the table reads the rows it covers.
 #include "gemm_common.cuh"  // cp.async helpers
 #include "philox.cuh"
 #include "wgmma.cuh"
@@ -291,17 +299,62 @@ __device__ __forceinline__ int fa_conv_query_end(const FaConv& c, int S, int kb)
   return (int)min((long long)nq, reach / FA_ROWS + 1);
 }
 
+// ---- SPARSE: tile-mask table (pitch >= the number of 64-row blocks of S)
+struct FaSparse {
+  const uint16_t* mask;
+  int pitch;
+};
+__device__ __forceinline__ uint32_t fa_sparse_tile(const FaSparse& sp, int qt, int kt) {
+  return sp.mask[(long long)qt * sp.pitch + kt];
+}
+// the first key block after j (<= qb) with a non-zero mask in query block qb's row, or qb + 1
+__device__ __forceinline__ int fa_sparse_next_key(const FaSparse& sp, int qb, int j) {
+  for (++j; j <= qb && fa_sparse_tile(sp, qb, j) == 0u; ++j) {
+  }
+  return j;
+}
+// the first query block after i (< nq) with a non-zero mask in key block kb's column, or nq
+__device__ __forceinline__ int fa_sparse_next_query(const FaSparse& sp, int kb, int i, int nq) {
+  for (++i; i < nq && fa_sparse_tile(sp, i, kb) == 0u; ++i) {
+  }
+  return i;
+}
+// Visible bits of this thread's 32 fragment elements (bit x = element x, as fa_conv_vis_bits) of the tile with mask tm
+// whose first row / column are r0 / c0.  QROWS: rows are queries and columns keys (forward, dQ); else rows are keys
+// and columns queries (dK / dV).  The thread's rows lie in 16-row block w (its warp), element 4 i + 2 hh + e in column
+// block i / 2.
+template <bool QROWS>
+__device__ __forceinline__ uint32_t fa_sparse_vis_bits(uint32_t tm, int S, int r0, int c0, const Frag& f) {
+  const int w = f.fr >> 4;
+  const uint32_t nib = QROWS ? (tm >> (4 * w)) & 15u
+                             : ((tm >> w) & 1u) | ((tm >> (w + 3)) & 2u) | ((tm >> (w + 6)) & 4u) | ((tm >> (w + 9)) & 8u);
+  uint32_t bits = 0u;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int row = r0 + f.fr + 8 * hh, col = c0 + 8 * i + f.fc + e;
+        const bool vis = ((nib >> (i >> 1)) & 1u) && (QROWS ? col <= row && col < S : row <= col && col < S);
+        bits |= (uint32_t)vis << (4 * i + 2 * hh + e);
+      }
+  return bits;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
 // forward: grid (query blocks, B * H); online softmax in the exp2 domain
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV, bool SPARSE>
 __global__ void __launch_bounds__(128, 1)
 attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __restrict__ lse, int S, int H,
-                float scale, const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv) {
+                float scale, const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv,
+                const FaSparse sp) {
   static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
   static_assert(!(CONV && (DROP || LOCAL || AXIAL)), "conv layers have no dropout, no window and no row map");
+  static_assert(!(SPARSE && (DROP || LOCAL || AXIAL || CONV)), "block-sparse layers have no dropout and one mask");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -330,8 +383,11 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
     fa_conv_rc(cv, q0 + f.fr, qr[0], qc[0]);
     fa_conv_rc(cv, q0 + f.fr + 8, qr[1], qc[1]);
   }
-  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : ((AXIAL || CONV) && jt == 0 ? js : 0);
-  for (int j = j0; j <= qb; j = (AXIAL || CONV) ? fa_axial_next(j, jt, js) : j + 1) {
+  const int j0 = SPARSE  ? fa_sparse_next_key(sp, qb, -1)
+               : LOCAL ? max(0, q0 - radius + 1) / FA_ROWS
+                       : ((AXIAL || CONV) && jt == 0 ? js : 0);
+  for (int j = j0; j <= qb;
+       j = SPARSE ? fa_sparse_next_key(sp, qb, j) : (AXIAL || CONV) ? fa_axial_next(j, jt, js) : j + 1) {
     const int k0 = j * FA_ROWS;
     __syncthreads();  // the previous block's K / V tiles are no longer read
     if constexpr (AXIAL) {
@@ -344,7 +400,9 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
     fa_tiles_ready();
     float s[32];
     fa_qk<DH>(s, sQ, sK);
-    const uint32_t vb = CONV ? fa_conv_vis_bits<true>(cv, S, q0, k0, qr, qc, f) : 0u;
+    const uint32_t vb = CONV     ? fa_conv_vis_bits<true>(cv, S, q0, k0, qr, qc, f)
+                        : SPARSE ? fa_sparse_vis_bits<true>(fa_sparse_tile(sp, qb, j), S, q0, k0, f)
+                                 : 0u;
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int i = 0; i < 8; ++i)
@@ -355,7 +413,7 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           float& v = s[4 * i + 2 * hh + e];
           if constexpr (AXIAL) v = (col <= row && (col < ax.text_len || col >= slo[hh])) ? v * sl2 : -INFINITY;
-          else if constexpr (CONV) v = ((vb >> (4 * i + 2 * hh + e)) & 1u) ? v * sl2 : -INFINITY;
+          else if constexpr (CONV || SPARSE) v = ((vb >> (4 * i + 2 * hh + e)) & 1u) ? v * sl2 : -INFINITY;
           else v = (col <= row && col < S && (!LOCAL || col > row - radius)) ? v * sl2 : -INFINITY;
           mx[hh] = fmaxf(mx[hh], v);
         }
@@ -407,13 +465,14 @@ attn_fwd_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ out, float* __r
 // ------------------------------------------------------------------------------------------------------------------
 // backward, dQ: grid (query blocks, B * H).  P = exp(scale S - lse), dS = P (dO V^T - delta), dQ = scale dS K
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV, bool SPARSE>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                    const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                   const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv) {
+                   const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv, const FaSparse sp) {
   static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
   static_assert(!(CONV && (DROP || LOCAL || AXIAL)), "conv layers have no dropout, no window and no row map");
+  static_assert(!(SPARSE && (DROP || LOCAL || AXIAL || CONV)), "block-sparse layers have no dropout and one mask");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -460,8 +519,11 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
     fa_conv_rc(cv, q0 + f.fr, qr[0], qc[0]);
     fa_conv_rc(cv, q0 + f.fr + 8, qr[1], qc[1]);
   }
-  const int j0 = LOCAL ? max(0, q0 - radius + 1) / FA_ROWS : ((AXIAL || CONV) && jt == 0 ? js : 0);
-  for (int j = j0; j <= qb; j = (AXIAL || CONV) ? fa_axial_next(j, jt, js) : j + 1) {
+  const int j0 = SPARSE  ? fa_sparse_next_key(sp, qb, -1)
+               : LOCAL ? max(0, q0 - radius + 1) / FA_ROWS
+                       : ((AXIAL || CONV) && jt == 0 ? js : 0);
+  for (int j = j0; j <= qb;
+       j = SPARSE ? fa_sparse_next_key(sp, qb, j) : (AXIAL || CONV) ? fa_axial_next(j, jt, js) : j + 1) {
     const int k0 = j * FA_ROWS;
     __syncthreads();
     if constexpr (AXIAL) {
@@ -477,7 +539,9 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
     fa_qk<DH>(dp, sdO, sV);
     // dropout: dS = P (dP keep scale - delta)
     const uint32_t kb = DROP ? fa_keep_bits<true>(dr, b, h, H, (S + 1) >> 1, q0, k0, f) : 0u;
-    const uint32_t vb = CONV ? fa_conv_vis_bits<true>(cv, S, q0, k0, qr, qc, f) : 0u;
+    const uint32_t vb = CONV     ? fa_conv_vis_bits<true>(cv, S, q0, k0, qr, qc, f)
+                        : SPARSE ? fa_sparse_vis_bits<true>(fa_sparse_tile(sp, qb, j), S, q0, k0, f)
+                                 : 0u;
 #pragma unroll
     for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -487,7 +551,7 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
           const int row = q0 + f.fr + 8 * hh, col = k0 + 8 * i + f.fc + e;
           const int x = 4 * i + 2 * hh + e;
           const bool vis = AXIAL ? col <= row && (col < ax.text_len || col >= slo[hh])
-                         : CONV  ? ((vb >> x) & 1u) != 0u
+                         : (CONV || SPARSE) ? ((vb >> x) & 1u) != 0u
                                  : col <= row && col < S && row < S && (!LOCAL || col > row - radius);
           const float p = vis ? exp2f(s[x] * sl2 - lse2[hh]) : 0.f;
           s[x] = p * ((DROP ? dp[x] * fa_keep_mul(kb, x, dr.scale) : dp[x]) - dl[hh]);
@@ -503,13 +567,14 @@ attn_bwd_dq_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, 
 // backward, dK / dV: grid (key blocks, B * H), transposed products so that the key index is the accumulator row.
 //   P^T = exp(scale K Q^T - lse), dV = P^T dO, dS^T = P^T (V dO^T - delta), dK = scale dS^T Q
 // ------------------------------------------------------------------------------------------------------------------
-template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV>
+template <int DH, bool DROP, bool LOCAL, bool AXIAL, bool CONV, bool SPARSE>
 __global__ void __launch_bounds__(128, 1)
 attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, const float* __restrict__ lse,
                     const float* __restrict__ delta, bf16* __restrict__ dqkv, int S, int H, float scale,
-                    const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv) {
+                    const db200_dropout dr, int radius, const FaAxial ax, const FaConv cv, const FaSparse sp) {
   static_assert(!(AXIAL && (DROP || LOCAL)), "axial layers have no dropout and no window");
   static_assert(!(CONV && (DROP || LOCAL || AXIAL)), "conv layers have no dropout, no window and no row map");
+  static_assert(!(SPARSE && (DROP || LOCAL || AXIAL || CONV)), "block-sparse layers have no dropout and one mask");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   constexpr uint32_t TILE = FA_ROWS * DH * 2;
@@ -550,7 +615,8 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
   float dk[DH / 2], dv[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
-  for (int i = kb; i < nqb; ++i) {
+  for (int i = SPARSE ? fa_sparse_next_query(sp, kb, kb - 1, nqb) : kb; i < nqb;
+       i = SPARSE ? fa_sparse_next_query(sp, kb, i, nqb) : i + 1) {
     const int q0 = i * FA_ROWS;
     __syncthreads();
     if constexpr (AXIAL) {
@@ -575,7 +641,9 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
     fa_tiles_ready();
     float st[32], dpt[32];
     fa_qk<DH>(st, sK, sQ);
-    const uint32_t vb = CONV ? fa_conv_vis_bits<false>(cv, S, k0, q0, kr, kc, f) : 0u;
+    const uint32_t vb = CONV     ? fa_conv_vis_bits<false>(cv, S, k0, q0, kr, kc, f)
+                        : SPARSE ? fa_sparse_vis_bits<false>(fa_sparse_tile(sp, i, kb), S, k0, q0, f)
+                                 : 0u;
 #pragma unroll
     for (int ii = 0; ii < 8; ++ii)
 #pragma unroll
@@ -585,7 +653,7 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
           const int key = k0 + f.fr + 8 * hh, cq = 8 * ii + f.fc + e, q = q0 + cq;
           const int x = 4 * ii + 2 * hh + e;
           const bool vis = AXIAL ? key <= q && (key < ax.text_len || q <= kend[hh])
-                         : CONV  ? ((vb >> x) & 1u) != 0u
+                         : (CONV || SPARSE) ? ((vb >> x) & 1u) != 0u
                                  : key <= q && q < S && key < S && (!LOCAL || key > q - radius);
           st[x] = vis ? exp2f(st[x] * sl2 - s_lse[cq]) : 0.f;
         }
@@ -618,40 +686,38 @@ attn_bwd_dkv_kernel(const bf16* __restrict__ qkv, const bf16* __restrict__ dout,
 }
 
 // AXIAL: the grid covers ax.rows kernel-order rows instead of S
-template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false, bool CONV = false>
+template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false, bool CONV = false, bool SPARSE = false>
 static int fa_fwd(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H, float scale,
                   const db200_dropout& dr, int radius = 0, const FaAxial& ax = FaAxial{},
-                  const FaConv& cv = FaConv{}) {
+                  const FaConv& cv = FaConv{}, const FaSparse& sp = FaSparse{}) {
   constexpr size_t smem = fa_smem<DH>(3);
-  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL, AXIAL, CONV>,
+  static const cudaError_t attr_rc = cudaFuncSetAttribute(attn_fwd_kernel<DH, DROP, LOCAL, AXIAL, CONV, SPARSE>,
                                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(attr_rc);
   const dim3 grid(((AXIAL ? ax.rows : S) + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_fwd_kernel<DH, DROP, LOCAL, AXIAL, CONV><<<grid, 128, smem, stream>>>((const bf16*)qkv, (bf16*)out, lse, S, H,
-                                                                             scale, dr, radius, ax, cv);
+  attn_fwd_kernel<DH, DROP, LOCAL, AXIAL, CONV, SPARSE><<<grid, 128, smem, stream>>>(
+      (const bf16*)qkv, (bf16*)out, lse, S, H, scale, dr, radius, ax, cv, sp);
   return check_launch("attn_fwd_kernel");
 }
 
-template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false, bool CONV = false>
+template <int DH, bool DROP, bool LOCAL = false, bool AXIAL = false, bool CONV = false, bool SPARSE = false>
 static int fa_bwd(cudaStream_t stream, const void* qkv, const void* dout, const float* lse, const float* delta,
                   void* dqkv, int B, int S, int H, float scale, const db200_dropout& dr, int radius = 0,
-                  const FaAxial& ax = FaAxial{}, const FaConv& cv = FaConv{}) {
+                  const FaAxial& ax = FaAxial{}, const FaConv& cv = FaConv{}, const FaSparse& sp = FaSparse{}) {
   constexpr size_t smem = fa_smem<DH>(4);
-  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL, CONV>,
+  static const cudaError_t rc1 = cudaFuncSetAttribute(attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL, CONV, SPARSE>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL, CONV>,
+  static const cudaError_t rc2 = cudaFuncSetAttribute(attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL, CONV, SPARSE>,
                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   DB200_CUDA(rc1);
   DB200_CUDA(rc2);
   const dim3 grid(((AXIAL ? ax.rows : S) + FA_ROWS - 1) / FA_ROWS, B * H);
-  attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL, CONV><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout,
-                                                                                lse, delta, (bf16*)dqkv, S, H, scale,
-                                                                                dr, radius, ax, cv);
+  attn_bwd_dq_kernel<DH, DROP, LOCAL, AXIAL, CONV, SPARSE><<<grid, 128, smem, stream>>>(
+      (const bf16*)qkv, (const bf16*)dout, lse, delta, (bf16*)dqkv, S, H, scale, dr, radius, ax, cv, sp);
   int rc = check_launch("attn_bwd_dq_kernel");
   if (rc != DB200_OK) return rc;
-  attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL, CONV><<<grid, 128, smem, stream>>>((const bf16*)qkv, (const bf16*)dout,
-                                                                                 lse, delta, (bf16*)dqkv, S, H, scale,
-                                                                                 dr, radius, ax, cv);
+  attn_bwd_dkv_kernel<DH, DROP, LOCAL, AXIAL, CONV, SPARSE><<<grid, 128, smem, stream>>>(
+      (const bf16*)qkv, (const bf16*)dout, lse, delta, (bf16*)dqkv, S, H, scale, dr, radius, ax, cv, sp);
   return check_launch("attn_bwd_dkv_kernel");
 }
 
@@ -733,6 +799,27 @@ int attn_conv_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout,
   return dh == 128
              ? fa_bwd<128, false, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, {}, cv)
              : fa_bwd<64, false, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale, none, 0, {}, cv);
+}
+
+// block-sparse attention over the tile masks of `mask` (row pitch `pitch`); no dropout
+int attn_block_sparse_fwd_launch(cudaStream_t stream, const void* qkv, void* out, float* lse, int B, int S, int H,
+                                 int dh, const uint16_t* mask, int pitch, float scale) {
+  const db200_dropout none{};
+  const FaSparse sp{mask, pitch};
+  return dh == 128
+             ? fa_fwd<128, false, false, false, false, true>(stream, qkv, out, lse, B, S, H, scale, none, 0, {}, {}, sp)
+             : fa_fwd<64, false, false, false, false, true>(stream, qkv, out, lse, B, S, H, scale, none, 0, {}, {}, sp);
+}
+
+int attn_block_sparse_bwd_launch(cudaStream_t stream, const void* qkv, const void* dout, const float* lse,
+                                 const float* delta, void* dqkv, int B, int S, int H, int dh, const uint16_t* mask,
+                                 int pitch, float scale) {
+  const db200_dropout none{};
+  const FaSparse sp{mask, pitch};
+  return dh == 128 ? fa_bwd<128, false, false, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale,
+                                                                   none, 0, {}, {}, sp)
+                   : fa_bwd<64, false, false, false, false, true>(stream, qkv, dout, lse, delta, dqkv, B, S, H, scale,
+                                                                  none, 0, {}, {}, sp);
 }
 
 }  // namespace db200

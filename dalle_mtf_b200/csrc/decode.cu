@@ -11,6 +11,7 @@
 //                  image position (grid row r, column c), by row r's columns 0..c or column c's rows 0..r
 //                  CONV (convolutional layers, kernel k): the text run followed by one run per row r' of the k x k
 //                  window, max(0, r - k + 1) <= r' <= r, each over columns max(0, c - k + 1) .. c
+//                  SPARSE (block-sparse layers): over the 16-key blocks listed for row block pos / 16, clipped at pos
 //   sample_rows    idx = lo + argmax_{lo<=c<hi}(logits[c] * inv_temp + gumbel(u[c-lo]))   (first maximum; u NULL = greedy)
 //   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
 //   sample_rows_guided     either of the two over the classifier-free-guidance mix u + s (c - u) of a conditional
@@ -45,12 +46,15 @@ __global__ void embed_at_kernel(const int* __restrict__ ids, const bf16* __restr
 // key ist + i * istr (the image run of the position's row or column); at most text_len + grid_w entries.
 // CONV: the same text run; entry n1 + i is key ist + (i / m) grid_w + i % m (m window columns per row, ist the window's
 // top-left key); at most text_len + min(k, grid_w)^2 entries.
-template <int DH, bool AXIAL = false, bool CONV = false>
+// SPARSE: row g = pos / 16 of the block list (blocks + g * bpitch: a count, then ascending block indices <= g); entry
+// j is key 16 bl[j / 16] + j % 16.  Only the last listed block can reach past pos, so the list holds 16 (count - 1) +
+// min(16, pos - 16 last + 1) keys, at most pos + 1.
+template <int DH, bool AXIAL = false, bool CONV = false, bool SPARSE = false>
 __global__ void __launch_bounds__(256)
 attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __restrict__ vc, bf16* __restrict__ out,
                    int S, int H, int pos, float scale, const int* __restrict__ pos_dev, int radius, int text_len,
-                   int grid_w, int axis, int kernel) {
-  static_assert(!(AXIAL && CONV), "one key list");
+                   int grid_w, int axis, int kernel, const int* __restrict__ blocks, int bpitch) {
+  static_assert(int(AXIAL) + int(CONV) + int(SPARSE) <= 1, "one key list");
   extern __shared__ float sc[];
   __shared__ float red[8];
   __shared__ float part[8][DH];
@@ -72,7 +76,7 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
 #pragma unroll
   for (int e = 0; e < EPL; ++e) qr[e] = __bfloat162float(q[lane * EPL + e]);
   __syncthreads();  // this block's own global writes are visible to it after the barrier
-  const int lo = (AXIAL || CONV) ? 0 : max(0, pos - radius + 1);
+  const int lo = (AXIAL || CONV || SPARSE) ? 0 : max(0, pos - radius + 1);
   int n = pos + 1 - lo, n1 = 0, ist = 0, istr = 0, m = 1;
   if constexpr (AXIAL) {
     n1 = min(pos, text_len - 1) + 1;
@@ -95,9 +99,17 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
       n += (r - r0 + 1) * m;
     }
   }
+  const int* bl = nullptr;
+  if constexpr (SPARSE) {
+    const int* row = blocks + (long long)(pos >> 4) * bpitch;
+    const int cnt = row[0];
+    bl = row + 1;
+    n = cnt > 0 ? 16 * (cnt - 1) + min(16, pos - 16 * bl[cnt - 1] + 1) : 0;
+  }
   // key row of list entry j
   auto key = [&](int j) {
-    if constexpr (CONV) return j < n1 ? j : ist + (j - n1) / m * grid_w + (j - n1) % m;
+    if constexpr (SPARSE) return 16 * bl[j >> 4] + (j & 15);
+    else if constexpr (CONV) return j < n1 ? j : ist + (j - n1) / m * grid_w + (j - n1) % m;
     else return AXIAL ? (j < n1 ? j : ist + (j - n1) * istr) : j;
   };
   const bf16* kw = kcb + (long long)lo * rs;         // key / value rows of the window: j - lo = 0 .. n - 1
@@ -174,7 +186,7 @@ attn_decode_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kc, bf16* __
 #pragma unroll
   for (int e = 0; e < EPL; ++e) part[warp][lane * EPL + e] = acc[e];
   __syncthreads();
-  const float inv = 1.f / sum;
+  const float inv = (SPARSE && sum == 0.f) ? 0.f : 1.f / sum;  // SPARSE: a row without keys gives 0
   for (int t = tid; t < DH; t += 256) {
     float o = 0.f;
 #pragma unroll
@@ -552,9 +564,12 @@ extern "C" int db200_incr_i32(db200_stream_t stream_, int32_t* p, int delta) {
 // floats when the position is read on the device).
 // kernel >= 1: a convolutional layer (attn_decode_kernel<DH, false, true>, radius and axis unused): the key list of
 // `pos` (text_len + kernel min(kernel, grid_w) floats when the position is read on the device).
+// blocks != NULL: a block-sparse layer (attn_decode_kernel<DH, false, false, true>, radius S): the keys of the blocks
+// listed for pos / 16, at most as many as a global layer's.
 static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k_cache, void* v_cache, void* out, int B,
                               int S, int H, int dh, int pos, float scale, const int32_t* pos_dev, int radius,
-                              int text_len = 0, int grid_w = 1, int axis = -1, int kernel = 0) {
+                              int text_len = 0, int grid_w = 1, int axis = -1, int kernel = 0,
+                              const int32_t* blocks = nullptr, int bpitch = 0) {
   DB200_REQUIRE(qkv_step && k_cache && v_cache && out, DB200_E_INVALID, "attn_decode: null pointer");
   DB200_REQUIRE(B > 0 && H > 0 && S > 0 && pos >= 0 && pos < S, DB200_E_INVALID, "attn_decode: B %d H %d pos %d of %d",
                 B, H, pos, S);
@@ -600,13 +615,22 @@ static int attn_decode_launch(cudaStream_t stream, const void* qkv_step, void* k
   DB200_CUDA(x64);
   DB200_CUDA(c128);
   DB200_CUDA(c64);
-  auto fn = dh == 128 ? (conv ? attn_decode_kernel<128, false, true>
-                              : axial ? attn_decode_kernel<128, true> : attn_decode_kernel<128>)
-                      : (conv ? attn_decode_kernel<64, false, true>
-                              : axial ? attn_decode_kernel<64, true> : attn_decode_kernel<64>);
+  static const cudaError_t s128 = cudaFuncSetAttribute(attn_decode_kernel<128, false, false, true>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  static const cudaError_t s64 = cudaFuncSetAttribute(attn_decode_kernel<64, false, false, true>,
+                                                      cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  DB200_CUDA(s128);
+  DB200_CUDA(s64);
+  const bool sparse = blocks != nullptr;
+  auto fn = dh == 128 ? (sparse ? attn_decode_kernel<128, false, false, true>
+                         : conv ? attn_decode_kernel<128, false, true>
+                                : axial ? attn_decode_kernel<128, true> : attn_decode_kernel<128>)
+                      : (sparse ? attn_decode_kernel<64, false, false, true>
+                         : conv ? attn_decode_kernel<64, false, true>
+                                : axial ? attn_decode_kernel<64, true> : attn_decode_kernel<64>);
   fn<<<grid, 256, smem, stream>>>(static_cast<const bf16*>(qkv_step), static_cast<bf16*>(k_cache),
                                   static_cast<bf16*>(v_cache), static_cast<bf16*>(out), S, H, pos, scale, pos_dev,
-                                  radius, text_len, grid_w, axis, kernel);
+                                  radius, text_len, grid_w, axis, kernel, blocks, bpitch);
   return check_launch("attn_decode_kernel");
 }
 
@@ -696,6 +720,28 @@ extern "C" int db200_attn_decode_conv_dev(db200_stream_t stream_, const void* qk
   if (rc != DB200_OK) return rc;
   return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
                             pos_dev, S, text_len, grid_w, -1, kernel);
+}
+
+// block-sparse layers: the query of `pos` attends to the keys of the 16-key blocks listed in row pos / 16 of `blocks`
+extern "C" int db200_attn_decode_block_sparse(db200_stream_t stream_, const void* qkv_step, void* k_cache,
+                                              void* v_cache, void* out, int B, int S, int H, int dh, int pos,
+                                              const int32_t* blocks, int blocks_pitch, float scale) {
+  DB200_REQUIRE(blocks && blocks_pitch >= (S + 15) / 16 + 1, DB200_E_INVALID,
+                "attn_decode_block_sparse: NULL block table or pitch %d < ceil(S / 16) + 1 for S %d", blocks_pitch, S);
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, pos, scale,
+                            nullptr, S, 0, 1, -1, 0, blocks, blocks_pitch);
+}
+
+extern "C" int db200_attn_decode_block_sparse_dev(db200_stream_t stream_, const void* qkv_step, void* k_cache,
+                                                  void* v_cache, void* out, int B, int S, int H, int dh,
+                                                  const int32_t* pos_dev, const int32_t* blocks, int blocks_pitch,
+                                                  float scale) {
+  DB200_REQUIRE(pos_dev, DB200_E_INVALID, "attn_decode_block_sparse_dev: null position pointer");
+  DB200_REQUIRE(blocks && blocks_pitch >= (S + 15) / 16 + 1, DB200_E_INVALID,
+                "attn_decode_block_sparse_dev: NULL block table or pitch %d < ceil(S / 16) + 1 for S %d", blocks_pitch,
+                S);
+  return attn_decode_launch(static_cast<cudaStream_t>(stream_), qkv_step, k_cache, v_cache, out, B, S, H, dh, 0, scale,
+                            pos_dev, S, 0, 1, -1, 0, blocks, blocks_pitch);
 }
 
 extern "C" int db200_sample_rows(db200_stream_t stream_, const float* logits, const float* u_or_null, int32_t* idx,

@@ -135,7 +135,7 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     return lay
 
 
-ATTENTION_TYPES = ("global", "local", "axial_row", "axial_col", "conv", "mlp")
+ATTENTION_TYPES = ("global", "local", "axial_row", "axial_col", "conv", "mlp", "block_sparse")
 AXIAL_AXIS = {"axial_row": 0, "axial_col": 1}
 
 
@@ -206,6 +206,68 @@ def layer_conv(attention_types, text_seq_len, image_seq_len, kernel, n_layers):
         raise ValueError(f"convolutional attention layers need a square image-token grid, but image_seq_len = "
                          f"{image_seq_len} is not a square")
     return [(int(text_seq_len), W, kernel) if t == "conv" else None for t in types]
+
+
+SPARSE_BLOCK_SIZES = (16, 32, 64)
+
+
+def _sparse_int(name, v, lo):
+    if isinstance(v, bool) or not isinstance(v, numbers.Integral) or v < lo:
+        raise ValueError(f"{name} must be an integer >= {lo}, got {v!r}")
+    return int(v)
+
+
+def validate_block_sparse(block_size, local_window_blocks, random_blocks, layout_seed, seq_len):
+    """(block, window, random, seed) of block-sparse attention layers: sparse_block_size (16, the default, 32 or 64),
+    sparse_local_window_blocks (an integer >= 1, default 4), sparse_random_blocks (an integer >= 0, default
+    seq_len // block // 4, DALLE-pytorch's) and sparse_layout_seed (an integer >= 0, default 0).  None takes the
+    default; anything else that is not such an integer raises a ValueError naming the key."""
+    b = 16 if block_size is None else block_size
+    if isinstance(b, bool) or not isinstance(b, numbers.Integral) or b not in SPARSE_BLOCK_SIZES:
+        raise ValueError(f"sparse_block_size must be one of {SPARSE_BLOCK_SIZES}, got {block_size!r}")
+    b = int(b)
+    w = _sparse_int("sparse_local_window_blocks", 4 if local_window_blocks is None else local_window_blocks, 1)
+    r = _sparse_int("sparse_random_blocks", seq_len // b // 4 if random_blocks is None else random_blocks, 0)
+    seed = _sparse_int("sparse_layout_seed", 0 if layout_seed is None else layout_seed, 0)
+    return b, w, r, seed
+
+
+def block_sparse_layout(seq_len, text_seq_len, block, local_window_blocks, random_blocks, seed, owner):
+    """The block layout of a block-sparse layer (DeepSpeed's VariableSparsityConfig as DALLE-pytorch configures it,
+    unidirectional, one layout for every head): bool [nb, nb], nb = ceil(seq_len / block), where layout[r][c] lets the
+    queries of block r see the keys of block c <= r.  An entry is set when
+    - c < ceil(text_seq_len / block) (global blocks: the caption, vertical only);
+    - c // w == r // w (local windows of w = local_window_blocks blocks aligned from block 0, the diagonal included);
+    - c is one of min(R, r + 1) distinct blocks of [0, r] drawn at random, R = random_blocks: the rows r = 0 .. nb - 1
+      in order, each rng.choice(r + 1, min(R, r + 1), replace=False) with rng = numpy.random.Generator(PCG64(
+      SeedSequence([seed, owner]))).  owner is the layer that owns the token mixer (shared_attn_ids), so layers that
+      share attention share the layout.
+    The random draw is from the causal range [0, r], unlike DeepSpeed's (DESIGN.md).  A pure function of its
+    arguments: the same on every rank and at generation time."""
+    import numpy as np
+    nb = -(-seq_len // block)
+    lay = np.zeros((nb, nb), dtype=bool)
+    rng = np.random.Generator(np.random.PCG64(np.random.SeedSequence([int(seed), int(owner)])))
+    for r in range(nb):
+        lay[r, rng.choice(r + 1, min(random_blocks, r + 1), replace=False)] = True
+    idx = np.arange(nb)
+    lay |= (idx[None, :] // local_window_blocks) == (idx[:, None] // local_window_blocks)
+    lay[:, :-(-text_seq_len // block)] = True
+    return np.tril(lay)
+
+
+def layer_block_sparse(attention_types, text_seq_len, image_seq_len, n_layers, attn_owner=None, block_size=None,
+                       local_window_blocks=None, random_blocks=None, layout_seed=None):
+    """Per-layer block-sparse layout: block_sparse_layout of the layer's token-mixer owner for a "block_sparse" layer
+    and None for any other.  The keys are validated (validate_block_sparse) whether or not such a layer exists."""
+    S = text_seq_len + image_seq_len
+    b, w, r, seed = validate_block_sparse(block_size, local_window_blocks, random_blocks, layout_seed, S)
+    if attention_types is None:
+        return [None] * n_layers
+    owner = list(range(n_layers)) if attn_owner is None else attn_owner
+    layouts = {o: block_sparse_layout(S, text_seq_len, b, w, r, seed, o)
+               for o, t in zip(owner, attention_types) if t == "block_sparse"}
+    return [layouts[owner[i]] if t == "block_sparse" else None for i, t in enumerate(attention_types)]
 
 
 POSITION_EMBEDDINGS = ("absolute", "row_col")
@@ -464,6 +526,7 @@ class DalleEngine:
     VECTOR_PARAMS = ("ln1_g", "ln1_b", "o_b", "ln2_g", "ln2_b", "b1", "b2", "lna_g", "lna_b", "lnm_g", "lnm_b", "lnf_g",
                      "lnf_b", "bout", "gm_bin", "sgu_g", "sgu_b", "sgu_c", "gm_bout", "lsa", "lsm")
     conv = None   # per-layer conv geometry (layer_conv), set by the constructor; None: no conv layer
+    block_sparse = None   # per-layer ops.BlockSparse (layer_block_sparse), set by the constructor; None: none
     gated_mlp = False   # the gated MLP (validate_gated_mlp), set by the constructor
     shift_tokens = False   # the token shift (validate_shift_tokens), set by the constructor
     sandwich_norm = False   # the sandwich LayerNorm (validate_sandwich_norm), set by the constructor
@@ -478,7 +541,8 @@ class DalleEngine:
                  conv_attention_kernel=5, image_position_embedding=None, per_position_padding=False,
                  activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False,
                  shift_tokens=False, sandwich_norm=False, layer_scale=None, stable=False, share_input_output_emb=False,
-                 shared_attn_ids=None, shared_ff_ids=None):
+                 shared_attn_ids=None, shared_ff_ids=None, sparse_block_size=16, sparse_local_window_blocks=4,
+                 sparse_random_blocks=None, sparse_layout_seed=0):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -588,7 +652,14 @@ class DalleEngine:
         ff id one MLP (w1, b1, w2, b2).  LayerNorms, sandwich LayerNorms, LayerScale and decode caches stay per layer.
         A shared module belongs to its lowest user (attn_owner / ff_owner): it is initialised and checkpointed there,
         and the other users' names are layout aliases of its entries, so their gradients add into its slot.  Layers
-        sharing an attention id must have the same attention type."""
+        sharing an attention id must have the same attention type.
+
+        A "block_sparse" entry of attention_types makes that layer DeepSpeed-style block-sparse attention
+        (DALLE-pytorch's SparseAttention): query i sees key j <= i iff layout[i // b][j // b] of block_sparse_layout,
+        with b = sparse_block_size, the local window sparse_local_window_blocks, sparse_random_blocks random blocks per
+        row and sparse_layout_seed (validate_block_sparse).  The layout is drawn per token-mixer owner and is the same
+        for every head; it is not a variable, so sampling must use the training config's keys.  No attention dropout
+        (the layer's site is unused); residual dropout is unchanged."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
@@ -645,6 +716,14 @@ class DalleEngine:
         # per layer: None or the (text_len, grid_w, kernel) of a conv layer, and the attention ops' keyword for it
         self.conv = layer_conv(attention_types, text_seq_len, image_seq_len, conv_attention_kernel, n_layers)
         self.conv_kw = [{} if c is None else {"conv": c} for c in self.conv]
+        # per layer: None or the ops.BlockSparse of a block-sparse layer (one per token-mixer owner), and its keyword
+        sparse = validate_block_sparse(sparse_block_size, sparse_local_window_blocks, sparse_random_blocks,
+                                       sparse_layout_seed, self.S)
+        layouts = layer_block_sparse(attention_types, text_seq_len, image_seq_len, n_layers, self.attn_owner,
+                                     *sparse)
+        tables = {id(lay): ops.BlockSparse(lay, sparse[0], self.S, self.device) for lay in layouts if lay is not None}
+        self.block_sparse = [None if lay is None else tables[id(lay)] for lay in layouts]
+        self.block_sparse_kw = [{} if m is None else {"block_sparse": m} for m in self.block_sparse]
         # per layer: True for a gMLP token-mixing layer
         self.mlp = layer_mlp(attention_types, n_layers, self.S, n_embd)
         lw = (None, None) if loss_weights is None else tuple(loss_weights)
@@ -1290,7 +1369,7 @@ class DalleEngine:
             "wte": mk(emb, L.SITE_WTE, rows0), "wpe": mk(emb, L.SITE_WPE, 0),
             "attn": [mk(att, L.dropout_site_attn(i), row0)
                      if self.radii[i] is None and self.axial[i] is None and (self.conv is None or self.conv[i] is None)
-                     and not self._is_mlp(i) else None
+                     and (self.block_sparse is None or self.block_sparse[i] is None) and not self._is_mlp(i) else None
                      for i in range(self.L)],
             "attn_out": [mk(res, L.dropout_site_attn_out(i), rows0) for i in range(self.L)],
             "mlp_out": [mk(res, L.dropout_site_mlp_out(i), rows0) for i in range(self.L)],
@@ -1348,7 +1427,7 @@ class DalleEngine:
                 ops.rope_fwd(sv["qkv"], self.rope_table, S or self.S, self.H, self.dh, self.rotary_dim)
             ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
                          dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
-                         **self.conv_kw[i])  # :257-299
+                         **self.conv_kw[i], **self.block_sparse_kw[i])  # :257-299
             self._branch_out(p, "a", sv["attn"], self.W(p + "wo"), self.P(p + "o_b"), x_in, sv["xmid"],
                              self._site("attn_out", i), sv)                     # :303-314,330
         self._layernorm_fwd(sv["xmid"], p, 2, sv, S or self.S)
@@ -1670,7 +1749,7 @@ class DalleEngine:
             ops.linear_wgrad(sv["attn"], da, self.G(p + "wo"))
             ops.attn_bwd(sv["qkv"], sv["attn"], bufs["dtmp"], sv["lse"], bufs["dq_acc"], bufs["delta"], bufs["dqkv"],
                          B, self.S, self.H, self.dh, self.attn_scale, dropout=self._site("attn", i),
-                         radius=self.radii[i], **self.axial_kw[i], **self.conv_kw[i])
+                         radius=self.radii[i], **self.axial_kw[i], **self.conv_kw[i], **self.block_sparse_kw[i])
             if self.rotary:   # d(q|k|v) before the rotation
                 ops.rope_bwd(bufs["dqkv"], self.rope_table, self.S, self.H, self.dh, self.rotary_dim)
             ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                  # dLN1 out

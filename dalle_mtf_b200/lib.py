@@ -160,6 +160,10 @@ _SIGNATURES = {
                                 c_f32],
     "db200_attn_decode_axial_dev": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                     c_f32],
+    "db200_attn_decode_block_sparse": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int,
+                                       c_f32],
+    "db200_attn_decode_block_sparse_dev": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int,
+                                           c_f32],
     "db200_attn_decode_conv": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                c_f32],
     "db200_attn_decode_conv_dev": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
@@ -211,6 +215,9 @@ _SIGNATURES = {
     "db200_attn_axial_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_axial_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                              c_int, c_f32],
+    "db200_attn_block_sparse_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_f32],
+    "db200_attn_block_sparse_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp,
+                                    c_int, c_f32],
     "db200_attn_conv_fwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f32],
     "db200_attn_conv_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int,
                             c_int, c_f32],

@@ -17,7 +17,7 @@ from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
     validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
     validate_layer_scale, validate_rotary, validate_sandwich_norm, validate_share_input_output_emb, \
-    validate_shared_ids, validate_shift_tokens, validate_stable
+    validate_shared_ids, validate_shift_tokens, validate_stable, validate_block_sparse
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -116,9 +116,10 @@ def attention_layers(params):
     local_attention_radius: the reference's key (src/dalle_mtf/models.py:259, default 256), an integer >= 1.
     attention_types: per-layer attention types in GPT-Neo's form, e.g. [[["global", "local"], 3]]: each inner list is
     repeated `count` times and the expansion must give "global", "local", "axial_row", "axial_col" or "conv" (DALL-E's
-    row, column and convolutional attention over the image-token grid, DalleEngine) for exactly n_layers layers.  A
-    missing or null key is None: every layer global.  Returns the expanded list (or None) and the radius; the kernel
-    size of conv layers is conv_kernel's."""
+    row, column and convolutional attention over the image-token grid, DalleEngine), "mlp" (gMLP) or "block_sparse"
+    (DeepSpeed-style block-sparse attention) for exactly n_layers layers.  A missing or null key is None: every layer
+    global.  Returns the expanded list (or None) and the radius; the kernel size of conv layers is conv_kernel's, the
+    layout of block-sparse layers block_sparse_options'."""
     v = params.get("local_attention_radius")
     radius = 256 if v is None else v
     if isinstance(radius, bool) or not isinstance(radius, int) or radius < 1:
@@ -256,6 +257,18 @@ def conv_kernel(params):
         raise ValueError(f"conv_attention_kernel = {v!r}: must be an integer >= 1") from None
 
 
+def block_sparse_options(params):
+    """The DalleEngine keywords of block-sparse layers from a DALL-E config: sparse_block_size (16, 32 or 64; default
+    16), sparse_local_window_blocks (an integer >= 1; default 4), sparse_random_blocks (an integer >= 0; a missing or
+    null key is DALLE-pytorch's seq_len // block // 4, resolved by the engine) and sparse_layout_seed (an integer >= 0;
+    default 0, independent of `seed`).  Any other value raises a ValueError naming the key.  The layout is not stored
+    in checkpoints, so sampling must use the training config's keys."""
+    keys = ("sparse_block_size", "sparse_local_window_blocks", "sparse_random_blocks", "sparse_layout_seed")
+    opts = {k: params.get(k) for k in keys}
+    validate_block_sparse(*opts.values(), seq_len=0)
+    return opts
+
+
 def caption_dropout(params):
     """(rate, padding_id) of the config's caption dropout: in mode "train", each sequence's caption is replaced by
     padding_id at every text position with probability `caption_dropout` (a missing or null key is 0), so the model
@@ -334,6 +347,7 @@ def dalle_model_fn(features, labels, mode, params):
     cap_rate, pad_id = caption_dropout(params)
     attention_types, local_radius = attention_layers(params)
     conv_k = conv_kernel(params)
+    sparse = block_sparse_options(params)
     weights, z_loss = loss_weights(params)
     pos_scheme, per_pos, pp_pad = input_embedding(params)
     activation = activation_function(params)
@@ -381,7 +395,8 @@ def dalle_model_fn(features, labels, mode, params):
                         image_position_embedding=pos_scheme, per_position_padding=per_pos,
                         activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
                         gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich, layer_scale=scale,
-                        stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids)
+                        stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids,
+                        **sparse)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

@@ -6,9 +6,9 @@ import torch
 
 from . import lib as L
 from .dalle_engine import DalleEngine
-from .model_fns import activation_function, attention_layers, conv_kernel, dropout_rates, gated_mlp, \
-    input_embedding, layer_scale, logits_mask, loss_weights, rotary_embedding, sandwich_norm, share_input_output_emb, \
-    shared_attn_ids, shared_ff_ids, shift_tokens, stable, validate_kl_weight
+from .model_fns import activation_function, attention_layers, block_sparse_options, conv_kernel, dropout_rates, \
+    gated_mlp, input_embedding, layer_scale, logits_mask, loss_weights, rotary_embedding, sandwich_norm, \
+    share_input_output_emb, shared_attn_ids, shared_ff_ids, shift_tokens, stable, validate_kl_weight
 from .model_fns import build_vae_engine, vae_architecture
 from .model_fns import reconstruction_loss as _reconstruction_loss
 
@@ -27,6 +27,7 @@ class DALLE:
         params = params or {}
         attention_types, local_radius = attention_layers({**params, "n_layers": n_layers})
         conv_k = conv_kernel(params)
+        sparse = block_sparse_options(params)
         weights, z_loss = loss_weights(params)
         pos_scheme, per_pos, _ = input_embedding({**params, "text_vocab_size": text_vocab_size})
         activation = activation_function(params)
@@ -56,7 +57,8 @@ class DALLE:
                                   activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
                                   rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift,
                                   sandwich_norm=sandwich, layer_scale=scale, stable=stab,
-                                  share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids)
+                                  share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids,
+                                  **sparse)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

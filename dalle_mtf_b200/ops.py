@@ -555,8 +555,8 @@ def split_f32(src, hi, lo=None):
 # bench.py sets ATTN_PROFILE to a list to time every attention launch like GEMM_PROFILE: entries are
 # (start_event, end_event, causal-algorithmic flops, "fwd" | "bwd").  Forward = 2 products over the visible half of the
 # S x S logits: 4 S^2 dh B H / 2; backward = 2.5 x that (5 products).  A local launch counts the (query, key) pairs of
-# its band instead: sum_i min(i + 1, radius); an axial (convolutional) launch those of its mask (attn_pairs_axial,
-# attn_pairs_conv).
+# its band instead: sum_i min(i + 1, radius); an axial (convolutional, block-sparse) launch those of its mask
+# (attn_pairs_axial, attn_pairs_conv, attn_pairs_block_sparse).
 ATTN_PROFILE = None
 
 
@@ -592,7 +592,55 @@ def attn_pairs_conv(S, text_len, grid_w, kernel):
     return float(m * (m + 1) // 2 + n * text_len + image)
 
 
-def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None, conv=None):
+def attn_pairs_block_sparse(S, layout, block):
+    """(query, key) pairs a block-sparse attention of length S computes: the pairs j <= i < S with
+    layout[i // block][j // block] set."""
+    import numpy as np
+    lay = np.asarray(layout, dtype=bool)
+    n = -(-S // block)
+    size = np.minimum(block, S - block * np.arange(n))   # positions of each block below S
+    lay = np.tril(lay[:n, :n], -1)
+    diag = np.asarray(layout, dtype=bool).diagonal()[:n]
+    return float(size @ lay @ size + (diag * size * (size + 1) // 2).sum())
+
+
+class BlockSparse:
+    """The mask of a block-sparse attention layer of length S: layout[r][c] (bool [ceil(S / block)]^2, lower
+    triangular) lets the queries of block r see the keys of block c, under the causal mask; block is a multiple of 16.
+    Holds it as the kernels read it (include/dalle_b200.h): `tiles`, int16 [ceil(S / 64)]^2 tile masks for
+    db200_attn_block_sparse_fwd / _bwd, and `blocks`, int32 [ceil(S / 16), ceil(S / 16) + 1] block lists for
+    db200_attn_decode_block_sparse(_dev).  A launch of length P <= S (a prefill) uses the same tables."""
+
+    def __init__(self, layout, block, S, device="cuda"):
+        import numpy as np
+        lay = np.asarray(layout, dtype=bool)
+        nb = -(-S // block)
+        if block < 16 or block % 16 or lay.shape != (nb, nb) or (np.triu(lay, 1)).any():
+            raise L.DB200Error(f"BlockSparse: a lower-triangular [{nb}, {nb}] layout of blocks of a multiple of 16 "
+                               f"tokens is needed for S {S}, got shape {lay.shape}, block {block}")
+        self.layout, self.block, self.S = lay, int(block), int(S)
+        f = block // 16
+        ng = -(-S // 16)
+        g = np.arange(ng) // f
+        lay16 = np.tril(lay[g][:, g])             # the layout at 16-token granularity, [ng, ng]
+        nt = -(-S // 64)
+        pad = np.zeros((4 * nt, 4 * nt), dtype=bool)
+        pad[:ng, :ng] = lay16
+        bits = pad.reshape(nt, 4, nt, 4).transpose(0, 2, 1, 3).reshape(nt, nt, 16)   # [qt, kt, 4 a + c]
+        tiles = (bits.astype(np.int64) << np.arange(16)).sum(-1)
+        self.tiles = torch.from_numpy(tiles.astype(np.uint16).view(np.int16)).to(device)
+        lists = np.zeros((ng, ng + 1), dtype=np.int32)
+        for r in range(ng):
+            cols = np.flatnonzero(lay16[r])
+            lists[r, 0] = cols.size
+            lists[r, 1:1 + cols.size] = cols
+        self.blocks = torch.from_numpy(lists).to(device)
+
+    def pairs(self, S):
+        return attn_pairs_block_sparse(S, self.layout, self.block)
+
+
+def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None, conv=None, block_sparse=None):
     prof = ATTN_PROFILE
     if prof is None:
         return call()
@@ -601,7 +649,8 @@ def _attn_timed(kind, B, S, H, dh, call, radius=None, axial=None, conv=None):
     call()
     ev1.record()
     pairs = attn_pairs_axial(S, *axial) if axial is not None else \
-        attn_pairs_conv(S, *conv) if conv is not None else attn_pairs(S, radius)
+        attn_pairs_conv(S, *conv) if conv is not None else \
+        block_sparse.pairs(S) if block_sparse is not None else attn_pairs(S, radius)
     prof.append((ev0, ev1, 4.0 * pairs * dh * B * H * (1.0 if kind == "fwd" else 2.5), kind))
 
 
@@ -635,20 +684,41 @@ def _conv(conv, radius, axial, dropout, what):
     return tuple(int(v) for v in conv)
 
 
-def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, axial=None, conv=None):
+def _block_sparse(bs, radius, axial, conv, dropout, S, what):
+    """Validated BlockSparse of a block-sparse launch of length S, or None."""
+    if bs is None:
+        return None
+    if radius is not None or axial is not None or conv is not None or dropout is not None:
+        raise L.DB200Error(f"{what}: block-sparse attention takes no radius, no axial or conv geometry and no dropout")
+    if not isinstance(bs, BlockSparse):
+        raise L.DB200Error(f"{what}: block_sparse must be an ops.BlockSparse, got {type(bs).__name__}")
+    if S > bs.S:
+        raise L.DB200Error(f"{what}: length {S} exceeds the block-sparse layout's {bs.S}")
+    return bs
+
+
+def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, axial=None, conv=None,
+             block_sparse=None):
     """dropout: lib.Dropout of the attention-weights site (row0 = global index of sequence 0), or None.
     radius: None = causal attention; else local attention, query i over keys (i - radius, i] (no dropout).
     axial: (text_len, grid_w, axis) = row (axis 0) or column (axis 1) attention of the image tokens of a text_len
     caption and a grid_w x grid_w image (db200_attn_axial_fwd); excludes radius and dropout.
     conv: (text_len, grid_w, kernel) = convolutional attention over the same grid, the image query at (r, c) over the
     caption and the kernel x kernel window of image tokens (r - kernel, r] x (c - kernel, c] (db200_attn_conv_fwd);
-    excludes radius, axial and dropout."""
+    excludes radius, axial and dropout.
+    block_sparse: a BlockSparse of length >= S = block-sparse attention over its layout (db200_attn_block_sparse_fwd);
+    excludes radius, axial, conv and dropout."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(lse, F32, "lse")
+    bs = _block_sparse(block_sparse, radius, axial, conv, dropout, S, "attn_fwd")
     conv = _conv(conv, radius, axial, dropout, "attn_fwd")
     axial = _axial(axial, radius, dropout, "attn_fwd")
     radius = _radius(radius)
-    if conv is not None:
+    if bs is not None:
+        call = lambda: check(L.load().db200_attn_block_sparse_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H,
+                                                                  dh, ptr(bs.tiles), bs.tiles.shape[1], scale),
+                             "attn_block_sparse_fwd")
+    elif conv is not None:
         call = lambda: check(L.load().db200_attn_conv_fwd(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                           *conv, scale), "attn_conv_fwd")
     elif axial is not None:
@@ -665,20 +735,26 @@ def attn_fwd(qkv, out, lse, B, S, H, dh, scale=1.0, dropout=None, radius=None, a
     else:
         call = lambda: check(L.load().db200_attn_causal_fwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(lse), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_fwd_ex")
-    _attn_timed("fwd", B, S, H, dh, call, radius, axial, conv)
+    _attn_timed("fwd", B, S, H, dh, call, radius, axial, conv, bs)
     return out
 
 
 def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0, dropout=None, radius=None,
-             axial=None, conv=None):
-    """radius, axial, conv: as attn_fwd's (None = causal)."""
+             axial=None, conv=None, block_sparse=None):
+    """radius, axial, conv, block_sparse: as attn_fwd's (None = causal)."""
     L.require_device()
     _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(dout, BF16, "dout"); _chk(dqkv, BF16, "dqkv")
     _chk(lse, F32, "lse"); _chk(dq_accum, F32, "dq_accum"); _chk(delta, F32, "delta")
+    bs = _block_sparse(block_sparse, radius, axial, conv, dropout, S, "attn_bwd")
     conv = _conv(conv, radius, axial, dropout, "attn_bwd")
     axial = _axial(axial, radius, dropout, "attn_bwd")
     radius = _radius(radius)
-    if conv is not None:
+    if bs is not None:
+        call = lambda: check(L.load().db200_attn_block_sparse_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
+                                                                  ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh,
+                                                                  ptr(bs.tiles), bs.tiles.shape[1], scale),
+                             "attn_block_sparse_bwd")
+    elif conv is not None:
         call = lambda: check(L.load().db200_attn_conv_bwd(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                           ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh, *conv,
                                                           scale), "attn_conv_bwd")
@@ -700,7 +776,7 @@ def attn_bwd(qkv, out, dout, lse, dq_accum, delta, dqkv, B, S, H, dh, scale=1.0,
         call = lambda: check(L.load().db200_attn_causal_bwd_ex(stream_ptr(), ptr(qkv), ptr(out), ptr(dout), ptr(lse),
                                                                ptr(dq_accum), ptr(delta), ptr(dqkv), B, S, H, dh,
                                                                scale, ctypes.byref(dropout)), "attn_causal_bwd_ex")
-    _attn_timed("bwd", B, S, H, dh, call, radius, axial, conv)
+    _attn_timed("bwd", B, S, H, dh, call, radius, axial, conv, bs)
     return dqkv
 
 
@@ -1007,18 +1083,27 @@ def embed_fwd_at(ids, wte, wpe, out, pos):
     return out
 
 
-def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None, axial=None, conv=None):
+def attn_decode(qkv_step, k_cache, v_cache, out, pos, scale, radius=None, axial=None, conv=None, block_sparse=None):
     """Append this position's k, v to the caches and attend with its q over keys <= pos (models.py:246-254, 281-299);
     radius (local layer, models.py:257-273): over keys [max(0, pos - radius + 1), pos] only; axial (text_len, grid_w,
     axis) (row / column layer, attn_fwd's): over the text keys and pos's image row (axis 0) or column (axis 1); conv
-    (text_len, grid_w, kernel) (convolutional layer, attn_fwd's): over the text keys and pos's kernel x kernel window."""
+    (text_len, grid_w, kernel) (convolutional layer, attn_fwd's): over the text keys and pos's kernel x kernel window;
+    block_sparse (a BlockSparse of the caches' length, attn_fwd's): over the keys <= pos of the blocks its layout lets
+    pos's block see."""
     L.require_device()
     _chk(qkv_step, BF16, "qkv_step"); _chk(k_cache, BF16, "k_cache"); _chk(v_cache, BF16, "v_cache"); _chk(out, BF16, "out")
     B, S, H, dh = k_cache.shape
     assert v_cache.shape == k_cache.shape and qkv_step.numel() == B * 3 * H * dh and out.numel() == B * H * dh
+    bs = _block_sparse(block_sparse, radius, axial, conv, None, S, "attn_decode")
     conv = _conv(conv, radius, axial, None, "attn_decode")
     axial = _axial(axial, radius, None, "attn_decode")
     radius = _radius(radius)
+    if bs is not None:
+        check(L.load().db200_attn_decode_block_sparse(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache),
+                                                      ptr(out), B, S, H, dh, int(pos), ptr(bs.blocks),
+                                                      bs.blocks.shape[1], float(scale)),
+              "db200_attn_decode_block_sparse")
+        return out
     if conv is not None:
         check(L.load().db200_attn_decode_conv(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B, S,
                                               H, dh, int(pos), *conv, float(scale)), "db200_attn_decode_conv")
@@ -1058,13 +1143,21 @@ def embed_fwd_at_dev(tokens, wte, wpe, out, pos_dev):
     return out
 
 
-def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None, axial=None, conv=None):
+def attn_decode_dev(qkv_step, k_cache, v_cache, out, pos_dev, scale, radius=None, axial=None, conv=None,
+                    block_sparse=None):
     """attn_decode with the position read on the device from pos_dev (graph replay)."""
     L.require_device()
     B, S, H, dh = k_cache.shape
+    bs = _block_sparse(block_sparse, radius, axial, conv, None, S, "attn_decode_dev")
     conv = _conv(conv, radius, axial, None, "attn_decode_dev")
     axial = _axial(axial, radius, None, "attn_decode_dev")
     radius = _radius(radius)
+    if bs is not None:
+        check(L.load().db200_attn_decode_block_sparse_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache),
+                                                          ptr(out), B, S, H, dh, ptr(pos_dev), ptr(bs.blocks),
+                                                          bs.blocks.shape[1], float(scale)),
+              "db200_attn_decode_block_sparse_dev")
+        return out
     if conv is not None:
         check(L.load().db200_attn_decode_conv_dev(stream_ptr(), ptr(qkv_step), ptr(k_cache), ptr(v_cache), ptr(out), B,
                                                   S, H, dh, ptr(pos_dev), *conv, float(scale)),

@@ -9,7 +9,8 @@ parameters and the same kernels' numerics as training:
   per position p:   x = wte[token] + wpe[p]                                     (embed_fwd_at)
   per layer:        q|k|v = LN1(x) Wqkv;  cache[p] = k, v;  a = softmax_{j<=p}(q.k_j) v_j   (attn_decode;
                     a local layer of radius r takes j > p - r only, models.py:257-273; an axial layer the text
-                    positions and p's image row or column; a conv layer the text positions and p's k x k window)
+                    positions and p's image row or column; a conv layer the text positions and p's k x k window;
+                    a block-sparse layer the positions <= p of the blocks its layout lets p's block see)
                     x = x + a Wo + o_b;  x = x + act(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows;
                     act = ReLU, or GELU without a pre-activation output); with rotary embeddings q and k are
                     rotated to position p (rope_decode) before k enters the cache; with the token shift each
@@ -148,7 +149,7 @@ class DalleSampler:
                 if e.rotary:
                     ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
                 ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
-                                **e.axial_kw[i], **e.conv_kw[i])
+                                **e.axial_kw[i], **e.conv_kw[i], **e.block_sparse_kw[i])
                 self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
@@ -179,7 +180,7 @@ class DalleSampler:
                 if e.rotary:
                     ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
                 ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
-                                    radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i])
+                                    radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i], **e.block_sparse_kw[i])
                 self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:

@@ -18,8 +18,8 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
-from dalle_mtf_b200.model_fns import activation_function, attention_layers, conv_kernel, gated_mlp, \
-    input_embedding, layer_scale, logits_mask, rotary_embedding, sandwich_norm, share_input_output_emb, \
+from dalle_mtf_b200.model_fns import activation_function, attention_layers, block_sparse_options, conv_kernel, \
+    gated_mlp, input_embedding, layer_scale, logits_mask, rotary_embedding, sandwich_norm, share_input_output_emb, \
     shared_attn_ids, shared_ff_ids, shift_tokens, stable, \
     vae_checkpoint, vae_grid_size
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
@@ -154,6 +154,7 @@ def main(argv=None):
     tl, tv, iv = params["text_seq_len"], params["text_vocab_size"], params["image_vocab_size"]
     attention_types, local_radius = attention_layers(params)    # the layer types the checkpoint was trained with
     conv_k = conv_kernel(params)
+    sparse = block_sparse_options(params)              # and the block-sparse layout (not stored in the checkpoint)
     pos_scheme, per_pos, _ = input_embedding(params)   # the input embedding the checkpoint was trained with
     activation = activation_function(params)           # and its MLP nonlinearity
     gated = gated_mlp(params)                           # and whether that MLP is gated
@@ -206,7 +207,7 @@ def main(argv=None):
                       per_position_padding=per_pos, activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
                       rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich,
                       layer_scale=scale, stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids,
-                      shared_ff_ids=ff_ids)
+                      shared_ff_ids=ff_ids, **sparse)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})

@@ -407,6 +407,20 @@ int db200_attn_conv_bwd(db200_stream_t stream, const void* qkv_bf16, const void*
                         const float* lse, float* dq_accum, float* delta, void* dqkv_bf16, int B, int S, int H, int dh,
                         int text_len, int grid_w, int kernel, float scale);
 
+/* Block-sparse attention (DeepSpeed's fixed / variable sparsity layouts, DALLE-pytorch's SparseAttention), described
+ * at 16-token granularity by a device table of 16-bit tile masks: tile_mask[qt * mask_pitch + kt] (kt <= qt) for the
+ * 64 x 64 tile of queries 64 qt .. 64 qt + 63 and keys 64 kt .. 64 kt + 63; bit 4 a + c set means the queries
+ * 64 qt + 16 a .. + 15 may see the keys 64 kt + 16 c .. + 15.  Query i attends to key j iff j <= i, j < S and the bit of
+ * (i, j) is set; the same mask serves every head and sequence.  The kernels skip the tiles whose mask is 0 and read
+ * the rows qt < ceil(S / 64) of the table only, so a prompt prefill (S shorter than the layout's length) passes the
+ * full table.  A query that sees no key gets out = 0.  Layouts, workspaces and numerics as db200_attn_causal_fwd /
+ * _bwd; with every causal bit set the results are bit for bit db200_attn_causal_fwd / _bwd's.  No dropout.  A NULL tile_mask or mask_pitch < ceil(S / 64): DB200_E_INVALID. */
+int db200_attn_block_sparse_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, float* lse, int B, int S,
+                                int H, int dh, const uint16_t* tile_mask, int mask_pitch, float scale);
+int db200_attn_block_sparse_bwd(db200_stream_t stream, const void* qkv_bf16, const void* out_bf16,
+                                const void* dout_bf16, const float* lse, float* dq_accum, float* delta, void* dqkv_bf16,
+                                int B, int S, int H, int dh, const uint16_t* tile_mask, int mask_pitch, float scale);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * small HBM-bound helpers
  * ------------------------------------------------------------------------------------------------------------------ */
@@ -651,6 +665,18 @@ int db200_attn_decode_conv(db200_stream_t stream, const void* qkv_step_bf16, voi
 int db200_attn_decode_conv_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
                                void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
                                const int32_t* pos_dev, int text_len, int grid_w, int kernel, float scale);
+/* attn_decode / attn_decode_dev of a block-sparse layer: the query of position p attends to the keys of the 16-key
+ * blocks listed for 16-row block g = p / 16, clipped at p.  `blocks` is a device table of rows of blocks_pitch int32:
+ * row g holds a count n_g followed by n_g distinct block indices in ascending order, each <= g (the layout of
+ * db200_attn_block_sparse_fwd at 16-token granularity).  A position whose row lists no block gets out = 0.  Shared
+ * memory and key counts as db200_attn_decode / _dev.  A NULL table or blocks_pitch < ceil(S / 16) + 1:
+ * DB200_E_INVALID. */
+int db200_attn_decode_block_sparse(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
+                                   void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh, int pos,
+                                   const int32_t* blocks, int blocks_pitch, float scale);
+int db200_attn_decode_block_sparse_dev(db200_stream_t stream, const void* qkv_step_bf16, void* k_cache_bf16,
+                                       void* v_cache_bf16, void* out_bf16, int B, int S, int H, int dh,
+                                       const int32_t* pos_dev, const int32_t* blocks, int blocks_pitch, float scale);
 int db200_sample_rows_at(db200_stream_t stream, const float* logits, const float* u_or_null, int32_t* tokens,
                          long long ld_tokens, int rows, long long ld, int lo, int hi, float inv_temp,
                          const int32_t* pos_dev);

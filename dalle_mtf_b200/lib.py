@@ -248,6 +248,11 @@ _SIGNATURES = {
     "db200_gumbel_softmax_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_int],
     "db200_gumbel_softmax_bwd": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32],
     "db200_argmax_rows_f32": [c_vp, c_vp, c_vp, c_int, c_int],
+    "db200_groupnorm_stats": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32, c_vp, c_i64],
+    "db200_groupnorm_apply": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_attn_noncausal_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_f32],
+    "db200_gather_rows_split": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
+    "db200_clamp_bf16_to_f32": [c_vp, c_vp, c_vp, c_i64, c_f32, c_f32],
     "db200_vae_kl_stats": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_vp, c_i64],
     "db200_gumbel_softmax_bwd_kl": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_f32],
     "db200_mse_fwd_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_sz, c_f32],
@@ -279,6 +284,7 @@ _WORKSPACE_QUERIES = {
     "db200_vae_kl_stats_workspace_bytes": [c_int, c_int],
     "db200_logit_laplace_workspace_bytes": [c_i64, c_int],
     "db200_conv7x7_in_wgrad_workspace_bytes": [c_int, c_int, c_int, c_int, c_int],
+    "db200_groupnorm_stats_workspace_bytes": [c_int, c_int, c_int, c_int],
 }
 EXPORTED_SYMBOLS = ["db200_last_error", "db200_launch_count"] + sorted(_SIGNATURES) + sorted(_WORKSPACE_QUERIES)
 

@@ -23,6 +23,7 @@ from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
 from .vae_engine import RECONSTRUCTION_LOSSES, VaeEngine, codebook_usage
 from .vae_paper_engine import PaperVaeEngine, check_paper_geometry
+from .vqgan_engine import VqganEngine, check_vqgan_geometry
 
 TRAIN, EVAL, PREDICT = "train", "eval", "predict"   # tf.estimator.ModeKeys values
 
@@ -577,7 +578,8 @@ def reconstruction_loss(value):
     return value
 
 
-VAE_ARCHITECTURES = ("reference", "dalle_paper")
+VAE_ARCHITECTURES = ("reference", "dalle_paper", "vqgan")
+VQGAN_KEYS = ("ch", "ch_mult", "num_res_blocks", "attn_resolutions", "z_channels", "embed_dim", "resolution")
 PAPER_VAE_DEFAULTS = {"n_hid": 256, "n_blk_per_group": 2, "group_count": 4, "n_init": 128}
 
 
@@ -589,6 +591,8 @@ def vae_architecture(params, image_size):
     arch = params.get("architecture")
     if arch is None or arch == "reference":
         return None
+    if arch == "vqgan":
+        return vqgan_geometry(params, image_size)
     if arch != "dalle_paper":
         raise ValueError(f"architecture = {arch!r}: must be one of {VAE_ARCHITECTURES} (or null)")
     if params.get("convblocks") is not None:
@@ -602,10 +606,37 @@ def vae_architecture(params, image_size):
     return geo
 
 
+def vqgan_geometry(params, image_size):
+    """The geometry of a VAE config with architecture "vqgan" (taming's ddconfig key names; num_tokens is taming's
+    n_embed): {ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim, resolution}.  Raises ValueError,
+    naming the key, for a missing key, for keys of the other networks, for use_bf16 false (the tokenizer runs bf16
+    activations only) and for a geometry the kernels do not cover."""
+    for k in ("convblocks", "n_hid", "n_blk_per_group", "group_count", "n_init"):
+        if params.get(k) is not None:
+            raise ValueError(f"{k} sizes another network; architecture \"vqgan\" is sized by taming's keys "
+                             f"{VQGAN_KEYS}")
+    sf = params.get("stack_factor")
+    if sf is not None and sf != 1:
+        raise ValueError(f"stack_factor = {sf!r}: architecture \"vqgan\" takes no stack_factor > 1")
+    if params.get("use_bf16") is False:
+        raise ValueError("use_bf16 = false: architecture \"vqgan\" runs bf16 activations only (DESIGN.md §4)")
+    for k in ("reconstruction_loss", "kl_loss_weight"):
+        if params.get(k) is not None:
+            raise ValueError(f"{k}: a VQGAN tokenizer is used frozen and has no training objective here")
+    missing = [k for k in VQGAN_KEYS + ("num_tokens",) if params.get(k) is None]
+    if missing:
+        raise ValueError(f"{missing[0]}: missing from the architecture \"vqgan\" config (keys: {VQGAN_KEYS})")
+    geo = {k: params[k] for k in VQGAN_KEYS}
+    check_vqgan_geometry(image_size, num_tokens=params["num_tokens"], **geo)
+    return geo
+
+
 def vae_grid_size(params, image_size):
-    """Side of a VAE config's token grid: image_size / 2^(group_count - 1) for the paper's network, image_size /
-    stack_factor / 2^len(convblocks) for the reference's."""
+    """Side of a VAE config's token grid: image_size / 2^(len(ch_mult) - 1) for a VQGAN, image_size /
+    2^(group_count - 1) for the paper's network, image_size / stack_factor / 2^len(convblocks) for the reference's."""
     geo = vae_architecture(params, image_size)
+    if params.get("architecture") == "vqgan":
+        return image_size // 2 ** (len(geo["ch_mult"]) - 1)
     if geo is not None:
         return image_size // 2 ** (geo["group_count"] - 1)
     convblocks = params.get("convblocks") or [(3, 64), (3, 128), (3, 256)]
@@ -616,6 +647,9 @@ def build_vae_engine(params, image_size, device, kl=False):
     """The VAE engine of a VAE config (vae_architecture picks the network)."""
     recon = reconstruction_loss(params.get("reconstruction_loss"))
     geo = vae_architecture(params, image_size)
+    if params.get("architecture") == "vqgan":
+        return VqganEngine(num_tokens=params["num_tokens"], image_size=image_size,
+                           input_channels=params.get("input_channels") or 3, device=device, **geo)
     if geo is not None:
         return PaperVaeEngine(num_tokens=params["num_tokens"], image_size=image_size,
                               input_channels=params.get("input_channels") or 3, use_bf16=bool(params.get("use_bf16")),
@@ -645,6 +679,9 @@ def vae_model_fn(features, labels, mode, params):
     kl_on = kl_beta is not None
     recon_loss = reconstruction_loss(params.get("reconstruction_loss"))
     ll = recon_loss == "logit_laplace"
+    if params.get("architecture") == "vqgan":
+        raise ValueError("architecture = \"vqgan\": a VQGAN is imported from taming-transformers "
+                         "(tools/import_vqgan.py), not trained here (that needs LPIPS weights and a discriminator)")
     vae_architecture(params, params["dataset"]["image_size"])   # rejects an invalid network before any device work
     n_aux = 3 if ll else (2 if kl_on else 1)    # aux slots: [recon term, KL, image-space MSE]
     L.require_device()

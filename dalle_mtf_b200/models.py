@@ -10,6 +10,7 @@ from .model_fns import activation_function, attention_layers, block_sparse_optio
     gated_mlp, input_embedding, layer_scale, logits_mask, loss_weights, rotary_embedding, sandwich_norm, \
     share_input_output_emb, shared_attn_ids, shared_ff_ids, shift_tokens, stable, validate_kl_weight
 from .model_fns import build_vae_engine, vae_architecture
+from .utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 from .model_fns import reconstruction_loss as _reconstruction_loss
 
 
@@ -184,3 +185,37 @@ class DiscreteVAE:
         one-hot codes through the tied codebook and the decoder (src/vae_tf/models.py:123-163)."""
         ids = image_token_ids.to(device=self.engine.device, dtype=torch.int32).contiguous()
         return self.engine.decode_tokens(ids, offset)
+
+
+class VQGanVAE:
+    def __init__(self, vae_model, checkpoint=None):
+        """DALLE-pytorch's VQGanVAE over a taming VQGAN imported with tools/import_vqgan.py.  vae_model is a VAE config
+        name or path with architecture "vqgan" (e.g. "vae_vqgan_f16_16384_b200"); checkpoint is this project's
+        checkpoint file (default: the latest one under the config's model_path).
+
+        Images follow this project's convention, f32 NHWC in [-1, 1], not DALLE-pytorch's NCHW in [0, 1]:
+        get_codebook_indices takes such images and decode returns them."""
+        params = fetch_model_params(vae_model) if isinstance(vae_model, str) else vae_model
+        if params.get("architecture") != "vqgan":
+            raise ValueError(f"VQGanVAE: architecture = {params.get('architecture')!r}, expected \"vqgan\"")
+        ckpt = checkpoint or (latest_checkpoint(params["model_path"]) if params.get("model_path") else None)
+        if ckpt is None:
+            raise ValueError(f"VQGanVAE: no checkpoint under {params.get('model_path')!r}: import one with "
+                             "tools/import_vqgan.py")
+        self.engine = build_vae_engine(params, params["dataset"]["image_size"], "cuda")
+        state = load_checkpoint(local_path(ckpt))
+        self.engine.load_params({k[len("vae/"):]: v for k, v in state.items() if k.startswith("vae/")})
+        e = self.engine
+        self.num_tokens, self.image_size = e.K, e.img_H
+        self.num_layers = len(params["ch_mult"]) - 1      # DALLE-pytorch: log2(image_size / grid side)
+        self.channels = 3
+
+    def get_codebook_indices(self, img):
+        """img f32 NHWC [B, H, W, 3] in [-1, 1] -> int32 [B, h * w] nearest codes (raster order)."""
+        img = img.to(device=self.engine.device, dtype=torch.float32).contiguous()
+        return self.engine.encode_tokens(img).clone()
+
+    def decode(self, img_seq, offset=0):
+        """Codes [B, h * w] (minus `offset`) -> images f32 NHWC [B, H, W, 3] in [-1, 1]."""
+        ids = img_seq.to(device=self.engine.device, dtype=torch.int32).contiguous()
+        return self.engine.decode_tokens(ids, offset).clone()

@@ -1015,6 +1015,72 @@ def argmax_rows(x, idx, rows, K):
     check(L.load().db200_argmax_rows_f32(stream_ptr(), ptr(x), ptr(idx), rows, K), "argmax_rows")
 
 
+# the VQGAN tokenizer (include/dalle_b200.h, K14): NHWC bf16 activations
+def groupnorm_stats(x, mean, rstd, groups=32, eps=1e-6):
+    """mean / rstd f32 [N, groups] of x bf16 [N, H, W, C] (biased variance, fp32, fixed-order reduction)."""
+    L.require_device()
+    _chk(x, BF16, "x"); _chk(mean, F32, "mean"); _chk(rstd, F32, "rstd")
+    N, C = x.shape[0], x.shape[-1]
+    HW = x.numel() // (N * C)
+    if mean.numel() != N * groups or rstd.numel() != N * groups:
+        raise L.DB200Error(f"groupnorm_stats: mean / rstd need {N * groups} elements")
+    ws = L.workspace(L.load().db200_groupnorm_stats_workspace_bytes(N, HW, C, groups))
+    check(L.load().db200_groupnorm_stats(stream_ptr(), ptr(x), ptr(mean), ptr(rstd), N, HW, C, groups, float(eps),
+                                         ptr(ws), _nbytes(ws)), "groupnorm_stats")
+
+
+def groupnorm_apply(x, mean, rstd, gamma, beta, y, groups=32, swish=False):
+    """y = (x - mean) rstd gamma + beta [swish], bf16 [N, H, W, C] like x."""
+    L.require_device()
+    _chk(x, BF16, "x"); _chk(y, BF16, "y"); _chk(gamma, F32, "gamma"); _chk(beta, F32, "beta")
+    N, C = x.shape[0], x.shape[-1]
+    if tuple(y.shape) != tuple(x.shape) or gamma.numel() != C or beta.numel() != C:
+        raise L.DB200Error(f"groupnorm_apply: shapes x {tuple(x.shape)} y {tuple(y.shape)} gamma {tuple(gamma.shape)}")
+    check(L.load().db200_groupnorm_apply(stream_ptr(), ptr(x), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(y), N,
+                                         x.numel() // (N * C), C, groups, int(bool(swish))), "groupnorm_apply")
+    return y
+
+
+def groupnorm(x, mean, rstd, gamma, beta, y, groups=32, eps=1e-6, swish=False):
+    groupnorm_stats(x, mean, rstd, groups, eps)
+    return groupnorm_apply(x, mean, rstd, gamma, beta, y, groups, swish)
+
+
+def attn_noncausal(qkv, out, B, S, C, scale):
+    """out bf16 [B, S, C] = softmax(scale q k^T) v of each image's q | k | v bf16 [B, S, 3C]."""
+    L.require_device()
+    _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out")
+    if qkv.numel() != B * S * 3 * C or out.numel() != B * S * C:
+        raise L.DB200Error(f"attn_noncausal: qkv {tuple(qkv.shape)} / out {tuple(out.shape)} do not match B={B}, "
+                           f"S={S}, C={C}")
+    check(L.load().db200_attn_noncausal_fwd(stream_ptr(), ptr(qkv), ptr(out), B, S, C, float(scale)),
+          "attn_noncausal_fwd")
+    return out
+
+
+def gather_rows_split(idx, table, hi, lo=None, offset=0):
+    """hi [rows, D] = bf16(table[idx - offset]), lo = bf16(row - hi); ids outside [offset, offset + K) give zeros."""
+    L.require_device()
+    _chk(idx, I32, "idx"); _chk(table, F32, "table"); _chk(hi, BF16, "hi"); _chk(lo, BF16, "lo")
+    K, D = table.shape
+    rows = idx.numel()
+    if hi.numel() != rows * D or (lo is not None and lo.numel() != rows * D):
+        raise L.DB200Error(f"gather_rows_split: hi / lo need {rows} x {D} elements")
+    check(L.load().db200_gather_rows_split(stream_ptr(), ptr(idx), ptr(table), ptr(hi), ptr(lo), rows, D, K,
+                                           int(offset)), "gather_rows_split")
+
+
+def clamp_bf16_to_f32(src, dst, lo=-1.0, hi=1.0):
+    """dst f32 = clamp(src bf16, lo, hi), elementwise."""
+    L.require_device()
+    _chk(src, BF16, "src"); _chk(dst, F32, "dst")
+    if src.numel() != dst.numel():
+        raise L.DB200Error("clamp_bf16_to_f32: src and dst sizes differ")
+    check(L.load().db200_clamp_bf16_to_f32(stream_ptr(), ptr(src), ptr(dst), src.numel(), float(lo), float(hi)),
+          "clamp_bf16_to_f32")
+    return dst
+
+
 def vae_kl_stats(logits, lse, ent, hist, kl_accum, rows, K, scale):
     """KL(softmax(l) || Uniform(K)) statistics of f32 logits [rows, K]: lse / ent f32 [rows] (logsumexp, sum q (l - lse)),
     hist int32 [K] += the first-maximum code counts, kl_accum[0] += scale * sum of the rows' KL."""

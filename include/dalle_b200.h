@@ -556,6 +556,37 @@ int db200_gumbel_softmax_fwd(db200_stream_t stream, const float* logits, const f
 int db200_gumbel_softmax_bwd(db200_stream_t stream, const float* y_soft, const float* dy, float* dlogits, int rows,
                              int K, float tau);
 int db200_argmax_rows_f32(db200_stream_t stream, const float* x, int32_t* idx, int rows, int K);
+/* ------------------------------------------------------------------------------------------------------------------
+ * K14  a taming-transformers VQGAN tokenizer's forward (extension, architecture "vqgan"; DESIGN.md §4): what its
+ *      encoder and decoder need beyond K11's convolutions, the GEMM, upsample2x_fwd, split and argmax_rows.  NHWC bf16
+ *      activations.  No float atomics; launch geometries depend on HW and C only, so an image's result does not depend
+ *      on N (the batch it is computed in).
+ *   groupnorm_stats: mean / rstd f32 [N][G] of x bf16 [N][HW][C] over each image's HW x C/G values of group g
+ *                    (channels [g C/G, (g + 1) C/G)): per-thread per-channel Welford states over whole pixel rows,
+ *                    combined with Chan's pairwise update in a fixed order, first per chunk of pixel rows into the
+ *                    workspace, then across chunks in chunk order; rstd = 1 / sqrt(M2 / count + eps) (biased).
+ *                    C % 8 == 0, C % G == 0 and C <= 2048, else DB200_E_UNSUPPORTED; x 16-byte aligned.
+ *   groupnorm_apply: y = (x - mean) rstd gamma + beta in f32, then swish(v) = v sigmoid(v) when swish != 0, rounded
+ *                    once to bf16.  gamma / beta f32 [C]; x, y 16-byte aligned.
+ *   attn_noncausal_fwd: one head over each image's S positions: qkv bf16 [B][S][3C] (q | k | v), out bf16 [B][S][C],
+ *                    out_i = sum_j softmax_j(scale q_i . k_j) v_j with fp32 scores, the row maximum subtracted and an
+ *                    fp32 weighted sum, rounded once.  S % 64 == 0 and S <= 256, C % 64 == 0 and C <= 512, else
+ *                    DB200_E_UNSUPPORTED.  One launch for all B images.
+ *   gather_rows_split: hi[r] = bf16(table[idx[r] - offset]), lo[r] = bf16(table row - hi) (lo may be NULL); table f32
+ *                    [K][D], hi / lo bf16 [rows][D].  A row whose id is outside [offset, offset + K) is all zeros (as
+ *                    db200_onehot_rows_f32 gives a zero one-hot row).
+ *   clamp_bf16_to_f32: dst[i] = min(max(float(src[i]), lo), hi) (the decoder's output as an f32 image).
+ * ------------------------------------------------------------------------------------------------------------------ */
+int db200_groupnorm_stats(db200_stream_t stream, const void* x_bf16, float* mean, float* rstd, int N, int HW, int C,
+                          int G, float eps, void* workspace, int64_t workspace_bytes);
+int64_t db200_groupnorm_stats_workspace_bytes(int N, int HW, int C, int G);
+int db200_groupnorm_apply(db200_stream_t stream, const void* x_bf16, const float* mean, const float* rstd,
+                          const float* gamma, const float* beta, void* y_bf16, int N, int HW, int C, int G, int swish);
+int db200_attn_noncausal_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, int B, int S, int C,
+                             float scale);
+int db200_gather_rows_split(db200_stream_t stream, const int32_t* idx, const float* table, void* hi_bf16,
+                            void* lo_bf16_or_null, int rows, int D, int K, int offset);
+int db200_clamp_bf16_to_f32(db200_stream_t stream, const void* src_bf16, float* dst, int64_t n, float lo, float hi);
 /* KL(q_r || Uniform(K)) of the encoder logits l_r, q_r = softmax(l_r) (extension: the KL term of the DALL-E paper's
  * ELB, DALLE-pytorch's kl_div_loss_weight; the reference has neither).  All f32 except the int32 histogram.
  *   vae_kl_stats: lse[r] = logsumexp(l_r);  ent[r] = sum_k q_rk (l_rk - lse[r]);  hist[argmax l_r] += 1 (first maximum,

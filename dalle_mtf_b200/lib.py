@@ -251,6 +251,7 @@ _SIGNATURES = {
     "db200_groupnorm_stats": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_f32, c_vp, c_i64],
     "db200_groupnorm_apply": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_attn_noncausal_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_f32],
+    "db200_attn_noncausal_long_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_f32],
     "db200_gather_rows_split": [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int],
     "db200_clamp_bf16_to_f32": [c_vp, c_vp, c_vp, c_i64, c_f32, c_f32],
     "db200_vae_kl_stats": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_f32, c_vp, c_i64],

@@ -608,7 +608,8 @@ def vae_architecture(params, image_size):
 
 def vqgan_geometry(params, image_size):
     """The geometry of a VAE config with architecture "vqgan" (taming's ddconfig key names; num_tokens is taming's
-    n_embed): {ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim, resolution}.  Raises ValueError,
+    n_embed): {ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim, resolution, quantizer}, quantizer
+    "vq" (taming's VectorQuantizer, the default) or "gumbel" (its GumbelQuantize).  Raises ValueError,
     naming the key, for a missing key, for keys of the other networks, for use_bf16 false (the tokenizer runs bf16
     activations only) and for a geometry the kernels do not cover."""
     for k in ("convblocks", "n_hid", "n_blk_per_group", "group_count", "n_init"):
@@ -627,6 +628,7 @@ def vqgan_geometry(params, image_size):
     if missing:
         raise ValueError(f"{missing[0]}: missing from the architecture \"vqgan\" config (keys: {VQGAN_KEYS})")
     geo = {k: params[k] for k in VQGAN_KEYS}
+    geo["quantizer"] = "vq" if params.get("quantizer") is None else params["quantizer"]
     check_vqgan_geometry(image_size, num_tokens=params["num_tokens"], **geo)
     return geo
 

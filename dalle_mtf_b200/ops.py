@@ -1058,6 +1058,18 @@ def attn_noncausal(qkv, out, B, S, C, scale):
     return out
 
 
+def attn_noncausal_long(qkv, out, B, S, C, scale):
+    """attn_noncausal over longer sequences on wgmma: C == 512, S % 64 == 0 and 256 < S <= 4096."""
+    L.require_device()
+    _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out")
+    if qkv.numel() != B * S * 3 * C or out.numel() != B * S * C:
+        raise L.DB200Error(f"attn_noncausal_long: qkv {tuple(qkv.shape)} / out {tuple(out.shape)} do not match B={B}, "
+                           f"S={S}, C={C}")
+    check(L.load().db200_attn_noncausal_long_fwd(stream_ptr(), ptr(qkv), ptr(out), B, S, C, float(scale)),
+          "attn_noncausal_long_fwd")
+    return out
+
+
 def gather_rows_split(idx, table, hi, lo=None, offset=0):
     """hi [rows, D] = bf16(table[idx - offset]), lo = bf16(row - hi); ids outside [offset, offset + K) give zeros."""
     L.require_device()

@@ -3,15 +3,18 @@ definition and the precision policy, oracle/vqgan.py restates it in PyTorch).  F
 training and decode_tokens for generation.
 
 Parameter names are taming's state-dict keys with "." -> "/" (encoder/down/0/block/0/conv1/weight, ...): conv kernels
-HWIO, GroupNorm weights and biases [C], the codebook quantize/embedding/weight [num_tokens, embed_dim].
+HWIO, GroupNorm weights and biases [C], the codebook quantize/embedding/weight [num_tokens, embed_dim] or, for a
+Gumbel quantiser ("quantizer": "gumbel", taming's GumbelVQ), quantize/proj/weight [1, 1, embed_dim, num_tokens],
+quantize/proj/bias [num_tokens] and quantize/embed/weight [num_tokens, embed_dim].
 import_taming_state_dict converts a taming state dict into these names; tools/import_vqgan.py writes the result as a
 checkpoint.
 
 Kernels: the 3x3 / 1x1 convolutions on K11 (the wgmma implicit GEMM where the shape qualifies, Cin % 64 == 0; the
 3 -> ch input conv and the ch -> 3 output conv on the direct kernel), GroupNorm (+ swish), the AttnBlock's attention,
-the codebook gather and the output clamp on K14, the attention's q|k|v and proj_out 1x1 convs on the GEMM (q, k and v
-fused into one [C, 3C] product), nearest 2x upsampling on K11p.  Activations are bf16; quant_conv, the nearest-code
-search and post_quant_conv run on bf16 hi + lo split operands (fp32-accurate).
+the codebook gather and the output clamp on K14 (attention over S > 256 positions at C = 512 on its wgmma kernel,
+csrc/vqgan_attn.cu), the attention's q|k|v and proj_out 1x1 convs on the GEMM (q, k and v fused into one [C, 3C]
+product), nearest 2x upsampling on K11p.  Activations are bf16; quant_conv, the nearest-code
+search (or the Gumbel logits) and post_quant_conv run on bf16 hi + lo split operands (fp32-accurate).
 """
 import math
 
@@ -24,6 +27,16 @@ from .vae_engine import BF16, F32, I32, DECODE_PASS_BYTES
 
 GROUPS, EPS = 32, 1e-6
 ATTN_MAX_S, ATTN_MAX_C = 256, 512        # db200_attn_noncausal_fwd's range
+ATTN_LONG_MAX_S, ATTN_LONG_C = 4096, 512  # db200_attn_noncausal_long_fwd's: ATTN_MAX_S < S <= 4096 at C == 512 only
+QUANTIZERS = ("vq", "gumbel")
+
+
+def attention_in_range(S, C):
+    """Whether an AttnBlock over S positions of C channels runs on a kernel: db200_attn_noncausal_fwd for S <= 256
+    with C <= 512, db200_attn_noncausal_long_fwd for 256 < S <= 4096 at C == 512 (S a multiple of 64 for both)."""
+    if S % 64:
+        return False
+    return (S <= ATTN_MAX_S and C <= ATTN_MAX_C) or (ATTN_MAX_S < S <= ATTN_LONG_MAX_S and C == ATTN_LONG_C)
 
 
 def _int(k, v, lo=1):
@@ -32,8 +45,13 @@ def _int(k, v, lo=1):
 
 
 def check_vqgan_geometry(image_size, ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim,
-                         num_tokens=None, resolution=None):
+                         num_tokens=None, resolution=None, quantizer="vq"):
     """Raises ValueError, naming the key, for a geometry the kernels do not cover."""
+    if quantizer not in QUANTIZERS:
+        raise ValueError(f"quantizer = {quantizer!r}: must be one of {QUANTIZERS} (or absent for \"vq\")")
+    if quantizer == "gumbel" and embed_dim != z_channels:
+        raise ValueError(f"embed_dim = {embed_dim}: a Gumbel quantiser needs embed_dim == z_channels = {z_channels} "
+                         "(taming builds its proj on z_channels inputs and applies it to quant_conv's embed_dim outputs)")
     _int("image_size", image_size)
     _int("ch", ch)
     _int("num_res_blocks", num_res_blocks)
@@ -60,10 +78,11 @@ def check_vqgan_geometry(image_size, ch, ch_mult, num_res_blocks, attn_resolutio
     for i, m in enumerate(ch_mult):
         if res in attn_resolutions or (i == len(ch_mult) - 1):   # the mid blocks attend at the last resolution
             C, S = ch * m, res * res
-            if S % 64 or S > ATTN_MAX_S or C > ATTN_MAX_C:
+            if not attention_in_range(S, C):
                 what = "attn_resolutions" if res in attn_resolutions else "image_size / ch_mult (the mid AttnBlock)"
-                raise ValueError(f"{what}: attention at {res} x {res} with {C} channels is outside the kernel's range "
-                                 f"(S = res^2 a multiple of 64 up to {ATTN_MAX_S}, C up to {ATTN_MAX_C})")
+                raise ValueError(f"{what}: attention at {res} x {res} with {C} channels is outside the kernels' range "
+                                 f"(S = res^2 a multiple of 64: up to {ATTN_MAX_S} with C up to {ATTN_MAX_C}, or up "
+                                 f"to {ATTN_LONG_MAX_S} with C = {ATTN_LONG_C})")
         res //= 2
     if num_tokens is not None:
         _int("num_tokens", num_tokens)
@@ -130,7 +149,11 @@ def network(geo):
     conv("decoder/conv_in", 3, zc, lv[-1][1]); steps(dec)
     norm("decoder/norm_out", cin); conv("decoder/conv_out", 3, cin, 3)
     conv("quant_conv", 1, zc, ed)
-    lay.add("quantize/embedding/weight", (geo["num_tokens"], ed))
+    if geo.get("quantizer", "vq") == "gumbel":
+        conv("quantize/proj", 1, ed, geo["num_tokens"])
+        lay.add("quantize/embed/weight", (geo["num_tokens"], ed))
+    else:
+        lay.add("quantize/embedding/weight", (geo["num_tokens"], ed))
     conv("post_quant_conv", 1, ed, zc)
     return enc, dec, lay
 
@@ -139,14 +162,20 @@ def network(geo):
 def import_taming_state_dict(sd, geo):
     """taming VQModel state dict (OIHW conv weights) -> this project's named tensors (f32, HWIO kernels).
 
-    geo: {ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim, num_tokens, resolution}.  taming's
-    loss.* entries (LPIPS, discriminator) are ignored.  Raises ValueError naming the variable for a Gumbel or
-    double_z checkpoint and for a missing, extra or wrongly shaped tensor."""
+    geo: {ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim, num_tokens, resolution} and optionally
+    quantizer ("vq", the default: a VectorQuantizer VQModel; "gumbel": a GumbelVQ).  taming's loss.* entries (LPIPS,
+    discriminator) are ignored.  Raises ValueError naming the variable for a checkpoint of the other quantiser, a
+    double_z checkpoint and a missing, extra or wrongly shaped tensor."""
     sd = {k: v for k, v in sd.items() if not k.startswith("loss.")}
-    gumbel = [k for k in sd if k == "quantize.embed.weight" or k.startswith("quantize.proj")]
-    if gumbel:
-        raise ValueError(f"{gumbel[0]}: a Gumbel-quantised checkpoint (GumbelVQ); only VectorQuantizer VQGANs are "
-                         "supported")
+    if geo.get("quantizer", "vq") == "gumbel":
+        if "quantize.embedding.weight" in sd:
+            raise ValueError("quantize.embedding.weight: a VectorQuantizer checkpoint (VQModel); set "
+                             "\"quantizer\": \"vq\" (or leave it out) in the VAE config")
+    else:
+        gumbel = [k for k in sd if k == "quantize.embed.weight" or k.startswith("quantize.proj")]
+        if gumbel:
+            raise ValueError(f"{gumbel[0]}: a Gumbel-quantised checkpoint (GumbelVQ); set \"quantizer\": \"gumbel\" "
+                             "in the VAE config")
     w = sd.get("encoder.conv_out.weight")
     if w is not None and w.shape[0] == 2 * geo["z_channels"]:
         raise ValueError(f"encoder.conv_out.weight has {w.shape[0]} = 2 * z_channels outputs: a double_z encoder, "
@@ -195,15 +224,18 @@ def load_taming_checkpoint(path):
 # ------------------------------------------------------------------------------------------------------ engine
 class VqganEngine:
     def __init__(self, num_tokens, image_size, ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim,
-                 resolution=None, input_channels=3, device="cuda"):
+                 resolution=None, input_channels=3, device="cuda", quantizer="vq"):
         L.require_device()
         check_vqgan_geometry(image_size, ch, ch_mult, num_res_blocks, attn_resolutions, z_channels, embed_dim,
-                             num_tokens, resolution)
+                             num_tokens, resolution, quantizer)
         if input_channels != 3:
             raise ValueError(f"input_channels = {input_channels}: a VQGAN reads RGB images (3 channels)")
         self.geo = dict(ch=ch, ch_mult=list(ch_mult), num_res_blocks=num_res_blocks,
                         attn_resolutions=list(attn_resolutions), z_channels=z_channels, embed_dim=embed_dim,
-                        num_tokens=num_tokens, resolution=image_size)
+                        num_tokens=num_tokens, resolution=image_size, quantizer=quantizer)
+        self.gumbel = quantizer == "gumbel"
+        # the table decode_tokens gathers codes from: taming's codebook, or GumbelQuantize's embed
+        self.codebook = "quantize/embed/weight" if self.gumbel else "quantize/embedding/weight"
         self.K = int(num_tokens)
         self.img_H = self.img_W = self.H = self.W = int(image_size)
         self.img_C = 3
@@ -225,8 +257,8 @@ class VqganEngine:
         self.qkv_b = {s[1]: e(3 * s[3], dtype=F32) for s in self.enc + self.dec if s[0] == "attn"}
         self.qc_hi, self.qc_lo = e(self.zc, self.ed), e(self.zc, self.ed)                       # quant_conv [zc, ed]
         self.pq_hi, self.pq_lo = e(self.ed, self.zc), e(self.ed, self.zc)                       # post_quant_conv
-        self.cb_hi, self.cb_lo = e(self.K, self.ed), e(self.K, self.ed)                         # codebook [K, ed]
-        self.cb_bias = e(self.K, dtype=F32)                                                     # -||e_n||^2 / 2
+        self.cb_hi, self.cb_lo = e(self.K, self.ed), e(self.K, self.ed)     # codebook, or Gumbel proj^T [K, ed]
+        self.cb_bias = e(self.K, dtype=F32)                                 # -||e_n||^2 / 2, or the proj bias
         self._B = None
         self._views = {}
         self._descs = {}
@@ -269,22 +301,23 @@ class VqganEngine:
 
     def init_params(self, seed=0):
         """Synthetic weights drawn on the device (throughput runs without a checkpoint): conv kernels N(0, 1 / fan_in),
-        GroupNorm scales 1, biases 0, codebook rows N(0, 1)."""
+        GroupNorm scales 1, biases 0, codebook (Gumbel embed) rows N(0, 1)."""
         g = torch.Generator(device=self.device).manual_seed(seed)
         self.master.zero_()
         for name in self.layout.order:
             shape = self.layout.entries[name][1]
             if len(shape) == 4:
                 self.P(name).copy_(torch.randn(shape, generator=g, device=self.device) / math.sqrt(math.prod(shape[:3])))
-            elif name == "quantize/embedding/weight":
+            elif name == self.codebook:
                 self.P(name).copy_(torch.randn(shape, generator=g, device=self.device))
             elif "/norm" in name and name.endswith("/weight"):
                 self.P(name).fill_(1.0)
         self._refresh()
 
     def _refresh(self):
-        """The compute copies of the weights: bf16 kernels, the fused q|k|v products, the split 1x1 convs and codebook,
-        and the codebook's score bias -||e_n||^2 / 2 (summed once here, in float64 on the host)."""
+        """The compute copies of the weights: bf16 kernels, the fused q|k|v products, the split 1x1 convs and the code
+        scores' split operand and bias: the codebook with -||e_n||^2 / 2 (summed once here, in float64 on the host), or
+        for a Gumbel quantiser proj's kernel transposed to [K, embed_dim] with proj's bias."""
         ops.cast_f32_to_bf16(self.master, self.shadow)
         for name, w in self.qkv_w.items():
             C = w.shape[0]
@@ -293,6 +326,10 @@ class VqganEngine:
                 self.qkv_b[name][i * C:(i + 1) * C].copy_(self.P(f"{name}/{p}/bias"))
         ops.split_f32(self.P("quant_conv/weight").view(self.zc, self.ed), self.qc_hi, self.qc_lo)
         ops.split_f32(self.P("post_quant_conv/weight").view(self.ed, self.zc), self.pq_hi, self.pq_lo)
+        if self.gumbel:
+            ops.split_f32(self.P("quantize/proj/weight").view(self.ed, self.K).t().contiguous(), self.cb_hi, self.cb_lo)
+            self.cb_bias.copy_(self.P("quantize/proj/bias"))
+            return
         cb = self.P("quantize/embedding/weight")
         ops.split_f32(cb, self.cb_hi, self.cb_lo)
         self.cb_bias.copy_((-0.5 * (cb.detach().cpu().double() ** 2).sum(1)).float())
@@ -406,7 +443,8 @@ class VqganEngine:
         t = self._norm(x, name + "/norm", self._buf(res, C, x), False)
         qkv, o = b[("qkv", C)][:rows], b[("o", C)][:rows]
         ops.linear_fwd(t.view(rows, C), self.qkv_w[name], qkv, bias=self.qkv_b[name])
-        ops.attn_noncausal(qkv, o, B, res * res, C, C ** -0.5)
+        attn = ops.attn_noncausal if res * res <= ATTN_MAX_S else ops.attn_noncausal_long
+        attn(qkv, o, B, res * res, C, C ** -0.5)
         y = self._buf(res, C, x, t)
         ops.linear_fwd(o, self.W16(name + "/proj_out/weight").view(C, C), y.view(rows, C),
                        bias=self.P(name + "/proj_out/bias"), residual=x.view(rows, C))
@@ -456,8 +494,9 @@ class VqganEngine:
                               self.P("quant_conv/bias"))
 
     def encode_tokens(self, img):
-        """Nearest codes of the images (first index on ties), int32 [B, image_seq_len]: score_n = z . e_n - ||e_n||^2 / 2
-        on hi + lo split operands (the lo x lo product dropped), then the first row maximum."""
+        """Codes of the images (first index on ties), int32 [B, image_seq_len]: the first row maximum of the scores on
+        hi + lo split operands (the lo x lo product dropped).  VQ: the nearest code, score_n = z . e_n - ||e_n||^2 / 2.
+        Gumbel: the mode of taming's draw, score_n = the logit z . proj_n + proj_bias_n (no noise is added)."""
         z = self.encode_z(img)
         b = self._b
         rows = z.shape[0]
@@ -486,8 +525,8 @@ class VqganEngine:
         b = self._b
         rows = B * self.hw * self.hw
         # the codebook rows gathered exactly (as hi + lo), post_quant_conv on split operands
-        ops.gather_rows_split(idx.reshape(rows).to(torch.int32).contiguous(), self.P("quantize/embedding/weight"),
-                              b["z_hi"], b["z_lo"], offset)
+        ops.gather_rows_split(idx.reshape(rows).to(torch.int32).contiguous(), self.P(self.codebook), b["z_hi"],
+                              b["z_lo"], offset)
         h = self._split_mm([(b["z_hi"], self.pq_hi), (b["z_hi"], self.pq_lo), (b["z_lo"], self.pq_hi)], b["h_f32"],
                            rows, self.zc, self.ed, True, self.P("post_quant_conv/bias"))
         x = ops.cast_f32_to_bf16(h, self._buf(self.hw, self.zc).view(rows, self.zc)).view(B, self.hw, self.hw, self.zc)

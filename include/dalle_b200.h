@@ -572,6 +572,11 @@ int db200_argmax_rows_f32(db200_stream_t stream, const float* x, int32_t* idx, i
  *                    out_i = sum_j softmax_j(scale q_i . k_j) v_j with fp32 scores, the row maximum subtracted and an
  *                    fp32 weighted sum, rounded once.  S % 64 == 0 and S <= 256, C % 64 == 0 and C <= 512, else
  *                    DB200_E_UNSUPPORTED.  One launch for all B images.
+ *   attn_noncausal_long_fwd: the same attention and layout over longer sequences on wgmma: C == 512, S % 64 == 0 and
+ *                    256 < S <= 4096, B <= 65535, else DB200_E_UNSUPPORTED.  bf16 q, k, v; fp32 scores (each
+ *                    query's two 256-channel halves summed in fp32), an fp32 online softmax over 64-key tiles in key
+ *                    order, P rounded to bf16 for the fp32-accumulated P v, rounded once.  No atomics: bit-reproducible,
+ *                    and an image's output does not depend on B.  qkv / out 16-byte aligned.
  *   gather_rows_split: hi[r] = bf16(table[idx[r] - offset]), lo[r] = bf16(table row - hi) (lo may be NULL); table f32
  *                    [K][D], hi / lo bf16 [rows][D].  A row whose id is outside [offset, offset + K) is all zeros (as
  *                    db200_onehot_rows_f32 gives a zero one-hot row).
@@ -584,6 +589,8 @@ int db200_groupnorm_apply(db200_stream_t stream, const void* x_bf16, const float
                           const float* gamma, const float* beta, void* y_bf16, int N, int HW, int C, int G, int swish);
 int db200_attn_noncausal_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, int B, int S, int C,
                              float scale);
+int db200_attn_noncausal_long_fwd(db200_stream_t stream, const void* qkv_bf16, void* out_bf16, int B, int S, int C,
+                                  float scale);
 int db200_gather_rows_split(db200_stream_t stream, const int32_t* idx, const float* table, void* hi_bf16,
                             void* lo_bf16_or_null, int rows, int D, int K, int offset);
 int db200_clamp_bf16_to_f32(db200_stream_t stream, const void* src_bf16, float* dst, int64_t n, float lo, float hi);

@@ -1,4 +1,5 @@
-"""Cost of the VQGAN tokenizer (architecture "vqgan") at the vqgan_imagenet_f16_16384 geometry on one GPU.
+"""Cost of the VQGAN tokenizer (architecture "vqgan") on one GPU, at the vqgan_imagenet_f16_16384 geometry
+(--geometry f16, the default) or taming's Gumbel vqgan_gumbel_f8 (--geometry gumbel_f8: 8192 codes, a 32 x 32 grid).
 
 Prints, as JSON lines that name the card, its power limit and SM clock:
   * encode (images -> codes) and decode (codes -> images) images/s at B = 16 and 32, this project's kernels alternated
@@ -6,9 +7,11 @@ Prints, as JSON lines that name the card, its power limit and SM clock:
   * per-kernel device time of one encode and one decode at B = 16 (CUDA events around each ops call): GroupNorm
     statistics and apply with the bytes they must move (TB/s), the attention (us) and the summed convolution time with
     its TFLOP/s, FLOPs counted from shapes here;
+  * gumbel_f8 only: the S = 1024, C = 512 attention kernel alone at B = 16 and 32, with its TFLOP/s (4 S^2 C per
+    image: the score and the weighted-sum products);
   * the tokenizer's share of a dalle_coco_b200-width training step (n_embd 1024, 24 layers, 16 heads, 16 images per
-    GPU, image_vocab_size 16 384) that tokenizes with it (vae_random_init).
-Usage: python tools/bench_vqgan.py [--rounds 3]
+    GPU, image_vocab_size the tokenizer's codes) that tokenizes with it (vae_random_init).
+Usage: python tools/bench_vqgan.py [--geometry f16|gumbel_f8] [--rounds 3]
 """
 import argparse
 import json
@@ -24,6 +27,7 @@ sys.path.insert(0, ROOT)
 
 from dalle_mtf_b200 import ops                        # noqa: E402
 from oracle import vqgan as O                         # noqa: E402
+from oracle import vqgan_gumbel as OG                 # noqa: E402
 
 
 def card():
@@ -54,7 +58,8 @@ def per_kernel(eng, img, ids):
     """Device time per kernel class of one encode + one decode (CUDA events around every wrapped ops call)."""
     rec = []
     wrapped = {}
-    for name in ("groupnorm_stats", "groupnorm_apply", "attn_noncausal", "conv2d_fwd", "conv2d_fwd_tc", "gemm"):
+    for name in ("groupnorm_stats", "groupnorm_apply", "attn_noncausal", "attn_noncausal_long", "conv2d_fwd",
+                 "conv2d_fwd_tc", "gemm"):
         fn = getattr(ops, name)
 
         def w(*a, _fn=fn, _name=name, **k):
@@ -82,7 +87,7 @@ def per_kernel(eng, img, ids):
             nbytes = x.numel() * 2 * (1 if name == "groupnorm_stats" else 2)
             d = agg.setdefault(key, {"ms": 0.0, "bytes": 0, "n": 0})
             d["bytes"] += nbytes
-        elif name == "attn_noncausal":
+        elif name.startswith("attn_noncausal"):
             key = f"attn S={a[3]} C={a[4]}"
             d = agg.setdefault(key, {"ms": 0.0, "n": 0})
         elif name.startswith("conv2d"):
@@ -105,58 +110,84 @@ def per_kernel(eng, img, ids):
     return agg
 
 
+def attn_kernel(info, S=1024, C=512, reps=50):
+    """The long-sequence attention kernel alone (CUDA events over `reps` launches)."""
+    g = torch.Generator(device="cuda").manual_seed(0)
+    for B in (16, 32):
+        qkv = torch.randn(B, S, 3 * C, generator=g, device="cuda").to(torch.bfloat16)
+        out = torch.empty(B, S, C, dtype=torch.bfloat16, device="cuda")
+        ms = timed(lambda: ops.attn_noncausal_long(qkv, out, B, S, C, C ** -0.5), reps=reps, warm=5)
+        print(json.dumps({**info, "what": "attn_noncausal_long kernel", "B": B, "S": S, "C": C,
+                          "us": round(1e3 * ms, 1), "TFLOP/s": round(4.0 * B * S * S * C / (ms * 1e-3) / 1e12, 1)}))
+
+
+GEOMETRIES = {"f16": (O.GEOMETRY_F16, "vae_vqgan_f16_16384_b200"),
+              "gumbel_f8": (OG.GEOMETRY_GUMBEL_F8, "vae_vqgan_gumbel_f8_8192_b200")}
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--geometry", choices=sorted(GEOMETRIES), default="f16")
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
     info = card()
     from dalle_mtf_b200.vqgan_engine import VqganEngine, import_taming_state_dict
-    geo = O.GEOMETRY_F16
-    sd = O.random_state_dict(geo, 0)
+    geo, vae_cfg = GEOMETRIES[args.geometry]
+    info["geometry"] = args.geometry
+    if args.geometry == "gumbel_f8":
+        attn_kernel(info)
+    Q = OG if OG.is_gumbel(geo) else O          # the oracle of the geometry's quantiser
+    sd = Q.random_state_dict(geo, 0)
     eng = VqganEngine(geo["num_tokens"], geo["resolution"], geo["ch"], geo["ch_mult"], geo["num_res_blocks"],
-                      geo["attn_resolutions"], geo["z_channels"], geo["embed_dim"])
+                      geo["attn_resolutions"], geo["z_channels"], geo["embed_dim"],
+                      quantizer=geo.get("quantizer", "vq"))
     eng.load_params(import_taming_state_dict(sd, geo))
     sd16 = O.to(sd, torch.bfloat16, "cuda")
+    sdq = {k: v.float() for k, v in sd16.items() if k.startswith("quantize.")}   # the code search in f32
     torch.backends.cudnn.benchmark = True
     g = torch.Generator(device="cuda").manual_seed(0)
+    n_codes = eng.image_seq_len
     res = {}
     for rnd in range(args.rounds):
         for B in (16, 32):
             img = torch.rand(B, 256, 256, 3, generator=g, device="cuda") * 2 - 1
-            ids = torch.randint(0, geo["num_tokens"], (B, 256), generator=g, device="cuda", dtype=torch.int32)
+            ids = torch.randint(0, geo["num_tokens"], (B, n_codes), generator=g, device="cuda", dtype=torch.int32)
             img_cl = img.to(torch.bfloat16)
-            ref_z = lambda: O.nearest_codes(O.encode_z(sd16, geo, img_cl).float().reshape(-1, 256),
-                                            sd16["quantize.embedding.weight"].float())
+            if OG.is_gumbel(geo):
+                ref_z = lambda: OG.codes(sdq, O.encode_z(sd16, geo, img_cl).float())
+            else:
+                ref_z = lambda: O.nearest_codes(O.encode_z(sd16, geo, img_cl).float().reshape(-1, geo["embed_dim"]),
+                                                sdq["quantize.embedding.weight"])
             with torch.no_grad():
                 for name, fn in (("ours encode", lambda: eng.encode_tokens(img)),
                                  ("pytorch encode", ref_z),
                                  ("ours decode", lambda: eng.decode_tokens(ids)),
-                                 ("pytorch decode", lambda: O.decode(sd16, geo, ids.long()))):
+                                 ("pytorch decode", lambda: Q.decode(sd16, geo, ids.long()))):
                     ms = timed(fn)
                     res.setdefault((name, B), []).append(B / (ms * 1e-3))
     for (name, B), v in res.items():
         print(json.dumps({**info, "what": f"{name} images/s", "B": B, "rounds": [round(x, 1) for x in v],
                           "best": round(max(v), 1)}))
     img = torch.rand(16, 256, 256, 3, generator=g, device="cuda") * 2 - 1
-    ids = torch.randint(0, geo["num_tokens"], (16, 256), generator=g, device="cuda", dtype=torch.int32)
+    ids = torch.randint(0, geo["num_tokens"], (16, n_codes), generator=g, device="cuda", dtype=torch.int32)
     per_kernel(eng, img, ids)
     for key, d in per_kernel(eng, img, ids).items():
         print(json.dumps({**info, "what": "per-kernel, one encode + one decode at B=16", "kernel": key,
                           **{k: (round(v, 4) if isinstance(v, float) else v) for k, v in d.items()}}))
     del eng
     torch.cuda.empty_cache()
-    share(info)
+    share(info, vae_cfg, geo["num_tokens"])
 
 
-def share(info):
+def share(info, vae_cfg, vocab):
     """The tokenizer's share of a dalle_coco_b200-width step that tokenizes with the VQGAN (random weights)."""
     from collections import defaultdict
     from dalle_mtf_b200.model_fns import TRAIN, dalle_model_fn
     from dalle_mtf_b200.utils import fetch_model_params
     p = defaultdict(lambda: None, fetch_model_params("dalle_coco_b200"))
-    p.update({"vae_model": "vae_vqgan_f16_16384_b200", "image_vocab_size": 16384, "mesh_shape": "data:1",
+    p.update({"vae_model": vae_cfg, "image_vocab_size": vocab, "mesh_shape": "data:1",
               "train_batch_size": 16, "vae_random_init": True, "model_path": None})
-    p["vae_params"] = fetch_model_params("vae_vqgan_f16_16384_b200")
+    p["vae_params"] = fetch_model_params(vae_cfg)
     g = torch.Generator().manual_seed(0)
     img = torch.rand(16, 256, 256, 3, generator=g) * 2 - 1
     cap = torch.randint(0, 50000, (16, p["text_seq_len"]), generator=g, dtype=torch.int32)

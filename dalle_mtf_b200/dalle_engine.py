@@ -74,7 +74,7 @@ FF_MODULE = ("w1", "b1", "w2", "b2")                 # the MLP
 
 
 def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False, sandwich_norm=False, mlp_layers=None,
-                 layer_scale=False, tied=False, attn_owner=None, ff_owner=None):
+                 layer_scale=False, tied=False, attn_owner=None, ff_owner=None, wpe=True):
     """The flat-buffer layout of a DalleEngine of width d, n_layers blocks, vocabulary V (EOS included) and sequence
     length S: forward order, the vocabulary projection and its bias padded to a multiple of 64 columns.  grid_w (row /
     column image positions, S = text_len + grid_w^2): wpe holds the text_len text positions and image_row / image_col
@@ -88,7 +88,8 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     tied (share_input_output_emb): wte is [Vpad, d], its pad rows exactly zero, and is also the vocabulary projection;
     there is no wout.  attn_owner / ff_owner (shared_attn_ids / shared_ff_ids): per layer, the layer whose token mixer
     (ATTN_MODULE or GMLP_MODULE) / MLP (FF_MODULE) it uses.  A layer that is not its module's owner gets aliases of the
-    owner's entries, so that layer i's own entries still run contiguously from l{i}.ln1_g."""
+    owner's entries, so that layer i's own entries still run contiguously from l{i}.ln1_g.
+    wpe False (rotary_emb): no learned position embedding; wte is followed by the first layer."""
     w1_cols = 8 * d if gated_mlp else 4 * d
     Vpad = _round_up(V, 64)
     attn_owner = list(range(n_layers)) if attn_owner is None else attn_owner
@@ -96,7 +97,8 @@ def param_layout(d, n_layers, V, S, text_len=None, grid_w=None, gated_mlp=False,
     lay = ParamLayout()
     lay.add("wte", (Vpad if tied else V, d))
     if grid_w is None:
-        lay.add("wpe", (S, d))
+        if wpe:
+            lay.add("wpe", (S, d))
     else:
         lay.add("wpe", (text_len, d))
         lay.add("image_row", (grid_w, d)); lay.add("image_col", (grid_w, d))
@@ -414,6 +416,59 @@ def validate_rotary(rotary_dim, rotary_base, head_dim):
     return int(rotary_dim), float(base)
 
 
+def validate_rotary_emb(rotary_emb, image_seq_len, rotary=None, image_position_embedding=None):
+    """DALLE-pytorch's rotary embedding switch: None or False -> False; True -> True.  On, it needs a square image-token
+    grid and excludes rotary_dim / rotary_base (the validated `rotary`, None when off) and any non-null
+    image_position_embedding: the model then has no learned position embedding at all.  Anything else (1, "true", ...)
+    is a ValueError."""
+    if rotary_emb is None or rotary_emb is False:
+        return False
+    if rotary_emb is not True:
+        raise ValueError(f"rotary_emb = {rotary_emb!r}: must be true, false or null")
+    if math.isqrt(image_seq_len) ** 2 != image_seq_len:
+        raise ValueError(f"rotary_emb needs a square image-token grid, but image_seq_len = {image_seq_len} is not a "
+                         "square")
+    if rotary is not None:
+        raise ValueError("rotary_emb cannot be combined with rotary_dim / rotary_base (GPT-NeoX rotary embeddings)")
+    if image_position_embedding is not None:
+        raise ValueError(f"rotary_emb replaces the learned position embeddings: image_position_embedding must be null, "
+                         f"got {image_position_embedding!r}")
+    return True
+
+
+def rotary_emb_freqs(dh, grid_w):
+    """The ‡ constants of DALLE-pytorch's rotary embedding (DESIGN.md §4), in one place: (nf, theta, phi, y, t_image,
+    t_text_axial) with rot = dh // 3 and nf = rot // 2 pairs per part; theta_j = 1 / 10000^(2j / rot) (rotary-
+    embedding-torch's 'lang' frequencies of dim rot), phi_j = pi linspace(1, max_freq / 2, nf)[j] with max_freq 10
+    (its 'pixel' frequencies), y = linspace(-1, 1, grid_w) the image-grid coordinate, t_image = 8192 the text-part
+    position of every image token and t_text_axial = -10 the row / column coordinate of every text token.  All float32
+    as torch computes them."""
+    rot = dh // 3
+    nf = rot // 2
+    theta = 1.0 / (10000 ** (torch.arange(0, rot, 2)[:nf].float() / rot))
+    phi = torch.linspace(1.0, 10 / 2, nf) * math.pi
+    y = torch.linspace(-1.0, 1.0, grid_w)
+    return nf, theta, phi, y, 8192.0, -10.0
+
+
+def rotary_emb_table(text_len, grid_w, dh):
+    """The fp32 [S, 2, 3 nf] table of the rope_emb kernels, S = text_len + grid_w^2 (rotary_emb_freqs): position p's
+    3 nf cosines, then its sines.  Pair m < nf (part A) has the angle t theta_m with t = p for a text position and
+    t_image for every image token; pair nf + j (part B) t phi_j with t = y[row] for an image token and t_text_axial for
+    text; pair 2 nf + j (part C) the same with y[column].  The angle is the float32 product; its cos and sin are
+    evaluated in float64 and rounded once to fp32."""
+    nf, theta, phi, y, t_image, t_text_axial = rotary_emb_freqs(dh, grid_w)
+    n_img = grid_w * grid_w
+    t_a = torch.cat([torch.arange(text_len, dtype=torch.float32), torch.full((n_img,), t_image)])
+    rows = y.repeat_interleave(grid_w)          # image token r W + c: row r
+    cols = y.repeat(grid_w)                     # and column c
+    t_b = torch.cat([torch.full((text_len,), t_text_axial), rows])
+    t_c = torch.cat([torch.full((text_len,), t_text_axial), cols])
+    angle = torch.cat([t_a[:, None] * theta[None, :], t_b[:, None] * phi[None, :], t_c[:, None] * phi[None, :]], 1)
+    angle = angle.double()
+    return torch.stack([torch.cos(angle), torch.sin(angle)], dim=1).to(F32)
+
+
 def validate_sandwich_norm(sandwich_norm):
     """The sandwich LayerNorm switch: a bool (numbers, strings and None are a ValueError here; the config key's null is
     handled by model_fns.sandwich_norm)."""
@@ -534,6 +589,7 @@ class DalleEngine:
     layer_scale = None   # LayerScale (validate_layer_scale), set by the constructor; None: off
     stable = False   # DALLE-pytorch's stable option (validate_stable), set by the constructor
     tied = False   # share_input_output_emb (validate_share_input_output_emb), set by the constructor
+    rotary_emb = False   # DALLE-pytorch's rotary embedding (validate_rotary_emb), set by the constructor
 
     def __init__(self, n_embd, n_layers, n_heads, text_vocab_size, image_vocab_size, text_seq_len, image_seq_len,
                  device="cuda", recompute_grad=False, attn_scale=1.0, ln_eps=1e-5, zero=None, dropout=(0.0, 0.0, 0.0),
@@ -542,7 +598,7 @@ class DalleEngine:
                  activation="relu", logits_mask=False, rotary_dim=None, rotary_base=None, gated_mlp=False,
                  shift_tokens=False, sandwich_norm=False, layer_scale=None, stable=False, share_input_output_emb=False,
                  shared_attn_ids=None, shared_ff_ids=None, sparse_block_size=16, sparse_local_window_blocks=4,
-                 sparse_random_blocks=None, sparse_layout_seed=0):
+                 sparse_random_blocks=None, sparse_layout_seed=0, rotary_emb=None):
         """dropout = (embed_dropout, attention_dropout, residual_dropout) rates in [0, 1) (src/dalle_mtf/models.py:
         198-200, 215-217, 290-299, 312-314, 321-323).  They apply only to a forward() given a `step`; the masks are a
         pure function of (dropout_seed, step, site, global element index) (include/dalle_b200.h, D0).
@@ -659,7 +715,15 @@ class DalleEngine:
         with b = sparse_block_size, the local window sparse_local_window_blocks, sparse_random_blocks random blocks per
         row and sparse_layout_seed (validate_block_sparse).  The layout is drawn per token-mixer owner and is the same
         for every head; it is not a variable, so sampling must use the training config's keys.  No attention dropout
-        (the layer's site is unused); residual dropout is unchanged."""
+        (the layer's site is unused); residual dropout is unchanged.
+
+        rotary_emb (validate_rotary_emb): DALLE-pytorch's rotary embedding in place of learned positions.  After the
+        q|k|v product, the interleaved pairs (2m, 2m+1), m < 3 nf, of every q, k and v head of every attention layer
+        are rotated by the angles of rotary_emb_table (text position, image row, image column; gMLP layers are not
+        rotated), in fp32 and rounded to bf16 (ops.rope_emb_fwd); backward applies the transpose to d(q|k|v), and the
+        decoder rotates each step's q, k and v before k and v reach the cache.  There is no wpe: the embedding kernels
+        read an all-zero bf16 [S, d] table the engine owns (pos_table), and their position gradient goes to a scratch
+        nothing reads (_dpos)."""
         self.dh = validate_geometry(n_embd, n_heads, text_seq_len, image_seq_len, text_vocab_size, image_vocab_size,
                                     n_layers)
         self.shift_tokens = validate_shift_tokens(shift_tokens, image_seq_len)
@@ -668,6 +732,7 @@ class DalleEngine:
         self.layer_scale = validate_layer_scale(layer_scale)
         self.stable = validate_stable(stable)
         self.rotary = validate_rotary(rotary_dim, rotary_base, self.dh)
+        self.rotary_emb = validate_rotary_emb(rotary_emb, image_seq_len, self.rotary, image_position_embedding)
         self.activation = validate_activation(activation)
         self.gated_mlp = validate_gated_mlp(gated_mlp)
         self.glu = self.activation if self.gated_mlp else None   # the gate's nonlinearity, or None: no gate
@@ -736,10 +801,11 @@ class DalleEngine:
         mlp_layers = self.mlp if any(self.mlp) else None
         kw = dict(gated_mlp=self.gated_mlp, sandwich_norm=self.sandwich_norm, mlp_layers=mlp_layers,
                   layer_scale=self.layer_scale is not None, tied=self.tied, attn_owner=self.attn_owner,
-                  ff_owner=self.ff_owner)
+                  ff_owner=self.ff_owner, wpe=not self.rotary_emb)
         self.layout = lay = param_layout(d, Lyr, V, S, text_seq_len, self.grid_w, **kw) if self.row_col else \
             param_layout(d, Lyr, V, S, **kw)
-        self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else ("wte", "wpe")
+        self.embed_names = ("wte", "wpe", "image_row", "image_col") if self.row_col else \
+            ("wte",) if self.rotary_emb else ("wte", "wpe")
         self.n_params_padded = lay.size
         # trailing 64 floats of the gradient buffer carry scalars that ride along with the gradient all-reduce:
         #   [0] = sum of per-token losses of this rank (weighted loss: sum of a_t * loss_t)
@@ -779,13 +845,18 @@ class DalleEngine:
                     self._vec_off[name] = self._vec_off[owner]
             self.vec32 = torch.zeros(off, dtype=F32, device=dev)
             self._vec_table = torch.tensor(table, dtype=torch.int64, device=dev)
-        if self.row_col:   # the composed bf16 position table the embedding kernels read, and its fp32 gradient
+        # the composed bf16 position table the embedding kernels read, and its fp32 gradient (rotary_emb: all zeros,
+        # and a scratch gradient nothing reads)
+        if self.row_col or self.rotary_emb:
             self.pos_table = torch.zeros(S, d, dtype=BF16, device=dev)
             self._dpos = torch.zeros(S, d, dtype=F32, device=dev)
         self.gnorm_sq = torch.zeros(1, dtype=F32, device=dev)
         # rotary position embeddings: r (None: off) and the cos / sin table of every position, built once
         self.rotary_dim = self.rotary[0] if self.rotary else None
         self.rope_table = rope_table(S, *self.rotary).to(dev) if self.rotary else None
+        # rotary_emb: the cos / sin table of the text, row and column angles of every position, built once
+        self.rope_emb_table = rotary_emb_table(text_seq_len, math.isqrt(image_seq_len), self.dh).to(dev) \
+            if self.rotary_emb else None
         self._grads_clean = False
         self._bufs = None
         self._buf_key = None
@@ -859,8 +930,8 @@ class DalleEngine:
 
     def pos_embedding(self):
         """The bf16 [S, d] position table the embedding kernels read: wpe, or with row / column image positions the
-        table composed from wpe, image_row and image_col."""
-        return self.pos_table if self.row_col else self.W("wpe")
+        table composed from wpe, image_row and image_col; with rotary_emb an all-zero table."""
+        return self.pos_table if self.row_col or self.rotary_emb else self.W("wpe")
 
     def _compose_pos(self):
         """Rebuild the composed position table from the bf16 parameters (row / column image positions only)."""
@@ -870,7 +941,7 @@ class DalleEngine:
     def n_params(self):
         """Trainable parameter count as the reference would print it (src/utils/utils.py:55-70)."""
         d, V, S, Lyr = self.d, self.V, self.S, self.L
-        n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else S
+        n_pos = (self.text_seq_len + 2 * self.grid_w) if self.row_col else 0 if self.rotary_emb else S
         gate = (4 * d * d + 4 * d) if self.gated_mlp else 0   # the gate half of W1 and b1
         sandwich = 4 * d if self.sandwich_norm else 0         # LNa and LNm: g and b each
         scales = 2 * d if self.layer_scale is not None else 0  # the two LayerScale vectors
@@ -1043,6 +1114,17 @@ class DalleEngine:
             raise L.DB200Error(f"load_params: {k}: a LayerScale variable, but this model has layer_scale = "
                                f"{self.layer_scale}")
 
+    def _check_position_names(self, named):
+        """Refuse a checkpoint of the other position kind: learned positions loaded into a rotary_emb model (which
+        would otherwise be ignored), or a rotary_emb checkpoint, which has none, loaded into a model that needs them."""
+        wpe = self.EMBED_REF_NAMES["wpe"]
+        if self.rotary_emb and wpe in named:
+            raise L.DB200Error(f"load_params: {wpe}: a learned position embedding, but this model has rotary_emb = "
+                               "true and no learned positions")
+        if not self.rotary_emb and wpe not in named:
+            raise L.DB200Error(f"load_params: {wpe}: missing from the checkpoint (a rotary_emb checkpoint has no "
+                               "learned positions; set rotary_emb to load it)")
+
     def load_params(self, named):
         """Load a dict keyed by the reference's variable names (SURVEY.md Appendix B); CPU or CUDA fp32 tensors."""
         self.load_flat(self.master, named)
@@ -1085,6 +1167,7 @@ class DalleEngine:
         self._check_layer_kinds(named)
         self._check_layer_scale_names(named)
         self._check_sharing_names(named)
+        self._check_position_names(named)
         if self.zero is not None:
             if flat is not self.master:
                 raise L.DB200Error("ZeRO-1 mode: loading sharded Adam slots is not implemented (throughput configuration)")
@@ -1180,7 +1263,9 @@ class DalleEngine:
                 t = t[:rows]
             t.copy_(torch.randn(t.shape, generator=g, device=self.device, dtype=F32) * std)
 
-        normal("wte", 0.02, rows=self.V); normal("wpe", 0.01)
+        normal("wte", 0.02, rows=self.V)
+        if not self.rotary_emb:
+            normal("wpe", 0.01)
         if self.row_col:
             normal("image_row", 0.01); normal("image_col", 0.01)
         for i in range(Lyr):
@@ -1425,6 +1510,8 @@ class DalleEngine:
             ops.linear_fwd(sv["ln1"], self.W(p + "wqkv"), sv["qkv"])                   # q|k|v, no bias (:242-244)
             if self.rotary:
                 ops.rope_fwd(sv["qkv"], self.rope_table, S or self.S, self.H, self.dh, self.rotary_dim)
+            if self.rotary_emb:
+                ops.rope_emb_fwd(sv["qkv"], self.rope_emb_table, S or self.S, self.H, self.dh)
             ops.attn_fwd(sv["qkv"], sv["attn"], sv["lse"], B, S or self.S, self.H, self.dh, self.attn_scale,
                          dropout=self._site("attn", i), radius=self.radii[i], **self.axial_kw[i],
                          **self.conv_kw[i], **self.block_sparse_kw[i])  # :257-299
@@ -1752,6 +1839,8 @@ class DalleEngine:
                          radius=self.radii[i], **self.axial_kw[i], **self.conv_kw[i], **self.block_sparse_kw[i])
             if self.rotary:   # d(q|k|v) before the rotation
                 ops.rope_bwd(bufs["dqkv"], self.rope_table, self.S, self.H, self.dh, self.rotary_dim)
+            if self.rotary_emb:
+                ops.rope_emb_bwd(bufs["dqkv"], self.rope_emb_table, self.S, self.H, self.dh)
             ops.linear_dgrad(bufs["dqkv"], self.W(p + "wqkv"), bufs["dtmp"])                  # dLN1 out
             ops.linear_wgrad(sv["ln1"], bufs["dqkv"], self.G(p + "wqkv"))
         dln = self._shift_bwd(bufs["dtmp"], sv["ln1_raw"]) if self.shift_tokens else bufs["dtmp"]
@@ -1840,7 +1929,8 @@ class DalleEngine:
                 on_bucket_ready(s, e)
         # row / column positions: the gradient of the composed table goes into a zeroed scratch, then is folded into
         # wpe, image_row and image_col (one fully formed contribution per call, like the wpe gradient itself)
-        dpos = self._dpos.zero_() if self.row_col else self.G("wpe")
+        # (rotary_emb: the zero table's gradient goes to the scratch and is not read)
+        dpos = self._dpos.zero_() if self.row_col or self.rotary_emb else self.G("wpe")
         dwte = self.wte_rows(self.grads)   # tied: after the vocabulary wgrad, in this fixed order
         alpha = {"alpha": STABLE_ALPHA} if self.stable else {}   # pos_fold is linear: it carries the shrink along
         if self._drop is not None:

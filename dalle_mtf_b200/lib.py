@@ -181,6 +181,10 @@ _SIGNATURES = {
     "db200_rope_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_rope_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_rope_decode_dev": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
+    "db200_rope_emb_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_rope_emb_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
+    "db200_rope_emb_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
+    "db200_rope_emb_decode_dev": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
     "db200_shift_tokens_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_shift_tokens_bwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],
     "db200_shift_tokens_decode": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],

@@ -16,8 +16,8 @@ from . import lib as L
 from . import ops
 from .dalle_engine import ATTENTION_TYPES, DalleEngine, validate_activation, validate_conv_kernel, \
     validate_logits_mask, validate_loss_weights, validate_per_position_padding, validate_position_embedding, \
-    validate_layer_scale, validate_rotary, validate_sandwich_norm, validate_share_input_output_emb, \
-    validate_shared_ids, validate_shift_tokens, validate_stable, validate_block_sparse
+    validate_layer_scale, validate_rotary, validate_rotary_emb, validate_sandwich_norm, \
+    validate_share_input_output_emb, validate_shared_ids, validate_shift_tokens, validate_stable, validate_block_sparse
 from .dist import DataParallel
 from .optimizers import OptimizerConfig
 from .utils import latest_checkpoint, load_checkpoint, local_path, parse_mesh, print_n_params
@@ -339,6 +339,19 @@ def rotary_embedding(params, n_embd=None, n_heads=None):
     return (None, None) if rot is None else rot
 
 
+def rotary_emb(params, image_seq_len=None):
+    """rotary_emb of a DALL-E config (DALLE-pytorch's rotary embedding, DalleEngine): absent, null or false is off;
+    true rotates q, k and v of every attention layer by text / image-row / image-column angles in place of learned
+    positions.  Only a JSON bool is accepted; true is refused together with rotary_dim or rotary_base, or with any
+    non-null image_position_embedding, and needs a square image-token grid (checked here when image_seq_len is given,
+    and by the engine).  A rotary_emb model has no positional_embedding/wpe variable."""
+    v = params.get("rotary_emb")
+    rot = (params.get("rotary_dim"), params.get("rotary_base"))
+    on = validate_rotary_emb(v, 1 if image_seq_len is None else image_seq_len,
+                             None if rot == (None, None) else rot, params.get("image_position_embedding"))
+    return on
+
+
 def dalle_model_fn(features, labels, mode, params):
     """src/model_fns.py:55-236.  features: images f32 [B,H,W,C] in [-1,1] (NHWC); labels: caption ids i32
     [B, text_seq_len].  (The reference's own comment has them swapped; the code uses them this way.)"""
@@ -361,6 +374,10 @@ def dalle_model_fn(features, labels, mode, params):
     attn_ids, ff_ids = shared_attn_ids(params), shared_ff_ids(params)
     mask = logits_mask(params)
     rotary_dim, rotary_base = rotary_embedding(params)
+    # rotary_emb needs a square grid: checked here from the VAE config, before anything reaches the device
+    rot_emb = rotary_emb(params)
+    if rot_emb:
+        rotary_emb(params, vae_grid_size(params["vae_params"], params["dataset"]["image_size"]) ** 2)
     L.require_device()
     dp = params.get("_dp") or DataParallel().init()
     device = torch.device("cuda", torch.cuda.current_device())
@@ -393,11 +410,11 @@ def dalle_model_fn(features, labels, mode, params):
                         dropout=rates, dropout_seed=params.get("seed") or 0,
                         attention_types=attention_types, local_attention_radius=local_radius,  # models.py:229-301
                         conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
-                        image_position_embedding=pos_scheme, per_position_padding=per_pos,
+                        image_position_embedding=None if rot_emb else pos_scheme, per_position_padding=per_pos,
                         activation=activation, logits_mask=mask, rotary_dim=rotary_dim, rotary_base=rotary_base,
                         gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich, layer_scale=scale,
                         stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids,
-                        **sparse)
+                        rotary_emb=rot_emb, **sparse)
     if params["bf_16"] is False and dp.rank == 0:
         print("note: bf_16=false — the engine still runs activations and matmul operands in bf16 with fp32 "
               "accumulation, fp32 master weights / optimiser state (there is no fp32 tensor-core path yet)")

@@ -7,7 +7,7 @@ import torch
 from . import lib as L
 from .dalle_engine import DalleEngine
 from .model_fns import activation_function, attention_layers, block_sparse_options, conv_kernel, dropout_rates, \
-    gated_mlp, input_embedding, layer_scale, logits_mask, loss_weights, rotary_embedding, sandwich_norm, \
+    gated_mlp, input_embedding, layer_scale, logits_mask, loss_weights, rotary_emb, rotary_embedding, sandwich_norm, \
     share_input_output_emb, shared_attn_ids, shared_ff_ids, shift_tokens, stable, validate_kl_weight
 from .model_fns import build_vae_engine, vae_architecture
 from .utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
@@ -41,6 +41,7 @@ class DALLE:
         attn_ids, ff_ids = shared_attn_ids(params), shared_ff_ids(params)
         mask = logits_mask(params)
         rotary_dim, rotary_base = rotary_embedding(params, n_embd, n_heads)
+        rot_emb = rotary_emb(params, image_seq_len)
         self.n_embd, self.n_layers, self.n_heads = n_embd, n_layers, n_heads
         self.text_vocab_size, self.image_vocab_size = text_vocab_size, image_vocab_size
         self.text_seq_len, self.image_seq_len = text_seq_len, image_seq_len
@@ -54,12 +55,12 @@ class DALLE:
                                   dropout=dropout_rates(params), dropout_seed=params.get("seed") or 0,
                                   attention_types=attention_types, local_attention_radius=local_radius,
                                   conv_attention_kernel=conv_k, loss_weights=weights, z_loss=z_loss,
-                                  image_position_embedding=pos_scheme, per_position_padding=per_pos,
-                                  activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
-                                  rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift,
+                                  image_position_embedding=None if rot_emb else pos_scheme,
+                                  per_position_padding=per_pos, activation=activation, logits_mask=mask,
+                                  rotary_dim=rotary_dim, rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift,
                                   sandwich_norm=sandwich, layer_scale=scale, stable=stab,
                                   share_input_output_emb=tied, shared_attn_ids=attn_ids, shared_ff_ids=ff_ids,
-                                  **sparse)
+                                  rotary_emb=rot_emb, **sparse)
         self.loss_parts = None   # weighted loss: device [3] of the last forward (text / image mean CE, mean z-term)
         self._step = 0   # mode "train": each forward draws the dropout masks of the next step
         self.engine.eos_token_id = self.eos_token_id

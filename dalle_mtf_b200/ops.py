@@ -1438,6 +1438,53 @@ def shift_cache_fill(y, cache, P, rep=1):
           "db200_shift_cache_fill")
 
 
+def _rope_emb_args(qkv, table, H, dh, what):
+    """(rows, table positions, pairs) of a rotary_emb call after the dtype / shape checks."""
+    L.require_device()
+    _chk(qkv, BF16, what); _chk(table, F32, "table")
+    if not qkv.is_contiguous() or qkv.dim() != 2 or qkv.shape[1] != 3 * H * dh:
+        raise L.DB200Error(f"{what}: expected a contiguous [rows, {3 * H * dh}] q|k|v buffer, got {tuple(qkv.shape)}")
+    if not table.is_contiguous() or table.dim() != 3 or table.shape[1] != 2 or not 1 <= table.shape[2] <= dh // 2:
+        raise L.DB200Error(f"{what}: expected a contiguous [n_pos, 2, pairs <= {dh // 2}] table, got "
+                           f"{tuple(table.shape)}")
+    return qkv.shape[0], table.shape[0], table.shape[2]
+
+
+def rope_emb_fwd(qkv, table, S, H, dh):
+    """DALLE-pytorch's rotary embedding in place on every q, k and v head of qkv [rows, 3*H*dh] (bf16), row t at
+    position t mod S: the interleaved pairs (2m, 2m+1), m < pairs, rotated by the fp32 cos / sin table
+    [n_pos >= S, 2, pairs] (dalle_engine.rotary_emb_table; include/dalle_b200.h)."""
+    rows, n_pos, pairs = _rope_emb_args(qkv, table, H, dh, "rope_emb_fwd")
+    if S > n_pos:
+        raise L.DB200Error(f"rope_emb_fwd: period S {S} exceeds the table's {n_pos} positions")
+    check(L.load().db200_rope_emb_fwd(stream_ptr(), ptr(qkv), ptr(table), rows, int(S), H, dh, pairs),
+          "db200_rope_emb_fwd")
+
+
+def rope_emb_bwd(dqkv, table, S, H, dh):
+    """The transpose of rope_emb_fwd in place on the dq, dk and dv columns of dqkv [rows, 3*H*dh] (bf16)."""
+    rows, n_pos, pairs = _rope_emb_args(dqkv, table, H, dh, "rope_emb_bwd")
+    if S > n_pos:
+        raise L.DB200Error(f"rope_emb_bwd: period S {S} exceeds the table's {n_pos} positions")
+    check(L.load().db200_rope_emb_bwd(stream_ptr(), ptr(dqkv), ptr(table), rows, int(S), H, dh, pairs),
+          "db200_rope_emb_bwd")
+
+
+def rope_emb_decode(qkv, table, pos, H, dh):
+    """rope_emb_fwd of one decoding step: every row of qkv [rows, 3*H*dh] at position pos (0 <= pos < n_pos)."""
+    rows, n_pos, pairs = _rope_emb_args(qkv, table, H, dh, "rope_emb_decode")
+    check(L.load().db200_rope_emb_decode(stream_ptr(), ptr(qkv), ptr(table), rows, n_pos, H, dh, pairs, int(pos)),
+          "db200_rope_emb_decode")
+
+
+def rope_emb_decode_dev(qkv, table, pos_dev, H, dh):
+    """rope_emb_decode with the position read on the device from pos_dev (graph replay)."""
+    rows, n_pos, pairs = _rope_emb_args(qkv, table, H, dh, "rope_emb_decode_dev")
+    _chk(pos_dev, I32, "pos_dev")
+    check(L.load().db200_rope_emb_decode_dev(stream_ptr(), ptr(qkv), ptr(table), rows, n_pos, H, dh, pairs,
+                                             ptr(pos_dev)), "db200_rope_emb_decode_dev")
+
+
 def rows_repeat(src, dst, rep=1):
     """dst[b*rep + r] = src[b] for a [B, d] view src (rows may be strided, e.g. x.view(B, P, d)[:, P - 1])."""
     L.require_device()

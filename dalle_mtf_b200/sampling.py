@@ -13,7 +13,8 @@ parameters and the same kernels' numerics as training:
                     a block-sparse layer the positions <= p of the blocks its layout lets p's block see)
                     x = x + a Wo + o_b;  x = x + act(LN2(x) W1 + b1) W2 + b2   (the training GEMM, M = batch rows;
                     act = ReLU, or GELU without a pre-activation output); with rotary embeddings q and k are
-                    rotated to position p (rope_decode) before k enters the cache; with the token shift each
+                    rotated to position p (rope_decode) before k enters the cache (rotary_emb: q, k and v,
+                    rope_emb_decode, before k and v enter it); with the token shift each
                     LayerNorm output's first d/2 columns enter a per-layer cache and are replaced by the shifted
                     chunks of positions p - 1 and p - W (shift_tokens_decode); with the sandwich LayerNorm each
                     branch output is normalised before its residual add (layernorm_residual_fwd); with LayerScale
@@ -148,6 +149,8 @@ class DalleSampler:
                 ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
                 if e.rotary:
                     ops.rope_decode(self.qkv, e.rope_table, pos, e.H, e.dh, e.rotary_dim)
+                if e.rotary_emb:
+                    ops.rope_emb_decode(self.qkv, e.rope_emb_table, pos, e.H, e.dh)
                 ops.attn_decode(self.qkv, self.kc[i], self.vc[i], self.att, pos, e.attn_scale, radius=e.radii[i],
                                 **e.axial_kw[i], **e.conv_kw[i], **e.block_sparse_kw[i])
                 self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
@@ -179,6 +182,8 @@ class DalleSampler:
                 ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
                 if e.rotary:
                     ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
+                if e.rotary_emb:
+                    ops.rope_emb_decode_dev(self.qkv, e.rope_emb_table, self.pos_dev, e.H, e.dh)
                 ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
                                     radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i], **e.block_sparse_kw[i])
                 self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)

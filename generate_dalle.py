@@ -19,8 +19,8 @@ import numpy as np
 
 from dalle_mtf_b200.data_pipeline import truncate_or_pad_label
 from dalle_mtf_b200.model_fns import activation_function, attention_layers, block_sparse_options, conv_kernel, \
-    gated_mlp, input_embedding, layer_scale, logits_mask, rotary_embedding, sandwich_norm, share_input_output_emb, \
-    shared_attn_ids, shared_ff_ids, shift_tokens, stable, \
+    gated_mlp, input_embedding, layer_scale, logits_mask, rotary_emb, rotary_embedding, sandwich_norm, \
+    share_input_output_emb, shared_attn_ids, shared_ff_ids, shift_tokens, stable, \
     vae_checkpoint, vae_grid_size
 from dalle_mtf_b200.utils import fetch_model_params, latest_checkpoint, load_checkpoint, local_path
 
@@ -166,6 +166,8 @@ def main(argv=None):
     attn_ids, ff_ids = shared_attn_ids(params), shared_ff_ids(params)   # and which layers share their modules
     mask = logits_mask(params)                         # and its objective (sampling draws image ids either way)
     rotary_dim, rotary_base = rotary_embedding(params)  # and its rotary position embeddings
+    # or DALLE-pytorch's rotary embedding in place of learned positions
+    rot_emb = rotary_emb(params) and rotary_emb(params, token_grid_side(params) ** 2)
     # with per-position padding the captions are padded with the config's padding_id, which the sampler maps to the
     # per-position pads as training does
     pad = padding_id(params) if per_pos else PADDING_ID
@@ -203,11 +205,11 @@ def main(argv=None):
                          "codebook")
     eng = DalleEngine(params["n_embd"], params["n_layers"], params["n_heads"], tv, iv, tl, vae.image_seq_len,
                       device=device, attention_types=attention_types, local_attention_radius=local_radius,
-                      conv_attention_kernel=conv_k, image_position_embedding=pos_scheme,
+                      conv_attention_kernel=conv_k, image_position_embedding=None if rot_emb else pos_scheme,
                       per_position_padding=per_pos, activation=activation, logits_mask=mask, rotary_dim=rotary_dim,
                       rotary_base=rotary_base, gated_mlp=gated, shift_tokens=shift, sandwich_norm=sandwich,
                       layer_scale=scale, stable=stab, share_input_output_emb=tied, shared_attn_ids=attn_ids,
-                      shared_ff_ids=ff_ids, **sparse)
+                      shared_ff_ids=ff_ids, rotary_emb=rot_emb, **sparse)
     state = load_checkpoint(ckpt)
     eng.load_params({k: v for k, v in state.items()
                      if not k.endswith("/adam_m") and not k.endswith("/adam_v") and k != "global_step"})

@@ -786,6 +786,28 @@ int db200_rope_decode(db200_stream_t stream, void* qkv_bf16, const float* table,
 int db200_rope_decode_dev(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh,
                           int r, const int32_t* pos_dev);
 
+/* DALLE-pytorch's rotary embedding (rotary_emb; extension).  qkv is bf16 [rows][3][H][dh], rotated in place: for
+ * every q, k AND v head of row t at position p and every pair m < pairs (interleaved dims 2m, 2m+1),
+ *   x_2m' = bf16(x_2m c - x_2m+1 s),  x_2m+1' = bf16(x_2m+1 c + x_2m s),  c = table[p][0][m], s = table[p][1][m],
+ * every product and sum rounded separately in fp32 (no FMA contraction).  The dims 2 pairs .. dh-1 are unchanged.
+ * table: fp32 [S][2][pairs], position p's cosines then its sines (the engine's rotary_emb_table: pairs = 3 (dh / 3 / 2),
+ * text, image-row and image-column angles).  The position logic is rope_*'s:
+ *   rope_emb_fwd        : p = t mod S.
+ *   rope_emb_bwd        : the transpose rotation (s -> -s), applied to the dq, dk and dv columns of dqkv.
+ *   rope_emb_decode     : every row at position pos, 0 <= pos < S.
+ *   rope_emb_decode_dev : every row at position *pos_dev (graph replay); a position outside [0, S) leaves qkv unchanged.
+ * 1 <= pairs <= dh / 2, dh even, rows, S, H > 0 and non-NULL pointers, else DB200_E_INVALID; qkv must be 16-byte
+ * aligned when dh % 8 == 0 (16-byte vectors of 4 pairs) and 4-byte aligned otherwise, the table 4-byte aligned
+ * (DB200_E_ALIGN). */
+int db200_rope_emb_fwd(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh,
+                       int pairs);
+int db200_rope_emb_bwd(db200_stream_t stream, void* dqkv_bf16, const float* table, int rows, int S, int H, int dh,
+                       int pairs);
+int db200_rope_emb_decode(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H, int dh,
+                          int pairs, int pos);
+int db200_rope_emb_decode_dev(db200_stream_t stream, void* qkv_bf16, const float* table, int rows, int S, int H,
+                              int dh, int pairs, const int32_t* pos_dev);
+
 /* Token shift (extension; DALLE-pytorch's PreShiftToken) on a bf16 [rows][d] LayerNorm output y, c = d / 4.  Position
  * p < text_len (TL) is a text token, p >= TL the image token u = p - TL at grid row u / grid_w, column u % grid_w.
  * shift(y)[p] keeps y[p][2c, d) and replaces

@@ -16,6 +16,8 @@
 //   sample_rows_filtered   the same argmax restricted to the top-k / nucleus (top-p) set of logits * inv_temp
 //   sample_rows_guided     either of the two over the classifier-free-guidance mix u + s (c - u) of a conditional
 //                          and an unconditional row (the <true> instantiations); the draw goes to both rows' tokens
+//   caption_next   after a draw into text column c: the prompt id below the row's prompt length, else the column's pad
+//                  once column c - 1 or the draw is a padding token (caption completion)
 //   onehot_rows    y[r, idx[r]-offset] = 1, 0 elsewhere (codebook lookup input for the VAE decoder, vae_tf/models.py:127)
 #include "common.cuh"
 #include "ptx.cuh"
@@ -485,6 +487,27 @@ sample_rows_filtered_kernel(const float* __restrict__ logits, const float* __res
 
 __global__ void incr_i32_kernel(int* p, int delta) { *p += delta; }
 
+// ---- caption completion: finishes column c = pos + 1 of every row of the [rows][ld] token matrix after a draw has
+// been written there.  Row b keeps its prompt below lens[b]; past it a padding token in column c - 1 or drawn in column
+// c ends the caption: column c becomes c's pad (pad_base + c with per-position padding, else padding_id).  Integer
+// arithmetic only, one thread per row.
+__global__ void __launch_bounds__(128)
+caption_next_kernel(int* __restrict__ tokens, long long ld, const int* __restrict__ prefix, long long ld_prefix,
+                    const int* __restrict__ lens, int rows, int text_len, int text_vocab, int padding_id, int pad_base,
+                    int pos, const int* __restrict__ pos_dev) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= rows) return;
+  const int c = (pos_dev ? *pos_dev : pos) + 1;
+  if (c < 1 || c >= text_len) return;
+  int* row = tokens + b * ld;
+  if (c < lens[b]) {
+    row[c] = prefix[b * ld_prefix + c];
+    return;
+  }
+  auto is_pad = [&](int id) { return id == padding_id || (pad_base >= 0 && id >= text_vocab); };
+  if (is_pad(row[c - 1]) || is_pad(row[c])) row[c] = pad_base >= 0 ? pad_base + c : padding_id;
+}
+
 __global__ void onehot_rows_kernel(const int* __restrict__ idx, float* __restrict__ y, int K, int offset) {
   const int r = blockIdx.x;
   const int hot = idx[r] - offset;
@@ -835,6 +858,39 @@ extern "C" int db200_sample_rows_guided(db200_stream_t stream_, const float* log
   sample_rows_kernel<true><<<rows, 256, 0, stream>>>(logits, u_or_null, tokens, ld, lo, hi, inv_temp, pos_dev_or_null,
                                                      ld_tokens, rows, guidance_scale);
   return check_launch("sample_rows_kernel");
+}
+
+static int caption_next_launch(cudaStream_t stream, int32_t* tokens, long long ld, const int32_t* prefix,
+                               long long ld_prefix, const int32_t* lens, int rows, int text_len, int text_vocab_size,
+                               int padding_id, int pad_base, int pos, const int32_t* pos_dev) {
+  DB200_REQUIRE(tokens && prefix && lens, DB200_E_INVALID, "caption_next: null pointer");
+  DB200_REQUIRE(rows > 0 && text_len >= 1 && ld >= text_len && ld_prefix >= text_len, DB200_E_INVALID,
+                "caption_next: rows %d text_len %d ld %lld ld_prefix %lld", rows, text_len, ld, ld_prefix);
+  DB200_REQUIRE(text_vocab_size > 0 && padding_id >= 0 && padding_id < text_vocab_size, DB200_E_INVALID,
+                "caption_next: padding_id %d outside [0, %d)", padding_id, text_vocab_size);
+  DB200_REQUIRE(pad_base < 0 || (pad_base >= text_vocab_size && (long long)pad_base + text_len <= 2147483647LL),
+                DB200_E_INVALID, "caption_next: pad_base %d with text_vocab_size %d", pad_base, text_vocab_size);
+  DB200_REQUIRE(pos_dev || (pos >= 0 && pos + 1 < text_len), DB200_E_INVALID,
+                "caption_next: column %d outside [1, %d)", pos + 1, text_len);
+  caption_next_kernel<<<(rows + 127) / 128, 128, 0, stream>>>(tokens, ld, prefix, ld_prefix, lens, rows, text_len,
+                                                              text_vocab_size, padding_id, pad_base, pos, pos_dev);
+  return check_launch("caption_next_kernel");
+}
+
+extern "C" int db200_caption_next(db200_stream_t stream_, int32_t* tokens, long long ld_tokens, const int32_t* prefix,
+                                  long long ld_prefix, const int32_t* lens, int rows, int text_len,
+                                  int text_vocab_size, int padding_id, int pad_base, int pos) {
+  return caption_next_launch(static_cast<cudaStream_t>(stream_), tokens, ld_tokens, prefix, ld_prefix, lens, rows,
+                             text_len, text_vocab_size, padding_id, pad_base, pos, nullptr);
+}
+
+extern "C" int db200_caption_next_at(db200_stream_t stream_, int32_t* tokens, long long ld_tokens,
+                                     const int32_t* prefix, long long ld_prefix, const int32_t* lens, int rows,
+                                     int text_len, int text_vocab_size, int padding_id, int pad_base,
+                                     const int32_t* pos_dev) {
+  DB200_REQUIRE(pos_dev, DB200_E_INVALID, "caption_next_at: null position pointer");
+  return caption_next_launch(static_cast<cudaStream_t>(stream_), tokens, ld_tokens, prefix, ld_prefix, lens, rows,
+                             text_len, text_vocab_size, padding_id, pad_base, 0, pos_dev);
 }
 
 extern "C" int db200_onehot_rows_f32(db200_stream_t stream_, const int32_t* idx, float* y, int rows, int K,

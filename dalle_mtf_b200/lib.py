@@ -175,6 +175,8 @@ _SIGNATURES = {
                                       c_f32, c_vp],
     "db200_sample_rows_guided": [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_f32, c_f32, c_int,
                                  c_f32, c_vp],
+    "db200_caption_next": [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
+    "db200_caption_next_at": [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp],
     "db200_kv_cache_fill": [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int],
     "db200_rows_repeat": [c_vp, c_vp, c_i64, c_vp, c_int, c_int, c_int],
     "db200_rope_fwd": [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int],

@@ -122,6 +122,12 @@ class DALLE:
         return self._get_sampler().complete(text_ids, image_prefix, samples_per_prompt, temperature, top_k, top_p,
                                             guidance_scale)
 
+    def generate_texts(self, text_ids, temperature=1.0, top_k=None, top_p=None):
+        """Caption completion (DalleSampler.generate_texts, DALLE-pytorch's generate_texts): text_ids int [B,
+        text_seq_len], each row a non-empty prefix padded with padding_id -> int32 [B, text_seq_len], the prefix kept
+        and the rest drawn from the text window until a padding token ends the caption (temperature 0 = greedy)."""
+        return self._get_sampler().generate_texts(text_ids, temperature, top_k, top_p)
+
 
 class DiscreteVAE:
     def __init__(self, num_tokens, dimensions, convblocks=None, dim=512, hidden_dim=64, input_channels=3,

@@ -1314,6 +1314,40 @@ def sample_rows_guided(logits, u, tokens, lo, hi, inv_temp, guidance_scale, top_
     return tokens
 
 
+def _caption_args(tokens, prefix, lens, text_len):
+    L.require_device()
+    _chk(tokens, I32, "tokens"); _chk(prefix, I32, "prefix"); _chk(lens, I32, "lens")
+    rows = tokens.shape[0]
+    if tokens.dim() != 2 or tokens.stride(1) != 1 or prefix.dim() != 2 or prefix.stride(1) != 1 or \
+            prefix.shape[0] != rows or not lens.is_contiguous() or lens.numel() != rows or \
+            min(tokens.shape[1], prefix.shape[1]) < text_len:
+        raise L.DB200Error(f"caption_next: tokens and prefix must be [{rows}, >= {text_len}] with unit column stride, "
+                           f"lens [{rows}]")
+    return rows
+
+
+def caption_next(tokens, prefix, lens, pos, text_len, text_vocab_size, padding_id, pad_base=None):
+    """Finish text column c = pos + 1 of the token matrix tokens int32 [rows, >= text_len] after a draw: prefix[b, c]
+    (int32, token form) where c < lens[b], else c's pad (pad_base + c with per-position padding, else padding_id) when
+    column c - 1 or the draw is a padding token (padding_id, or with pad_base any id >= text_vocab_size)."""
+    rows = _caption_args(tokens, prefix, lens, text_len)
+    check(L.load().db200_caption_next(stream_ptr(), ptr(tokens), tokens.stride(0), ptr(prefix), prefix.stride(0),
+                                      ptr(lens), rows, int(text_len), int(text_vocab_size), int(padding_id),
+                                      -1 if pad_base is None else int(pad_base), int(pos)), "db200_caption_next")
+    return tokens
+
+
+def caption_next_at(tokens, prefix, lens, pos_dev, text_len, text_vocab_size, padding_id, pad_base=None):
+    """caption_next with the position read on the device from pos_dev (graph replay)."""
+    rows = _caption_args(tokens, prefix, lens, text_len)
+    _chk(pos_dev, I32, "pos_dev")
+    check(L.load().db200_caption_next_at(stream_ptr(), ptr(tokens), tokens.stride(0), ptr(prefix), prefix.stride(0),
+                                         ptr(lens), rows, int(text_len), int(text_vocab_size), int(padding_id),
+                                         -1 if pad_base is None else int(pad_base), ptr(pos_dev)),
+          "db200_caption_next_at")
+    return tokens
+
+
 def kv_cache_fill(qkv, k_cache, v_cache, P, rep=1):
     """k_cache[b*rep + r, p] = qkv[b, p, 1], v_cache[b*rep + r, p] = qkv[b, p, 2] for p < P (qkv [B*P, 3*H*dh], caches
     [B*rep, S_cache, H, dh]); later positions are left as they are."""

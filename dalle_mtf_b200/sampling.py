@@ -37,6 +37,11 @@ per-position padding the text_seq_len per-position pads).  The 2R rows run
 through the same step kernels (R conditional rows, then R unconditional ones) and each image token is drawn once per
 pair from u + s (c - u) of the two logit rows (db200_sample_rows_guided), then fed to both.  s = 1 (or None) is the
 plain sampler: no twin rows, the same kernels, the same tokens.
+
+Caption generation (generate_texts, DALLE-pytorch's generate_texts) draws the text positions instead: after a prefill
+of the shortest caption prefix, each text column is drawn over the text window [0, image_offset) by the same sampling
+kernels and finished by db200_caption_next (the prompt where a row's prefix is longer, padding once a padding token has
+been drawn), in a third captured graph.
 """
 import math
 import numbers
@@ -82,7 +87,7 @@ class DalleSampler:
     def _alloc(self, B):
         if self._B == B:
             return
-        self._graph_key = None      # captured graphs point at the buffers replaced here
+        self._graph_key = self._text_key = None      # captured graphs point at the buffers replaced here
         e = self.e
         dev, d = e.device, e.d
         mk = lambda *shape, dtype=BF16: torch.empty(*shape, dtype=dtype, device=dev)
@@ -165,31 +170,33 @@ class DalleSampler:
         return self.logit
 
     # -------------------------------------------------------------------------------------------- CUDA-graph path
-    def _step_dev(self, tokens):
-        """self.step with the position (and the input token column) read on the device from self.pos_dev."""
+    def _step_dev(self, tokens, pos_dev=None):
+        """self.step with the position (and the input token column) read on the device from pos_dev (default
+        self.pos_dev, the image graphs' position)."""
         e = self.e
-        ops.embed_fwd_at_dev(tokens, e.embed_table(), e.pos_embedding(), self.x[0], self.pos_dev)
+        pos_dev = self.pos_dev if pos_dev is None else pos_dev
+        ops.embed_fwd_at_dev(tokens, e.embed_table(), e.pos_embedding(), self.x[0], pos_dev)
         x_in, x_out = self.x
         for i in range(e.L):
             p = f"l{i}."
             ops.layernorm_fwd(x_in, e.P(p + "ln1_g"), e.P(p + "ln1_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
-                ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i], self.pos_dev, e.text_seq_len, e.shift_w)
+                ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i], pos_dev, e.text_seq_len, e.shift_w)
             if e.mlp[i]:
-                self._branch_out(p, "a", self._gmlp_step(p, i, pos_dev=self.pos_dev), e.W(p + "gm_wout"),
+                self._branch_out(p, "a", self._gmlp_step(p, i, pos_dev=pos_dev), e.W(p + "gm_wout"),
                                  e.P(p + "gm_bout"), x_in, self.xmid)
             else:
                 ops.linear_fwd(self.ln, e.W(p + "wqkv"), self.qkv)
                 if e.rotary:
-                    ops.rope_decode_dev(self.qkv, e.rope_table, self.pos_dev, e.H, e.dh, e.rotary_dim)
+                    ops.rope_decode_dev(self.qkv, e.rope_table, pos_dev, e.H, e.dh, e.rotary_dim)
                 if e.rotary_emb:
-                    ops.rope_emb_decode_dev(self.qkv, e.rope_emb_table, self.pos_dev, e.H, e.dh)
-                ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, self.pos_dev, e.attn_scale,
+                    ops.rope_emb_decode_dev(self.qkv, e.rope_emb_table, pos_dev, e.H, e.dh)
+                ops.attn_decode_dev(self.qkv, self.kc[i], self.vc[i], self.att, pos_dev, e.attn_scale,
                                     radius=e.radii[i], **e.axial_kw[i], **e.conv_kw[i], **e.block_sparse_kw[i])
                 self._branch_out(p, "a", self.att, e.W(p + "wo"), e.P(p + "o_b"), x_in, self.xmid)
             ops.layernorm_fwd(self.xmid, e.P(p + "ln2_g"), e.P(p + "ln2_b"), self.ln, self.mean, self.rstd, e.ln_eps)
             if e.shift_tokens:
-                ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i + 1], self.pos_dev, e.text_seq_len, e.shift_w)
+                ops.shift_tokens_decode_dev(self.ln, self.sc[2 * i + 1], pos_dev, e.text_seq_len, e.shift_w)
             ops.linear_fwd(self.ln, e.W(p + "w1"), self.h1, bias=e.P(p + "b1"), **e.mlp_act)
             self._branch_out(p, "m", self.h1, e.W(p + "w2"), e.P(p + "b2"), self.xmid, x_out)
             x_in, x_out = x_out, x_in
@@ -197,20 +204,25 @@ class DalleSampler:
         e.vocab_gemm(self.ln, self.logit, bias=e.P("bout"))
         return self.logit
 
-    def _filter(self, top_k, top_p):
+    def _filter(self, top_k, top_p, n_text=None):
         """(top_k, top_p) as the filtered kernel takes them, or None when neither truncates anything (the unfiltered
-        kernels then run, exactly as without the arguments)."""
+        kernels then run, exactly as without the arguments).  The draw is over the image_vocab_size image tokens, or
+        with n_text over the n_text ids of the text window."""
         if top_k is not None and (isinstance(top_k, bool) or int(top_k) != top_k or top_k < 1):
             raise ValueError(f"top_k must be an integer >= 1 (or None), got {top_k!r}")
         if top_p is not None and not 0.0 < top_p <= 1.0:
             raise ValueError(f"top_p must lie in (0, 1] (or be None), got {top_p!r}")
-        k = 0 if top_k is None or top_k >= self.e.image_vocab_size else int(top_k)
+        n = self.e.image_vocab_size if n_text is None else n_text
+        k = 0 if top_k is None or top_k >= n else int(top_k)
         p = 1.0 if top_p is None else float(top_p)
         if k == 0 and p == 1.0:
             return None
-        if self.e.image_vocab_size > FILTER_MAX_IDS:
-            raise ValueError(f"top_k / top_p filter at most {FILTER_MAX_IDS} image tokens, but image_vocab_size = "
-                             f"{self.e.image_vocab_size}; sample without a filter")
+        if n > FILTER_MAX_IDS:
+            if n_text is None:
+                raise ValueError(f"top_k / top_p filter at most {FILTER_MAX_IDS} image tokens, but image_vocab_size = "
+                                 f"{n}; sample without a filter")
+            raise ValueError(f"top_k / top_p filter at most {FILTER_MAX_IDS} ids, but the text window [0, "
+                             f"image_offset) holds {n}; sample without a filter")
         return k, p
 
     @staticmethod
@@ -363,6 +375,119 @@ class DalleSampler:
         for _ in range(P, e.S - 1):
             self.g_sample.replay()
         return self.tokens[:R].clone()
+
+    # ------------------------------------------------------------------------------------------- caption generation
+    def caption_lengths(self, text_ids):
+        """Prefix lengths n_b of caption rows text_ids int [B, text_seq_len]: the ids before the first padding_id
+        (text_seq_len when there is none), as an int32 tensor on text_ids' device.  Raises ValueError for a wrong shape,
+        an id outside [0, text_vocab_size) or an empty prefix."""
+        e = self.e
+        if not torch.is_tensor(text_ids) or text_ids.dim() != 2 or text_ids.shape[1] != e.text_seq_len or \
+                text_ids.shape[0] < 1 or text_ids.dtype.is_floating_point or text_ids.dtype == torch.bool:
+            raise ValueError(f"text_ids must be an integer tensor [B >= 1, {e.text_seq_len}], got "
+                             f"{tuple(text_ids.shape) if torch.is_tensor(text_ids) else type(text_ids).__name__}")
+        if int(text_ids.min()) < 0 or int(text_ids.max()) >= e.text_vocab_size:
+            raise ValueError(f"caption ids must lie in [0, {e.text_vocab_size})")
+        pad = text_ids == self.padding_id
+        lens = torch.where(pad.any(1), pad.to(I32).argmax(1), e.text_seq_len).to(I32)
+        empty = (lens == 0).nonzero().flatten().tolist()
+        if empty:
+            raise ValueError(f"caption rows {empty} start with padding_id {self.padding_id}: an empty prefix has "
+                             "nothing to continue from (position 0 is never a training target; DALLE-pytorch starts "
+                             "such a caption from id 0)")
+        return lens
+
+    def _capture_text(self, B, greedy, inv_t, flt):
+        """The text step graph over its own static buffers (token matrix, prompt, prompt lengths, position, noise):
+        step -> noise -> draw over the text window into column pos + 1 -> caption_next_at -> advance the position."""
+        e = self.e
+        key = (B, greedy, inv_t, flt)
+        if self._text_key == key:
+            return
+        dev, TL, hi = e.device, e.text_seq_len, e.image_offset
+        self.t_tokens = torch.zeros(B, TL, dtype=I32, device=dev)
+        self.t_prefix = torch.zeros(B, TL, dtype=I32, device=dev)
+        self.t_lens = torch.full((B,), TL, dtype=I32, device=dev)
+        self.t_pos = torch.zeros(1, dtype=I32, device=dev)
+        self.t_u = None if greedy else torch.empty(B, hi, dtype=F32, device=dev)
+
+        def step():
+            logits = self._step_dev(self.t_tokens, self.t_pos)
+            if self.t_u is not None:
+                self.t_u.uniform_(1e-9, 1.0)        # default CUDA generator: graph-safe Philox offsets
+            if flt is None:
+                ops.sample_rows_at(logits, self.t_u, self.t_tokens, 0, hi, inv_t, self.t_pos)
+            else:
+                ops.sample_rows_filtered_at(logits, self.t_u, self.t_tokens, 0, hi, inv_t, *flt, self.t_pos)
+            ops.caption_next_at(self.t_tokens, self.t_prefix, self.t_lens, self.t_pos, TL, e.text_vocab_size,
+                                self.padding_id, e.pad_base)
+
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):     # eager warm-up, as in _capture
+            step()
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        self.g_text = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.g_text):
+            step()
+            ops.incr_i32(self.t_pos, 1)
+        self._text_key = key
+
+    @torch.no_grad()
+    def generate_texts(self, text_ids, temperature=1.0, top_k=None, top_p=None):
+        """Caption completion (DALLE-pytorch's generate_texts): text_ids int [B, text_seq_len], captions padded with
+        padding_id as generate_dalle.pad_captions pads them -> int32 [B, text_seq_len] (device) in the same form,
+        ready for generate, generate_graphed or complete.
+
+        Row b's prefix is its ids before the first padding_id; its length n_b must be >= 1 (an empty prefix raises
+        ValueError: position 0 is never a training target, so there is nothing to draw it from; DALLE-pytorch starts
+        from id 0).  Ids outside [0, text_vocab_size) raise ValueError.  Columns c < n_b come back bit for bit.  Column
+        c >= n_b is drawn from the model's logits at position c - 1 restricted to the text window [0, image_offset)
+        (text_vocab_size ids, plus the text_seq_len per-position pads with per_position_padding): the logits mask's
+        text window, whether the model was trained with logits_mask or not.  The draw applies temperature, then top_k,
+        then top_p, then the Gumbel-max: the image sampler's semantics and kernels; temperature 0 or None is greedy.
+        A drawn padding token (padding_id, or with per-position padding any id >= text_vocab_size) ends the caption:
+        that column and every later one are padding_id in the result (in the decoder's token matrix, each column's
+        per-position pad), as training data is right-padded.  Rows with n_b = text_seq_len come back unchanged.
+
+        One prefill runs the common prefix P = min_b n_b, column P is drawn from its logits, and the captured text step
+        continues to the last text column; rows with a longer prefix are teacher-forced up to it.  Noise comes from
+        torch's default CUDA generator (seed it with torch.manual_seed); a seeded call draws the same whether or not it
+        had to capture.  There is no guidance and no samples_per_prompt: repeat the prompt rows for several samples."""
+        e = self.e
+        lens = self.caption_lengths(text_ids)
+        flt = self._filter(top_k, top_p, n_text=e.image_offset)
+        B, TL = text_ids.shape
+        text_ids = text_ids.to(device=e.device, dtype=I32).contiguous()
+        P = int(lens.min())
+        if P == TL:
+            return text_ids.clone()
+        greedy = temperature is None or temperature <= 0
+        inv_t = 1.0 if greedy else 1.0 / float(temperature)
+        self._alloc(B)
+        rng = torch.cuda.get_rng_state(e.device)   # as in complete: the capture's warm-up draws noise
+        self._capture_text(B, greedy, inv_t, flt)
+        torch.cuda.set_rng_state(rng, e.device)
+        prompt = self._captions(text_ids)
+        self.t_prefix.copy_(prompt)
+        self.t_lens.copy_(lens)
+        logits = e.prefill(prompt[:, :P].contiguous(), self.kc, self.vc, 1, shift_caches=self.sc)
+        if self.t_u is not None:
+            self.t_u.uniform_(1e-9, 1.0)
+        if flt is None:
+            ops.sample_rows(logits, self.t_u, self.tok, 0, e.image_offset, inv_t)
+        else:
+            ops.sample_rows_filtered(logits, self.t_u, self.tok, 0, e.image_offset, inv_t, *flt)
+        self.t_tokens.copy_(prompt)
+        self.t_tokens[:, P] = self.tok
+        ops.caption_next(self.t_tokens, self.t_prefix, self.t_lens, P - 1, TL, e.text_vocab_size, self.padding_id,
+                         e.pad_base)
+        self.t_pos.fill_(P)
+        for _ in range(P, TL - 1):
+            self.g_text.replay()
+        out = self.t_tokens.clone()
+        return out.masked_fill_(out >= e.text_vocab_size, self.padding_id) if e.per_position_padding else out
 
     @torch.no_grad()
     def generate(self, text_ids, temperature=1.0, generator=None, return_logits=False, top_k=None, top_p=None,

@@ -3,11 +3,16 @@ image tokens for each caption (optionally completing the top rows of a prompt im
 
     python generate_dalle.py --model dalle_example_b200 --out DIR (--captions FILE | --caption_ids FILE.npy)
         [--checkpoint PATH] [--image_prompt IMG ...] [--prompt_rows R] [--samples_per_prompt N]
-        [--temperature T] [--top_k K] [--top_p P] [--guidance_scale G] [--batch_size B] [--seed S]
+        [--temperature T] [--top_k K] [--top_p P] [--guidance_scale G] [--batch_size B] [--seed S] [--gentxt]
 
 Writes DIR/{caption:05d}_{sample:02d}.png and DIR/tokens.npy (int32 [captions * samples_per_prompt, S]: caption ids,
 then image-token ids offset as in training: by text_vocab_size, or with per_position_padding by text_vocab_size +
 text_seq_len, the caption's padding then shown as the per-position pad tokens the model saw).  One process, one GPU.
+
+--gentxt (DALLE-pytorch's flag) first completes every caption with the model's text half (DalleSampler.generate_texts,
+with the run's --temperature, --top_k and --top_p; the caption ends where the config's padding_id begins) and writes
+DIR/captions.npy (int32 [captions, text_seq_len]) and, when the GPT-2 BPE files are available, DIR/captions.txt (one
+decoded caption per line, padding dropped); the images are then drawn for the completed captions.
 """
 import argparse
 import math
@@ -46,6 +51,9 @@ def parse_args(argv=None):
                         "caption_dropout > 0.")
     p.add_argument("--batch_size", type=int, help="Captions per sampling call (default: predict_batch_size).")
     p.add_argument("--seed", type=int, default=0)
+    p.add_argument("--gentxt", action="store_true",
+                   help="Complete each caption with the model before drawing its images (writes captions.npy and, "
+                        "with local GPT-2 BPE files, captions.txt).")
     args = p.parse_args(argv)
     if (args.image_prompt is None) != (args.prompt_rows is None):
         p.error("--image_prompt and --prompt_rows go together")
@@ -118,6 +126,27 @@ def encode_captions(lines, tokenizer, text_seq_len, text_vocab_size, pad=PADDING
     return pad_captions(rows, text_seq_len, text_vocab_size, pad)
 
 
+def check_caption_prefixes(captions, pad):
+    """--gentxt continues each caption after its prefix (the ids before the first `pad`): an empty one has nothing to
+    continue from."""
+    empty = np.flatnonzero(captions[:, 0] == pad)
+    if len(empty):
+        raise SystemExit(f"--gentxt: caption(s) {empty.tolist()} have no ids before the padding id {pad}; give each "
+                         "caption at least one token to complete")
+
+
+def write_captions(out_dir, captions, pad, tokenizer=None):
+    """DIR/captions.npy (int32 [N, text_seq_len]) and, with a tokenizer that decodes, DIR/captions.txt: one caption per
+    line, its ids before the first `pad`."""
+    np.save(os.path.join(out_dir, "captions.npy"), captions.astype(np.int32))
+    if tokenizer is None or not hasattr(tokenizer, "decode"):
+        return
+    with open(os.path.join(out_dir, "captions.txt"), "w") as f:
+        for row in captions:
+            n = int(np.argmax(row == pad)) if (row == pad).any() else len(row)
+            f.write(tokenizer.decode([int(i) for i in row[:n]]).replace("\n", " ") + "\n")
+
+
 def token_grid_side(params):
     """Side of the VAE's token grid: image_size / 2^(group_count - 1) for the DALL-E paper's network, image_size /
     stack_factor / 2^len(convblocks) for the reference's."""
@@ -170,17 +199,22 @@ def main(argv=None):
     rot_emb = rotary_emb(params) and rotary_emb(params, token_grid_side(params) ** 2)
     # with per-position padding the captions are padded with the config's padding_id, which the sampler maps to the
     # per-position pads as training does
-    pad = padding_id(params) if per_pos else PADDING_ID
-    if args.guidance_scale is not None and not 0 <= padding_id(params) < tv:
-        raise SystemExit(f"--guidance_scale: padding id {padding_id(params)} outside [0, {tv}); set padding_id in the "
-                         "config")
+    # (--gentxt: a caption ends where the config's padding_id begins, the id the sampler then draws to end one)
+    pad = padding_id(params) if (per_pos or args.gentxt) else PADDING_ID
+    for flag, on in (("--guidance_scale", args.guidance_scale is not None), ("--gentxt", args.gentxt)):
+        if on and not 0 <= padding_id(params) < tv:
+            raise SystemExit(f"{flag}: padding id {padding_id(params)} outside [0, {tv}); set padding_id in the config")
+    tokenizer = None
     if args.caption_ids:
         captions = load_caption_ids(args.caption_ids, tl, tv, pad)
     else:
         from dalle_mtf_b200.tokenizer import get_tokenizer
         with open(args.captions) as f:
             lines = [ln.rstrip("\n") for ln in f if ln.strip()]
-        captions = encode_captions(lines, get_tokenizer(params["tokenizer"]), tl, tv, pad)
+        tokenizer = get_tokenizer(params["tokenizer"])
+        captions = encode_captions(lines, tokenizer, tl, tv, pad)
+    if args.gentxt:
+        check_caption_prefixes(captions, pad)
     N = len(captions)
     n = 0
     if args.image_prompt:
@@ -219,11 +253,20 @@ def main(argv=None):
         prefix = encode_image_prompts(args.image_prompt, params, vae, device)[:, :n]
         if len(prefix) == 1:
             prefix = prefix.expand(N, n)
-    sampler = DalleSampler(eng, padding_id=padding_id(params) if (args.guidance_scale is not None or per_pos) else None)
+    sampler = DalleSampler(eng, padding_id=padding_id(params) if (args.guidance_scale is not None or per_pos or
+                                                                  args.gentxt) else None)
     torch.manual_seed(args.seed)
     rep = args.samples_per_prompt
     bs = args.batch_size or params["predict_batch_size"] or 1
     os.makedirs(args.out, exist_ok=True)
+    if args.gentxt:
+        captions = np.concatenate([
+            sampler.generate_texts(torch.from_numpy(captions[c0:c0 + bs]).to(device), temperature=args.temperature,
+                                   top_k=args.top_k, top_p=args.top_p).cpu().numpy() for c0 in range(0, N, bs)])
+        if tokenizer is None:
+            from dalle_mtf_b200.tokenizer import get_tokenizer
+            tokenizer = get_tokenizer(params.get("tokenizer"))
+        write_captions(args.out, captions, pad, tokenizer)
     all_tokens = []
     for c0 in range(0, N, bs):
         text = torch.from_numpy(captions[c0:c0 + bs]).to(device)

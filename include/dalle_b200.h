@@ -753,6 +753,22 @@ int db200_sample_rows_guided(db200_stream_t stream, const float* logits, long lo
                              int32_t* tokens, long long ld_tokens, int32_t* kept_or_null, int rows, int lo, int hi,
                              float inv_temp, float guidance_scale, int top_k, float top_p,
                              const int32_t* pos_dev_or_null);
+/* Caption completion: finishes text column c = pos + 1 of every row of the int32 token matrix tokens [rows][ld_tokens]
+ * after a draw has been written into it (run it after any of the samplers above).  For row b, with n_b = lens[b]:
+ *   c < n_b              : tokens[b][c] = prefix[b][c]   (the prompt, prefix int32 [rows][ld_prefix] in token form)
+ *   else if tokens[b][c - 1] or tokens[b][c] is a padding token : tokens[b][c] = c's pad
+ *   else                 : the draw is kept.
+ * A padding token is padding_id or, with per-position padding (pad_base >= 0), any id >= text_vocab_size; c's pad is
+ * pad_base + c, or padding_id when pad_base < 0.  Integer arithmetic only: the result is exact.  The _at variant reads
+ * pos from device memory (graph replay) and leaves the matrix unchanged when c is outside [1, text_len).  A null
+ * pointer, rows < 1, ld_tokens or ld_prefix < text_len, padding_id outside [0, text_vocab_size), 0 <= pad_base <
+ * text_vocab_size, or (host position) c outside [1, text_len): DB200_E_INVALID. */
+int db200_caption_next(db200_stream_t stream, int32_t* tokens, long long ld_tokens, const int32_t* prefix,
+                       long long ld_prefix, const int32_t* lens, int rows, int text_len, int text_vocab_size,
+                       int padding_id, int pad_base, int pos);
+int db200_caption_next_at(db200_stream_t stream, int32_t* tokens, long long ld_tokens, const int32_t* prefix,
+                          long long ld_prefix, const int32_t* lens, int rows, int text_len, int text_vocab_size,
+                          int padding_id, int pad_base, const int32_t* pos_dev);
 /* Prompt prefill hand-off: a whole prompt runs through the training forward kernels at sequence length P, and these
  * copies turn its results into the decoder's state (bandwidth-bound, 16-byte vector accesses).
  *   kv_cache_fill : qkv bf16 [B][P][3][H][dh] (the fused q|k|v GEMM output attn_causal_fwd reads) -> caches bf16
